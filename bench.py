@@ -14,10 +14,11 @@ Prints ONE JSON line (rank 0):
   e2e        the same metric through the reference-facing call FRNet.infer_sequence() with HOST
              buffers: per step the H2D copy of the LR frames and the D2H copy of the uint8 HR
              frames are inside the timed region
-  roofline   the dominant kernel (conv_chain_kernel: SRNet conv_in + 10 residual blocks = 21 convs
-             64->64 in one persistent tcgen05 launch) timed live with CUDA events against the measured
-             tensor peak; `traffic` = its DRAM bytes from one ncu --set full capture
-  roofline_conv_single  one residual conv 64->64 as its own launch (conv_tcgen05_kernel)
+  roofline   the SRNet body's conv timed live with CUDA events against the tensor peak (see peaks()):
+             one residual conv 64->64 launch (conv_wgmma_kernel) on the default path, or with
+             TECOGAN_B200_CHAIN=1 the persistent conv_chain_kernel (conv_in + 10 residual blocks =
+             21 convs 64->64 in one launch)
+  roofline_conv_single  one residual conv 64->64 as its own launch (conv_wgmma_kernel)
   roofline_warp*  the fused warp+space_to_depth+concat kernel against the HBM roofline
   cpu_baseline   the reference's CPU path (oracle/frnet_torchref.py: same PyTorch CPU library
              ops as the reference) on the box's host cores, bounded sample (rank 0, N=1)
@@ -41,20 +42,20 @@ sys.path.insert(0, ROOT)
 
 # The two inference workloads of BASELINE.json; --workload selects one (default: the headline bd4).
 WORKLOADS = {
-    # configs[1]: TecoGAN 4x BD inference, synthetic 3x134x320, batch=4 lock-stepped clips per B200
+    # configs[1]: TecoGAN 4x BD inference, synthetic 3x134x320, batch=4 lock-stepped clips per GPU
     'bd4': dict(lr=(3, 134, 320), scale=4, degradation='BD', clips_per_gpu=4,
                 flop_per_frame=94.438e9,          # reference counter, SURVEY.md 8-d (FNet 10.511 + SRNet 83.927)
                 warp_bytes_per_frame=22983680,    # SURVEY.md 8-d byte formula, fp32
                 metric='hr_frames_per_sec_4xBD_3x134x320',
                 name='TecoGAN 4x BD inference, synthetic 3x134x320 -> 3x536x1280, batch=4 lock-stepped clips per '
-                     'B200 (BASELINE.json configs[1]); clips shard across GPUs, no collective'),
+                     'GPU (BASELINE.json configs[1]); clips shard across GPUs, no collective'),
     # configs[4]: TecoGAN 2x BI inference, synthetic 3x268x640 LR, 30-frame clips, sequence-sharded over GPUs
     'bi2': dict(lr=(3, 268, 640), scale=2, degradation='BI', clips_per_gpu=2,
                 flop_per_frame=313.916e9,         # FNet 43.019 + SRNet 270.897
                 warp_bytes_per_frame=26071040,
                 metric='hr_frames_per_sec_2xBI_3x268x640',
                 name='TecoGAN 2x BI inference, synthetic 3x268x640 -> 3x536x1280, 30-frame clips, 2 lock-stepped '
-                     'clips per B200 (BASELINE.json configs[4]); clips round-robin over GPUs (main.py:169), '
+                     'clips per GPU (BASELINE.json configs[4]); clips round-robin over GPUs (main.py:169), '
                      'no collective'),
 }
 WL = WORKLOADS['bd4']                # set by main()
@@ -77,16 +78,20 @@ def workload_config(world):
     """`config` of the JSON line -- identical for our arm and the reference arm."""
     return {'workload': WL['name'], 'clips_per_gpu': CLIPS_PER_GPU, 'frames_per_step': CLIPS_PER_GPU * world,
             'weights': 'seeded random init (no checkpoint)',
-            'l2': 'inputs larger than L2: ~1.3 GB of activations per step >> 126 MB, no explicit flush'}
+            'l2': 'inputs larger than L2: ~1.3 GB of activations per step >> 50 MB, no explicit flush'}
 
 
 def peaks():
+    """Peaks the roofline fractions are taken against: a MEASURED_PEAKS.json of the machine if present, else
+    NVIDIA's data-sheet figures for the H100 SXM at 700 W (dense fp16/bf16; never reached rates -- a card
+    at a lower power limit or clock gets less)."""
     path = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.isfile(path):
         d = json.load(open(path))
         return {'hbm_gbs': d['hbm_gbs'], 'tflops_burst': d['bf16_tflops'],
                 'tflops_sustained': d['bf16_tflops_sustained'], 'src': 'measured'}
-    return {'hbm_gbs': 6650.0, 'tflops_burst': 1590.0, 'tflops_sustained': 1400.0, 'src': 'fallback'}
+    return {'hbm_gbs': 3350.0, 'tflops_burst': 989.0, 'tflops_sustained': 989.0,
+            'src': 'H100 SXM data sheet (700 W), not measured'}
 
 
 class ClockSampler:
@@ -167,7 +172,7 @@ def _host_threads(threads=None):
 
 
 def reference_net(device):
-    """The UNMODIFIED reference FRNet (baseline/_ref, installed by tools/vendor_reference.py) holding the
+    """The UNMODIFIED reference FRNet (oracle/_ref, installed by oracle/vendor_reference.py) holding the
     benchmark's seeded weights; None when the install is absent."""
     import refimport
     if not refimport.available():
@@ -181,7 +186,7 @@ def reference_net(device):
 def cpu_reference_fps(steps, warmup, n=None):
     """The reference's own CPU path: FRNet.step on `n` lock-stepped clip-frames per step (default: the
     workload's clips_per_gpu, i.e. the SAME step as our arm), fp32, all host threads.  Falls back to the
-    operator-for-operator port (oracle/frnet_torchref.py) when baseline/_ref is not installed."""
+    operator-for-operator port (oracle/frnet_torchref.py) when oracle/_ref is not installed."""
     import torch
     n = CLIPS_PER_GPU if n is None else n
     cores = _host_threads()
@@ -213,8 +218,8 @@ def run_reference(args, rank):
         return
     n = CLIPS_PER_GPU
     fps, dt, cores, kind = cpu_reference_fps(args.steps, max(args.warmup, 1))
-    src = ('unmodified reference FRNet.step from baseline/_ref (codes/models/networks/tecogan_nets.py:227-252)'
-           if kind == 'reference' else 'port oracle/frnet_torchref.py (baseline/_ref not installed)')
+    src = ('unmodified reference FRNet.step from oracle/_ref (codes/models/networks/tecogan_nets.py:227-252)'
+           if kind == 'reference' else 'port oracle/frnet_torchref.py (oracle/_ref not installed)')
     sample = (f'{args.steps} steps x {n} lock-stepped clip-frames {"x".join(map(str, LR))} -> x{SCALE} '
               f'(the same step as the GPU arm), {src}, fp32, {cores} host threads')
     line = {
@@ -230,14 +235,14 @@ def run_reference(args, rank):
 
 
 def eager_gpu_results(steps, warmup):
-    """Context comparator: the UNMODIFIED reference FRNet (baseline/_ref) on the same B200 through
+    """Context comparator: the UNMODIFIED reference FRNet (oracle/_ref) on the same GPU through
     PyTorch's CUDA library kernels (cuDNN), same lock-stepped step, CUDA events: fp32, TF32 and fp16
-    autocast.  Answers "what does the stock reference get on this GPU" (no B200 number is published)."""
+    autocast.  Answers "what does the stock reference get on this GPU" (no H100 number is published)."""
     import torch
     dev = torch.device('cuda', torch.cuda.current_device())
     net = reference_net(dev)
     if net is None:
-        return {'unavailable': 'baseline/_ref not installed'}
+        return {'unavailable': 'oracle/_ref not installed'}
     torch.backends.cudnn.benchmark = True                      # codes/main.py:216
     g = torch.Generator().manual_seed(0)
     n = CLIPS_PER_GPU
@@ -283,8 +288,8 @@ def run_eager_gpu(args, rank):
 
 # =============================================================================== training workloads
 # BASELINE.json configs[2] / [3]: TecoGAN 4x BD training (G + D + ping-pong), synthetic REDS-shape 10-frame
-# 3x64x64 LR crops, batch 32 per B200; N > 1 = DDP over NCCL (gradient all-reduce), weak scaling.
-# The loop is the REFERENCE's own (VSRGANModel.train from baseline/_ref: discriminator, VGG, losses and
+# 3x64x64 LR crops, batch 32 per GPU; N > 1 = DDP over NCCL (gradient all-reduce), weak scaling.
+# The loop is the REFERENCE's own (VSRGANModel.train from oracle/_ref: discriminator, VGG, losses and
 # optimisers stay PyTorch -- SURVEY.md section 2 puts them out of scope); the generator is this repo's
 # (forward + backward on the library's kernels) or, for the comparison arms, the reference's.
 TRAIN = dict(lr=(3, 64, 64), scale=4, t=10, batch=32, border=4,
@@ -294,11 +299,11 @@ TRAIN = dict(lr=(3, 64, 64), scale=4, t=10, batch=32, border=4,
 def train_config(model, batch, world):
     return {'workload': f'{"TecoGAN (G + ST-discriminator + VGG + ping-pong)" if model == "tecogan" else "FRVSR (generator only)"} '
                         f'4x BD training, synthetic REDS-shape {TRAIN["t"]}-frame 3x64x64 LR crops (GT 264x264 incl. the BD '
-                        f'border), reference training loop (baseline/_ref) with the generator under test; DDP/NCCL gradient '
+                        f'border), reference training loop (oracle/_ref) with the generator under test; DDP/NCCL gradient '
                         f'all-reduce for N > 1 (BASELINE.json configs[2]/[3])',
             'batch_per_gpu': batch, 'global_batch': batch * world, 'frames_per_step': batch * TRAIN['t'] * world,
             'weights': 'seeded random init (no checkpoint; VGG19 = random weights of the same architecture)',
-            'l2': 'activations of one step (tens of GB) >> 126 MB L2, no explicit flush'}
+            'l2': 'activations of one step (tens of GB) >> 50 MB L2, no explicit flush'}
 
 
 def _train_model(model, device, generator, dist_on, rank, world):
@@ -374,7 +379,7 @@ def time_train_kernels(dev, pk, batch):
     dw = torch.zeros(64, 64, 3, 3, device=dev)
     t = _time_graph(lambda i: ops.wgrad(pc, xs[i], dzs[i], dw), 2, 6, torch)
     fl = RES_CONV_FLOP_PER_PX * n_img * h * w
-    out['roofline_wgrad'] = {'kernel': f'wgrad_tcgen05_kernel<conv3x3> (64->64, {n_img} images {h}x{w} = one layer of one step)',
+    out['roofline_wgrad'] = {'kernel': f'wgrad_wgmma_kernel<conv3x3> (64->64, {n_img} images {h}x{w} = one layer of one step)',
                              'bound': 'tensor', 'achieved': fl / t / 1e12, 'peak': pk['tflops_burst'], 'unit': 'TFLOP/s',
                              'frac': fl / t / 1e12 / pk['tflops_burst'], 'us_per_launch': t * 1e6, 'flop_per_launch': fl,
                              'traffic': ncu_traffic('wgrad_train')[0], 'traffic_src': ncu_traffic('wgrad_train')[1],
@@ -385,7 +390,7 @@ def time_train_kernels(dev, pk, batch):
     md = [torch.randn(batch, h, w, 64, device=dev).half() for _ in range(nb)]
     t = _time_graph(lambda i: dgr(xd[i], y=yd[i], mask=md[i], mask_act=L.ACT_RELU), nb, 40, torch)
     fl = RES_CONV_FLOP_PER_PX * batch * h * w
-    out['roofline_dgrad'] = {'kernel': f'conv_tcgen05_kernel<conv3x3, halo, BWD> (dgrad 64->64 * ReLU\'(mask), {batch} images {h}x{w})',
+    out['roofline_dgrad'] = {'kernel': f'conv_wgmma_kernel<conv3x3, halo, BWD> (dgrad 64->64 * ReLU\'(mask), {batch} images {h}x{w})',
                              'bound': 'tensor', 'achieved': fl / t / 1e12, 'peak': pk['tflops_burst'], 'unit': 'TFLOP/s',
                              'frac': fl / t / 1e12 / pk['tflops_burst'], 'us_per_launch': t * 1e6, 'flop_per_launch': fl,
                              'traffic': None, 'how': f'40 launches in one CUDA graph over {nb} rotating buffer sets, CUDA events'}
@@ -416,7 +421,7 @@ def run_train(args, rank, world, local_rank):
                 'config': train_config(model, args.batch or TRAIN['batch'], args.gpus),
                 'cpu_baseline': {'value': fps, 'unit': 'frames/s', 'cores': cores, 'kind': 'reference',
                                  'sample': f'{steps} training iterations of {n} clip ({TRAIN["t"]} frames, 64x64 LR) with the unmodified '
-                                           f'reference (baseline/_ref) on {cores} host threads -- a bounded sample of the batch'},
+                                           f'reference (oracle/_ref) on {cores} host threads -- a bounded sample of the batch'},
                 'e2e': {'value': fps, 'unit': 'frames/s', 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0},
                 'gpu_launches': 0}
         print(json.dumps(line), flush=True)
@@ -478,7 +483,7 @@ def run_train(args, rank, world, local_rank):
                         'api': 'reference VSR(GAN)Model.prepare_training_data(pinned gt) + .train() with define_generator = tecogan_b200'},
                 'gpu_launches': launches, 'launches_per_step': launches / K if K else 0, 'clocks': clocks,
                 'peak_memory_gb': peak_gb, 'last_log': log,
-                'generator': 'tecogan_b200 (fp16 tcgen05 forward + backward)' if impl == 'ours' else 'reference FRNet on cuDNN (fp32/TF32)'}
+                'generator': 'tecogan_b200 (fp16 wgmma forward + backward)' if impl == 'ours' else 'reference FRNet on cuDNN (fp32/TF32)'}
         if impl != 'ours':
             line['impl'] = 'eager-gpu'
     del m
@@ -491,7 +496,7 @@ def run_train(args, rank, world, local_rank):
         ref_ms = _generator_only_ms('reference', dev, gb)
         line['generator_fwd_bwd'] = {'batch': gb, 'frames': 2 * TRAIN['t'] - 1, 'ours_ms': ours_ms, 'reference_cudnn_ms': ref_ms,
                                      'speedup': ref_ms / ours_ms,
-                                     'note': 'forward_sequence + backward of the generator alone on the same B200'}
+                                     'note': 'forward_sequence + backward of the generator alone on the same GPU'}
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
@@ -502,9 +507,8 @@ def run_train(args, rank, world, local_rank):
 # =============================================================================== our arm
 def ncu_traffic(kernel_key):
     """dram__bytes_read.sum + dram__bytes_write.sum per launch of a kernel, taken from the latest
-    `ncu --set full` capture summarised in profiles/ncu_traffic.json (written by
-    tools/summarize_ncu.py --traffic-json from the .ncu-rep of the CURRENT kernels); None when that
-    kernel has no capture -- never a remembered constant."""
+    `ncu --set full` capture summarised in profiles/ncu_traffic.json (kernel key -> {dram_bytes_per_launch,
+    src}); None when that file or kernel has no capture -- never a remembered constant."""
     path = os.path.join(ROOT, 'profiles', 'ncu_traffic.json')
     try:
         ent = json.load(open(path)).get(kernel_key)
@@ -551,13 +555,13 @@ def time_kernels(dev, pk):
     # ---- dominant kernel: SRNet residual-block conv 64->64 (+bias, ReLU), n frames per launch
     wt = torch.randn(64, 64, 3, 3, device=dev) * 0.04
     pc = ops.PackedConv(wt, torch.zeros(64, device=dev), L.CONV_3X3, L.ACT_RELU)
-    nbuf = max(3, int(220 / mb) + 1)            # bd4: 10 x (22 MB in + 22 MB out) = 440 MB > 126 MB L2
+    nbuf = max(3, int(220 / mb) + 1)            # bd4: 10 x (22 MB in + 22 MB out) = 440 MB > 50 MB L2
     xs = [torch.randn(n, h, w, 64, device=dev).half() for _ in range(nbuf)]
     ys = [torch.empty_like(x) for x in xs]
     t_conv = _time_graph(lambda i: pc(xs[i], y=ys[i]), nbuf, reps, torch)
     flops = RES_CONV_FLOP_PER_PX * n * h * w
     out['roofline'] = {
-        'kernel': f'conv_tcgen05_kernel<conv3x3, halo> (SRNet resblock conv 64->64, {n} frames/launch)',
+        'kernel': f'conv_wgmma_kernel<conv3x3, halo> (SRNet resblock conv 64->64, {n} frames/launch)',
         'bound': 'tensor', 'achieved': flops / t_conv / 1e12, 'peak': pk['tflops_burst'], 'unit': 'TFLOP/s',
         'frac': flops / t_conv / 1e12 / pk['tflops_burst'],
         'traffic': ncu_traffic('conv_single_' + WL_KEY)[0], 'traffic_src': ncu_traffic('conv_single_' + WL_KEY)[1],
@@ -574,7 +578,7 @@ def time_kernels(dev, pk):
         for b in range(10):
             specs += [(pcs[1 + 2 * b], 1, 2, None), (pcs[2 + 2 * b], 2, 1, 1)]
         chain = ops.ConvChain(specs)
-        nb3 = min(3, nbuf)                       # bd4: 3 x (22 MB in + 2 x 22 MB work) = 198 MB > 126 MB L2
+        nb3 = min(3, nbuf)                       # bd4: 3 x (22 MB in + 2 x 22 MB work) = 198 MB > 50 MB L2
         sets = [[xs[i], ys[i], torch.empty_like(xs[i])] for i in range(nb3)]
         creps = 12
         t_chain = _time_graph(lambda i: chain(sets[i]), nb3, creps, torch)
@@ -616,6 +620,20 @@ def time_kernels(dev, pk):
             'bytes_actually_moved_per_launch': moved, 'moved_gbs': moved / t / 1e9,
             'peak_src': pk['src'], 'how': f'{reps} launches in one CUDA graph, {nb2} rotating buffer sets > L2'}
     return out
+
+
+def dump_outputs(out_dir, eng, p):
+    """What the timed step loop's last step handed to its caller: the fp32 HR frames (in full), the uint8
+    frames as a fixed, seeded sample of 2**20 values (float32) and the sample's flat indices (float64) --
+    45 MB for the bd4 workload."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    hr = eng.hr[p].float().cpu().numpy()
+    np.save(os.path.join(out_dir, 'hr.npy'), hr)
+    u8 = eng.u8[p].cpu().numpy().reshape(-1)
+    idx = np.sort(np.random.default_rng(0).choice(u8.size, size=min(u8.size, 1 << 20), replace=False))
+    np.save(os.path.join(out_dir, 'u8_sample.npy'), u8[idx].astype(np.float32))
+    np.save(os.path.join(out_dir, 'u8_sample_index.npy'), idx.astype(np.float64))
 
 
 def run_ours(args, rank, world, local_rank):
@@ -668,6 +686,8 @@ def run_ours(args, rank, world, local_rank):
     if world > 1:
         dist.barrier()
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, (Wm + K - 1) & 1)
     t = torch.tensor([ms], device=dev, dtype=torch.float64)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -737,7 +757,7 @@ def run_ours(args, rank, world, local_rank):
             fps, dt, cores, kind = cpu_reference_fps(steps_cpu, 1)
             cpu = {'value': fps, 'unit': 'frames/s', 'cores': cores, 'kind': kind,
                    'sample': f'{steps_cpu} steps x {n} lock-stepped clip-frames {"x".join(map(str, LR))} (fp32, '
-                             + ('unmodified reference FRNet.step from baseline/_ref' if kind == 'reference' else
+                             + ('unmodified reference FRNet.step from oracle/_ref' if kind == 'reference' else
                                 'port oracle/frnet_torchref.py') + f'), {dt:.1f} s of CPU work'}
             if not args.no_eager:
                 eager = eager_gpu_results(10, 3)
@@ -749,9 +769,9 @@ def run_ours(args, rank, world, local_rank):
             'config': workload_config(world),
             'notes': {
                 'l2': 'per-step working set ~1.3 GB of activations (HR 64-channel map alone 351 MB for 4 frames) '
-                      '>> 126 MB L2; no explicit flush', 'conv_impl': ops.default_conv_impl(),
+                      '>> 50 MB L2; no explicit flush', 'conv_impl': ops.default_conv_impl(),
                 'baseline_note': 'vs_baseline = value / 27 FPS published for 1x GTX 1080 Ti, batch 1, 4x BD '
-                                 '(resources/benchmark.png); no B200 number is published'},
+                                 '(resources/benchmark.png); no H100 number is published'},
             'gflop_per_frame': WL['flop_per_frame'] / 1e9,
             'model_tflops': value * WL['flop_per_frame'] / 1e12 / world,
             'model_tensor_frac_of_sustained': value * WL['flop_per_frame'] / 1e12 / world / pk['tflops_sustained'],
@@ -787,9 +807,14 @@ def main():
     ap.add_argument('--batch', type=int, default=0, help='training workloads: clips per GPU (default 32)')
     ap.add_argument('--sustain-s', type=float, default=3.0, help='seconds of the sustained block (0 = skip)')
     ap.add_argument('--no-eager', action='store_true', help='skip the gpu_eager_baseline block (N=1 only)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write the outputs of the last step as DIR/<name>.npy '
+                         '(inference workloads of --impl ours only; rejected otherwise)')
     ap.add_argument('--profile-only', action='store_true',
                     help='run only the device-resident step loop (for ncu captures); prints nothing')
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload.startswith('train') or args.impl != 'ours'):
+        ap.error('--dump-outputs is available for the inference workloads of --impl ours only')
     rank = int(os.environ.get('RANK', '0'))
     world = int(os.environ.get('WORLD_SIZE', '1'))
     local_rank = int(os.environ.get('LOCAL_RANK', '0'))

@@ -1,5 +1,6 @@
 /*
- * tecogan_b200.h -- C ABI of libtecogan_b200.so (sm_100a).
+ * tecogan_b200.h -- C ABI of libtecogan_b200.so (sm_90a, H100).  Entry points keep their
+ * historical *_tcgen05 names; on sm_90a they run wgmma kernels.
  *
  * The reference (skycrapers/TecoGAN-PyTorch @ 903b070) has NO native / FFI
  * boundary: its generator hot path is Python calling PyTorch library ops
@@ -52,7 +53,7 @@ enum {
   TG_CONV_3X3 = 0,
   TG_CONVT_3X3_S2 = 1,
   TG_CONV_3X3_S2 = 2    /* stride-2 conv, pad 1: y[oy,ox] = sum x[2oy+ky-1, 2ox+kx-1] * w[.,.,ky,kx] -- the data
-                           gradient of TG_CONVT_3X3_S2 (tcgen05: tap mode over the four parity planes of x) */
+                           gradient of TG_CONVT_3X3_S2 (wgmma: tap mode over the four parity planes of x) */
 };
 enum { TG_UP_BICUBIC = 0, TG_UP_BILINEAR = 1 };
 enum {
@@ -60,19 +61,19 @@ enum {
   TG_EPI_FLOW_NCHW_F32 = 1, /* y = 24*tanh(conv + bias)           -> NCHW fp32 [N,2,H,W] */
   TG_EPI_OUT_NCHW_F32 = 2,  /* y = conv + bias                    -> NCHW fp32 [N,C,H,W] */
   TG_EPI_NHWC_F16_POOL2 = 3 /* y = maxpool2x2(act(conv + bias))   -> NHWC fp16 [n,h/2,w/2,cout]: nn.MaxPool2d(2,2)
-                               (tecogan_nets.py:28,35,42) folded into the producing conv's epilogue (tcgen05 kernel,
+                               (tecogan_nets.py:28,35,42) folded into the producing conv's epilogue (wgmma kernel,
                                conv3x3 only, no residual); the full-resolution map is never written */
 };
 enum { TG_AMODE_AUTO = 0, TG_AMODE_HALO = 1, TG_AMODE_TAP = 2 };
 
 int tg_version(void);
 const char* tg_last_error_string(void);
-/* number of SMs of the current device (148 on B200) */
+/* number of SMs of the current device (132 on H100 SXM) */
 int tg_device_sm_count(int* out_sm_count);
 
 /* ------------------------------------------------------------------------
  * Weight packing (run once per optimizer step / checkpoint load).
- * Packed layout = the exact shared-memory image the tcgen05 kernel consumes:
+ * Packed layout = the exact shared-memory image the wgmma kernel consumes:
  * tiles [group g][chunk c][cout_pad rows][64 k] fp16, 128-byte rows with the
  * 128B swizzle (16-byte chunk index XOR (row & 7)); g = ky*3+kx for conv3x3.
  * ---------------------------------------------------------------------- */
@@ -103,7 +104,7 @@ int tg_pack_conv3x3_weights_tapn(const float* w_oihw, int cout, int cin, void* p
                                  void* stream);
 
 /* ------------------------------------------------------------------------
- * 3x3 convolution / stride-2 transposed convolution as tcgen05 implicit GEMM.
+ * 3x3 convolution / stride-2 transposed convolution as wgmma implicit GEMM.
  * Replaces nn.Conv2d+activation (tecogan_nets.py:23-65, 92-98, 111-116, 131),
  * nn.ConvTranspose2d+ReLU (:119-126), torch.tanh(.)*24 (:80) and the add of
  * `out += upsample_func(lr_curr)` (:145): TG_EPI_OUT_NCHW_F32 stores conv+bias and the caller
@@ -125,10 +126,10 @@ typedef struct tg_conv_desc {
   int32_t kind;         /* TG_CONV_3X3 | TG_CONVT_3X3_S2                                 */
   int32_t act;          /* TG_ACT_*                                                      */
   int32_t epilogue;     /* TG_EPI_*                                                      */
-  int32_t a_mode;       /* TG_AMODE_* (tcgen05 kernel only; AUTO = fastest validated)    */
+  int32_t a_mode;       /* TG_AMODE_* (wgmma kernel only; AUTO = fastest validated)      */
   int32_t max_ctas;     /* 0 = one persistent CTA per SM                                 */
-  int32_t cin_real;     /* input channels that can be non-zero (0 = cin): for cin = 64 the tcgen05 kernel skips the
-                           UMMA k-steps of 16 channels at or beyond it -- the packed weights are zero there, so the
+  int32_t cin_real;     /* input channels that can be non-zero (0 = cin): for cin = 64 the wgmma kernel skips the
+                           k-steps of 16 channels at or beyond it -- the packed weights are zero there, so the
                            result is bit-identical (thin layers: FNet 6->32, 32->32, 32->64, 32->2)  */
   const void* mask;     /* TG_ACT_DRELU / TG_ACT_DLRELU02: NHWC fp16, shape of y; else NULL */
 } tg_conv_desc;
@@ -142,7 +143,8 @@ int tg_conv_simt(const tg_conv_desc* d, void* stream);
  * SRNet tail in one launch: last nn.ConvTranspose2d(64,64,3,2,1,op=1) + ReLU -> conv_out (64 -> out_nc)
  * -> + upsample_func(lr_curr) (tecogan_nets.py:119-131,143-145), optionally also float32_to_uint8 +
  * CHW->HWC (data_utils.py:80-87, tecogan_nets.py:278-281).  The 64-channel HR map only exists as one
- * 32x16-pixel tile in shared memory instead of a round trip through HBM.
+ * 32x16-pixel tile in shared memory (four parity blocks, used directly as conv_out's wgmma operand)
+ * instead of a round trip through HBM.  No allocation, no synchronisation.
  * ---------------------------------------------------------------------- */
 typedef struct tg_tail_desc {
   const void* x;        /* input of the transposed conv, NHWC fp16 [n,h,w,64]                       */
@@ -167,22 +169,22 @@ int tg_convT_convout_tcgen05(const tg_tail_desc* d, void* stream);
 
 /* ------------------------------------------------------------------------
  * A chain of 64->64 3x3 convolutions (SRNet conv_in + the residual blocks,
- * tecogan_nets.py:92-100, 111-116, 139-141) as ONE persistent launch: every CTA walks all
+ * tecogan_nets.py:92-100, 111-116, 139-141) as ONE persistent cooperative launch: every CTA walks all
  * layers over its fixed set of 16x8 tiles; a tile of layer l starts as soon as the (up to 9)
  * tiles of layer l-1 under its 18x10 halo have been published (per-tile progress flags in
- * `sync_ws`), so there is no launch, pipeline fill/drain or whole-grid barrier between layers,
- * and the next layer's weights stream into a ring of shared-memory tap slots behind the current
- * layer.  Bit-identical to n_layers calls of tg_conv_tcgen05.
+ * `sync_ws`), so there is no launch or whole-grid barrier between layers.  Bit-identical to
+ * n_layers calls of tg_conv_tcgen05.
  *   layers[l].x / y / residual : NHWC fp16 [n,h,w,64]; y[l] is normally x[l+1].  y[l] may alias
  *       residual[l] (in place) or a buffer last READ by layer <= l-1; it must not alias x[l].
  *       At most 4 distinct x buffers per chain.
  *   sync_ws : device memory of tg_conv_chain_workspace_bytes(n,h,w) bytes, zeroed ONCE by the
- *       caller before first use, then owned by the library (epoch-stamped; one chain launch in
- *       flight per workspace).
- * Needs every CTA co-resident (grid = min(#SM, tiles), 1 CTA/SM): launch at most ONE chain at a
- * time per device (two chains racing for SMs from different streams can starve each other) and
- * do not run it under an SM partition smaller than the device (waits are bounded and trap
- * instead of hanging).
+ *       caller before first use, then owned by the library: word 0 = launch epoch, word 1 = count of
+ *       finished CTAs, then one progress flag per tile, stamped with the epoch.  One chain launch in
+ *       flight per workspace.
+ * Needs every CTA co-resident (grid = min(#SM, tiles), 1 CTA/SM, cooperative launch: the driver
+ * starts the grid only when all of its CTAs fit, or fails the launch): launch at most ONE chain at
+ * a time per device and do not run it under an SM partition smaller than the device (waits are
+ * bounded and trap instead of hanging).
  * ---------------------------------------------------------------------- */
 typedef struct tg_chain_layer {
   const void* x;        /* NHWC fp16 [n,h,w,64]                          */
@@ -281,15 +283,15 @@ int tg_bias_grad_nhwc_f16(const void* dz, size_t npix, int c, int c_real, const 
 /* Weight gradient of a conv3x3 / convT3x3s2 layer: dw += 1/scale * sum_p x[p+tap] (x) dz[p], written in
  * the parameter's own layout (nn.Conv2d [cout_real,cin_real,3,3]; nn.ConvTranspose2d
  * [cin_real,cout_real,3,3]) with fp32 atomics -- the caller zeroes dw (or accumulates on purpose).
- * tcgen05: GEMM over pixels (K), x and dz both channel-contiguous ("MN-major") operands. */
+ * wgmma: GEMM over pixels (K), x and dz both channel-contiguous ("MN-major") operands. */
 typedef struct tg_wgrad_desc {
   const void* x;        /* layer input,  NHWC fp16 [n,h,w,cin]                              */
   const void* dz;       /* gradient of the pre-activation output, NHWC fp16 [n,h,w,cout]
                            (convT: [n,2h,2w,cout]), loss-scaled                           */
   float* dw;            /* fp32 gradient, parameter layout                                  */
   const float* scale;   /* {scale, 1/scale} or NULL                                         */
-  float* db;            /* conv3x3 only, may be NULL: bias gradient db[co] += 1/scale * sum_p dz[p][co], computed by
-                           the same MMAs (the unused half of the last tap pair reads a block of ones) */
+  float* db;            /* conv3x3 only, may be NULL: bias gradient db[co] += 1/scale * sum_p dz[p][co]
+                           (tg_bias_grad_nhwc_f16 after the GEMM)                          */
   int32_t n, h, w;      /* of the layer INPUT                                               */
   int32_t cin, cout;    /* stored channel counts (64/128/256)                               */
   int32_t cin_real, cout_real;
@@ -339,10 +341,8 @@ int tg_st_disc_input_bwd_nchw_f32(const float* gout, const float* flow, float* g
 int tg_depth_to_space_nchw_f32(const float* gy, float* gx, int n, int c, int h, int w, int s, void* stream);
 
 /* ------------------------------------------------------------------------
- * Diagnostics: when a device buffer of 16*gridDim uint64 is registered, every
- * tg_conv_tcgen05 launch writes per-CTA role timers (cycles spent by the TMA
- * producer / MMA issuer / epilogue in each wait and work phase) into it.
- * NULL (default) disables timing. Layout: tools/conv_timers.py.
+ * Diagnostics: per-CTA role timers.  The sm_90a kernels record none: NULL is
+ * accepted (and is the default), a buffer returns TG_E_UNSUPPORTED.
  * ---------------------------------------------------------------------- */
 int tg_debug_set_conv_timers(void* device_buffer);
 

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY -- CPU precision model of the CUDA path.
 
-Same algorithm as frnet_torchref.step, but with the storage precision of the sm_100a kernels:
+Same algorithm as frnet_torchref.step, but with the storage precision of the sm_90a kernels:
 weights and every inter-layer activation rounded to fp16, accumulation / bias / activation /
 residual add in fp32, and the flow head, warp coordinates, bicubic residual and final output in
 fp32 (DESIGN.md "precision").  It separates two questions in the GPU tests:

@@ -1,9 +1,8 @@
 """Generate tests/golden/*.npz by running the UNMODIFIED reference
-(/root/reference, skycrapers/TecoGAN-PyTorch @ 903b070) on seeded inputs.
+(skycrapers/TecoGAN-PyTorch @ 903b070, installed into oracle/_ref by build()) on seeded inputs:
 
-Run in the build container only (the GPU box has no /root/reference):
-
-    python oracle/gen_golden.py
+    python oracle/gen_golden.py            # all fixtures
+    python oracle/gen_golden.py full       # only the full-size sample
 
 Import recipe = SURVEY.md section 9 (two module stubs, no edits to the reference).
 Inputs and weights are NOT stored: they are regenerated from seeds by
@@ -49,6 +48,21 @@ GRAD_FULL = ('fnet.encoder1.0.weight', 'fnet.flow.2.weight', 'fnet.flow.2.bias',
              'srnet.resblocks.1.conv.2.bias', 'srnet.conv_up.2.bias', 'srnet.conv_out.weight', 'srnet.conv_out.bias')
 
 
+def gen_full_size_sample(FRNet, out_dir):
+    """FRNet.step at the bench size (1 clip, 3x134x320 -> 536x1280, 2x weights): the full frame is 8 MB, so a
+    fixed, seeded sample of 65536 output values is stored with its flat indices."""
+    from oracle.frnet_oracle import make_frnet_params
+    net = FRNet(3, 3, 64, 10, 'BD', 4)
+    net.load_state_dict(make_frnet_params(5, gain=2.0), strict=True)
+    net.eval()
+    lr_curr, lr_prev, hr_prev = rand(1, 1, 3, 134, 320), rand(2, 1, 3, 134, 320), rand(3, 1, 3, 536, 1280)
+    with torch.no_grad():
+        hr = net.step(lr_curr, lr_prev, hr_prev).numpy().reshape(-1)
+    idx = np.sort(np.random.default_rng(0).choice(hr.size, size=1 << 16, replace=False))
+    np.savez_compressed(os.path.join(out_dir, 'step_bd4_134x320_g2_sample.npz'), index=idx.astype(np.int64),
+                        hr_curr=hr[idx].astype(np.float32))
+
+
 def gen_sequence_grads(FRNet, out_dir):
     from oracle.frnet_oracle import make_frnet_params
     net = FRNet(3, 3, 64, 2, 'BD', 4)
@@ -81,6 +95,8 @@ def main():
         return
     if sys.argv[1:] == ['grads']:
         return gen_sequence_grads(FRNet, out_dir)
+    if sys.argv[1:] == ['full']:
+        return gen_full_size_sample(FRNet, out_dir)
 
     def ref_model(scale, degradation, seed, gain, nb=10):
         net = FRNet(3, 3, 64, nb, degradation, scale)
@@ -132,6 +148,7 @@ def main():
     # loss = <hr_data, R1> + 0.05 <lr_flow, R2>; stored: loss, d/d lr_data, a few whole parameter
     # gradients and the L2 norm of every parameter gradient
     gen_sequence_grads(FRNet, out_dir)
+    gen_full_size_sample(FRNet, out_dir)
 
     # ---- 5. functional ops
     x = rand(20, 2, 3, 20, 24)

@@ -1,4 +1,4 @@
-"""tecogan-pytorch_b200: the FRNet generator hot path of TecoGAN-PyTorch on hand-written sm_100a
+"""tecogan-pytorch_b200: the FRNet generator hot path of TecoGAN-PyTorch on hand-written sm_90a
 kernels, behind the reference's Python surface.  Import with
 ``importlib.import_module('tecogan-pytorch_b200')`` or through the ``tecogan_b200`` alias module
 at the repo root."""

@@ -11,8 +11,8 @@ What autograd sees                                   reference lines
 
 Design (DESIGN.md section 8): activations are kept as the forward stored them (NHWC fp16, one buffer
 per layer covering all T frames), gradients travel between conv layers as loss-scaled NHWC fp16,
-  dgrad  = the forward tcgen05 implicit GEMM with swapped roles / flipped taps (+ act' epilogue),
-  wgrad  = a tcgen05 GEMM over pixels, ONE launch per layer over all T*n images,
+  dgrad  = the forward wgmma implicit GEMM with swapped roles / flipped taps (+ act' epilogue),
+  wgrad  = a wgmma GEMM over pixels, ONE launch per layer over all T*n images,
   warp   = scatter-add into the fp32 state gradient + gather for the flow gradient,
 parameter gradients come out fp32 in the parameters' own layouts.  Nothing here calls a PyTorch
 library kernel for arithmetic; torch is used for allocation, views and transposes of the fp32
@@ -55,7 +55,7 @@ def _param_grads(pc, module, x, dz, scale, grads):
     if n is not None:                      # [T,n,h,w,c] buffers: one launch over all T*n images
         x = x.view(-1, *x.shape[2:])
         dz = dz.view(-1, *dz.shape[2:])
-    # the bias gradient comes out of the same tcgen05 launch (conv layers) or a separate reduction (transposed convs)
+    # the bias gradient comes from the wgrad call (conv layers: a reduction after its GEMM) or a separate reduction
     ops.wgrad(pc, x, dz, grads.of(module.weight), scale, db=grads.of(module.bias))
 
 

@@ -16,7 +16,7 @@ namespace {
 
 inline int bgrid(size_t total, int block) {
   size_t g = (total + block - 1) / block;
-  const size_t cap = 148 * 32;
+  const size_t cap = (size_t)tg_sms() * 32;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
@@ -551,7 +551,7 @@ int tg_bias_grad_nhwc_f16(const void* dz, size_t npix, int c, int c_real, const 
   TG_REQUIRE(c > 0 && c % 8 == 0 && c <= 256 && c_real > 0 && c_real <= c, TG_E_UNSUPPORTED, "bias_grad: c=%d", c);
   const int c8 = c / 8, rows = 256 / c8;
   size_t blocks = (npix + (size_t)rows * 16 - 1) / ((size_t)rows * 16);
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > (size_t)tg_sms() * 4) blocks = (size_t)tg_sms() * 4;
   if (blocks < 1) blocks = 1;
   tg_launch(bias_grad_kernel, dim3((unsigned)blocks), dim3(256), (size_t)rows * c * sizeof(float),
             (cudaStream_t)stream, (const uint4*)dz, npix, c8, c_real, scale, db);

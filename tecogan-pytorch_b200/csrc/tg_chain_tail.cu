@@ -1,0 +1,598 @@
+// Two fused parts of SRNet on sm_90a (H100), built from the same TMA / mbarrier / wgmma pieces as
+// tg_conv_wgmma.cu:
+//
+// conv_chain_kernel -- SRNet conv_in + the residual blocks (64->64 3x3 convs) as ONE persistent
+//   cooperative launch.  Every CTA walks all layers over its fixed set of 16x8 tiles (halo mode: one
+//   18x10 TMA box per tile, the nine taps are shifted wgmma descriptor views of it).  A tile of layer l
+//   is loaded as soon as the (up to 9) tiles of layer l-1 under its halo have been published: per-tile
+//   progress flags in the caller's workspace, stamped with a launch epoch so the workspace is zeroed only
+//   once.  There is no launch, pipeline fill / drain or grid-wide barrier between layers; a layer's
+//   weights are reloaded into shared memory as soon as both consumers are done with the previous ones.
+//
+// convT_convout_kernel -- SRNet tail: last ConvTranspose2d(64,64,3,2,1,op=1) + ReLU -> conv_out 3x3
+//   (64 -> out_nc <= 3) -> + upsample_func(lr_curr) or + the pre-written frame -> fp32 NCHW (+ uint8 NHWC).
+//   Per 16x8 tile of the transposed conv's input (17x9 halo box): the four parity accumulators are
+//   computed one after the other and written, +bias, ReLU, fp16, straight from the wgmma fragments into
+//   shared memory as four 128-pixel K-major 128B-swizzled operand blocks (pixels outside the image are
+//   zero = conv_out's zero padding).  conv_out then runs as "tap-major N" wgmmas (N = 48 = 9 taps x 4
+//   couts) on those blocks; the tap products overwrite the block they came from, and the 3x3 shift-add
+//   produces the 30x14 interior HR pixels of the tile (tiles advance by 15x7 input pixels, the
+//   transposed conv is recomputed on a one-pixel ring).  The 64-channel HR map never reaches HBM.
+#include <cuda.h>
+
+#include <mutex>
+
+#include "tg_common.cuh"
+#include "tg_wgmma.cuh"
+
+namespace {
+
+constexpr int TH = 16, TW = 8;
+constexpr uint32_t kSmemLimit = 232448;
+constexpr uint32_t kWtBytes = 9 * 64 * 128;          // nine [64 cout][64 cin] fp16 weight tiles
+constexpr uint32_t kFlagBase = 32;                   // workspace words: [0] epoch, [1] done count, [32..] tile flags
+constexpr uint32_t kEpochStride = 32;                // flag value = epoch * 32 + layer + 1 (<= 24 layers)
+
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+EncodeTiledFn encode_fn() {
+  static EncodeTiledFn fn = nullptr;
+  static std::once_flag once;
+  std::call_once(once, [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<EncodeTiledFn>(p);
+  });
+  return fn;
+}
+// NHWC fp16 [n][h][w][64] with a (box_w x box_h) pixel box of all 64 channels, 128B swizzle
+int encode_c64(CUtensorMap* m, const void* ptr, int n, int h, int w, int box_w, int box_h) {
+  EncodeTiledFn fn = encode_fn();
+  TG_REQUIRE(fn != nullptr, TG_E_DRIVER, "cuTensorMapEncodeTiled not available from the driver");
+  cuuint64_t dims[4] = {64, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
+  cuuint64_t strides[3] = {128, (cuuint64_t)w * 128, (cuuint64_t)h * w * 128};
+  cuuint32_t box[4] = {64, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  TG_REQUIRE(r == CUDA_SUCCESS, TG_E_DRIVER, "cuTensorMapEncodeTiled failed (%d) n=%d h=%d w=%d", (int)r, n, h, w);
+  return TG_OK;
+}
+
+__device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release_u32(uint32_t* p, uint32_t v) {
+  asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// plain (L1-coherent within the SM) 16-byte load: chain residuals were written earlier in the same launch
+__device__ __forceinline__ uint4 ld_global_u4(const void* p) {
+  uint4 v;
+  asm volatile("ld.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
+  return v;
+}
+
+// halo-mode conv taps of one 16x8 tile: acc[h] (+)= A view(tap) x W[tap], tile rows 8h..8h+7.  box_w = 10 for
+// the conv (origin -1), 9 for the transposed conv (origin 0, groups of parity accumulator `acc_sel`).
+template <int KIND>
+__device__ __forceinline__ void halo_mmas(float (&acc)[2][32], uint32_t sa16, uint32_t w16, int acc_sel) {
+  constexpr int kBoxW = KIND == TG_CONV_3X3 ? TW + 2 : TW + 1;
+  constexpr int kOrg = KIND == TG_CONV_3X3 ? -1 : 0;
+  const uint64_t a_hi = gmma_desc_hi((uint32_t)kBoxW * 128u), b_hi = gmma_desc_hi(1024u);
+  constexpr uint32_t half16 = (8u * kBoxW * 128u) >> 4;
+#pragma unroll
+  for (int g = 0; g < 9; ++g) {
+    const TgGroup gr = tg_group(KIND, g);
+    if (KIND != TG_CONV_3X3 && gr.acc != acc_sel) continue;
+    const bool first = g == 0 || tg_group(KIND, g > 0 ? g - 1 : 0).acc != gr.acc;
+    const uint32_t a16 = sa16 + (uint32_t)((gr.dy - kOrg) * kBoxW + (gr.dx - kOrg)) * 8u;
+    const uint32_t b16 = w16 + (uint32_t)g * (kWtBytes / 9 / 16);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint32_t sc = (first && k == 0) ? 0u : 1u;
+      wgmma_n64(acc[0], a_hi | (uint64_t)(a16 + 2u * k), b_hi | (uint64_t)(b16 + 2u * k), sc);
+      wgmma_n64(acc[1], a_hi | (uint64_t)(a16 + half16 + 2u * k), b_hi | (uint64_t)(b16 + 2u * k), sc);
+    }
+  }
+}
+
+// ================================================================== conv chain
+constexpr int kChainThreads = 384;                   // producer warpgroup + 2 consumer warpgroups
+constexpr uint32_t kChainHalo = (TW + 2) * (TH + 2) * 128;           // 23040
+constexpr uint32_t kChainStage = (kChainHalo + 1023u) & ~1023u;      // 23552
+constexpr uint32_t kChainStride = 68;                                // fp32 staging row pitch (floats)
+constexpr uint32_t kChainScratch = 128 * kChainStride * 4;           // 34816 per consumer
+constexpr uint32_t kChainOffW = 2048;
+constexpr uint32_t kChainOffStage = kChainOffW + kWtBytes;           // 75776
+constexpr uint32_t kChainOffScratch = kChainOffStage + 2 * kChainStage;
+constexpr uint32_t kChainSmem = 1024 + kChainOffScratch + 2 * kChainScratch;
+static_assert(kChainSmem <= kSmemLimit, "chain smem");
+constexpr int kMaxMaps = 4;
+
+struct ChainLayerP {
+  const unsigned char* w;
+  const float* bias;
+  const __half* res;
+  __half* y;
+  int map, act;
+};
+struct ChainParams {
+  CUtensorMap maps[kMaxMaps];
+  ChainLayerP layers[TG_CHAIN_MAX_LAYERS];
+  int n_layers, n, h, w, tiles_x, tiles_y, num_tiles;
+  uint32_t* sync;
+};
+
+__global__ void __launch_bounds__(kChainThreads, 1) conv_chain_kernel(const __grid_constant__ ChainParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;
+  uint8_t* sm = smem_raw + (base - raw);
+  const int warp = __shfl_sync(0xFFFFFFFFu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+  const uint32_t bar_full = base, bar_empty = base + 16, bar_w = base + 32, bar_wfree = base + 40;
+
+  if (warp == 1 && lane == 0) {
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(bar_full + 8 * s, 1);
+      mbar_init(bar_empty + 8 * s, 4);
+    }
+    mbar_init(bar_w, 1);
+    mbar_init(bar_wfree, 8);               // every warp of both consumers, once per layer
+    fence_barrier_init();
+  }
+  __syncthreads();
+  const uint32_t epoch = *reinterpret_cast<volatile const uint32_t*>(p.sync);
+  uint32_t* flags = p.sync + kFlagBase;
+  const int grid = (int)gridDim.x;
+  const int cnt = (p.num_tiles - (int)blockIdx.x + grid - 1) / grid;   // tiles of this CTA per layer
+  const int per_img = p.tiles_x * p.tiles_y;
+
+  if (warp == 0) {
+    // ============================================================ producer: weights per layer + halo boxes
+    if (lane == 0) {
+      uint32_t phase[2] = {0, 0};
+      for (int l = 0; l < p.n_layers; ++l) {
+        const ChainLayerP& L = p.layers[l];
+        if (l > 0) mbar_wait_mma(bar_wfree, (uint32_t)(l - 1) & 1u);
+        mbar_expect_tx(bar_w, kWtBytes);
+        for (int t = 0; t < 9; ++t) bulk_load(base + kChainOffW + t * 8192u, L.w + (size_t)t * 8192u, 8192u, bar_w);
+        for (int k = 0; k < cnt; ++k) {
+          const int tile = (int)blockIdx.x + k * grid, cw = (l * cnt + k) & 1;
+          const int img = tile / per_img, rr = tile - img * per_img, ty = rr / p.tiles_x, tx = rr - ty * p.tiles_x;
+          if (l > 0) {
+            // the tiles of layer l-1 under this tile's halo must have been published
+            const uint32_t want = epoch * kEpochStride + (uint32_t)l;
+            for (int dy = -1; dy <= 1; ++dy)
+              for (int dx = -1; dx <= 1; ++dx) {
+                const int y2 = ty + dy, x2 = tx + dx;
+                if (y2 < 0 || y2 >= p.tiles_y || x2 < 0 || x2 >= p.tiles_x) continue;
+                const uint32_t* f = flags + img * per_img + y2 * p.tiles_x + x2;
+                if ((int)(ld_acquire_u32(f) - want) >= 0) continue;
+                const long long t0 = clock64();
+                while ((int)(ld_acquire_u32(f) - want) < 0) {
+                  if (clock64() - t0 > 3000000000LL) __trap();   // bounded: a missing CTA must not hang the GPU
+                }
+              }
+            fence_proxy_async_global();   // the halo is read by TMA (async proxy) after generic-proxy stores
+          }
+          const int s = cw;                 // one stage per consumer
+          mbar_wait_mma(bar_empty + 8 * s, phase[cw] ^ 1);
+          mbar_expect_tx(bar_full + 8 * s, kChainHalo);
+          tma_load_4d(base + kChainOffStage + (uint32_t)s * kChainStage, &p.maps[L.map], bar_full + 8 * s, 0,
+                      tx * TW - 1, ty * TH - 1, img);
+          phase[cw] ^= 1u;
+        }
+      }
+    }
+  } else if (warp >= 4) {
+    // ============================================================ consumers
+    const int cw = (warp - 4) >> 2;
+    const int r = threadIdx.x - 128 * (1 + cw), q = r >> 5;
+    float* S = reinterpret_cast<float*>(sm + kChainOffScratch + (uint32_t)cw * kChainScratch);
+    float* bias_s = reinterpret_cast<float*>(sm + 1024 + cw * 256);
+    const uint32_t sa16 = gmma_addr16(base + kChainOffStage + (uint32_t)cw * kChainStage);
+    const uint32_t w16 = gmma_addr16(base + kChainOffW);
+    const int bar_id = 1 + cw;
+    uint32_t phase = 0;
+    float acc[2][32];
+    for (int l = 0; l < p.n_layers; ++l) {
+      const ChainLayerP& L = p.layers[l];
+      if (r < 64) bias_s[r] = __ldg(L.bias + r);
+      named_bar_sync(bar_id, 128);
+      mbar_wait_mma(bar_w, (uint32_t)l & 1u);
+      for (int k = 0; k < cnt; ++k) {
+        if (((l * cnt + k) & 1) != cw) continue;
+        const int tile = (int)blockIdx.x + k * grid;
+        const int img = tile / per_img, rr = tile - img * per_img, ty = rr / p.tiles_x, tx = rr - ty * p.tiles_x;
+        mbar_wait_mma(bar_full + 8 * cw, phase);
+        phase ^= 1u;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
+        wgmma_fence();
+        halo_mmas<TG_CONV_3X3>(acc, sa16, w16, 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_empty + 8 * cw);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int i = 0; i < 32; i += 2) {
+            const int row = h * 64 + q * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+            const int col = 8 * (i >> 2) + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(S + row * kChainStride + col) = make_float2(acc[h][i], acc[h][i + 1]);
+          }
+        named_bar_sync(bar_id, 128);
+        // epilogue: thread = pixel, act(acc + bias) [+ residual] -> fp16 -> the pixel's 128-byte NHWC row
+        const int py = ty * TH + (r >> 3), px = tx * TW + (r & 7);
+        if (py < p.h && px < p.w) {
+          const size_t off = (((size_t)img * p.h + py) * p.w + px) * 64;
+          const float* srow = S + r * kChainStride;
+#pragma unroll
+          for (int c8 = 0; c8 < 8; ++c8) {
+            uint4 rv = make_uint4(0u, 0u, 0u, 0u);
+            if (L.res) rv = ld_global_u4(L.res + off + c8 * 8);
+            const __half2* rh = reinterpret_cast<const __half2*>(&rv);
+            const float4 a0 = reinterpret_cast<const float4*>(srow + c8 * 8)[0];
+            const float4 a1 = reinterpret_cast<const float4*>(srow + c8 * 8)[1];
+            const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+            uint4 ov;
+            __half2* o = reinterpret_cast<__half2*>(&ov);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              float v0 = tg_act(av[2 * j] + bias_s[c8 * 8 + 2 * j], L.act);
+              float v1 = tg_act(av[2 * j + 1] + bias_s[c8 * 8 + 2 * j + 1], L.act);
+              if (L.res) {
+                const float2 rf = __half22float2(rh[j]);
+                v0 += rf.x; v1 += rf.y;
+              }
+              o[j] = __floats2half2_rn(v0, v1);
+            }
+            *reinterpret_cast<uint4*>(L.y + off + c8 * 8) = ov;
+          }
+        }
+        named_bar_sync(bar_id, 128);
+        if (r == 0) {
+          __threadfence();
+          st_release_u32(flags + tile, epoch * kEpochStride + (uint32_t)l + 1u);
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_wfree);   // this consumer no longer reads layer l's weights
+    }
+  }
+  // the last CTA to finish advances the epoch for the next launch on this workspace
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    const uint32_t done = atomicAdd(p.sync + 1, 1u);
+    if (done == gridDim.x - 1) {
+      p.sync[1] = 0;
+      __threadfence();
+      atomicAdd(p.sync, 1u);
+    }
+  }
+}
+
+// ================================================================== SRNet tail
+constexpr int kTailThreads = 256;                    // producer warpgroup + 1 consumer warpgroup
+constexpr int kStepY = 15, kStepX = 7;               // input pixels a tile advances by
+constexpr uint32_t kTailHalo = (TW + 1) * (TH + 1) * 128;            // 19584
+constexpr uint32_t kTailStage = (kTailHalo + 1023u) & ~1023u;        // 20480
+constexpr uint32_t kWoBytes = TG_TAPN_ROWS * 128;                    // [48 rows = tap*4+co][64]
+constexpr uint32_t kHrBlock = 128 * 128;                             // one parity block: 128 px x 128 B
+constexpr uint32_t kTailOffWt = 2048;
+constexpr uint32_t kTailOffWo = kTailOffWt + kWtBytes;               // 75776
+constexpr uint32_t kTailOffStage = kTailOffWo + kWoBytes;            // 81920
+constexpr uint32_t kTailOffHr = kTailOffStage + 2 * kTailStage;      // 122880
+constexpr uint32_t kTailSmem = 1024 + kTailOffHr + 4 * kHrBlock;     // 189440
+static_assert(kTailSmem <= kSmemLimit, "tail smem");
+constexpr int kD2Pitch = 27;                         // tap products kept per HR pixel: 9 taps x 3 couts (fp32)
+static_assert(128 * kD2Pitch * 4 <= (int)kHrBlock, "tap products of a block fit into the block");
+
+struct TailParams {
+  CUtensorMap map_x;
+  const unsigned char* w_up;
+  const unsigned char* w_out;
+  const float* b_up;
+  const float* b_out;
+  const float* lr;
+  float* y;
+  uint8_t* y_u8;
+  int n, h, w, cout_real, lr_scale, up_mode, accumulate;
+  int tiles_x, tiles_y, num_tiles;
+};
+
+__global__ void __launch_bounds__(kTailThreads, 1) convT_convout_kernel(const __grid_constant__ TailParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;
+  uint8_t* sm = smem_raw + (base - raw);
+  const int warp = __shfl_sync(0xFFFFFFFFu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+  const uint32_t bar_full = base, bar_empty = base + 16, bar_w = base + 32;
+  float* bup_s = reinterpret_cast<float*>(sm + 1024);
+  float* bout_s = reinterpret_cast<float*>(sm + 1024 + 256);
+
+  if (warp == 1 && lane == 0) {
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(bar_full + 8 * s, 1);
+      mbar_init(bar_empty + 8 * s, 4);
+    }
+    mbar_init(bar_w, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  // weights are static: load them before the programmatic-dependent-launch wait
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&p.map_x);
+    mbar_expect_tx(bar_w, kWtBytes + kWoBytes);
+    for (int t = 0; t < 9; ++t) bulk_load(base + kTailOffWt + t * 8192u, p.w_up + (size_t)t * 8192u, 8192u, bar_w);
+    bulk_load(base + kTailOffWo, p.w_out, kWoBytes, bar_w);
+  }
+  tg_pdl_wait();
+  tg_pdl_trigger();
+  if (threadIdx.x < 64) bup_s[threadIdx.x] = __ldg(p.b_up + threadIdx.x);
+  if (threadIdx.x < 4) bout_s[threadIdx.x] = threadIdx.x < p.cout_real ? __ldg(p.b_out + threadIdx.x) : 0.f;
+  __syncthreads();
+  const int per_img = p.tiles_x * p.tiles_y;
+
+  if (warp == 0) {
+    if (lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        const int img = tile / per_img, rr = tile - img * per_img;
+        const int y0 = (rr / p.tiles_x) * kStepY - 1, x0 = (rr % p.tiles_x) * kStepX - 1;
+        mbar_wait_mma(bar_empty + 8 * stage, phase ^ 1);
+        mbar_expect_tx(bar_full + 8 * stage, kTailHalo);
+        tma_load_4d(base + kTailOffStage + (uint32_t)stage * kTailStage, &p.map_x, bar_full + 8 * stage, 0, x0, y0,
+                    img);
+        if (++stage == 2) { stage = 0; phase ^= 1u; }
+      }
+    }
+  } else if (warp >= 4) {
+    const int r = threadIdx.x - 128, q = r >> 5;
+    const uint32_t hr = base + kTailOffHr;
+    uint8_t* hr_p = sm + kTailOffHr;
+    const uint32_t wt16 = gmma_addr16(base + kTailOffWt);
+    const uint64_t b_hi = gmma_desc_hi(1024u);
+    const uint32_t wo16 = gmma_addr16(base + kTailOffWo);
+    const int H = 2 * p.h, W = 2 * p.w;
+    const int lh = H / p.lr_scale, lw = W / p.lr_scale;
+    int stage = 0;
+    uint32_t phase = 0;
+    mbar_wait_mma(bar_w, 0);
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      const int img = tile / per_img, rr = tile - img * per_img;
+      const int y0 = (rr / p.tiles_x) * kStepY - 1, x0 = (rr % p.tiles_x) * kStepX - 1;
+      mbar_wait_mma(bar_full + 8 * stage, phase);
+      const uint32_t sa16 = gmma_addr16(base + kTailOffStage + (uint32_t)stage * kTailStage);
+      // 1. transposed conv, one parity accumulator at a time -> +bias, ReLU, fp16 -> HR operand block a
+      {
+        float acc[2][32];
+#pragma unroll 1
+        for (int a = 0; a < 4; ++a) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
+          wgmma_fence();
+          halo_mmas<TG_CONVT_3X3_S2>(acc, sa16, wt16, a);
+          wgmma_commit();
+          wgmma_wait<0>();
+          if (a == 3) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(bar_empty + 8 * stage);
+          }
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < 32; i += 2) {
+              const int row = h * 64 + q * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+              const int col = 8 * (i >> 2) + 2 * (lane & 3);
+              const int iy = y0 + (row >> 3), ix = x0 + (row & 7);
+              const bool in = iy >= 0 && iy < p.h && ix >= 0 && ix < p.w;
+              const float v0 = in ? tg_act(acc[h][i] + bup_s[col], TG_ACT_RELU) : 0.f;
+              const float v1 = in ? tg_act(acc[h][i + 1] + bup_s[col + 1], TG_ACT_RELU) : 0.f;
+              *reinterpret_cast<__half2*>(hr_p + a * kHrBlock + row * 128 + ((((col >> 3) ^ (row & 7))) << 4) +
+                                          (col & 7) * 2) = __floats2half2_rn(v0, v1);
+            }
+        }
+      }
+      if (++stage == 2) { stage = 0; phase ^= 1u; }
+      fence_proxy_async_smem();     // generic-proxy writes -> read by wgmma (async proxy)
+      named_bar_sync(1, 128);
+      // 2. conv_out as tap-major N (N = 48) on each parity block; the tap products replace the block
+#pragma unroll 1
+      for (int blk = 0; blk < 4; ++blk) {
+        float d2[2][24];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int i = 0; i < 24; ++i) d2[h][i] = 0.f;
+        const uint32_t a16 = gmma_addr16(hr + blk * kHrBlock);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          wgmma_n48(d2[0], b_hi | (uint64_t)(a16 + 2u * k), b_hi | (uint64_t)(wo16 + 2u * k), k > 0 ? 1u : 0u);
+          wgmma_n48(d2[1], b_hi | (uint64_t)(a16 + 512u + 2u * k), b_hi | (uint64_t)(wo16 + 2u * k), k > 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        named_bar_sync(1, 128);      // every warp is done reading the block
+        float* D2 = reinterpret_cast<float*>(hr_p + blk * kHrBlock);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int i = 0; i < 24; ++i) {
+            const int row = h * 64 + q * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+            const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);   // = tap * 4 + co
+            if (col < 36 && (col & 3) < 3) D2[row * kD2Pitch + (col >> 2) * 3 + (col & 3)] = d2[h][i];
+          }
+      }
+      named_bar_sync(1, 128);
+      // 3. shift-add over the 32x16 HR pixels of the tile: interior 30x14 are outputs
+#pragma unroll 1
+      for (int j = 0; j < 4; ++j) {
+        const int P = r + 128 * j, Y = P >> 4, X = P & 15;
+        const int gy = 2 * y0 + Y, gx = 2 * x0 + X;
+        if (Y < 1 || Y > 30 || X < 1 || X > 14 || gy < 0 || gy >= H || gx < 0 || gx >= W) continue;
+        float o[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap) {
+          const int Yn = Y + tap / 3 - 1, Xn = X + tap % 3 - 1;
+          const float* D2 = reinterpret_cast<const float*>(hr_p + ((Yn & 1) * 2 + (Xn & 1)) * kHrBlock) +
+                            ((Yn >> 1) * 8 + (Xn >> 1)) * kD2Pitch + tap * 3;
+#pragma unroll
+          for (int co = 0; co < 3; ++co) o[co] += D2[co];
+        }
+        uint32_t q8[3] = {0u, 0u, 0u};
+        for (int co = 0; co < p.cout_real; ++co) {
+          float* yp = p.y + (((size_t)img * p.cout_real + co) * H + gy) * W + gx;
+          float v = o[co] + bout_s[co];
+          if (p.accumulate) v = *yp + v;
+          else if (p.lr) v = v + tg_upsample_at(p.lr + ((size_t)img * p.cout_real + co) * lh * lw, lh, lw, lh, lw,
+                                                p.lr_scale, p.up_mode, gy, gx);
+          *yp = v;
+          q8[co] = (uint32_t)fminf(fmaxf(rintf(v * 255.f), 0.f), 255.f);
+        }
+        if (p.y_u8) {
+          uint8_t* up = p.y_u8 + (((size_t)img * H + gy) * W + gx) * p.cout_real;
+          for (int co = 0; co < p.cout_real; ++co) up[co] = (uint8_t)q8[co];
+        }
+      }
+      named_bar_sync(1, 128);        // the HR blocks are rewritten by the next tile
+    }
+  }
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t tg_conv_chain_workspace_bytes(int n, int h, int w) {
+  if (n <= 0 || h <= 0 || w <= 0) return 0;
+  const size_t tiles = (size_t)tg_ceil_div(w, TW) * tg_ceil_div(h, TH) * n;
+  return (kFlagBase + tiles) * sizeof(uint32_t);
+}
+
+int tg_conv_chain_tcgen05(const tg_chain_layer* layers, int n_layers, int n, int h, int w, void* sync_ws,
+                          int max_ctas, void* stream) {
+  TG_REQUIRE(layers != nullptr && sync_ws != nullptr, TG_E_INVALID, "conv_chain: null pointer");
+  TG_REQUIRE(n_layers >= 1 && n_layers <= TG_CHAIN_MAX_LAYERS, TG_E_UNSUPPORTED,
+             "conv_chain: n_layers=%d (1..%d)", n_layers, TG_CHAIN_MAX_LAYERS);
+  TG_REQUIRE(n > 0 && h > 0 && w > 0, TG_E_INVALID, "conv_chain: bad size n=%d h=%d w=%d", n, h, w);
+  TG_REQUIRE(((uintptr_t)sync_ws & 15) == 0, TG_E_INVALID, "conv_chain: sync_ws must be 16-byte aligned");
+  ChainParams p;
+  p.n_layers = n_layers; p.n = n; p.h = h; p.w = w;
+  p.tiles_x = tg_ceil_div(w, TW);
+  p.tiles_y = tg_ceil_div(h, TH);
+  p.num_tiles = p.tiles_x * p.tiles_y * n;
+  p.sync = reinterpret_cast<uint32_t*>(sync_ws);
+  const void* bufs[kMaxMaps];
+  int n_maps = 0;
+  for (int l = 0; l < n_layers; ++l) {
+    const tg_chain_layer& s = layers[l];
+    TG_REQUIRE(s.x && s.weights && s.bias && s.y, TG_E_INVALID, "conv_chain: layer %d: null pointer", l);
+    TG_REQUIRE(s.act >= TG_ACT_NONE && s.act <= TG_ACT_LRELU02, TG_E_INVALID, "conv_chain: layer %d: act", l);
+    TG_REQUIRE(s.reserved == 0, TG_E_INVALID, "conv_chain: layer %d: reserved must be 0", l);
+    TG_REQUIRE(s.y != s.x, TG_E_INVALID, "conv_chain: layer %d: y aliases x (halo reads of other tiles)", l);
+    TG_REQUIRE(((uintptr_t)s.x & 15) == 0 && ((uintptr_t)s.y & 31) == 0 && ((uintptr_t)s.weights & 15) == 0 &&
+                   ((uintptr_t)s.residual & 31) == 0 && ((uintptr_t)s.bias & 3) == 0,
+               TG_E_INVALID, "conv_chain: layer %d: pointer alignment", l);
+    int m = -1;
+    for (int i = 0; i < n_maps; ++i)
+      if (bufs[i] == s.x) m = i;
+    if (m < 0) {
+      TG_REQUIRE(n_maps < kMaxMaps, TG_E_UNSUPPORTED, "conv_chain: more than %d distinct input buffers", kMaxMaps);
+      const int rc = encode_c64(&p.maps[n_maps], s.x, n, h, w, TW + 2, TH + 2);
+      if (rc != TG_OK) return rc;
+      bufs[n_maps] = s.x;
+      m = n_maps++;
+    }
+    p.layers[l] = ChainLayerP{reinterpret_cast<const unsigned char*>(s.weights), s.bias,
+                              reinterpret_cast<const __half*>(s.residual), reinterpret_cast<__half*>(s.y), m, s.act};
+  }
+  for (int i = n_maps; i < kMaxMaps; ++i) p.maps[i] = p.maps[0];
+  for (int l = n_layers; l < TG_CHAIN_MAX_LAYERS; ++l) p.layers[l] = p.layers[0];
+
+  static TgPerDeviceOnce attr_once;
+  const cudaError_t attr_err = attr_once.run([] {
+    return cudaFuncSetAttribute(conv_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kChainSmem);
+  });
+  TG_REQUIRE(attr_err == cudaSuccess, (int)attr_err, "conv_chain: cudaFuncSetAttribute: %s", cudaGetErrorString(attr_err));
+  int sms = 0;
+  int rc = tg_device_sm_count(&sms);
+  if (rc != TG_OK) return rc;
+  // Every CTA must be resident at once (tiles wait on tiles of other CTAs): one CTA per SM, and a
+  // COOPERATIVE launch, so the driver starts the grid only when all of its CTAs can be co-scheduled.
+  int per_sm = 0;
+  const cudaError_t oerr =
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, conv_chain_kernel, kChainThreads, kChainSmem);
+  TG_REQUIRE(oerr == cudaSuccess, (int)oerr, "conv_chain: occupancy query: %s", cudaGetErrorString(oerr));
+  TG_REQUIRE(per_sm >= 1, TG_E_UNSUPPORTED, "conv_chain: kernel does not fit on an SM of this device");
+  int grid = (max_ctas > 0 && max_ctas < sms) ? max_ctas : sms;
+  if (grid > p.num_tiles) grid = p.num_tiles;
+  const cudaError_t lerr =
+      tg_launch_cooperative(conv_chain_kernel, dim3(grid), dim3(kChainThreads), kChainSmem, (cudaStream_t)stream, p);
+  TG_REQUIRE(lerr == cudaSuccess, (int)lerr, "conv_chain: launch failed: %s", cudaGetErrorString(lerr));
+  TG_CUDA_LAUNCH_CHECK("conv_chain");
+  return TG_OK;
+}
+
+int tg_convT_convout_tcgen05(const tg_tail_desc* d, void* stream) {
+  TG_REQUIRE(d != nullptr, TG_E_INVALID, "convT_convout: null descriptor");
+  TG_REQUIRE(d->x && d->w_up && d->b_up && d->w_out && d->b_out && d->y, TG_E_INVALID, "convT_convout: null pointer");
+  TG_REQUIRE(d->n > 0 && d->h > 0 && d->w > 0, TG_E_INVALID, "convT_convout: bad size");
+  TG_REQUIRE(d->cout_real >= 1 && d->cout_real <= 3, TG_E_UNSUPPORTED, "convT_convout: out_nc=%d (1..3)", d->cout_real);
+  TG_REQUIRE(d->reserved == 0, TG_E_INVALID, "convT_convout: reserved must be 0");
+  TG_REQUIRE(!(d->accumulate && d->lr), TG_E_INVALID, "convT_convout: accumulate and lr are exclusive");
+  TG_REQUIRE(((uintptr_t)d->x & 15) == 0 && ((uintptr_t)d->w_up & 15) == 0 && ((uintptr_t)d->w_out & 15) == 0 &&
+                 ((uintptr_t)d->y & 7) == 0, TG_E_INVALID, "convT_convout: pointer alignment");
+  if (d->lr != nullptr) {
+    TG_REQUIRE(d->lr_scale == 2 || d->lr_scale == 4, TG_E_UNSUPPORTED, "convT_convout: lr_scale %d (2 or 4)", d->lr_scale);
+    TG_REQUIRE((2 * d->h) % d->lr_scale == 0 && (2 * d->w) % d->lr_scale == 0, TG_E_INVALID,
+               "convT_convout: output size is not lr_scale x the LR size");
+    TG_REQUIRE(d->up_mode == TG_UP_BICUBIC || d->up_mode == TG_UP_BILINEAR, TG_E_INVALID, "convT_convout: up_mode");
+  }
+  TailParams p;
+  int rc = encode_c64(&p.map_x, d->x, d->n, d->h, d->w, TW + 1, TH + 1);
+  if (rc != TG_OK) return rc;
+  p.w_up = reinterpret_cast<const unsigned char*>(d->w_up);
+  p.w_out = reinterpret_cast<const unsigned char*>(d->w_out);
+  p.b_up = d->b_up; p.b_out = d->b_out; p.lr = d->lr; p.y = d->y; p.y_u8 = d->y_u8;
+  p.n = d->n; p.h = d->h; p.w = d->w; p.cout_real = d->cout_real;
+  p.lr_scale = d->lr ? d->lr_scale : 2; p.up_mode = d->up_mode; p.accumulate = d->accumulate;
+  // HR rows -1 .. 2h-1 are covered in strips of 30 (the first strip starts at the even row -2)
+  p.tiles_y = tg_ceil_div(2 * d->h + 1, 2 * kStepY);
+  p.tiles_x = tg_ceil_div(2 * d->w + 1, 2 * kStepX);
+  p.num_tiles = p.tiles_x * p.tiles_y * d->n;
+  static TgPerDeviceOnce attr_once;
+  const cudaError_t attr_err = attr_once.run([] {
+    return cudaFuncSetAttribute(convT_convout_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTailSmem);
+  });
+  TG_REQUIRE(attr_err == cudaSuccess, (int)attr_err, "convT_convout: cudaFuncSetAttribute: %s",
+             cudaGetErrorString(attr_err));
+  int sms = 0;
+  rc = tg_device_sm_count(&sms);
+  if (rc != TG_OK) return rc;
+  int grid = d->max_ctas > 0 && d->max_ctas < sms ? d->max_ctas : sms;
+  if (grid > p.num_tiles) grid = p.num_tiles;
+  const cudaError_t lerr =
+      tg_launch(convT_convout_kernel, dim3(grid), dim3(kTailThreads), kTailSmem, (cudaStream_t)stream, p);
+  TG_REQUIRE(lerr == cudaSuccess, (int)lerr, "convT_convout: launch failed: %s", cudaGetErrorString(lerr));
+  TG_CUDA_LAUNCH_CHECK("convT_convout");
+  return TG_OK;
+}
+
+}  // extern "C"

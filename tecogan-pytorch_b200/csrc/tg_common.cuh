@@ -1,4 +1,4 @@
-// Shared host/device helpers for libtecogan_b200 (sm_100a only).
+// Shared host/device helpers for libtecogan_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -29,6 +29,11 @@ void tg_set_error(const char* fmt, ...);
   } while (0)
 
 static inline int tg_ceil_div(int a, int b) { return (a + b - 1) / b; }
+// SMs of the current device, for grid caps (1 if the query fails: a small grid is still correct)
+static inline int tg_sms() {
+  int s = 0;
+  return tg_device_sm_count(&s) == TG_OK && s > 0 ? s : 1;
+}
 
 // ---------------------------------------------------------------- programmatic dependent launch
 // Every kernel of the library is launched with cudaLaunchAttributeProgrammaticStreamSerialization

@@ -132,7 +132,7 @@ static int pack_common(const float* w, int kind, int cout, int cin, void* packed
              "pack_weights: cin_pad %% 64, cout_pad %% 16, cout_pad <= 256 required");
   const size_t total = (size_t)9 * cin_pad * cout_pad;
   int grid = (int)((total + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > tg_sms() * 16) grid = tg_sms() * 16;
   tg_launch(pack_weights_kernel, dim3(grid), dim3(256), 0, (cudaStream_t)stream, w, (__half*)packed, kind, cout, cin,
             cout_pad, cin_pad, dgrad);
   TG_CUDA_LAUNCH_CHECK("pack_weights");
@@ -186,7 +186,7 @@ int tg_conv_simt(const tg_conv_desc* d, void* stream) {
   const size_t total = (size_t)d->n * d->h * d->w * n_acc *
                        (d->epilogue != TG_EPI_NHWC_F16 ? 1 : d->cout / 8);
   size_t grid = (total + 127) / 128;
-  if (grid > 148 * 64) grid = 148 * 64;
+  if (grid > (size_t)tg_sms() * 64) grid = (size_t)tg_sms() * 64;
   tg_launch(conv_simt_kernel, dim3((unsigned)grid), dim3(128), 0, (cudaStream_t)stream, *d);
   TG_CUDA_LAUNCH_CHECK("conv_simt");
   return TG_OK;

@@ -1,0 +1,705 @@
+// 3x3 convolution / stride-2 transposed convolution / stride-2 convolution as a persistent,
+// warp-specialised wgmma implicit GEMM for sm_90a (H100).
+//
+//   M tile  = 128 output pixels = a 16x8 patch of one image (row m <-> pixel (m>>3, m&7)), issued as
+//             two m64 wgmmas (tile rows 0-7 and 8-15)
+//   N       = 64 output channels per CTA (layers with 128 / 256 are split over 2 / 4 CTAs); 48 for
+//             the thin heads (MODE_TAPN: 9 taps x 4 couts in N, 3x3 shift-add in the epilogue)
+//   K       = 64-channel chunks x 9 taps; wgmma K = 16 -> 4 k-steps per (tap, chunk)
+//   A       : NHWC fp16 activations, fetched by TMA (4-D tiled map, 128B swizzle, OOB zero fill =
+//             the conv's zero padding) either as ONE halo box (18x10 px) per (tile, chunk) whose
+//             nine shifted views are addressed through the wgmma descriptor (start address +=
+//             (dy*10+dx)*128 B, 8-row-group stride = 10*128 B), or as one 16x8 box per tap.
+//   B       : weights pre-packed on the device in the exact swizzled smem image
+//             (tg_pack_*_weights), either resident in smem for the whole kernel (SRNet, thin
+//             FNet layers) or streamed per (tap, chunk) with cp.async.bulk (fat FNet layers).
+//   D       : fp32 accumulators in the registers of the consumer warpgroup (64 per thread).
+//   roles   : warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers that take the
+//             CTA's tiles alternately, each with its own ring of smem stages: wgmma -> accumulators
+//             staged to a per-consumer fp32 smem tile -> one thread per pixel applies bias / act /
+//             residual (or the derivative, pool, pixel-shuffle and thin-head epilogues) and writes
+//             the pixel's 128-byte NHWC row.  One consumer's epilogue overlaps the other's MMAs.
+//             The transposed conv keeps 4 parity accumulators (1/2/2/4 taps), computed and stored
+//             one after the other; each stores its pixel's output of that parity (pixel shuffle).
+#include <cuda.h>
+
+#include <cstdlib>
+#include <mutex>
+
+#include "tg_common.cuh"
+#include "tg_epilogue.cuh"
+#include "tg_wgmma.cuh"
+
+namespace {
+
+constexpr int TH = 16, TW = 8;
+constexpr int kThreads = 384;             // producer warpgroup + 2 consumer warpgroups
+constexpr int kMaxRing = 4;               // smem stages per consumer ring
+constexpr uint32_t kHeaderBytes = 2048;   // barriers (first 1 KB) + bias (second 1 KB)
+constexpr uint32_t kTapABytes = TH * TW * 128;  // 16 KB
+constexpr uint32_t kSmemLimit = 232448;   // 227 KB opt-in limit per CTA
+// A-operand modes (template parameter MODE)
+constexpr int MODE_TAP = 0;    // one 16x8 box per (tap, chunk)
+constexpr int MODE_HALO = 1;   // one 18x10 halo box per (tile, chunk), taps = descriptor shifts
+constexpr int MODE_TAPN = 2;   // thin heads: one 16x8 box per (tile, chunk), N = 9 taps x 4 couts,
+                               // 3x3 shift-add in the epilogue; tiles overlap by one pixel ring
+constexpr int kTapnStepY = TH - 2, kTapnStepX = TW - 2;   // 14 x 6 valid outputs per TAPN tile
+// fp32 staging tile of a consumer: 128 rows x (N + 4) floats (the pad keeps the per-row float4
+// reads of the epilogue free of bank conflicts)
+__host__ __device__ constexpr uint32_t stage_stride(int mode) { return mode == MODE_TAPN ? 52u : 68u; }
+__host__ __device__ constexpr uint32_t scratch_bytes(int mode) { return 128u * stage_stride(mode) * 4u; }
+// up to four tensor maps: [0] = the NHWC input; TG_CONV_3X3_S2 reads the input's four parity planes
+struct TgMaps { CUtensorMap m[4]; };
+
+struct KParams {
+  tg_conv_desc d;
+  int tiles_x, tiles_y, num_tiles;
+  int chunks, n_acc;
+  int halo, b_resident;
+  int box_w, box_h, org_x, org_y;
+  int step_y, step_x;              // output pixels a tile advances by (16x8; 14x6 for MODE_TAPN)
+  int ring;                        // smem stages per consumer
+  int ksteps;                      // wgmma k-steps (16 channels) per 64-channel chunk that can hold non-zero input (1..4)
+  int n_split, bn;                 // output channels are split over n_split CTAs of bn columns
+  uint32_t stage_bytes, a_bytes, b_tile_bytes, b_stage_bytes;
+  uint32_t off_b, off_stage, off_scratch;
+};
+
+struct TileCoord { int n, y0, x0, nb; };
+__device__ __forceinline__ TileCoord tile_coord(const KParams& p, int tile) {
+  TileCoord t;
+  const int per_img = p.tiles_x * p.tiles_y;
+  const int sp = tile / p.n_split;          // CTAs that share an A tile are adjacent (L2 reuse)
+  t.nb = tile - sp * p.n_split;
+  t.n = sp / per_img;
+  const int r = sp - t.n * per_img;
+  t.y0 = (r / p.tiles_x) * p.step_y;
+  t.x0 = (r % p.tiles_x) * p.step_x;
+  return t;
+}
+
+__device__ __forceinline__ void st_global_128x2(void* ptr, const uint4& a, const uint4& b) {
+  uint4* q = reinterpret_cast<uint4*>(ptr);
+  q[0] = a;
+  q[1] = b;
+}
+
+// NHWC epilogue of one accumulator for the pixel of tile row r: 64 fp32 values in S[r] -> act(acc + bias)
+// [+ residual] (or the derivative epilogue) -> fp16 -> the pixel's 128-byte NHWC row.
+template <int KIND, bool BWD, bool POOL>
+__device__ __forceinline__ void epilogue_nhwc(const KParams& p, const TileCoord& tc, int r, int lane, int acc,
+                                              const float* S, const float* bias_s) {
+  const tg_conv_desc& d = p.d;
+  const int ty = r >> 3, tx = r & 7;
+  const int py = tc.y0 + ty, px = tc.x0 + tx;
+  const bool inb = py < d.h && px < d.w;
+  constexpr bool kCanRes = KIND != TG_CONVT_3X3_S2;
+  const bool has_res = kCanRes && !POOL && (d.residual != nullptr) && inb;
+  const bool has_mask = BWD && kCanRes && d.act >= TG_ACT_DRELU && inb;
+  const size_t in_off = (((size_t)tc.n * d.h + py) * d.w + px) * d.cout + tc.nb * p.bn;
+  int oy = py, ox = px, OW = d.w, OH = d.h;
+  if (KIND == TG_CONVT_3X3_S2) { oy = 2 * py + (acc >> 1); ox = 2 * px + (acc & 1); OW = 2 * d.w; OH = 2 * d.h; }
+  if (POOL) { OH = d.h >> 1; OW = d.w >> 1; oy = py >> 1; ox = px >> 1; }
+  uint4* orow = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(d.y) +
+                                         (((size_t)tc.n * OH + oy) * OW + ox) * d.cout + tc.nb * p.bn);
+  const float* srow = S + (size_t)r * stage_stride(MODE_TAP);
+#pragma unroll
+  for (int pc = 0; pc < 2; ++pc) {                // bn == 64: two 32-column pieces
+    uint4 res[4], msk[4];
+    if (has_res) {
+      const uint4* rp = reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(d.residual) + in_off) + pc * 4;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) res[i] = __ldg(rp + i);
+    }
+    if (has_mask) {
+      const uint4* mp = reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(d.mask) + in_off) + pc * 4;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) msk[i] = __ldg(mp + i);
+    }
+    float v[32];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float4 f = reinterpret_cast<const float4*>(srow + pc * 32)[i];
+      v[i * 4] = f.x; v[i * 4 + 1] = f.y; v[i * 4 + 2] = f.z; v[i * 4 + 3] = f.w;
+    }
+    const float4* bias4 = reinterpret_cast<const float4*>(bias_s + tc.nb * p.bn + pc * 32);
+    uint4 ov[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      __half2* o = reinterpret_cast<__half2*>(&ov[i]);
+      const __half2* rh = reinterpret_cast<const __half2*>(&res[i]);
+      const __half2* mh = reinterpret_cast<const __half2*>(&msk[i]);
+      const float4 b0 = bias4[i * 2], b1 = bias4[i * 2 + 1];
+      const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int cidx = i * 8 + j * 2;
+        float a0, a1;
+        if (!BWD) {
+          a0 = tg_epi_val(v[cidx], bb[j * 2], d.act);
+          a1 = tg_epi_val(v[cidx + 1], bb[j * 2 + 1], d.act);
+          if (has_res) {
+            const float2 rf = __half22float2(rh[j]);
+            a0 += rf.x; a1 += rf.y;
+          }
+        } else {
+          a0 = v[cidx] + bb[j * 2];
+          a1 = v[cidx + 1] + bb[j * 2 + 1];
+          if (has_res) {
+            const float2 rf = __half22float2(rh[j]);
+            a0 += rf.x; a1 += rf.y;
+          }
+          if (has_mask) {
+            const float2 mf = __half22float2(mh[j]);
+            a0 *= tg_dact(mf.x, d.act); a1 *= tg_dact(mf.y, d.act);
+          }
+        }
+        o[j] = __floats2half2_rn(a0, a1);
+      }
+    }
+    if (POOL) {
+      // max over the 2x2 block (all 32 lanes take part: lane ^ 1 = x neighbour, lane ^ 8 = y neighbour;
+      // floor pooling: blocks that reach outside the image are not stored)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        uint32_t* wv = reinterpret_cast<uint32_t*>(&ov[i]);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          uint32_t o1 = __shfl_xor_sync(0xFFFFFFFFu, wv[j], 1);
+          __half2 mx = __hmax2(*reinterpret_cast<__half2*>(&wv[j]), *reinterpret_cast<__half2*>(&o1));
+          uint32_t m32 = *reinterpret_cast<uint32_t*>(&mx);
+          uint32_t o8 = __shfl_xor_sync(0xFFFFFFFFu, m32, 8);
+          mx = __hmax2(mx, *reinterpret_cast<__half2*>(&o8));
+          wv[j] = *reinterpret_cast<uint32_t*>(&mx);
+        }
+      }
+      if (((tx | ty) & 1) == 0 && py + 1 < d.h && px + 1 < d.w) {
+        st_global_128x2(orow + pc * 4, ov[0], ov[1]);
+        st_global_128x2(orow + pc * 4 + 2, ov[2], ov[3]);
+      }
+    } else if (inb) {
+      st_global_128x2(orow + pc * 4, ov[0], ov[1]);
+      st_global_128x2(orow + pc * 4 + 2, ov[2], ov[3]);
+    }
+  }
+  (void)lane;
+}
+
+// ------------------------------------------------------------------ the kernel
+// BWD = data-gradient instantiation: epilogue y = (acc + bias [+ residual]) * act'(mask)  (TG_ACT_DRELU /
+// TG_ACT_DLRELU02; TG_ACT_NONE = no derivative).
+// POOL = TG_EPI_NHWC_F16_POOL2 instantiation: 2x2 max over the tile's pixels by warp shuffles, one store
+// per 2x2 block.
+template <int KIND, int MODE, bool BWD = false, bool POOL = false>
+__global__ void __launch_bounds__(kThreads, 1)
+conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;   // 128B swizzle atoms need 1024B alignment
+  uint8_t* sm = smem_raw + (base - raw);
+  constexpr int BN = MODE == MODE_TAPN ? TG_TAPN_ROWS : 64;
+  constexpr int NF = BN / 2;                      // accumulator registers per m64 half
+
+  const int warp = __shfl_sync(0xFFFFFFFFu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+  const tg_conv_desc& d = p.d;
+
+  // header: barriers, ring k of consumer c at index c * kMaxRing + k
+  const uint32_t bar_full = base;                          // [2 * kMaxRing]
+  const uint32_t bar_empty = base + 16 * kMaxRing;         // [2 * kMaxRing]
+  const uint32_t bar_b = base + 32 * kMaxRing;             // [1]
+  float* bias_s = reinterpret_cast<float*>(sm + 1024);
+  static_assert(!(KIND == TG_CONV_3X3_S2 && MODE != MODE_TAP), "the stride-2 conv runs in tap mode only");
+
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&maps.m[0]);
+    if (KIND == TG_CONV_3X3_S2) { tma_prefetch_desc(&maps.m[1]); tma_prefetch_desc(&maps.m[2]); tma_prefetch_desc(&maps.m[3]); }
+  }
+  if (warp == 1 && lane == 0) {
+    for (int s = 0; s < 2 * kMaxRing; ++s) {
+      mbar_init(bar_full + 8 * s, 1);
+      mbar_init(bar_empty + 8 * s, 4);     // one arrival per consumer warp
+    }
+    mbar_init(bar_b, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  const uint32_t smem_b = base + p.off_b;
+  const uint32_t smem_stage0 = base + p.off_stage;
+  const unsigned char* wglob = reinterpret_cast<const unsigned char*>(d.weights);
+  const int n_tiles_w = (MODE == MODE_TAPN ? 1 : 9) * p.chunks;
+
+  // Resident weights do not depend on the previous kernel (static during graph replay; the eager path
+  // separates tg_pack_* from the conv by a bias copy): start their load, then join the
+  // programmatic-dependent-launch wait.  The previous kernel's OUTPUT is only read after tg_pdl_wait().
+  if (warp == 0 && lane == 0 && p.b_resident) {
+    const uint32_t nb = blockIdx.x % (uint32_t)p.n_split;   // fixed per CTA: gridDim.x % n_split == 0
+    mbar_expect_tx(bar_b, (uint32_t)n_tiles_w * p.b_stage_bytes);
+    for (int t = 0; t < n_tiles_w; ++t)
+      bulk_load(smem_b + t * p.b_stage_bytes, wglob + (size_t)t * p.b_tile_bytes + (size_t)nb * p.b_stage_bytes,
+                p.b_stage_bytes, bar_b);
+  }
+  tg_pdl_wait();
+  tg_pdl_trigger();
+  for (int i = threadIdx.x; i < d.cout; i += kThreads) bias_s[i] = d.bias[i];
+  __syncthreads();
+
+  if (warp == 0) {
+    // ============================================================ TMA producer
+    if (lane == 0) {
+      int stage[2] = {0, 0};
+      uint32_t phase[2] = {0, 0};
+      int it = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
+        const int cw = it & 1;
+        const TileCoord tc = tile_coord(p, tile);
+        const int n_loads = MODE == MODE_TAP ? 9 * p.chunks : p.chunks;
+        for (int l = 0; l < n_loads; ++l) {
+          const int s = cw * kMaxRing + stage[cw];
+          mbar_wait_mma(bar_empty + 8 * s, phase[cw] ^ 1);
+          const uint32_t sa = smem_stage0 + (uint32_t)(cw * p.ring + stage[cw]) * p.stage_bytes;
+          if (MODE != MODE_TAP) {
+            mbar_expect_tx(bar_full + 8 * s, p.a_bytes);
+            tma_load_4d(sa, &maps.m[0], bar_full + 8 * s, l * 64, tc.x0 + p.org_x, tc.y0 + p.org_y, tc.n);
+          } else {
+            const int g = l / p.chunks, c = l - g * p.chunks;
+            const TgGroup gr = tg_group(KIND, g);
+            mbar_expect_tx(bar_full + 8 * s, p.a_bytes + (p.b_resident ? 0u : p.b_stage_bytes));
+            tma_load_4d(sa, &maps.m[KIND == TG_CONV_3X3_S2 ? tg_s2_plane(g) : 0], bar_full + 8 * s, c * 64,
+                        tc.x0 + gr.dx, tc.y0 + gr.dy, tc.n);
+            if (!p.b_resident)
+              bulk_load(sa + kTapABytes,
+                        wglob + (size_t)(g * p.chunks + c) * p.b_tile_bytes + (size_t)tc.nb * p.b_stage_bytes,
+                        p.b_stage_bytes, bar_full + 8 * s);
+          }
+          if (++stage[cw] == p.ring) { stage[cw] = 0; phase[cw] ^= 1u; }
+        }
+      }
+    }
+  } else if (warp >= 4) {
+    // ============================================================ consumers
+    const int cw = (warp - 4) >> 2;
+    const int r = threadIdx.x - 128 * (1 + cw);        // 0..127: tile row in the epilogue
+    const int q = r >> 5;                              // warp of the warpgroup
+    float* S = reinterpret_cast<float*>(sm + p.off_scratch + (uint32_t)cw * scratch_bytes(MODE));
+    if (p.b_resident) mbar_wait_mma(bar_b, 0);
+
+    constexpr int kBoxW = (KIND == TG_CONV_3X3) ? TW + 2 : TW + 1;
+    constexpr int kOrg = (KIND == TG_CONV_3X3) ? -1 : 0;
+    const uint32_t a_sbo = (MODE == MODE_HALO ? (uint32_t)kBoxW : (uint32_t)TW) * 128u;
+    const uint64_t a_hi = gmma_desc_hi(a_sbo), b_hi = gmma_desc_hi(1024u);
+    const uint32_t half16 = (8u * a_sbo) >> 4;         // tile rows 8..15 = the second m64 half
+    const uint32_t btb16 = p.b_stage_bytes >> 4;
+    const uint32_t smem_b16 = gmma_addr16(smem_b);
+    int stage = 0;
+    uint32_t phase = 0;
+    int pend = -1;                                     // stage whose MMAs may still be reading it
+
+    float acc[2][NF];
+    auto mma_group = [&](uint32_t a16, uint32_t b16, bool first) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        if (k < p.ksteps) {
+          const uint32_t sc = (first && k == 0) ? 0u : 1u;
+          wgmma_k16<NF>(acc[0], a_hi | (uint64_t)(a16 + 2u * k), b_hi | (uint64_t)(b16 + 2u * k), sc);
+          wgmma_k16<NF>(acc[1], a_hi | (uint64_t)(a16 + half16 + 2u * k), b_hi | (uint64_t)(b16 + 2u * k), sc);
+        }
+      }
+    };
+    auto release = [&](int s) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * (cw * kMaxRing + s));
+    };
+    auto next_stage = [&]() -> int {   // wait for the next stage of this consumer's ring; returns its index
+      const int s = stage;
+      mbar_wait_mma(bar_full + 8 * (cw * kMaxRing + s), phase);
+      if (++stage == p.ring) { stage = 0; phase ^= 1u; }
+      return s;
+    };
+    auto stage_addr = [&](int s) { return smem_stage0 + (uint32_t)(cw * p.ring + s) * p.stage_bytes; };
+    // accumulators -> S (fp32, row-major [128][stride]); the caller synchronises the warpgroup around it
+    auto stash = [&]() {
+      constexpr uint32_t ST = stage_stride(MODE);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int i = 0; i < NF; i += 2) {
+          const int row = h * 64 + q * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+          const int col = 8 * (i >> 2) + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(S + (size_t)row * ST + col) = make_float2(acc[h][i], acc[h][i + 1]);
+        }
+      }
+    };
+    const int bar_id = 1 + cw;
+
+    int it = cw;
+    for (int tile = blockIdx.x + cw * (int)gridDim.x; tile < p.num_tiles; tile += 2 * (int)gridDim.x, it += 2) {
+      const TileCoord tc = tile_coord(p, tile);
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < NF; ++i) acc[h][i] = 0.f;
+
+      if (MODE == MODE_TAPN) {
+        // D[pos][tap*4+co] = x[pos] . W[tap][co]; out[p] = sum_taps D[p+off(tap)][tap]
+        for (int c = 0; c < p.chunks; ++c) {
+          const int s = next_stage();
+          wgmma_fence();
+          mma_group(gmma_addr16(stage_addr(s)), smem_b16 + (uint32_t)c * btb16, c == 0);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (pend >= 0) release(pend);
+          pend = s;
+        }
+        wgmma_wait<0>();
+        release(pend);
+        pend = -1;
+        stash();
+        named_bar_sync(bar_id, 128);
+        const int ty = r >> 3, tx = r & 7;
+        const int py = tc.y0 + ty - 1, px = tc.x0 + tx - 1;
+        const bool inb = ty >= 1 && ty <= TH - 2 && tx >= 1 && tx <= TW - 2 && py < d.h && px < d.w;
+        if (inb) {
+          constexpr uint32_t ST = stage_stride(MODE_TAPN);
+          float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+          for (int tap = 0; tap < 9; ++tap) {
+            const float4 e = *reinterpret_cast<const float4*>(S + (size_t)(r + (tap / 3 - 1) * TW + (tap % 3 - 1)) * ST + tap * 4);
+            a.x += e.x; a.y += e.y; a.z += e.z; a.w += e.w;
+          }
+          const float av[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+          for (int ch = 0; ch < 4; ++ch) {
+            if (d.epilogue == TG_EPI_FLOW_NCHW_F32) {
+              tg_epi_flow(d, tc.n, py, px, d.h, d.w, ch, av[ch]);
+            } else {
+              tg_epi_out(d, tc.n, py, px, d.h, d.w, ch, av[ch]);
+            }
+          }
+        }
+        named_bar_sync(bar_id, 128);
+      } else if (MODE == MODE_HALO && KIND == TG_CONVT_3X3_S2) {
+        // one halo stage (chunks == 1), four parity accumulators one after the other
+        const int s = next_stage();
+        const uint32_t sa16 = gmma_addr16(stage_addr(s));
+#pragma unroll 1
+        for (int a = 0; a < 4; ++a) {
+          if (a > 0) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int i = 0; i < NF; ++i) acc[h][i] = 0.f;
+          }
+          wgmma_fence();
+#pragma unroll
+          for (int g = 0; g < 9; ++g) {
+            const TgGroup gr = tg_group(KIND, g);
+            if (gr.acc != a) continue;
+            const bool first = g == 0 || tg_group(KIND, g > 0 ? g - 1 : 0).acc != gr.acc;
+            mma_group(sa16 + (uint32_t)((gr.dy - kOrg) * kBoxW + (gr.dx - kOrg)) * 8u, smem_b16 + (uint32_t)g * btb16, first);
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          if (a == 3) release(s);
+          stash();
+          named_bar_sync(bar_id, 128);
+          epilogue_nhwc<KIND, BWD, POOL>(p, tc, r, lane, a, S, bias_s);
+          named_bar_sync(bar_id, 128);
+        }
+      } else if (MODE == MODE_HALO) {
+        for (int c = 0; c < p.chunks; ++c) {
+          const int s = next_stage();
+          const uint32_t sa16 = gmma_addr16(stage_addr(s));
+          wgmma_fence();
+#pragma unroll
+          for (int g = 0; g < 9; ++g) {
+            const TgGroup gr = tg_group(KIND, g);
+            mma_group(sa16 + (uint32_t)((gr.dy - kOrg) * kBoxW + (gr.dx - kOrg)) * 8u,
+                      smem_b16 + (uint32_t)(g * p.chunks + c) * btb16, g == 0 && c == 0);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (pend >= 0) release(pend);
+          pend = s;
+        }
+        wgmma_wait<0>();
+        release(pend);
+        pend = -1;
+        stash();
+        named_bar_sync(bar_id, 128);
+        epilogue_nhwc<KIND, BWD, POOL>(p, tc, r, lane, 0, S, bias_s);
+        named_bar_sync(bar_id, 128);
+      } else {
+        // MODE_TAP: one stage per (tap, chunk); the groups of one accumulator are consecutive
+#pragma unroll 1
+        for (int g = 0; g < 9; ++g) {
+          const TgGroup gr = tg_group(KIND, g);
+          const bool first_of_acc = g == 0 || tg_group(KIND, g - 1).acc != gr.acc;
+          const bool last_of_acc = g == 8 || tg_group(KIND, g + 1).acc != gr.acc;
+          for (int c = 0; c < p.chunks; ++c) {
+            const int s = next_stage();
+            const uint32_t sa = stage_addr(s);
+            const uint32_t b16 = p.b_resident ? smem_b16 + (uint32_t)(g * p.chunks + c) * btb16
+                                              : gmma_addr16(sa + kTapABytes);
+            wgmma_fence();
+            mma_group(gmma_addr16(sa), b16, first_of_acc && c == 0);
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (pend >= 0) release(pend);
+            pend = s;
+          }
+          if (last_of_acc) {
+            wgmma_wait<0>();
+            release(pend);
+            pend = -1;
+            stash();
+            named_bar_sync(bar_id, 128);
+            epilogue_nhwc<KIND, BWD, POOL>(p, tc, r, lane, gr.acc, S, bias_s);
+            named_bar_sync(bar_id, 128);
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int i = 0; i < NF; ++i) acc[h][i] = 0.f;
+          }
+        }
+      }
+    }
+  }
+}
+
+// ------------------------------------------------------------------ host side
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
+                                  const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
+                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+EncodeTiledFn get_encode_fn() {
+  static EncodeTiledFn fn = nullptr;
+  static std::once_flag once;
+  std::call_once(once, [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<EncodeTiledFn>(p);
+  });
+  return fn;
+}
+
+// NHWC fp16 tensor [n][h][w][c] with explicit element strides for w/h/n (parity views)
+int encode_nhwc(CUtensorMap* m, const void* ptr, int c, int w, int h, int n, size_t sw, size_t sh,
+                size_t sn, int box_c, int box_w, int box_h) {
+  EncodeTiledFn fn = get_encode_fn();
+  TG_REQUIRE(fn != nullptr, TG_E_DRIVER, "cuTensorMapEncodeTiled not available from the driver");
+  cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
+  cuuint64_t strides[3] = {(cuuint64_t)sw * 2, (cuuint64_t)sh * 2, (cuuint64_t)sn * 2};
+  cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), dims, strides, box,
+                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  TG_REQUIRE(r == CUDA_SUCCESS, TG_E_DRIVER,
+             "cuTensorMapEncodeTiled failed (%d) c=%d w=%d h=%d n=%d box=%dx%dx%d", (int)r, c, w, h, n,
+             box_c, box_w, box_h);
+  return TG_OK;
+}
+
+template <int K, int M, bool B, bool P>
+cudaError_t set_smem_attr() {
+  return cudaFuncSetAttribute(conv_wgmma_kernel<K, M, B, P>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              (int)kSmemLimit);
+}
+
+}  // namespace
+
+extern "C" {
+
+int tg_debug_set_conv_timers(void* device_buffer) {
+  TG_REQUIRE(device_buffer == nullptr, TG_E_UNSUPPORTED,
+             "debug_set_conv_timers: the sm_90a kernels record no role timers");
+  return TG_OK;
+}
+
+int tg_conv_validate(const tg_conv_desc* d, const char* who) {
+  TG_REQUIRE(d != nullptr, TG_E_INVALID, "%s: null descriptor", who);
+  TG_REQUIRE(d->x && d->weights && d->bias && d->y, TG_E_INVALID, "%s: null pointer", who);
+  TG_REQUIRE(d->n > 0 && d->h > 0 && d->w > 0, TG_E_INVALID, "%s: bad size n=%d h=%d w=%d", who, d->n, d->h, d->w);
+  TG_REQUIRE(d->kind == TG_CONV_3X3 || d->kind == TG_CONVT_3X3_S2 || d->kind == TG_CONV_3X3_S2, TG_E_INVALID,
+             "%s: kind", who);
+  TG_REQUIRE(d->act >= TG_ACT_NONE && d->act <= TG_ACT_DLRELU02, TG_E_INVALID, "%s: act", who);
+  TG_REQUIRE((d->act >= TG_ACT_DRELU) == (d->mask != nullptr), TG_E_INVALID,
+             "%s: mask must be given exactly for TG_ACT_DRELU / TG_ACT_DLRELU02", who);
+  TG_REQUIRE(!(d->act >= TG_ACT_DRELU && (d->epilogue != TG_EPI_NHWC_F16 || d->kind == TG_CONVT_3X3_S2)),
+             TG_E_UNSUPPORTED, "%s: derivative epilogues need NHWC output and a conv3x3 / conv3x3s2 layer", who);
+  TG_REQUIRE(!(d->kind == TG_CONV_3X3_S2 && d->epilogue != TG_EPI_NHWC_F16), TG_E_UNSUPPORTED,
+             "%s: conv3x3s2 needs the NHWC epilogue", who);
+  TG_REQUIRE(d->cin == 64 || d->cin == 128 || d->cin == 256, TG_E_UNSUPPORTED,
+             "%s: cin=%d (stored channels must be 64, 128 or 256)", who, d->cin);
+  if (d->epilogue == TG_EPI_NHWC_F16_POOL2)
+    TG_REQUIRE(d->kind == TG_CONV_3X3 && d->residual == nullptr && d->act <= TG_ACT_LRELU02 && d->h >= 2 && d->w >= 2,
+               TG_E_UNSUPPORTED, "%s: the pooled epilogue needs a conv3x3 without residual / derivative epilogue", who);
+  if (d->epilogue == TG_EPI_NHWC_F16 || d->epilogue == TG_EPI_NHWC_F16_POOL2) {
+    TG_REQUIRE(d->cout == 64 || d->cout == 128 || d->cout == 256, TG_E_UNSUPPORTED,
+               "%s: cout=%d (64, 128 or 256 for the NHWC epilogue)", who, d->cout);
+    TG_REQUIRE(!(d->residual && d->kind == TG_CONVT_3X3_S2), TG_E_UNSUPPORTED, "%s: residual with convT", who);
+    TG_REQUIRE(!(d->kind == TG_CONVT_3X3_S2 && d->cout != 64), TG_E_UNSUPPORTED,
+               "%s: convT needs cout == 64 (4 parity accumulators per tile)", who);
+  } else if (d->epilogue == TG_EPI_FLOW_NCHW_F32 || d->epilogue == TG_EPI_OUT_NCHW_F32) {
+    TG_REQUIRE(d->kind == TG_CONV_3X3 && d->cout == TG_TAPN_ROWS && d->cout_real >= 1 && d->cout_real <= 4,
+               TG_E_UNSUPPORTED, "%s: NCHW epilogues need conv3x3, cout=48 (tap-major N), cout_real<=4", who);
+    TG_REQUIRE(d->residual == nullptr, TG_E_UNSUPPORTED, "%s: residual with NCHW epilogue", who);
+  } else {
+    TG_REQUIRE(false, TG_E_INVALID, "%s: epilogue %d", who, d->epilogue);
+  }
+  return TG_OK;
+}
+
+int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
+  int rc = tg_conv_validate(d, "conv");
+  if (rc != TG_OK) return rc;
+  TG_REQUIRE(d->a_mode >= TG_AMODE_AUTO && d->a_mode <= TG_AMODE_TAP, TG_E_INVALID, "conv: a_mode");
+  TG_REQUIRE(((uintptr_t)d->x & 15) == 0 && ((uintptr_t)d->weights & 15) == 0 && ((uintptr_t)d->y & 15) == 0,
+             TG_E_INVALID, "conv: pointers must be 16-byte aligned");
+
+  KParams p;
+  p.d = *d;
+  const bool tapn = d->epilogue == TG_EPI_FLOW_NCHW_F32 || d->epilogue == TG_EPI_OUT_NCHW_F32;
+  const bool pool = d->epilogue == TG_EPI_NHWC_F16_POOL2;
+  p.step_y = tapn ? kTapnStepY : TH;
+  p.step_x = tapn ? kTapnStepX : TW;
+  p.tiles_x = tg_ceil_div(d->w, p.step_x);
+  p.tiles_y = tg_ceil_div(d->h, p.step_y);
+  p.num_tiles = p.tiles_x * p.tiles_y * d->n;
+  p.chunks = d->cin / 64;
+  TG_REQUIRE(d->cin_real >= 0 && d->cin_real <= d->cin, TG_E_INVALID, "conv: cin_real=%d outside [0, cin=%d]",
+             d->cin_real, d->cin);
+  p.ksteps = (p.chunks == 1 && d->cin_real > 0) ? (d->cin_real + 15) / 16 : 4;
+  p.n_acc = d->kind == TG_CONVT_3X3_S2 ? 4 : 1;
+  p.b_tile_bytes = (uint32_t)d->cout * 128u;
+
+  // Output channels beyond 64 are split over CTAs (N = 64 per CTA): cout/64 x more CTAs on the
+  // low-resolution FNet layers, and each CTA only needs its own 64-row slice of every weight tile.
+  p.n_split = (!tapn && d->cout > 64) ? d->cout / 64 : 1;
+  p.bn = d->cout / p.n_split;
+  p.b_stage_bytes = (uint32_t)p.bn * 128u;
+  const uint32_t b_total = (tapn ? 1u : 9u) * p.chunks * p.b_stage_bytes;   // resident slice per CTA
+  const int hbox_w = d->kind != TG_CONVT_3X3_S2 ? TW + 2 : TW + 1;
+  const int hbox_h = d->kind != TG_CONVT_3X3_S2 ? TH + 2 : TH + 1;
+  const uint32_t halo_bytes = (uint32_t)hbox_w * hbox_h * 128u;
+  const uint32_t halo_stage = (halo_bytes + 1023u) & ~1023u;
+  const uint32_t scratch = 2u * scratch_bytes(tapn ? MODE_TAPN : MODE_TAP);
+  const uint32_t fixed = 1024u /*align slack*/ + kHeaderBytes + scratch;
+
+  // every consumer needs at least one stage of its own
+  const bool can_resident_halo = fixed + b_total + 2u * halo_stage <= kSmemLimit &&
+                                 !(d->kind == TG_CONVT_3X3_S2 && p.chunks != 1);
+  const bool can_resident_tap = fixed + b_total + 2u * kTapABytes <= kSmemLimit;
+  int mode = d->a_mode;
+  TG_REQUIRE(!(d->kind == TG_CONV_3X3_S2 && mode == TG_AMODE_HALO), TG_E_UNSUPPORTED,
+             "conv: conv3x3s2 runs in tap mode (a stride-2 view is not a wgmma descriptor)");
+  if (d->kind == TG_CONV_3X3_S2 || tapn) mode = TG_AMODE_TAP;   // thin heads run MODE_TAPN below
+  if (mode == TG_AMODE_AUTO) mode = can_resident_halo ? TG_AMODE_HALO : TG_AMODE_TAP;
+  TG_REQUIRE(!(mode == TG_AMODE_HALO && !can_resident_halo), TG_E_UNSUPPORTED,
+             "conv: halo mode needs the weights resident in smem (cin=%d cout=%d)", d->cin, d->cout);
+  p.halo = mode == TG_AMODE_HALO;
+  p.b_resident = p.halo ? 1 : (can_resident_tap ? 1 : 0);
+  p.num_tiles *= p.n_split;
+  TG_REQUIRE(p.bn == 64 || (tapn && p.bn == TG_TAPN_ROWS), TG_E_UNSUPPORTED,
+             "conv: per-CTA N must be 64 (48 for the thin heads)");
+  TG_REQUIRE(!tapn || p.b_resident, TG_E_UNSUPPORTED, "conv: thin head weights must fit in smem");
+  if (tapn) {
+    p.box_w = TW; p.box_h = TH; p.org_x = -1; p.org_y = -1;
+    p.a_bytes = kTapABytes;
+    p.stage_bytes = kTapABytes;
+  } else if (p.halo) {
+    p.box_w = hbox_w; p.box_h = hbox_h;
+    p.org_x = d->kind == TG_CONV_3X3 ? -1 : 0;
+    p.org_y = p.org_x;
+    p.a_bytes = halo_bytes;
+    p.stage_bytes = halo_stage;
+  } else {
+    p.box_w = TW; p.box_h = TH; p.org_x = 0; p.org_y = 0;
+    p.a_bytes = kTapABytes;
+    p.stage_bytes = kTapABytes + (p.b_resident ? 0u : p.b_stage_bytes);
+  }
+  const uint32_t avail = kSmemLimit - fixed - (p.b_resident ? b_total : 0u);
+  int ring = (int)(avail / p.stage_bytes) / 2;
+  if (ring > kMaxRing) ring = kMaxRing;
+  TG_REQUIRE(ring >= 1, TG_E_UNSUPPORTED, "conv: shared memory budget (cin=%d cout=%d)", d->cin, d->cout);
+  p.ring = ring;
+  p.off_b = kHeaderBytes;
+  p.off_stage = kHeaderBytes + (p.b_resident ? b_total : 0u);
+  p.off_scratch = p.off_stage + 2u * (uint32_t)ring * p.stage_bytes;   // consumer c's ring: stages [c*ring, (c+1)*ring)
+  const uint32_t smem_bytes = 1024u + p.off_scratch + scratch;
+  TG_REQUIRE(smem_bytes <= kSmemLimit, TG_E_UNSUPPORTED, "conv: smem %u > limit", smem_bytes);
+
+  // tensor maps
+  TgMaps map_a;
+  if (d->kind != TG_CONV_3X3_S2) {
+    rc = encode_nhwc(&map_a.m[0], d->x, d->cin, d->w, d->h, d->n, (size_t)d->cin, (size_t)d->w * d->cin,
+                     (size_t)d->h * d->w * d->cin, 64, p.box_w, p.box_h);
+    if (rc != TG_OK) return rc;
+    map_a.m[1] = map_a.m[2] = map_a.m[3] = map_a.m[0];
+  } else {
+    // x [n,2h,2w,cin]: parity plane (py,px) = pixels (2i+py, 2j+px), each an [n,h,w,cin] strided view
+    const size_t W2 = (size_t)2 * d->w, C = (size_t)d->cin;
+    for (int pl = 0; pl < 4; ++pl) {
+      const __half* base = reinterpret_cast<const __half*>(d->x) + ((size_t)(pl >> 1) * W2 + (pl & 1)) * C;
+      rc = encode_nhwc(&map_a.m[pl], base, d->cin, d->w, d->h, d->n, 2 * C, 2 * W2 * C,
+                       (size_t)4 * d->h * d->w * C, 64, p.box_w, p.box_h);
+      if (rc != TG_OK) return rc;
+    }
+  }
+
+  static TgPerDeviceOnce attr_once;
+  const cudaError_t attr_err = attr_once.run([] {
+    const cudaError_t errs[] = {
+        set_smem_attr<TG_CONV_3X3, MODE_HALO, false, false>(), set_smem_attr<TG_CONV_3X3, MODE_TAP, false, false>(),
+        set_smem_attr<TG_CONV_3X3, MODE_TAPN, false, false>(), set_smem_attr<TG_CONVT_3X3_S2, MODE_HALO, false, false>(),
+        set_smem_attr<TG_CONVT_3X3_S2, MODE_TAP, false, false>(), set_smem_attr<TG_CONV_3X3, MODE_HALO, false, true>(),
+        set_smem_attr<TG_CONV_3X3, MODE_TAP, false, true>(), set_smem_attr<TG_CONV_3X3, MODE_HALO, true, false>(),
+        set_smem_attr<TG_CONV_3X3, MODE_TAP, true, false>(), set_smem_attr<TG_CONV_3X3_S2, MODE_TAP, true, false>()};
+    for (cudaError_t e : errs)
+      if (e != cudaSuccess) return e;
+    return cudaSuccess;
+  });
+  TG_REQUIRE(attr_err == cudaSuccess, (int)attr_err, "conv: cudaFuncSetAttribute: %s",
+             cudaGetErrorString(attr_err));
+
+  int sms = 0;
+  rc = tg_device_sm_count(&sms);
+  if (rc != TG_OK) return rc;
+  int grid = d->max_ctas > 0 ? d->max_ctas : sms;
+  if (grid > p.num_tiles) grid = p.num_tiles;
+  grid -= grid % p.n_split;             // every CTA keeps one fixed N slice (resident weights)
+  if (grid < p.n_split) grid = p.n_split;
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 g(grid), b(kThreads);
+  cudaError_t lerr = cudaSuccess;
+  const bool bwd = d->act >= TG_ACT_DRELU || d->kind == TG_CONV_3X3_S2;
+  if (pool) {
+    lerr = p.halo ? tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_HALO, false, true>, g, b, kSmemLimit, st, map_a, p)
+                  : tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_TAP, false, true>, g, b, kSmemLimit, st, map_a, p);
+  } else if (bwd) {
+    if (d->kind == TG_CONV_3X3_S2)
+      lerr = tg_launch(conv_wgmma_kernel<TG_CONV_3X3_S2, MODE_TAP, true>, g, b, kSmemLimit, st, map_a, p);
+    else if (p.halo)
+      lerr = tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_HALO, true>, g, b, kSmemLimit, st, map_a, p);
+    else
+      lerr = tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_TAP, true>, g, b, kSmemLimit, st, map_a, p);
+  } else if (tapn) {
+    lerr = tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_TAPN>, g, b, kSmemLimit, st, map_a, p);
+  } else if (d->kind == TG_CONV_3X3) {
+    lerr = p.halo ? tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_HALO>, g, b, kSmemLimit, st, map_a, p)
+                  : tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_TAP>, g, b, kSmemLimit, st, map_a, p);
+  } else {
+    lerr = p.halo ? tg_launch(conv_wgmma_kernel<TG_CONVT_3X3_S2, MODE_HALO>, g, b, kSmemLimit, st, map_a, p)
+                  : tg_launch(conv_wgmma_kernel<TG_CONVT_3X3_S2, MODE_TAP>, g, b, kSmemLimit, st, map_a, p);
+  }
+  TG_REQUIRE(lerr == cudaSuccess, (int)lerr, "conv: launch failed: %s", cudaGetErrorString(lerr));
+  TG_CUDA_LAUNCH_CHECK("conv");
+  return TG_OK;
+}
+
+
+}  // extern "C"

@@ -293,7 +293,7 @@ upsample2x_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int n, int
 
 // FNet input: cat([x1,x2],1) of two 3-channel NCHW fp32 images -> NHWC fp16 c64 (tecogan_nets.py:71).
 // One thread = one pixel: 2*c coalesced plane loads, then the pixel's whole 128-byte row (six
-// values + zeros) in four 256-bit stores -- full 32-byte sectors per store instruction.
+// values + zeros) in eight 128-bit stores.
 __global__ void __launch_bounds__(256)
 pack_pair_c64_kernel(const float* __restrict__ x1, const float* __restrict__ x2, uint4* __restrict__ y,
                      int n, int c, int hw) {
@@ -312,11 +312,9 @@ pack_pair_c64_kernel(const float* __restrict__ x1, const float* __restrict__ x2,
     }
     const uint4 v0 = *reinterpret_cast<const uint4*>(vals), z = make_uint4(0u, 0u, 0u, 0u);
     uint4* row = y + (size_t)i * 8;
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(row), "r"(v0.x), "r"(v0.y),
-                 "r"(v0.z), "r"(v0.w), "r"(0u), "r"(0u), "r"(0u), "r"(0u) : "memory");
+    row[0] = v0;
 #pragma unroll
-    for (int q = 1; q < 4; ++q)
-      asm volatile("st.global.v8.b32 [%0], {%1, %1, %1, %1, %1, %1, %1, %1};" ::"l"(row + 2 * q), "r"(z.x) : "memory");
+    for (int q = 1; q < 8; ++q) row[q] = z;
   }
 }
 
@@ -536,7 +534,7 @@ namespace {
 
 inline int grid_for(size_t total, int block) {
   size_t g = (total + block - 1) / block;
-  const size_t cap = 148 * 32;
+  const size_t cap = (size_t)tg_sms() * 32;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
@@ -580,8 +578,7 @@ static int warp_launch(const float* hr_prev, const float* flow, const float* lr_
     return TG_OK;
   }
   // Default: all S HR rows of an LR row per pass (12*S gathers in flight per thread, 5 CTAs/SM).
-  // TG_WARP_SP=2: two rows per pass at <= 64 registers (8 CTAs/SM) -- measured NOT faster on B200
-  // (34.3 vs 32.0 us per 4-frame launch, profiles/bench_r2a*.json): occupancy is not the limiter.
+  // TG_WARP_SP=2: two rows per pass at <= 64 registers (8 CTAs/SM), for A/B measurements.
   static int sp_full = -1;
   if (sp_full < 0) { const char* e = getenv("TG_WARP_SP"); sp_full = (e && e[0] == '2') ? 0 : 1; }
 #define TG_WARP_LAUNCH(SS, FM)                                                                                 \

@@ -14,7 +14,7 @@ namespace {
 
 inline int sgrid(size_t total, int block) {
   size_t g = (total + block - 1) / block;
-  const size_t cap = 148 * 32;
+  const size_t cap = (size_t)tg_sms() * 32;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 

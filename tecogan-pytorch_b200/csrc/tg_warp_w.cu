@@ -5,13 +5,9 @@
 // one LR row; the warp stages its flow neighbourhood, gathers, transposes through a warp-private
 // shared-memory tile and stores -- synchronised with __syncwarp only.  The CTA-wide version runs its four
 // warps in lock step (two __syncthreads per LR row), so while one phase waits on DRAM nothing else of that
-// CTA is in flight: ncu showed it latency-bound at 14 % DRAM throughput, and doubling the occupancy by
-// halving the loads per thread did not help (profiles/bench_r2a*.json).  Here warps drift apart and the
-// gathers of one overlap the stores / flow staging of the others; units are handed out grid-stride, and the
-// small flow / lr reads of the next unit are prefetched into registers so a unit costs one dependent DRAM
-// round trip: 27.8 us per 4-frame launch against 31.9 (profiles/bench_r2j_*.json).  A third variant that
-// issued the corner gathers of the next unit as 4-byte cp.async into a double-buffered shared-memory
-// array (no registers held) was measured at 46.5 us -- twice the LSU work per gather -- and removed.
+// CTA is in flight.  Here warps drift apart and the gathers of one overlap the stores / flow staging of the
+// others; units are handed out grid-stride, and the small flow / lr reads of the next unit are prefetched
+// into registers so a unit costs one dependent DRAM round trip.
 #include "tg_common.cuh"
 
 #include <cstdlib>
@@ -227,7 +223,7 @@ cudaError_t tg_warp_w_launch(const float* hr_prev, const float* flow, const floa
     occ = e != nullptr ? atoi(e) : kDefaultOcc;
     if (occ < 5 || occ > 8) occ = kDefaultOcc;
   }
-  const long long cap = 148LL * occ;             // one resident wave: every warp walks several units and the warps
+  const long long cap = (long long)tg_sms() * occ;            // one resident wave: every warp walks several units and the warps
                                                  // of an SM drift out of phase
   if (ctas > cap) ctas = cap;
   if (ctas < 1) ctas = 1;

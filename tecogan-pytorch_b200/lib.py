@@ -133,7 +133,7 @@ def load():
         return _lib
     if not os.path.isfile(LIB_PATH):
         raise TecoganB200Error(
-            f'{LIB_PATH} is missing: the sm_100a CUDA library has not been built. Run '
+            f'{LIB_PATH} is missing: the sm_90a CUDA library has not been built. Run '
             f'`python -c "import __graft_entry__ as g; g.build()"` (or `make -C '
             f'{os.path.join(_HERE, "csrc")}`). There is no CPU / PyTorch fallback.')
     lib = ctypes.CDLL(LIB_PATH)

@@ -6,7 +6,7 @@ infer_sequence / generate_dummy_data / profile), same attributes (fnet, srnet, u
 scale) and the same state_dict keys and shapes (strict load of reference ``G_iter*.pth`` works).
 
 The nn.Conv2d / nn.ConvTranspose2d objects below are PARAMETER HOLDERS ONLY -- their forward is
-never called.  All arithmetic goes through ``ops`` (hand-written sm_100a kernels); a CPU tensor
+never called.  All arithmetic goes through ``ops`` (hand-written sm_90a kernels); a CPU tensor
 raises, there is no PyTorch fallback.
 """
 from collections import OrderedDict
@@ -179,7 +179,7 @@ class SRNet(nn.Module):
                      c.get(('r', i, 2), blk.conv[2], L.CONV_3X3, L.ACT_NONE)]
         if (ops.chain_enabled() and ops.default_conv_impl() == 'tcgen05' and x.shape[-1] == 64
                 and ops.ConvChain.supported(body)):
-            # conv_in + all residual blocks in ONE persistent launch: buffers 0 = x (read only),
+            # conv_in + all residual blocks in ONE persistent launch (TECOGAN_B200_CHAIN=1): buffers 0 = x (read only),
             # 1 = block input/output (conv2 writes it in place over its own residual), 2 = conv1 output
             if self._chain is None or [s[0] for s in self._chain.specs] != body:
                 specs = [(body[0], 0, 1, None)]
@@ -198,7 +198,7 @@ class SRNet(nn.Module):
         if (tail and ops.default_conv_impl() == 'tcgen05' and ups[-1].cin == 64 and ups[-1].cout == 64
                 and pc_out.cin == 64 and pc_out.cout_real <= 3):
             # last transposed conv + ReLU + conv_out + residual in ONE launch: the 64-channel HR map (88 MB per
-            # frame) never reaches HBM.  mode 'acc': `out` is first filled with upsample_func(lr_curr) by the
+            # frame) stays in shared memory and never reaches HBM.  mode 'acc': `out` is first filled with upsample_func(lr_curr) by the
             # (pure-write) upsample kernel and the tail accumulates onto it -- one coalesced read per pixel;
             # mode 'fused': the residual (and the uint8 frame) are evaluated inside the tail kernel.
             for up in ups[:-1]:
@@ -263,7 +263,7 @@ def _conv_gflops(layers):
 
 
 class FRNet(BaseSequenceGenerator):
-    """Frame-recurrent generator (reference tecogan_nets.py:150-314) on sm_100a kernels."""
+    """Frame-recurrent generator (reference tecogan_nets.py:150-314) on sm_90a kernels."""
 
     def __init__(self, in_nc, out_nc, nf, nb, degradation, scale):
         super().__init__()

@@ -106,7 +106,7 @@ class PackedConv:
 
     def __call__(self, x, y=None, residual=None, impl=None, a_mode=None, max_ctas=0, pool=False):
         """x NHWC fp16 [n,h,w,cin] -> y (allocated when None).  pool=True: nn.MaxPool2d(2,2) folded into the
-        epilogue, y = [n,h//2,w//2,cout] (conv3x3 layers with the NHWC epilogue, tcgen05 only)."""
+        epilogue, y = [n,h//2,w//2,cout] (conv3x3 layers with the NHWC epilogue, wgmma path only)."""
         _req(x, torch.float16, 'conv input', 4)
         n, h, w, cin = x.shape
         if cin != self.cin:
@@ -231,10 +231,9 @@ def fused_tail(up, outc, x, lr_curr, lr_scale, up_mode, y=None, y_u8=None, max_c
 
 def tail_mode():
     """TECOGAN_B200_TAIL: '0' = last transposed conv, conv_out, residual upsample and uint8 as four launches;
-    'acc' = tg_convT_convout_tcgen05 accumulating onto a pre-written residual; 'fused' = residual and uint8
-    evaluated inside the tail kernel.  Default 'acc': measured 0.786 ms per step against 0.849 ('0') and 0.897
-    ('fused': the in-kernel gathers and 2-byte uint8 stores sit on the epilogue's critical path) --
-    profiles/bench_r2f_tail_*.json."""
+    'acc' = tg_convT_convout_tcgen05 accumulating onto a pre-written residual (default: one coalesced read per
+    pixel instead of the in-kernel 4x4 LR gathers); 'fused' = residual and uint8 evaluated inside the tail
+    kernel."""
     v = os.environ.get('TECOGAN_B200_TAIL', 'acc')
     return {'0': None, '': None, '1': 'fused', 'fused': 'fused', '2': 'acc', 'acc': 'acc'}[v]
 
@@ -246,13 +245,15 @@ def pool_fused():
 
 
 def chain_enabled():
-    """TECOGAN_B200_CHAIN=0 runs SRNet's conv_in + residual blocks as 21 launches of
-    tg_conv_tcgen05 instead of one tg_conv_chain_tcgen05 launch (A/B measurements)."""
-    return os.environ.get('TECOGAN_B200_CHAIN', '1') != '0'
+    """TECOGAN_B200_CHAIN=1 runs SRNet's conv_in + residual blocks as one persistent tg_conv_chain_tcgen05 launch
+    instead of 21 PDL launches of tg_conv_tcgen05 (bit-identical).  Off by default: on an H100 the 21 launches
+    measured faster (the chain kernel keeps one halo stage per consumer and stalls on every layer's weight
+    reload): 1205 us per 21-layer chain against 21 x 41.7 us, bd4 shape."""
+    return os.environ.get('TECOGAN_B200_CHAIN', '0') == '1'
 
 
 def default_conv_impl():
-    """'tcgen05' (the product path) unless TECOGAN_B200_CONV=simt selects the CUDA-core
+    """'tcgen05' (the product path: the wgmma kernels; the name is historical) unless TECOGAN_B200_CONV=simt selects the CUDA-core
     cross-check kernel (bring-up / debugging only)."""
     return os.environ.get('TECOGAN_B200_CONV', 'tcgen05')
 
@@ -440,7 +441,7 @@ def _scale_ptr(scale):
 
 
 class PackedDgrad:
-    """Data-gradient operand of a conv layer: the same tcgen05 implicit GEMM with the roles of the
+    """Data-gradient operand of a conv layer: the same wgmma implicit GEMM with the roles of the
     channel dimensions swapped -- conv3x3: taps flipped (tg_pack_conv3x3_weights_dgrad); convT3x3s2: a
     stride-2 conv over the output gradient (TG_CONV_3X3_S2).  Built from the forward PackedConv."""
 

@@ -6,7 +6,7 @@ from autograd hooks, then -- every iteration -- `reduce_log` builds a tensor fro
 policy adds two scalar all-reduces + a barrier + an `.item()` (vsrgan_model.py:161-176).  Each of those is a
 host round trip on the critical path of an 8-GPU step.
 
-FlatGradientReducer is the B200-native replacement for that exchange step: every gradient of the module
+FlatGradientReducer is the GPU-native replacement for that exchange step: every gradient of the module
 lives in ONE flat fp32 buffer (the backward kernels accumulate straight into views of it), and ONE
 asynchronous NCCL all-reduce over NVLink per iteration carries the gradients AND the iteration's scalars
 (losses, discriminator statistics) in its tail -- one collective, one device->host copy when the log is read.

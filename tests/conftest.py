@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a real B200 (run by the driver with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs an sm_90a GPU (H100); select with -m gpu')
 
 
 @pytest.fixture(scope='session')

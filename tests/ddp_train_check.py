@@ -4,7 +4,7 @@ DDP with world size 1 in `reference_training_integration_ddp`):
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29541 \
         tests/ddp_train_check.py
 
-Each rank builds the reference's VSRModel (baseline/_ref, FRVSR train.yml, dist=True -> DistributedDataParallel
+Each rank builds the reference's VSRModel (oracle/_ref, FRVSR train.yml, dist=True -> DistributedDataParallel
 exactly as base_model.model_to_device wraps it) around tecogan_b200's generator, feeds DIFFERENT clips, runs one
 train() step, and the ranks then verify that (a) every parameter gradient is finite and identical on both ranks
 (NCCL all-reduce happened on gradients our backward kernels produced), (b) it equals the mean of the two

@@ -234,9 +234,8 @@ def check_conv_vs_simt(a_mode=None, cin=64, cout=64, h=134, w=320, n=1, kind=Non
 
 
 def check_conv_issue_variants(kind=None, cin_real=64, cout_real=64, h=61, w=45, n=3, residual=False):
-    """The halo convs' issue variants are the same arithmetic in the same order and must agree BIT FOR BIT:
-    two MMA issuer warps (default) vs one (TG_DBG_FLAGS=16, read per launch), and the thin-layer k-step skip
-    (tg_conv_desc.cin_real) vs all four k-steps (cin_real = 0: the skipped products are x * 0)."""
+    """The thin-layer k-step skip (tg_conv_desc.cin_real) vs all four k-steps (cin_real = 0: the skipped
+    products are x * 0) is the same arithmetic in the same order and must agree BIT FOR BIT."""
     kind = L.CONV_3X3 if kind is None else kind
     cin, cout = 64, 64
     x = nhwc(rand(140, n, cin_real, h, w, lo=-1, hi=1), cin)
@@ -245,24 +244,13 @@ def check_conv_issue_variants(kind=None, cin_real=64, cout_real=64, h=61, w=45, 
     pc = ops.PackedConv(rand(141, *wshape, lo=-bound, hi=bound).to(DEV),
                         rand(142, cout_real, lo=-0.5, hi=0.5).to(DEV), kind, L.ACT_RELU)
     res = nhwc(rand(143, n, cout_real, h, w, lo=-1, hi=1), cout) if (residual and kind == L.CONV_3X3) else None
-    old = os.environ.get('TG_DBG_FLAGS')
-    try:
-        os.environ.pop('TG_DBG_FLAGS', None)
-        dual = pc(x, residual=res, impl='tcgen05', a_mode=L.AMODE_HALO)
-        real = pc.cin_real
-        pc.cin_real = 0                                  # descriptor says: every stored input channel may be non-zero
-        dual_all_k = pc(x, residual=res, impl='tcgen05', a_mode=L.AMODE_HALO)
-        pc.cin_real = real
-        os.environ['TG_DBG_FLAGS'] = '16'
-        single = pc(x, residual=res, impl='tcgen05', a_mode=L.AMODE_HALO)
-    finally:
-        if old is None:
-            os.environ.pop('TG_DBG_FLAGS', None)
-        else:
-            os.environ['TG_DBG_FLAGS'] = old
+    dual = pc(x, residual=res, impl='tcgen05', a_mode=L.AMODE_HALO)
+    real = pc.cin_real
+    pc.cin_real = 0                                      # descriptor says: every stored input channel may be non-zero
+    dual_all_k = pc(x, residual=res, impl='tcgen05', a_mode=L.AMODE_HALO)
+    pc.cin_real = real
     ref = pc(x, residual=res, impl='simt')
     torch.cuda.synchronize()
-    assert torch.equal(dual, single), 'two issuers vs one issuer differ'
     assert torch.equal(dual, dual_all_k), 'k-step skip (cin_real) changed the result'
     e = float((dual.float() - ref.float()).abs().max() / ref.float().abs().max())
     assert e <= 2e-3, f'tcgen05 vs simt: rel max {e}'
@@ -646,7 +634,7 @@ def check_bi2_workload_parity(n=1, t=5, h=268, w=640):
 
 
 def check_reference_callers_integration():
-    """Drop-in through the reference's OWN callers (unmodified, from baseline/_ref): VSRModel built
+    """Drop-in through the reference's OWN callers (unmodified, from oracle/_ref): VSRModel built
     from the reference test YAML with define_generator patched to tecogan_b200's, driven through
     prepare_inference_data -> infer() (reflect pad_sequence, base_model.py:230-251, vsr_model.py:97-113)
     and compared with the same VSRModel holding the reference generator on the CPU; then main.profile's
@@ -781,9 +769,9 @@ def check_conv_dgrad(impl='tcgen05', kind=None, cin=64, cout=64, h=20, w=24, n=2
     return out
 
 
-def check_wgrad(kind=None, cin=64, cout=64, h=20, w=24, n=2, cin_real=None, cout_real=None, seed=320, flags=(0,)):
-    """weight gradient (tcgen05 GEMM over pixels, MN-major operands) against torch CPU autograd and the
-    CUDA-core cross-check; `flags` = TG_WGRAD_FLAGS variants to report (only the first must pass)."""
+def check_wgrad(kind=None, cin=64, cout=64, h=20, w=24, n=2, cin_real=None, cout_real=None, seed=320):
+    """weight gradient (wgmma GEMM over pixels, MN-major operands) against torch CPU autograd and the
+    CUDA-core cross-check."""
     kind = L.CONV_3X3 if kind is None else kind
     cin_real, cout_real = cin_real or cin, cout_real or cout
     x = rand(seed, n, cin_real, h, w, lo=-1, hi=1)
@@ -800,36 +788,27 @@ def check_wgrad(kind=None, cin=64, cout=64, h=20, w=24, n=2, cin_real=None, cout
     torch.cuda.synchronize()
     out['simt_rel_l2'] = rell2(dw.cpu().numpy(), dw_ref.numpy())
     assert out['simt_rel_l2'] <= 1e-4, out
-    prev = os.environ.get('TG_WGRAD_FLAGS')
-    try:
-        for fl in flags:
-            os.environ['TG_WGRAD_FLAGS'] = str(fl)
-            dw = torch.zeros(wshape, device=DEV)
-            sc = ops.GradScale(DEV).from_amax(gy.to(DEV))          # exercises the 1/scale epilogue too
-            dzs = ops.grad_pack(gy.to(DEV), scale=sc, cpad=ops.pad64(cout_real))
-            ops.wgrad(fwd, xg, dzs, dw, scale=sc)
-            ops.wgrad(fwd, xg, dzs, dw, scale=sc)                   # accumulates: 2x
-            torch.cuda.synchronize()
-            got = dw.cpu().numpy() / 2
-            out[f'tc_rel_l2_flags{fl}'] = rell2(got, dw_ref.numpy())
-            if fl == flags[0] and out[f'tc_rel_l2_flags{fl}'] > 1e-3:      # bring-up aid: where is it wrong?
-                r = dw_ref.numpy()
-                out['per_tap_rel_l2'] = [round(rell2(got[:, :, t // 3, t % 3], r[:, :, t // 3, t % 3]), 4) for t in range(9)]
-                out['transposed_rel_l2'] = rell2(got.transpose(1, 0, 2, 3), r) if got.shape[0] == got.shape[1] else None
-                out['flipped_rel_l2'] = rell2(got[:, :, ::-1, ::-1], r)
-                out['norm_ratio'] = float(np.linalg.norm(got) / np.linalg.norm(r))
-    finally:
-        if prev is None:
-            os.environ.pop('TG_WGRAD_FLAGS', None)
-        else:
-            os.environ['TG_WGRAD_FLAGS'] = prev
-    assert out[f'tc_rel_l2_flags{flags[0]}'] <= 1e-3, out
+    dw = torch.zeros(wshape, device=DEV)
+    sc = ops.GradScale(DEV).from_amax(gy.to(DEV))          # exercises the 1/scale epilogue too
+    dzs = ops.grad_pack(gy.to(DEV), scale=sc, cpad=ops.pad64(cout_real))
+    ops.wgrad(fwd, xg, dzs, dw, scale=sc)
+    ops.wgrad(fwd, xg, dzs, dw, scale=sc)                   # accumulates: 2x
+    torch.cuda.synchronize()
+    got = dw.cpu().numpy() / 2
+    out['tc_rel_l2'] = rell2(got, dw_ref.numpy())
+    if out['tc_rel_l2'] > 1e-3:                             # bring-up aid: where is it wrong?
+        r = dw_ref.numpy()
+        out['per_tap_rel_l2'] = [round(rell2(got[:, :, t // 3, t % 3], r[:, :, t // 3, t % 3]), 4) for t in range(9)]
+        out['transposed_rel_l2'] = rell2(got.transpose(1, 0, 2, 3), r) if got.shape[0] == got.shape[1] else None
+        out['flipped_rel_l2'] = rell2(got[:, :, ::-1, ::-1], r)
+        out['norm_ratio'] = float(np.linalg.norm(got) / np.linalg.norm(r))
+    assert out['tc_rel_l2'] <= 1e-3, out
     db = torch.zeros(cout_real, device=DEV)
     ops.bias_grad(dzg, db)
     torch.cuda.synchronize()
     out['bias_rel_l2'] = rell2(db.cpu().numpy(), f16(gy).sum((0, 2, 3)).numpy())
     assert out['bias_rel_l2'] <= 1e-4, out
-    # bias gradient fused into the wgrad launch (conv layers: the spare half of the last tap pair reads ones)
+    # bias gradient through the wgrad call (conv layers: a reduction over dz after the GEMM)
     db2, dw2 = torch.zeros(cout_real, device=DEV), torch.zeros(wshape, device=DEV)
     ops.wgrad(fwd, xg, dzg, dw2, db=db2)
     torch.cuda.synchronize()
@@ -1003,7 +982,7 @@ def check_fnet_autograd_public():
 
 def check_reference_training_integration(ddp=False):
     """The reference's OWN training loop on the swapped-in generator: VSRModel (FRVSR train.yml:
-    Charbonnier pixel loss + warping loss through net_utils.backward_warp, Adam) built from baseline/_ref
+    Charbonnier pixel loss + warping loss through net_utils.backward_warp, Adam) built from oracle/_ref
     with define_generator patched, one train() step on the GPU vs the same step with the reference
     generator on the CPU: logged losses, gradient norms, and the updated weights of both optimisers.
     ddp=True wraps the generator in DistributedDataParallel (NCCL, world size 1 here; 2 ranks in
@@ -1075,7 +1054,7 @@ def check_reference_training_integration(ddp=False):
 def check_reference_gan_training_integration():
     """BASELINE config 3 in miniature: the reference's TecoGAN training loop (VSRGANModel.train: adaptive
     ST-discriminator, VGG perceptual loss, ping-pong, warping and GAN losses; vsrgan_model.py:98-286) from
-    baseline/_ref with tecogan_b200's generator dropped in, one step on the GPU against the same step with
+    oracle/_ref with tecogan_b200's generator dropped in, one step on the GPU against the same step with
     the reference generator on the CPU (same D / VGG weights): every logged loss and the generator's
     gradient norms.  Gradients reach the generator through hr_data (pixel / VGG / ping-pong / GAN via the
     discriminator's own backward_warp) and through lr_flow (warping loss)."""
@@ -1119,7 +1098,7 @@ def check_reference_gan_training_integration():
 
 def check_st_discriminator_input():
     """tg_st_disc_input (f3) against the reference's own SpatioTemporalDiscriminator.forward_sequence from
-    baseline/_ref: its input tensor is captured at conv_in, for use_pp_crit = True (flows taken from the
+    oracle/_ref: its input tensor is captured at conv_in, for use_pp_crit = True (flows taken from the
     generator's hr_flow) -- values and the gradient w.r.t. the frames."""
     import refimport
     refimport.import_generator()
@@ -1305,11 +1284,11 @@ CHECKS = {
     'dgrad_tc_conv_thin': lambda: check_conv_dgrad('tcgen05', cin=64, cout=64, cin_real=32, cout_real=2, mask_act=L.ACT_LRELU02),
     'dgrad_tc_convT': lambda: check_conv_dgrad('tcgen05', kind=L.CONVT_3X3_S2, h=21, w=12, mask_act=L.ACT_RELU),
     'dgrad_tc_convT_fullrow': lambda: check_conv_dgrad('tcgen05', kind=L.CONVT_3X3_S2, h=64, w=64, n=1),
-    'wgrad_conv': lambda: check_wgrad(flags=(0, 1, 2, 3)),
+    'wgrad_conv': lambda: check_wgrad(),
     'wgrad_conv_ragged': lambda: check_wgrad(h=37, w=29, n=3),
     'wgrad_conv_thin': lambda: check_wgrad(cin_real=51, cout_real=3, h=24, w=40),
     'wgrad_conv_128_256': lambda: check_wgrad(cin=128, cout=256, h=16, w=40),
-    'wgrad_convT': lambda: check_wgrad(kind=L.CONVT_3X3_S2, h=18, w=20, flags=(0, 1, 2, 3)),
+    'wgrad_convT': lambda: check_wgrad(kind=L.CONVT_3X3_S2, h=18, w=20),
     'wgrad_convT_ragged': lambda: check_wgrad(kind=L.CONVT_3X3_S2, h=21, w=13, n=3),
     'backward_elementwise': check_backward_elementwise,
     'fnet_autograd_public': check_fnet_autograd_public,

@@ -1,9 +1,8 @@
 """CPU: pin the oracle (oracle/) against outputs of the UNMODIFIED reference.
 
 The fixtures in tests/golden were written by oracle/gen_golden.py, which imports
-/root/reference and runs it on seeded inputs.  When /root/reference is present
-(build container) the oracle is additionally compared with the live reference at
-the BASELINE size 3x134x320.
+the reference and runs it on seeded inputs; at the BASELINE size 3x134x320 a
+seeded sample of the reference's output is stored.
 """
 import os
 import sys
@@ -149,25 +148,15 @@ def test_state_dict_layout_matches_reference_counts():
     assert n == 2589093
 
 
-# ------------------------------------------------------------------ live reference (build container only)
-@pytest.mark.skipif(not os.path.isdir('/root/reference/codes'), reason='reference not mounted')
+# ------------------------------------------------------------------ reference at full size
 def test_oracle_vs_live_reference_full_size():
-    R = '/root/reference/codes'
-    if R not in sys.path:
-        sys.path.insert(0, R)
-    m = types.ModuleType('metrics')
-    m.__path__ = [R + '/metrics']
-    sys.modules.setdefault('metrics', m)
-    from models.networks.tecogan_nets import FRNet
-    net = FRNet(3, 3, 64, 10, 'BD', 4)
+    """The unmodified reference FRNet.step at the bench size (1 clip, 3x134x320 -> 536x1280, 2x weights),
+    stored as a fixed, seeded sample of 65536 output values (the full frame exceeds the fixture budget)."""
+    g = np.load(os.path.join(G, 'step_bd4_134x320_g2_sample.npz'))
     p = O.make_frnet_params(5, gain=2.0)
-    net.load_state_dict(p, strict=True)
-    net.eval()
     lr_curr, lr_prev, hr_prev = rand(1, 1, 3, 134, 320), rand(2, 1, 3, 134, 320), rand(3, 1, 3, 536, 1280)
-    with torch.no_grad():
-        ref = net.step(lr_curr, lr_prev, hr_prev)
-    hr = O.frnet_step(p, lr_curr, lr_prev, hr_prev, 4, 'BD')
-    assert relerr(hr.numpy(), ref.numpy()) <= 5e-5
+    hr = O.frnet_step(p, lr_curr, lr_prev, hr_prev, 4, 'BD').numpy().reshape(-1)
+    assert relerr(hr[g['index']], g['hr_curr']) <= 5e-5
 
 
 # ------------------------------------------------------------------ library-op restatement (bench CPU baseline)
