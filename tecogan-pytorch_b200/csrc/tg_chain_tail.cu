@@ -72,7 +72,6 @@ __device__ __forceinline__ void st_release_u32(uint32_t* p, uint32_t v) {
   asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // plain (L1-coherent within the SM) 16-byte load: chain residuals were written earlier in the same launch
 __device__ __forceinline__ uint4 ld_global_u4(const void* p) {
   uint4 v;

@@ -21,6 +21,15 @@
 //             the pixel's 128-byte NHWC row.  One consumer's epilogue overlaps the other's MMAs.
 //             The transposed conv keeps 4 parity accumulators (1/2/2/4 taps), computed and stored
 //             one after the other; each stores its pixel's output of that parity (pixel shuffle).
+//
+// The forward 3x3 halo conv with NHWC output (the SRNet body and the FNet halo layers; see
+// consumer_halo_pxn) swaps the GEMM's roles: M = the 64 output channels (the packed weight tile is the
+// K-major A operand), N = the tile's 128 pixels (the halo view is the K-major B operand, 16 core groups
+// of 8 pixels), so each (tap, k-step) is ONE m64n128k16 that reads 6 KB of smem instead of two
+// m64n64k16 that read 8 KB.  Its epilogue works from registers: bias / act / residual -> fp16 ->
+// stmatrix into a 16 KB tile in the TMA box image -> one TMA tensor store per tile; the residual
+// arrives in that tile by one TMA load issued before the tile's MMAs.  Without the fp32 staging tiles
+// each consumer's ring holds two halo stages instead of one.
 #include <cuda.h>
 
 #include <cstdlib>
@@ -62,8 +71,15 @@ struct KParams {
   int ksteps;                      // wgmma k-steps (16 channels) per 64-channel chunk that can hold non-zero input (1..4)
   int n_split, bn;                 // output channels are split over n_split CTAs of bn columns
   uint32_t stage_bytes, a_bytes, b_tile_bytes, b_stage_bytes;
-  uint32_t off_b, off_stage, off_scratch;
+  uint32_t off_b, off_stage, off_scratch;   // off_scratch: the consumers' fp32 staging or fp16 output tiles
 };
+
+// The forward 3x3 halo conv with NHWC output puts the roles of the GEMM the other way round:
+// D[cout][pixel] = W . X^T, the 64 output channels on M and the tile's 128 pixels on N.
+template <int KIND, int MODE, bool BWD, bool POOL>
+__host__ __device__ constexpr bool pixels_on_n() {
+  return KIND == TG_CONV_3X3 && MODE == MODE_HALO && !BWD && !POOL;
+}
 
 struct TileCoord { int n, y0, x0, nb; };
 __device__ __forceinline__ TileCoord tile_coord(const KParams& p, int tile) {
@@ -185,6 +201,109 @@ __device__ __forceinline__ void epilogue_nhwc(const KParams& p, const TileCoord&
   (void)lane;
 }
 
+// ------------------------------------------------------------------ consumer of the pixels-on-N path
+// One consumer warpgroup (cw) of the forward 3x3 halo conv, NHWC fp16 output: for each of its tiles
+//   D[64 cout][128 px] = sum over (tap, chunk, k-step) of m64n128k16(A = resident weight tile, K-major,
+//                        SBO 1024; B = the tap's shifted view of the halo stage, K-major, SBO = one box row)
+// then an epilogue from registers into a 16 KB tile in the TMA box image (16x8 px x 64 ch, 128B swizzle)
+// that one TMA tensor store writes out (clipped at the image edge).  The residual, if any, is TMA-loaded
+// into the same tile before the tile's MMAs and overwritten in place.  Thread t of the warpgroup holds
+// rows (couts) 16*(t/32) + (t%32)/4 + {0, 8} and pixel columns 8*j + 2*(t%4) + {0, 1}, j = 0..15.
+__device__ __forceinline__ void consumer_halo_pxn(const TgMaps& maps, const KParams& p, uint32_t base,
+                                                  const float* bias_s, int cw) {
+  const tg_conv_desc& d = p.d;
+  const int r = threadIdx.x - 128 * (1 + cw);
+  const int q = r >> 5, lane = threadIdx.x & 31;
+  const uint32_t bar_full = base + 8u * (cw * kMaxRing), bar_empty = base + 16 * kMaxRing + 8u * (cw * kMaxRing);
+  const uint32_t bar_res = base + 32 * kMaxRing + 8 + 8u * cw;
+  const uint32_t stage0 = base + p.off_stage + (uint32_t)(cw * p.ring) * p.stage_bytes;
+  const uint32_t out_s = base + p.off_scratch + (uint32_t)cw * kTapABytes;
+  constexpr uint32_t kBoxW = TW + 2;
+  const uint64_t w_hi = gmma_desc_hi(1024u), x_hi = gmma_desc_hi(kBoxW * 128u);
+  const uint32_t w16 = gmma_addr16(base + p.off_b), btb16 = p.b_stage_bytes >> 4;
+  const bool has_res = d.residual != nullptr;
+  const int bar_id = 1 + cw;
+  // stmatrix / ldmatrix: lane l addresses pixel row l%8 of 8x8 matrix m = l/8 = (tile row 2*jp + m/2,
+  // 8-channel chunk 2*q + m%2); the swizzled offset of (pixel px, chunk) is px*128 + ((chunk ^ px%8) << 4)
+  const uint32_t mat_off = (uint32_t)(8 * ((lane >> 3) >> 1) + (lane & 7)) * 128u +
+                           ((uint32_t)((2 * q + ((lane >> 3) & 1)) ^ (lane & 7)) << 4);
+  int stage = 0;
+  uint32_t phase = 0, rphase = 0;
+  float acc[64];
+
+  for (int tile = blockIdx.x + cw * (int)gridDim.x; tile < p.num_tiles; tile += 2 * (int)gridDim.x) {
+    const TileCoord tc = tile_coord(p, tile);
+    if (r == 0) {
+      bulk_wait_group_read0();           // the previous tile's store has left the output tile
+      if (has_res) {
+        mbar_expect_tx(bar_res, kTapABytes);
+        tma_load_4d(out_s, &maps.m[1], bar_res, tc.nb * 64, tc.x0, tc.y0, tc.n);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    int pend = -1;                       // stage whose MMAs may still be reading it
+    for (int c = 0; c < p.chunks; ++c) {
+      const int s = stage;
+      mbar_wait_mma(bar_full + 8 * s, phase);
+      if (++stage == p.ring) { stage = 0; phase ^= 1u; }
+      const uint32_t x16 = gmma_addr16(stage0 + (uint32_t)s * p.stage_bytes);
+      wgmma_fence();
+#pragma unroll
+      for (int g = 0; g < 9; ++g) {
+        const TgGroup gr = tg_group(TG_CONV_3X3, g);
+        const uint32_t a16 = w16 + (uint32_t)(g * p.chunks + c) * btb16;
+        const uint32_t b16 = x16 + (uint32_t)((gr.dy + 1) * (int)kBoxW + (gr.dx + 1)) * 8u;
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          if (k < p.ksteps)
+            wgmma_n128(acc, w_hi | (uint64_t)(a16 + 2u * k), x_hi | (uint64_t)(b16 + 2u * k),
+                       (g == 0 && c == 0 && k == 0) ? 0u : 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (pend >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_empty + 8 * pend); }
+      pend = s;
+    }
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_empty + 8 * pend);
+
+    // the output tile is free once thread 0 saw the previous store read it (it issued the residual load after)
+    if (has_res) { mbar_wait_mma(bar_res, rphase); rphase ^= 1u; }
+    else named_bar_sync(bar_id, 128);
+    const float b0 = bias_s[tc.nb * 64 + 16 * q + (lane >> 2)], b1 = bias_s[tc.nb * 64 + 16 * q + (lane >> 2) + 8];
+#pragma unroll
+    for (int jp = 0; jp < 8; ++jp) {
+      const uint32_t addr = out_s + (uint32_t)jp * 2048u + mat_off;
+      uint32_t rv[4], ov[4];
+      if (has_res) ldmatrix_x4_trans(addr, rv);
+#pragma unroll
+      for (int m = 0; m < 4; ++m) {
+        const int i = 4 * (2 * jp + (m >> 1)) + 2 * (m & 1);
+        const float bb = (m & 1) ? b1 : b0;
+        float a0 = tg_epi_val(acc[i], bb, d.act), a1 = tg_epi_val(acc[i + 1], bb, d.act);
+        if (has_res) {
+          const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(&rv[m]));
+          a0 += rf.x; a1 += rf.y;
+        }
+        const __half2 o = __floats2half2_rn(a0, a1);
+        ov[m] = *reinterpret_cast<const uint32_t*>(&o);
+      }
+      stmatrix_x4_trans(addr, ov);
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(bar_id, 128);
+    if (r == 0) {
+      tma_store_4d(&maps.m[2], out_s, tc.nb * 64, tc.x0, tc.y0, tc.n);
+      bulk_commit_group();
+    }
+  }
+  // the stores must be complete before the CTA exits (its shared memory goes, and a dependent kernel's
+  // griddepcontrol.wait must see the data)
+  if (r == 0) bulk_wait_group0();
+}
+
 // ------------------------------------------------------------------ the kernel
 // BWD = data-gradient instantiation: epilogue y = (acc + bias [+ residual]) * act'(mask)  (TG_ACT_DRELU /
 // TG_ACT_DLRELU02; TG_ACT_NONE = no derivative).
@@ -207,12 +326,15 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
   const uint32_t bar_full = base;                          // [2 * kMaxRing]
   const uint32_t bar_empty = base + 16 * kMaxRing;         // [2 * kMaxRing]
   const uint32_t bar_b = base + 32 * kMaxRing;             // [1]
+  const uint32_t bar_res = bar_b + 8;                      // [2] residual tile of consumer c
   float* bias_s = reinterpret_cast<float*>(sm + 1024);
   static_assert(!(KIND == TG_CONV_3X3_S2 && MODE != MODE_TAP), "the stride-2 conv runs in tap mode only");
+  constexpr bool kPxN = pixels_on_n<KIND, MODE, BWD, POOL>();
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&maps.m[0]);
     if (KIND == TG_CONV_3X3_S2) { tma_prefetch_desc(&maps.m[1]); tma_prefetch_desc(&maps.m[2]); tma_prefetch_desc(&maps.m[3]); }
+    if (kPxN) { tma_prefetch_desc(&maps.m[1]); tma_prefetch_desc(&maps.m[2]); }
   }
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < 2 * kMaxRing; ++s) {
@@ -220,6 +342,8 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
       mbar_init(bar_empty + 8 * s, 4);     // one arrival per consumer warp
     }
     mbar_init(bar_b, 1);
+    mbar_init(bar_res, 1);
+    mbar_init(bar_res + 8, 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -275,6 +399,12 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
           if (++stage[cw] == p.ring) { stage[cw] = 0; phase[cw] ^= 1u; }
         }
       }
+    }
+  } else if (kPxN) {
+    // ============================================================ consumers, pixels on N
+    if (warp >= 4) {
+      if (p.b_resident) mbar_wait_mma(bar_b, 0);
+      consumer_halo_pxn(maps, p, base, bias_s, (warp - 4) >> 2);
     }
   } else if (warp >= 4) {
     // ============================================================ consumers
@@ -622,7 +752,12 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
     p.a_bytes = kTapABytes;
     p.stage_bytes = kTapABytes + (p.b_resident ? 0u : p.b_stage_bytes);
   }
-  const uint32_t avail = kSmemLimit - fixed - (p.b_resident ? b_total : 0u);
+  // the consumers' epilogue tiles: fp16 output / residual tiles (16 KB each) on the pixels-on-N path,
+  // fp32 accumulator staging otherwise
+  const bool bwd = d->act >= TG_ACT_DRELU || d->kind == TG_CONV_3X3_S2;
+  const bool pxn = p.halo && d->kind == TG_CONV_3X3 && !bwd && !pool && !tapn;
+  const uint32_t epi_tiles = pxn ? 2u * kTapABytes : scratch;
+  const uint32_t avail = kSmemLimit - 1024u - kHeaderBytes - epi_tiles - (p.b_resident ? b_total : 0u);
   int ring = (int)(avail / p.stage_bytes) / 2;
   if (ring > kMaxRing) ring = kMaxRing;
   TG_REQUIRE(ring >= 1, TG_E_UNSUPPORTED, "conv: shared memory budget (cin=%d cout=%d)", d->cin, d->cout);
@@ -630,7 +765,7 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
   p.off_b = kHeaderBytes;
   p.off_stage = kHeaderBytes + (p.b_resident ? b_total : 0u);
   p.off_scratch = p.off_stage + 2u * (uint32_t)ring * p.stage_bytes;   // consumer c's ring: stages [c*ring, (c+1)*ring)
-  const uint32_t smem_bytes = 1024u + p.off_scratch + scratch;
+  const uint32_t smem_bytes = 1024u + p.off_scratch + epi_tiles;
   TG_REQUIRE(smem_bytes <= kSmemLimit, TG_E_UNSUPPORTED, "conv: smem %u > limit", smem_bytes);
 
   // tensor maps
@@ -640,6 +775,19 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
                      (size_t)d->h * d->w * d->cin, 64, p.box_w, p.box_h);
     if (rc != TG_OK) return rc;
     map_a.m[1] = map_a.m[2] = map_a.m[3] = map_a.m[0];
+    if (pxn) {
+      // [1] = residual, [2] = output: NHWC [n][h][w][cout], one 16x8 px x 64 ch box per tile and N slice
+      const size_t C = (size_t)d->cout;
+      if (d->residual) {
+        TG_REQUIRE(((uintptr_t)d->residual & 15) == 0, TG_E_INVALID, "conv: residual must be 16-byte aligned");
+        rc = encode_nhwc(&map_a.m[1], d->residual, d->cout, d->w, d->h, d->n, C, (size_t)d->w * C,
+                         (size_t)d->h * d->w * C, 64, TW, TH);
+        if (rc != TG_OK) return rc;
+      }
+      rc = encode_nhwc(&map_a.m[2], d->y, d->cout, d->w, d->h, d->n, C, (size_t)d->w * C,
+                       (size_t)d->h * d->w * C, 64, TW, TH);
+      if (rc != TG_OK) return rc;
+    }
   } else {
     // x [n,2h,2w,cin]: parity plane (py,px) = pixels (2i+py, 2j+px), each an [n,h,w,cin] strided view
     const size_t W2 = (size_t)2 * d->w, C = (size_t)d->cin;
@@ -676,7 +824,6 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const dim3 g(grid), b(kThreads);
   cudaError_t lerr = cudaSuccess;
-  const bool bwd = d->act >= TG_ACT_DRELU || d->kind == TG_CONV_3X3_S2;
   if (pool) {
     lerr = p.halo ? tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_HALO, false, true>, g, b, kSmemLimit, st, map_a, p)
                   : tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_TAP, false, true>, g, b, kSmemLimit, st, map_a, p);

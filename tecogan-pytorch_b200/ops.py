@@ -246,9 +246,10 @@ def pool_fused():
 
 def chain_enabled():
     """TECOGAN_B200_CHAIN=1 runs SRNet's conv_in + residual blocks as one persistent tg_conv_chain_tcgen05 launch
-    instead of 21 PDL launches of tg_conv_tcgen05 (bit-identical).  Off by default: on an H100 the 21 launches
-    measured faster (the chain kernel keeps one halo stage per consumer and stalls on every layer's weight
-    reload): 1205 us per 21-layer chain against 21 x 41.7 us, bd4 shape."""
+    instead of 21 PDL launches of tg_conv_tcgen05 (same products in the same order, with its own mainloop; held
+    to a 4e-3 relative tolerance against them).  Off by default: on an H100 the 21 launches measured faster
+    (the chain kernel keeps one halo stage per consumer and stalls on every layer's weight reload): 1205 us per
+    21-layer chain against 21 x 41.7 us of the previous per-layer kernel, bd4 shape."""
     return os.environ.get('TECOGAN_B200_CHAIN', '0') == '1'
 
 
