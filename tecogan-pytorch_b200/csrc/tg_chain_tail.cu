@@ -11,13 +11,16 @@
 //
 // convT_convout_kernel -- SRNet tail: last ConvTranspose2d(64,64,3,2,1,op=1) + ReLU -> conv_out 3x3
 //   (64 -> out_nc <= 3) -> + upsample_func(lr_curr) or + the pre-written frame -> fp32 NCHW (+ uint8 NHWC).
-//   Per 16x8 tile of the transposed conv's input (17x9 halo box): the four parity accumulators are
-//   computed one after the other and written, +bias, ReLU, fp16, straight from the wgmma fragments into
-//   shared memory as four 128-pixel K-major 128B-swizzled operand blocks (pixels outside the image are
-//   zero = conv_out's zero padding).  conv_out then runs as "tap-major N" wgmmas (N = 48 = 9 taps x 4
-//   couts) on those blocks; the tap products overwrite the block they came from, and the 3x3 shift-add
-//   produces the 30x14 interior HR pixels of the tile (tiles advance by 15x7 input pixels, the
-//   transposed conv is recomputed on a one-pixel ring).  The 64-channel HR map never reaches HBM.
+//   Per 16x8 tile of the transposed conv's input (17x9 halo box), parity by parity: the transposed conv
+//   runs pixels-on-N (M = 64 couts, N = the 128 input pixels, one m64n128k16 per (tap group, k-step));
+//   its accumulators are written, +bias, ReLU, fp16, by stmatrix into one 128-pixel K-major 128B-swizzled
+//   operand block (pixels outside the image are zero = conv_out's zero padding); conv_out runs as
+//   "tap-major N" wgmmas (N = 48 = 9 taps x 4 couts) on that block; each thread adds the fp32 tap
+//   products that land on its 4 output pixels into registers, while the next parity's transposed conv
+//   is already in flight.  The tile's 30x14 interior HR pixels are outputs (tiles advance by 15x7 input
+//   pixels, the transposed conv is recomputed on a one-pixel ring).  Two consumer warpgroups take the
+//   CTA's tiles alternately, so one's epilogue and global I/O overlap the other's MMAs; the frame the
+//   tile adds onto is read into registers before the tile's MMAs.  The 64-channel HR map never reaches HBM.
 #include <cuda.h>
 
 #include <mutex>
@@ -79,27 +82,52 @@ __device__ __forceinline__ uint4 ld_global_u4(const void* p) {
   return v;
 }
 
-// halo-mode conv taps of one 16x8 tile: acc[h] (+)= A view(tap) x W[tap], tile rows 8h..8h+7.  box_w = 10 for
-// the conv (origin -1), 9 for the transposed conv (origin 0, groups of parity accumulator `acc_sel`).
-template <int KIND>
-__device__ __forceinline__ void halo_mmas(float (&acc)[2][32], uint32_t sa16, uint32_t w16, int acc_sel) {
-  constexpr int kBoxW = KIND == TG_CONV_3X3 ? TW + 2 : TW + 1;
-  constexpr int kOrg = KIND == TG_CONV_3X3 ? -1 : 0;
+// halo-mode conv taps of one 16x8 tile (18x10 box, origin -1): acc[h] (+)= A view(tap) x W[tap], tile rows 8h..8h+7
+__device__ __forceinline__ void halo_mmas(float (&acc)[2][32], uint32_t sa16, uint32_t w16) {
+  constexpr int kBoxW = TW + 2;
   const uint64_t a_hi = gmma_desc_hi((uint32_t)kBoxW * 128u), b_hi = gmma_desc_hi(1024u);
   constexpr uint32_t half16 = (8u * kBoxW * 128u) >> 4;
 #pragma unroll
   for (int g = 0; g < 9; ++g) {
-    const TgGroup gr = tg_group(KIND, g);
-    if (KIND != TG_CONV_3X3 && gr.acc != acc_sel) continue;
-    const bool first = g == 0 || tg_group(KIND, g > 0 ? g - 1 : 0).acc != gr.acc;
-    const uint32_t a16 = sa16 + (uint32_t)((gr.dy - kOrg) * kBoxW + (gr.dx - kOrg)) * 8u;
+    const TgGroup gr = tg_group(TG_CONV_3X3, g);
+    const uint32_t a16 = sa16 + (uint32_t)((gr.dy + 1) * kBoxW + (gr.dx + 1)) * 8u;
     const uint32_t b16 = w16 + (uint32_t)g * (kWtBytes / 9 / 16);
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const uint32_t sc = (first && k == 0) ? 0u : 1u;
+      const uint32_t sc = (g == 0 && k == 0) ? 0u : 1u;
       wgmma_n64(acc[0], a_hi | (uint64_t)(a16 + 2u * k), b_hi | (uint64_t)(b16 + 2u * k), sc);
       wgmma_n64(acc[1], a_hi | (uint64_t)(a16 + half16 + 2u * k), b_hi | (uint64_t)(b16 + 2u * k), sc);
     }
+  }
+}
+
+// transposed-conv taps of parity accumulator `a` (1/2/2/4 groups) of one 16x8 tile, pixels on N:
+//   acc[64 cout][128 px] (+)= W[group] (A: the packed [cout][64] tile, K-major, SBO 1024)
+//                             x the group's shifted view of the 17x9 halo box (B: K-major, 16 core groups of
+//                             8 pixels, SBO = one box row of 9 x 128 B, origin 0, start += (dy*9+dx)*128 B)
+// one m64n128k16 per (group, k-step).  The first MMA of the parity overwrites acc (scale-d = 0).
+template <int A>
+__device__ __forceinline__ void convT_pxn_parity(float (&acc)[64], uint32_t x16, uint32_t w16) {
+  constexpr uint32_t kBoxW = TW + 1;
+  const uint64_t w_hi = gmma_desc_hi(1024u), x_hi = gmma_desc_hi(kBoxW * 128u);
+#pragma unroll
+  for (int g = 0; g < 9; ++g) {
+    const TgGroup gr = tg_group(TG_CONVT_3X3_S2, g);
+    if (gr.acc != A) continue;
+    const bool first = g == 0 || tg_group(TG_CONVT_3X3_S2, g > 0 ? g - 1 : 0).acc != gr.acc;
+    const uint32_t a16 = w16 + (uint32_t)g * (kWtBytes / 9 / 16);
+    const uint32_t b16 = x16 + (uint32_t)(gr.dy * (int)kBoxW + gr.dx) * 8u;
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      wgmma_n128(acc, w_hi | (uint64_t)(a16 + 2u * k), x_hi | (uint64_t)(b16 + 2u * k), (first && k == 0) ? 0u : 1u);
+  }
+}
+__device__ __forceinline__ void convT_pxn_mmas(float (&acc)[64], uint32_t x16, uint32_t w16, int a) {
+  switch (a) {
+    case 0: convT_pxn_parity<0>(acc, x16, w16); break;
+    case 1: convT_pxn_parity<1>(acc, x16, w16); break;
+    case 2: convT_pxn_parity<2>(acc, x16, w16); break;
+    default: convT_pxn_parity<3>(acc, x16, w16); break;
   }
 }
 
@@ -218,7 +246,7 @@ __global__ void __launch_bounds__(kChainThreads, 1) conv_chain_kernel(const __gr
 #pragma unroll
           for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
         wgmma_fence();
-        halo_mmas<TG_CONV_3X3>(acc, sa16, w16, 0);
+        halo_mmas(acc, sa16, w16);
         wgmma_commit();
         wgmma_wait<0>();
         __syncwarp();
@@ -284,20 +312,25 @@ __global__ void __launch_bounds__(kChainThreads, 1) conv_chain_kernel(const __gr
 }
 
 // ================================================================== SRNet tail
-constexpr int kTailThreads = 256;                    // producer warpgroup + 1 consumer warpgroup
+// two consumer warpgroups, each loading its own halo boxes (no producer warp: 256 threads leave up to 255
+// registers per thread for acc, the conv_out products and the 12 output sums)
+constexpr int kTailThreads = 256;
 constexpr int kStepY = 15, kStepX = 7;               // input pixels a tile advances by
 constexpr uint32_t kTailHalo = (TW + 1) * (TH + 1) * 128;            // 19584
 constexpr uint32_t kTailStage = (kTailHalo + 1023u) & ~1023u;        // 20480
 constexpr uint32_t kWoBytes = TG_TAPN_ROWS * 128;                    // [48 rows = tap*4+co][64]
 constexpr uint32_t kHrBlock = 128 * 128;                             // one parity block: 128 px x 128 B
+constexpr int kD2Pitch = 27;                         // tap products kept per HR pixel: 9 taps x 3 couts (fp32)
+// the tap products of one parity block [128 px][27] fp32, + room for the shift-add's reads one block row and one
+// tap row past the end (the reads one block row before the start land in the operand block)
+constexpr uint32_t kD2Bytes = (((128 + 9) * kD2Pitch + 12) * 4 + 1023u) & ~1023u;   // 15360
+// per consumer: two halo stages, one parity's operand block, that parity's fp32 tap products
+constexpr uint32_t kTailCons = 2 * kTailStage + kHrBlock + kD2Bytes;  // 72704
 constexpr uint32_t kTailOffWt = 2048;
 constexpr uint32_t kTailOffWo = kTailOffWt + kWtBytes;               // 75776
-constexpr uint32_t kTailOffStage = kTailOffWo + kWoBytes;            // 81920
-constexpr uint32_t kTailOffHr = kTailOffStage + 2 * kTailStage;      // 122880
-constexpr uint32_t kTailSmem = 1024 + kTailOffHr + 4 * kHrBlock;     // 189440
+constexpr uint32_t kTailOffCons = kTailOffWo + kWoBytes;             // 81920
+constexpr uint32_t kTailSmem = 1024 + kTailOffCons + 2 * kTailCons;  // 228352
 static_assert(kTailSmem <= kSmemLimit, "tail smem");
-constexpr int kD2Pitch = 27;                         // tap products kept per HR pixel: 9 taps x 3 couts (fp32)
-static_assert(128 * kD2Pitch * 4 <= (int)kHrBlock, "tap products of a block fit into the block");
 
 struct TailParams {
   CUtensorMap map_x;
@@ -318,21 +351,19 @@ __global__ void __launch_bounds__(kTailThreads, 1) convT_convout_kernel(const __
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* sm = smem_raw + (base - raw);
   const int warp = __shfl_sync(0xFFFFFFFFu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
-  const uint32_t bar_full = base, bar_empty = base + 16, bar_w = base + 32;
+  // halo stage s of consumer c: barrier at index 2 * c + s
+  const uint32_t bar_full = base, bar_w = base + 32;
   float* bup_s = reinterpret_cast<float*>(sm + 1024);
   float* bout_s = reinterpret_cast<float*>(sm + 1024 + 256);
 
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, 4);
-    }
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < 4; ++s) mbar_init(bar_full + 8 * s, 1);
     mbar_init(bar_w, 1);
     fence_barrier_init();
   }
   __syncthreads();
   // weights are static: load them before the programmatic-dependent-launch wait
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.map_x);
     mbar_expect_tx(bar_w, kWtBytes + kWoBytes);
     for (int t = 0; t < 9; ++t) bulk_load(base + kTailOffWt + t * 8192u, p.w_up + (size_t)t * 8192u, 8192u, bar_w);
@@ -344,92 +375,104 @@ __global__ void __launch_bounds__(kTailThreads, 1) convT_convout_kernel(const __
   if (threadIdx.x < 4) bout_s[threadIdx.x] = threadIdx.x < p.cout_real ? __ldg(p.b_out + threadIdx.x) : 0.f;
   __syncthreads();
   const int per_img = p.tiles_x * p.tiles_y;
+  const int grid = (int)gridDim.x;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        const int img = tile / per_img, rr = tile - img * per_img;
-        const int y0 = (rr / p.tiles_x) * kStepY - 1, x0 = (rr % p.tiles_x) * kStepX - 1;
-        mbar_wait_mma(bar_empty + 8 * stage, phase ^ 1);
-        mbar_expect_tx(bar_full + 8 * stage, kTailHalo);
-        tma_load_4d(base + kTailOffStage + (uint32_t)stage * kTailStage, &p.map_x, bar_full + 8 * stage, 0, x0, y0,
-                    img);
-        if (++stage == 2) { stage = 0; phase ^= 1u; }
-      }
-    }
-  } else if (warp >= 4) {
-    const int r = threadIdx.x - 128, q = r >> 5;
-    const uint32_t hr = base + kTailOffHr;
-    uint8_t* hr_p = sm + kTailOffHr;
-    const uint32_t wt16 = gmma_addr16(base + kTailOffWt);
-    const uint64_t b_hi = gmma_desc_hi(1024u);
-    const uint32_t wo16 = gmma_addr16(base + kTailOffWo);
+  {
+    // ============================================================ consumers
+    const int cw = warp >> 2;
+    const int r = threadIdx.x - 128 * cw, q = r >> 5;
+    const int bar_id = 1 + cw;
+    const uint32_t cons = base + kTailOffCons + (uint32_t)cw * kTailCons;
+    const uint32_t blk = cons + 2 * kTailStage;
+    float* D2 = reinterpret_cast<float*>(sm + (blk - base) + kHrBlock);
+    const uint32_t wt16 = gmma_addr16(base + kTailOffWt), wo16 = gmma_addr16(base + kTailOffWo);
+    const uint32_t blk16 = gmma_addr16(blk);
+    const uint64_t k_hi = gmma_desc_hi(1024u);
+    // stmatrix: lane l addresses pixel row l%8 of 8x8 matrix m = l/8 = (tile row 2*jp + m/2, 8-channel chunk
+    // 2*q + m%2); the swizzled offset of (pixel px, chunk) in the block is px*128 + ((chunk ^ px%8) << 4)
+    const uint32_t mat_off = (uint32_t)(8 * ((lane >> 3) >> 1) + (lane & 7)) * 128u +
+                             ((uint32_t)((2 * q + ((lane >> 3) & 1)) ^ (lane & 7)) << 4);
+    const float b0 = bup_s[16 * q + (lane >> 2)], b1 = bup_s[16 * q + (lane >> 2) + 8];
+    // this thread's HR pixels of the tile's 32x16: (Y0 + 8j, X), j = 0..3; the interior 30x14 are outputs
+    const int Y0 = r >> 4, X = r & 15;
     const int H = 2 * p.h, W = 2 * p.w;
     const int lh = H / p.lr_scale, lw = W / p.lr_scale;
+    // the consumer's k-th tile is blockIdx.x + (2k + cw) * grid, its halo box goes to stage k % 2
+    auto load_halo = [&](int tile, int st) {
+      const int img = tile / per_img, rr = tile - img * per_img;
+      mbar_expect_tx(bar_full + 8 * (2 * cw + st), kTailHalo);
+      tma_load_4d(cons + (uint32_t)st * kTailStage, &p.map_x, bar_full + 8 * (2 * cw + st), 0,
+                  (rr % p.tiles_x) * kStepX - 1, (rr / p.tiles_x) * kStepY - 1, img);
+    };
+    if (r == 0)
+      for (int k = 0; k < 2; ++k)
+        if ((int)blockIdx.x + (2 * k + cw) * grid < p.num_tiles) load_halo((int)blockIdx.x + (2 * k + cw) * grid, k);
     int stage = 0;
     uint32_t phase = 0;
+    float acc[64];
     mbar_wait_mma(bar_w, 0);
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    for (int tile = blockIdx.x + cw * grid; tile < p.num_tiles; tile += 2 * grid) {
       const int img = tile / per_img, rr = tile - img * per_img;
       const int y0 = (rr / p.tiles_x) * kStepY - 1, x0 = (rr % p.tiles_x) * kStepX - 1;
-      mbar_wait_mma(bar_full + 8 * stage, phase);
-      const uint32_t sa16 = gmma_addr16(base + kTailOffStage + (uint32_t)stage * kTailStage);
-      // 1. transposed conv, one parity accumulator at a time -> +bias, ReLU, fp16 -> HR operand block a
-      {
-        float acc[2][32];
-#pragma unroll 1
-        for (int a = 0; a < 4; ++a) {
+      // the frame this tile adds onto is loaded into the output registers now; the loads complete under the MMAs
+      bool ok[4];
+      float o[4][3];
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
+      for (int j = 0; j < 4; ++j) {
+        const int Y = Y0 + 8 * j, gy = 2 * y0 + Y, gx = 2 * x0 + X;
+        ok[j] = Y >= 1 && Y <= 30 && X >= 1 && X <= 14 && gy >= 0 && gy < H && gx >= 0 && gx < W;
 #pragma unroll
-            for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
-          wgmma_fence();
-          halo_mmas<TG_CONVT_3X3_S2>(acc, sa16, wt16, a);
-          wgmma_commit();
-          wgmma_wait<0>();
-          if (a == 3) {
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_empty + 8 * stage);
-          }
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-              const int row = h * 64 + q * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
-              const int col = 8 * (i >> 2) + 2 * (lane & 3);
-              const int iy = y0 + (row >> 3), ix = x0 + (row & 7);
-              const bool in = iy >= 0 && iy < p.h && ix >= 0 && ix < p.w;
-              const float v0 = in ? tg_act(acc[h][i] + bup_s[col], TG_ACT_RELU) : 0.f;
-              const float v1 = in ? tg_act(acc[h][i + 1] + bup_s[col + 1], TG_ACT_RELU) : 0.f;
-              *reinterpret_cast<__half2*>(hr_p + a * kHrBlock + row * 128 + ((((col >> 3) ^ (row & 7))) << 4) +
-                                          (col & 7) * 2) = __floats2half2_rn(v0, v1);
-            }
+        for (int co = 0; co < 3; ++co) {
+          o[j][co] = 0.f;
+          if (p.accumulate && ok[j] && co < p.cout_real)
+            o[j][co] = p.y[(((size_t)img * p.cout_real + co) * H + gy) * W + gx];
         }
       }
+      const int s = stage;
+      mbar_wait_mma(bar_full + 8 * (2 * cw + s), phase);
       if (++stage == 2) { stage = 0; phase ^= 1u; }
-      fence_proxy_async_smem();     // generic-proxy writes -> read by wgmma (async proxy)
-      named_bar_sync(1, 128);
-      // 2. conv_out as tap-major N (N = 48) on each parity block; the tap products replace the block
+      const uint32_t x16 = gmma_addr16(cons + (uint32_t)s * kTailStage);
+      wgmma_fence();
+      convT_pxn_mmas(acc, x16, wt16, 0);
+      wgmma_commit();
+      // parity a = (py, px) of the HR pixels: transposed conv -> operand block -> conv_out tap products ->
+      // summed into the output pixels they land on; parity a + 1's transposed conv runs under the summation
 #pragma unroll 1
-      for (int blk = 0; blk < 4; ++blk) {
+      for (int a = 0; a < 4; ++a) {
+        wgmma_wait<0>();
+        // +bias, ReLU, zero for input pixels outside the image (conv_out's zero padding), fp16 -> the block
+#pragma unroll
+        for (int jp = 0; jp < 8; ++jp) {
+          uint32_t ov[4];
+#pragma unroll
+          for (int m = 0; m < 4; ++m) {
+            const int i = 4 * (2 * jp + (m >> 1)) + 2 * (m & 1);
+            const int iy = y0 + 2 * jp + (m >> 1), ix = x0 + 2 * (lane & 3);
+            const bool rin = iy >= 0 && iy < p.h;
+            const float bb = (m & 1) ? b1 : b0;
+            const float v0 = rin && ix >= 0 && ix < p.w ? tg_act(acc[i] + bb, TG_ACT_RELU) : 0.f;
+            const float v1 = rin && ix + 1 >= 0 && ix + 1 < p.w ? tg_act(acc[i + 1] + bb, TG_ACT_RELU) : 0.f;
+            const __half2 hv = __floats2half2_rn(v0, v1);
+            ov[m] = *reinterpret_cast<const uint32_t*>(&hv);
+          }
+          stmatrix_x4_trans(blk + (uint32_t)jp * 2048u + mat_off, ov);
+        }
+        fence_proxy_async_smem();      // generic-proxy writes -> read by wgmma (async proxy)
+        named_bar_sync(bar_id, 128);
+        // every warp is past its wait for the last transposed-conv MMAs: the halo stage takes the tile after next
+        if (a == 3 && r == 0 && tile + 4 * grid < p.num_tiles) load_halo(tile + 4 * grid, s);
+        // conv_out as tap-major N (N = 48 = 9 taps x 4 couts) on the block
         float d2[2][24];
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int i = 0; i < 24; ++i) d2[h][i] = 0.f;
-        const uint32_t a16 = gmma_addr16(hr + blk * kHrBlock);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          wgmma_n48(d2[0], b_hi | (uint64_t)(a16 + 2u * k), b_hi | (uint64_t)(wo16 + 2u * k), k > 0 ? 1u : 0u);
-          wgmma_n48(d2[1], b_hi | (uint64_t)(a16 + 512u + 2u * k), b_hi | (uint64_t)(wo16 + 2u * k), k > 0 ? 1u : 0u);
+          wgmma_n48(d2[0], k_hi | (uint64_t)(blk16 + 2u * k), k_hi | (uint64_t)(wo16 + 2u * k), k > 0 ? 1u : 0u);
+          wgmma_n48(d2[1], k_hi | (uint64_t)(blk16 + 512u + 2u * k), k_hi | (uint64_t)(wo16 + 2u * k), k > 0 ? 1u : 0u);
         }
         wgmma_commit();
         wgmma_wait<0>();
-        named_bar_sync(1, 128);      // every warp is done reading the block
-        float* D2 = reinterpret_cast<float*>(hr_p + blk * kHrBlock);
+        // every thread has read the previous parity's tap products before the barrier above, and the block is
+        // rewritten only after the barrier below
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -438,39 +481,57 @@ __global__ void __launch_bounds__(kTailThreads, 1) convT_convout_kernel(const __
             const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);   // = tap * 4 + co
             if (col < 36 && (col & 3) < 3) D2[row * kD2Pitch + (col >> 2) * 3 + (col & 3)] = d2[h][i];
           }
+        if (a < 3) {
+          wgmma_fence();
+          convT_pxn_mmas(acc, x16, wt16, a + 1);
+          wgmma_commit();
+        }
+        named_bar_sync(bar_id, 128);
+        // HR pixel (Y, X) takes tap (ty, tx) from HR pixel (Y + ty - 1, X + tx - 1); that pixel has parity a for
+        // ty = ty0, ty0 + 2 (< 3) and tx = tx0, tx0 + 2 (< 3).  Straight-line code, so that parity a + 1's MMAs
+        // stay in flight: every slot is loaded (the padding around D2 keeps the reads of unused slots and of the
+        // ring pixels inside shared memory) and unused slots are dropped by a select.
+        const int ty0 = 1 - ((a >> 1) ^ (Y0 & 1)), tx0 = 1 - ((a & 1) ^ (X & 1));
+#pragma unroll
+        for (int sl = 0; sl < 4; ++sl) {
+            const int ty = ty0 + 2 * (sl >> 1), tx = tx0 + 2 * (sl & 1);
+            const bool use = ty <= 2 && tx <= 2;
+            const float* d = D2 + (((Y0 + ty - 1) >> 1) * 8 + ((X + tx - 1) >> 1)) * kD2Pitch + (ty * 3 + tx) * 3;
+#pragma unroll
+            for (int j = 0; j < 4; ++j)        // HR row Y0 + 8j = block row ((Y0 + ty - 1) >> 1) + 4j
+#pragma unroll
+              for (int co = 0; co < 3; ++co) {
+                const float v = d[j * 32 * kD2Pitch + co];
+                o[j][co] += use ? v : 0.f;
+              }
+          }
       }
-      named_bar_sync(1, 128);
-      // 3. shift-add over the 32x16 HR pixels of the tile: interior 30x14 are outputs
+      // + bias (+ upsample_func(lr)) -> fp32 NCHW (+ uint8 NHWC).  One pixel per iteration (the selects keep o in
+      // registers): the in-kernel upsample is inlined three times rather than twelve.
 #pragma unroll 1
       for (int j = 0; j < 4; ++j) {
-        const int P = r + 128 * j, Y = P >> 4, X = P & 15;
-        const int gy = 2 * y0 + Y, gx = 2 * x0 + X;
+        float oj[3];
+#pragma unroll
+        for (int co = 0; co < 3; ++co) oj[co] = j == 0 ? o[0][co] : j == 1 ? o[1][co] : j == 2 ? o[2][co] : o[3][co];
+        const int Y = Y0 + 8 * j, gy = 2 * y0 + Y, gx = 2 * x0 + X;
         if (Y < 1 || Y > 30 || X < 1 || X > 14 || gy < 0 || gy >= H || gx < 0 || gx >= W) continue;
-        float o[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-        for (int tap = 0; tap < 9; ++tap) {
-          const int Yn = Y + tap / 3 - 1, Xn = X + tap % 3 - 1;
-          const float* D2 = reinterpret_cast<const float*>(hr_p + ((Yn & 1) * 2 + (Xn & 1)) * kHrBlock) +
-                            ((Yn >> 1) * 8 + (Xn >> 1)) * kD2Pitch + tap * 3;
-#pragma unroll
-          for (int co = 0; co < 3; ++co) o[co] += D2[co];
-        }
         uint32_t q8[3] = {0u, 0u, 0u};
-        for (int co = 0; co < p.cout_real; ++co) {
-          float* yp = p.y + (((size_t)img * p.cout_real + co) * H + gy) * W + gx;
-          float v = o[co] + bout_s[co];
-          if (p.accumulate) v = *yp + v;
-          else if (p.lr) v = v + tg_upsample_at(p.lr + ((size_t)img * p.cout_real + co) * lh * lw, lh, lw, lh, lw,
-                                                p.lr_scale, p.up_mode, gy, gx);
-          *yp = v;
+#pragma unroll
+        for (int co = 0; co < 3; ++co) {
+          if (co >= p.cout_real) continue;
+          float v = oj[co] + bout_s[co];
+          if (p.lr) v = v + tg_upsample_at(p.lr + ((size_t)img * p.cout_real + co) * lh * lw, lh, lw, lh, lw,
+                                           p.lr_scale, p.up_mode, gy, gx);
+          p.y[(((size_t)img * p.cout_real + co) * H + gy) * W + gx] = v;
           q8[co] = (uint32_t)fminf(fmaxf(rintf(v * 255.f), 0.f), 255.f);
         }
         if (p.y_u8) {
           uint8_t* up = p.y_u8 + (((size_t)img * H + gy) * W + gx) * p.cout_real;
-          for (int co = 0; co < p.cout_real; ++co) up[co] = (uint8_t)q8[co];
+#pragma unroll
+          for (int co = 0; co < 3; ++co)
+            if (co < p.cout_real) up[co] = (uint8_t)q8[co];
         }
       }
-      named_bar_sync(1, 128);        // the HR blocks are rewritten by the next tile
     }
   }
 }
