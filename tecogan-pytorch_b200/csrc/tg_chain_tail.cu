@@ -101,36 +101,6 @@ __device__ __forceinline__ void halo_mmas(float (&acc)[2][32], uint32_t sa16, ui
   }
 }
 
-// transposed-conv taps of parity accumulator `a` (1/2/2/4 groups) of one 16x8 tile, pixels on N:
-//   acc[64 cout][128 px] (+)= W[group] (A: the packed [cout][64] tile, K-major, SBO 1024)
-//                             x the group's shifted view of the 17x9 halo box (B: K-major, 16 core groups of
-//                             8 pixels, SBO = one box row of 9 x 128 B, origin 0, start += (dy*9+dx)*128 B)
-// one m64n128k16 per (group, k-step).  The first MMA of the parity overwrites acc (scale-d = 0).
-template <int A>
-__device__ __forceinline__ void convT_pxn_parity(float (&acc)[64], uint32_t x16, uint32_t w16) {
-  constexpr uint32_t kBoxW = TW + 1;
-  const uint64_t w_hi = gmma_desc_hi(1024u), x_hi = gmma_desc_hi(kBoxW * 128u);
-#pragma unroll
-  for (int g = 0; g < 9; ++g) {
-    const TgGroup gr = tg_group(TG_CONVT_3X3_S2, g);
-    if (gr.acc != A) continue;
-    const bool first = g == 0 || tg_group(TG_CONVT_3X3_S2, g > 0 ? g - 1 : 0).acc != gr.acc;
-    const uint32_t a16 = w16 + (uint32_t)g * (kWtBytes / 9 / 16);
-    const uint32_t b16 = x16 + (uint32_t)(gr.dy * (int)kBoxW + gr.dx) * 8u;
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-      wgmma_n128(acc, w_hi | (uint64_t)(a16 + 2u * k), x_hi | (uint64_t)(b16 + 2u * k), (first && k == 0) ? 0u : 1u);
-  }
-}
-__device__ __forceinline__ void convT_pxn_mmas(float (&acc)[64], uint32_t x16, uint32_t w16, int a) {
-  switch (a) {
-    case 0: convT_pxn_parity<0>(acc, x16, w16); break;
-    case 1: convT_pxn_parity<1>(acc, x16, w16); break;
-    case 2: convT_pxn_parity<2>(acc, x16, w16); break;
-    default: convT_pxn_parity<3>(acc, x16, w16); break;
-  }
-}
-
 // ================================================================== conv chain
 constexpr int kChainThreads = 384;                   // producer warpgroup + 2 consumer warpgroups
 constexpr uint32_t kChainHalo = (TW + 2) * (TH + 2) * 128;           // 23040

@@ -19,17 +19,19 @@
 //             staged to a per-consumer fp32 smem tile -> one thread per pixel applies bias / act /
 //             residual (or the derivative, pool, pixel-shuffle and thin-head epilogues) and writes
 //             the pixel's 128-byte NHWC row.  One consumer's epilogue overlaps the other's MMAs.
-//             The transposed conv keeps 4 parity accumulators (1/2/2/4 taps), computed and stored
-//             one after the other; each stores its pixel's output of that parity (pixel shuffle).
+//             The tap-mode transposed conv keeps 4 parity accumulators (1/2/2/4 taps), computed and
+//             stored one after the other; each stores its pixel's output of that parity (pixel shuffle).
 //
-// The forward 3x3 halo conv with NHWC output (the SRNet body and the FNet halo layers; see
-// consumer_halo_pxn) swaps the GEMM's roles: M = the 64 output channels (the packed weight tile is the
-// K-major A operand), N = the tile's 128 pixels (the halo view is the K-major B operand, 16 core groups
-// of 8 pixels), so each (tap, k-step) is ONE m64n128k16 that reads 6 KB of smem instead of two
-// m64n64k16 that read 8 KB.  Its epilogue works from registers: bias / act / residual -> fp16 ->
-// stmatrix into a 16 KB tile in the TMA box image -> one TMA tensor store per tile; the residual
-// arrives in that tile by one TMA load issued before the tile's MMAs.  Without the fp32 staging tiles
-// each consumer's ring holds two halo stages instead of one.
+// The forward halo conv and transposed conv with NHWC output (the SRNet body, the first SRNet
+// transposed conv and the FNet halo layers, pooled or not; see consumer_halo_pxn / consumer_convT_pxn)
+// swap the GEMM's roles: M = the 64 output channels (the packed weight tile is the K-major A operand),
+// N = the tile's 128 pixels (the halo view is the K-major B operand, 16 core groups of 8 pixels), so
+// each (tap, k-step) is ONE m64n128k16 that reads 6 KB of smem instead of two m64n64k16 that read 8 KB.
+// The epilogue works from registers: bias / act / residual -> fp16 -> stmatrix into a 16 KB tile in the
+// TMA box image -> one TMA tensor store per tile (per parity for the transposed conv, into a 5-D view
+// of its output); the residual arrives in that tile by one TMA load issued before the tile's MMAs.  With
+// the pool, the 2x2 max is taken in registers and a 4 KB pooled tile is stored.  Without the fp32
+// staging tiles each consumer's ring holds two halo stages or more.
 #include <cuda.h>
 
 #include <cstdlib>
@@ -46,6 +48,7 @@ constexpr int kThreads = 384;             // producer warpgroup + 2 consumer war
 constexpr int kMaxRing = 4;               // smem stages per consumer ring
 constexpr uint32_t kHeaderBytes = 2048;   // barriers (first 1 KB) + bias (second 1 KB)
 constexpr uint32_t kTapABytes = TH * TW * 128;  // 16 KB
+constexpr uint32_t kPoolTileBytes = kTapABytes / 4;   // the pooled 8x4 px x 64 ch output tile
 constexpr uint32_t kSmemLimit = 232448;   // 227 KB opt-in limit per CTA
 // A-operand modes (template parameter MODE)
 constexpr int MODE_TAP = 0;    // one 16x8 box per (tap, chunk)
@@ -74,11 +77,11 @@ struct KParams {
   uint32_t off_b, off_stage, off_scratch;   // off_scratch: the consumers' fp32 staging or fp16 output tiles
 };
 
-// The forward 3x3 halo conv with NHWC output puts the roles of the GEMM the other way round:
-// D[cout][pixel] = W . X^T, the 64 output channels on M and the tile's 128 pixels on N.
-template <int KIND, int MODE, bool BWD, bool POOL>
+// The forward halo conv / transposed conv with NHWC output (pooled or not) puts the roles of the GEMM the
+// other way round: D[cout][pixel] = W . X^T, the 64 output channels on M and the tile's 128 pixels on N.
+template <int KIND, int MODE, bool BWD>
 __host__ __device__ constexpr bool pixels_on_n() {
-  return KIND == TG_CONV_3X3 && MODE == MODE_HALO && !BWD && !POOL;
+  return (KIND == TG_CONV_3X3 || KIND == TG_CONVT_3X3_S2) && MODE == MODE_HALO && !BWD;
 }
 
 struct TileCoord { int n, y0, x0, nb; };
@@ -209,6 +212,10 @@ __device__ __forceinline__ void epilogue_nhwc(const KParams& p, const TileCoord&
 // that one TMA tensor store writes out (clipped at the image edge).  The residual, if any, is TMA-loaded
 // into the same tile before the tile's MMAs and overwritten in place.  Thread t of the warpgroup holds
 // rows (couts) 16*(t/32) + (t%32)/4 + {0, 8} and pixel columns 8*j + 2*(t%4) + {0, 1}, j = 0..15.
+// POOL (MaxPool2d(2, 2) folded in): the 2x2 block (tile rows 2i, 2i+1; columns 2*(t%4), +1) of a cout lies in
+// four registers of one thread, so the pooled 8x4 px x 64 ch tile (4 KB) is formed without shuffles and
+// stored through the pooled tensor's map; clipping at that map's edge is the floor pooling.
+template <bool POOL>
 __device__ __forceinline__ void consumer_halo_pxn(const TgMaps& maps, const KParams& p, uint32_t base,
                                                   const float* bias_s, int cw) {
   const tg_conv_desc& d = p.d;
@@ -217,16 +224,19 @@ __device__ __forceinline__ void consumer_halo_pxn(const TgMaps& maps, const KPar
   const uint32_t bar_full = base + 8u * (cw * kMaxRing), bar_empty = base + 16 * kMaxRing + 8u * (cw * kMaxRing);
   const uint32_t bar_res = base + 32 * kMaxRing + 8 + 8u * cw;
   const uint32_t stage0 = base + p.off_stage + (uint32_t)(cw * p.ring) * p.stage_bytes;
-  const uint32_t out_s = base + p.off_scratch + (uint32_t)cw * kTapABytes;
+  const uint32_t out_s = base + p.off_scratch + (uint32_t)cw * (POOL ? kPoolTileBytes : kTapABytes);
   constexpr uint32_t kBoxW = TW + 2;
   const uint64_t w_hi = gmma_desc_hi(1024u), x_hi = gmma_desc_hi(kBoxW * 128u);
   const uint32_t w16 = gmma_addr16(base + p.off_b), btb16 = p.b_stage_bytes >> 4;
-  const bool has_res = d.residual != nullptr;
+  const bool has_res = !POOL && d.residual != nullptr;
   const int bar_id = 1 + cw;
   // stmatrix / ldmatrix: lane l addresses pixel row l%8 of 8x8 matrix m = l/8 = (tile row 2*jp + m/2,
-  // 8-channel chunk 2*q + m%2); the swizzled offset of (pixel px, chunk) is px*128 + ((chunk ^ px%8) << 4)
-  const uint32_t mat_off = (uint32_t)(8 * ((lane >> 3) >> 1) + (lane & 7)) * 128u +
-                           ((uint32_t)((2 * q + ((lane >> 3) & 1)) ^ (lane & 7)) << 4);
+  // 8-channel chunk 2*q + m%2); the swizzled offset of (pixel px, chunk) is px*128 + ((chunk ^ px%8) << 4).
+  // POOL: matrix m = (pooled row pair 2*ip + m/2, chunk 2*q + m%2), its column 2*c + e = pooled pixel
+  // (row 2*(2*ip + m/2) + e, column c), i.e. lane l addresses tile pixel 8*(m/2) + kk, kk = 4*(l%2) + (l%8)/2.
+  const uint32_t kk = POOL ? 4u * (lane & 1) + ((lane & 7) >> 1) : (uint32_t)(lane & 7);
+  const uint32_t mat_off = (uint32_t)(8 * ((lane >> 3) >> 1) + kk) * 128u +
+                           ((uint32_t)((2 * q + ((lane >> 3) & 1)) ^ kk) << 4);
   int stage = 0;
   uint32_t phase = 0, rphase = 0;
   float acc[64];
@@ -273,29 +283,55 @@ __device__ __forceinline__ void consumer_halo_pxn(const TgMaps& maps, const KPar
     if (has_res) { mbar_wait_mma(bar_res, rphase); rphase ^= 1u; }
     else named_bar_sync(bar_id, 128);
     const float b0 = bias_s[tc.nb * 64 + 16 * q + (lane >> 2)], b1 = bias_s[tc.nb * 64 + 16 * q + (lane >> 2) + 8];
+    if (POOL) {
 #pragma unroll
-    for (int jp = 0; jp < 8; ++jp) {
-      const uint32_t addr = out_s + (uint32_t)jp * 2048u + mat_off;
-      uint32_t rv[4], ov[4];
-      if (has_res) ldmatrix_x4_trans(addr, rv);
+      for (int ip = 0; ip < 2; ++ip) {
+        uint32_t ov[4];
 #pragma unroll
-      for (int m = 0; m < 4; ++m) {
-        const int i = 4 * (2 * jp + (m >> 1)) + 2 * (m & 1);
-        const float bb = (m & 1) ? b1 : b0;
-        float a0 = tg_epi_val(acc[i], bb, d.act), a1 = tg_epi_val(acc[i + 1], bb, d.act);
-        if (has_res) {
-          const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(&rv[m]));
-          a0 += rf.x; a1 += rf.y;
+        for (int m = 0; m < 4; ++m) {
+          const float bb = (m & 1) ? b1 : b0;
+          __half v[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            // pooled row pr = tile rows 2*pr, 2*pr + 1; the same fp16 values the unpooled epilogue stores
+            const int pr = 2 * (2 * ip + (m >> 1)) + e;
+            const int i0 = 4 * (2 * pr) + 2 * (m & 1), i1 = i0 + 4;
+            const __half2 r0 = __floats2half2_rn(tg_epi_val(acc[i0], bb, d.act), tg_epi_val(acc[i0 + 1], bb, d.act));
+            const __half2 r1 = __floats2half2_rn(tg_epi_val(acc[i1], bb, d.act), tg_epi_val(acc[i1 + 1], bb, d.act));
+            const __half2 mx = __hmax2(r0, r1);
+            v[e] = __hmax(__low2half(mx), __high2half(mx));
+          }
+          const __half2 o = __halves2half2(v[0], v[1]);
+          ov[m] = *reinterpret_cast<const uint32_t*>(&o);
         }
-        const __half2 o = __floats2half2_rn(a0, a1);
-        ov[m] = *reinterpret_cast<const uint32_t*>(&o);
+        stmatrix_x4_trans(out_s + (uint32_t)ip * 2048u + mat_off, ov);
       }
-      stmatrix_x4_trans(addr, ov);
+    } else {
+#pragma unroll
+      for (int jp = 0; jp < 8; ++jp) {
+        const uint32_t addr = out_s + (uint32_t)jp * 2048u + mat_off;
+        uint32_t rv[4], ov[4];
+        if (has_res) ldmatrix_x4_trans(addr, rv);
+#pragma unroll
+        for (int m = 0; m < 4; ++m) {
+          const int i = 4 * (2 * jp + (m >> 1)) + 2 * (m & 1);
+          const float bb = (m & 1) ? b1 : b0;
+          float a0 = tg_epi_val(acc[i], bb, d.act), a1 = tg_epi_val(acc[i + 1], bb, d.act);
+          if (has_res) {
+            const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(&rv[m]));
+            a0 += rf.x; a1 += rf.y;
+          }
+          const __half2 o = __floats2half2_rn(a0, a1);
+          ov[m] = *reinterpret_cast<const uint32_t*>(&o);
+        }
+        stmatrix_x4_trans(addr, ov);
+      }
     }
     fence_proxy_async_smem();
     named_bar_sync(bar_id, 128);
     if (r == 0) {
-      tma_store_4d(&maps.m[2], out_s, tc.nb * 64, tc.x0, tc.y0, tc.n);
+      if (POOL) tma_store_4d(&maps.m[2], out_s, tc.nb * 64, tc.x0 >> 1, tc.y0 >> 1, tc.n);
+      else tma_store_4d(&maps.m[2], out_s, tc.nb * 64, tc.x0, tc.y0, tc.n);
       bulk_commit_group();
     }
   }
@@ -304,11 +340,74 @@ __device__ __forceinline__ void consumer_halo_pxn(const TgMaps& maps, const KPar
   if (r == 0) bulk_wait_group0();
 }
 
+// One consumer warpgroup of the forward stride-2 transposed conv (17x9 halo box, origin 0), pixels on N: for
+// each of its tiles and each output parity a = (py, px), acc[64 cout][128 px] = convT_pxn_mmas(a), then
+// bias / act -> fp16 -> stmatrix into one of the consumer's two 16 KB output tiles -> one TMA store of the
+// parity's 16x8 output pixels (2*(y0+ty) + py, 2*(x0+tx) + px) through the 5-D output map (maps.m[2]).  The
+// tiles alternate by parity, so parity a's store drains while parity a + 1 is computed.
+__device__ __forceinline__ void consumer_convT_pxn(const TgMaps& maps, const KParams& p, uint32_t base,
+                                                   const float* bias_s, int cw) {
+  const tg_conv_desc& d = p.d;
+  const int r = threadIdx.x - 128 * (1 + cw);
+  const int q = r >> 5, lane = threadIdx.x & 31;
+  const uint32_t bar_full = base + 8u * (cw * kMaxRing), bar_empty = base + 16 * kMaxRing + 8u * (cw * kMaxRing);
+  const uint32_t stage0 = base + p.off_stage + (uint32_t)(cw * p.ring) * p.stage_bytes;
+  const uint32_t out0 = base + p.off_scratch + (uint32_t)cw * 2u * kTapABytes;
+  const uint32_t w16 = gmma_addr16(base + p.off_b);
+  const int bar_id = 1 + cw;
+  // as in consumer_halo_pxn: lane l addresses pixel row l%8 of matrix l/8 = (tile row 2*jp + m/2, chunk 2*q + m%2)
+  const uint32_t mat_off = (uint32_t)(8 * ((lane >> 3) >> 1) + (lane & 7)) * 128u +
+                           ((uint32_t)((2 * q + ((lane >> 3) & 1)) ^ (lane & 7)) << 4);
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[64];
+
+  for (int tile = blockIdx.x + cw * (int)gridDim.x; tile < p.num_tiles; tile += 2 * (int)gridDim.x) {
+    const TileCoord tc = tile_coord(p, tile);
+    const float b0 = bias_s[tc.nb * 64 + 16 * q + (lane >> 2)], b1 = bias_s[tc.nb * 64 + 16 * q + (lane >> 2) + 8];
+    const int s = stage;
+    mbar_wait_mma(bar_full + 8 * s, phase);
+    if (++stage == p.ring) { stage = 0; phase ^= 1u; }
+    const uint32_t x16 = gmma_addr16(stage0 + (uint32_t)s * p.stage_bytes);
+#pragma unroll 1
+    for (int a = 0; a < 4; ++a) {
+      wgmma_fence();
+      convT_pxn_mmas(acc, x16, w16, a);
+      wgmma_commit();
+      // the output tile of this parity was last read by the store before the previous one
+      if (r == 0) bulk_wait_group_read1();
+      named_bar_sync(bar_id, 128);
+      wgmma_wait<0>();
+      if (a == 3) { __syncwarp(); if (lane == 0) mbar_arrive(bar_empty + 8 * s); }
+      const uint32_t out_s = out0 + (uint32_t)(a & 1) * kTapABytes;
+#pragma unroll
+      for (int jp = 0; jp < 8; ++jp) {
+        uint32_t ov[4];
+#pragma unroll
+        for (int m = 0; m < 4; ++m) {
+          const int i = 4 * (2 * jp + (m >> 1)) + 2 * (m & 1);
+          const float bb = (m & 1) ? b1 : b0;
+          const __half2 o = __floats2half2_rn(tg_epi_val(acc[i], bb, d.act), tg_epi_val(acc[i + 1], bb, d.act));
+          ov[m] = *reinterpret_cast<const uint32_t*>(&o);
+        }
+        stmatrix_x4_trans(out_s + (uint32_t)jp * 2048u + mat_off, ov);
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(bar_id, 128);
+      if (r == 0) {
+        tma_store_5d(&maps.m[2], out_s, (a & 1) * d.cout + tc.nb * 64, tc.x0, a >> 1, tc.y0, tc.n);
+        bulk_commit_group();
+      }
+    }
+  }
+  if (r == 0) bulk_wait_group0();
+}
+
 // ------------------------------------------------------------------ the kernel
 // BWD = data-gradient instantiation: epilogue y = (acc + bias [+ residual]) * act'(mask)  (TG_ACT_DRELU /
 // TG_ACT_DLRELU02; TG_ACT_NONE = no derivative).
-// POOL = TG_EPI_NHWC_F16_POOL2 instantiation: 2x2 max over the tile's pixels by warp shuffles, one store
-// per 2x2 block.
+// POOL = TG_EPI_NHWC_F16_POOL2 instantiation: 2x2 max over the tile's pixels (tap mode: by warp shuffles,
+// one store per 2x2 block; halo mode: in registers, one TMA store of the pooled tile).
 template <int KIND, int MODE, bool BWD = false, bool POOL = false>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
@@ -329,7 +428,7 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
   const uint32_t bar_res = bar_b + 8;                      // [2] residual tile of consumer c
   float* bias_s = reinterpret_cast<float*>(sm + 1024);
   static_assert(!(KIND == TG_CONV_3X3_S2 && MODE != MODE_TAP), "the stride-2 conv runs in tap mode only");
-  constexpr bool kPxN = pixels_on_n<KIND, MODE, BWD, POOL>();
+  constexpr bool kPxN = pixels_on_n<KIND, MODE, BWD>();
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&maps.m[0]);
@@ -404,7 +503,8 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
     // ============================================================ consumers, pixels on N
     if (warp >= 4) {
       if (p.b_resident) mbar_wait_mma(bar_b, 0);
-      consumer_halo_pxn(maps, p, base, bias_s, (warp - 4) >> 2);
+      if constexpr (KIND == TG_CONVT_3X3_S2) consumer_convT_pxn(maps, p, base, bias_s, (warp - 4) >> 2);
+      else consumer_halo_pxn<POOL>(maps, p, base, bias_s, (warp - 4) >> 2);
     }
   } else if (warp >= 4) {
     // ============================================================ consumers
@@ -508,34 +608,6 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
           }
         }
         named_bar_sync(bar_id, 128);
-      } else if (MODE == MODE_HALO && KIND == TG_CONVT_3X3_S2) {
-        // one halo stage (chunks == 1), four parity accumulators one after the other
-        const int s = next_stage();
-        const uint32_t sa16 = gmma_addr16(stage_addr(s));
-#pragma unroll 1
-        for (int a = 0; a < 4; ++a) {
-          if (a > 0) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-#pragma unroll
-              for (int i = 0; i < NF; ++i) acc[h][i] = 0.f;
-          }
-          wgmma_fence();
-#pragma unroll
-          for (int g = 0; g < 9; ++g) {
-            const TgGroup gr = tg_group(KIND, g);
-            if (gr.acc != a) continue;
-            const bool first = g == 0 || tg_group(KIND, g > 0 ? g - 1 : 0).acc != gr.acc;
-            mma_group(sa16 + (uint32_t)((gr.dy - kOrg) * kBoxW + (gr.dx - kOrg)) * 8u, smem_b16 + (uint32_t)g * btb16, first);
-          }
-          wgmma_commit();
-          wgmma_wait<0>();
-          if (a == 3) release(s);
-          stash();
-          named_bar_sync(bar_id, 128);
-          epilogue_nhwc<KIND, BWD, POOL>(p, tc, r, lane, a, S, bias_s);
-          named_bar_sync(bar_id, 128);
-        }
       } else if (MODE == MODE_HALO) {
         for (int c = 0; c < p.chunks; ++c) {
           const int s = next_stage();
@@ -616,22 +688,43 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// NHWC fp16 tensor [n][h][w][c] with explicit element strides for w/h/n (parity views)
-int encode_nhwc(CUtensorMap* m, const void* ptr, int c, int w, int h, int n, size_t sw, size_t sh,
-                size_t sn, int box_c, int box_w, int box_h) {
+// fp16 tensor of `rank` dims (dims[0] contiguous), element strides of dims 1.., 128B swizzle
+int encode_f16(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const size_t* elem_strides,
+               const cuuint32_t* box) {
   EncodeTiledFn fn = get_encode_fn();
   TG_REQUIRE(fn != nullptr, TG_E_DRIVER, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
-  cuuint64_t strides[3] = {(cuuint64_t)sw * 2, (cuuint64_t)sh * 2, (cuuint64_t)sn * 2};
-  cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), dims, strides, box,
+  cuuint64_t strides[4];
+  for (int i = 0; i + 1 < rank; ++i) strides[i] = (cuuint64_t)elem_strides[i] * 2;
+  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides, box,
                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   TG_REQUIRE(r == CUDA_SUCCESS, TG_E_DRIVER,
-             "cuTensorMapEncodeTiled failed (%d) c=%d w=%d h=%d n=%d box=%dx%dx%d", (int)r, c, w, h, n,
-             box_c, box_w, box_h);
+             "cuTensorMapEncodeTiled failed (%d) rank=%d dims=%llux%llux%llux%llu box=%ux%ux%u", (int)r, rank,
+             (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2],
+             (unsigned long long)dims[3], box[0], box[1], box[2]);
   return TG_OK;
+}
+
+// NHWC fp16 tensor [n][h][w][c] with explicit element strides for w/h/n (parity views)
+int encode_nhwc(CUtensorMap* m, const void* ptr, int c, int w, int h, int n, size_t sw, size_t sh,
+                size_t sn, int box_c, int box_w, int box_h) {
+  const cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
+  const size_t strides[3] = {sw, sh, sn};
+  const cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+  return encode_f16(m, ptr, 4, dims, strides, box);
+}
+
+// Output [n][2h][2w][c] of the transposed conv with input size h x w, as the 5-D tensor (2c, w, 2, h, n):
+// element (px*c + ch, x, py, y, n) is output pixel (2y + py, 2x + px).  Parity (py, px) of the 16x8 input
+// pixels at (y0, x0) is the box (64, 8, 1, 16, 1) at (px*c + nb*64, x0, py, y0, n); it clips at the right and
+// bottom image edges, and never crosses into the next image.
+int encode_convT_out(CUtensorMap* m, const void* ptr, int c, int w, int h, int n) {
+  const size_t C = (size_t)c, W = (size_t)w;
+  const cuuint64_t dims[5] = {2 * (cuuint64_t)c, (cuuint64_t)w, 2, (cuuint64_t)h, (cuuint64_t)n};
+  const size_t strides[4] = {2 * C, 2 * W * C, 4 * W * C, 4 * (size_t)h * W * C};
+  const cuuint32_t box[5] = {64, TW, 1, TH, 1};
+  return encode_f16(m, ptr, 5, dims, strides, box);
 }
 
 template <int K, int M, bool B, bool P>
@@ -752,11 +845,13 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
     p.a_bytes = kTapABytes;
     p.stage_bytes = kTapABytes + (p.b_resident ? 0u : p.b_stage_bytes);
   }
-  // the consumers' epilogue tiles: fp16 output / residual tiles (16 KB each) on the pixels-on-N path,
+  // the consumers' epilogue tiles on the pixels-on-N path: one fp16 output / residual tile (16 KB) each, two
+  // per consumer for the transposed conv (alternating parities), one 4 KB pooled tile each with the pool;
   // fp32 accumulator staging otherwise
   const bool bwd = d->act >= TG_ACT_DRELU || d->kind == TG_CONV_3X3_S2;
-  const bool pxn = p.halo && d->kind == TG_CONV_3X3 && !bwd && !pool && !tapn;
-  const uint32_t epi_tiles = pxn ? 2u * kTapABytes : scratch;
+  const bool convT = d->kind == TG_CONVT_3X3_S2;
+  const bool pxn = p.halo && !bwd && !tapn;
+  const uint32_t epi_tiles = !pxn ? scratch : convT ? 4u * kTapABytes : pool ? 2u * kPoolTileBytes : 2u * kTapABytes;
   const uint32_t avail = kSmemLimit - 1024u - kHeaderBytes - epi_tiles - (p.b_resident ? b_total : 0u);
   int ring = (int)(avail / p.stage_bytes) / 2;
   if (ring > kMaxRing) ring = kMaxRing;
@@ -775,9 +870,18 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
                      (size_t)d->h * d->w * d->cin, 64, p.box_w, p.box_h);
     if (rc != TG_OK) return rc;
     map_a.m[1] = map_a.m[2] = map_a.m[3] = map_a.m[0];
-    if (pxn) {
+    const size_t C = (size_t)d->cout;
+    if (pxn && convT) {
+      rc = encode_convT_out(&map_a.m[2], d->y, d->cout, d->w, d->h, d->n);
+      if (rc != TG_OK) return rc;
+    } else if (pxn && pool) {
+      // [2] = the pooled output [n][h/2][w/2][cout], one 8x4 px x 64 ch box per tile and N slice
+      const int pw = d->w / 2, ph = d->h / 2;
+      rc = encode_nhwc(&map_a.m[2], d->y, d->cout, pw, ph, d->n, C, (size_t)pw * C, (size_t)ph * pw * C, 64,
+                       TW / 2, TH / 2);
+      if (rc != TG_OK) return rc;
+    } else if (pxn) {
       // [1] = residual, [2] = output: NHWC [n][h][w][cout], one 16x8 px x 64 ch box per tile and N slice
-      const size_t C = (size_t)d->cout;
       if (d->residual) {
         TG_REQUIRE(((uintptr_t)d->residual & 15) == 0, TG_E_INVALID, "conv: residual must be 16-byte aligned");
         rc = encode_nhwc(&map_a.m[1], d->residual, d->cout, d->w, d->h, d->n, C, (size_t)d->w * C,

@@ -78,10 +78,20 @@ __device__ __forceinline__ void tma_store_4d(const void* map, uint32_t src, int 
       ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+__device__ __forceinline__ void tma_store_5d(const void* map, uint32_t src, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
+      ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+      : "memory");
+}
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // the issuing thread's bulk stores have finished READING shared memory (the source may be reused)
 __device__ __forceinline__ void bulk_wait_group_read0() {
   asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+}
+// all but the most recent of the issuing thread's bulk store groups have finished reading shared memory
+__device__ __forceinline__ void bulk_wait_group_read1() {
+  asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
 }
 // the issuing thread's bulk stores are complete (their writes are done)
 __device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
@@ -177,6 +187,36 @@ __device__ __forceinline__ void wgmma_k16(float (&d)[NF], uint64_t da, uint64_t 
   static_assert(NF == 32 || NF == 24, "N = 64 or 48");
   if constexpr (NF == 32) wgmma_n64(d, da, db, scale_d);
   else wgmma_n48(d, da, db, scale_d);
+}
+
+// transposed-conv taps of parity accumulator `a` (1/2/2/4 groups) of one 16x8 tile, pixels on N:
+//   acc[64 cout][128 px] (+)= W[group] (A: the packed [cout][64] tile, K-major, SBO 1024, 8 KB per group)
+//                             x the group's shifted view of the 17x9 halo box (B: K-major, 16 core groups of
+//                             8 pixels, SBO = one box row of 9 x 128 B, origin 0, start += (dy*9+dx)*128 B)
+// one m64n128k16 per (group, k-step).  The first MMA of the parity overwrites acc (scale-d = 0).
+template <int A>
+__device__ __forceinline__ void convT_pxn_parity(float (&acc)[64], uint32_t x16, uint32_t w16) {
+  constexpr uint32_t kBoxW = 9;
+  const uint64_t w_hi = gmma_desc_hi(1024u), x_hi = gmma_desc_hi(kBoxW * 128u);
+#pragma unroll
+  for (int g = 0; g < 9; ++g) {
+    const TgGroup gr = tg_group(TG_CONVT_3X3_S2, g);
+    if (gr.acc != A) continue;
+    const bool first = g == 0 || tg_group(TG_CONVT_3X3_S2, g > 0 ? g - 1 : 0).acc != gr.acc;
+    const uint32_t a16 = w16 + (uint32_t)g * (64u * 128u / 16u);
+    const uint32_t b16 = x16 + (uint32_t)(gr.dy * (int)kBoxW + gr.dx) * 8u;
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      wgmma_n128(acc, w_hi | (uint64_t)(a16 + 2u * k), x_hi | (uint64_t)(b16 + 2u * k), (first && k == 0) ? 0u : 1u);
+  }
+}
+__device__ __forceinline__ void convT_pxn_mmas(float (&acc)[64], uint32_t x16, uint32_t w16, int a) {
+  switch (a) {
+    case 0: convT_pxn_parity<0>(acc, x16, w16); break;
+    case 1: convT_pxn_parity<1>(acc, x16, w16); break;
+    case 2: convT_pxn_parity<2>(acc, x16, w16); break;
+    default: convT_pxn_parity<3>(acc, x16, w16); break;
+  }
 }
 
 }  // namespace
