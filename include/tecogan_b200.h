@@ -249,6 +249,18 @@ int tg_nhwc_f16_to_nchw_f32(const void* x, float* y, int n, int c, int h, int w,
  * x NCHW fp32 [n,c,h,w] -> uint8 [n,h,w,c], round-half-even, clip [0,255] */
 int tg_float_to_uint8_nhwc(const float* x, uint8_t* y, int n, int c, int h, int w, void* stream);
 
+/* Frame input of one streamed step (codes/data/paired_folder_dataset.py:49, tecogan_nets.py:269-276).
+ * in_u8 : uint8 [n,h,w,c] HWC frames, or NULL (lr_curr was filled by the caller)
+ *         -> lr_curr fp32 NCHW [n,c,h,w] = float(v) / 255 (IEEE division, == numpy float32 / 255.0);
+ *            bgr != 0 reverses the channel order (cv2's BGR -> the reference's RGB)
+ * reset : int32 [n] in device memory, or NULL; slot k with reset[k] != 0 starts a new video:
+ *         lr_prev[k] and hr_prev[k] (fp32, [c,h,w] / [c,s*h,s*w]) are zeroed, as the reference's
+ *         infer_sequence does for frame 0 (tecogan_nets.py:269-270); other slots are not touched
+ * lr_curr, lr_prev and hr_prev must be non-NULL and 4-byte aligned; c <= 4; s in {2,4}.  The mask is read
+ * on the device, so one captured launch serves every pattern of resets. */
+int tg_stream_frame_in(const uint8_t* in_u8, const int32_t* reset, float* lr_curr, float* lr_prev,
+                       float* hr_prev, int n, int c, int h, int w, int s, int bgr, void* stream);
+
 /* BD degradation of the data side (codes/utils/data_utils.py:30-53, called on GT frames by
  * base_model.py:75,115): optional reflect pad by (k-1)/2 | k-1-(k-1)/2, then a depthwise valid
  * correlation with the k x k kernel `k2d` (device, fp32, = create_kernel(sigma)[0,0]) and stride s.

@@ -210,3 +210,233 @@ def infer_clips(net, lr_data, device):
         src = src.pin_memory()           # pageable input: one staging copy (pass pinned to avoid)
     out = eng.run_clips(src)
     return out.numpy().transpose(1, 0, 2, 3, 4)
+
+
+class StreamEngine(ClipEngine):
+    """ClipEngine's static buffers, streams and per-parity step graphs, with the recurrent state (lr[p^1],
+    hr[p^1], the parity) kept between calls of `run`, for video that arrives in chunks.  Like ClipEngine it holds
+    its net weakly; VideoStream (FRNet.stream) holds the strong reference.
+
+    Each graph starts with tg_stream_frame_in: it decodes the uint8 HWC frames of inp[p] into lr[p] (fp32 input:
+    the caller copied lr[p], the kernel only resets) and zeroes lr[p^1][k] / hr[p^1][k] of the slots flagged in
+    the device mask mask[p] -- the reset of one slot happens inside the captured step, and one graph serves every
+    pattern of resets.  The step itself is the unchanged net.step_into.
+
+    Copies overlap compute as in ClipEngine.run_clips.  uint8 input: inp[p] is itself the 2-deep staging ring (the
+    step of parity p^1 never reads it), so the H2D of frame i+1 lands directly in the graph's input while frame i
+    runs.  fp32 input: lr[p] is still read as lr_prev by frame i, so frames are staged as in run_clips."""
+
+    def __init__(self, net, n, c, h, w, device, u8_input=True, bgr=False):
+        dev = torch.device(device)
+        self.u8_input, self.bgr = u8_input, bgr
+        self.mask = [torch.zeros(n, dtype=torch.int32, device=dev) for _ in range(2)]
+        self.inp = [torch.zeros(n, h, w, c, dtype=torch.uint8, device=dev) for _ in range(2)] if u8_input else None
+        self.sig = _param_signature(net)
+        self.parity = 0                  # parity of the next frame
+        self.mask_set = [False, False]   # mask[p] holds a reset pattern (cleared before the next replay)
+        self.in_free = [None, None]      # event: the replay that last read inp[p] / stage[p] finished
+        self.out_copied = [None, None]   # event: the D2H of u8[p] finished
+        super().__init__(net, n, c, h, w, dev)     # lr / hr / u8, streams, the two graphs of _enqueue below
+
+    def close(self):
+        super().close()
+        self.mask, self.inp = [], None
+
+    def _enqueue(self, p):
+        ops.stream_frame_in(self.inp[p] if self.u8_input else None, self.mask[p], self.lr[p], self.lr[p ^ 1],
+                            self.hr[p ^ 1], self.net.scale, self.bgr)
+        super()._enqueue(p)
+
+    def _set_mask(self, p, slots):
+        """On the main stream, before the replay of parity p: mask[p] = 1 for `slots`, 0 elsewhere."""
+        if slots:
+            self.mask[p].zero_()
+            for k in slots:
+                self.mask[p][k].fill_(1)
+            self.mask_set[p] = True
+        elif self.mask_set[p]:
+            self.mask[p].zero_()
+            self.mask_set[p] = False
+
+    def run(self, frames, reset_slots, out_host):
+        """frames: uint8 [n,k,h,w,c] (u8_input) or fp32 [n,k,c,h,w], each frame contiguous, pinned host or on this
+        device.
+        Slots in `reset_slots` start a new video at frame 0.  Returns uint8 [n,k,H,W,c]: a pinned host tensor
+        (out_host; one synchronisation, at the end) or a new tensor on the device, ordered on the current
+        stream (no synchronisation)."""
+        n, k = self.n, frames.shape[1]
+        with torch.cuda.device(self.device):
+            cur = torch.cuda.current_stream()
+            self.net.refresh_packed_weights()        # a load_state_dict between pushes takes effect
+            for st in (self.main, self.h2d, self.d2h):
+                st.wait_stream(cur)
+            shape = (n, k, self.H, self.W, self.c)
+            if out_host:
+                out = torch.empty(shape, dtype=torch.uint8, pin_memory=True)
+            else:
+                out = torch.empty(shape, dtype=torch.uint8, device=self.device)
+            if not self.u8_input and self.stage is None:
+                self.stage = [torch.empty_like(self.lr[0]) for _ in range(2)]
+            dst = self.inp if self.u8_input else self.stage
+            for i in range(k):
+                p = self.parity
+                with torch.cuda.stream(self.h2d):
+                    if self.in_free[p] is not None:
+                        self.h2d.wait_event(self.in_free[p])
+                    for j in range(n):
+                        dst[p][j].copy_(frames[j, i], non_blocking=True)
+                    staged = torch.cuda.Event()
+                    staged.record(self.h2d)
+                with torch.cuda.stream(self.main):
+                    self.main.wait_event(staged)
+                    if not self.u8_input:
+                        self.lr[p].copy_(self.stage[p], non_blocking=True)
+                    self._set_mask(p, reset_slots if i == 0 else None)
+                    if out_host and self.out_copied[p] is not None:
+                        self.main.wait_event(self.out_copied[p])     # u8[p] free to overwrite
+                    self.run_frame(p)
+                    done = torch.cuda.Event()
+                    done.record(self.main)
+                    self.in_free[p] = done
+                    if not out_host:
+                        out[:, i].copy_(self.u8[p], non_blocking=True)
+                if out_host:
+                    with torch.cuda.stream(self.d2h):
+                        self.d2h.wait_event(done)
+                        for j in range(n):
+                            out[j, i].copy_(self.u8[p][j], non_blocking=True)
+                        self.out_copied[p] = torch.cuda.Event()
+                        self.out_copied[p].record(self.d2h)
+                self.parity ^= 1
+            if out_host:
+                self.d2h.synchronize()   # after every replay (D2H waited on each) and so after every H2D
+            else:
+                cur.wait_stream(self.main)
+                cur.wait_stream(self.h2d)    # a device input may be freed once the call returns
+        return out
+
+
+class VideoStream:
+    """n lock-stepped video slots through FRNet with the recurrent state carried between `push` calls.
+    Created by FRNet.stream(); see there."""
+
+    def __init__(self, net, n, h, w, device=None, input='uint8', channel_order='rgb'):
+        if input not in ('uint8', 'float32'):
+            raise ValueError(f"input must be 'uint8' or 'float32', got {input!r}")
+        if channel_order not in ('rgb', 'bgr'):
+            raise ValueError(f"channel_order must be 'rgb' or 'bgr', got {channel_order!r}")
+        if input == 'float32' and channel_order != 'rgb':
+            raise ValueError("channel_order='bgr' applies to uint8 input only")
+        if not all(isinstance(v, int) and v > 0 for v in (n, h, w)):
+            raise ValueError(f'n, h, w must be positive ints, got {(n, h, w)}')
+        device = torch.device('cuda') if device is None else torch.device(device)
+        if device.type != 'cuda':
+            raise ops.L.TecoganB200Error('tecogan-b200 runs on CUDA devices only (no CPU path)')
+        self.net, self.n, self.h, self.w = net, n, h, w
+        self.c = net.fnet.in_nc
+        self.device, self.input, self.channel_order = device, input, channel_order
+        self._engine = None                  # built (graphs captured) by the first push
+        self._pending = [True] * n           # a new stream starts every slot from zero state
+        _check_inference(net)
+
+    def reset(self, slots):
+        """Mark `slots` (indices) to start a new video at the first frame of the next push."""
+        for k in slots:
+            if not 0 <= int(k) < self.n:
+                raise IndexError(f'slot {k} out of range for a stream of {self.n} slots')
+            self._pending[int(k)] = True
+
+    def close(self):
+        """Free the CUDA graphs and the device buffers; the stream cannot be pushed to afterwards."""
+        if self._engine:
+            self._engine.close()
+        self._engine = False
+
+    def push(self, frames, reset=None, out='host'):
+        """Run the next k frames of every slot.
+
+        frames: uint8 [n,k,h,w,c] (input='uint8'; [k,h,w,c] when n == 1) or fp32 [n,k,c,h,w] (input='float32';
+                [k,c,h,w] when n == 1), each frame contiguous (a slice [:, i:i+k] of a clip is fine), as a torch
+                tensor on the host (pinned or pageable) or on the stream's device, or a NumPy array.  Nothing is
+                converted: another dtype, layout or size raises.
+        reset:  n bools; slot k starts a new video at the first frame of this push (its recurrent state is zeroed,
+                as for frame 0 of FRNet.infer_sequence).
+        out:    'host' -> NumPy uint8 [n,k,H,W,c] (one synchronisation); 'device' -> a new CUDA uint8 tensor
+                [n,k,H,W,c], ordered on the current stream (no synchronisation; a pinned host input must then
+                stay unchanged until that stream has passed this push).
+        """
+        if self._engine is False:
+            raise ops.L.TecoganB200Error('VideoStream.push: the stream is closed')
+        if out not in ('host', 'device'):
+            raise ValueError(f"out must be 'host' or 'device', got {out!r}")
+        frames = self._check_frames(frames)
+        slots = list(self._pending)
+        if reset is not None:
+            reset = list(reset)
+            if len(reset) != self.n:
+                raise ValueError(f'reset has {len(reset)} entries, the stream has {self.n} slots')
+            slots = [a or bool(b) for a, b in zip(slots, reset)]
+        _check_inference(self.net)
+        if self._engine is None:
+            self._engine = self._build()
+        elif _param_signature(self.net) != self._engine.sig:
+            raise ops.L.TecoganB200Error('VideoStream.push: the net\'s parameters moved since the stream was '
+                                         'built (net.to(...)?); open a new stream')
+        if not frames.is_cuda and not frames.is_pinned():
+            # pageable input: one staging copy of exactly this chunk (pass pinned memory to avoid it)
+            frames = torch.empty(frames.shape, dtype=frames.dtype, pin_memory=True).copy_(frames)
+        res = self._engine.run(frames, [k for k in range(self.n) if slots[k]], out == 'host')
+        self._pending = [False] * self.n
+        return res.numpy() if out == 'host' else res
+
+    def _check_frames(self, frames):
+        L = ops.L
+        if isinstance(frames, np.ndarray):
+            if any(st < 0 for st in frames.strides):
+                raise L.TecoganB200Error('VideoStream.push: each frame must be contiguous; got negative strides '
+                                         '(cv2 [..., ::-1]: use channel_order="bgr" or np.ascontiguousarray)')
+            frames = torch.from_numpy(frames)
+        if not isinstance(frames, torch.Tensor):
+            raise TypeError(f'VideoStream.push: frames must be a tensor or ndarray, got {type(frames).__name__}')
+        u8 = self.input == 'uint8'
+        dtype = torch.uint8 if u8 else torch.float32
+        if frames.dtype != dtype:
+            raise L.TecoganB200Error(f'VideoStream.push: {self.input} stream expects {dtype} frames, got '
+                                     f'{frames.dtype}')
+        if frames.dim() == 4 and self.n == 1:
+            frames = frames.unsqueeze(0)
+        frame = (self.h, self.w, self.c) if u8 else (self.c, self.h, self.w)
+        if frames.dim() != 5 or frames.shape[0] != self.n or frames.shape[1] < 1 or tuple(frames.shape[2:]) != frame:
+            layout = 'n,k,h,w,c' if u8 else 'n,k,c,h,w'
+            raise L.TecoganB200Error(f'VideoStream.push: frames {tuple(frames.shape)} do not match [{layout}] '
+                                     f'with n={self.n}, {"x".join(map(str, frame))} per frame')
+        if not frames[0, 0].is_contiguous():      # frames are copied one at a time: [n,k] may be a slice
+            raise L.TecoganB200Error('VideoStream.push: each frame must be contiguous')
+        if frames.is_cuda and frames.device != self._resolved_device():
+            raise L.TecoganB200Error(f'VideoStream.push: frames on {frames.device}, the stream runs on '
+                                     f'{self._resolved_device()}')
+        if frames.requires_grad:
+            raise L.TecoganB200Error('VideoStream.push: frames require grad (no backward exists for a stream)')
+        return frames
+
+    def _resolved_device(self):
+        d = self.device
+        return d if d.index is not None else torch.device('cuda', torch.cuda.current_device())
+
+    def _build(self):
+        if not torch.cuda.is_available():
+            raise ops.L.TecoganB200Error('VideoStream: no CUDA device available (no CPU path)')
+        dev = self._resolved_device()
+        pdev = next(self.net.parameters()).device
+        if pdev != dev:
+            raise ops.L.TecoganB200Error(f'VideoStream: the net\'s parameters are on {pdev}, the stream runs on '
+                                         f'{dev}; move the net first (net.to(device))')
+        self.device = dev
+        return StreamEngine(self.net, self.n, self.c, self.h, self.w, dev, u8_input=self.input == 'uint8',
+                            bgr=self.channel_order == 'bgr')
+
+
+def _check_inference(net):
+    if net.training and any(p.requires_grad for p in net.parameters()):
+        raise ops.L.TecoganB200Error('FRNet.stream is inference only: call net.eval() (or set requires_grad=False '
+                                     'on the parameters) first')

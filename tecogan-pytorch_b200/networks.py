@@ -355,6 +355,21 @@ class FRNet(BaseSequenceGenerator):
             return infer_clips(self, lr_data.unsqueeze(0), device)[0]
         return infer_clips(self, lr_data, device)
 
+    def stream(self, n, h, w, device=None, input='uint8', channel_order='rgb'):
+        """A VideoStream of n lock-stepped slots of h x w LR frames: video pushed in chunks of any length, the
+        recurrent state carried from one push to the next, and a slot restarted (reset=) when its video ends and
+        the next one begins while the other slots keep running.
+
+        input='uint8': frames uint8 [n,k,h,w,c] as decoders and cv2.imread produce them, converted on the device
+        to float32 / 255 exactly as the reference's loader does (paired_folder_dataset.py:49); channel_order='bgr'
+        takes cv2's BGR order.  input='float32': frames fp32 [n,k,c,h,w] in [0,1], the reference layout.
+        push() returns uint8 [n,k,H,W,c] frames, byte-identical to infer_sequence over the concatenated pushes.
+        Temporal padding (pad_sequence, base_model.py:230-251) stays the caller's job: for p reflect-padded
+        frames, push frames[:, 1:1+p].flip(1) first and drop those p outputs.  The CUDA graphs are captured by the first push; the stream holds the
+        net."""
+        from .engine import VideoStream
+        return VideoStream(self, n, h, w, device, input, channel_order)
+
     def refresh_packed_weights(self, force=False):
         self.fnet._cache.refresh_all(force)
         self.srnet._cache.refresh_all(force)

@@ -411,6 +411,32 @@ def float_to_uint8_nhwc(x, y=None):
     return y
 
 
+def stream_frame_in(u8, reset, lr_curr, lr_prev, hr_prev, scale, bgr=False):
+    """Frame input of a streamed step (tg_stream_frame_in): u8 uint8 [n,h,w,c] (or None) -> lr_curr fp32
+    [n,c,h,w] = u8 / 255, channels reversed when bgr; slots k with reset[k] != 0 (int32 [n] on the device,
+    or None) get lr_prev[k] = hr_prev[k] = 0 ([n,c,h,w] / [n,c,scale*h,scale*w] fp32)."""
+    _req(lr_curr, torch.float32, 'lr_curr', 4)
+    _req(lr_prev, torch.float32, 'lr_prev', 4)
+    _req(hr_prev, torch.float32, 'hr_prev', 4)
+    n, c, h, w = lr_curr.shape
+    if tuple(lr_prev.shape) != (n, c, h, w) or tuple(hr_prev.shape) != (n, c, scale * h, scale * w):
+        raise L.TecoganB200Error('stream_frame_in: lr_prev / hr_prev shape mismatch')
+    if u8 is not None:
+        _req(u8, torch.uint8, 'frames', 4)
+        if tuple(u8.shape) != (n, h, w, c):
+            raise L.TecoganB200Error(f'stream_frame_in: frames {tuple(u8.shape)} != {(n, h, w, c)} (nhwc)')
+    if reset is not None:
+        _req(reset, torch.int32, 'reset', 1)
+        if reset.shape[0] != n:
+            raise L.TecoganB200Error(f'stream_frame_in: reset has {reset.shape[0]} entries, expected {n}')
+    for t in (lr_prev, hr_prev, u8, reset):
+        if t is not None and t.device != lr_curr.device:
+            raise L.TecoganB200Error('stream_frame_in: tensors on different devices')
+    L.check(L.load().tg_stream_frame_in(_ptr(u8), _ptr(reset), _ptr(lr_curr), _ptr(lr_prev), _ptr(hr_prev),
+                                        n, c, h, w, scale, int(bool(bgr)), _stream()), 'tg_stream_frame_in')
+    return lr_curr
+
+
 # ============================================================================ training (backward) ops
 class GradScale:
     """Device-resident loss scale {scale, 1/scale} of the fp16 gradient path (tg_grad_scale_from_amax /

@@ -1,0 +1,131 @@
+#!/usr/bin/env python
+"""HR frames/s of streamed inference (FRNet.stream) against FRNet.infer_sequence on bench.py's bd4 workload:
+4 lock-stepped clips of 3x134x320 LR (-> 3x536x1280), bench weights, --frames frames per clip.
+
+    python tools/stream_bench.py [--frames 64] [--reps 3]
+
+Prints one JSON line with, per path, the median and all --reps runs (HR frames/s = clips * frames / wall time;
+each run ends in a device synchronisation; one untimed warm-up run of every path first):
+  infer_sequence_fp32_host   FRNet.infer_sequence(pinned fp32 [n,t,c,h,w]) -> uint8 host
+  push_u8_host_chunk1/16     VideoStream.push(pinned uint8 [n,k,h,w,c], out='host'), k = 1 / 16
+  push_u8_device             VideoStream.push(uint8 on the device, out='device'), k = 16
+  frame_in_us                tg_stream_frame_in per step (decode of 4 frames, zero reset mask; and with every
+                             slot reset), CUDA events over a graph of launches on rotating buffers
+All paths process the same frames (uint8, and the reference loader's float32 / 255 of them), so their outputs are
+also compared byte for byte.  Card name and power limit are read in the same run.  Writes nothing."""
+import argparse
+import json
+import os
+import statistics
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def power_limit_w():
+    try:
+        r = subprocess.run(['nvidia-smi', '-i', '0', '--query-gpu=power.limit', '--format=csv,noheader,nounits'],
+                           capture_output=True, text=True, timeout=20)
+        return float(r.stdout.strip().splitlines()[0])
+    except Exception:
+        return None
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--frames', type=int, default=64)
+    ap.add_argument('--reps', type=int, default=3)
+    args = ap.parse_args()
+    if args.frames < 60:
+        ap.error('--frames must be >= 60')
+    import numpy as np
+    import torch
+    import bench
+    import tecogan_b200 as T
+    ops = sys.modules['tecogan-pytorch_b200.ops']
+    assert torch.cuda.is_available(), 'stream_bench.py needs a GPU'
+    dev = torch.device('cuda', 0)
+    torch.cuda.set_device(dev)
+    bench.select_workload('bd4')
+    n, (c, h, w), s = bench.CLIPS_PER_GPU, bench.LR, bench.SCALE
+    t = args.frames
+    net = T.FRNet(3, 3, 64, 10, 'BD', s)
+    net.load_state_dict(bench.make_params(), strict=True)
+    net = net.to(dev).eval()
+
+    clips = bench.synthetic_clips(n, t, seed=100).numpy()                            # [n,t,c,h,w] in [0,1]
+    u8 = np.ascontiguousarray(np.rint(clips * 255.0).astype(np.uint8).transpose(0, 1, 3, 4, 2))
+    f32 = torch.from_numpy(u8.astype(np.float32) / np.float32(255.0)).permute(0, 1, 4, 2, 3).contiguous()
+    f32_pin, u8_pin = f32.pin_memory(), torch.from_numpy(u8).pin_memory()
+    u8_dev = u8_pin.to(dev)
+
+    def timed(fn):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        out = fn()
+        torch.cuda.synchronize()
+        return n * t / (time.perf_counter() - t0), out
+
+    def pushes(stream, src, chunk, out):
+        return [stream.push(src[:, i:i + chunk], out=out) for i in range(0, t, chunk)]
+
+    streams = {'push_u8_host_chunk1': (1, u8_pin, 'host'), 'push_u8_host_chunk16': (16, u8_pin, 'host'),
+               'push_u8_device': (16, u8_dev, 'device')}
+    opened = {k: net.stream(n, h, w, device=dev) for k in streams}
+    runs = {k: [] for k in ['infer_sequence_fp32_host', *streams]}
+    outputs = {}
+    # rep 0 is the untimed warm-up: graph capture, and the caching host allocator's pinned output blocks (each
+    # path's previous output is dropped before its call, so later reps reuse them instead of pinning new memory)
+    for rep in range(args.reps + 1):                                                 # paths alternate per rep
+        outputs['infer_sequence_fp32_host'] = None
+        fps, outputs['infer_sequence_fp32_host'] = timed(lambda: net.infer_sequence(f32_pin, dev))
+        if rep:
+            runs['infer_sequence_fp32_host'].append(fps)
+        for k, (chunk, src, out) in streams.items():
+            opened[k].reset(range(n))
+            outputs[k] = None
+            fps, outputs[k] = timed(lambda: pushes(opened[k], src, chunk, out))
+            if rep:
+                runs[k].append(fps)
+    ref = outputs['infer_sequence_fp32_host']
+    identical = {}
+    for k, (chunk, src, out) in streams.items():
+        got = np.concatenate([o.cpu().numpy() if out == 'device' else o for o in outputs[k]], axis=1)
+        identical[k] = bool(np.array_equal(got, ref))
+    stream_launches = opened['push_u8_device']._engine.launches_per_step
+    for st in opened.values():
+        st.close()
+
+    # tg_stream_frame_in alone: 8 rotating buffer sets (8 x 4 x 2 MB of lr_curr), 60 launches per graph
+    nb, reps = 8, 60
+    H, W = s * h, s * w
+    ins = [torch.randint(0, 256, (n, h, w, c), dtype=torch.uint8, device=dev) for _ in range(nb)]
+    lrs = [torch.empty(n, c, h, w, device=dev) for _ in range(nb)]
+    prev = torch.empty(n, c, h, w, device=dev)
+    hrp = torch.empty(n, c, H, W, device=dev)
+    frame_in = {}
+    for name, val in (('decode', 0), ('decode_and_reset_all', 1)):
+        mask = torch.full((n,), val, dtype=torch.int32, device=dev)
+        sec = bench._time_graph(lambda i: ops.stream_frame_in(ins[i], mask, lrs[i], prev, hrp, s), nb, reps, torch)
+        frame_in[name] = sec * 1e6
+
+    line = {
+        'metric': 'hr_frames_per_sec_4xBD_3x134x320_streamed', 'unit': 'frames/s',
+        'device': torch.cuda.get_device_name(0), 'power_limit_w': power_limit_w(),
+        'clips': n, 'frames_per_clip': t, 'reps': args.reps,
+        'results': {k: {'median': statistics.median(v), 'runs': v} for k, v in runs.items()},
+        'identical_to_infer_sequence': identical,
+        'frame_in_us': frame_in,
+        'h2d_bytes_per_step': {'fp32': n * c * h * w * 4, 'uint8': n * c * h * w},
+        'd2h_bytes_per_step': n * c * H * W,
+        'launches_per_step': {'infer_sequence': T.engine.get_engine(net, n, c, h, w, dev).launches_per_step,
+                              'push': stream_launches},
+    }
+    print(json.dumps(line), flush=True)
+
+
+if __name__ == '__main__':
+    main()
