@@ -260,6 +260,18 @@ int tg_float_to_uint8_nhwc(const float* x, uint8_t* y, int n, int c, int h, int 
  * on the device, so one captured launch serves every pattern of resets. */
 int tg_stream_frame_in(const uint8_t* in_u8, const int32_t* reset, float* lr_curr, float* lr_prev,
                        float* hr_prev, int n, int c, int h, int w, int s, int bgr, void* stream);
+/* The same step input from YUV 4:2:0 frames, as video decoders produce them (BT.601 limited range).
+ * in    : uint8 [n, 3h/2, w], each frame the h x w Y plane followed by the interleaved (h/2) x w UV plane
+ *         (nv12 != 0) or by the (h/2) x (w/2) U and V planes (nv12 == 0: I420 / yuv420p), or NULL
+ *         -> lr_curr fp32 NCHW [n,3,h,w] = float(rgb) / 255 with rgb = cv2.cvtColor(frame, COLOR_YUV2RGB_NV12 /
+ *            COLOR_YUV2RGB_I420) bit for bit (20-bit fixed point, nearest chroma)
+ * reset : as above.  h and w must be even (TG_E_UNSUPPORTED otherwise). */
+int tg_stream_frame_in_yuv420(const uint8_t* in, int nv12, const int32_t* reset, float* lr_curr, float* lr_prev,
+                              float* hr_prev, int n, int h, int w, int s, void* stream);
+/* Encode of the streamed output: rgb uint8 NHWC [n,H,W,3] (the step's out_u8) -> out uint8 [n, 3H/2, W] in
+ * NV12 (nv12 != 0) or I420, the layouts above; == cv2.cvtColor(rgb, COLOR_RGB2YUV_I420) bit for bit (U and V
+ * of each 2x2 block from its top-left pixel), NV12 with the U and V planes interleaved.  H and W must be even. */
+int tg_rgb_u8_to_yuv420(const uint8_t* rgb, uint8_t* out, int nv12, int n, int H, int W, void* stream);
 
 /* BD degradation of the data side (codes/utils/data_utils.py:30-53, called on GT frames by
  * base_model.py:75,115): optional reflect pad by (k-1)/2 | k-1-(k-1)/2, then a depthwise valid

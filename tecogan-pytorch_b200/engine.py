@@ -222,30 +222,44 @@ class StreamEngine(ClipEngine):
     the device mask mask[p] -- the reset of one slot happens inside the captured step, and one graph serves every
     pattern of resets.  The step itself is the unchanged net.step_into.
 
+    YUV 4:2:0 input (yuv_in = 'nv12' / 'i420'): inp[p] holds [n,3h/2,w] frames and the first launch is
+    tg_stream_frame_in_yuv420 instead, with the same reset.  YUV output (yuv_out): each graph ends with
+    tg_rgb_u8_to_yuv420 of u8[p] into yuv[p] [n,3H/2,W], and the copies out read yuv[p] instead of u8[p].
+
     Copies overlap compute as in ClipEngine.run_clips.  uint8 input: inp[p] is itself the 2-deep staging ring (the
     step of parity p^1 never reads it), so the H2D of frame i+1 lands directly in the graph's input while frame i
     runs.  fp32 input: lr[p] is still read as lr_prev by frame i, so frames are staged as in run_clips."""
 
-    def __init__(self, net, n, c, h, w, device, u8_input=True, bgr=False):
+    def __init__(self, net, n, c, h, w, device, u8_input=True, bgr=False, yuv_in=None, yuv_out=None):
         dev = torch.device(device)
-        self.u8_input, self.bgr = u8_input, bgr
+        self.u8_input, self.bgr = u8_input or yuv_in is not None, bgr
+        self.yuv_in, self.yuv_out = yuv_in, yuv_out          # None, 'nv12' or 'i420'
         self.mask = [torch.zeros(n, dtype=torch.int32, device=dev) for _ in range(2)]
-        self.inp = [torch.zeros(n, h, w, c, dtype=torch.uint8, device=dev) for _ in range(2)] if u8_input else None
+        frame = (3 * h // 2, w) if yuv_in else (h, w, c)
+        self.inp = [torch.zeros(n, *frame, dtype=torch.uint8, device=dev) for _ in range(2)] if self.u8_input else None
+        H, W = net.scale * h, net.scale * w
+        self.yuv = [torch.empty(n, 3 * H // 2, W, dtype=torch.uint8, device=dev) for _ in range(2)] if yuv_out else None
         self.sig = _param_signature(net)
         self.parity = 0                  # parity of the next frame
         self.mask_set = [False, False]   # mask[p] holds a reset pattern (cleared before the next replay)
         self.in_free = [None, None]      # event: the replay that last read inp[p] / stage[p] finished
-        self.out_copied = [None, None]   # event: the D2H of u8[p] finished
+        self.out_copied = [None, None]   # event: the D2H of u8[p] (yuv[p]) finished
         super().__init__(net, n, c, h, w, dev)     # lr / hr / u8, streams, the two graphs of _enqueue below
 
     def close(self):
         super().close()
-        self.mask, self.inp = [], None
+        self.mask, self.inp, self.yuv = [], None, None
 
     def _enqueue(self, p):
-        ops.stream_frame_in(self.inp[p] if self.u8_input else None, self.mask[p], self.lr[p], self.lr[p ^ 1],
-                            self.hr[p ^ 1], self.net.scale, self.bgr)
+        if self.yuv_in:
+            ops.stream_frame_in_yuv420(self.inp[p], self.yuv_in, self.mask[p], self.lr[p], self.lr[p ^ 1],
+                                       self.hr[p ^ 1], self.net.scale)
+        else:
+            ops.stream_frame_in(self.inp[p] if self.u8_input else None, self.mask[p], self.lr[p], self.lr[p ^ 1],
+                                self.hr[p ^ 1], self.net.scale, self.bgr)
         super()._enqueue(p)
+        if self.yuv_out:
+            ops.rgb_u8_to_yuv420(self.u8[p], self.yuv_out, out=self.yuv[p])
 
     def _set_mask(self, p, slots):
         """On the main stream, before the replay of parity p: mask[p] = 1 for `slots`, 0 elsewhere."""
@@ -259,18 +273,19 @@ class StreamEngine(ClipEngine):
             self.mask_set[p] = False
 
     def run(self, frames, reset_slots, out_host):
-        """frames: uint8 [n,k,h,w,c] (u8_input) or fp32 [n,k,c,h,w], each frame contiguous, pinned host or on this
-        device.
-        Slots in `reset_slots` start a new video at frame 0.  Returns uint8 [n,k,H,W,c]: a pinned host tensor
-        (out_host; one synchronisation, at the end) or a new tensor on the device, ordered on the current
-        stream (no synchronisation)."""
+        """frames: uint8 [n,k,h,w,c] (u8_input), uint8 [n,k,3h/2,w] (yuv_in) or fp32 [n,k,c,h,w], each frame
+        contiguous, pinned host or on this device.
+        Slots in `reset_slots` start a new video at frame 0.  Returns uint8 [n,k,H,W,c] (or [n,k,3H/2,W] with
+        yuv_out): a pinned host tensor (out_host; one synchronisation, at the end) or a new tensor on the device,
+        ordered on the current stream (no synchronisation)."""
         n, k = self.n, frames.shape[1]
         with torch.cuda.device(self.device):
             cur = torch.cuda.current_stream()
             self.net.refresh_packed_weights()        # a load_state_dict between pushes takes effect
             for st in (self.main, self.h2d, self.d2h):
                 st.wait_stream(cur)
-            shape = (n, k, self.H, self.W, self.c)
+            res = self.yuv if self.yuv_out else self.u8      # what the step graph leaves for the copy out
+            shape = (n, k, *res[0].shape[1:])
             if out_host:
                 out = torch.empty(shape, dtype=torch.uint8, pin_memory=True)
             else:
@@ -293,18 +308,18 @@ class StreamEngine(ClipEngine):
                         self.lr[p].copy_(self.stage[p], non_blocking=True)
                     self._set_mask(p, reset_slots if i == 0 else None)
                     if out_host and self.out_copied[p] is not None:
-                        self.main.wait_event(self.out_copied[p])     # u8[p] free to overwrite
+                        self.main.wait_event(self.out_copied[p])     # res[p] free to overwrite
                     self.run_frame(p)
                     done = torch.cuda.Event()
                     done.record(self.main)
                     self.in_free[p] = done
                     if not out_host:
-                        out[:, i].copy_(self.u8[p], non_blocking=True)
+                        out[:, i].copy_(res[p], non_blocking=True)
                 if out_host:
                     with torch.cuda.stream(self.d2h):
                         self.d2h.wait_event(done)
                         for j in range(n):
-                            out[j, i].copy_(self.u8[p][j], non_blocking=True)
+                            out[j, i].copy_(res[p][j], non_blocking=True)
                         self.out_copied[p] = torch.cuda.Event()
                         self.out_copied[p].record(self.d2h)
                 self.parity ^= 1
@@ -316,25 +331,35 @@ class StreamEngine(ClipEngine):
         return out
 
 
+YUV420 = ops.YUV420_LAYOUTS       # 'nv12', 'i420'
+
+
 class VideoStream:
     """n lock-stepped video slots through FRNet with the recurrent state carried between `push` calls.
     Created by FRNet.stream(); see there."""
 
-    def __init__(self, net, n, h, w, device=None, input='uint8', channel_order='rgb'):
-        if input not in ('uint8', 'float32'):
-            raise ValueError(f"input must be 'uint8' or 'float32', got {input!r}")
+    def __init__(self, net, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb'):
+        if input not in ('uint8', 'float32', *YUV420):
+            raise ValueError(f"input must be 'uint8', 'float32', 'nv12' or 'i420', got {input!r}")
         if channel_order not in ('rgb', 'bgr'):
             raise ValueError(f"channel_order must be 'rgb' or 'bgr', got {channel_order!r}")
-        if input == 'float32' and channel_order != 'rgb':
-            raise ValueError("channel_order='bgr' applies to uint8 input only")
+        if out_format not in ('rgb', *YUV420):
+            raise ValueError(f"out_format must be 'rgb', 'nv12' or 'i420', got {out_format!r}")
+        if input != 'uint8' and channel_order != 'rgb':
+            raise ValueError(f"channel_order='bgr' applies to uint8 HWC input only, not input={input!r}")
         if not all(isinstance(v, int) and v > 0 for v in (n, h, w)):
             raise ValueError(f'n, h, w must be positive ints, got {(n, h, w)}')
+        yuv = [f for f in (input, out_format) if f in YUV420]
+        if yuv and (h % 2 or w % 2):
+            raise ValueError(f'{yuv[0]} frames are YUV 4:2:0: h and w must be even, got {h}x{w}')
+        if yuv and net.fnet.in_nc != 3:
+            raise ValueError(f'{yuv[0]} frames carry 3 colour channels, the net takes {net.fnet.in_nc}')
         device = torch.device('cuda') if device is None else torch.device(device)
         if device.type != 'cuda':
             raise ops.L.TecoganB200Error('tecogan-b200 runs on CUDA devices only (no CPU path)')
         self.net, self.n, self.h, self.w = net, n, h, w
         self.c = net.fnet.in_nc
-        self.device, self.input, self.channel_order = device, input, channel_order
+        self.device, self.input, self.channel_order, self.out_format = device, input, channel_order, out_format
         self._engine = None                  # built (graphs captured) by the first push
         self._pending = [True] * n           # a new stream starts every slot from zero state
         _check_inference(net)
@@ -355,15 +380,17 @@ class VideoStream:
     def push(self, frames, reset=None, out='host'):
         """Run the next k frames of every slot.
 
-        frames: uint8 [n,k,h,w,c] (input='uint8'; [k,h,w,c] when n == 1) or fp32 [n,k,c,h,w] (input='float32';
-                [k,c,h,w] when n == 1), each frame contiguous (a slice [:, i:i+k] of a clip is fine), as a torch
-                tensor on the host (pinned or pageable) or on the stream's device, or a NumPy array.  Nothing is
-                converted: another dtype, layout or size raises.
+        frames: uint8 [n,k,h,w,c] (input='uint8'; [k,h,w,c] when n == 1), uint8 [n,k,3h/2,w] (input='nv12' or
+                'i420'; [k,3h/2,w] when n == 1) or fp32 [n,k,c,h,w] (input='float32'; [k,c,h,w] when n == 1), each
+                frame contiguous (a slice [:, i:i+k] of a clip is fine), as a torch tensor on the host (pinned or
+                pageable) or on the stream's device, or a NumPy array.  Nothing is converted: another dtype,
+                layout or size raises.
         reset:  n bools; slot k starts a new video at the first frame of this push (its recurrent state is zeroed,
                 as for frame 0 of FRNet.infer_sequence).
         out:    'host' -> NumPy uint8 [n,k,H,W,c] (one synchronisation); 'device' -> a new CUDA uint8 tensor
                 [n,k,H,W,c], ordered on the current stream (no synchronisation; a pinned host input must then
-                stay unchanged until that stream has passed this push).
+                stay unchanged until that stream has passed this push).  With out_format 'nv12' / 'i420' the
+                frames are uint8 [n,k,3H/2,W] instead.
         """
         if self._engine is False:
             raise ops.L.TecoganB200Error('VideoStream.push: the stream is closed')
@@ -398,16 +425,17 @@ class VideoStream:
             frames = torch.from_numpy(frames)
         if not isinstance(frames, torch.Tensor):
             raise TypeError(f'VideoStream.push: frames must be a tensor or ndarray, got {type(frames).__name__}')
-        u8 = self.input == 'uint8'
-        dtype = torch.uint8 if u8 else torch.float32
+        dtype = torch.float32 if self.input == 'float32' else torch.uint8
         if frames.dtype != dtype:
             raise L.TecoganB200Error(f'VideoStream.push: {self.input} stream expects {dtype} frames, got '
                                      f'{frames.dtype}')
-        if frames.dim() == 4 and self.n == 1:
+        frame, layout = {'uint8': ((self.h, self.w, self.c), 'n,k,h,w,c'),
+                         'float32': ((self.c, self.h, self.w), 'n,k,c,h,w')}.get(
+                             self.input, ((3 * self.h // 2, self.w), 'n,k,3h/2,w'))
+        if frames.dim() == len(frame) + 1 and self.n == 1:
             frames = frames.unsqueeze(0)
-        frame = (self.h, self.w, self.c) if u8 else (self.c, self.h, self.w)
-        if frames.dim() != 5 or frames.shape[0] != self.n or frames.shape[1] < 1 or tuple(frames.shape[2:]) != frame:
-            layout = 'n,k,h,w,c' if u8 else 'n,k,c,h,w'
+        if (frames.dim() != len(frame) + 2 or frames.shape[0] != self.n or frames.shape[1] < 1
+                or tuple(frames.shape[2:]) != frame):
             raise L.TecoganB200Error(f'VideoStream.push: frames {tuple(frames.shape)} do not match [{layout}] '
                                      f'with n={self.n}, {"x".join(map(str, frame))} per frame')
         if not frames[0, 0].is_contiguous():      # frames are copied one at a time: [n,k] may be a slice
@@ -432,8 +460,10 @@ class VideoStream:
             raise ops.L.TecoganB200Error(f'VideoStream: the net\'s parameters are on {pdev}, the stream runs on '
                                          f'{dev}; move the net first (net.to(device))')
         self.device = dev
+        yuv_in = self.input if self.input in YUV420 else None
+        yuv_out = self.out_format if self.out_format in YUV420 else None
         return StreamEngine(self.net, self.n, self.c, self.h, self.w, dev, u8_input=self.input == 'uint8',
-                            bgr=self.channel_order == 'bgr')
+                            bgr=self.channel_order == 'bgr', yuv_in=yuv_in, yuv_out=yuv_out)
 
 
 def _check_inference(net):

@@ -93,6 +93,8 @@ _SIGNATURES = {
     'tg_nhwc_f16_to_nchw_f32': (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_float_to_uint8_nhwc': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     'tg_stream_frame_in': (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    'tg_stream_frame_in_yuv420': (c_int, [_P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
+    'tg_rgb_u8_to_yuv420': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     'tg_downsample_bd_nchw_f32': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_debug_set_conv_timers': (c_int, [_P]),
     # ---- training (generator backward)

@@ -355,7 +355,7 @@ class FRNet(BaseSequenceGenerator):
             return infer_clips(self, lr_data.unsqueeze(0), device)[0]
         return infer_clips(self, lr_data, device)
 
-    def stream(self, n, h, w, device=None, input='uint8', channel_order='rgb'):
+    def stream(self, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb'):
         """A VideoStream of n lock-stepped slots of h x w LR frames: video pushed in chunks of any length, the
         recurrent state carried from one push to the next, and a slot restarted (reset=) when its video ends and
         the next one begins while the other slots keep running.
@@ -364,11 +364,19 @@ class FRNet(BaseSequenceGenerator):
         to float32 / 255 exactly as the reference's loader does (paired_folder_dataset.py:49); channel_order='bgr'
         takes cv2's BGR order.  input='float32': frames fp32 [n,k,c,h,w] in [0,1], the reference layout.
         push() returns uint8 [n,k,H,W,c] frames, byte-identical to infer_sequence over the concatenated pushes.
+
+        YUV 4:2:0 video (BT.601 limited range, as ffmpeg's yuv420p / PyAV give it, NVDEC decodes and NVENC takes):
+        input='nv12' or 'i420' takes uint8 [n,k,3h/2,w] frames (the Y plane, then the interleaved UV plane or the U
+        and V planes) and converts them on the device exactly as cv2.cvtColor(frame, COLOR_YUV2RGB_NV12 / _I420)
+        followed by the loader's / 255.  out_format='nv12' or 'i420' returns uint8 [n,k,3H/2,W] frames:
+        cv2.cvtColor(rgb, COLOR_RGB2YUV_I420) of the RGB output (chroma of each 2x2 block from its top-left
+        pixel), for 'nv12' with U and V interleaved.  Both need even h and w; any input works with any
+        out_format.
         Temporal padding (pad_sequence, base_model.py:230-251) stays the caller's job: for p reflect-padded
         frames, push frames[:, 1:1+p].flip(1) first and drop those p outputs.  The CUDA graphs are captured by the first push; the stream holds the
         net."""
         from .engine import VideoStream
-        return VideoStream(self, n, h, w, device, input, channel_order)
+        return VideoStream(self, n, h, w, device, input, channel_order, out_format)
 
     def refresh_packed_weights(self, force=False):
         self.fnet._cache.refresh_all(force)

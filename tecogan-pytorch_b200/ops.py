@@ -437,6 +437,66 @@ def stream_frame_in(u8, reset, lr_curr, lr_prev, hr_prev, scale, bgr=False):
     return lr_curr
 
 
+YUV420_LAYOUTS = ('nv12', 'i420')
+
+
+def _yuv_layout(layout, name):
+    if layout not in YUV420_LAYOUTS:
+        raise L.TecoganB200Error(f'{name}: layout must be one of {YUV420_LAYOUTS}, got {layout!r}')
+    return int(layout == 'nv12')
+
+
+def stream_frame_in_yuv420(yuv, layout, reset, lr_curr, lr_prev, hr_prev, scale):
+    """stream_frame_in from YUV 4:2:0 frames (tg_stream_frame_in_yuv420): yuv uint8 [n,3h/2,w] in layout 'nv12' or
+    'i420' (or None) -> lr_curr fp32 [n,3,h,w] = cv2.cvtColor(frame, COLOR_YUV2RGB_<layout>) / 255; reset as in
+    stream_frame_in."""
+    nv12 = _yuv_layout(layout, 'stream_frame_in_yuv420')
+    _req(lr_curr, torch.float32, 'lr_curr', 4)
+    _req(lr_prev, torch.float32, 'lr_prev', 4)
+    _req(hr_prev, torch.float32, 'hr_prev', 4)
+    n, c, h, w = lr_curr.shape
+    if c != 3:
+        raise L.TecoganB200Error(f'stream_frame_in_yuv420: lr_curr has {c} channels, YUV frames decode to 3')
+    if tuple(lr_prev.shape) != (n, c, h, w) or tuple(hr_prev.shape) != (n, c, scale * h, scale * w):
+        raise L.TecoganB200Error('stream_frame_in_yuv420: lr_prev / hr_prev shape mismatch')
+    if yuv is not None:
+        _req(yuv, torch.uint8, 'frames', 3)
+        if tuple(yuv.shape) != (n, 3 * h // 2, w) or h % 2:
+            raise L.TecoganB200Error(f'stream_frame_in_yuv420: frames {tuple(yuv.shape)} != '
+                                     f'{(n, 3 * h // 2, w)} ([n,3h/2,w], h even)')
+    if reset is not None:
+        _req(reset, torch.int32, 'reset', 1)
+        if reset.shape[0] != n:
+            raise L.TecoganB200Error(f'stream_frame_in_yuv420: reset has {reset.shape[0]} entries, expected {n}')
+    for t in (lr_prev, hr_prev, yuv, reset):
+        if t is not None and t.device != lr_curr.device:
+            raise L.TecoganB200Error('stream_frame_in_yuv420: tensors on different devices')
+    L.check(L.load().tg_stream_frame_in_yuv420(_ptr(yuv), nv12, _ptr(reset), _ptr(lr_curr), _ptr(lr_prev),
+                                               _ptr(hr_prev), n, h, w, scale, _stream()), 'tg_stream_frame_in_yuv420')
+    return lr_curr
+
+
+def rgb_u8_to_yuv420(rgb, layout, out=None):
+    """tg_rgb_u8_to_yuv420: uint8 NHWC RGB [n,H,W,3] -> uint8 [n,3H/2,W] in layout 'nv12' or 'i420'
+    (== cv2.cvtColor(rgb, COLOR_RGB2YUV_I420), U and V interleaved for 'nv12')."""
+    nv12 = _yuv_layout(layout, 'rgb_u8_to_yuv420')
+    _req(rgb, torch.uint8, 'rgb', 4)
+    n, H, W, c = rgb.shape
+    if c != 3:
+        raise L.TecoganB200Error(f'rgb_u8_to_yuv420: expected [n,H,W,3] RGB, got {tuple(rgb.shape)}')
+    if H % 2 or W % 2:
+        raise L.TecoganB200Error(f'rgb_u8_to_yuv420: YUV 4:2:0 needs an even height and width, got {H}x{W}')
+    if out is None:
+        out = torch.empty((n, 3 * H // 2, W), dtype=torch.uint8, device=rgb.device)
+    _req(out, torch.uint8, 'out', 3)
+    if tuple(out.shape) != (n, 3 * H // 2, W):
+        raise L.TecoganB200Error(f'rgb_u8_to_yuv420: out {tuple(out.shape)} != {(n, 3 * H // 2, W)}')
+    if out.device != rgb.device:
+        raise L.TecoganB200Error('rgb_u8_to_yuv420: tensors on different devices')
+    L.check(L.load().tg_rgb_u8_to_yuv420(_ptr(rgb), _ptr(out), nv12, n, H, W, _stream()), 'tg_rgb_u8_to_yuv420')
+    return out
+
+
 # ============================================================================ training (backward) ops
 class GradScale:
     """Device-resident loss scale {scale, 1/scale} of the fp16 gradient path (tg_grad_scale_from_amax /

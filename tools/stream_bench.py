@@ -9,10 +9,17 @@ each run ends in a device synchronisation; one untimed warm-up run of every path
   infer_sequence_fp32_host   FRNet.infer_sequence(pinned fp32 [n,t,c,h,w]) -> uint8 host
   push_u8_host_chunk1/16     VideoStream.push(pinned uint8 [n,k,h,w,c], out='host'), k = 1 / 16
   push_u8_device             VideoStream.push(uint8 on the device, out='device'), k = 16
+  push_nv12_host_chunk1/16   VideoStream.push(pinned NV12 [n,k,3h/2,w], out='host') of an input='nv12',
+                             out_format='nv12' stream -> NV12 [n,k,3H/2,W], k = 1 / 16
+  push_nv12_device           the same with NV12 on the device and out='device', k = 16
   frame_in_us                tg_stream_frame_in per step (decode of 4 frames, zero reset mask; and with every
-                             slot reset), CUDA events over a graph of launches on rotating buffers
-All paths process the same frames (uint8, and the reference loader's float32 / 255 of them), so their outputs are
-also compared byte for byte.  Card name and power limit are read in the same run.  Writes nothing."""
+                             slot reset) and tg_stream_frame_in_yuv420 per step (NV12, I420), CUDA events over a
+                             graph of launches on rotating buffers
+  encode_us                  tg_rgb_u8_to_yuv420 per step (4 HR frames -> NV12 / I420), timed the same way
+All uint8 paths process the same frames (uint8, and the reference loader's float32 / 255 of them), so their
+outputs are also compared byte for byte.  The NV12 paths take oracle/yuv_oracle.py's NV12 of those frames; their
+output is compared with the oracle's NV12 of the RGB output for the frames that NV12 decodes to.  Card name and
+power limit are read in the same run.  Writes nothing."""
 import argparse
 import json
 import os
@@ -45,6 +52,7 @@ def main():
     import torch
     import bench
     import tecogan_b200 as T
+    from oracle import yuv_oracle as Y
     ops = sys.modules['tecogan-pytorch_b200.ops']
     assert torch.cuda.is_available(), 'stream_bench.py needs a GPU'
     dev = torch.device('cuda', 0)
@@ -61,6 +69,9 @@ def main():
     f32 = torch.from_numpy(u8.astype(np.float32) / np.float32(255.0)).permute(0, 1, 4, 2, 3).contiguous()
     f32_pin, u8_pin = f32.pin_memory(), torch.from_numpy(u8).pin_memory()
     u8_dev = u8_pin.to(dev)
+    nv12 = Y.rgb_to_yuv420(u8, 'nv12')                                                # [n,t,3h/2,w]
+    nv12_pin = torch.from_numpy(nv12).pin_memory()
+    nv12_dev = nv12_pin.to(dev)
 
     def timed(fn):
         torch.cuda.synchronize()
@@ -73,8 +84,10 @@ def main():
         return [stream.push(src[:, i:i + chunk], out=out) for i in range(0, t, chunk)]
 
     streams = {'push_u8_host_chunk1': (1, u8_pin, 'host'), 'push_u8_host_chunk16': (16, u8_pin, 'host'),
-               'push_u8_device': (16, u8_dev, 'device')}
-    opened = {k: net.stream(n, h, w, device=dev) for k in streams}
+               'push_u8_device': (16, u8_dev, 'device'), 'push_nv12_host_chunk1': (1, nv12_pin, 'host'),
+               'push_nv12_host_chunk16': (16, nv12_pin, 'host'), 'push_nv12_device': (16, nv12_dev, 'device')}
+    opened = {k: net.stream(n, h, w, device=dev, **(dict(input='nv12', out_format='nv12') if 'nv12' in k else {}))
+              for k in streams}
     runs = {k: [] for k in ['infer_sequence_fp32_host', *streams]}
     outputs = {}
     # rep 0 is the untimed warm-up: graph capture, and the caching host allocator's pinned output blocks (each
@@ -91,11 +104,20 @@ def main():
             if rep:
                 runs[k].append(fps)
     ref = outputs['infer_sequence_fp32_host']
+    # the NV12 paths' specification: the oracle's NV12 of the RGB output for the frames the NV12 input decodes to
+    rgb_in = Y.yuv420_to_rgb(nv12, 'nv12')
+    ref_rgb = net.infer_sequence(torch.from_numpy(rgb_in.astype(np.float32) / np.float32(255.0))
+                                 .permute(0, 1, 4, 2, 3).contiguous(), dev)
     identical = {}
     for k, (chunk, src, out) in streams.items():
         got = np.concatenate([o.cpu().numpy() if out == 'device' else o for o in outputs[k]], axis=1)
-        identical[k] = bool(np.array_equal(got, ref))
+        if 'nv12' in k:        # frame by frame: the oracle's int64 temporaries of a whole clip are GBs
+            identical[k] = got.shape == (n, t, 3 * s * h // 2, s * w) and all(
+                np.array_equal(got[j, i], Y.rgb_to_yuv420(ref_rgb[j, i], 'nv12')) for j in range(n) for i in range(t))
+        else:
+            identical[k] = bool(np.array_equal(got, ref))
     stream_launches = opened['push_u8_device']._engine.launches_per_step
+    nv12_launches = opened['push_nv12_device']._engine.launches_per_step
     for st in opened.values():
         st.close()
 
@@ -111,6 +133,19 @@ def main():
         mask = torch.full((n,), val, dtype=torch.int32, device=dev)
         sec = bench._time_graph(lambda i: ops.stream_frame_in(ins[i], mask, lrs[i], prev, hrp, s), nb, reps, torch)
         frame_in[name] = sec * 1e6
+    yuv_ins = [torch.randint(0, 256, (n, 3 * h // 2, w), dtype=torch.uint8, device=dev) for _ in range(nb)]
+    for layout in ('nv12', 'i420'):
+        sec = bench._time_graph(lambda i: ops.stream_frame_in_yuv420(yuv_ins[i], layout, None, lrs[i], prev, hrp, s),
+                                nb, reps, torch)
+        frame_in[f'decode_{layout}'] = sec * 1e6
+    # tg_rgb_u8_to_yuv420 alone: 8 rotating sets of 4 HR frames (8 x 8.2 MB in, 8 x 4.1 MB out)
+    rgbs = [torch.randint(0, 256, (n, H, W, c), dtype=torch.uint8, device=dev) for _ in range(nb)]
+    yuvs = [torch.empty(n, 3 * H // 2, W, dtype=torch.uint8, device=dev) for _ in range(nb)]
+    encode = {}
+    for layout in ('nv12', 'i420'):
+        sec = bench._time_graph(lambda i: ops.rgb_u8_to_yuv420(rgbs[i], layout, out=yuvs[i]), nb, reps, torch)
+        encode[layout] = sec * 1e6
+    encode_bytes = n * H * W * 3 + n * 3 * H // 2 * W
 
     line = {
         'metric': 'hr_frames_per_sec_4xBD_3x134x320_streamed', 'unit': 'frames/s',
@@ -119,10 +154,13 @@ def main():
         'results': {k: {'median': statistics.median(v), 'runs': v} for k, v in runs.items()},
         'identical_to_infer_sequence': identical,
         'frame_in_us': frame_in,
-        'h2d_bytes_per_step': {'fp32': n * c * h * w * 4, 'uint8': n * c * h * w},
-        'd2h_bytes_per_step': n * c * H * W,
+        'encode_us': encode,
+        'encode_bytes_per_step': encode_bytes,
+        'encode_gb_per_s': {k: encode_bytes / v * 1e-3 for k, v in encode.items()},
+        'h2d_bytes_per_step': {'fp32': n * c * h * w * 4, 'uint8': n * c * h * w, 'nv12': n * 3 * h // 2 * w},
+        'd2h_bytes_per_step': {'uint8': n * c * H * W, 'nv12': n * 3 * H // 2 * W},
         'launches_per_step': {'infer_sequence': T.engine.get_engine(net, n, c, h, w, dev).launches_per_step,
-                              'push': stream_launches},
+                              'push': stream_launches, 'push_nv12': nv12_launches},
     }
     print(json.dumps(line), flush=True)
 
