@@ -62,6 +62,27 @@ static inline cudaError_t tg_launch(void (*kernel)(KArgs...), dim3 grid, dim3 bl
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
+// tg_launch with a 1-D thread-block cluster of `cluster_x` CTAs (gridDim.x must be a multiple of it)
+template <typename... KArgs, typename... Args>
+static inline cudaError_t tg_launch_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
+                                            cudaStream_t stream, int cluster_x, Args... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = (unsigned)cluster_x;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[1].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = tg_pdl_enabled() ? 2 : 1;
+  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+
 // Cooperative launch: the driver schedules the grid only when EVERY CTA can be resident at once
 // (or fails the launch) -- required by kernels whose CTAs wait on each other (conv_chain_kernel).
 // Not combined with programmatic dependent launch: such a kernel starts after its predecessor.

@@ -12,7 +12,8 @@
 //             (dy*10+dx)*128 B, 8-row-group stride = 10*128 B), or as one 16x8 box per tap.
 //   B       : weights pre-packed on the device in the exact swizzled smem image
 //             (tg_pack_*_weights), either resident in smem for the whole kernel (SRNet, thin
-//             FNet layers) or streamed per (tap, chunk) with cp.async.bulk (fat FNet layers).
+//             FNet layers, one K chunk per CTA of a cluster for the 128 / 256-channel FNet layers: see
+//             consumer_splitk) or streamed per (tap, chunk) with cp.async.bulk (tap mode).
 //   D       : fp32 accumulators in the registers of the consumer warpgroup (64 per thread).
 //   roles   : warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers that take the
 //             CTA's tiles alternately, each with its own ring of smem stages: wgmma -> accumulators
@@ -55,6 +56,8 @@ constexpr int MODE_TAP = 0;    // one 16x8 box per (tap, chunk)
 constexpr int MODE_HALO = 1;   // one 18x10 halo box per (tile, chunk), taps = descriptor shifts
 constexpr int MODE_TAPN = 2;   // thin heads: one 16x8 box per (tile, chunk), N = 9 taps x 4 couts,
                                // 3x3 shift-add in the epilogue; tiles overlap by one pixel ring
+constexpr int MODE_SPLITK = 3; // forward conv3x3 with cin 128 / 256: the K chunks split over a cluster
+                               // (see consumer_splitk)
 constexpr int kTapnStepY = TH - 2, kTapnStepX = TW - 2;   // 14 x 6 valid outputs per TAPN tile
 // fp32 staging tile of a consumer: 128 rows x (N + 4) floats (the pad keeps the per-row float4
 // reads of the epilogue free of bank conflicts)
@@ -75,6 +78,7 @@ struct KParams {
   int n_split, bn;                 // output channels are split over n_split CTAs of bn columns
   uint32_t stage_bytes, a_bytes, b_tile_bytes, b_stage_bytes;
   uint32_t off_b, off_stage, off_scratch;   // off_scratch: the consumers' fp32 staging or fp16 output tiles
+  uint32_t epi_bytes;              // MODE_SPLITK: per-consumer receive buffer (the output tile overlaps it)
 };
 
 // The forward halo conv / transposed conv with NHWC output (pooled or not) puts the roles of the GEMM the
@@ -340,6 +344,163 @@ __device__ __forceinline__ void consumer_halo_pxn(const TgMaps& maps, const KPar
   if (r == 0) bulk_wait_group0();
 }
 
+// ------------------------------------------------------------------ consumer of the split-K path
+// Forward 3x3 conv with cin = 64 * C (C = 2 or 4), NHWC output (pooled or not).  The C CTAs of a thread-block
+// cluster share every (tile, N slice): CTA rank r keeps the weights of K chunk r resident, loads one halo box
+// at channel offset 64 r and runs the 64->64 pixels-on-N mainloop of consumer_halo_pxn on it, giving a
+// partial D_r[64 cout][128 px].  The partials are reduced through distributed shared memory, partitioned by
+// output channel: warp q (couts 16q..16q+15) belongs to rank q / (4 / C).  Each thread of a warp that another
+// rank owns sends its 64 accumulators with st.async to the same thread's slot in the owner's receive buffer
+// (slot layout [sender slot][owner warp][16 float4][32 lanes]; transaction bytes complete the owner's
+// per-consumer "full" barrier).  The owner adds the partials in rank order, p0 + p1 (+ p2 + p3), so the
+// result does not depend on which CTA owns the couts or on the grid, then runs the register epilogue and
+// stores its 64/C-channel slice of the tile with one TMA store (unswizzled box, 2 * 64/C bytes per pixel).
+// The output tile overlaps the receive buffer: once a tile's store has read it, the owner's store thread
+// hands the buffer back with a remote arrive on each peer's per-consumer "free" barrier (C - 1 arrivals),
+// which a sender waits on before it sends its next tile.  All CTAs of a cluster walk the same tile sequence.
+template <bool POOL>
+__device__ __forceinline__ void consumer_splitk(const TgMaps& maps, const KParams& p, uint32_t base,
+                                                const float* bias_s, int cw) {
+  const tg_conv_desc& d = p.d;
+  const int r = threadIdx.x - 128 * (1 + cw);
+  const int q = r >> 5, lane = threadIdx.x & 31;
+  const int C = p.chunks;
+  const int rank = (int)cluster_ctarank();
+  const int wpr = 4 / C;                   // warps (16 couts each) owned per rank
+  const int owner = q / wpr;
+  const bool own = owner == rank;
+  const bool lead = r == rank * wpr * 32;  // first thread of the rank's first owned warp: stores, hand-backs
+  const int sc = 64 / C;                   // output channels per rank
+  const uint32_t sb = 2u * (uint32_t)sc;   // bytes per pixel of the rank's output slice tile
+  const uint32_t bar_full = base + 8u * (cw * kMaxRing), bar_empty = base + 16 * kMaxRing + 8u * (cw * kMaxRing);
+  const uint32_t bar_rfull = base + 32 * kMaxRing + 24 + 8u * cw, bar_free = base + 32 * kMaxRing + 40 + 8u * cw;
+  const uint32_t stage0 = base + p.off_stage + (uint32_t)(cw * p.ring) * p.stage_bytes;
+  const uint32_t epi_s = base + p.off_scratch + (uint32_t)cw * p.epi_bytes;
+  constexpr uint32_t kBoxW = TW + 2;
+  const uint64_t w_hi = gmma_desc_hi(1024u), x_hi = gmma_desc_hi(kBoxW * 128u);
+  const uint32_t w16 = gmma_addr16(base + p.off_b), btb16 = p.b_stage_bytes >> 4;
+  const int bar_id = 1 + cw;
+  // where this thread's partial goes in the owner's receive buffer (senders only)
+  const int my_slot = rank < owner ? rank : rank - 1;
+  const uint32_t send_off = (uint32_t)((my_slot * wpr + (q - owner * wpr)) * 16) * 512u + (uint32_t)lane * 16u;
+  const uint32_t peer_buf = mapa_shared(epi_s + send_off, (uint32_t)owner);
+  const uint32_t peer_bar = mapa_shared(bar_rfull, (uint32_t)owner);
+  const uint32_t recv_bytes = (uint32_t)((C - 1) * wpr) * 8192u;
+  // stmatrix: lane l addresses pixel row kk of matrix m = l/8 = (tile row pair, 8-channel chunk 2*q + m%2); in the
+  // rank's slice tile that chunk is local chunk 2*(q - rank*wpr) + m%2 (owners only)
+  const uint32_t kk = POOL ? 4u * (lane & 1) + ((lane & 7) >> 1) : (uint32_t)(lane & 7);
+  const uint32_t mat_off = (uint32_t)(8 * ((lane >> 3) >> 1) + kk) * sb +
+                           ((uint32_t)(2 * (q - rank * wpr) + ((lane >> 3) & 1)) << 4);
+  const int t0 = (int)cluster_id_x(), tstep = (int)cluster_count_x();
+  int stage = 0, it = 0;
+  uint32_t phase = 0;
+  float acc[64];
+
+  for (int tile = t0 + cw * tstep; tile < p.num_tiles; tile += 2 * tstep, ++it) {
+    const TileCoord tc = tile_coord(p, tile);
+    if (lead) {
+      bulk_wait_group_read0();           // the previous tile's store has left the output tile / receive buffer
+      if (it > 0)
+        for (int s = 0; s < C; ++s)
+          if (s != rank) mbar_arrive_cluster(mapa_shared(bar_free, (uint32_t)s));
+      mbar_expect_tx(bar_rfull, recv_bytes);
+    }
+    const int s = stage;
+    mbar_wait_mma(bar_full + 8 * s, phase);
+    if (++stage == p.ring) { stage = 0; phase ^= 1u; }
+    const uint32_t x16 = gmma_addr16(stage0 + (uint32_t)s * p.stage_bytes);
+    wgmma_fence();
+#pragma unroll
+    for (int g = 0; g < 9; ++g) {
+      const TgGroup gr = tg_group(TG_CONV_3X3, g);
+      const uint32_t a16 = w16 + (uint32_t)g * btb16;
+      const uint32_t b16 = x16 + (uint32_t)((gr.dy + 1) * (int)kBoxW + (gr.dx + 1)) * 8u;
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_n128(acc, w_hi | (uint64_t)(a16 + 2u * k), x_hi | (uint64_t)(b16 + 2u * k), (g == 0 && k == 0) ? 0u : 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_empty + 8 * s);
+
+    if (!own) {
+      // the owner has handed back the buffer its previous tile's partials went to
+      if (it > 0) mbar_wait_cluster(bar_free, (uint32_t)(it - 1) & 1u);
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+        st_async_v4(peer_buf + (uint32_t)j * 512u, make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]),
+                    peer_bar);
+    } else {
+      mbar_wait_cluster(bar_rfull, (uint32_t)it & 1u);
+      const uint32_t lq_off = (uint32_t)((q - rank * wpr) * 16) * 512u + (uint32_t)lane * 16u;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const float4 mine = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
+        float4 sum = mine;
+#pragma unroll
+        for (int src = 0; src < 4; ++src) {
+          if (src >= C) break;
+          const int slot = src < rank ? src : src - 1;
+          const float4 v = src == rank ? mine
+                                       : ld_shared_v4(epi_s + (uint32_t)(slot * wpr * 16) * 512u + lq_off + (uint32_t)j * 512u);
+          if (src == 0) sum = v;
+          else { sum.x += v.x; sum.y += v.y; sum.z += v.z; sum.w += v.w; }
+        }
+        acc[4 * j] = sum.x; acc[4 * j + 1] = sum.y; acc[4 * j + 2] = sum.z; acc[4 * j + 3] = sum.w;
+      }
+    }
+    named_bar_sync(bar_id, 128);         // the receive buffer is read: the output tile may overwrite it
+    if (own) {
+      const float b0 = bias_s[tc.nb * 64 + 16 * q + (lane >> 2)], b1 = bias_s[tc.nb * 64 + 16 * q + (lane >> 2) + 8];
+      if (POOL) {
+#pragma unroll
+        for (int ip = 0; ip < 2; ++ip) {
+          uint32_t ov[4];
+#pragma unroll
+          for (int m = 0; m < 4; ++m) {
+            const float bb = (m & 1) ? b1 : b0;
+            __half v[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int pr = 2 * (2 * ip + (m >> 1)) + e;
+              const int i0 = 4 * (2 * pr) + 2 * (m & 1), i1 = i0 + 4;
+              const __half2 r0 = __floats2half2_rn(tg_epi_val(acc[i0], bb, d.act), tg_epi_val(acc[i0 + 1], bb, d.act));
+              const __half2 r1 = __floats2half2_rn(tg_epi_val(acc[i1], bb, d.act), tg_epi_val(acc[i1 + 1], bb, d.act));
+              const __half2 mx = __hmax2(r0, r1);
+              v[e] = __hmax(__low2half(mx), __high2half(mx));
+            }
+            const __half2 o = __halves2half2(v[0], v[1]);
+            ov[m] = *reinterpret_cast<const uint32_t*>(&o);
+          }
+          stmatrix_x4_trans(epi_s + (uint32_t)ip * 16u * sb + mat_off, ov);
+        }
+      } else {
+#pragma unroll
+        for (int jp = 0; jp < 8; ++jp) {
+          uint32_t ov[4];
+#pragma unroll
+          for (int m = 0; m < 4; ++m) {
+            const int i = 4 * (2 * jp + (m >> 1)) + 2 * (m & 1);
+            const float bb = (m & 1) ? b1 : b0;
+            const __half2 o = __floats2half2_rn(tg_epi_val(acc[i], bb, d.act), tg_epi_val(acc[i + 1], bb, d.act));
+            ov[m] = *reinterpret_cast<const uint32_t*>(&o);
+          }
+          stmatrix_x4_trans(epi_s + (uint32_t)jp * 16u * sb + mat_off, ov);
+        }
+      }
+      fence_proxy_async_smem();
+    }
+    named_bar_sync(bar_id, 128);
+    if (lead) {
+      if (POOL) tma_store_4d(&maps.m[2], epi_s, tc.nb * 64 + rank * sc, tc.x0 >> 1, tc.y0 >> 1, tc.n);
+      else tma_store_4d(&maps.m[2], epi_s, tc.nb * 64 + rank * sc, tc.x0, tc.y0, tc.n);
+      bulk_commit_group();
+    }
+  }
+  if (lead) bulk_wait_group0();
+}
+
 // One consumer warpgroup of the forward stride-2 transposed conv (17x9 halo box, origin 0), pixels on N: for
 // each of its tiles and each output parity a = (py, px), acc[64 cout][128 px] = convT_pxn_mmas(a), then
 // bias / act -> fp16 -> stmatrix into one of the consumer's two 16 KB output tiles -> one TMA store of the
@@ -426,14 +587,19 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
   const uint32_t bar_empty = base + 16 * kMaxRing;         // [2 * kMaxRing]
   const uint32_t bar_b = base + 32 * kMaxRing;             // [1]
   const uint32_t bar_res = bar_b + 8;                      // [2] residual tile of consumer c
+  const uint32_t bar_rfull = bar_b + 24;                   // [2] MODE_SPLITK: partials received, consumer c
+  const uint32_t bar_free = bar_b + 40;                    // [2] MODE_SPLITK: peers handed back their buffers
   float* bias_s = reinterpret_cast<float*>(sm + 1024);
   static_assert(!(KIND == TG_CONV_3X3_S2 && MODE != MODE_TAP), "the stride-2 conv runs in tap mode only");
   constexpr bool kPxN = pixels_on_n<KIND, MODE, BWD>();
+  constexpr bool kSplitK = MODE == MODE_SPLITK;
+  static_assert(!kSplitK || (KIND == TG_CONV_3X3 && !BWD), "split-K: forward conv3x3 only");
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&maps.m[0]);
     if (KIND == TG_CONV_3X3_S2) { tma_prefetch_desc(&maps.m[1]); tma_prefetch_desc(&maps.m[2]); tma_prefetch_desc(&maps.m[3]); }
     if (kPxN) { tma_prefetch_desc(&maps.m[1]); tma_prefetch_desc(&maps.m[2]); }
+    if (kSplitK) tma_prefetch_desc(&maps.m[2]);
   }
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < 2 * kMaxRing; ++s) {
@@ -443,24 +609,40 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
     mbar_init(bar_b, 1);
     mbar_init(bar_res, 1);
     mbar_init(bar_res + 8, 1);
+    if (kSplitK) {
+      for (int c = 0; c < 2; ++c) {
+        mbar_init(bar_rfull + 8 * c, 1);             // the owner's expect_tx; the bytes come from the peers
+        mbar_init(bar_free + 8 * c, p.chunks - 1);   // one hand-back per peer
+      }
+    }
     fence_barrier_init();
   }
-  __syncthreads();
+  // split-K: the peers' barriers must be initialised before any remote arrive or st.async reaches them
+  if constexpr (kSplitK) cluster_sync();
+  else __syncthreads();
 
   const uint32_t smem_b = base + p.off_b;
   const uint32_t smem_stage0 = base + p.off_stage;
   const unsigned char* wglob = reinterpret_cast<const unsigned char*>(d.weights);
-  const int n_tiles_w = (MODE == MODE_TAPN ? 1 : 9) * p.chunks;
+  const int n_tiles_w = (MODE == MODE_TAPN ? 1 : 9) * (kSplitK ? 1 : p.chunks);
+  // tile schedule: CTA i of the grid, or cluster i of the grid for split-K (all CTAs of a cluster take the
+  // same tiles; CTA rank r of the cluster works on K chunk r)
+  const int sched0 = kSplitK ? (int)cluster_id_x() : (int)blockIdx.x;
+  const int sched_step = kSplitK ? (int)cluster_count_x() : (int)gridDim.x;
+  const int k_rank = kSplitK ? (int)cluster_ctarank() : 0;
 
   // Resident weights do not depend on the previous kernel (static during graph replay; the eager path
   // separates tg_pack_* from the conv by a bias copy): start their load, then join the
   // programmatic-dependent-launch wait.  The previous kernel's OUTPUT is only read after tg_pdl_wait().
   if (warp == 0 && lane == 0 && p.b_resident) {
-    const uint32_t nb = blockIdx.x % (uint32_t)p.n_split;   // fixed per CTA: gridDim.x % n_split == 0
+    // fixed per CTA: the number of CTAs (clusters for split-K) is a multiple of n_split
+    const uint32_t nb = (uint32_t)sched0 % (uint32_t)p.n_split;
     mbar_expect_tx(bar_b, (uint32_t)n_tiles_w * p.b_stage_bytes);
-    for (int t = 0; t < n_tiles_w; ++t)
-      bulk_load(smem_b + t * p.b_stage_bytes, wglob + (size_t)t * p.b_tile_bytes + (size_t)nb * p.b_stage_bytes,
+    for (int t = 0; t < n_tiles_w; ++t) {
+      const int src = kSplitK ? t * p.chunks + k_rank : t;   // split-K: the 9 taps of chunk k_rank
+      bulk_load(smem_b + t * p.b_stage_bytes, wglob + (size_t)src * p.b_tile_bytes + (size_t)nb * p.b_stage_bytes,
                 p.b_stage_bytes, bar_b);
+    }
   }
   tg_pdl_wait();
   tg_pdl_trigger();
@@ -473,17 +655,17 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
       int stage[2] = {0, 0};
       uint32_t phase[2] = {0, 0};
       int it = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
+      for (int tile = sched0; tile < p.num_tiles; tile += sched_step, ++it) {
         const int cw = it & 1;
         const TileCoord tc = tile_coord(p, tile);
-        const int n_loads = MODE == MODE_TAP ? 9 * p.chunks : p.chunks;
+        const int n_loads = MODE == MODE_TAP ? 9 * p.chunks : kSplitK ? 1 : p.chunks;
         for (int l = 0; l < n_loads; ++l) {
           const int s = cw * kMaxRing + stage[cw];
           mbar_wait_mma(bar_empty + 8 * s, phase[cw] ^ 1);
           const uint32_t sa = smem_stage0 + (uint32_t)(cw * p.ring + stage[cw]) * p.stage_bytes;
           if (MODE != MODE_TAP) {
             mbar_expect_tx(bar_full + 8 * s, p.a_bytes);
-            tma_load_4d(sa, &maps.m[0], bar_full + 8 * s, l * 64, tc.x0 + p.org_x, tc.y0 + p.org_y, tc.n);
+            tma_load_4d(sa, &maps.m[0], bar_full + 8 * s, (l + k_rank) * 64, tc.x0 + p.org_x, tc.y0 + p.org_y, tc.n);
           } else {
             const int g = l / p.chunks, c = l - g * p.chunks;
             const TgGroup gr = tg_group(KIND, g);
@@ -498,6 +680,12 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
           if (++stage[cw] == p.ring) { stage[cw] = 0; phase[cw] ^= 1u; }
         }
       }
+    }
+  } else if (kSplitK) {
+    // ============================================================ consumers, split-K over the cluster
+    if (warp >= 4) {
+      mbar_wait_mma(bar_b, 0);
+      consumer_splitk<POOL>(maps, p, base, bias_s, (warp - 4) >> 2);
     }
   } else if (kPxN) {
     // ============================================================ consumers, pixels on N
@@ -667,6 +855,8 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
       }
     }
   }
+  // split-K: no CTA leaves (and frees its shared memory) while a peer may still arrive on its barriers
+  if constexpr (kSplitK) cluster_sync();
 }
 
 // ------------------------------------------------------------------ host side
@@ -688,16 +878,16 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// fp16 tensor of `rank` dims (dims[0] contiguous), element strides of dims 1.., 128B swizzle
+// fp16 tensor of `rank` dims (dims[0] contiguous), element strides of dims 1.., 128B swizzle (or none)
 int encode_f16(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const size_t* elem_strides,
-               const cuuint32_t* box) {
+               const cuuint32_t* box, bool swizzle = true) {
   EncodeTiledFn fn = get_encode_fn();
   TG_REQUIRE(fn != nullptr, TG_E_DRIVER, "cuTensorMapEncodeTiled not available from the driver");
   cuuint64_t strides[4];
   for (int i = 0; i + 1 < rank; ++i) strides[i] = (cuuint64_t)elem_strides[i] * 2;
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
   CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides, box,
-                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   TG_REQUIRE(r == CUDA_SUCCESS, TG_E_DRIVER,
              "cuTensorMapEncodeTiled failed (%d) rank=%d dims=%llux%llux%llux%llu box=%ux%ux%u", (int)r, rank,
@@ -708,11 +898,11 @@ int encode_f16(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims
 
 // NHWC fp16 tensor [n][h][w][c] with explicit element strides for w/h/n (parity views)
 int encode_nhwc(CUtensorMap* m, const void* ptr, int c, int w, int h, int n, size_t sw, size_t sh,
-                size_t sn, int box_c, int box_w, int box_h) {
+                size_t sn, int box_c, int box_w, int box_h, bool swizzle = true) {
   const cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
   const size_t strides[3] = {sw, sh, sn};
   const cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
-  return encode_f16(m, ptr, 4, dims, strides, box);
+  return encode_f16(m, ptr, 4, dims, strides, box, swizzle);
 }
 
 // Output [n][2h][2w][c] of the transposed conv with input size h x w, as the 5-D tensor (2c, w, 2, h, n):
@@ -731,6 +921,35 @@ template <int K, int M, bool B, bool P>
 cudaError_t set_smem_attr() {
   return cudaFuncSetAttribute(conv_wgmma_kernel<K, M, B, P>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                               (int)kSmemLimit);
+}
+
+// Clusters of `cluster` split-K CTAs (one per SM) that can be resident at once, per device; 0 if the query fails.
+template <bool P>
+int splitk_max_clusters(int cluster) {
+  static int cache[64][5] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
+  int& v = cache[dev][cluster];
+  if (v == 0) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(cluster);
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = kSmemLimit;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)cluster;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int n = 0;
+    if (cudaOccupancyMaxActiveClusters(&n, conv_wgmma_kernel<TG_CONV_3X3, MODE_SPLITK, false, P>, &cfg) != cudaSuccess) {
+      (void)cudaGetLastError();
+      n = 0;
+    }
+    v = n;
+  }
+  return v;
 }
 
 }  // namespace
@@ -805,7 +1024,13 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
   p.n_split = (!tapn && d->cout > 64) ? d->cout / 64 : 1;
   p.bn = d->cout / p.n_split;
   p.b_stage_bytes = (uint32_t)p.bn * 128u;
-  const uint32_t b_total = (tapn ? 1u : 9u) * p.chunks * p.b_stage_bytes;   // resident slice per CTA
+  const bool bwd = d->act >= TG_ACT_DRELU || d->kind == TG_CONV_3X3_S2;
+  const bool convT = d->kind == TG_CONVT_3X3_S2;
+  // Forward 3x3 convs with 128 / 256 input channels (NHWC output, pooled or not) split K over a cluster of
+  // cin/64 CTAs (MODE_SPLITK), each with one chunk's weights resident; TG_AMODE_TAP keeps the tap kernel.
+  const bool splitk = d->a_mode == TG_AMODE_AUTO && d->kind == TG_CONV_3X3 && !bwd && !tapn && p.chunks >= 2 &&
+                      d->residual == nullptr;
+  const uint32_t b_total = (tapn ? 1u : 9u) * (splitk ? 1u : (uint32_t)p.chunks) * p.b_stage_bytes;   // resident slice per CTA
   const int hbox_w = d->kind != TG_CONVT_3X3_S2 ? TW + 2 : TW + 1;
   const int hbox_h = d->kind != TG_CONVT_3X3_S2 ? TH + 2 : TH + 1;
   const uint32_t halo_bytes = (uint32_t)hbox_w * hbox_h * 128u;
@@ -821,8 +1046,8 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
   TG_REQUIRE(!(d->kind == TG_CONV_3X3_S2 && mode == TG_AMODE_HALO), TG_E_UNSUPPORTED,
              "conv: conv3x3s2 runs in tap mode (a stride-2 view is not a wgmma descriptor)");
   if (d->kind == TG_CONV_3X3_S2 || tapn) mode = TG_AMODE_TAP;   // thin heads run MODE_TAPN below
-  if (mode == TG_AMODE_AUTO) mode = can_resident_halo ? TG_AMODE_HALO : TG_AMODE_TAP;
-  TG_REQUIRE(!(mode == TG_AMODE_HALO && !can_resident_halo), TG_E_UNSUPPORTED,
+  if (mode == TG_AMODE_AUTO) mode = (splitk || can_resident_halo) ? TG_AMODE_HALO : TG_AMODE_TAP;
+  TG_REQUIRE(!(mode == TG_AMODE_HALO && !splitk && !can_resident_halo), TG_E_UNSUPPORTED,
              "conv: halo mode needs the weights resident in smem (cin=%d cout=%d)", d->cin, d->cout);
   p.halo = mode == TG_AMODE_HALO;
   p.b_resident = p.halo ? 1 : (can_resident_tap ? 1 : 0);
@@ -848,10 +1073,12 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
   // the consumers' epilogue tiles on the pixels-on-N path: one fp16 output / residual tile (16 KB) each, two
   // per consumer for the transposed conv (alternating parities), one 4 KB pooled tile each with the pool;
   // fp32 accumulator staging otherwise
-  const bool bwd = d->act >= TG_ACT_DRELU || d->kind == TG_CONV_3X3_S2;
-  const bool convT = d->kind == TG_CONVT_3X3_S2;
-  const bool pxn = p.halo && !bwd && !tapn;
-  const uint32_t epi_tiles = !pxn ? scratch : convT ? 4u * kTapABytes : pool ? 2u * kPoolTileBytes : 2u * kTapABytes;
+  // Split-K: a receive buffer per consumer for the peers' partials of the couts this CTA owns ((C - 1) x 4/C
+  // warps x 8 KB: 16 KB for C = 2, 24 KB for C = 4); the consumer's output slice tile overlaps it.
+  const bool pxn = p.halo && !bwd && !tapn && !splitk;
+  p.epi_bytes = splitk ? (uint32_t)((p.chunks - 1) * (4 / p.chunks)) * 8192u : 0u;
+  const uint32_t epi_tiles = splitk ? 2u * p.epi_bytes
+                             : !pxn ? scratch : convT ? 4u * kTapABytes : pool ? 2u * kPoolTileBytes : 2u * kTapABytes;
   const uint32_t avail = kSmemLimit - 1024u - kHeaderBytes - epi_tiles - (p.b_resident ? b_total : 0u);
   int ring = (int)(avail / p.stage_bytes) / 2;
   if (ring > kMaxRing) ring = kMaxRing;
@@ -871,7 +1098,15 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
     if (rc != TG_OK) return rc;
     map_a.m[1] = map_a.m[2] = map_a.m[3] = map_a.m[0];
     const size_t C = (size_t)d->cout;
-    if (pxn && convT) {
+    if (splitk) {
+      // [2] = the output (pooled or not), one box per tile, N slice and rank: 64/C channels x 16x8 px (8x4 pooled),
+      // unswizzled (the rank's slice tile is dense, 2 * 64/C bytes per pixel)
+      const int sc = 64 / p.chunks;
+      const int ow = pool ? d->w / 2 : d->w, oh = pool ? d->h / 2 : d->h;
+      rc = encode_nhwc(&map_a.m[2], d->y, d->cout, ow, oh, d->n, C, (size_t)ow * C, (size_t)oh * ow * C, sc,
+                       pool ? TW / 2 : TW, pool ? TH / 2 : TH, /*swizzle=*/false);
+      if (rc != TG_OK) return rc;
+    } else if (pxn && convT) {
       rc = encode_convT_out(&map_a.m[2], d->y, d->cout, d->w, d->h, d->n);
       if (rc != TG_OK) return rc;
     } else if (pxn && pool) {
@@ -910,7 +1145,8 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
         set_smem_attr<TG_CONV_3X3, MODE_TAPN, false, false>(), set_smem_attr<TG_CONVT_3X3_S2, MODE_HALO, false, false>(),
         set_smem_attr<TG_CONVT_3X3_S2, MODE_TAP, false, false>(), set_smem_attr<TG_CONV_3X3, MODE_HALO, false, true>(),
         set_smem_attr<TG_CONV_3X3, MODE_TAP, false, true>(), set_smem_attr<TG_CONV_3X3, MODE_HALO, true, false>(),
-        set_smem_attr<TG_CONV_3X3, MODE_TAP, true, false>(), set_smem_attr<TG_CONV_3X3_S2, MODE_TAP, true, false>()};
+        set_smem_attr<TG_CONV_3X3, MODE_TAP, true, false>(), set_smem_attr<TG_CONV_3X3_S2, MODE_TAP, true, false>(),
+        set_smem_attr<TG_CONV_3X3, MODE_SPLITK, false, false>(), set_smem_attr<TG_CONV_3X3, MODE_SPLITK, false, true>()};
     for (cudaError_t e : errs)
       if (e != cudaSuccess) return e;
     return cudaSuccess;
@@ -921,13 +1157,33 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
   int sms = 0;
   rc = tg_device_sm_count(&sms);
   if (rc != TG_OK) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 b(kThreads);
+  cudaError_t lerr = cudaSuccess;
+  if (splitk) {
+    // clusters of C = cin/64 CTAs, as many as can be resident (max_ctas: at most that many CTAs); every
+    // cluster keeps one fixed N slice, so the cluster count is a multiple of n_split
+    const int C = p.chunks;
+    const int resident = pool ? splitk_max_clusters<true>(C) : splitk_max_clusters<false>(C);
+    TG_REQUIRE(resident > 0, TG_E_DRIVER, "conv: cudaOccupancyMaxActiveClusters found no room for a %d-CTA cluster", C);
+    int ncl = d->max_ctas > 0 ? d->max_ctas / C : resident;
+    if (ncl > p.num_tiles) ncl = p.num_tiles;
+    ncl -= ncl % p.n_split;
+    if (ncl < p.n_split) ncl = p.n_split;
+    const dim3 g(ncl * C);
+    lerr = pool ? tg_launch_cluster(conv_wgmma_kernel<TG_CONV_3X3, MODE_SPLITK, false, true>, g, b, kSmemLimit, st, C,
+                                    map_a, p)
+                : tg_launch_cluster(conv_wgmma_kernel<TG_CONV_3X3, MODE_SPLITK, false, false>, g, b, kSmemLimit, st, C,
+                                    map_a, p);
+    TG_REQUIRE(lerr == cudaSuccess, (int)lerr, "conv: launch failed: %s", cudaGetErrorString(lerr));
+    TG_CUDA_LAUNCH_CHECK("conv");
+    return TG_OK;
+  }
   int grid = d->max_ctas > 0 ? d->max_ctas : sms;
   if (grid > p.num_tiles) grid = p.num_tiles;
   grid -= grid % p.n_split;             // every CTA keeps one fixed N slice (resident weights)
   if (grid < p.n_split) grid = p.n_split;
-  cudaStream_t st = (cudaStream_t)stream;
-  const dim3 g(grid), b(kThreads);
-  cudaError_t lerr = cudaSuccess;
+  const dim3 g(grid);
   if (pool) {
     lerr = p.halo ? tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_HALO, false, true>, g, b, kSmemLimit, st, map_a, p)
                   : tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_TAP, false, true>, g, b, kSmemLimit, st, map_a, p);
