@@ -273,6 +273,36 @@ int tg_stream_frame_in_yuv420(const uint8_t* in, int nv12, const int32_t* reset,
  * of each 2x2 block from its top-left pixel), NV12 with the U and V planes interleaved.  H and W must be even. */
 int tg_rgb_u8_to_yuv420(const uint8_t* rgb, uint8_t* out, int nv12, int n, int H, int W, void* stream);
 
+/* YUV 4:2:0 frame I/O in any supported layout and colour.
+ * layout : TG_YUV_NV12 / TG_YUV_I420 (uint8 words, as above), TG_YUV_P010 (NV12 planes, uint16 words, sample in the
+ *          high 10 bits: v << 6; NVDEC / NVENC, ffmpeg p010le), TG_YUV_I420_10 (I420 planes, uint16 words, sample in
+ *          the low 10 bits; ffmpeg yuv420p10le).  Frames are [n, 3h/2, w] words; 10-bit frames 2-byte aligned.
+ * matrix : 601 (Kr, Kb = 0.299, 0.114) or 709 (0.2126, 0.0722); full_range 0 = limited ("tv"), 1 = full ("pc")
+ *          quantisation of ITU-T H.273 at the layout's bit depth; reserved must be 0.
+ * The fixed-point matrices are tg_yuv_coefficients' table (oracle/yuv_color.py derives the same numbers); matrix
+ * 601, limited range, 8 bit is cv2's BT.601 and gives the bytes of the two entry points above. */
+enum { TG_YUV_NV12 = 0, TG_YUV_I420 = 1, TG_YUV_P010 = 2, TG_YUV_I420_10 = 3 };
+typedef struct tg_yuv_format {
+  int32_t layout;       /* TG_YUV_*                   */
+  int32_t matrix;       /* 601 or 709                 */
+  int32_t full_range;   /* 0 limited, 1 full          */
+  int32_t reserved;     /* must be 0                  */
+} tg_yuv_format;
+/* tg_stream_frame_in_yuv420 for any format: lr_curr = float(rgb) / 255 (8 bit) or / 1023 (10 bit, P010 read as
+ * v >> 6, I420_10 as min(v, 1023)), rgb decoded with nearest chroma; reset as in tg_stream_frame_in. */
+int tg_stream_frame_in_yuv(const void* in, const tg_yuv_format* fmt, const int32_t* reset, float* lr_curr,
+                           float* lr_prev, float* hr_prev, int n, int h, int w, int s, void* stream);
+/* Encode of the streamed output into any format.  8-bit layouts read rgb_u8 (uint8 NHWC [n,H,W,3], the step's
+ * out_u8; rgb_f32 must be NULL), 10-bit layouts read rgb_f32 (fp32 NCHW [n,3,H,W], the step's HR frame, quantised as
+ * clip(rint(x * 1023), 0, 1023); rgb_u8 must be NULL).  Chroma of each 2x2 block from its top-left pixel.
+ * TG_E_INVALID: null pointers, the wrong source for the bit depth, a non-zero reserved; TG_E_UNSUPPORTED: odd sizes,
+ * unknown layout or matrix. */
+int tg_rgb_to_yuv(const uint8_t* rgb_u8, const float* rgb_f32, void* out, const tg_yuv_format* fmt, int n, int H,
+                  int W, void* stream);
+/* Host only: the 16 int32 of the kernels' table row for fmt (its bit depth and colour): encode cRY cGY cBY cRU cGU
+ * cBU cRV cGV cBV, decode CY CUB CUG CVG CVR, then the fraction bits and the luma offset. */
+int tg_yuv_coefficients(const tg_yuv_format* fmt, int32_t* out16);
+
 /* BD degradation of the data side (codes/utils/data_utils.py:30-53, called on GT frames by
  * base_model.py:75,115): optional reflect pad by (k-1)/2 | k-1-(k-1)/2, then a depthwise valid
  * correlation with the k x k kernel `k2d` (device, fp32, = create_kernel(sigma)[0,0]) and stride s.

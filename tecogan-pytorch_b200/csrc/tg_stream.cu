@@ -1,7 +1,10 @@
-// Frame I/O of one streamed inference step: uint8 HWC or YUV 4:2:0 (NV12 / I420) frames decoded on the device
-// into the step's fp32 NCHW lr_curr, the per-slot reset of the recurrent state, and the encode of the step's
-// uint8 RGB output into NV12 / I420.  Contract: include/tecogan_b200.h (tg_stream_frame_in,
-// tg_stream_frame_in_yuv420, tg_rgb_u8_to_yuv420).
+// Frame I/O of one streamed inference step: uint8 HWC or YUV 4:2:0 (NV12 / I420, 8 bit; P010 / I420_10, 10 bit)
+// frames decoded on the device into the step's fp32 NCHW lr_curr, the per-slot reset of the recurrent state, and
+// the encode of the step's RGB output (uint8 NHWC, or the fp32 NCHW HR frame for 10-bit output) into YUV 4:2:0.
+// Contract: include/tecogan_b200.h (tg_stream_frame_in, tg_stream_frame_in_yuv420, tg_rgb_u8_to_yuv420,
+// tg_stream_frame_in_yuv, tg_rgb_to_yuv, tg_yuv_coefficients).
+#include <type_traits>
+
 #include "tg_common.cuh"
 
 namespace {
@@ -10,17 +13,73 @@ constexpr int kThreads = 256;
 constexpr int kTilePx = 256;            // decode / encode CTA: kTilePx pixels of a row, one per thread
 constexpr int kMaxC = 4;
 
-enum FrameFormat { kHWC = 0, kNV12 = 1, kI420 = 2 };
+enum FrameFormat { kHWC = 0, kNV12 = 1, kI420 = 2, kP010 = 3, kI420_10 = 4 };
 
-// cv2's BT.601 limited-range YUV 4:2:0 conversions (color_yuv: 20-bit fixed point); oracle/yuv_oracle.py restates
-// them in numpy.  Every intermediate fits in int32: |sum| < 2^30.
-constexpr int kShift = 20, kHalf = 1 << (kShift - 1);
-constexpr int kCRY = 269484, kCGY = 528482, kCBY = 102760;
-constexpr int kCRU = -155188, kCGU = -305135, kCBU = 460324;
-constexpr int kCRV = 460324, kCGV = -385875, kCBV = -74448;
-constexpr int kCY = 1220542, kCUB = 2116026, kCUG = -409993, kCVG = -852492, kCVR = 1673527;
+template <int kFmt>
+struct Yuv {
+  static constexpr bool kInterleaved = kFmt == kNV12 || kFmt == kP010;     // NV12 plane layout
+  static constexpr bool k10 = kFmt == kP010 || kFmt == kI420_10;
+  using Word = typename std::conditional<k10, uint16_t, uint8_t>::type;
+  static constexpr int kShift = k10 ? 18 : 20;                              // fraction bits of the table row
+  static constexpr int kTop = k10 ? 1023 : 255;
+  static constexpr int kCoff = k10 ? 512 : 128;
+  // the sample of a stored word: P010 keeps it in the high 10 bits, I420_10 in the low 10 (larger words clamp)
+  static __device__ __forceinline__ int sample(Word v) {
+    return kFmt == kP010 ? (int)(v >> 6) : kFmt == kI420_10 ? min((int)v, 1023) : (int)v;
+  }
+  static __device__ __forceinline__ Word word(int v) { return (Word)(kFmt == kP010 ? v << 6 : v); }
+};
 
-__device__ __forceinline__ int clamp_u8(int v) { return min(max(v, 0), 255); }
+// The colour table (oracle/yuv_color.py derives the same numbers): [depth 8 / 10][colour][16] with colour
+// 0 bt601, 1 bt709, 2 bt601-full, 3 bt709-full and the row
+//   cRY cGY cBY cRU cGU cBU cRV cGV cBV   encode, per RGB code value
+//   CY CUB CUG CVG CVR                    decode
+//   shift yoff                            fraction bits (20 at 8 bits, 18 at 10), luma offset (0: full range)
+// Rows are (Kr, Kb) quantised as ITU-T H.273 does for the bit depth, rounded half away from zero.  The 8-bit
+// bt601 row is cv2's BT.601 limited-range constants (color_yuv), so the NV12 / I420 bytes stay cv2's; its
+// decode also keeps cv2's max(Y - 16, 0) before the multiply, the derived rows clamp only the RGB result.
+// Every fixed-point intermediate fits in int32: |sum| < 6e8.
+struct YuvTable {
+  int v[2][4][16];
+};
+
+constexpr int yuv_round(double x) { return x >= 0 ? (int)(x + 0.5) : -(int)(-x + 0.5); }
+
+constexpr YuvTable make_yuv_table() {
+  YuvTable t{};
+  const int cv2[16] = {269484, 528482, 102760, -155188, -305135, 460324, 460324, -385875, -74448,
+                       1220542, 2116026, -409993, -852492, 1673527, 20, 16};
+  for (int di = 0; di < 2; ++di) {
+    const int depth = di ? 10 : 8, shift = di ? 18 : 20;
+    for (int ci = 0; ci < 4; ++ci) {
+      int* r = t.v[di][ci];
+      if (di == 0 && ci == 0) {
+        for (int k = 0; k < 16; ++k) r[k] = cv2[k];
+        continue;
+      }
+      const bool full = ci >= 2;
+      const double kr = (ci & 1) ? 0.2126 : 0.299, kb = (ci & 1) ? 0.0722 : 0.114;
+      const double kg = 1.0 - kr - kb;
+      const double d = (double)((1 << depth) - 1), sc = (double)(1 << (depth - 8));
+      const double ky = full ? d : 219.0 * sc, kc = full ? d : 224.0 * sc;
+      const double one = (double)(1 << shift);
+      const double m[14] = {kr * ky / d, kg * ky / d, kb * ky / d,
+                            -kr / (2.0 * (1.0 - kb)) * kc / d, -kg / (2.0 * (1.0 - kb)) * kc / d, 0.5 * kc / d,
+                            0.5 * kc / d, -kg / (2.0 * (1.0 - kr)) * kc / d, -kb / (2.0 * (1.0 - kr)) * kc / d,
+                            d / ky, d * 2.0 * (1.0 - kb) / kc, -d * 2.0 * (1.0 - kb) * kb / (kg * kc),
+                            -d * 2.0 * (1.0 - kr) * kr / (kg * kc), d * 2.0 * (1.0 - kr) / kc};
+      for (int k = 0; k < 14; ++k) r[k] = yuv_round(m[k] * one);
+      r[14] = shift;
+      r[15] = full ? 0 : 16 << (depth - 8);
+    }
+  }
+  return t;
+}
+
+constexpr YuvTable kYuvTable = make_yuv_table();
+__constant__ YuvTable c_yuv = make_yuv_table();
+static_assert(kYuvTable.v[0][0][14] == Yuv<kNV12>::kShift && kYuvTable.v[1][3][14] == Yuv<kP010>::kShift,
+              "table shift and kernel shift disagree");
 
 // zero floats [0, count) of p (4-byte aligned): 16-byte stores over the aligned interior, at most three
 // scalar stores at each end.  `worker` of `workers` threads; writes nothing outside the range.
@@ -86,46 +145,65 @@ __device__ __forceinline__ void decode_hwc(const uint8_t* __restrict__ in, float
   }
 }
 
-// decode CTA of YUV 4:2:0 frames ([3h/2, w] bytes each): kTilePx pixels of the luma rows 2*yp and 2*yp + 1 and
-// the chroma samples they share (cv2 COLOR_YUV2RGB_NV12 / _I420: nearest chroma), written as RGB / 255
+// decode CTA of YUV 4:2:0 frames ([3h/2, w] words each): kTilePx pixels of the luma rows 2*yp and 2*yp + 1 and
+// the chroma samples they share (nearest chroma), written as RGB / 255 (8 bit) or RGB / 1023 (10 bit).  Colour
+// row `color` of the table; with the 8-bit bt601 row this is cv2 COLOR_YUV2RGB_NV12 / _I420 bit for bit.
 template <int kFmt>
 __device__ __forceinline__ void decode_yuv420(const uint8_t* __restrict__ in, float* __restrict__ lr_curr, int b,
-                                              int t, int h, int w, int x_tiles) {
-  __shared__ __align__(16) uint8_t sy[2][kTilePx + 16];
-  __shared__ __align__(16) uint8_t sc[2][kTilePx + 16];     // NV12: sc[0] = U V U V ...; I420: sc[0] = U, sc[1] = V
+                                              int t, int h, int w, int x_tiles, int color) {
+  using F = Yuv<kFmt>;
+  using W = typename F::Word;
+  constexpr int kB = (int)sizeof(W);
+  __shared__ __align__(16) uint8_t sy[2][kTilePx * kB + 16];
+  __shared__ __align__(16) uint8_t sc[2][kTilePx * kB + 16];   // NV12 layout: sc[0] = U V U V ...; I420: U, V
   const int xt = b % x_tiles, r = b / x_tiles;
   const int hp = h >> 1, yp = r % hp, img = r / hp;
   const int x0 = xt * kTilePx;
   const int npx = min(kTilePx, w - x0);                      // even: w and x0 are
-  const uint8_t* frame = in + (size_t)img * (3 * hp) * w;
-  const uint8_t* yrow = frame + (size_t)(2 * yp) * w + x0;
-  const uint8_t* crow = frame + (size_t)h * w;               // chroma of the frame
-  int lc0, lc1 = 0;
-  const int ly0 = stage_bytes(sy[0], yrow, npx, t);
-  const int ly1 = stage_bytes(sy[1], yrow + w, npx, t);
-  if (kFmt == kNV12) {
-    lc0 = stage_bytes(sc[0], crow + (size_t)yp * w + x0, npx, t);
+  const W* frame = reinterpret_cast<const W*>(in) + (size_t)img * (3 * hp) * w;
+  const W* yrow = frame + (size_t)(2 * yp) * w + x0;
+  const W* crow = frame + (size_t)h * w;                     // chroma of the frame
+  const uint8_t* ysrc = reinterpret_cast<const uint8_t*>(yrow);
+  const uint8_t* csrc = reinterpret_cast<const uint8_t*>(crow);
+  const uint8_t* c0 = csrc + (F::kInterleaved ? (size_t)yp * w + x0 : (size_t)yp * (w >> 1) + (x0 >> 1)) * kB;
+  const uint8_t* c1 = c0 + (size_t)hp * (w >> 1) * kB;        // I420 layout: the V sample of the same block
+  stage_bytes(sy[0], ysrc, npx * kB, t);
+  stage_bytes(sy[1], ysrc + (size_t)w * kB, npx * kB, t);
+  if (F::kInterleaved) {
+    stage_bytes(sc[0], c0, npx * kB, t);
   } else {
-    const size_t cu = (size_t)yp * (w >> 1) + (x0 >> 1);
-    lc0 = stage_bytes(sc[0], crow + cu, npx >> 1, t);
-    lc1 = stage_bytes(sc[1], crow + (size_t)hp * (w >> 1) + cu, npx >> 1, t);
+    stage_bytes(sc[0], c0, (npx >> 1) * kB, t);
+    stage_bytes(sc[1], c1, (npx >> 1) * kB, t);
   }
   __syncthreads();
   if (t >= npx) return;
+  // the staged words start at the sources' offsets within 16 bytes (cheaper to recompute than to keep live)
+  const int ly0 = lead_of(ysrc), ly1 = lead_of(ysrc + (size_t)w * kB), lc0 = lead_of(c0);
+  const int lc1 = F::kInterleaved ? 0 : lead_of(c1);
+  // the leads are multiples of the word size: sources are word aligned
+  const auto at = [](const uint8_t* sb, int lead, int j) { return F::sample(reinterpret_cast<const W*>(sb + lead)[j]); };
   const int j = t >> 1;
-  const int u = kFmt == kNV12 ? sc[0][lc0 + 2 * j] : sc[0][lc0 + j];
-  const int v = kFmt == kNV12 ? sc[0][lc0 + 2 * j + 1] : sc[1][lc1 + j];
-  const int ruv = kHalf + kCVR * (v - 128);
-  const int guv = kHalf + kCVG * (v - 128) + kCUG * (u - 128);
-  const int buv = kHalf + kCUB * (u - 128);
+  const int u = F::kInterleaved ? at(sc[0], lc0, 2 * j) : at(sc[0], lc0, j);
+  const int v = F::kInterleaved ? at(sc[0], lc0, 2 * j + 1) : at(sc[1], lc1, j);
+  const int* k = c_yuv.v[F::k10][color];
+  constexpr int kHalf = 1 << (F::kShift - 1);
+  const int ruv = kHalf + k[13] * (v - F::kCoff);
+  const int guv = kHalf + k[12] * (v - F::kCoff) + k[11] * (u - F::kCoff);
+  const int buv = kHalf + k[10] * (u - F::kCoff);
+  const int cy = k[9], yoff = k[15];
+  const bool cv2_clamp = !F::k10 && color == 0;              // cv2: max(Y - 16, 0) before the multiply
+  constexpr float kScale = F::k10 ? 1023.f : 255.f;
+  auto rgb = [](int a) { return __fdiv_rn((float)min(max(a >> F::kShift, 0), F::kTop), kScale); };
   const size_t plane = (size_t)h * w;
   float* dst = lr_curr + (size_t)img * 3 * plane + (size_t)(2 * yp) * w + x0 + t;
 #pragma unroll
   for (int dy = 0; dy < 2; ++dy) {
-    const int yy = max((int)sy[dy][(dy ? ly1 : ly0) + t] - 16, 0) * kCY;
-    dst[dy * w] = __fdiv_rn((float)clamp_u8((yy + ruv) >> kShift), 255.f);
-    dst[dy * w + plane] = __fdiv_rn((float)clamp_u8((yy + guv) >> kShift), 255.f);
-    dst[dy * w + 2 * plane] = __fdiv_rn((float)clamp_u8((yy + buv) >> kShift), 255.f);
+    int yv = at(sy[dy], dy ? ly1 : ly0, t) - yoff;
+    if (cv2_clamp) yv = max(yv, 0);
+    const int yy = yv * cy;
+    dst[dy * w] = rgb(yy + ruv);
+    dst[dy * w + plane] = rgb(yy + guv);
+    dst[dy * w + 2 * plane] = rgb(yy + buv);
   }
 }
 
@@ -135,7 +213,7 @@ template <int kFmt>
 __global__ void __launch_bounds__(kThreads)
 stream_frame_in_kernel(const uint8_t* __restrict__ in, const int32_t* __restrict__ reset,
                        float* __restrict__ lr_curr, float* __restrict__ lr_prev, float* __restrict__ hr_prev,
-                       int c, int h, int w, int s, int bgr, int x_tiles, int decode_ctas, int zpc) {
+                       int c, int h, int w, int s, int bgr, int x_tiles, int decode_ctas, int zpc, int color) {
   // lr_curr, lr_prev and hr_prev belong to the previous step until it has finished
   tg_pdl_wait();
   tg_pdl_trigger();
@@ -145,7 +223,7 @@ stream_frame_in_kernel(const uint8_t* __restrict__ in, const int32_t* __restrict
     if constexpr (kFmt == kHWC)
       decode_hwc(in, lr_curr, b, t, c, h, w, bgr, x_tiles);
     else
-      decode_yuv420<kFmt>(in, lr_curr, b, t, h, w, x_tiles);
+      decode_yuv420<kFmt>(in, lr_curr, b, t, h, w, x_tiles, color);
     return;
   }
   const int rb = b - decode_ctas;
@@ -158,8 +236,8 @@ stream_frame_in_kernel(const uint8_t* __restrict__ in, const int32_t* __restrict
 }
 
 template <int kFmt>
-int launch_frame_in(const char* name, const uint8_t* in, const int32_t* reset, float* lr_curr, float* lr_prev,
-                    float* hr_prev, int n, int c, int h, int w, int s, int bgr, cudaStream_t stream) {
+int launch_frame_in(const char* name, const void* in, const int32_t* reset, float* lr_curr, float* lr_prev,
+                    float* hr_prev, int n, int c, int h, int w, int s, int bgr, int color, cudaStream_t stream) {
   TG_REQUIRE(in || reset, TG_E_INVALID, "%s: in_u8 and reset are both NULL", name);
   TG_REQUIRE(lr_curr && lr_prev && hr_prev, TG_E_INVALID, "%s: null pointer (lr_curr / lr_prev / hr_prev)", name);
   TG_REQUIRE(n > 0 && c > 0 && h > 0 && w > 0, TG_E_INVALID, "%s: bad size n=%d c=%d h=%d w=%d", name, n, c, h, w);
@@ -169,26 +247,36 @@ int launch_frame_in(const char* name, const uint8_t* in, const int32_t* reset, f
   TG_REQUIRE(s == 2 || s == 4, TG_E_UNSUPPORTED, "%s: scale %d (2 or 4)", name, s);
   TG_REQUIRE((((uintptr_t)lr_curr | (uintptr_t)lr_prev | (uintptr_t)hr_prev) & 3u) == 0, TG_E_INVALID,
              "%s: fp32 buffers must be 4-byte aligned", name);
+  TG_REQUIRE(!(kFmt == kP010 || kFmt == kI420_10) || ((uintptr_t)in & 1u) == 0, TG_E_INVALID,
+             "%s: 10-bit frames must be 2-byte aligned", name);
   const int x_tiles = tg_ceil_div(w, kTilePx);
   const size_t decode = in ? (size_t)x_tiles * (kFmt == kHWC ? h : h / 2) * n : 0;
   const size_t hr4 = (size_t)c * s * h * s * w / 4;
   const int zpc = reset ? (int)(hr4 / (kThreads * 8) + 1 < 64 ? hr4 / (kThreads * 8) + 1 : 64) : 0;
   const size_t ctas = decode + (size_t)zpc * n;
   TG_REQUIRE(ctas <= 0x7fffffff, TG_E_UNSUPPORTED, "%s: grid too large", name);
-  tg_launch(stream_frame_in_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), 0, stream, in, reset, lr_curr,
-            lr_prev, hr_prev, c, h, w, s, bgr, x_tiles, (int)decode, zpc);
+  tg_launch(stream_frame_in_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), 0, stream,
+            static_cast<const uint8_t*>(in), reset, lr_curr, lr_prev, hr_prev, c, h, w, s, bgr, x_tiles, (int)decode,
+            zpc, color);
   TG_CUDA_LAUNCH_CHECK(name);
   return TG_OK;
 }
 
-// one CTA: kTilePx pixels of the RGB rows 2*yp and 2*yp + 1 -> their Y bytes and the chroma bytes of the pair
-// (cv2 COLOR_RGB2YUV_I420: U and V of a 2x2 block from its top-left pixel)
-template <int kFmt>
+// one CTA: kTilePx pixels of the RGB rows 2*yp and 2*yp + 1 -> their Y words and the chroma words of the pair
+// (U and V of a 2x2 block from its top-left pixel, as cv2 COLOR_RGB2YUV_I420).  The source is the step's uint8
+// NHWC RGB (8-bit output; staged with 16-byte loads) or its fp32 NCHW HR frame (kF32, 10-bit output: coalesced
+// row reads of the three planes, q = clip(rint(x * 1023), 0, 1023)).  Colour row `color` of the table.
+template <int kFmt, bool kF32>
 __global__ void __launch_bounds__(kThreads)
-rgb_u8_to_yuv420_kernel(const uint8_t* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, int x_tiles) {
-  __shared__ __align__(16) uint8_t sin[2][kTilePx * 3 + 16];
-  __shared__ __align__(16) uint8_t sy[2][kTilePx + 16];
-  __shared__ __align__(16) uint8_t sc[2][kTilePx + 16];     // NV12: sc[0] = U V U V ...; I420: sc[0] = U, sc[1] = V
+rgb_to_yuv420_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, int x_tiles,
+                     int color) {
+  using F = Yuv<kFmt>;
+  using Wd = typename F::Word;
+  static_assert(kF32 == F::k10, "8-bit output reads uint8 RGB, 10-bit output the fp32 frame");
+  constexpr int kB = (int)sizeof(Wd);
+  __shared__ __align__(16) uint8_t sin[2][kF32 ? 16 : kTilePx * 3 + 16];
+  __shared__ __align__(16) uint8_t sy[2][kTilePx * kB + 16];
+  __shared__ __align__(16) uint8_t sc[2][kTilePx * kB + 16];   // NV12 layout: sc[0] = U V U V ...; I420: U, V
   // rgb is the previous kernel's output; out may still be read by the copy of an earlier step
   tg_pdl_wait();
   tg_pdl_trigger();
@@ -197,82 +285,173 @@ rgb_u8_to_yuv420_kernel(const uint8_t* __restrict__ rgb, uint8_t* __restrict__ o
   const int hp = H >> 1, yp = r % hp, img = r / hp;
   const int x0 = xt * kTilePx;
   const int npx = min(kTilePx, W - x0);                      // even
-  const uint8_t* src = rgb + (((size_t)img * H + 2 * yp) * W + x0) * 3;
-  const int li0 = stage_bytes(sin[0], src, npx * 3, t);
-  const int li1 = stage_bytes(sin[1], src + (size_t)W * 3, npx * 3, t);
-  uint8_t* frame = out + (size_t)img * (3 * hp) * W;
-  uint8_t* yrow = frame + (size_t)(2 * yp) * W + x0;
-  uint8_t* crow = frame + (size_t)H * W;
-  uint8_t *c0, *c1 = nullptr;
-  if (kFmt == kNV12) {
+  int li0 = 0, li1 = 0;
+  if constexpr (!kF32) {
+    const uint8_t* src = static_cast<const uint8_t*>(rgb) + (((size_t)img * H + 2 * yp) * W + x0) * 3;
+    li0 = stage_bytes(sin[0], src, npx * 3, t);
+    li1 = stage_bytes(sin[1], src + (size_t)W * 3, npx * 3, t);
+  }
+  Wd* frame = reinterpret_cast<Wd*>(out) + (size_t)img * (3 * hp) * W;
+  Wd* yrow = frame + (size_t)(2 * yp) * W + x0;
+  Wd* crow = frame + (size_t)H * W;
+  Wd *c0, *c1 = nullptr;
+  if (F::kInterleaved) {
     c0 = crow + (size_t)yp * W + x0;
   } else {
     c0 = crow + (size_t)yp * (W >> 1) + (x0 >> 1);
     c1 = c0 + (size_t)hp * (W >> 1);
   }
-  const int ly0 = lead_of(yrow), ly1 = lead_of(yrow + W), lc0 = lead_of(c0), lc1 = kFmt == kNV12 ? 0 : lead_of(c1);
-  __syncthreads();
+  const int ly0 = lead_of(yrow), ly1 = lead_of(yrow + W), lc0 = lead_of(c0), lc1 = F::kInterleaved ? 0 : lead_of(c1);
+  auto put = [](uint8_t* sb, int lead, int j, int v) { reinterpret_cast<Wd*>(sb + lead)[j] = F::word(v); };
+  const int* k = c_yuv.v[F::k10][color];
+  constexpr int kHalf = 1 << (F::kShift - 1);
+  const int yoff = k[15] << F::kShift;
+  constexpr int coff = F::kCoff << F::kShift;
+  auto q = [](int a) { return min(max(a >> F::kShift, 0), F::kTop); };
+  if constexpr (!kF32) __syncthreads();
   if (t < npx) {
 #pragma unroll
     for (int dy = 0; dy < 2; ++dy) {
-      const uint8_t* p = sin[dy] + (dy ? li1 : li0) + 3 * t;
-      const int R = p[0], G = p[1], B = p[2];
-      sy[dy][(dy ? ly1 : ly0) + t] =
-          (uint8_t)clamp_u8((kCRY * R + kCGY * G + kCBY * B + kHalf + (16 << kShift)) >> kShift);
+      int R, G, B;
+      if constexpr (kF32) {
+        const size_t plane = (size_t)H * W;
+        const float* p = static_cast<const float*>(rgb) + (size_t)img * 3 * plane + (size_t)(2 * yp + dy) * W + x0 + t;
+        auto q10 = [](float x) { return (int)fminf(fmaxf(rintf(x * 1023.f), 0.f), 1023.f); };
+        R = q10(__ldg(p));
+        G = q10(__ldg(p + plane));
+        B = q10(__ldg(p + 2 * plane));
+      } else {
+        const uint8_t* p = sin[dy] + (dy ? li1 : li0) + 3 * t;
+        R = p[0], G = p[1], B = p[2];
+      }
+      put(sy[dy], dy ? ly1 : ly0, t, q(k[0] * R + k[1] * G + k[2] * B + kHalf + yoff));
       if (dy == 0 && (t & 1) == 0) {
-        const uint8_t u = (uint8_t)clamp_u8((kCRU * R + kCGU * G + kCBU * B + kHalf + (128 << kShift)) >> kShift);
-        const uint8_t v = (uint8_t)clamp_u8((kCRV * R + kCGV * G + kCBV * B + kHalf + (128 << kShift)) >> kShift);
-        if (kFmt == kNV12) {
-          sc[0][lc0 + t] = u;
-          sc[0][lc0 + t + 1] = v;
+        const int u = q(k[3] * R + k[4] * G + k[5] * B + kHalf + coff);
+        const int v = q(k[6] * R + k[7] * G + k[8] * B + kHalf + coff);
+        if (F::kInterleaved) {
+          put(sc[0], lc0, t, u);
+          put(sc[0], lc0, t + 1, v);
         } else {
-          sc[0][lc0 + (t >> 1)] = u;
-          sc[1][lc1 + (t >> 1)] = v;
+          put(sc[0], lc0, t >> 1, u);
+          put(sc[1], lc1, t >> 1, v);
         }
       }
     }
   }
   __syncthreads();
-  flush_bytes(yrow, sy[0], npx, t);
-  flush_bytes(yrow + W, sy[1], npx, t);
-  if (kFmt == kNV12) {
-    flush_bytes(c0, sc[0], npx, t);
+  auto flush = [&](Wd* dst, const uint8_t* sb, int words) {
+    flush_bytes(reinterpret_cast<uint8_t*>(dst), sb, words * kB, t);
+  };
+  flush(yrow, sy[0], npx);
+  flush(yrow + W, sy[1], npx);
+  if (F::kInterleaved) {
+    flush(c0, sc[0], npx);
   } else {
-    flush_bytes(c0, sc[0], npx >> 1, t);
-    flush_bytes(c1, sc[1], npx >> 1, t);
+    flush(c0, sc[0], npx >> 1);
+    flush(c1, sc[1], npx >> 1);
   }
+}
+
+template <int kFmt>
+int launch_to_yuv(const char* name, const void* rgb, void* out, int n, int H, int W, int color,
+                  cudaStream_t stream) {
+  TG_REQUIRE(n > 0 && H > 0 && W > 0, TG_E_INVALID, "%s: bad size n=%d H=%d W=%d", name, n, H, W);
+  TG_REQUIRE(H % 2 == 0 && W % 2 == 0, TG_E_UNSUPPORTED,
+             "%s: YUV 4:2:0 needs an even height and width, got %dx%d", name, H, W);
+  const int x_tiles = tg_ceil_div(W, kTilePx);
+  const size_t ctas = (size_t)x_tiles * (H / 2) * n;
+  TG_REQUIRE(ctas <= 0x7fffffff, TG_E_UNSUPPORTED, "%s: grid too large", name);
+  constexpr bool k10 = Yuv<kFmt>::k10;
+  tg_launch(rgb_to_yuv420_kernel<kFmt, k10>, dim3((unsigned)ctas), dim3(kThreads), 0, stream, rgb,
+            static_cast<uint8_t*>(out), H, W, x_tiles, color);
+  TG_CUDA_LAUNCH_CHECK(name);
+  return TG_OK;
+}
+
+// tg_yuv_format -> (frame format, colour row)
+int parse_yuv_format(const char* name, const tg_yuv_format* f, int* fmt, int* color) {
+  TG_REQUIRE(f, TG_E_INVALID, "%s: null format", name);
+  TG_REQUIRE(f->reserved == 0, TG_E_INVALID, "%s: format.reserved must be 0, got %d", name, f->reserved);
+  TG_REQUIRE(f->full_range == 0 || f->full_range == 1, TG_E_INVALID, "%s: format.full_range must be 0 or 1, got %d",
+             name, f->full_range);
+  TG_REQUIRE(f->matrix == 601 || f->matrix == 709, TG_E_UNSUPPORTED, "%s: matrix %d (601 or 709)", name, f->matrix);
+  switch (f->layout) {
+    case TG_YUV_NV12: *fmt = kNV12; break;
+    case TG_YUV_I420: *fmt = kI420; break;
+    case TG_YUV_P010: *fmt = kP010; break;
+    case TG_YUV_I420_10: *fmt = kI420_10; break;
+    default: TG_REQUIRE(false, TG_E_UNSUPPORTED, "%s: unknown layout %d", name, f->layout);
+  }
+  *color = (f->matrix == 709 ? 1 : 0) + 2 * f->full_range;
+  return TG_OK;
 }
 
 }  // namespace
 
 extern "C" int tg_stream_frame_in(const uint8_t* in_u8, const int32_t* reset, float* lr_curr, float* lr_prev,
                                   float* hr_prev, int n, int c, int h, int w, int s, int bgr, void* stream) {
-  return launch_frame_in<kHWC>("stream_frame_in", in_u8, reset, lr_curr, lr_prev, hr_prev, n, c, h, w, s, bgr,
+  return launch_frame_in<kHWC>("stream_frame_in", in_u8, reset, lr_curr, lr_prev, hr_prev, n, c, h, w, s, bgr, 0,
                                (cudaStream_t)stream);
 }
 
 extern "C" int tg_stream_frame_in_yuv420(const uint8_t* in, int nv12, const int32_t* reset, float* lr_curr,
                                          float* lr_prev, float* hr_prev, int n, int h, int w, int s, void* stream) {
   return nv12 ? launch_frame_in<kNV12>("stream_frame_in_yuv420", in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w,
-                                       s, 0, (cudaStream_t)stream)
+                                       s, 0, 0, (cudaStream_t)stream)
               : launch_frame_in<kI420>("stream_frame_in_yuv420", in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w,
-                                       s, 0, (cudaStream_t)stream);
+                                       s, 0, 0, (cudaStream_t)stream);
 }
 
 extern "C" int tg_rgb_u8_to_yuv420(const uint8_t* rgb, uint8_t* out, int nv12, int n, int H, int W, void* stream) {
   TG_REQUIRE(rgb && out, TG_E_INVALID, "rgb_u8_to_yuv420: null pointer (rgb / out)");
-  TG_REQUIRE(n > 0 && H > 0 && W > 0, TG_E_INVALID, "rgb_u8_to_yuv420: bad size n=%d H=%d W=%d", n, H, W);
-  TG_REQUIRE(H % 2 == 0 && W % 2 == 0, TG_E_UNSUPPORTED,
-             "rgb_u8_to_yuv420: YUV 4:2:0 needs an even height and width, got %dx%d", H, W);
-  const int x_tiles = tg_ceil_div(W, kTilePx);
-  const size_t ctas = (size_t)x_tiles * (H / 2) * n;
-  TG_REQUIRE(ctas <= 0x7fffffff, TG_E_UNSUPPORTED, "rgb_u8_to_yuv420: grid too large");
-  if (nv12)
-    tg_launch(rgb_u8_to_yuv420_kernel<kNV12>, dim3((unsigned)ctas), dim3(kThreads), 0, (cudaStream_t)stream, rgb,
-              out, H, W, x_tiles);
-  else
-    tg_launch(rgb_u8_to_yuv420_kernel<kI420>, dim3((unsigned)ctas), dim3(kThreads), 0, (cudaStream_t)stream, rgb,
-              out, H, W, x_tiles);
-  TG_CUDA_LAUNCH_CHECK("rgb_u8_to_yuv420");
+  return nv12 ? launch_to_yuv<kNV12>("rgb_u8_to_yuv420", rgb, out, n, H, W, 0, (cudaStream_t)stream)
+              : launch_to_yuv<kI420>("rgb_u8_to_yuv420", rgb, out, n, H, W, 0, (cudaStream_t)stream);
+}
+
+extern "C" int tg_stream_frame_in_yuv(const void* in, const tg_yuv_format* fmt, const int32_t* reset, float* lr_curr,
+                                      float* lr_prev, float* hr_prev, int n, int h, int w, int s, void* stream) {
+  const char* name = "stream_frame_in_yuv";
+  int f = 0, color = 0;
+  const int rc = parse_yuv_format(name, fmt, &f, &color);
+  if (rc != TG_OK) return rc;
+  const cudaStream_t st = (cudaStream_t)stream;
+  switch (f) {
+    case kNV12: return launch_frame_in<kNV12>(name, in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w, s, 0, color, st);
+    case kI420: return launch_frame_in<kI420>(name, in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w, s, 0, color, st);
+    case kP010: return launch_frame_in<kP010>(name, in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w, s, 0, color, st);
+    default:
+      return launch_frame_in<kI420_10>(name, in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w, s, 0, color, st);
+  }
+}
+
+extern "C" int tg_rgb_to_yuv(const uint8_t* rgb_u8, const float* rgb_f32, void* out, const tg_yuv_format* fmt, int n,
+                             int H, int W, void* stream) {
+  const char* name = "rgb_to_yuv";
+  int f = 0, color = 0;
+  const int rc = parse_yuv_format(name, fmt, &f, &color);
+  if (rc != TG_OK) return rc;
+  const bool ten = f == kP010 || f == kI420_10;
+  TG_REQUIRE(out, TG_E_INVALID, "%s: null pointer (out)", name);
+  TG_REQUIRE(ten ? (rgb_f32 && !rgb_u8) : (rgb_u8 && !rgb_f32), TG_E_INVALID,
+             "%s: %s output is encoded from %s (and only that source)", name, ten ? "10-bit" : "8-bit",
+             ten ? "rgb_f32" : "rgb_u8");
+  TG_REQUIRE(!ten || ((((uintptr_t)rgb_f32) & 3u) == 0 && (((uintptr_t)out) & 1u) == 0), TG_E_INVALID,
+             "%s: rgb_f32 must be 4-byte and 10-bit output 2-byte aligned", name);
+  const cudaStream_t st = (cudaStream_t)stream;
+  switch (f) {
+    case kNV12: return launch_to_yuv<kNV12>(name, rgb_u8, out, n, H, W, color, st);
+    case kI420: return launch_to_yuv<kI420>(name, rgb_u8, out, n, H, W, color, st);
+    case kP010: return launch_to_yuv<kP010>(name, rgb_f32, out, n, H, W, color, st);
+    default: return launch_to_yuv<kI420_10>(name, rgb_f32, out, n, H, W, color, st);
+  }
+}
+
+extern "C" int tg_yuv_coefficients(const tg_yuv_format* fmt, int32_t* out16) {
+  int f = 0, color = 0;
+  const int rc = parse_yuv_format("yuv_coefficients", fmt, &f, &color);
+  if (rc != TG_OK) return rc;
+  TG_REQUIRE(out16, TG_E_INVALID, "yuv_coefficients: null pointer (out16)");
+  const int* r = kYuvTable.v[(f == kP010 || f == kI420_10) ? 1 : 0][color];
+  for (int k = 0; k < 16; ++k) out16[k] = r[k];
   return TG_OK;
 }

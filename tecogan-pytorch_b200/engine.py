@@ -222,23 +222,32 @@ class StreamEngine(ClipEngine):
     the device mask mask[p] -- the reset of one slot happens inside the captured step, and one graph serves every
     pattern of resets.  The step itself is the unchanged net.step_into.
 
-    YUV 4:2:0 input (yuv_in = 'nv12' / 'i420'): inp[p] holds [n,3h/2,w] frames and the first launch is
-    tg_stream_frame_in_yuv420 instead, with the same reset.  YUV output (yuv_out): each graph ends with
-    tg_rgb_u8_to_yuv420 of u8[p] into yuv[p] [n,3H/2,W], and the copies out read yuv[p] instead of u8[p].
+    YUV 4:2:0 input (yuv_in = 'nv12' / 'i420' / 'p010' / 'i420_10'): inp[p] holds [n,3h/2,w] frames (uint16 for
+    the 10-bit layouts) and the first launch is tg_stream_frame_in_yuv420 (8 bit, BT.601 limited range: cv2's
+    conversion) or tg_stream_frame_in_yuv (any other layout or colour) instead, with the same reset.  YUV output
+    (yuv_out): each graph ends with the encode into yuv[p] [n,3H/2,W] -- tg_rgb_u8_to_yuv420 of u8[p] (8 bit,
+    BT.601 limited range), tg_rgb_to_yuv of u8[p] (8 bit, other colours) or tg_rgb_to_yuv of the fp32 HR frame
+    hr[p] (10 bit, uint16 yuv[p]) -- and the copies out read yuv[p] instead of u8[p].
 
     Copies overlap compute as in ClipEngine.run_clips.  uint8 input: inp[p] is itself the 2-deep staging ring (the
     step of parity p^1 never reads it), so the H2D of frame i+1 lands directly in the graph's input while frame i
     runs.  fp32 input: lr[p] is still read as lr_prev by frame i, so frames are staged as in run_clips."""
 
-    def __init__(self, net, n, c, h, w, device, u8_input=True, bgr=False, yuv_in=None, yuv_out=None):
+    def __init__(self, net, n, c, h, w, device, u8_input=True, bgr=False, yuv_in=None, yuv_out=None,
+                 in_color='bt601', out_color='bt601'):
         dev = torch.device(device)
         self.u8_input, self.bgr = u8_input or yuv_in is not None, bgr
-        self.yuv_in, self.yuv_out = yuv_in, yuv_out          # None, 'nv12' or 'i420'
+        self.yuv_in, self.yuv_out = yuv_in, yuv_out          # None or one of ops.YUV_LAYOUTS
+        self.in_color, self.out_color = in_color, out_color
         self.mask = [torch.zeros(n, dtype=torch.int32, device=dev) for _ in range(2)]
         frame = (3 * h // 2, w) if yuv_in else (h, w, c)
-        self.inp = [torch.zeros(n, *frame, dtype=torch.uint8, device=dev) for _ in range(2)] if self.u8_input else None
+        # 10-bit words: zeroed as int16, the same bits
+        in_dtype = torch.int16 if yuv_in and ops.yuv_depth(yuv_in) == 10 else torch.uint8
+        self.inp = ([torch.zeros(n, *frame, dtype=in_dtype, device=dev).view(_word_dtype(yuv_in)) for _ in range(2)]
+                    if self.u8_input else None)
         H, W = net.scale * h, net.scale * w
-        self.yuv = [torch.empty(n, 3 * H // 2, W, dtype=torch.uint8, device=dev) for _ in range(2)] if yuv_out else None
+        self.yuv = ([torch.empty(n, 3 * H // 2, W, dtype=_word_dtype(yuv_out), device=dev) for _ in range(2)]
+                    if yuv_out else None)
         self.sig = _param_signature(net)
         self.parity = 0                  # parity of the next frame
         self.mask_set = [False, False]   # mask[p] holds a reset pattern (cleared before the next replay)
@@ -251,15 +260,23 @@ class StreamEngine(ClipEngine):
         self.mask, self.inp, self.yuv = [], None, None
 
     def _enqueue(self, p):
-        if self.yuv_in:
+        if self.yuv_in in YUV420 and self.in_color == 'bt601':
             ops.stream_frame_in_yuv420(self.inp[p], self.yuv_in, self.mask[p], self.lr[p], self.lr[p ^ 1],
                                        self.hr[p ^ 1], self.net.scale)
+        elif self.yuv_in:
+            ops.stream_frame_in_yuv(self.inp[p], self.yuv_in, self.in_color, self.mask[p], self.lr[p],
+                                    self.lr[p ^ 1], self.hr[p ^ 1], self.net.scale)
         else:
             ops.stream_frame_in(self.inp[p] if self.u8_input else None, self.mask[p], self.lr[p], self.lr[p ^ 1],
                                 self.hr[p ^ 1], self.net.scale, self.bgr)
         super()._enqueue(p)
-        if self.yuv_out:
+        if self.yuv_out in YUV420 and self.out_color == 'bt601':
             ops.rgb_u8_to_yuv420(self.u8[p], self.yuv_out, out=self.yuv[p])
+        elif self.yuv_out and ops.yuv_depth(self.yuv_out) == 8:
+            ops.rgb_to_yuv(self.yuv_out, self.out_color, rgb_u8=self.u8[p], out=self.yuv[p])
+        elif self.yuv_out:
+            # 10 bit: from the step's fp32 HR frame, two more bits than the uint8 output keeps
+            ops.rgb_to_yuv(self.yuv_out, self.out_color, rgb_f32=self.hr[p], out=self.yuv[p])
 
     def _set_mask(self, p, slots):
         """On the main stream, before the replay of parity p: mask[p] = 1 for `slots`, 0 elsewhere."""
@@ -273,9 +290,9 @@ class StreamEngine(ClipEngine):
             self.mask_set[p] = False
 
     def run(self, frames, reset_slots, out_host):
-        """frames: uint8 [n,k,h,w,c] (u8_input), uint8 [n,k,3h/2,w] (yuv_in) or fp32 [n,k,c,h,w], each frame
-        contiguous, pinned host or on this device.
-        Slots in `reset_slots` start a new video at frame 0.  Returns uint8 [n,k,H,W,c] (or [n,k,3H/2,W] with
+        """frames: uint8 [n,k,h,w,c] (u8_input), uint8 / uint16 [n,k,3h/2,w] (yuv_in) or fp32 [n,k,c,h,w], each
+        frame contiguous, pinned host or on this device.
+        Slots in `reset_slots` start a new video at frame 0.  Returns uint8 [n,k,H,W,c] (or [n,k,3H/2,W] words with
         yuv_out): a pinned host tensor (out_host; one synchronisation, at the end) or a new tensor on the device,
         ordered on the current stream (no synchronisation)."""
         n, k = self.n, frames.shape[1]
@@ -287,9 +304,9 @@ class StreamEngine(ClipEngine):
             res = self.yuv if self.yuv_out else self.u8      # what the step graph leaves for the copy out
             shape = (n, k, *res[0].shape[1:])
             if out_host:
-                out = torch.empty(shape, dtype=torch.uint8, pin_memory=True)
+                out = torch.empty(shape, dtype=res[0].dtype, pin_memory=True)
             else:
-                out = torch.empty(shape, dtype=torch.uint8, device=self.device)
+                out = torch.empty(shape, dtype=res[0].dtype, device=self.device)
             if not self.u8_input and self.stage is None:
                 self.stage = [torch.empty_like(self.lr[0]) for _ in range(2)]
             dst = self.inp if self.u8_input else self.stage
@@ -332,24 +349,36 @@ class StreamEngine(ClipEngine):
 
 
 YUV420 = ops.YUV420_LAYOUTS       # 'nv12', 'i420'
+YUV = ops.YUV_LAYOUTS             # those and the 10-bit 'p010', 'i420_10'
+COLORS = ops.YUV_COLORS           # 'bt601' (the default, cv2's conversion), 'bt709', 'bt601-full', 'bt709-full'
+
+
+def _word_dtype(layout):
+    return torch.uint16 if layout and ops.yuv_depth(layout) == 10 else torch.uint8
 
 
 class VideoStream:
     """n lock-stepped video slots through FRNet with the recurrent state carried between `push` calls.
     Created by FRNet.stream(); see there."""
 
-    def __init__(self, net, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb'):
-        if input not in ('uint8', 'float32', *YUV420):
-            raise ValueError(f"input must be 'uint8', 'float32', 'nv12' or 'i420', got {input!r}")
+    def __init__(self, net, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb',
+                 in_color='bt601', out_color='bt601'):
+        if input not in ('uint8', 'float32', *YUV):
+            raise ValueError(f"input must be 'uint8', 'float32' or one of {YUV}, got {input!r}")
         if channel_order not in ('rgb', 'bgr'):
             raise ValueError(f"channel_order must be 'rgb' or 'bgr', got {channel_order!r}")
-        if out_format not in ('rgb', *YUV420):
-            raise ValueError(f"out_format must be 'rgb', 'nv12' or 'i420', got {out_format!r}")
+        if out_format not in ('rgb', *YUV):
+            raise ValueError(f"out_format must be 'rgb' or one of {YUV}, got {out_format!r}")
+        for arg, color, side in (('in_color', in_color, input), ('out_color', out_color, out_format)):
+            if not isinstance(color, str) or color not in COLORS:
+                raise ValueError(f'{arg} must be one of {COLORS}, got {color!r}')
+            if side not in YUV and color != 'bt601':
+                raise ValueError(f'{arg}={color!r} applies to YUV frames only, not to {side!r}')
         if input != 'uint8' and channel_order != 'rgb':
             raise ValueError(f"channel_order='bgr' applies to uint8 HWC input only, not input={input!r}")
         if not all(isinstance(v, int) and v > 0 for v in (n, h, w)):
             raise ValueError(f'n, h, w must be positive ints, got {(n, h, w)}')
-        yuv = [f for f in (input, out_format) if f in YUV420]
+        yuv = [f for f in (input, out_format) if f in YUV]
         if yuv and (h % 2 or w % 2):
             raise ValueError(f'{yuv[0]} frames are YUV 4:2:0: h and w must be even, got {h}x{w}')
         if yuv and net.fnet.in_nc != 3:
@@ -360,6 +389,7 @@ class VideoStream:
         self.net, self.n, self.h, self.w = net, n, h, w
         self.c = net.fnet.in_nc
         self.device, self.input, self.channel_order, self.out_format = device, input, channel_order, out_format
+        self.in_color, self.out_color = in_color, out_color
         self._engine = None                  # built (graphs captured) by the first push
         self._pending = [True] * n           # a new stream starts every slot from zero state
         _check_inference(net)
@@ -390,7 +420,9 @@ class VideoStream:
         out:    'host' -> NumPy uint8 [n,k,H,W,c] (one synchronisation); 'device' -> a new CUDA uint8 tensor
                 [n,k,H,W,c], ordered on the current stream (no synchronisation; a pinned host input must then
                 stay unchanged until that stream has passed this push).  With out_format 'nv12' / 'i420' the
-                frames are uint8 [n,k,3H/2,W] instead.
+                frames are uint8 [n,k,3H/2,W] instead, with 'p010' / 'i420_10' uint16 [n,k,3H/2,W].
+        10-bit input ('p010', 'i420_10') takes uint16 frames [n,k,3h/2,w] ([k,3h/2,w] when n == 1), torch.uint16 or
+        NumPy uint16; uint8 frames into a 10-bit stream raise, and so do uint16 frames into an 8-bit one.
         """
         if self._engine is False:
             raise ops.L.TecoganB200Error('VideoStream.push: the stream is closed')
@@ -425,7 +457,7 @@ class VideoStream:
             frames = torch.from_numpy(frames)
         if not isinstance(frames, torch.Tensor):
             raise TypeError(f'VideoStream.push: frames must be a tensor or ndarray, got {type(frames).__name__}')
-        dtype = torch.float32 if self.input == 'float32' else torch.uint8
+        dtype = torch.float32 if self.input == 'float32' else _word_dtype(self.input if self.input in YUV else None)
         if frames.dtype != dtype:
             raise L.TecoganB200Error(f'VideoStream.push: {self.input} stream expects {dtype} frames, got '
                                      f'{frames.dtype}')
@@ -460,10 +492,11 @@ class VideoStream:
             raise ops.L.TecoganB200Error(f'VideoStream: the net\'s parameters are on {pdev}, the stream runs on '
                                          f'{dev}; move the net first (net.to(device))')
         self.device = dev
-        yuv_in = self.input if self.input in YUV420 else None
-        yuv_out = self.out_format if self.out_format in YUV420 else None
+        yuv_in = self.input if self.input in YUV else None
+        yuv_out = self.out_format if self.out_format in YUV else None
         return StreamEngine(self.net, self.n, self.c, self.h, self.w, dev, u8_input=self.input == 'uint8',
-                            bgr=self.channel_order == 'bgr', yuv_in=yuv_in, yuv_out=yuv_out)
+                            bgr=self.channel_order == 'bgr', yuv_in=yuv_in, yuv_out=yuv_out,
+                            in_color=self.in_color, out_color=self.out_color)
 
 
 def _check_inference(net):

@@ -18,6 +18,7 @@ CONV_3X3, CONVT_3X3_S2, CONV_3X3_S2 = 0, 1, 2
 UP_BICUBIC, UP_BILINEAR = 0, 1
 EPI_NHWC_F16, EPI_FLOW_NCHW_F32, EPI_OUT_NCHW_F32, EPI_NHWC_F16_POOL2 = 0, 1, 2, 3
 AMODE_AUTO, AMODE_HALO, AMODE_TAP = 0, 1, 2
+YUV_NV12, YUV_I420, YUV_P010, YUV_I420_10 = 0, 1, 2, 3
 
 
 class ConvDesc(ctypes.Structure):
@@ -62,6 +63,11 @@ class TailDesc(ctypes.Structure):
     ]
 
 
+class YuvFormat(ctypes.Structure):
+    """struct tg_yuv_format"""
+    _fields_ = [('layout', c_int32), ('matrix', c_int32), ('full_range', c_int32), ('reserved', c_int32)]
+
+
 CHAIN_MAX_LAYERS = 24
 
 _P = c_void_p
@@ -95,6 +101,9 @@ _SIGNATURES = {
     'tg_stream_frame_in': (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_stream_frame_in_yuv420': (c_int, [_P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'tg_rgb_u8_to_yuv420': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
+    'tg_stream_frame_in_yuv': (c_int, [_P, ctypes.POINTER(YuvFormat), _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
+    'tg_rgb_to_yuv': (c_int, [_P, _P, _P, ctypes.POINTER(YuvFormat), c_int, c_int, c_int, _P]),
+    'tg_yuv_coefficients': (c_int, [ctypes.POINTER(YuvFormat), ctypes.POINTER(c_int32)]),
     'tg_downsample_bd_nchw_f32': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_debug_set_conv_timers': (c_int, [_P]),
     # ---- training (generator backward)

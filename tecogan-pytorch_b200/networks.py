@@ -355,7 +355,8 @@ class FRNet(BaseSequenceGenerator):
             return infer_clips(self, lr_data.unsqueeze(0), device)[0]
         return infer_clips(self, lr_data, device)
 
-    def stream(self, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb'):
+    def stream(self, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb', in_color='bt601',
+               out_color='bt601'):
         """A VideoStream of n lock-stepped slots of h x w LR frames: video pushed in chunks of any length, the
         recurrent state carried from one push to the next, and a slot restarted (reset=) when its video ends and
         the next one begins while the other slots keep running.
@@ -372,11 +373,20 @@ class FRNet(BaseSequenceGenerator):
         cv2.cvtColor(rgb, COLOR_RGB2YUV_I420) of the RGB output (chroma of each 2x2 block from its top-left
         pixel), for 'nv12' with U and V interleaved.  Both need even h and w; any input works with any
         out_format.
+        10-bit video: 'p010' (NV12 planes, uint16 words, sample in the high 10 bits; NVDEC / NVENC, ffmpeg p010le)
+        and 'i420_10' (I420 planes, uint16 words, sample in the low 10 bits; ffmpeg / PyAV yuv420p10le), as input
+        (uint16 [n,k,3h/2,w], converted to RGB / 1023) or out_format (uint16 [n,k,3H/2,W], encoded from the fp32 HR
+        frame, so the two bits below the uint8 output are kept).
+        in_color / out_color pick the YUV side's colour: 'bt601' (the default, limited range; for 8-bit frames
+        exactly cv2's conversion), 'bt709', 'bt601-full', 'bt709-full' (ITU-T H.273 quantisation, integer fixed
+        point as oracle/yuv_color.py specifies).  Take in_color from the decoder (ffprobe's color_space /
+        color_range) and tag the encoded output with out_color.  A colour other than 'bt601' on an RGB or float32
+        side raises ValueError.
         Temporal padding (pad_sequence, base_model.py:230-251) stays the caller's job: for p reflect-padded
         frames, push frames[:, 1:1+p].flip(1) first and drop those p outputs.  The CUDA graphs are captured by the first push; the stream holds the
         net."""
         from .engine import VideoStream
-        return VideoStream(self, n, h, w, device, input, channel_order, out_format)
+        return VideoStream(self, n, h, w, device, input, channel_order, out_format, in_color, out_color)
 
     def refresh_packed_weights(self, force=False):
         self.fnet._cache.refresh_all(force)

@@ -497,6 +497,100 @@ def rgb_u8_to_yuv420(rgb, layout, out=None):
     return out
 
 
+YUV_LAYOUTS = ('nv12', 'i420', 'p010', 'i420_10')      # 8-bit uint8 words; 10-bit uint16 words
+YUV_COLORS = ('bt601', 'bt709', 'bt601-full', 'bt709-full')
+_LAYOUT_CODE = {'nv12': L.YUV_NV12, 'i420': L.YUV_I420, 'p010': L.YUV_P010, 'i420_10': L.YUV_I420_10}
+
+
+def yuv_depth(layout):
+    """Bit depth of a YUV layout: 8 (uint8 frames) or 10 (uint16 frames)."""
+    return 10 if layout in ('p010', 'i420_10') else 8
+
+
+def yuv_format(layout, color, name='yuv_format'):
+    """(layout, colour) names -> struct tg_yuv_format."""
+    if layout not in YUV_LAYOUTS:
+        raise L.TecoganB200Error(f'{name}: layout must be one of {YUV_LAYOUTS}, got {layout!r}')
+    if color not in YUV_COLORS:
+        raise L.TecoganB200Error(f'{name}: colour must be one of {YUV_COLORS}, got {color!r}')
+    return L.YuvFormat(_LAYOUT_CODE[layout], 709 if color.startswith('bt709') else 601,
+                       int(color.endswith('-full')), 0)
+
+
+def yuv_coefficients(layout, color):
+    """tg_yuv_coefficients: the 16 int32 of the kernels' colour table row (host only, no GPU needed)."""
+    out = (ctypes.c_int32 * 16)()
+    L.check(L.load().tg_yuv_coefficients(ctypes.byref(yuv_format(layout, color, 'yuv_coefficients')), out),
+            'tg_yuv_coefficients')
+    return list(out)
+
+
+def stream_frame_in_yuv(frames, layout, color, reset, lr_curr, lr_prev, hr_prev, scale):
+    """tg_stream_frame_in_yuv: frames [n,3h/2,w] (uint8 for 'nv12' / 'i420', uint16 for 'p010' / 'i420_10'; or
+    None) in colour `color` -> lr_curr fp32 [n,3,h,w] = RGB / 255 (8 bit) or RGB / 1023 (10 bit), as
+    oracle/yuv_color.py; reset as in stream_frame_in."""
+    name = 'stream_frame_in_yuv'
+    fmt = yuv_format(layout, color, name)
+    _req(lr_curr, torch.float32, 'lr_curr', 4)
+    _req(lr_prev, torch.float32, 'lr_prev', 4)
+    _req(hr_prev, torch.float32, 'hr_prev', 4)
+    n, c, h, w = lr_curr.shape
+    if c != 3:
+        raise L.TecoganB200Error(f'{name}: lr_curr has {c} channels, YUV frames decode to 3')
+    if h % 2 or w % 2:
+        raise L.TecoganB200Error(f'{name}: YUV 4:2:0 needs an even height and width, got {h}x{w}')
+    if tuple(lr_prev.shape) != (n, c, h, w) or tuple(hr_prev.shape) != (n, c, scale * h, scale * w):
+        raise L.TecoganB200Error(f'{name}: lr_prev / hr_prev shape mismatch')
+    if frames is not None:
+        _req(frames, torch.uint16 if yuv_depth(layout) == 10 else torch.uint8, 'frames', 3)
+        if tuple(frames.shape) != (n, 3 * h // 2, w):
+            raise L.TecoganB200Error(f'{name}: frames {tuple(frames.shape)} != {(n, 3 * h // 2, w)} ([n,3h/2,w])')
+    if reset is not None:
+        _req(reset, torch.int32, 'reset', 1)
+        if reset.shape[0] != n:
+            raise L.TecoganB200Error(f'{name}: reset has {reset.shape[0]} entries, expected {n}')
+    for t in (lr_prev, hr_prev, frames, reset):
+        if t is not None and t.device != lr_curr.device:
+            raise L.TecoganB200Error(f'{name}: tensors on different devices')
+    L.check(L.load().tg_stream_frame_in_yuv(_ptr(frames), ctypes.byref(fmt), _ptr(reset), _ptr(lr_curr),
+                                            _ptr(lr_prev), _ptr(hr_prev), n, h, w, scale, _stream()),
+            'tg_stream_frame_in_yuv')
+    return lr_curr
+
+
+def rgb_to_yuv(layout, color, rgb_u8=None, rgb_f32=None, out=None):
+    """tg_rgb_to_yuv: 8-bit layouts encode rgb_u8 (uint8 NHWC [n,H,W,3]) into uint8 [n,3H/2,W]; 10-bit layouts
+    encode rgb_f32 (fp32 NCHW [n,3,H,W], quantised as clip(rint(x * 1023), 0, 1023)) into uint16 [n,3H/2,W]."""
+    name = 'rgb_to_yuv'
+    fmt = yuv_format(layout, color, name)
+    ten = yuv_depth(layout) == 10
+    if ten:
+        if rgb_f32 is None or rgb_u8 is not None:
+            raise L.TecoganB200Error(f'{name}: 10-bit {layout} is encoded from rgb_f32 (fp32 NCHW) only')
+        src = _req(rgb_f32, torch.float32, 'rgb_f32', 4)
+        n, c, H, W = src.shape
+    else:
+        if rgb_u8 is None or rgb_f32 is not None:
+            raise L.TecoganB200Error(f'{name}: 8-bit {layout} is encoded from rgb_u8 (uint8 NHWC) only')
+        src = _req(rgb_u8, torch.uint8, 'rgb_u8', 4)
+        n, H, W, c = src.shape
+    if c != 3:
+        raise L.TecoganB200Error(f'{name}: expected 3 colour channels, got {tuple(src.shape)}')
+    if H % 2 or W % 2:
+        raise L.TecoganB200Error(f'{name}: YUV 4:2:0 needs an even height and width, got {H}x{W}')
+    dtype = torch.uint16 if ten else torch.uint8
+    if out is None:
+        out = torch.empty((n, 3 * H // 2, W), dtype=dtype, device=src.device)
+    _req(out, dtype, 'out', 3)
+    if tuple(out.shape) != (n, 3 * H // 2, W):
+        raise L.TecoganB200Error(f'{name}: out {tuple(out.shape)} != {(n, 3 * H // 2, W)}')
+    if out.device != src.device:
+        raise L.TecoganB200Error(f'{name}: tensors on different devices')
+    L.check(L.load().tg_rgb_to_yuv(_ptr(rgb_u8), _ptr(rgb_f32), _ptr(out), ctypes.byref(fmt), n, H, W, _stream()),
+            'tg_rgb_to_yuv')
+    return out
+
+
 # ============================================================================ training (backward) ops
 class GradScale:
     """Device-resident loss scale {scale, 1/scale} of the fp16 gradient path (tg_grad_scale_from_amax /

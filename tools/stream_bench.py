@@ -12,13 +12,19 @@ each run ends in a device synchronisation; one untimed warm-up run of every path
   push_nv12_host_chunk1/16   VideoStream.push(pinned NV12 [n,k,3h/2,w], out='host') of an input='nv12',
                              out_format='nv12' stream -> NV12 [n,k,3H/2,W], k = 1 / 16
   push_nv12_device           the same with NV12 on the device and out='device', k = 16
+  push_p010_709_host_chunk16 a P010 / BT.709 -> P010 / BT.709 stream (uint16 [n,k,3h/2,w] -> [n,k,3H/2,W]), k = 16
+  push_nv12_601_709_host_chunk16  an NV12 / BT.601 -> NV12 / BT.709 stream, k = 16
   frame_in_us                tg_stream_frame_in per step (decode of 4 frames, zero reset mask; and with every
                              slot reset) and tg_stream_frame_in_yuv420 per step (NV12, I420), CUDA events over a
                              graph of launches on rotating buffers
-  encode_us                  tg_rgb_u8_to_yuv420 per step (4 HR frames -> NV12 / I420), timed the same way
+                             and tg_stream_frame_in_yuv per step (P010 / BT.709)
+  encode_us                  tg_rgb_u8_to_yuv420 per step (4 HR frames -> NV12 / I420) and tg_rgb_to_yuv per step
+                             (uint8 -> NV12 / BT.709; fp32 NCHW -> P010 / BT.709), timed the same way
 All uint8 paths process the same frames (uint8, and the reference loader's float32 / 255 of them), so their
 outputs are also compared byte for byte.  The NV12 paths take oracle/yuv_oracle.py's NV12 of those frames; their
-output is compared with the oracle's NV12 of the RGB output for the frames that NV12 decodes to.  Card name and
+output is compared with the oracle's NV12 of the RGB output for the frames that NV12 decodes to; the BT.709 NV12
+output with oracle/yuv_color.py's BT.709 encode of that RGB output, and the P010 output with its encode of the fp32 HR
+frames of a device loop of FRNet.step over the frames P010 decodes to.  Card name and
 power limit are read in the same run.  Writes nothing."""
 import argparse
 import json
@@ -53,6 +59,7 @@ def main():
     import bench
     import tecogan_b200 as T
     from oracle import yuv_oracle as Y
+    from oracle import yuv_color as C
     ops = sys.modules['tecogan-pytorch_b200.ops']
     assert torch.cuda.is_available(), 'stream_bench.py needs a GPU'
     dev = torch.device('cuda', 0)
@@ -72,6 +79,8 @@ def main():
     nv12 = Y.rgb_to_yuv420(u8, 'nv12')                                                # [n,t,3h/2,w]
     nv12_pin = torch.from_numpy(nv12).pin_memory()
     nv12_dev = nv12_pin.to(dev)
+    p010 = C.rgb_to_yuv(np.rint(u8.astype(np.float64) * (1023.0 / 255.0)).astype(np.int64), 'p010', 'bt709')
+    p010_pin = torch.from_numpy(p010).pin_memory()
 
     def timed(fn):
         torch.cuda.synchronize()
@@ -85,8 +94,13 @@ def main():
 
     streams = {'push_u8_host_chunk1': (1, u8_pin, 'host'), 'push_u8_host_chunk16': (16, u8_pin, 'host'),
                'push_u8_device': (16, u8_dev, 'device'), 'push_nv12_host_chunk1': (1, nv12_pin, 'host'),
-               'push_nv12_host_chunk16': (16, nv12_pin, 'host'), 'push_nv12_device': (16, nv12_dev, 'device')}
-    opened = {k: net.stream(n, h, w, device=dev, **(dict(input='nv12', out_format='nv12') if 'nv12' in k else {}))
+               'push_nv12_host_chunk16': (16, nv12_pin, 'host'), 'push_nv12_device': (16, nv12_dev, 'device'),
+               'push_p010_709_host_chunk16': (16, p010_pin, 'host'),
+               'push_nv12_601_709_host_chunk16': (16, nv12_pin, 'host')}
+    kinds = {'push_p010_709_host_chunk16': dict(input='p010', out_format='p010', in_color='bt709', out_color='bt709'),
+             'push_nv12_601_709_host_chunk16': dict(input='nv12', out_format='nv12', out_color='bt709')}
+    opened = {k: net.stream(n, h, w, device=dev, **kinds.get(k, dict(input='nv12', out_format='nv12') if 'nv12' in k
+                                                                 else {}))
               for k in streams}
     runs = {k: [] for k in ['infer_sequence_fp32_host', *streams]}
     outputs = {}
@@ -108,16 +122,39 @@ def main():
     rgb_in = Y.yuv420_to_rgb(nv12, 'nv12')
     ref_rgb = net.infer_sequence(torch.from_numpy(rgb_in.astype(np.float32) / np.float32(255.0))
                                  .permute(0, 1, 4, 2, 3).contiguous(), dev)
+    def p010_matches(got):
+        """frame by frame against the oracle's P010 of the fp32 HR frames of a device loop of FRNet.step"""
+        lr = torch.from_numpy((C.yuv_to_rgb(p010, 'p010', 'bt709').astype(np.float32) / np.float32(1023.0))
+                              .transpose(0, 1, 4, 2, 3).copy())
+        lr_prev = torch.zeros(n, c, h, w, device=dev)
+        hr_prev = torch.zeros(n, c, s * h, s * w, device=dev)
+        with torch.no_grad():
+            for i in range(t):
+                cur = lr[:, i].contiguous().to(dev)
+                hr = net.step(cur, lr_prev, hr_prev)
+                want = C.rgb_f32_to_yuv(hr.permute(0, 2, 3, 1).cpu().numpy(), 'p010', 'bt709')
+                if not np.array_equal(got[:, i], want):
+                    return False
+                lr_prev, hr_prev = cur, hr
+        return True
+
     identical = {}
     for k, (chunk, src, out) in streams.items():
         got = np.concatenate([o.cpu().numpy() if out == 'device' else o for o in outputs[k]], axis=1)
-        if 'nv12' in k:        # frame by frame: the oracle's int64 temporaries of a whole clip are GBs
+        if k == 'push_p010_709_host_chunk16':
+            identical[k] = got.shape == (n, t, 3 * s * h // 2, s * w) and p010_matches(got)
+        elif k == 'push_nv12_601_709_host_chunk16':
+            identical[k] = got.shape == (n, t, 3 * s * h // 2, s * w) and all(
+                np.array_equal(got[j, i], C.rgb_to_yuv(ref_rgb[j, i], 'nv12', 'bt709')) for j in range(n)
+                for i in range(t))
+        elif 'nv12' in k:        # frame by frame: the oracle's int64 temporaries of a whole clip are GBs
             identical[k] = got.shape == (n, t, 3 * s * h // 2, s * w) and all(
                 np.array_equal(got[j, i], Y.rgb_to_yuv420(ref_rgb[j, i], 'nv12')) for j in range(n) for i in range(t))
         else:
             identical[k] = bool(np.array_equal(got, ref))
     stream_launches = opened['push_u8_device']._engine.launches_per_step
     nv12_launches = opened['push_nv12_device']._engine.launches_per_step
+    p010_launches = opened['push_p010_709_host_chunk16']._engine.launches_per_step
     for st in opened.values():
         st.close()
 
@@ -138,6 +175,11 @@ def main():
         sec = bench._time_graph(lambda i: ops.stream_frame_in_yuv420(yuv_ins[i], layout, None, lrs[i], prev, hrp, s),
                                 nb, reps, torch)
         frame_in[f'decode_{layout}'] = sec * 1e6
+    p010_ins = [torch.randint(0, 1 << 15, (n, 3 * h // 2, w), dtype=torch.int16, device=dev).view(torch.uint16)
+                for _ in range(nb)]
+    sec = bench._time_graph(lambda i: ops.stream_frame_in_yuv(p010_ins[i], 'p010', 'bt709', None, lrs[i], prev, hrp, s),
+                            nb, reps, torch)
+    frame_in['decode_p010_bt709'] = sec * 1e6
     # tg_rgb_u8_to_yuv420 alone: 8 rotating sets of 4 HR frames (8 x 8.2 MB in, 8 x 4.1 MB out)
     rgbs = [torch.randint(0, 256, (n, H, W, c), dtype=torch.uint8, device=dev) for _ in range(nb)]
     yuvs = [torch.empty(n, 3 * H // 2, W, dtype=torch.uint8, device=dev) for _ in range(nb)]
@@ -145,7 +187,14 @@ def main():
     for layout in ('nv12', 'i420'):
         sec = bench._time_graph(lambda i: ops.rgb_u8_to_yuv420(rgbs[i], layout, out=yuvs[i]), nb, reps, torch)
         encode[layout] = sec * 1e6
+    sec = bench._time_graph(lambda i: ops.rgb_to_yuv('nv12', 'bt709', rgb_u8=rgbs[i], out=yuvs[i]), nb, reps, torch)
+    encode['nv12_bt709'] = sec * 1e6
+    hrs = [torch.rand(n, c, H, W, device=dev) for _ in range(nb)]
+    p010s = [torch.empty(n, 3 * H // 2, W, dtype=torch.uint16, device=dev) for _ in range(nb)]
+    sec = bench._time_graph(lambda i: ops.rgb_to_yuv('p010', 'bt709', rgb_f32=hrs[i], out=p010s[i]), nb, reps, torch)
+    encode['p010_bt709'] = sec * 1e6
     encode_bytes = n * H * W * 3 + n * 3 * H // 2 * W
+    encode10_bytes = n * H * W * 3 * 4 + n * 3 * H // 2 * W * 2
 
     line = {
         'metric': 'hr_frames_per_sec_4xBD_3x134x320_streamed', 'unit': 'frames/s',
@@ -156,11 +205,13 @@ def main():
         'frame_in_us': frame_in,
         'encode_us': encode,
         'encode_bytes_per_step': encode_bytes,
-        'encode_gb_per_s': {k: encode_bytes / v * 1e-3 for k, v in encode.items()},
+        'encode10_bytes_per_step': encode10_bytes,
+        'encode_gb_per_s': {k: (encode10_bytes if k.startswith('p010') else encode_bytes) / v * 1e-3
+                            for k, v in encode.items()},
         'h2d_bytes_per_step': {'fp32': n * c * h * w * 4, 'uint8': n * c * h * w, 'nv12': n * 3 * h // 2 * w},
         'd2h_bytes_per_step': {'uint8': n * c * H * W, 'nv12': n * 3 * H // 2 * W},
         'launches_per_step': {'infer_sequence': T.engine.get_engine(net, n, c, h, w, dev).launches_per_step,
-                              'push': stream_launches, 'push_nv12': nv12_launches},
+                              'push': stream_launches, 'push_nv12': nv12_launches, 'push_p010': p010_launches},
     }
     print(json.dumps(line), flush=True)
 
