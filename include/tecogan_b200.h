@@ -303,6 +303,30 @@ int tg_rgb_to_yuv(const uint8_t* rgb_u8, const float* rgb_f32, void* out, const 
  * cBU cRV cGV cBV, decode CY CUB CUG CVG CVR, then the fraction bits and the luma offset. */
 int tg_yuv_coefficients(const tg_yuv_format* fmt, int32_t* out16);
 
+/* Resize of the streamed output: Pillow's antialiased bicubic (a = -0.5, support 2) or Lanczos-3 (support 3)
+ * filters, as Image.resize on 'F' images (oracle/resample.py restates them).  A downscale widens the filter by the
+ * ratio.  Each axis needs in/4 <= out <= 2*in, so an axis has at most 17 (bicubic) or 25 (Lanczos) taps.
+ * Per axis the kernel reads a caller-owned table: first[out] int32 (window start) and weights[out * taps] fp32 (the
+ * window's normalised weights, zero for padding taps).  The window ends inside the axis where it fits: first =
+ * max(0, min(xmin, in - taps)); on an axis shorter than taps the kernel clamps the index. */
+enum { TG_RESAMPLE_BICUBIC = 0, TG_RESAMPLE_LANCZOS3 = 1 };
+/* Host only: *taps = 2 * ceil(support * max(in / out, 1)) + 1.  TG_E_INVALID: null taps, non-positive sizes;
+ * TG_E_UNSUPPORTED: unknown filter, ratio outside [1/4, 2]. */
+int tg_resample_taps(int in, int out, int filter, int* taps);
+/* Host only: fills first[out] and weights[out * taps] (host memory; float64 weights rounded to fp32).  taps must be
+ * tg_resample_taps' value (TG_E_INVALID otherwise); other errors as tg_resample_taps. */
+int tg_resample_table(int in, int out, int filter, int taps, int32_t* first, float* weights);
+/* x fp32 NCHW [n,c,H,W] (the step's HR frame) -> exactly one of
+ *   y_u8  uint8 NHWC [n,Ho,Wo,c] = clip(rint(y * 255), 0, 255), round half to even (float32_to_uint8), or
+ *   y_f32 fp32 NCHW [n,c,Ho,Wo].
+ * Vertical pass (row tables, H -> Ho) then horizontal (column tables, W -> Wo), fp32 sums in tap order: the result
+ * does not depend on the grid.  Tables in device memory; x, the tables and y_f32 4-byte aligned.
+ * TG_E_INVALID: null pointers, both or neither output, non-positive sizes or taps, c > 4, misalignment;
+ * TG_E_UNSUPPORTED: a ratio outside [1/4, 2] on either axis, taps above 25, a grid too large. */
+int tg_resample_nchw_f32(const float* x, int n, int c, int H, int W, const int32_t* row_first, const float* row_w,
+                         int row_taps, const int32_t* col_first, const float* col_w, int col_taps, int Ho, int Wo,
+                         uint8_t* y_u8, float* y_f32, void* stream);
+
 /* BD degradation of the data side (codes/utils/data_utils.py:30-53, called on GT frames by
  * base_model.py:75,115): optional reflect pad by (k-1)/2 | k-1-(k-1)/2, then a depthwise valid
  * correlation with the k x k kernel `k2d` (device, fp32, = create_kernel(sigma)[0,0]) and stride s.

@@ -7,6 +7,7 @@ uint8 conversion per frame; here a frame is one graph replay, the uint8/HWC conv
 kernel (tg_float_to_uint8_nhwc) and the copies overlap compute on side streams.
 """
 import collections
+import numbers
 import os
 import weakref
 
@@ -229,12 +230,17 @@ class StreamEngine(ClipEngine):
     BT.601 limited range), tg_rgb_to_yuv of u8[p] (8 bit, other colours) or tg_rgb_to_yuv of the fp32 HR frame
     hr[p] (10 bit, uint16 yuv[p]) -- and the copies out read yuv[p] instead of u8[p].
 
+    Resized output (out_size = (Ho, Wo)): the step runs without its uint8 output (nothing would read it) and is
+    followed by tg_resample_nchw_f32 of the fp32 HR frame hr[p] into rs[p] -- uint8 [n,Ho,Wo,c], or fp32 [n,c,Ho,Wo]
+    when a 10-bit encode follows -- with the per-axis tables built once (tables[0] rows, tables[1] columns).  The
+    encode then reads rs[p] instead of u8[p] / hr[p], and the copies out read rs[p] (or yuv[p]).
+
     Copies overlap compute as in ClipEngine.run_clips.  uint8 input: inp[p] is itself the 2-deep staging ring (the
     step of parity p^1 never reads it), so the H2D of frame i+1 lands directly in the graph's input while frame i
     runs.  fp32 input: lr[p] is still read as lr_prev by frame i, so frames are staged as in run_clips."""
 
     def __init__(self, net, n, c, h, w, device, u8_input=True, bgr=False, yuv_in=None, yuv_out=None,
-                 in_color='bt601', out_color='bt601'):
+                 in_color='bt601', out_color='bt601', out_size=None, resize_filter='bicubic'):
         dev = torch.device(device)
         self.u8_input, self.bgr = u8_input or yuv_in is not None, bgr
         self.yuv_in, self.yuv_out = yuv_in, yuv_out          # None or one of ops.YUV_LAYOUTS
@@ -246,7 +252,16 @@ class StreamEngine(ClipEngine):
         self.inp = ([torch.zeros(n, *frame, dtype=in_dtype, device=dev).view(_word_dtype(yuv_in)) for _ in range(2)]
                     if self.u8_input else None)
         H, W = net.scale * h, net.scale * w
-        self.yuv = ([torch.empty(n, 3 * H // 2, W, dtype=_word_dtype(yuv_out), device=dev) for _ in range(2)]
+        self.out_size = tuple(out_size) if out_size else None
+        Ho, Wo = self.out_size or (H, W)
+        self.tables, self.rs = None, None
+        if self.out_size:
+            self.tables = [tuple(t.to(dev) for t in ops.resample_table(a, b, resize_filter))
+                           for a, b in ((H, Ho), (W, Wo))]
+            f32 = yuv_out is not None and ops.yuv_depth(yuv_out) == 10
+            self.rs = [torch.empty((n, c, Ho, Wo) if f32 else (n, Ho, Wo, c),
+                                   dtype=torch.float32 if f32 else torch.uint8, device=dev) for _ in range(2)]
+        self.yuv = ([torch.empty(n, 3 * Ho // 2, Wo, dtype=_word_dtype(yuv_out), device=dev) for _ in range(2)]
                     if yuv_out else None)
         self.sig = _param_signature(net)
         self.parity = 0                  # parity of the next frame
@@ -258,6 +273,7 @@ class StreamEngine(ClipEngine):
     def close(self):
         super().close()
         self.mask, self.inp, self.yuv = [], None, None
+        self.tables, self.rs = None, None
 
     def _enqueue(self, p):
         if self.yuv_in in YUV420 and self.in_color == 'bt601':
@@ -269,14 +285,21 @@ class StreamEngine(ClipEngine):
         else:
             ops.stream_frame_in(self.inp[p] if self.u8_input else None, self.mask[p], self.lr[p], self.lr[p ^ 1],
                                 self.hr[p ^ 1], self.net.scale, self.bgr)
-        super()._enqueue(p)
+        if self.out_size is None:
+            super()._enqueue(p)
+            rgb_u8, rgb_f32 = self.u8[p], self.hr[p]
+        else:
+            self.net.step_into(self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1], self.hr[p], out_u8=None)
+            f32 = self.rs[p].dtype == torch.float32
+            ops.resample(self.hr[p], *self.tables, out_u8=None if f32 else self.rs[p], out_f32=self.rs[p] if f32 else None)
+            rgb_u8 = rgb_f32 = self.rs[p]
         if self.yuv_out in YUV420 and self.out_color == 'bt601':
-            ops.rgb_u8_to_yuv420(self.u8[p], self.yuv_out, out=self.yuv[p])
+            ops.rgb_u8_to_yuv420(rgb_u8, self.yuv_out, out=self.yuv[p])
         elif self.yuv_out and ops.yuv_depth(self.yuv_out) == 8:
-            ops.rgb_to_yuv(self.yuv_out, self.out_color, rgb_u8=self.u8[p], out=self.yuv[p])
+            ops.rgb_to_yuv(self.yuv_out, self.out_color, rgb_u8=rgb_u8, out=self.yuv[p])
         elif self.yuv_out:
-            # 10 bit: from the step's fp32 HR frame, two more bits than the uint8 output keeps
-            ops.rgb_to_yuv(self.yuv_out, self.out_color, rgb_f32=self.hr[p], out=self.yuv[p])
+            # 10 bit: from the step's fp32 HR frame (or its resize), two more bits than the uint8 output keeps
+            ops.rgb_to_yuv(self.yuv_out, self.out_color, rgb_f32=rgb_f32, out=self.yuv[p])
 
     def _set_mask(self, p, slots):
         """On the main stream, before the replay of parity p: mask[p] = 1 for `slots`, 0 elsewhere."""
@@ -293,7 +316,7 @@ class StreamEngine(ClipEngine):
         """frames: uint8 [n,k,h,w,c] (u8_input), uint8 / uint16 [n,k,3h/2,w] (yuv_in) or fp32 [n,k,c,h,w], each
         frame contiguous, pinned host or on this device.
         Slots in `reset_slots` start a new video at frame 0.  Returns uint8 [n,k,H,W,c] (or [n,k,3H/2,W] words with
-        yuv_out): a pinned host tensor (out_host; one synchronisation, at the end) or a new tensor on the device,
+        yuv_out; Ho, Wo instead of H, W with out_size): a pinned host tensor (out_host; one synchronisation, at the end) or a new tensor on the device,
         ordered on the current stream (no synchronisation)."""
         n, k = self.n, frames.shape[1]
         with torch.cuda.device(self.device):
@@ -301,7 +324,8 @@ class StreamEngine(ClipEngine):
             self.net.refresh_packed_weights()        # a load_state_dict between pushes takes effect
             for st in (self.main, self.h2d, self.d2h):
                 st.wait_stream(cur)
-            res = self.yuv if self.yuv_out else self.u8      # what the step graph leaves for the copy out
+            # what the step graph leaves for the copy out
+            res = self.yuv if self.yuv_out else self.rs if self.out_size else self.u8
             shape = (n, k, *res[0].shape[1:])
             if out_host:
                 out = torch.empty(shape, dtype=res[0].dtype, pin_memory=True)
@@ -362,7 +386,7 @@ class VideoStream:
     Created by FRNet.stream(); see there."""
 
     def __init__(self, net, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb',
-                 in_color='bt601', out_color='bt601'):
+                 in_color='bt601', out_color='bt601', out_size=None, resize_filter='bicubic'):
         if input not in ('uint8', 'float32', *YUV):
             raise ValueError(f"input must be 'uint8', 'float32' or one of {YUV}, got {input!r}")
         if channel_order not in ('rgb', 'bgr'):
@@ -378,6 +402,12 @@ class VideoStream:
             raise ValueError(f"channel_order='bgr' applies to uint8 HWC input only, not input={input!r}")
         if not all(isinstance(v, int) and v > 0 for v in (n, h, w)):
             raise ValueError(f'n, h, w must be positive ints, got {(n, h, w)}')
+        if not isinstance(resize_filter, str) or resize_filter not in ops.RESIZE_FILTERS:
+            raise ValueError(f'resize_filter must be one of {ops.RESIZE_FILTERS}, got {resize_filter!r}')
+        if out_size is None and resize_filter != 'bicubic':
+            raise ValueError(f'resize_filter={resize_filter!r} applies to a resized stream only (give out_size)')
+        if out_size is not None:
+            out_size = _check_out_size(out_size, net.scale * h, net.scale * w, out_format)
         yuv = [f for f in (input, out_format) if f in YUV]
         if yuv and (h % 2 or w % 2):
             raise ValueError(f'{yuv[0]} frames are YUV 4:2:0: h and w must be even, got {h}x{w}')
@@ -390,6 +420,7 @@ class VideoStream:
         self.c = net.fnet.in_nc
         self.device, self.input, self.channel_order, self.out_format = device, input, channel_order, out_format
         self.in_color, self.out_color = in_color, out_color
+        self.out_size, self.resize_filter = out_size, resize_filter
         self._engine = None                  # built (graphs captured) by the first push
         self._pending = [True] * n           # a new stream starts every slot from zero state
         _check_inference(net)
@@ -420,7 +451,8 @@ class VideoStream:
         out:    'host' -> NumPy uint8 [n,k,H,W,c] (one synchronisation); 'device' -> a new CUDA uint8 tensor
                 [n,k,H,W,c], ordered on the current stream (no synchronisation; a pinned host input must then
                 stay unchanged until that stream has passed this push).  With out_format 'nv12' / 'i420' the
-                frames are uint8 [n,k,3H/2,W] instead, with 'p010' / 'i420_10' uint16 [n,k,3H/2,W].
+                frames are uint8 [n,k,3H/2,W] instead, with 'p010' / 'i420_10' uint16 [n,k,3H/2,W].  A stream
+                opened with out_size=(Ho, Wo) returns Ho x Wo frames in place of H x W.
         10-bit input ('p010', 'i420_10') takes uint16 frames [n,k,3h/2,w] ([k,3h/2,w] when n == 1), torch.uint16 or
         NumPy uint16; uint8 frames into a 10-bit stream raise, and so do uint16 frames into an 8-bit one.
         """
@@ -496,7 +528,23 @@ class VideoStream:
         yuv_out = self.out_format if self.out_format in YUV else None
         return StreamEngine(self.net, self.n, self.c, self.h, self.w, dev, u8_input=self.input == 'uint8',
                             bgr=self.channel_order == 'bgr', yuv_in=yuv_in, yuv_out=yuv_out,
-                            in_color=self.in_color, out_color=self.out_color)
+                            in_color=self.in_color, out_color=self.out_color, out_size=self.out_size,
+                            resize_filter=self.resize_filter)
+
+
+def _check_out_size(out_size, H, W, out_format):
+    """out_size -> (Ho, Wo) ints, or ValueError: two positive ints within the resize's ratios of the H x W output,
+    even for a YUV out_format."""
+    if (not isinstance(out_size, (tuple, list)) or len(out_size) != 2
+            or not all(isinstance(v, numbers.Integral) and not isinstance(v, bool) and v > 0 for v in out_size)):
+        raise ValueError(f'out_size must be (Ho, Wo), two positive ints, got {out_size!r}')
+    Ho, Wo = int(out_size[0]), int(out_size[1])
+    if not (ops.resample_ratio_ok(H, Ho) and ops.resample_ratio_ok(W, Wo)):
+        raise ValueError(f'out_size {Ho}x{Wo} from a {H}x{W} output: each axis must be within 1/4 to 2 times the '
+                         f'output size')
+    if out_format in YUV and (Ho % 2 or Wo % 2):
+        raise ValueError(f'{out_format} frames are YUV 4:2:0: out_size must be even, got {Ho}x{Wo}')
+    return Ho, Wo
 
 
 def _check_inference(net):

@@ -19,6 +19,7 @@ UP_BICUBIC, UP_BILINEAR = 0, 1
 EPI_NHWC_F16, EPI_FLOW_NCHW_F32, EPI_OUT_NCHW_F32, EPI_NHWC_F16_POOL2 = 0, 1, 2, 3
 AMODE_AUTO, AMODE_HALO, AMODE_TAP = 0, 1, 2
 YUV_NV12, YUV_I420, YUV_P010, YUV_I420_10 = 0, 1, 2, 3
+RESAMPLE_BICUBIC, RESAMPLE_LANCZOS3 = 0, 1
 
 
 class ConvDesc(ctypes.Structure):
@@ -104,6 +105,10 @@ _SIGNATURES = {
     'tg_stream_frame_in_yuv': (c_int, [_P, ctypes.POINTER(YuvFormat), _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'tg_rgb_to_yuv': (c_int, [_P, _P, _P, ctypes.POINTER(YuvFormat), c_int, c_int, c_int, _P]),
     'tg_yuv_coefficients': (c_int, [ctypes.POINTER(YuvFormat), ctypes.POINTER(c_int32)]),
+    'tg_resample_taps': (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_int)]),
+    'tg_resample_table': (c_int, [c_int, c_int, c_int, c_int, _P, _P]),
+    'tg_resample_nchw_f32': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, _P, c_int, c_int, c_int,
+                                     _P, _P, _P]),
     'tg_downsample_bd_nchw_f32': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_debug_set_conv_timers': (c_int, [_P]),
     # ---- training (generator backward)

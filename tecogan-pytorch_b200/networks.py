@@ -356,7 +356,7 @@ class FRNet(BaseSequenceGenerator):
         return infer_clips(self, lr_data, device)
 
     def stream(self, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb', in_color='bt601',
-               out_color='bt601'):
+               out_color='bt601', out_size=None, resize_filter='bicubic'):
         """A VideoStream of n lock-stepped slots of h x w LR frames: video pushed in chunks of any length, the
         recurrent state carried from one push to the next, and a slot restarted (reset=) when its video ends and
         the next one begins while the other slots keep running.
@@ -382,11 +382,18 @@ class FRNet(BaseSequenceGenerator):
         point as oracle/yuv_color.py specifies).  Take in_color from the decoder (ffprobe's color_space /
         color_range) and tag the encoded output with out_color.  A colour other than 'bt601' on an RGB or float32
         side raises ValueError.
+        out_size=(Ho, Wo) resizes every output frame from H x W to Ho x Wo on the device, from the fp32 HR frame
+        and before the uint8 quantisation or the YUV encode: push() then returns uint8 [n,k,Ho,Wo,c] or YUV words
+        [n,k,3Ho/2,Wo].  resize_filter is 'bicubic' (the default) or 'lanczos': Pillow's antialiased filters
+        (Image.resize on 'F' images, as oracle/resample.py specifies), widened by the ratio on a downscale.  Each
+        axis needs H/4 <= Ho <= 2H (likewise W), and even Ho and Wo for YUV output.  out_size=(H, W) gives the
+        bytes of the stream without it.
         Temporal padding (pad_sequence, base_model.py:230-251) stays the caller's job: for p reflect-padded
         frames, push frames[:, 1:1+p].flip(1) first and drop those p outputs.  The CUDA graphs are captured by the first push; the stream holds the
         net."""
         from .engine import VideoStream
-        return VideoStream(self, n, h, w, device, input, channel_order, out_format, in_color, out_color)
+        return VideoStream(self, n, h, w, device, input, channel_order, out_format, in_color, out_color, out_size,
+                           resize_filter)
 
     def refresh_packed_weights(self, force=False):
         self.fnet._cache.refresh_all(force)

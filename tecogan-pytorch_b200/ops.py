@@ -591,6 +591,68 @@ def rgb_to_yuv(layout, color, rgb_u8=None, rgb_f32=None, out=None):
     return out
 
 
+RESIZE_FILTERS = ('bicubic', 'lanczos')
+_FILTER_CODE = {'bicubic': L.RESAMPLE_BICUBIC, 'lanczos': L.RESAMPLE_LANCZOS3}
+
+
+def resample_ratio_ok(n_in, n_out):
+    """The resize supports in/4 <= out <= 2*in on each axis."""
+    return n_in > 0 and n_out > 0 and 4 * n_out >= n_in and n_out <= 2 * n_in
+
+
+def resample_table(n_in, n_out, filt='bicubic'):
+    """tg_resample_table (host only, no GPU needed): the kernel's table of one axis, (first int32 [out],
+    weights fp32 [out, taps]) as CPU tensors; oracle/resample.py's table rounded to fp32."""
+    if filt not in _FILTER_CODE:
+        raise L.TecoganB200Error(f'resample_table: filter must be one of {RESIZE_FILTERS}, got {filt!r}')
+    lib = L.load()
+    taps = ctypes.c_int(0)
+    L.check(lib.tg_resample_taps(int(n_in), int(n_out), _FILTER_CODE[filt], ctypes.byref(taps)), 'tg_resample_taps')
+    first = torch.empty(n_out, dtype=torch.int32)
+    weights = torch.empty(n_out, taps.value, dtype=torch.float32)
+    L.check(lib.tg_resample_table(int(n_in), int(n_out), _FILTER_CODE[filt], taps.value, _ptr(first), _ptr(weights)),
+            'tg_resample_table')
+    return first, weights
+
+
+def resample(x, rows, cols, out_u8=None, out_f32=None):
+    """tg_resample_nchw_f32: x fp32 NCHW [n,c,H,W] resized with the device tables rows = (first [Ho], weights
+    [Ho, taps]) and cols = (first [Wo], weights [Wo, taps]) into exactly one of out_u8 (uint8 NHWC [n,Ho,Wo,c],
+    float32_to_uint8 of the result) or out_f32 (fp32 NCHW [n,c,Ho,Wo]).  With neither given, a new uint8 tensor."""
+    name = 'resample'
+    _req(x, torch.float32, 'x', 4)
+    n, c, H, W = x.shape
+    tabs = []
+    for axis, (first, weights), n_in in (('rows', rows, H), ('cols', cols, W)):
+        _req(first, torch.int32, f'{axis} first', 1)
+        _req(weights, torch.float32, f'{axis} weights', 2)
+        if weights.shape[0] != first.shape[0]:
+            raise L.TecoganB200Error(f'{name}: {axis} first {tuple(first.shape)} and weights '
+                                     f'{tuple(weights.shape)} disagree')
+        if first.device != x.device or weights.device != x.device:
+            raise L.TecoganB200Error(f'{name}: tensors on different devices')
+        if not resample_ratio_ok(n_in, first.shape[0]):
+            raise L.TecoganB200Error(f'{name}: {axis} {n_in} -> {first.shape[0]} outside in/4 <= out <= 2*in')
+        tabs.append((first, weights, weights.shape[1]))
+    Ho, Wo = rows[0].shape[0], cols[0].shape[0]
+    if out_u8 is not None and out_f32 is not None:
+        raise L.TecoganB200Error(f'{name}: give out_u8 or out_f32, not both')
+    if out_f32 is None and out_u8 is None:
+        out_u8 = torch.empty((n, Ho, Wo, c), dtype=torch.uint8, device=x.device)
+    if out_u8 is not None:
+        out, want = _req(out_u8, torch.uint8, 'out_u8', 4), (n, Ho, Wo, c)
+    else:
+        out, want = _req(out_f32, torch.float32, 'out_f32', 4), (n, c, Ho, Wo)
+    if tuple(out.shape) != want:
+        raise L.TecoganB200Error(f'{name}: out {tuple(out.shape)} != {want}')
+    if out.device != x.device:
+        raise L.TecoganB200Error(f'{name}: tensors on different devices')
+    (rf, rw, rt), (cf, cw, ct) = tabs
+    L.check(L.load().tg_resample_nchw_f32(_ptr(x), n, c, H, W, _ptr(rf), _ptr(rw), rt, _ptr(cf), _ptr(cw), ct, Ho, Wo,
+                                          _ptr(out_u8), _ptr(out_f32), _stream()), 'tg_resample_nchw_f32')
+    return out
+
+
 # ============================================================================ training (backward) ops
 class GradScale:
     """Device-resident loss scale {scale, 1/scale} of the fp16 gradient path (tg_grad_scale_from_amax /

@@ -18,13 +18,22 @@ each run ends in a device synchronisation; one untimed warm-up run of every path
                              slot reset) and tg_stream_frame_in_yuv420 per step (NV12, I420), CUDA events over a
                              graph of launches on rotating buffers
                              and tg_stream_frame_in_yuv per step (P010 / BT.709)
+  push_u8_resize_<Ho>x<Wo>[_lanczos]_host_chunk16
+                             an RGB stream with out_size=(Ho, Wo) (bicubic unless marked), k = 16: 402x960 (3/4) and
+                             804x1920 (3/2)
+  push_nv12_709_resize_402x960_host_chunk16  uint8 in, NV12 / BT.709 out at out_size=(402, 960), k = 16
+  resample_us                tg_resample_nchw_f32 per step (4 HR frames -> uint8 NHWC or fp32 NCHW), timed as below,
+                             with its algorithmic bytes (n*3*H*W*4 read, n*Ho*Wo*3 or *12 written) and TB/s
   encode_us                  tg_rgb_u8_to_yuv420 per step (4 HR frames -> NV12 / I420) and tg_rgb_to_yuv per step
                              (uint8 -> NV12 / BT.709; fp32 NCHW -> P010 / BT.709), timed the same way
 All uint8 paths process the same frames (uint8, and the reference loader's float32 / 255 of them), so their
 outputs are also compared byte for byte.  The NV12 paths take oracle/yuv_oracle.py's NV12 of those frames; their
 output is compared with the oracle's NV12 of the RGB output for the frames that NV12 decodes to; the BT.709 NV12
 output with oracle/yuv_color.py's BT.709 encode of that RGB output, and the P010 output with its encode of the fp32 HR
-frames of a device loop of FRNet.step over the frames P010 decodes to.  Card name and
+frames of a device loop of FRNet.step over the frames P010 decodes to.  The resized RGB outputs are compared with
+oracle/resample.py's float64 resize of the fp32 HR frames of a device loop of FRNet.step (equal, or 1 apart where
+x * 255 is within 1e-3 of a rounding boundary), the resized NV12 output with the BT.709 encode of the resized RGB
+output.  Card name and
 power limit are read in the same run.  Writes nothing."""
 import argparse
 import json
@@ -60,6 +69,7 @@ def main():
     import tecogan_b200 as T
     from oracle import yuv_oracle as Y
     from oracle import yuv_color as C
+    from oracle import resample as R
     ops = sys.modules['tecogan-pytorch_b200.ops']
     assert torch.cuda.is_available(), 'stream_bench.py needs a GPU'
     dev = torch.device('cuda', 0)
@@ -99,6 +109,14 @@ def main():
                'push_nv12_601_709_host_chunk16': (16, nv12_pin, 'host')}
     kinds = {'push_p010_709_host_chunk16': dict(input='p010', out_format='p010', in_color='bt709', out_color='bt709'),
              'push_nv12_601_709_host_chunk16': dict(input='nv12', out_format='nv12', out_color='bt709')}
+    resized = {'push_u8_resize_402x960_host_chunk16': dict(out_size=(402, 960)),
+               'push_u8_resize_804x1920_host_chunk16': dict(out_size=(804, 1920)),
+               'push_u8_resize_402x960_lanczos_host_chunk16': dict(out_size=(402, 960), resize_filter='lanczos'),
+               'push_nv12_709_resize_402x960_host_chunk16': dict(out_size=(402, 960), out_format='nv12',
+                                                                 out_color='bt709')}
+    for k, kw in resized.items():
+        streams[k] = (16, u8_pin, 'host')
+        kinds[k] = kw
     opened = {k: net.stream(n, h, w, device=dev, **kinds.get(k, dict(input='nv12', out_format='nv12') if 'nv12' in k
                                                                  else {}))
               for k in streams}
@@ -138,10 +156,46 @@ def main():
                 lr_prev, hr_prev = cur, hr
         return True
 
+    hr_loop = None
+
+    def resized_matches(got, size, filt):
+        """frame by frame against the oracle's float64 resize of the fp32 HR frames of a device loop of FRNet.step
+        (its dense matrices applied in float64 on the device), under the uint8 rule"""
+        nonlocal hr_loop
+        if hr_loop is None:
+            hr_loop, lr_prev, hr_prev = [], torch.zeros(n, c, h, w, device=dev), torch.zeros(n, c, s * h, s * w,
+                                                                                              device=dev)
+            with torch.no_grad():
+                for i in range(t):
+                    cur = f32[:, i].to(dev)
+                    hr_prev = net.step(cur, lr_prev, hr_prev)
+                    lr_prev = cur
+                    hr_loop.append(hr_prev.clone())
+        my = torch.from_numpy(R.matrix(s * h, size[0], filt)).to(dev)
+        mx = torch.from_numpy(R.matrix(s * w, size[1], filt)).to(dev)
+        if got.shape != (n, t, *size, c):
+            return False
+        for i in range(t):            # R.to_uint8 and R.near_boundary, evaluated on the device
+            ref = (my @ (hr_loop[i].double() @ mx.T)).permute(0, 2, 3, 1)
+            q = torch.round(ref.float() * 255.0).clamp(0, 255).int()
+            v = ref * 255.0
+            near = (v - v.floor() - 0.5).abs() < 1e-3
+            d = (torch.from_numpy(got[:, i]).to(dev).int() - q).abs()
+            if int(d.max()) > 1 or bool((d[~near] > 0).any()):
+                return False
+        return True
+
     identical = {}
     for k, (chunk, src, out) in streams.items():
         got = np.concatenate([o.cpu().numpy() if out == 'device' else o for o in outputs[k]], axis=1)
-        if k == 'push_p010_709_host_chunk16':
+        if k == 'push_nv12_709_resize_402x960_host_chunk16':
+            rgb = np.concatenate(outputs['push_u8_resize_402x960_host_chunk16'], axis=1)
+            identical[k] = got.shape == (n, t, 3 * 402 // 2, 960) and all(
+                np.array_equal(got[j, i], C.rgb_to_yuv(rgb[j, i], 'nv12', 'bt709')) for j in range(n)
+                for i in range(t))
+        elif k in resized:
+            identical[k] = resized_matches(got, resized[k]['out_size'], resized[k].get('resize_filter', 'bicubic'))
+        elif k == 'push_p010_709_host_chunk16':
             identical[k] = got.shape == (n, t, 3 * s * h // 2, s * w) and p010_matches(got)
         elif k == 'push_nv12_601_709_host_chunk16':
             identical[k] = got.shape == (n, t, 3 * s * h // 2, s * w) and all(
@@ -155,6 +209,7 @@ def main():
     stream_launches = opened['push_u8_device']._engine.launches_per_step
     nv12_launches = opened['push_nv12_device']._engine.launches_per_step
     p010_launches = opened['push_p010_709_host_chunk16']._engine.launches_per_step
+    resize_launches = opened['push_u8_resize_402x960_host_chunk16']._engine.launches_per_step
     for st in opened.values():
         st.close()
 
@@ -194,6 +249,20 @@ def main():
     sec = bench._time_graph(lambda i: ops.rgb_to_yuv('p010', 'bt709', rgb_f32=hrs[i], out=p010s[i]), nb, reps, torch)
     encode['p010_bt709'] = sec * 1e6
     encode_bytes = n * H * W * 3 + n * 3 * H // 2 * W
+    # tg_resample_nchw_f32 alone: the same 8 rotating sets of 4 fp32 HR frames (8 x 33 MB)
+    resample, resample_bytes = {}, {}
+    for name, (Ho, Wo), filt, f32_out in (('u8_402x960_bicubic', (402, 960), 'bicubic', False),
+                                          ('u8_804x1920_bicubic', (804, 1920), 'bicubic', False),
+                                          ('u8_402x960_lanczos', (402, 960), 'lanczos', False),
+                                          ('f32_402x960_bicubic', (402, 960), 'bicubic', True)):
+        tabs = [tuple(v.to(dev) for v in ops.resample_table(a, b, filt)) for a, b in ((H, Ho), (W, Wo))]
+        outs = [torch.empty((n, c, Ho, Wo) if f32_out else (n, Ho, Wo, c), dtype=torch.float32 if f32_out else
+                            torch.uint8, device=dev) for _ in range(nb)]
+        kw = (lambda i: {'out_f32': outs[i]}) if f32_out else (lambda i: {'out_u8': outs[i]})
+        sec = bench._time_graph(lambda i: ops.resample(hrs[i], *tabs, **kw(i)), nb, reps, torch)
+        resample[name] = sec * 1e6
+        resample_bytes[name] = n * c * H * W * 4 + n * Ho * Wo * c * (4 if f32_out else 1)
+        del outs
     encode10_bytes = n * H * W * 3 * 4 + n * 3 * H // 2 * W * 2
 
     line = {
@@ -204,6 +273,9 @@ def main():
         'identical_to_infer_sequence': identical,
         'frame_in_us': frame_in,
         'encode_us': encode,
+        'resample_us': resample,
+        'resample_bytes_per_step': resample_bytes,
+        'resample_tb_per_s': {k: resample_bytes[k] / v * 1e-6 for k, v in resample.items()},
         'encode_bytes_per_step': encode_bytes,
         'encode10_bytes_per_step': encode10_bytes,
         'encode_gb_per_s': {k: (encode10_bytes if k.startswith('p010') else encode_bytes) / v * 1e-3
@@ -211,7 +283,8 @@ def main():
         'h2d_bytes_per_step': {'fp32': n * c * h * w * 4, 'uint8': n * c * h * w, 'nv12': n * 3 * h // 2 * w},
         'd2h_bytes_per_step': {'uint8': n * c * H * W, 'nv12': n * 3 * H // 2 * W},
         'launches_per_step': {'infer_sequence': T.engine.get_engine(net, n, c, h, w, dev).launches_per_step,
-                              'push': stream_launches, 'push_nv12': nv12_launches, 'push_p010': p010_launches},
+                              'push': stream_launches, 'push_nv12': nv12_launches, 'push_p010': p010_launches,
+                              'push_resize': resize_launches},
     }
     print(json.dumps(line), flush=True)
 
