@@ -327,6 +327,27 @@ int tg_resample_nchw_f32(const float* x, int n, int c, int H, int W, const int32
                          int row_taps, const int32_t* col_first, const float* col_w, int col_taps, int Ho, int Wo,
                          uint8_t* y_u8, float* y_f32, void* stream);
 
+/* Scene-cut detection of a streamed step (oracle/scene_cut.py is the specification).  Per slot k, with a = lr_curr[k]
+ * and b = lr_prev[k] (fp32 [c,h,w], as the step sees them: decoded, and zeroed by a reset of this step):
+ *   q(x) = clip(rint(x * 255), 0, 255) (fp32 product, round half to even; NaN counts as 0),
+ *   SAD  = sum |q(a) - q(b)| (exact integer), mafd = float64(SAD) * 100 / (c*h*w) / 255 (float64, in that order);
+ *   reset[k] != 0     : score 0, cut 0, prev_mafd[k] = -1
+ *   prev_mafd[k] < 0  : score 0, cut 0, prev_mafd[k] = mafd
+ *   otherwise         : score = min(max(min(mafd, |mafd - prev_mafd[k]|), 0), 100), cut = score >= threshold,
+ *                       prev_mafd[k] = cut ? -1 : mafd.
+ * score[n] (float64) and cut[n] (int32 0 / 1) are written for every slot on every launch; with cut as the reset mask
+ * of tg_stream_frame_in (in_u8 = NULL) a detected cut restarts the slot exactly as a reset at that frame would.
+ * reset : int32 [n] in device memory (tg_stream_frame_in's mask), or NULL (no caller resets).
+ * work  : caller-owned device workspace of n * TG_SCENE_CUT_WORK_BYTES bytes, zeroed once by the caller; every launch
+ *         leaves it zeroed again, so a captured launch replays without a memset.
+ * Every sum is an integer, so the result does not depend on the grid.  lr_curr, lr_prev, reset and cut 4-byte aligned;
+ * prev_mafd, work and score 8-byte aligned.
+ * TG_E_INVALID: null pointers (reset aside), non-positive sizes, misalignment, a threshold that is not finite or lies
+ * outside (0, 100]; TG_E_UNSUPPORTED: c > 4, a grid too large. */
+#define TG_SCENE_CUT_WORK_BYTES 16
+int tg_scene_cut(const float* lr_curr, const float* lr_prev, int n, int c, int h, int w, const int32_t* reset,
+                 double threshold, double* prev_mafd, void* work, double* score, int32_t* cut, void* stream);
+
 /* BD degradation of the data side (codes/utils/data_utils.py:30-53, called on GT frames by
  * base_model.py:75,115): optional reflect pad by (k-1)/2 | k-1-(k-1)/2, then a depthwise valid
  * correlation with the k x k kernel `k2d` (device, fp32, = create_kernel(sigma)[0,0]) and stride s.

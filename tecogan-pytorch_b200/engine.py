@@ -7,6 +7,7 @@ uint8 conversion per frame; here a frame is one graph replay, the uint8/HWC conv
 kernel (tg_float_to_uint8_nhwc) and the copies overlap compute on side streams.
 """
 import collections
+import math
 import numbers
 import os
 import weakref
@@ -235,12 +236,19 @@ class StreamEngine(ClipEngine):
     when a 10-bit encode follows -- with the per-axis tables built once (tables[0] rows, tables[1] columns).  The
     encode then reads rs[p] instead of u8[p] / hr[p], and the copies out read rs[p] (or yuv[p]).
 
+    Scene cuts (scene_cut = threshold): after the frame input, tg_scene_cut scores lr[p] against lr[p^1] for every
+    slot (the caller's resets of mask[p] score 0) into score[p] / cut[p], updating the per-slot state prev_mafd, and
+    a second tg_stream_frame_in, reset-only with cut[p] as its mask, zeroes lr[p^1][k] / hr[p^1][k] of the slots
+    with a detected cut -- the restart a reset of that slot at this frame would have made.  score[p] (float64 [n])
+    and cut[p] (int32 [n]) are views of one int32 buffer rep[p] [3n], copied after each replay into the push's
+    report [k,3n] (one device-to-device copy per frame).
+
     Copies overlap compute as in ClipEngine.run_clips.  uint8 input: inp[p] is itself the 2-deep staging ring (the
     step of parity p^1 never reads it), so the H2D of frame i+1 lands directly in the graph's input while frame i
     runs.  fp32 input: lr[p] is still read as lr_prev by frame i, so frames are staged as in run_clips."""
 
     def __init__(self, net, n, c, h, w, device, u8_input=True, bgr=False, yuv_in=None, yuv_out=None,
-                 in_color='bt601', out_color='bt601', out_size=None, resize_filter='bicubic'):
+                 in_color='bt601', out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None):
         dev = torch.device(device)
         self.u8_input, self.bgr = u8_input or yuv_in is not None, bgr
         self.yuv_in, self.yuv_out = yuv_in, yuv_out          # None or one of ops.YUV_LAYOUTS
@@ -263,17 +271,31 @@ class StreamEngine(ClipEngine):
                                    dtype=torch.float32 if f32 else torch.uint8, device=dev) for _ in range(2)]
         self.yuv = ([torch.empty(n, 3 * Ho // 2, Wo, dtype=_word_dtype(yuv_out), device=dev) for _ in range(2)]
                     if yuv_out else None)
+        self.scene_cut = scene_cut
+        self.prev_mafd = self.work = self.rep = self.score = self.cut = None
+        self.report = None               # [k,3n] int32 of the last run: score[p] / cut[p] after each frame
+        self._report_dev = self._report_host = None
+        if scene_cut is not None:
+            self.prev_mafd = torch.full((n,), -1.0, dtype=torch.float64, device=dev)
+            self.work = ops.scene_cut_work(n, dev)
+            self.rep = [torch.zeros(3 * n, dtype=torch.int32, device=dev) for _ in range(2)]
+            self.score = [r[:2 * n].view(torch.float64) for r in self.rep]
+            self.cut = [r[2 * n:] for r in self.rep]
         self.sig = _param_signature(net)
         self.parity = 0                  # parity of the next frame
         self.mask_set = [False, False]   # mask[p] holds a reset pattern (cleared before the next replay)
         self.in_free = [None, None]      # event: the replay that last read inp[p] / stage[p] finished
         self.out_copied = [None, None]   # event: the D2H of u8[p] (yuv[p]) finished
+        # the capture's warm-up steps update prev_mafd; that state is never read, because the first push resets every
+        # slot (VideoStream._pending) and a reset sets prev_mafd := -1 without reading it
         super().__init__(net, n, c, h, w, dev)     # lr / hr / u8, streams, the two graphs of _enqueue below
 
     def close(self):
         super().close()
         self.mask, self.inp, self.yuv = [], None, None
         self.tables, self.rs = None, None
+        self.prev_mafd = self.work = self.rep = self.score = self.cut = self.report = None
+        self._report_dev = self._report_host = None
 
     def _enqueue(self, p):
         if self.yuv_in in YUV420 and self.in_color == 'bt601':
@@ -285,6 +307,11 @@ class StreamEngine(ClipEngine):
         else:
             ops.stream_frame_in(self.inp[p] if self.u8_input else None, self.mask[p], self.lr[p], self.lr[p ^ 1],
                                 self.hr[p ^ 1], self.net.scale, self.bgr)
+        if self.scene_cut is not None:
+            ops.scene_cut(self.lr[p], self.lr[p ^ 1], self.mask[p], self.scene_cut, self.prev_mafd, self.work,
+                          self.score[p], self.cut[p])
+            # a detected cut restarts the slot: the reset-only frame input with cut[p] as its mask
+            ops.stream_frame_in(None, self.cut[p], self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1], self.net.scale)
         if self.out_size is None:
             super()._enqueue(p)
             rgb_u8, rgb_f32 = self.u8[p], self.hr[p]
@@ -331,6 +358,12 @@ class StreamEngine(ClipEngine):
                 out = torch.empty(shape, dtype=res[0].dtype, pin_memory=True)
             else:
                 out = torch.empty(shape, dtype=res[0].dtype, device=self.device)
+            report = None
+            if self.scene_cut is not None:
+                # kept between pushes (read on the current stream, which the next push's streams wait for)
+                if self._report_dev is None or self._report_dev.shape[0] < k:
+                    self._report_dev = torch.empty((max(k, 16), 3 * n), dtype=torch.int32, device=self.device)
+                report = self._report_dev[:k]
             if not self.u8_input and self.stage is None:
                 self.stage = [torch.empty_like(self.lr[0]) for _ in range(2)]
             dst = self.inp if self.u8_input else self.stage
@@ -351,6 +384,8 @@ class StreamEngine(ClipEngine):
                     if out_host and self.out_copied[p] is not None:
                         self.main.wait_event(self.out_copied[p])     # res[p] free to overwrite
                     self.run_frame(p)
+                    if report is not None:
+                        report[i].copy_(self.rep[p], non_blocking=True)
                     done = torch.cuda.Event()
                     done.record(self.main)
                     self.in_free[p] = done
@@ -365,10 +400,17 @@ class StreamEngine(ClipEngine):
                         self.out_copied[p].record(self.d2h)
                 self.parity ^= 1
             if out_host:
+                if report is not None:       # the D2H stream has waited on the last replay's event
+                    if self._report_host is None or self._report_host.shape[0] < k:
+                        self._report_host = torch.empty(self._report_dev.shape, dtype=torch.int32, pin_memory=True)
+                    with torch.cuda.stream(self.d2h):
+                        self._report_host[:k].copy_(report, non_blocking=True)
+                    report = self._report_host[:k]
                 self.d2h.synchronize()   # after every replay (D2H waited on each) and so after every H2D
             else:
                 cur.wait_stream(self.main)
                 cur.wait_stream(self.h2d)    # a device input may be freed once the call returns
+        self.report = report
         return out
 
 
@@ -386,7 +428,9 @@ class VideoStream:
     Created by FRNet.stream(); see there."""
 
     def __init__(self, net, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb',
-                 in_color='bt601', out_color='bt601', out_size=None, resize_filter='bicubic'):
+                 in_color='bt601', out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None):
+        if scene_cut is not None:
+            scene_cut = _check_scene_cut(scene_cut)
         if input not in ('uint8', 'float32', *YUV):
             raise ValueError(f"input must be 'uint8', 'float32' or one of {YUV}, got {input!r}")
         if channel_order not in ('rgb', 'bgr'):
@@ -421,6 +465,10 @@ class VideoStream:
         self.device, self.input, self.channel_order, self.out_format = device, input, channel_order, out_format
         self.in_color, self.out_color = in_color, out_color
         self.out_size, self.resize_filter = out_size, resize_filter
+        self.scene_cut = scene_cut
+        # the latest push's detected cuts (bool [n,k]) and scores (float64 [n,k]): NumPy after out='host', CUDA
+        # tensors after out='device'; None before the first push and without scene_cut
+        self.last_cuts = self.last_scores = None
         self._engine = None                  # built (graphs captured) by the first push
         self._pending = [True] * n           # a new stream starts every slot from zero state
         _check_inference(net)
@@ -455,6 +503,10 @@ class VideoStream:
                 opened with out_size=(Ho, Wo) returns Ho x Wo frames in place of H x W.
         10-bit input ('p010', 'i420_10') takes uint16 frames [n,k,3h/2,w] ([k,3h/2,w] when n == 1), torch.uint16 or
         NumPy uint16; uint8 frames into a 10-bit stream raise, and so do uint16 frames into an 8-bit one.
+        A stream opened with scene_cut=threshold restarts a slot at every detected cut, as reset= would have, and
+        sets last_cuts (bool [n,k]) and last_scores (float64 [n,k]) for this push: NumPy with out='host', CUDA
+        tensors ordered on the current stream with out='device'.  A reset requested by the caller scores 0 and is
+        not reported as a cut.
         """
         if self._engine is False:
             raise ops.L.TecoganB200Error('VideoStream.push: the stream is closed')
@@ -478,6 +530,22 @@ class VideoStream:
             frames = torch.empty(frames.shape, dtype=frames.dtype, pin_memory=True).copy_(frames)
         res = self._engine.run(frames, [k for k in range(self.n) if slots[k]], out == 'host')
         self._pending = [False] * self.n
+        rep = self._engine.report
+        if rep is not None:
+            # [k,3n] int32: words [0,2n) the n float64 scores, [2n,3n) the n cut flags.  rep is the engine's report
+            # buffer, reused by the next push, so the score words are copied into a new [k,2n] array first: a
+            # slice's .contiguous() / ascontiguousarray is no copy when k == 1, and its row stride of 3n words
+            # cannot be viewed as float64 for odd n.  On the device this runs on the current stream.
+            n = self.n
+            if out == 'host':
+                r = rep.numpy()
+                self.last_scores = r[:, :2 * n].copy(order='C').view(np.float64).T.copy()
+                self.last_cuts = (r[:, 2 * n:] != 0).T.copy()
+            else:
+                words = torch.empty((rep.shape[0], 2 * n), dtype=torch.int32, device=rep.device)
+                words.copy_(rep[:, :2 * n])
+                self.last_scores = words.view(torch.float64).t().contiguous()
+                self.last_cuts = (rep[:, 2 * n:] != 0).t().contiguous()
         return res.numpy() if out == 'host' else res
 
     def _check_frames(self, frames):
@@ -529,7 +597,17 @@ class VideoStream:
         return StreamEngine(self.net, self.n, self.c, self.h, self.w, dev, u8_input=self.input == 'uint8',
                             bgr=self.channel_order == 'bgr', yuv_in=yuv_in, yuv_out=yuv_out,
                             in_color=self.in_color, out_color=self.out_color, out_size=self.out_size,
-                            resize_filter=self.resize_filter)
+                            resize_filter=self.resize_filter, scene_cut=self.scene_cut)
+
+
+def _check_scene_cut(threshold):
+    """scene_cut -> float threshold, or ValueError: a real number (not a bool) in (0, 100]; NaN and inf refused."""
+    if isinstance(threshold, bool) or not isinstance(threshold, numbers.Real):
+        raise ValueError(f'scene_cut must be None or a threshold in (0, 100], got {threshold!r}')
+    t = float(threshold)
+    if not (math.isfinite(t) and ops.scene_cut_threshold_ok(t)):
+        raise ValueError(f'scene_cut threshold must be finite and in (0, 100], got {threshold!r}')
+    return t
 
 
 def _check_out_size(out_size, H, W, out_format):

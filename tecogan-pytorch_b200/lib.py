@@ -5,7 +5,7 @@ The library is built in-tree by ``__graft_entry__.build()`` (``make -C csrc``).
 """
 import ctypes
 import os
-from ctypes import c_char_p, c_float, c_int, c_int32, c_size_t, c_void_p
+from ctypes import c_char_p, c_double, c_float, c_int, c_int32, c_size_t, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libtecogan_b200.so')
@@ -20,6 +20,7 @@ EPI_NHWC_F16, EPI_FLOW_NCHW_F32, EPI_OUT_NCHW_F32, EPI_NHWC_F16_POOL2 = 0, 1, 2,
 AMODE_AUTO, AMODE_HALO, AMODE_TAP = 0, 1, 2
 YUV_NV12, YUV_I420, YUV_P010, YUV_I420_10 = 0, 1, 2, 3
 RESAMPLE_BICUBIC, RESAMPLE_LANCZOS3 = 0, 1
+SCENE_CUT_WORK_BYTES = 16            # TG_SCENE_CUT_WORK_BYTES: workspace of tg_scene_cut per slot
 
 
 class ConvDesc(ctypes.Structure):
@@ -109,6 +110,7 @@ _SIGNATURES = {
     'tg_resample_table': (c_int, [c_int, c_int, c_int, c_int, _P, _P]),
     'tg_resample_nchw_f32': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, _P, c_int, c_int, c_int,
                                      _P, _P, _P]),
+    'tg_scene_cut': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, c_double, _P, _P, _P, _P, _P]),
     'tg_downsample_bd_nchw_f32': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_debug_set_conv_timers': (c_int, [_P]),
     # ---- training (generator backward)

@@ -356,7 +356,7 @@ class FRNet(BaseSequenceGenerator):
         return infer_clips(self, lr_data, device)
 
     def stream(self, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb', in_color='bt601',
-               out_color='bt601', out_size=None, resize_filter='bicubic'):
+               out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None):
         """A VideoStream of n lock-stepped slots of h x w LR frames: video pushed in chunks of any length, the
         recurrent state carried from one push to the next, and a slot restarted (reset=) when its video ends and
         the next one begins while the other slots keep running.
@@ -388,12 +388,18 @@ class FRNet(BaseSequenceGenerator):
         (Image.resize on 'F' images, as oracle/resample.py specifies), widened by the ratio on a downscale.  Each
         axis needs H/4 <= Ho <= 2H (likewise W), and even Ho and Wo for YUV output.  out_size=(H, W) gives the
         bytes of the stream without it.
+        scene_cut=threshold (a number in (0, 100]; 10.0 is a good start, the default of ffmpeg's scdet) detects
+        hard cuts on the device, inside the step: each frame is scored against the previous one of its slot (the
+        mean absolute difference of the 8-bit codes and its change, as oracle/scene_cut.py specifies), and a score
+        >= threshold restarts the slot at that frame exactly as reset= would have.  After each push the stream's
+        last_cuts (bool [n,k]) and last_scores (float64 [n,k]) tell where, e.g. to ask the encoder for a keyframe.
+        None (the default) turns detection off; any input and output format work with it.
         Temporal padding (pad_sequence, base_model.py:230-251) stays the caller's job: for p reflect-padded
         frames, push frames[:, 1:1+p].flip(1) first and drop those p outputs.  The CUDA graphs are captured by the first push; the stream holds the
         net."""
         from .engine import VideoStream
         return VideoStream(self, n, h, w, device, input, channel_order, out_format, in_color, out_color, out_size,
-                           resize_filter)
+                           resize_filter, scene_cut)
 
     def refresh_packed_weights(self, force=False):
         self.fnet._cache.refresh_all(force)

@@ -653,6 +653,44 @@ def resample(x, rows, cols, out_u8=None, out_f32=None):
     return out
 
 
+def scene_cut_threshold_ok(threshold):
+    """tg_scene_cut takes a finite threshold in (0, 100]."""
+    return 0.0 < threshold <= 100.0
+
+
+def scene_cut_work(n, device):
+    """The zeroed workspace of tg_scene_cut for n slots (each launch leaves it zeroed again)."""
+    return torch.zeros(n * L.SCENE_CUT_WORK_BYTES // 8, dtype=torch.int64, device=device)
+
+
+def scene_cut(lr_curr, lr_prev, reset, threshold, prev_mafd, work, score, cut):
+    """tg_scene_cut: per slot k of lr_curr / lr_prev (fp32 [n,c,h,w]), score[k] (float64) and cut[k] (int32 0 / 1)
+    of oracle/scene_cut.py, with prev_mafd (float64 [n]) the state it updates and reset (int32 [n], or None) the
+    caller's resets of this step.  work: scene_cut_work(n) (int64 tensor of n * SCENE_CUT_WORK_BYTES bytes)."""
+    name = 'scene_cut'
+    _req(lr_curr, torch.float32, 'lr_curr', 4)
+    _req(lr_prev, torch.float32, 'lr_prev', 4)
+    n, c, h, w = lr_curr.shape
+    if tuple(lr_prev.shape) != (n, c, h, w):
+        raise L.TecoganB200Error(f'{name}: lr_prev {tuple(lr_prev.shape)} != lr_curr {(n, c, h, w)}')
+    for t, dtype, nm in ((prev_mafd, torch.float64, 'prev_mafd'), (score, torch.float64, 'score'),
+                         (cut, torch.int32, 'cut'), (reset, torch.int32, 'reset')):
+        if t is None and nm == 'reset':
+            continue
+        _req(t, dtype, nm, 1)
+        if t.shape[0] != n:
+            raise L.TecoganB200Error(f'{name}: {nm} has {t.shape[0]} entries, expected {n}')
+    _req(work, torch.int64, 'work', 1)
+    if work.numel() * 8 != n * L.SCENE_CUT_WORK_BYTES:
+        raise L.TecoganB200Error(f'{name}: work has {work.numel() * 8} bytes, expected {n * L.SCENE_CUT_WORK_BYTES}')
+    for t in (lr_prev, reset, prev_mafd, work, score, cut):
+        if t is not None and t.device != lr_curr.device:
+            raise L.TecoganB200Error(f'{name}: tensors on different devices')
+    L.check(L.load().tg_scene_cut(_ptr(lr_curr), _ptr(lr_prev), n, c, h, w, _ptr(reset), float(threshold),
+                                  _ptr(prev_mafd), _ptr(work), _ptr(score), _ptr(cut), _stream()), 'tg_scene_cut')
+    return score, cut
+
+
 # ============================================================================ training (backward) ops
 class GradScale:
     """Device-resident loss scale {scale, 1/scale} of the fp16 gradient path (tg_grad_scale_from_amax /

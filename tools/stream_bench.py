@@ -22,10 +22,19 @@ each run ends in a device synchronisation; one untimed warm-up run of every path
                              an RGB stream with out_size=(Ho, Wo) (bicubic unless marked), k = 16: 402x960 (3/4) and
                              804x1920 (3/2)
   push_nv12_709_resize_402x960_host_chunk16  uint8 in, NV12 / BT.709 out at out_size=(402, 960), k = 16
+  push_u8_scene_host_chunk1/16
+                             push_u8_host_chunk1/16 on a stream with scene_cut=10 (the same frames have no cut, so
+                             the bytes must equal infer_sequence's and no cut may be reported); each push's last_cuts
+                             is read inside the timed pushes and summed over the timed reps (scene_cuts_reported);
+                             alternates with the paths above in every rep
   resample_us                tg_resample_nchw_f32 per step (4 HR frames -> uint8 NHWC or fp32 NCHW), timed as below,
                              with its algorithmic bytes (n*3*H*W*4 read, n*Ho*Wo*3 or *12 written) and TB/s
   encode_us                  tg_rgb_u8_to_yuv420 per step (4 HR frames -> NV12 / I420) and tg_rgb_to_yuv per step
                              (uint8 -> NV12 / BT.709; fp32 NCHW -> P010 / BT.709), timed the same way
+  scene_us                   tg_scene_cut per step (4 slots of 3x134x320 scored against another 4, with its
+                             algorithmic bytes 2*n*c*h*w*4 and TB/s; 16 disjoint pairs of frame sets, 66 MB, rotate so
+                             that L2 does not hold the next launch's input) and the reset-only tg_stream_frame_in that
+                             follows it in the graph, on a step without cuts (an all-zero cut mask), timed the same way
 All uint8 paths process the same frames (uint8, and the reference loader's float32 / 255 of them), so their
 outputs are also compared byte for byte.  The NV12 paths take oracle/yuv_oracle.py's NV12 of those frames; their
 output is compared with the oracle's NV12 of the RGB output for the frames that NV12 decodes to; the BT.709 NV12
@@ -99,8 +108,13 @@ def main():
         torch.cuda.synchronize()
         return n * t / (time.perf_counter() - t0), out
 
-    def pushes(stream, src, chunk, out):
-        return [stream.push(src[:, i:i + chunk], out=out) for i in range(0, t, chunk)]
+    def pushes(stream, src, chunk, out, cuts=None):
+        res = []
+        for i in range(0, t, chunk):
+            res.append(stream.push(src[:, i:i + chunk], out=out))
+            if cuts is not None:                 # a caller of a scene_cut stream reads each push's report
+                cuts[0] += int(stream.last_cuts.sum())
+        return res
 
     streams = {'push_u8_host_chunk1': (1, u8_pin, 'host'), 'push_u8_host_chunk16': (16, u8_pin, 'host'),
                'push_u8_device': (16, u8_dev, 'device'), 'push_nv12_host_chunk1': (1, nv12_pin, 'host'),
@@ -117,6 +131,10 @@ def main():
     for k, kw in resized.items():
         streams[k] = (16, u8_pin, 'host')
         kinds[k] = kw
+    for chunk in (1, 16):
+        streams[f'push_u8_scene_host_chunk{chunk}'] = (chunk, u8_pin, 'host')
+        kinds[f'push_u8_scene_host_chunk{chunk}'] = dict(scene_cut=10.0)
+    scene_cuts = {k: 0 for k in streams if 'scene' in k}
     opened = {k: net.stream(n, h, w, device=dev, **kinds.get(k, dict(input='nv12', out_format='nv12') if 'nv12' in k
                                                                  else {}))
               for k in streams}
@@ -132,9 +150,12 @@ def main():
         for k, (chunk, src, out) in streams.items():
             opened[k].reset(range(n))
             outputs[k] = None
-            fps, outputs[k] = timed(lambda: pushes(opened[k], src, chunk, out))
+            counter = [0] if k in scene_cuts else None
+            fps, outputs[k] = timed(lambda: pushes(opened[k], src, chunk, out, counter))
             if rep:
                 runs[k].append(fps)
+                if counter is not None:
+                    scene_cuts[k] += counter[0]
     ref = outputs['infer_sequence_fp32_host']
     # the NV12 paths' specification: the oracle's NV12 of the RGB output for the frames the NV12 input decodes to
     rgb_in = Y.yuv420_to_rgb(nv12, 'nv12')
@@ -210,6 +231,7 @@ def main():
     nv12_launches = opened['push_nv12_device']._engine.launches_per_step
     p010_launches = opened['push_p010_709_host_chunk16']._engine.launches_per_step
     resize_launches = opened['push_u8_resize_402x960_host_chunk16']._engine.launches_per_step
+    scene_launches = opened['push_u8_scene_host_chunk16']._engine.launches_per_step
     for st in opened.values():
         st.close()
 
@@ -264,6 +286,26 @@ def main():
         resample_bytes[name] = n * c * H * W * 4 + n * Ho * Wo * c * (4 if f32_out else 1)
         del outs
     encode10_bytes = n * H * W * 3 * 4 + n * 3 * H // 2 * W * 2
+    # tg_scene_cut alone: 16 disjoint (current, previous) pairs of 4 x 3x134x320 fp32 frames (66 MB, more than the
+    # 50 MB L2), then the reset-only tg_stream_frame_in with an all-zero cut mask (what the graph runs on a step
+    # without cuts)
+    ns = 16
+    scene_a = [torch.rand(n, c, h, w, device=dev) for _ in range(ns)]
+    scene_b = [torch.rand(n, c, h, w, device=dev) for _ in range(ns)]
+    prev_mafd = torch.full((n,), -1.0, dtype=torch.float64, device=dev)
+    work = ops.scene_cut_work(n, dev)
+    score = torch.empty(n, dtype=torch.float64, device=dev)
+    cut = torch.zeros(n, dtype=torch.int32, device=dev)
+    no_reset = torch.zeros(n, dtype=torch.int32, device=dev)
+    scene = {}
+    sec = bench._time_graph(lambda i: ops.scene_cut(scene_a[i], scene_b[i], no_reset, 10.0, prev_mafd, work, score,
+                                                    cut), ns, reps, torch)
+    scene['scene_cut'] = sec * 1e6
+    del scene_a, scene_b
+    cut.zero_()                          # the scene_cut launches above left their own flags in cut
+    sec = bench._time_graph(lambda i: ops.stream_frame_in(None, cut, lrs[i], prev, hrp, s), nb, reps, torch)
+    scene['reset_only_frame_in_no_cut'] = sec * 1e6
+    scene_bytes = 2 * n * c * h * w * 4
 
     line = {
         'metric': 'hr_frames_per_sec_4xBD_3x134x320_streamed', 'unit': 'frames/s',
@@ -274,6 +316,10 @@ def main():
         'frame_in_us': frame_in,
         'encode_us': encode,
         'resample_us': resample,
+        'scene_us': scene,
+        'scene_bytes_per_step': scene_bytes,
+        'scene_tb_per_s': scene_bytes / scene['scene_cut'] * 1e-6,
+        'scene_cuts_reported': scene_cuts,          # summed over the timed pushes of every timed rep
         'resample_bytes_per_step': resample_bytes,
         'resample_tb_per_s': {k: resample_bytes[k] / v * 1e-6 for k, v in resample.items()},
         'encode_bytes_per_step': encode_bytes,
@@ -284,7 +330,7 @@ def main():
         'd2h_bytes_per_step': {'uint8': n * c * H * W, 'nv12': n * 3 * H // 2 * W},
         'launches_per_step': {'infer_sequence': T.engine.get_engine(net, n, c, h, w, dev).launches_per_step,
                               'push': stream_launches, 'push_nv12': nv12_launches, 'push_p010': p010_launches,
-                              'push_resize': resize_launches},
+                              'push_resize': resize_launches, 'push_scene': scene_launches},
     }
     print(json.dumps(line), flush=True)
 
