@@ -366,7 +366,8 @@ int tg_downsample_bd_nchw_f32(const float* x, const float* k2d, float* y, int n,
  * them); kernels producing fp32 results multiply by 1/scale.  scale == NULL means 1.
  * ====================================================================== */
 size_t tg_grad_scale_workspace_bytes(void);   /* 16: {scale, 1/scale} fp32 + amax scratch (zero it once) */
-/* scale = 2^floor(log2(target / max(|a|,|b|))) clamped to 2^+-24 (1 when all-zero); b may be NULL */
+/* scale = 2^floor(log2(target / max(|a|,|b|))) clamped to 2^+-24, the exponent computed exactly (1 when all-zero
+ * or when the maximum is inf / NaN); b may be NULL */
 int tg_grad_scale_from_amax(const float* a, size_t na, const float* b, size_t nb, float target, void* ws,
                             void* stream);
 /* (a [+ b]) * scale : NCHW fp32 [n,c,h,w] -> NHWC fp16 [n,h,w,cpad] (pad channels zero) */

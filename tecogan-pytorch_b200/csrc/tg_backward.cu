@@ -22,7 +22,7 @@ inline int bgrid(size_t total, int block) {
 
 // ------------------------------------------------------------------ loss scale
 // amax over up to two fp32 tensors (uint compare of |x| bit patterns), then
-// scale = 2^floor(log2(target / amax)) clamped to [2^-24, 2^24]; amax == 0 -> scale 1.
+// scale = 2^floor(log2(target / amax)) clamped to [2^-24, 2^24]; amax == 0 or not finite -> scale 1.
 __global__ void amax_kernel(const float* __restrict__ a, size_t na, const float* __restrict__ b, size_t nb,
                             unsigned int* __restrict__ amax_bits) {
   tg_pdl_wait();
@@ -40,7 +40,13 @@ __global__ void scale_from_amax_kernel(unsigned int* __restrict__ amax_bits, flo
   const float amax = __uint_as_float(*amax_bits);
   float s = 1.f;
   if (amax > 0.f && isfinite(amax)) {
-    int e = (int)floorf(log2f(target / amax));
+    // the exponent exactly, without rounding target / amax or its log2 (floorf(log2f(target / amax)) is one
+    // too large when the quotient falls just below a power of two): with amax = ma * 2^ea and
+    // target = mt * 2^et, ma and mt in [0.5, 1) (frexpf, exact for denormals too), target / amax =
+    // (mt / ma) * 2^(et - ea) with mt / ma in (0.5, 2), below 1 exactly when mt < ma.
+    int ea, et;
+    const float ma = frexpf(amax, &ea), mt = frexpf(target, &et);
+    int e = et - ea - (mt < ma ? 1 : 0);
     e = e < -24 ? -24 : (e > 24 ? 24 : e);
     s = exp2f((float)e);
   }

@@ -7,6 +7,8 @@ residual skips, frame order of the BPTT, n-major vs t-major flow layouts) can be
 against the reference-generated gradient fixture BEFORE any GPU time is spent; the GPU tests then
 only have to establish that each kernel honours its contract.  Never imported by the package.
 """
+import math
+
 import torch
 import torch.nn.functional as F
 
@@ -23,14 +25,15 @@ def pad64(c):
 
 
 def to_nchw(x, c):            # NHWC fp16 -> NCHW fp32 (first c channels)
-    return x[..., :c].float().permute(0, 3, 1, 2).contiguous()
+    return x[..., :c].to(COMPUTE).permute(0, 3, 1, 2).contiguous()
 
 
 STORAGE = torch.float16      # torch.float32: no rounding anywhere -> the orchestration must be EXACT
+COMPUTE = torch.float32      # arithmetic type (tests/kernel_contracts.py: float64 references on the kernels' inputs)
 
 
 def _store(v):
-    return v.to(STORAGE).float()
+    return v.to(STORAGE).to(COMPUTE)
 
 
 def to_nhwc(x, cpad, out=None):   # NCHW fp32 -> NHWC (fp16 storage) padded
@@ -70,7 +73,7 @@ class PackedConv:
 
     def refresh(self, weight, bias, force=False):
         self.w = _store(weight.detach())        # fp16 storage of the packed weights
-        self.b = bias.detach().float()
+        self.b = bias.detach().to(COMPUTE)
         self.packed = self.w
 
     def __call__(self, x, y=None, residual=None, **kw):
@@ -129,18 +132,21 @@ class GradScale:
         self.ws = torch.tensor([1.0, 1.0, 0.0, 0.0])
 
     def _set(self, amax, target=None):
+        # 2^floor(log2(target / amax)) with the exponent computed exactly: amax = ma * 2^ea, target = mt * 2^et
+        # (ma, mt in [0.5, 1)) -> floor(log2(target / amax)) = et - ea - (mt < ma)
         s = 1.0
-        if amax > 0:
-            import math
-            e = max(-24, min(24, math.floor(math.log2((target or self.TARGET) / amax))))
-            s = 2.0 ** e
+        if amax > 0 and math.isfinite(amax):
+            ma, ea = math.frexp(amax)
+            mt, et = math.frexp(target or self.TARGET)
+            s = 2.0 ** max(-24, min(24, et - ea - (mt < ma)))
         self.ws[0], self.ws[1] = s, 1.0 / s
         return self
 
     def from_amax(self, a, b=None, target=None):
         amax = float(a.abs().max())
         if b is not None:
-            amax = max(amax, float(b.abs().max()))
+            bmax = float(b.abs().max())
+            amax = bmax if math.isnan(bmax) else max(amax, bmax)
         return self._set(amax, target)
 
     @property
@@ -169,7 +175,7 @@ def wgrad(fwd, x, dz, dw, scale=None, impl=None, max_ctas=0, db=None):
 
 
 def bias_grad(dz, db, scale=None):
-    db += dz[..., :db.numel()].float().sum((0, 1, 2)) / _s(scale)
+    db += dz[..., :db.numel()].to(COMPUTE).sum((0, 1, 2)) / _s(scale)
     return db
 
 
@@ -179,7 +185,7 @@ def grad_pack(a, b=None, scale=None, cpad=64, y=None):
 
 
 def pack_pair(x1, x2, y=None, cpad=64):
-    return to_nhwc(torch.cat([x1, x2], 1), cpad)
+    return to_nhwc(torch.cat([x1, x2], 1), cpad, out=y)
 
 
 def nchw_to_nhwc(x, cpad=None, y=None):
@@ -188,17 +194,21 @@ def nchw_to_nhwc(x, cpad=None, y=None):
 
 def maxpool2x2(x, y=None):
     c = x.shape[-1]
-    return to_nhwc(F.max_pool2d(to_nchw(x, c), 2, 2), c)
+    return to_nhwc(F.max_pool2d(to_nchw(x, c), 2, 2), c, out=y)
 
 
 def upsample2x(x, y=None):
     c = x.shape[-1]
-    return to_nhwc(F.interpolate(to_nchw(x, c), scale_factor=2, mode='bilinear', align_corners=False), c)
+    return to_nhwc(F.interpolate(to_nchw(x, c), scale_factor=2, mode='bilinear', align_corners=False), c, out=y)
+
+
+ABS_TAPS = False             # |filter taps|: the magnitude of the terms, for the error bounds of tests/kernel_contracts.py
 
 
 def _up(x, scale, up_mode):
     from oracle.ops_oracle import bicubic_kernels
-    p = {'upsample_func.kernels': torch.from_numpy(bicubic_kernels(scale))}
+    k = torch.from_numpy(bicubic_kernels(scale)).to(x.dtype)
+    p = {'upsample_func.kernels': k.abs() if ABS_TAPS else k}
     return R.upsample(p, x, scale, 'BD' if up_mode == UP_BICUBIC else 'BI')
 
 
@@ -216,9 +226,15 @@ def upsample(x, scale, up_mode, out_hw=None, mul=1.0, y=None, accumulate=False):
 @torch.enable_grad()
 def upsample_bwd(gy, scale_factor, up_mode, mul=1.0, gx=None, accumulate=False):
     n, c, H, W = gy.shape
-    x = torch.zeros(n, c, H // scale_factor, W // scale_factor, requires_grad=True)
+    x = torch.zeros(n, c, H // scale_factor, W // scale_factor, dtype=gy.dtype, requires_grad=True)
     g, = torch.autograd.grad(mul * _up(x, scale_factor, up_mode), [x], gy)
-    return g
+    if gx is None:
+        return g
+    if accumulate:
+        gx += g
+    else:
+        gx.copy_(g)
+    return gx
 
 
 def warp_s2d_concat_hrflow(hr_prev, hr_flow, lr_curr, scale, out=None, cpad=64):
@@ -246,7 +262,7 @@ def maxpool2x2_bwd(x, gy, act, gx=None):
     c = x.shape[-1]
     a = to_nchw(x, c).requires_grad_(True)
     g, = torch.autograd.grad(F.max_pool2d(a, 2, 2), [a], to_nchw(gy, c))
-    return to_nhwc(g * _dact(a.detach(), act), c)
+    return to_nhwc(g * _dact(a.detach(), act), c, out=gx)
 
 
 @torch.enable_grad()
@@ -255,18 +271,25 @@ def upsample2x_bwd(gy, m, act, gx=None):
     a = to_nchw(m, c).requires_grad_(True)
     g, = torch.autograd.grad(F.interpolate(a, scale_factor=2, mode='bilinear', align_corners=False), [a],
                              to_nchw(gy, c))
-    return to_nhwc(g * _dact(a.detach(), act), c)
+    return to_nhwc(g * _dact(a.detach(), act), c, out=gx)
 
 
 def flow_head_bwd(gflow, flow, scale, gflow2=None, cpad=64, dz=None):
     g = gflow if gflow2 is None else gflow + gflow2
     v = g * (24.0 - flow * flow / 24.0)
     scale._set(float(v.abs().max()))
-    return to_nhwc(v * scale.s, cpad)
+    return to_nhwc(v * scale.s, cpad, out=dz)
+
+
+def _out(v, y):
+    if y is None:
+        return v
+    y.copy_(v)
+    return y
 
 
 def backward_warp(x, flow, y=None):
-    return R.warp(x, flow)
+    return _out(R.warp(x, flow), y)
 
 
 @torch.enable_grad()
@@ -277,25 +300,30 @@ def backward_warp_bwd(x, flow, gy, need_x=True, need_flow=True):
 
 
 def space_to_depth(x, scale, y=None):
-    return R.s2d(x, scale)
+    return _out(R.s2d(x, scale), y)
 
 
 @torch.enable_grad()
 def depth_to_space(gy, scale_factor):
     n, cs, oh, ow = gy.shape
-    x = torch.zeros(n, cs // scale_factor ** 2, oh * scale_factor, ow * scale_factor, requires_grad=True)
+    x = torch.zeros(n, cs // scale_factor ** 2, oh * scale_factor, ow * scale_factor, dtype=gy.dtype,
+                    requires_grad=True)
     g, = torch.autograd.grad(R.s2d(x, scale_factor), [x], gy)
     return g
+
+
+# every op of the training path, in the package's op layer, that this module stands in for
+FAKED = ('PackedConv', 'PackedDgrad', 'GradScale', 'wgrad', 'bias_grad', 'grad_pack', 'pack_pair', 'nchw_to_nhwc',
+         'maxpool2x2', 'upsample2x', 'upsample', 'upsample_bwd', 'warp_s2d_concat_hrflow', 'warp_s2d_concat_bwd',
+         'maxpool2x2_bwd', 'upsample2x_bwd', 'flow_head_bwd', 'backward_warp', 'backward_warp_bwd',
+         'space_to_depth', 'depth_to_space')
 
 
 def install(monkeypatch, pkg_ops, networks, net_utils, autograd):
     """Route the package's op layer to this module (CPU tensors accepted)."""
     import sys
     me = sys.modules[__name__]
-    for name in ('PackedConv', 'PackedDgrad', 'GradScale', 'wgrad', 'bias_grad', 'grad_pack', 'pack_pair', 'nchw_to_nhwc',
-                 'maxpool2x2', 'upsample2x', 'upsample', 'upsample_bwd', 'warp_s2d_concat_hrflow', 'warp_s2d_concat_bwd',
-                 'maxpool2x2_bwd', 'upsample2x_bwd', 'flow_head_bwd', 'backward_warp', 'backward_warp_bwd',
-                 'space_to_depth', 'depth_to_space'):
+    for name in FAKED:
         monkeypatch.setattr(pkg_ops, name, getattr(me, name))
     monkeypatch.setattr(pkg_ops, 'chain_enabled', lambda: False)
     monkeypatch.setattr(networks, '_cuda_f32', lambda t, name: t.detach().float().contiguous())
