@@ -19,7 +19,8 @@
 //             CTA's tiles alternately, each with its own ring of smem stages: wgmma -> accumulators
 //             staged to a per-consumer fp32 smem tile -> one thread per pixel applies bias / act /
 //             residual (or the derivative, pool, pixel-shuffle and thin-head epilogues) and writes
-//             the pixel's 128-byte NHWC row.  One consumer's epilogue overlaps the other's MMAs.
+//             the pixel's 128-byte NHWC row.  On the forward halo and split-K paths the consumers take
+//             turns issuing their MMAs, so that one's epilogue runs under the other's MMAs.
 //             The tap-mode transposed conv keeps 4 parity accumulators (1/2/2/4 taps), computed and
 //             stored one after the other; each stores its pixel's output of that parity (pixel shuffle).
 //
@@ -234,6 +235,18 @@ __device__ __forceinline__ void consumer_halo_pxn(const TgMaps& maps, const KPar
   const uint32_t w16 = gmma_addr16(base + p.off_b), btb16 = p.b_stage_bytes >> 4;
   const bool has_res = !POOL && d.residual != nullptr;
   const int bar_id = 1 + cw;
+  // Turns on the tensor pipe.  The CTA's tiles blockIdx.x + i * gridDim.x, i = 0, 1, 2, ..., go to consumer i & 1.
+  // The owner of tile i > 0 issues its MMAs only after the other consumer has issued (and committed) tile i - 1:
+  // it waits on turn[cw], on which the other consumer's four warps arrive after each of their commits.  The
+  // tensor pipe then runs the two consumers' MMAs one tile after the other instead of sharing it, so one
+  // consumer's epilogue runs under the other's MMAs rather than both epilogues leaving the pipe idle together.
+  // No deadlock: every tile i > 0 has its tile i - 1 in the same CTA, and issuing tile i - 1 waits only for
+  // tile i - 2's issue and for memory (the stage, the store drain), never for anything of tile i or later,
+  // whatever the tile counts of the two consumers (1 / 0, or unequal).  Waits and arrivals on a barrier
+  // alternate (an arrival on turn[c] needs the wait that preceded the arriving consumer's own issue), so a parity
+  // wait is never more than one phase behind; the arrival after a consumer's last tile has no waiter and is harmless.
+  const uint32_t turn_mine = base + 32 * kMaxRing + 56 + 8u * cw, turn_other = base + 32 * kMaxRing + 56 + 8u * (cw ^ 1);
+  uint32_t tphase = 0;
   // stmatrix / ldmatrix: lane l addresses pixel row l%8 of 8x8 matrix m = l/8 = (tile row 2*jp + m/2,
   // 8-channel chunk 2*q + m%2); the swizzled offset of (pixel px, chunk) is px*128 + ((chunk ^ px%8) << 4).
   // POOL: matrix m = (pooled row pair 2*ip + m/2, chunk 2*q + m%2), its column 2*c + e = pooled pixel
@@ -261,6 +274,8 @@ __device__ __forceinline__ void consumer_halo_pxn(const TgMaps& maps, const KPar
       const int s = stage;
       mbar_wait_mma(bar_full + 8 * s, phase);
       if (++stage == p.ring) { stage = 0; phase ^= 1u; }
+      // take the turn only once the tile's first stage is here, so that it is never held while waiting on memory
+      if (c == 0 && tile >= (int)gridDim.x) { mbar_wait_mma(turn_mine, tphase); tphase ^= 1u; }
       const uint32_t x16 = gmma_addr16(stage0 + (uint32_t)s * p.stage_bytes);
       wgmma_fence();
 #pragma unroll
@@ -275,6 +290,7 @@ __device__ __forceinline__ void consumer_halo_pxn(const TgMaps& maps, const KPar
                        (g == 0 && c == 0 && k == 0) ? 0u : 1u);
       }
       wgmma_commit();
+      if (c == p.chunks - 1) { __syncwarp(); if (lane == 0) mbar_arrive(turn_other); }   // pass the turn
       wgmma_wait<1>();
       if (pend >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_empty + 8 * pend); }
       pend = s;
@@ -392,6 +408,10 @@ __device__ __forceinline__ void consumer_splitk(const TgMaps& maps, const KParam
   const uint32_t mat_off = (uint32_t)(8 * ((lane >> 3) >> 1) + kk) * sb +
                            ((uint32_t)(2 * (q - rank * wpr) + ((lane >> 3) & 1)) << 4);
   const int t0 = (int)cluster_id_x(), tstep = (int)cluster_count_x();
+  // turns on the tensor pipe as in consumer_halo_pxn, over the CTA's tiles t0 + i * tstep; the waits for
+  // peer CTAs (hand-back, partials) come after a tile's MMAs are issued, so the argument there holds here too
+  const uint32_t turn_mine = base + 32 * kMaxRing + 56 + 8u * cw, turn_other = base + 32 * kMaxRing + 56 + 8u * (cw ^ 1);
+  uint32_t tphase = 0;
   int stage = 0, it = 0;
   uint32_t phase = 0;
   float acc[64];
@@ -408,6 +428,7 @@ __device__ __forceinline__ void consumer_splitk(const TgMaps& maps, const KParam
     const int s = stage;
     mbar_wait_mma(bar_full + 8 * s, phase);
     if (++stage == p.ring) { stage = 0; phase ^= 1u; }
+    if (tile >= tstep) { mbar_wait_mma(turn_mine, tphase); tphase ^= 1u; }
     const uint32_t x16 = gmma_addr16(stage0 + (uint32_t)s * p.stage_bytes);
     wgmma_fence();
 #pragma unroll
@@ -420,6 +441,8 @@ __device__ __forceinline__ void consumer_splitk(const TgMaps& maps, const KParam
         wgmma_n128(acc, w_hi | (uint64_t)(a16 + 2u * k), x_hi | (uint64_t)(b16 + 2u * k), (g == 0 && k == 0) ? 0u : 1u);
     }
     wgmma_commit();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(turn_other);   // pass the turn
     wgmma_wait<0>();
     __syncwarp();
     if (lane == 0) mbar_arrive(bar_empty + 8 * s);
@@ -589,6 +612,7 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
   const uint32_t bar_res = bar_b + 8;                      // [2] residual tile of consumer c
   const uint32_t bar_rfull = bar_b + 24;                   // [2] MODE_SPLITK: partials received, consumer c
   const uint32_t bar_free = bar_b + 40;                    // [2] MODE_SPLITK: peers handed back their buffers
+  const uint32_t bar_turn = bar_b + 56;                    // [2] pixels-on-N conv3x3 / split-K: consumer c may issue
   float* bias_s = reinterpret_cast<float*>(sm + 1024);
   static_assert(!(KIND == TG_CONV_3X3_S2 && MODE != MODE_TAP), "the stride-2 conv runs in tap mode only");
   constexpr bool kPxN = pixels_on_n<KIND, MODE, BWD>();
@@ -614,6 +638,10 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
         mbar_init(bar_rfull + 8 * c, 1);             // the owner's expect_tx; the bytes come from the peers
         mbar_init(bar_free + 8 * c, p.chunks - 1);   // one hand-back per peer
       }
+    }
+    if (kSplitK || (kPxN && KIND == TG_CONV_3X3)) {
+      mbar_init(bar_turn, 4);              // one arrival per warp of the other consumer
+      mbar_init(bar_turn + 8, 4);
     }
     fence_barrier_init();
   }
