@@ -348,6 +348,54 @@ int tg_resample_nchw_f32(const float* x, int n, int c, int H, int W, const int32
 int tg_scene_cut(const float* lr_curr, const float* lr_prev, int n, int c, int h, int w, const int32_t* reset,
                  double threshold, double* prev_mafd, void* work, double* score, int32_t* cut, void* stream);
 
+/* ------------------------------------------------------------------------
+ * Video quality metrics: PSNR and tOF as TecoGAN's MetricCalculator computes them (oracle/metrics_oracle.py and
+ * oracle/farneback.py are the specification).
+ * ---------------------------------------------------------------------- */
+enum { TG_PSNR_NONE = 0, TG_PSNR_RGB = 1, TG_PSNR_Y = 2 };
+/* One read of t uint8 RGB frames true_u8 [t,ht,wt,3] and pred_u8 [t,hp,wp,3], both cropped to h = min(ht, hp),
+ * w = min(wt, wp) (their top-left corner):
+ *   gray [2,t,h,w] uint8 (true then pred) = (9798 R + 19235 G + 3735 B + 16384) >> 15, cv2 COLOR_RGB2GRAY bit for
+ *        bit; NULL when not wanted.  With pred_u8 NULL (psnr TG_PSNR_NONE) only the true frames: gray [t,ht,wt].
+ *   sse  [t] uint64 = the exact integer sum of squared differences per frame over R, G, B (TG_PSNR_RGB) or over the
+ *        Y of data_utils.rgb_to_ycbcr (TG_PSNR_Y: float64 r*T0 + g*T1 + b*T2 + 16 left to right without FMA, rounded
+ *        half to even, and one lower for the three colours (1,173,225), (12,174,191), (24,46,73) whose numpy matmul
+ *        rounds the other way).  Zeroed by the call (a memset on the stream); NULL exactly when psnr is
+ *        TG_PSNR_NONE.  PSNR = 20 log10(255 / sqrt(sse / count)) then equals the reference's numpy result.
+ * TG_E_INVALID: null true frames, non-positive sizes, bad psnr mode, sse given or missing against the mode, nothing
+ * requested, sse not 8-byte aligned; TG_E_UNSUPPORTED: t > 65535. */
+int tg_metrics_frames_in(const uint8_t* true_u8, int ht, int wt, const uint8_t* pred_u8, int hp, int wp, int t,
+                         int psnr, uint8_t* gray, unsigned long long* sse, void* stream);
+
+/* Farneback dense optical flow, cv2.calcOpticalFlowFarneback(prev, next, None, pyr_scale, levels, winsize,
+ * iterations, poly_n, poly_sigma, flags=0), in fp32.  (pyr_scale, poly_sigma float64.) */
+typedef struct tg_farneback_params {
+  double pyr_scale;     /* (0, 1) */
+  int32_t levels;       /* >= 0 */
+  int32_t winsize;      /* box window, [1, 63] */
+  int32_t iterations;   /* >= 1 */
+  int32_t poly_n;       /* 5 or 7 */
+  double poly_sigma;    /* > 0 */
+  int32_t flags;        /* 0: OPTFLOW_USE_INITIAL_FLOW and OPTFLOW_FARNEBACK_GAUSSIAN are not implemented */
+  int32_t reserved;
+} tg_farneback_params;
+/* Bytes of the workspace of tg_farneback for `groups` groups of t frames of h x w (0 for bad sizes). */
+size_t tg_farneback_workspace_bytes(int groups, int t, int h, int w);
+/* gray uint8 [groups * t, h, w]: every group of t consecutive frames gives the t - 1 flows of its consecutive pairs,
+ * flow[g (t-1) + j] = farneback(gray[g t + j], gray[g t + j + 1]), fp32 [groups * (t-1), h, w, 2] (dx, dy).  Each
+ * frame's polynomial expansion is computed once per pyramid level however many pairs use it.  Per level: blur +
+ * resize (2 launches), polynomial expansion (2), the level's first flow and matrices (1), then one launch per
+ * iteration (box mean + solve + matrix update on 32 x 16 tiles with a winsize/2 halo).  flow and work 16-byte
+ * aligned; work_bytes >= tg_farneback_workspace_bytes.  The result does not depend on the grid.
+ * TG_E_INVALID: null pointers, bad sizes (t < 2), bad parameters, misalignment, a short workspace;
+ * TG_E_UNSUPPORTED: frames below 2 x 2, more than 65535 frames, a coarsest blur above 63 taps. */
+int tg_farneback(const uint8_t* gray, int groups, int t, int h, int w, const tg_farneback_params* params,
+                 float* flow, void* work, size_t work_bytes, void* stream);
+/* sums[q] = sum over the h*w pixels of |a[q] - b[q]| (the end-point error of two fp32 flows [n,h,w,2]), accumulated
+ * in float64; sums is zeroed by the call.  a, b and sums 8-byte aligned.  TG_E_INVALID: null pointers, non-positive
+ * sizes, misalignment; TG_E_UNSUPPORTED: n > 65535. */
+int tg_flow_epe_sum(const float* a, const float* b, int n, int h, int w, double* sums, void* stream);
+
 /* BD degradation of the data side (codes/utils/data_utils.py:30-53, called on GT frames by
  * base_model.py:75,115): optional reflect pad by (k-1)/2 | k-1-(k-1)/2, then a depthwise valid
  * correlation with the k x k kernel `k2d` (device, fp32, = create_kernel(sigma)[0,0]) and stride s.

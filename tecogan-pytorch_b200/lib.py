@@ -21,6 +21,7 @@ AMODE_AUTO, AMODE_HALO, AMODE_TAP = 0, 1, 2
 YUV_NV12, YUV_I420, YUV_P010, YUV_I420_10 = 0, 1, 2, 3
 RESAMPLE_BICUBIC, RESAMPLE_LANCZOS3 = 0, 1
 SCENE_CUT_WORK_BYTES = 16            # TG_SCENE_CUT_WORK_BYTES: workspace of tg_scene_cut per slot
+PSNR_NONE, PSNR_RGB, PSNR_Y = 0, 1, 2
 
 
 class ConvDesc(ctypes.Structure):
@@ -70,6 +71,12 @@ class YuvFormat(ctypes.Structure):
     _fields_ = [('layout', c_int32), ('matrix', c_int32), ('full_range', c_int32), ('reserved', c_int32)]
 
 
+class FarnebackParams(ctypes.Structure):
+    """struct tg_farneback_params"""
+    _fields_ = [('pyr_scale', c_double), ('levels', c_int32), ('winsize', c_int32), ('iterations', c_int32),
+                ('poly_n', c_int32), ('poly_sigma', c_double), ('flags', c_int32), ('reserved', c_int32)]
+
+
 CHAIN_MAX_LAYERS = 24
 
 _P = c_void_p
@@ -111,6 +118,10 @@ _SIGNATURES = {
     'tg_resample_nchw_f32': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, _P, c_int, c_int, c_int,
                                      _P, _P, _P]),
     'tg_scene_cut': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, c_double, _P, _P, _P, _P, _P]),
+    'tg_metrics_frames_in': (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P, _P, _P]),
+    'tg_farneback_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
+    'tg_farneback': (c_int, [_P, c_int, c_int, c_int, c_int, ctypes.POINTER(FarnebackParams), _P, _P, c_size_t, _P]),
+    'tg_flow_epe_sum': (c_int, [_P, _P, c_int, c_int, c_int, _P, _P]),
     'tg_downsample_bd_nchw_f32': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_debug_set_conv_timers': (c_int, [_P]),
     # ---- training (generator backward)

@@ -691,6 +691,76 @@ def scene_cut(lr_curr, lr_prev, reset, threshold, prev_mafd, work, score, cut):
     return score, cut
 
 
+def metrics_frames_in(true_u8, pred_u8, psnr, gray):
+    """tg_metrics_frames_in: true_u8 [t,ht,wt,3] / pred_u8 [t,hp,wp,3] uint8 (pred_u8 None: gray of true_u8 only),
+    psnr one of L.PSNR_NONE / PSNR_RGB / PSNR_Y, gray uint8 [2,t,h,w] ([t,h,w] without pred_u8) or None.
+    -> the per-frame integer SSE (int64 [t] holding the uint64 sums), or None without PSNR."""
+    name = 'metrics_frames_in'
+    _req(true_u8, torch.uint8, 'true_u8', 4)
+    t, ht, wt, c = true_u8.shape
+    hp = wp = 0
+    if pred_u8 is not None:
+        _req(pred_u8, torch.uint8, 'pred_u8', 4)
+        if pred_u8.shape[0] != t or pred_u8.shape[3] != 3:
+            raise L.TecoganB200Error(f'{name}: pred {tuple(pred_u8.shape)} does not match true {tuple(true_u8.shape)}')
+        hp, wp = pred_u8.shape[1:3]
+    if c != 3:
+        raise L.TecoganB200Error(f'{name}: expected RGB frames [t,h,w,3], got {tuple(true_u8.shape)}')
+    h, w = (min(ht, hp), min(wt, wp)) if pred_u8 is not None else (ht, wt)
+    if gray is not None:
+        _req(gray, torch.uint8, 'gray')
+        want = (2, t, h, w) if pred_u8 is not None else (t, h, w)
+        if tuple(gray.shape) != want:
+            raise L.TecoganB200Error(f'{name}: gray {tuple(gray.shape)}, expected {want}')
+    sse = torch.empty(t, dtype=torch.int64, device=true_u8.device) if psnr != L.PSNR_NONE else None
+    for x in (pred_u8, gray):
+        if x is not None and x.device != true_u8.device:
+            raise L.TecoganB200Error(f'{name}: tensors on different devices')
+    L.check(L.load().tg_metrics_frames_in(_ptr(true_u8), ht, wt, _ptr(pred_u8), hp, wp, t, psnr, _ptr(gray),
+                                          _ptr(sse), _stream()), 'tg_metrics_frames_in')
+    return sse
+
+
+def farneback_params(pyr_scale, levels, winsize, iterations, poly_n, poly_sigma, flags):
+    return L.FarnebackParams(float(pyr_scale), int(levels), int(winsize), int(iterations), int(poly_n),
+                             float(poly_sigma), int(flags), 0)
+
+
+def farneback_workspace_bytes(groups, t, h, w):
+    """bytes of tg_farneback's workspace for `groups` groups of t frames of h x w"""
+    return int(L.load().tg_farneback_workspace_bytes(groups, t, h, w))
+
+
+def farneback(gray, groups, params, work=None):
+    """tg_farneback: gray uint8 [groups*t, h, w] -> fp32 flows [groups*(t-1), h, w, 2] of the consecutive pairs of
+    each group of t frames.  work: a uint8 CUDA tensor of at least farneback_workspace_bytes (allocated if None)."""
+    _req(gray, torch.uint8, 'gray', 3)
+    n, h, w = gray.shape
+    if groups <= 0 or n % groups or n // groups < 2:
+        raise L.TecoganB200Error(f'farneback: {n} frames do not make {groups} groups of at least 2')
+    t = n // groups
+    need = farneback_workspace_bytes(groups, t, h, w)
+    if work is None:
+        work = torch.empty(need, dtype=torch.uint8, device=gray.device)
+    _req(work, torch.uint8, 'work', 1)
+    flow = torch.empty(groups * (t - 1), h, w, 2, dtype=torch.float32, device=gray.device)
+    L.check(L.load().tg_farneback(_ptr(gray), groups, t, h, w, ctypes.byref(params), _ptr(flow), _ptr(work),
+                                  work.numel(), _stream()), 'tg_farneback')
+    return flow
+
+
+def flow_epe_sum(a, b):
+    """tg_flow_epe_sum: fp32 flows a, b [n,h,w,2] -> float64 [n], the per-pair sum of |a - b| over the pixels"""
+    _req(a, torch.float32, 'a', 4)
+    _req(b, torch.float32, 'b', 4)
+    if a.shape != b.shape or a.shape[3] != 2:
+        raise L.TecoganB200Error(f'flow_epe_sum: shapes {tuple(a.shape)} / {tuple(b.shape)}')
+    n, h, w, _ = a.shape
+    sums = torch.empty(n, dtype=torch.float64, device=a.device)
+    L.check(L.load().tg_flow_epe_sum(_ptr(a), _ptr(b), n, h, w, _ptr(sums), _stream()), 'tg_flow_epe_sum')
+    return sums
+
+
 # ============================================================================ training (backward) ops
 class GradScale:
     """Device-resident loss scale {scale, 1/scale} of the fp16 gradient path (tg_grad_scale_from_amax /

@@ -1,0 +1,146 @@
+"""Throughput of tecogan_b200.metrics.sequence_metrics (PSNR-Y + tOF) on bd4 HR sequences (536x1280, T = 32): scored
+frames/s end to end (host uint8 frames in, float64 metrics out), per-phase kernel times from CUDA events, the bytes
+each phase must move (from shapes) and their share of the H100 SXM's 3.35 TB/s, and the reference formulas
+(cv2 Farneback + numpy PSNR, as MetricCalculator runs them) on the host cores for comparison.
+
+    python tools/metrics_bench.py [--seqs 4] [--ref-frames 4] [--out metrics_bench.json]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import tecogan_b200 as T      # noqa: E402
+import synthetic              # noqa: E402
+
+M, ops, L = T.metrics, T.ops, sys.modules['tecogan-pytorch_b200.lib']
+HBM = 3.35e12
+
+
+def card():
+    try:
+        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception as e:      # noqa: BLE001
+        q = f'nvidia-smi unavailable: {e}'
+    return {'torch_name': torch.cuda.get_device_name(0), 'nvidia_smi': q}
+
+
+def sequence(seed, T_=32, h=536, w=1280):
+    clip = synthetic.make_clip(seed, T_, 3, h, w, shift=2)
+    true = np.ascontiguousarray((clip.permute(0, 2, 3, 1) * 255).round().to(torch.uint8).numpy())
+    rng = np.random.default_rng(seed + 100)
+    pred = np.clip(true.astype(np.int16) + rng.integers(-6, 7, true.shape), 0, 255).astype(np.uint8)
+    return true, pred
+
+
+def level_sizes(h, w, pyr_scale=0.5, levels=3):
+    """pyramid level sizes of tOF's Farneback, coarsest first: the level count stops where a side drops below 32"""
+    k = 0
+    while k < levels and min(h, w) * pyr_scale ** (k + 1) >= 32:
+        k += 1
+    return [(int(np.rint(h * pyr_scale ** i)), int(np.rint(w * pyr_scale ** i))) for i in range(k, -1, -1)]
+
+
+def phase_bytes(T_, h, w):
+    """algorithmic bytes per phase for one T_-frame sequence (2T_ gray frames, 2(T_-1) flows), each buffer read or
+    written once per pass"""
+    n, p, hw = 2 * T_, 2 * (T_ - 1), h * w
+    b = {'frames_in': 2 * T_ * hw * 3 + n * hw + 8 * T_}
+    pyr = flow = 0
+    for lh, lw in level_sizes(h, w):
+        lhw = lh * lw
+        pyr += n * (hw + lh * w * 4) + n * (lh * w * 4 + lhw * 4)        # blur + resize: V and H passes
+        pyr += n * (lhw * 4 + 3 * lhw * 4) + n * (3 * lhw * 4 + 5 * lhw * 4)   # poly V and H
+        flow += p * (5 * lhw * 4 * 2 + 8 * lhw)                          # init: R0 + R1 reads, M + flow writes
+        flow += 3 * p * (5 * lhw * 4 + 8 * lhw) + 2 * p * (5 * lhw * 4 * 3)   # iterations: M in, flow, R0/R1, M out
+    b['pyramid+poly'] = pyr
+    b['flow'] = flow
+    b['epe'] = p * hw * 8
+    return b
+
+
+def timed_phases(true, pred):
+    """one chunk-free run of the phases with CUDA events around each"""
+    dev = torch.device('cuda:0')
+    T_, h, w = true.shape[:3]
+    tc, pc = torch.from_numpy(true).to(dev), torch.from_numpy(pred).to(dev)
+    gray = torch.empty(2, T_, h, w, dtype=torch.uint8, device=dev)
+    params = ops.farneback_params(0.5, 3, 15, 3, 5, 1.2, 0)
+    work = torch.empty(ops.farneback_workspace_bytes(2, T_, h, w), dtype=torch.uint8, device=dev)
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+    ev[0].record()
+    ops.metrics_frames_in(tc, pc, L.PSNR_Y, gray)
+    ev[1].record()
+    flow = ops.farneback(gray.view(2 * T_, h, w), 2, params, work)
+    ev[2].record()
+    ops.flow_epe_sum(flow[:T_ - 1], flow[T_ - 1:])
+    ev[3].record()
+    torch.cuda.synchronize()
+    return {'frames_in': ev[0].elapsed_time(ev[1]), 'farneback': ev[1].elapsed_time(ev[2]),
+            'epe': ev[2].elapsed_time(ev[3])}
+
+
+def reference_rate(true, pred, frames):
+    import cv2
+    from oracle import metrics_oracle as MO
+    t0 = time.perf_counter()
+    for i in range(1, frames + 1):
+        MO.psnr(true[i], pred[i], 'y')
+        g = [cv2.cvtColor(x, cv2.COLOR_RGB2GRAY) for x in (true[i - 1], true[i], pred[i - 1], pred[i])]
+        a = cv2.calcOpticalFlowFarneback(g[0], g[1], None, 0.5, 3, 15, 3, 5, 1.2, 0)
+        b = cv2.calcOpticalFlowFarneback(g[2], g[3], None, 0.5, 3, 15, 3, 5, 1.2, 0)
+        np.mean(np.sqrt(np.sum((a - b) ** 2, axis=-1)))
+    return frames / (time.perf_counter() - t0), cv2.getNumThreads()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--seqs', type=int, default=4)
+    ap.add_argument('--ref-frames', type=int, default=4)
+    ap.add_argument('--out', default=None)
+    a = ap.parse_args()
+    assert torch.cuda.is_available(), 'metrics_bench needs a GPU'
+    seqs = [sequence(s) for s in range(a.seqs)]
+    T_, h, w = seqs[0][0].shape[:3]
+    M.sequence_metrics(*seqs[0])               # warm-up: module load, allocations
+    torch.cuda.synchronize()
+    rates = []
+    for _ in range(2):
+        t0 = time.perf_counter()
+        for t, p in seqs:
+            M.sequence_metrics(t, p, psnr='y', tof=True)
+        torch.cuda.synchronize()
+        rates.append(len(seqs) * T_ / (time.perf_counter() - t0))
+    timed_phases(*seqs[0])
+    ph = [timed_phases(*seqs[i % len(seqs)]) for i in range(3)]
+    phases = {k: float(np.median([x[k] for x in ph])) for k in ph[0]}
+    pb = phase_bytes(T_, h, w)
+    moved = {'frames_in': pb['frames_in'], 'farneback': pb['pyramid+poly'] + pb['flow'], 'epe': pb['epe']}
+    ref_rate, ref_threads = reference_rate(*seqs[0], a.ref_frames) if a.ref_frames else (None, None)
+    res = {
+        'card': card(),
+        'shape': [T_, h, w],
+        'scored_frames_per_s_host_to_host': rates,
+        'phase_ms_per_sequence': phases,
+        'phase_bytes_per_sequence': moved,
+        'phase_share_of_3.35TBps': {k: moved[k] / (phases[k] * 1e-3) / HBM for k in phases},
+        'reference_host_frames_per_s': ref_rate,
+        'reference_cv2_threads': ref_threads,
+    }
+    print(json.dumps(res))
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, 'w') as f:
+            json.dump(res, f, indent=1)
+
+
+if __name__ == '__main__':
+    main()
