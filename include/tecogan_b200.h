@@ -273,15 +273,29 @@ int tg_stream_frame_in_yuv420(const uint8_t* in, int nv12, const int32_t* reset,
  * of each 2x2 block from its top-left pixel), NV12 with the U and V planes interleaved.  H and W must be even. */
 int tg_rgb_u8_to_yuv420(const uint8_t* rgb, uint8_t* out, int nv12, int n, int H, int W, void* stream);
 
-/* YUV 4:2:0 frame I/O in any supported layout and colour.
+/* YUV frame I/O (4:2:0, 4:2:2, 4:4:4) in any supported layout and colour.
  * layout : TG_YUV_NV12 / TG_YUV_I420 (uint8 words, as above), TG_YUV_P010 (NV12 planes, uint16 words, sample in the
  *          high 10 bits: v << 6; NVDEC / NVENC, ffmpeg p010le), TG_YUV_I420_10 (I420 planes, uint16 words, sample in
  *          the low 10 bits; ffmpeg yuv420p10le).  Frames are [n, 3h/2, w] words; 10-bit frames 2-byte aligned.
  * matrix : 601 (Kr, Kb = 0.299, 0.114) or 709 (0.2126, 0.0722); full_range 0 = limited ("tv"), 1 = full ("pc")
  *          quantisation of ITU-T H.273 at the layout's bit depth; reserved must be 0.
+ *          4:2:2 and 4:4:4 (h of any parity):
+ *          TG_YUV_YUY2 / TG_YUV_UYVY: packed 4:2:2, uint8 frames [n, h, 2w] (w even; V4L2 YUYV, SDI "2vuy"), each
+ *            pixel pair one 4-byte group Y0 U Y1 V (YUY2) or U Y0 V Y1 (UYVY); frames and output 4-byte aligned.
+ *          TG_YUV_I444: planar 4:4:4, uint8 frames [n, 3h, w] (the Y, U, V planes of h x w; ffmpeg yuv444p).
+ *          TG_YUV_I444_10: as I444 in uint16 words [n, 3h, w], sample in the low 10 bits (ffmpeg yuv444p10le).
+ *          Value 7 is not a layout (it stays an unknown one).  oracle/yuv_422_444.py specifies these four.
+ * matrix : 601 (Kr, Kb = 0.299, 0.114) or 709 (0.2126, 0.0722); full_range 0 = limited ("tv"), 1 = full ("pc")
+ *          quantisation of ITU-T H.273 at the layout's bit depth; reserved must be 0.
  * The fixed-point matrices are tg_yuv_coefficients' table (oracle/yuv_color.py derives the same numbers); matrix
- * 601, limited range, 8 bit is cv2's BT.601 and gives the bytes of the two entry points above. */
-enum { TG_YUV_NV12 = 0, TG_YUV_I420 = 1, TG_YUV_P010 = 2, TG_YUV_I420_10 = 3 };
+ * 601, limited range, 8 bit is cv2's BT.601 and gives the bytes of the two entry points above.  Decode uses nearest
+ * chroma (both pixels of a 4:2:2 pair take its U and V).  The 4:2:2 encode takes U and V of the pair's mean,
+ * rounded half up: C = (c . (rgb0 + rgb1) + 2^(s-1) + (128 << s)) >> s with the table row's coefficients and
+ * s = 21, except for 601 / limited, where it is cv2's COLOR_RGB2YUV_YUY2 / _UYVY bit for bit, luma included:
+ * Y = ((4211 R + 8258 G + 1606 B + 8192) >> 14) + 16, U = ((-1212 SR - 2384 SG + 3596 SB + 8192) >> 14) + 128,
+ * V = ((3596 SR - 3015 SG - 582 SB + 8192) >> 14) + 128 with SR = R0 + R1 and so on. */
+enum { TG_YUV_NV12 = 0, TG_YUV_I420 = 1, TG_YUV_P010 = 2, TG_YUV_I420_10 = 3, TG_YUV_YUY2 = 4, TG_YUV_UYVY = 5,
+       TG_YUV_I444 = 6, TG_YUV_I444_10 = 8 };
 typedef struct tg_yuv_format {
   int32_t layout;       /* TG_YUV_*                   */
   int32_t matrix;       /* 601 or 709                 */
@@ -289,14 +303,15 @@ typedef struct tg_yuv_format {
   int32_t reserved;     /* must be 0                  */
 } tg_yuv_format;
 /* tg_stream_frame_in_yuv420 for any format: lr_curr = float(rgb) / 255 (8 bit) or / 1023 (10 bit, P010 read as
- * v >> 6, I420_10 as min(v, 1023)), rgb decoded with nearest chroma; reset as in tg_stream_frame_in. */
+ * v >> 6, I420_10 and I444_10 as min(v, 1023)), rgb decoded with nearest chroma; reset as in tg_stream_frame_in. */
 int tg_stream_frame_in_yuv(const void* in, const tg_yuv_format* fmt, const int32_t* reset, float* lr_curr,
                            float* lr_prev, float* hr_prev, int n, int h, int w, int s, void* stream);
 /* Encode of the streamed output into any format.  8-bit layouts read rgb_u8 (uint8 NHWC [n,H,W,3], the step's
  * out_u8; rgb_f32 must be NULL), 10-bit layouts read rgb_f32 (fp32 NCHW [n,3,H,W], the step's HR frame, quantised as
- * clip(rint(x * 1023), 0, 1023); rgb_u8 must be NULL).  Chroma of each 2x2 block from its top-left pixel.
- * TG_E_INVALID: null pointers, the wrong source for the bit depth, a non-zero reserved; TG_E_UNSUPPORTED: odd sizes,
- * unknown layout or matrix. */
+ * clip(rint(x * 1023), 0, 1023); rgb_u8 must be NULL).  4:2:0: chroma of each 2x2 block from its top-left pixel;
+ * 4:2:2: of each pixel pair's mean (above); 4:4:4: per pixel.  Output [n, 3H/2, W], [n, H, 2W] or [n, 3H, W] words.
+ * TG_E_INVALID: null pointers, the wrong source for the bit depth, a non-zero reserved, misaligned buffers;
+ * TG_E_UNSUPPORTED: odd sizes (H and W for 4:2:0, W for 4:2:2), unknown layout or matrix. */
 int tg_rgb_to_yuv(const uint8_t* rgb_u8, const float* rgb_f32, void* out, const tg_yuv_format* fmt, int n, int H,
                   int W, void* stream);
 /* Host only: the 16 int32 of the kernels' table row for fmt (its bit depth and colour): encode cRY cGY cBY cRU cGU

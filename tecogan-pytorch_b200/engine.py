@@ -224,10 +224,12 @@ class StreamEngine(ClipEngine):
     the device mask mask[p] -- the reset of one slot happens inside the captured step, and one graph serves every
     pattern of resets.  The step itself is the unchanged net.step_into.
 
-    YUV 4:2:0 input (yuv_in = 'nv12' / 'i420' / 'p010' / 'i420_10'): inp[p] holds [n,3h/2,w] frames (uint16 for
-    the 10-bit layouts) and the first launch is tg_stream_frame_in_yuv420 (8 bit, BT.601 limited range: cv2's
+    YUV input (yuv_in = 'nv12' / 'i420' / 'p010' / 'i420_10', or the 4:2:2 / 4:4:4 'yuy2' / 'uyvy' / 'i444' /
+    'i444_10'): inp[p] holds [n,3h/2,w] frames ([n,h,2w] for 4:2:2, [n,3h,w] for 4:4:4; uint16 for the 10-bit
+    layouts) and the first launch is tg_stream_frame_in_yuv420 (8 bit, BT.601 limited range: cv2's
     conversion) or tg_stream_frame_in_yuv (any other layout or colour) instead, with the same reset.  YUV output
-    (yuv_out): each graph ends with the encode into yuv[p] [n,3H/2,W] -- tg_rgb_u8_to_yuv420 of u8[p] (8 bit,
+    (yuv_out): each graph ends with the encode into yuv[p] [n,3H/2,W] (or that layout's shape) --
+    tg_rgb_u8_to_yuv420 of u8[p] (8 bit,
     BT.601 limited range), tg_rgb_to_yuv of u8[p] (8 bit, other colours) or tg_rgb_to_yuv of the fp32 HR frame
     hr[p] (10 bit, uint16 yuv[p]) -- and the copies out read yuv[p] instead of u8[p].
 
@@ -254,7 +256,7 @@ class StreamEngine(ClipEngine):
         self.yuv_in, self.yuv_out = yuv_in, yuv_out          # None or one of ops.YUV_LAYOUTS
         self.in_color, self.out_color = in_color, out_color
         self.mask = [torch.zeros(n, dtype=torch.int32, device=dev) for _ in range(2)]
-        frame = (3 * h // 2, w) if yuv_in else (h, w, c)
+        frame = ops.yuv_frame_shape(yuv_in, h, w) if yuv_in else (h, w, c)
         # 10-bit words: zeroed as int16, the same bits
         in_dtype = torch.int16 if yuv_in and ops.yuv_depth(yuv_in) == 10 else torch.uint8
         self.inp = ([torch.zeros(n, *frame, dtype=in_dtype, device=dev).view(_word_dtype(yuv_in)) for _ in range(2)]
@@ -269,7 +271,8 @@ class StreamEngine(ClipEngine):
             f32 = yuv_out is not None and ops.yuv_depth(yuv_out) == 10
             self.rs = [torch.empty((n, c, Ho, Wo) if f32 else (n, Ho, Wo, c),
                                    dtype=torch.float32 if f32 else torch.uint8, device=dev) for _ in range(2)]
-        self.yuv = ([torch.empty(n, 3 * Ho // 2, Wo, dtype=_word_dtype(yuv_out), device=dev) for _ in range(2)]
+        self.yuv = ([torch.empty(n, *ops.yuv_frame_shape(yuv_out, Ho, Wo), dtype=_word_dtype(yuv_out), device=dev)
+                     for _ in range(2)]
                     if yuv_out else None)
         self.scene_cut = scene_cut
         self.prev_mafd = self.work = self.rep = self.score = self.cut = None
@@ -340,7 +343,8 @@ class StreamEngine(ClipEngine):
             self.mask_set[p] = False
 
     def run(self, frames, reset_slots, out_host):
-        """frames: uint8 [n,k,h,w,c] (u8_input), uint8 / uint16 [n,k,3h/2,w] (yuv_in) or fp32 [n,k,c,h,w], each
+        """frames: uint8 [n,k,h,w,c] (u8_input), uint8 / uint16 [n,k,*yuv_frame_shape] (yuv_in) or fp32
+        [n,k,c,h,w], each
         frame contiguous, pinned host or on this device.
         Slots in `reset_slots` start a new video at frame 0.  Returns uint8 [n,k,H,W,c] (or [n,k,3H/2,W] words with
         yuv_out; Ho, Wo instead of H, W with out_size): a pinned host tensor (out_host; one synchronisation, at the end) or a new tensor on the device,
@@ -415,7 +419,8 @@ class StreamEngine(ClipEngine):
 
 
 YUV420 = ops.YUV420_LAYOUTS       # 'nv12', 'i420'
-YUV = ops.YUV_LAYOUTS             # those and the 10-bit 'p010', 'i420_10'
+YUV = ops.YUV_LAYOUTS             # those, the 10-bit 'p010', 'i420_10', 4:2:2 'yuy2', 'uyvy', 4:4:4 'i444', 'i444_10'
+_YUV_422_444 = ops.YUV422_LAYOUTS + ops.YUV444_LAYOUTS
 COLORS = ops.YUV_COLORS           # 'bt601' (the default, cv2's conversion), 'bt709', 'bt601-full', 'bt709-full'
 
 
@@ -453,8 +458,11 @@ class VideoStream:
         if out_size is not None:
             out_size = _check_out_size(out_size, net.scale * h, net.scale * w, out_format)
         yuv = [f for f in (input, out_format) if f in YUV]
-        if yuv and (h % 2 or w % 2):
-            raise ValueError(f'{yuv[0]} frames are YUV 4:2:0: h and w must be even, got {h}x{w}')
+        for f in yuv:
+            if f not in _YUV_422_444 and (h % 2 or w % 2):
+                raise ValueError(f'{f} frames are YUV 4:2:0: h and w must be even, got {h}x{w}')
+            if f in ops.YUV422_LAYOUTS and w % 2:
+                raise ValueError(f'{f} frames are YUV 4:2:2: w must be even, got {h}x{w}')
         if yuv and net.fnet.in_nc != 3:
             raise ValueError(f'{yuv[0]} frames carry 3 colour channels, the net takes {net.fnet.in_nc}')
         device = torch.device('cuda') if device is None else torch.device(device)
@@ -503,6 +511,8 @@ class VideoStream:
                 opened with out_size=(Ho, Wo) returns Ho x Wo frames in place of H x W.
         10-bit input ('p010', 'i420_10') takes uint16 frames [n,k,3h/2,w] ([k,3h/2,w] when n == 1), torch.uint16 or
         NumPy uint16; uint8 frames into a 10-bit stream raise, and so do uint16 frames into an 8-bit one.
+        4:2:2 and 4:4:4, in and out: 'yuy2' / 'uyvy' frames are uint8 [n,k,h,2w], 'i444' uint8 [n,k,3h,w] and
+        'i444_10' uint16 [n,k,3h,w] (H, W or Ho, Wo on the output side).
         A stream opened with scene_cut=threshold restarts a slot at every detected cut, as reset= would have, and
         sets last_cuts (bool [n,k]) and last_scores (float64 [n,k]) for this push: NumPy with out='host', CUDA
         tensors ordered on the current stream with out='device'.  A reset requested by the caller scores 0 and is
@@ -563,7 +573,11 @@ class VideoStream:
                                      f'{frames.dtype}')
         frame, layout = {'uint8': ((self.h, self.w, self.c), 'n,k,h,w,c'),
                          'float32': ((self.c, self.h, self.w), 'n,k,c,h,w')}.get(
-                             self.input, ((3 * self.h // 2, self.w), 'n,k,3h/2,w'))
+                             self.input, (None, None))
+        if frame is None:
+            frame = ops.yuv_frame_shape(self.input, self.h, self.w)
+            layout = ('n,k,h,2w' if self.input in ops.YUV422_LAYOUTS else
+                      'n,k,3h,w' if self.input in ops.YUV444_LAYOUTS else 'n,k,3h/2,w')
         if frames.dim() == len(frame) + 1 and self.n == 1:
             frames = frames.unsqueeze(0)
         if (frames.dim() != len(frame) + 2 or frames.shape[0] != self.n or frames.shape[1] < 1
@@ -612,7 +626,7 @@ def _check_scene_cut(threshold):
 
 def _check_out_size(out_size, H, W, out_format):
     """out_size -> (Ho, Wo) ints, or ValueError: two positive ints within the resize's ratios of the H x W output,
-    even for a YUV out_format."""
+    both even for a YUV 4:2:0 out_format, Wo even for 4:2:2."""
     if (not isinstance(out_size, (tuple, list)) or len(out_size) != 2
             or not all(isinstance(v, numbers.Integral) and not isinstance(v, bool) and v > 0 for v in out_size)):
         raise ValueError(f'out_size must be (Ho, Wo), two positive ints, got {out_size!r}')
@@ -620,8 +634,10 @@ def _check_out_size(out_size, H, W, out_format):
     if not (ops.resample_ratio_ok(H, Ho) and ops.resample_ratio_ok(W, Wo)):
         raise ValueError(f'out_size {Ho}x{Wo} from a {H}x{W} output: each axis must be within 1/4 to 2 times the '
                          f'output size')
-    if out_format in YUV and (Ho % 2 or Wo % 2):
+    if out_format in YUV and out_format not in _YUV_422_444 and (Ho % 2 or Wo % 2):
         raise ValueError(f'{out_format} frames are YUV 4:2:0: out_size must be even, got {Ho}x{Wo}')
+    if out_format in ops.YUV422_LAYOUTS and Wo % 2:
+        raise ValueError(f'{out_format} frames are YUV 4:2:2: the width of out_size must be even, got {Ho}x{Wo}')
     return Ho, Wo
 
 

@@ -19,6 +19,7 @@ UP_BICUBIC, UP_BILINEAR = 0, 1
 EPI_NHWC_F16, EPI_FLOW_NCHW_F32, EPI_OUT_NCHW_F32, EPI_NHWC_F16_POOL2 = 0, 1, 2, 3
 AMODE_AUTO, AMODE_HALO, AMODE_TAP = 0, 1, 2
 YUV_NV12, YUV_I420, YUV_P010, YUV_I420_10 = 0, 1, 2, 3
+YUV_YUY2, YUV_UYVY, YUV_I444, YUV_I444_10 = 4, 5, 6, 8      # 7 is not a layout
 RESAMPLE_BICUBIC, RESAMPLE_LANCZOS3 = 0, 1
 SCENE_CUT_WORK_BYTES = 16            # TG_SCENE_CUT_WORK_BYTES: workspace of tg_scene_cut per slot
 PSNR_NONE, PSNR_RGB, PSNR_Y = 0, 1, 2

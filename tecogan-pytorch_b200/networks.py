@@ -377,6 +377,11 @@ class FRNet(BaseSequenceGenerator):
         and 'i420_10' (I420 planes, uint16 words, sample in the low 10 bits; ffmpeg / PyAV yuv420p10le), as input
         (uint16 [n,k,3h/2,w], converted to RGB / 1023) or out_format (uint16 [n,k,3H/2,W], encoded from the fp32 HR
         frame, so the two bits below the uint8 output are kept).
+        4:2:2 and 4:4:4 video, as input or out_format: 'yuy2' / 'uyvy' (packed, uint8 [n,k,h,2w] per pixel pair
+        Y0 U Y1 V / U Y0 V Y1, w even; V4L2 webcams, SDI capture) decode and encode exactly as cv2.cvtColor's
+        COLOR_YUV2RGB_YUY2 / _UYVY and COLOR_RGB2YUV_YUY2 / _UYVY (chroma of each pair's mean); 'i444' (uint8) and
+        'i444_10' (uint16, sample in the low 10 bits) are planar [n,k,3h,w] frames with a chroma sample per pixel.
+        Neither needs an even h.
         in_color / out_color pick the YUV side's colour: 'bt601' (the default, limited range; for 8-bit frames
         exactly cv2's conversion), 'bt709', 'bt601-full', 'bt709-full' (ITU-T H.273 quantisation, integer fixed
         point as oracle/yuv_color.py specifies).  Take in_color from the decoder (ffprobe's color_space /
@@ -384,10 +389,11 @@ class FRNet(BaseSequenceGenerator):
         side raises ValueError.
         out_size=(Ho, Wo) resizes every output frame from H x W to Ho x Wo on the device, from the fp32 HR frame
         and before the uint8 quantisation or the YUV encode: push() then returns uint8 [n,k,Ho,Wo,c] or YUV words
-        [n,k,3Ho/2,Wo].  resize_filter is 'bicubic' (the default) or 'lanczos': Pillow's antialiased filters
+        ([n,k,3Ho/2,Wo] for 4:2:0, [n,k,Ho,2Wo] for 4:2:2, [n,k,3Ho,Wo] for 4:4:4).
+        resize_filter is 'bicubic' (the default) or 'lanczos': Pillow's antialiased filters
         (Image.resize on 'F' images, as oracle/resample.py specifies), widened by the ratio on a downscale.  Each
-        axis needs H/4 <= Ho <= 2H (likewise W), and even Ho and Wo for YUV output.  out_size=(H, W) gives the
-        bytes of the stream without it.
+        axis needs H/4 <= Ho <= 2H (likewise W), even Ho and Wo for 4:2:0 output, even Wo for 4:2:2.
+        out_size=(H, W) gives the bytes of the stream without it.
         scene_cut=threshold (a number in (0, 100]; 10.0 is a good start, the default of ffmpeg's scdet) detects
         hard cuts on the device, inside the step: each frame is scored against the previous one of its slot (the
         mean absolute difference of the 8-bit codes and its change, as oracle/scene_cut.py specifies), and a score

@@ -497,14 +497,35 @@ def rgb_u8_to_yuv420(rgb, layout, out=None):
     return out
 
 
-YUV_LAYOUTS = ('nv12', 'i420', 'p010', 'i420_10')      # 8-bit uint8 words; 10-bit uint16 words
+YUV422_LAYOUTS = ('yuy2', 'uyvy')                     # packed 4:2:2, uint8
+YUV444_LAYOUTS = ('i444', 'i444_10')                  # planar 4:4:4, uint8 / uint16
+# 4:2:0, then 4:2:2 and 4:4:4; 8-bit uint8 words; 10-bit uint16 words
+YUV_LAYOUTS = ('nv12', 'i420', 'p010', 'i420_10') + YUV422_LAYOUTS + YUV444_LAYOUTS
 YUV_COLORS = ('bt601', 'bt709', 'bt601-full', 'bt709-full')
-_LAYOUT_CODE = {'nv12': L.YUV_NV12, 'i420': L.YUV_I420, 'p010': L.YUV_P010, 'i420_10': L.YUV_I420_10}
+_LAYOUT_CODE = {'nv12': L.YUV_NV12, 'i420': L.YUV_I420, 'p010': L.YUV_P010, 'i420_10': L.YUV_I420_10,
+                'yuy2': L.YUV_YUY2, 'uyvy': L.YUV_UYVY, 'i444': L.YUV_I444, 'i444_10': L.YUV_I444_10}
 
 
 def yuv_depth(layout):
     """Bit depth of a YUV layout: 8 (uint8 frames) or 10 (uint16 frames)."""
-    return 10 if layout in ('p010', 'i420_10') else 8
+    return 10 if layout in ('p010', 'i420_10', 'i444_10') else 8
+
+
+def yuv_frame_shape(layout, h, w):
+    """The words of one h x w frame: (3h/2, w) for 4:2:0, (h, 2w) for packed 4:2:2, (3h, w) for planar 4:4:4."""
+    if layout in YUV422_LAYOUTS:
+        return (h, 2 * w)
+    return (3 * h, w) if layout in YUV444_LAYOUTS else (3 * h // 2, w)
+
+
+def yuv_size_error(layout, h, w):
+    """None if an h x w frame fits the layout's chroma subsampling, else why not: 4:2:0 needs an even height and
+    width, 4:2:2 an even width, 4:4:4 any size."""
+    if layout in YUV422_LAYOUTS:
+        return None if w % 2 == 0 else f'YUV 4:2:2 needs an even width, got {w}'
+    if layout in YUV444_LAYOUTS:
+        return None
+    return None if h % 2 == 0 and w % 2 == 0 else f'YUV 4:2:0 needs an even height and width, got {h}x{w}'
 
 
 def yuv_format(layout, color, name='yuv_format'):
@@ -526,9 +547,10 @@ def yuv_coefficients(layout, color):
 
 
 def stream_frame_in_yuv(frames, layout, color, reset, lr_curr, lr_prev, hr_prev, scale):
-    """tg_stream_frame_in_yuv: frames [n,3h/2,w] (uint8 for 'nv12' / 'i420', uint16 for 'p010' / 'i420_10'; or
-    None) in colour `color` -> lr_curr fp32 [n,3,h,w] = RGB / 255 (8 bit) or RGB / 1023 (10 bit), as
-    oracle/yuv_color.py; reset as in stream_frame_in."""
+    """tg_stream_frame_in_yuv: frames [n,*yuv_frame_shape(layout, h, w)] (uint8 for the 8-bit layouts, uint16 for
+    'p010' / 'i420_10' / 'i444_10'; or None) in colour `color` -> lr_curr fp32 [n,3,h,w] = RGB / 255 (8 bit) or
+    RGB / 1023 (10 bit), as oracle/yuv_color.py (4:2:0) and oracle/yuv_422_444.py (4:2:2, 4:4:4) specify; reset as
+    in stream_frame_in."""
     name = 'stream_frame_in_yuv'
     fmt = yuv_format(layout, color, name)
     _req(lr_curr, torch.float32, 'lr_curr', 4)
@@ -537,14 +559,16 @@ def stream_frame_in_yuv(frames, layout, color, reset, lr_curr, lr_prev, hr_prev,
     n, c, h, w = lr_curr.shape
     if c != 3:
         raise L.TecoganB200Error(f'{name}: lr_curr has {c} channels, YUV frames decode to 3')
-    if h % 2 or w % 2:
-        raise L.TecoganB200Error(f'{name}: YUV 4:2:0 needs an even height and width, got {h}x{w}')
+    err = yuv_size_error(layout, h, w)
+    if err:
+        raise L.TecoganB200Error(f'{name}: {err}')
     if tuple(lr_prev.shape) != (n, c, h, w) or tuple(hr_prev.shape) != (n, c, scale * h, scale * w):
         raise L.TecoganB200Error(f'{name}: lr_prev / hr_prev shape mismatch')
     if frames is not None:
         _req(frames, torch.uint16 if yuv_depth(layout) == 10 else torch.uint8, 'frames', 3)
-        if tuple(frames.shape) != (n, 3 * h // 2, w):
-            raise L.TecoganB200Error(f'{name}: frames {tuple(frames.shape)} != {(n, 3 * h // 2, w)} ([n,3h/2,w])')
+        want = (n, *yuv_frame_shape(layout, h, w))
+        if tuple(frames.shape) != want:
+            raise L.TecoganB200Error(f'{name}: frames {tuple(frames.shape)} != {want} ({layout} frames of {h}x{w})')
     if reset is not None:
         _req(reset, torch.int32, 'reset', 1)
         if reset.shape[0] != n:
@@ -559,8 +583,9 @@ def stream_frame_in_yuv(frames, layout, color, reset, lr_curr, lr_prev, hr_prev,
 
 
 def rgb_to_yuv(layout, color, rgb_u8=None, rgb_f32=None, out=None):
-    """tg_rgb_to_yuv: 8-bit layouts encode rgb_u8 (uint8 NHWC [n,H,W,3]) into uint8 [n,3H/2,W]; 10-bit layouts
-    encode rgb_f32 (fp32 NCHW [n,3,H,W], quantised as clip(rint(x * 1023), 0, 1023)) into uint16 [n,3H/2,W]."""
+    """tg_rgb_to_yuv: 8-bit layouts encode rgb_u8 (uint8 NHWC [n,H,W,3]) into uint8 [n,*yuv_frame_shape]; 10-bit
+    layouts encode rgb_f32 (fp32 NCHW [n,3,H,W], quantised as clip(rint(x * 1023), 0, 1023)) into uint16
+    [n,*yuv_frame_shape] ([n,3H/2,W] for 4:2:0, [n,H,2W] for 4:2:2, [n,3H,W] for 4:4:4)."""
     name = 'rgb_to_yuv'
     fmt = yuv_format(layout, color, name)
     ten = yuv_depth(layout) == 10
@@ -576,14 +601,16 @@ def rgb_to_yuv(layout, color, rgb_u8=None, rgb_f32=None, out=None):
         n, H, W, c = src.shape
     if c != 3:
         raise L.TecoganB200Error(f'{name}: expected 3 colour channels, got {tuple(src.shape)}')
-    if H % 2 or W % 2:
-        raise L.TecoganB200Error(f'{name}: YUV 4:2:0 needs an even height and width, got {H}x{W}')
+    err = yuv_size_error(layout, H, W)
+    if err:
+        raise L.TecoganB200Error(f'{name}: {err}')
     dtype = torch.uint16 if ten else torch.uint8
+    shape = (n, *yuv_frame_shape(layout, H, W))
     if out is None:
-        out = torch.empty((n, 3 * H // 2, W), dtype=dtype, device=src.device)
+        out = torch.empty(shape, dtype=dtype, device=src.device)
     _req(out, dtype, 'out', 3)
-    if tuple(out.shape) != (n, 3 * H // 2, W):
-        raise L.TecoganB200Error(f'{name}: out {tuple(out.shape)} != {(n, 3 * H // 2, W)}')
+    if tuple(out.shape) != shape:
+        raise L.TecoganB200Error(f'{name}: out {tuple(out.shape)} != {shape}')
     if out.device != src.device:
         raise L.TecoganB200Error(f'{name}: tensors on different devices')
     L.check(L.load().tg_rgb_to_yuv(_ptr(rgb_u8), _ptr(rgb_f32), _ptr(out), ctypes.byref(fmt), n, H, W, _stream()),

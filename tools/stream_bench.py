@@ -14,10 +14,14 @@ each run ends in a device synchronisation; one untimed warm-up run of every path
   push_nv12_device           the same with NV12 on the device and out='device', k = 16
   push_p010_709_host_chunk16 a P010 / BT.709 -> P010 / BT.709 stream (uint16 [n,k,3h/2,w] -> [n,k,3H/2,W]), k = 16
   push_nv12_601_709_host_chunk16  an NV12 / BT.601 -> NV12 / BT.709 stream, k = 16
+  push_<yuy2|uyvy|i444>_host_chunk16  a YUY2 -> YUY2, UYVY -> UYVY or I444 -> I444 stream (BT.601 limited range;
+                             uint8 [n,k,h,2w] / [n,k,3h,w] in and [n,k,H,2W] / [n,k,3H,W] out), k = 16
   frame_in_us                tg_stream_frame_in per step (decode of 4 frames, zero reset mask; and with every
                              slot reset) and tg_stream_frame_in_yuv420 per step (NV12, I420), CUDA events over a
                              graph of launches on rotating buffers
-                             and tg_stream_frame_in_yuv per step (P010 / BT.709)
+                             and tg_stream_frame_in_yuv per step (P010 / BT.709; YUY2, UYVY, I444 / BT.601;
+                             I444_10 / BT.709), the last four with their algorithmic bytes (frames read, lr_curr
+                             written) and TB/s in frame_in_422_444_tb_per_s
   push_u8_resize_<Ho>x<Wo>[_lanczos]_host_chunk16
                              an RGB stream with out_size=(Ho, Wo) (bicubic unless marked), k = 16: 402x960 (3/4) and
                              804x1920 (3/2)
@@ -30,7 +34,9 @@ each run ends in a device synchronisation; one untimed warm-up run of every path
   resample_us                tg_resample_nchw_f32 per step (4 HR frames -> uint8 NHWC or fp32 NCHW), timed as below,
                              with its algorithmic bytes (n*3*H*W*4 read, n*Ho*Wo*3 or *12 written) and TB/s
   encode_us                  tg_rgb_u8_to_yuv420 per step (4 HR frames -> NV12 / I420) and tg_rgb_to_yuv per step
-                             (uint8 -> NV12 / BT.709; fp32 NCHW -> P010 / BT.709), timed the same way
+                             (uint8 -> NV12 / BT.709; fp32 NCHW -> P010 / BT.709; uint8 -> YUY2, UYVY, I444;
+                             fp32 NCHW -> I444_10 / BT.709), timed the same way; the 4:2:2 / 4:4:4 ones with their
+                             algorithmic bytes and TB/s in encode_422_444_tb_per_s
   scene_us                   tg_scene_cut per step (4 slots of 3x134x320 scored against another 4, with its
                              algorithmic bytes 2*n*c*h*w*4 and TB/s; 16 disjoint pairs of frame sets, 66 MB, rotate so
                              that L2 does not hold the next launch's input) and the reset-only tg_stream_frame_in that
@@ -42,8 +48,8 @@ output with oracle/yuv_color.py's BT.709 encode of that RGB output, and the P010
 frames of a device loop of FRNet.step over the frames P010 decodes to.  The resized RGB outputs are compared with
 oracle/resample.py's float64 resize of the fp32 HR frames of a device loop of FRNet.step (equal, or 1 apart where
 x * 255 is within 1e-3 of a rounding boundary), the resized NV12 output with the BT.709 encode of the resized RGB
-output.  Card name and
-power limit are read in the same run.  Writes nothing."""
+output.  The YUY2, UYVY and I444 outputs are compared with oracle/yuv_422_444.py's encode of the RGB output for the
+frames each input decodes to.  Card name and power limit are read in the same run.  Writes nothing."""
 import argparse
 import json
 import os
@@ -78,6 +84,7 @@ def main():
     import tecogan_b200 as T
     from oracle import yuv_oracle as Y
     from oracle import yuv_color as C
+    from oracle import yuv_422_444 as C4
     from oracle import resample as R
     ops = sys.modules['tecogan-pytorch_b200.ops']
     assert torch.cuda.is_available(), 'stream_bench.py needs a GPU'
@@ -100,6 +107,8 @@ def main():
     nv12_dev = nv12_pin.to(dev)
     p010 = C.rgb_to_yuv(np.rint(u8.astype(np.float64) * (1023.0 / 255.0)).astype(np.int64), 'p010', 'bt709')
     p010_pin = torch.from_numpy(p010).pin_memory()
+    packed = {lay: C4.rgb_to_yuv(u8, lay) for lay in ('yuy2', 'uyvy', 'i444')}         # [n,t,h,2w] / [n,t,3h,w]
+    packed_pin = {lay: torch.from_numpy(v).pin_memory() for lay, v in packed.items()}
 
     def timed(fn):
         torch.cuda.synchronize()
@@ -131,6 +140,9 @@ def main():
     for k, kw in resized.items():
         streams[k] = (16, u8_pin, 'host')
         kinds[k] = kw
+    for lay in packed:
+        streams[f'push_{lay}_host_chunk16'] = (16, packed_pin[lay], 'host')
+        kinds[f'push_{lay}_host_chunk16'] = dict(input=lay, out_format=lay)
     for chunk in (1, 16):
         streams[f'push_u8_scene_host_chunk{chunk}'] = (chunk, u8_pin, 'host')
         kinds[f'push_u8_scene_host_chunk{chunk}'] = dict(scene_cut=10.0)
@@ -222,6 +234,13 @@ def main():
             identical[k] = got.shape == (n, t, 3 * s * h // 2, s * w) and all(
                 np.array_equal(got[j, i], C.rgb_to_yuv(ref_rgb[j, i], 'nv12', 'bt709')) for j in range(n)
                 for i in range(t))
+        elif k.startswith(tuple(f'push_{lay}_' for lay in packed)):
+            lay = k.split('_')[1]
+            rgb_lay = C4.yuv_to_rgb(packed[lay], lay)
+            ref_lay = net.infer_sequence(torch.from_numpy(rgb_lay.astype(np.float32) / np.float32(255.0))
+                                         .permute(0, 1, 4, 2, 3).contiguous(), dev)
+            identical[k] = got.shape == (n, t, *C4.frame_shape(lay, s * h, s * w)) and all(
+                np.array_equal(got[j, i], C4.rgb_to_yuv(ref_lay[j, i], lay)) for j in range(n) for i in range(t))
         elif 'nv12' in k:        # frame by frame: the oracle's int64 temporaries of a whole clip are GBs
             identical[k] = got.shape == (n, t, 3 * s * h // 2, s * w) and all(
                 np.array_equal(got[j, i], Y.rgb_to_yuv420(ref_rgb[j, i], 'nv12')) for j in range(n) for i in range(t))
@@ -257,6 +276,16 @@ def main():
     sec = bench._time_graph(lambda i: ops.stream_frame_in_yuv(p010_ins[i], 'p010', 'bt709', None, lrs[i], prev, hrp, s),
                             nb, reps, torch)
     frame_in['decode_p010_bt709'] = sec * 1e6
+    frame_in_bytes = {}
+    for lay, color in (('yuy2', 'bt601'), ('uyvy', 'bt601'), ('i444', 'bt601'), ('i444_10', 'bt709')):
+        shape = (n, *C4.frame_shape(lay, h, w))
+        src = [torch.randint(0, 1 << 15, shape, dtype=torch.int16, device=dev).view(torch.uint16) if lay == 'i444_10'
+               else torch.randint(0, 256, shape, dtype=torch.uint8, device=dev) for _ in range(nb)]
+        sec = bench._time_graph(lambda i: ops.stream_frame_in_yuv(src[i], lay, color, None, lrs[i], prev, hrp, s),
+                                nb, reps, torch)
+        frame_in[f'decode_{lay}_{color}'] = sec * 1e6
+        frame_in_bytes[f'decode_{lay}_{color}'] = src[0].numel() * src[0].element_size() + n * c * h * w * 4
+        del src
     # tg_rgb_u8_to_yuv420 alone: 8 rotating sets of 4 HR frames (8 x 8.2 MB in, 8 x 4.1 MB out)
     rgbs = [torch.randint(0, 256, (n, H, W, c), dtype=torch.uint8, device=dev) for _ in range(nb)]
     yuvs = [torch.empty(n, 3 * H // 2, W, dtype=torch.uint8, device=dev) for _ in range(nb)]
@@ -270,6 +299,19 @@ def main():
     p010s = [torch.empty(n, 3 * H // 2, W, dtype=torch.uint16, device=dev) for _ in range(nb)]
     sec = bench._time_graph(lambda i: ops.rgb_to_yuv('p010', 'bt709', rgb_f32=hrs[i], out=p010s[i]), nb, reps, torch)
     encode['p010_bt709'] = sec * 1e6
+    encode_new_bytes = {}
+    for lay in ('yuy2', 'uyvy', 'i444'):
+        outs = [torch.empty(n, *C4.frame_shape(lay, H, W), dtype=torch.uint8, device=dev) for _ in range(nb)]
+        sec = bench._time_graph(lambda i: ops.rgb_to_yuv(lay, 'bt601', rgb_u8=rgbs[i], out=outs[i]), nb, reps, torch)
+        encode[lay] = sec * 1e6
+        encode_new_bytes[lay] = n * H * W * 3 + outs[0].numel()
+        del outs
+    outs = [torch.empty(n, 3 * H, W, dtype=torch.uint16, device=dev) for _ in range(nb)]
+    sec = bench._time_graph(lambda i: ops.rgb_to_yuv('i444_10', 'bt709', rgb_f32=hrs[i], out=outs[i]), nb, reps,
+                            torch)
+    encode['i444_10_bt709'] = sec * 1e6
+    encode_new_bytes['i444_10_bt709'] = n * c * H * W * 4 + n * 3 * H * W * 2
+    del outs
     encode_bytes = n * H * W * 3 + n * 3 * H // 2 * W
     # tg_resample_nchw_f32 alone: the same 8 rotating sets of 4 fp32 HR frames (8 x 33 MB)
     resample, resample_bytes = {}, {}
@@ -325,7 +367,11 @@ def main():
         'encode_bytes_per_step': encode_bytes,
         'encode10_bytes_per_step': encode10_bytes,
         'encode_gb_per_s': {k: (encode10_bytes if k.startswith('p010') else encode_bytes) / v * 1e-3
-                            for k, v in encode.items()},
+                            for k, v in encode.items() if k not in encode_new_bytes},
+        'frame_in_422_444_bytes_per_step': frame_in_bytes,
+        'frame_in_422_444_tb_per_s': {k: b / frame_in[k] * 1e-6 for k, b in frame_in_bytes.items()},
+        'encode_422_444_bytes_per_step': encode_new_bytes,
+        'encode_422_444_tb_per_s': {k: b / encode[k] * 1e-6 for k, b in encode_new_bytes.items()},
         'h2d_bytes_per_step': {'fp32': n * c * h * w * 4, 'uint8': n * c * h * w, 'nv12': n * 3 * h // 2 * w},
         'd2h_bytes_per_step': {'uint8': n * c * H * W, 'nv12': n * 3 * H // 2 * W},
         'launches_per_step': {'infer_sequence': T.engine.get_engine(net, n, c, h, w, dev).launches_per_step,
