@@ -48,6 +48,7 @@ namespace {
 constexpr int TH = 16, TW = 8;
 constexpr int kThreads = 384;             // producer warpgroup + 2 consumer warpgroups
 constexpr int kMaxRing = 4;               // smem stages per consumer ring
+constexpr int kBiasBar = 3;               // named barrier of both consumer warpgroups (1 + cw: one consumer's)
 constexpr uint32_t kHeaderBytes = 2048;   // barriers (first 1 KB) + bias (second 1 KB)
 constexpr uint32_t kTapABytes = TH * TW * 128;  // 16 KB
 constexpr uint32_t kPoolTileBytes = kTapABytes / 4;   // the pooled 8x4 px x 64 ch output tile
@@ -674,8 +675,12 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
   }
   tg_pdl_wait();
   tg_pdl_trigger();
-  for (int i = threadIdx.x; i < d.cout; i += kThreads) bias_s[i] = d.bias[i];
-  __syncthreads();
+  // Only the consumer warpgroups read the bias.  They load it among themselves, so the producer issues its
+  // first TMA loads right after the wait, and their latency overlaps the bias load's.
+  if (warp >= 4) {
+    for (int i = threadIdx.x - 128; i < d.cout; i += kThreads - 128) bias_s[i] = d.bias[i];
+    named_bar_sync(kBiasBar, kThreads - 128);
+  }
 
   if (warp == 0) {
     // ============================================================ TMA producer
