@@ -1,4 +1,5 @@
-"""TEST INFRASTRUCTURE ONLY -- a torch/CPU stand-in for the kernels behind `tecogan-pytorch_b200/ops.py`,
+"""TEST INFRASTRUCTURE ONLY -- a torch/CPU stand-in for the kernels behind `tecogan-pytorch_b200/ops.py`
+(the training path and the inference step),
 with exactly the contracts of include/tecogan_b200.h (NHWC fp16 activations padded to 64 channels,
 loss-scaled fp16 gradients, fp32 parameter gradients in the parameters' layouts).
 
@@ -76,7 +77,7 @@ class PackedConv:
         self.b = bias.detach().to(COMPUTE)
         self.packed = self.w
 
-    def __call__(self, x, y=None, residual=None, **kw):
+    def __call__(self, x, y=None, residual=None, impl=None, a_mode=None, max_ctas=0, pool=False):
         xin = to_nchw(x, self.cin_real)
         if self.kind == CONV_3X3:
             v = F.conv2d(xin, self.w, self.b, 1, 1)
@@ -88,6 +89,8 @@ class PackedConv:
             v = _act(v, self.act)
             if residual is not None:
                 v = v + to_nchw(residual, self.cout_real)
+            if pool:                     # nn.MaxPool2d(2, 2) of the activated map (floor: odd last row / col dropped)
+                v = F.max_pool2d(v, 2, 2)
         if self.epilogue == EPI_NHWC_F16:
             out = to_nhwc(v, self.cout)
         else:
@@ -212,8 +215,16 @@ def _up(x, scale, up_mode):
     return R.upsample(p, x, scale, 'BD' if up_mode == UP_BICUBIC else 'BI')
 
 
+def _reflect_pad(x, hw):
+    """F.pad(x, 'reflect') on the bottom / right up to hw = (h, w) (tecogan_nets.py:239-241)"""
+    if hw is None:
+        return x
+    h, w = hw
+    return F.pad(x, (0, w - x.shape[3], 0, h - x.shape[2]), mode='reflect')
+
+
 def upsample(x, scale, up_mode, out_hw=None, mul=1.0, y=None, accumulate=False):
-    v = mul * _up(x, scale, up_mode)
+    v = mul * _up(_reflect_pad(x, out_hw), scale, up_mode)
     if y is not None:
         if accumulate:
             y += v
@@ -240,6 +251,34 @@ def upsample_bwd(gy, scale_factor, up_mode, mul=1.0, gx=None, accumulate=False):
 def warp_s2d_concat_hrflow(hr_prev, hr_flow, lr_curr, scale, out=None, cpad=64):
     v = torch.cat([lr_curr, R.s2d(R.warp(hr_prev, hr_flow), scale)], 1)
     return to_nhwc(v, cpad, out=out)
+
+
+def warp_s2d_concat_lrflow(hr_prev, lr_flow, lr_curr, scale, up_mode, out=None, cpad=64):
+    h, w = lr_curr.shape[2], lr_curr.shape[3]
+    hr_flow = scale * _up(_reflect_pad(lr_flow, (h, w)), scale, up_mode)
+    return warp_s2d_concat_hrflow(hr_prev, hr_flow, lr_curr, scale, out=out, cpad=cpad)
+
+
+def float_to_uint8_nhwc(x, y=None):
+    """uint8(clip(rint(x * 255), 0, 255)) as NHWC; the product is taken in fp32 (oracle.ops_oracle.float32_to_uint8),
+    torch.round is round-half-to-even"""
+    v = torch.round(x.to(torch.float32) * 255.0).clamp_(0, 255).to(torch.uint8).permute(0, 2, 3, 1)
+    return _out(v.contiguous(), y)
+
+
+def fused_tail(up, outc, x, lr_curr, lr_scale, up_mode, y=None, y_u8=None, max_ctas=0, accumulate=False):
+    """SRNet tail: t = relu(convT(x) + b_up) at the storage precision, v = conv_out(t) + b_out;
+    accumulate: y += v, else y = v + upsample_func(lr_curr) (lr_curr None: no residual) [, y_u8 = uint8(y)]"""
+    v = outc(up(x))
+    if accumulate:
+        y += v
+        return y
+    if lr_curr is not None:
+        v = v + _up(lr_curr, lr_scale, up_mode)
+    y = _out(v, y)
+    if y_u8 is not None:
+        float_to_uint8_nhwc(y, y_u8)
+    return y
 
 
 @torch.enable_grad()
@@ -317,13 +356,15 @@ FAKED = ('PackedConv', 'PackedDgrad', 'GradScale', 'wgrad', 'bias_grad', 'grad_p
          'maxpool2x2', 'upsample2x', 'upsample', 'upsample_bwd', 'warp_s2d_concat_hrflow', 'warp_s2d_concat_bwd',
          'maxpool2x2_bwd', 'upsample2x_bwd', 'flow_head_bwd', 'backward_warp', 'backward_warp_bwd',
          'space_to_depth', 'depth_to_space')
+# the ops only the inference step (FRNet.step_into) adds to those
+INFER_FAKED = ('fused_tail', 'warp_s2d_concat_lrflow', 'float_to_uint8_nhwc')
 
 
 def install(monkeypatch, pkg_ops, networks, net_utils, autograd):
     """Route the package's op layer to this module (CPU tensors accepted)."""
     import sys
     me = sys.modules[__name__]
-    for name in FAKED:
+    for name in FAKED + INFER_FAKED:
         monkeypatch.setattr(pkg_ops, name, getattr(me, name))
     monkeypatch.setattr(pkg_ops, 'chain_enabled', lambda: False)
     monkeypatch.setattr(networks, '_cuda_f32', lambda t, name: t.detach().float().contiguous())

@@ -507,9 +507,10 @@ def check_batch_consistency(n=3, h=24, w=40):
     return {}
 
 
-def check_engine_matches_eager(n=2, t=5, h=24, w=40):
-    """CUDA-graph clip engine == eager step loop, bit exact on the uint8 output."""
-    net, p = _net(16, 4, 'BD', 1.5, nb=3)
+def check_engine_matches_eager(n=2, t=5, h=24, w=40, nb=3):
+    """CUDA-graph clip engine == eager step loop, bit exact on the uint8 output; and per frame, the graph replay of a
+    ClipEngine == the same engine launching its kernels eagerly, bit exact on the fp32 HR frames too."""
+    net, p = _net(16, 4, 'BD', 1.5, nb=nb)
     clips = torch.stack([O.make_clip(70 + i, t, 3, h, w) for i in range(n)])       # n,t,c,h,w
     got = T.infer_clips(net, clips, torch.device(DEV))
     lr_prev = torch.zeros(n, 3, h, w, device=DEV)
@@ -521,6 +522,20 @@ def check_engine_matches_eager(n=2, t=5, h=24, w=40):
         assert np.array_equal(got[:, i], ref_u8), f'frame {i}'
         lr_prev, hr_prev = lr_curr, hr
     assert got.shape == (n, t, 4 * h, 4 * w, 3)
+    engs = [T.ClipEngine(net, n, 3, h, w, DEV, use_graph=g) for g in (True, False)]
+    for eng in engs:
+        eng.reset()
+    graph, eager = engs
+    for i in range(t):
+        par = i & 1
+        for eng in engs:
+            eng.lr[par].copy_(clips[:, i].to(DEV))
+            eng.run_frame(par)
+        torch.cuda.synchronize()
+        assert torch.equal(graph.hr[par].view(torch.int32), eager.hr[par].view(torch.int32)), f'frame {i}: fp32 hr differs'
+        assert torch.equal(graph.u8[par], eager.u8[par]), f'frame {i}: uint8 differs'
+    for eng in engs:
+        eng.close()
     return {}
 
 
@@ -1258,6 +1273,7 @@ CHECKS = {
     'forward_sequence_golden': check_forward_sequence_golden,
     'batch_consistency': check_batch_consistency,
     'engine_matches_eager': check_engine_matches_eager,
+    'engine_matches_eager_bench': lambda: check_engine_matches_eager(n=4, t=3, h=134, w=320, nb=10),
     'properties_fullsize': check_properties_fullsize,
     'ragged_sizes': check_ragged_sizes,
     'bi2_fullsize': check_bi2_fullsize,

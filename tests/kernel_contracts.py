@@ -1,12 +1,12 @@
-"""TEST INFRASTRUCTURE ONLY -- replays every op call of a training step against its contract in
-tests/fake_ops.py, on the arguments the step actually passes.
+"""TEST INFRASTRUCTURE ONLY -- replays every op call of a training step or of an inference step against its
+contract in tests/fake_ops.py, on the arguments the step actually passes.
 
 A Recorder wraps, on the package's op layer, exactly the names fake_ops.install replaces (the PackedConv /
 PackedDgrad / GradScale classes through subclasses that also note each layer's fp32 weight and bias).  For
 every top-level call it
 
   * copies every tensor argument to the CPU before the call (in-place outputs too: dw, db, d_hr_prev, y of an
-    accumulating upsample), and poisons write-only outputs with NaN;
+    accumulating upsample), and poisons write-only outputs with NaN (uint8 ones with the byte 77);
   * runs the stand-in on those copies in float64 (weights rounded to fp16 as the kernels store them), so each
     call is judged on its own inputs and errors do not compound;
   * compares every output per element: data movement and the loss scale bit for bit; arithmetic against
@@ -14,8 +14,12 @@ every top-level call it
     K the number of addends (plus a coordinate-rounding term for the bilinear warps).  ulp_out(0) = 0: pad
     channels and poisoned buffers must come back exactly written.
 
+Ops with a bound of their own: a pooled conv is held to the max-pool of its unpooled bound; fused_tail's fp32 frame
+to a bound that carries the fp16 HR map through conv_out (Recorder._tail), and its uint8 frame to the bits of
+float32_to_uint8 of that fp32 frame.
+
 Launches through the op layer from outside a wrapped call are collected as `unfaked`, so a kernel that enters
-the training path without a stand-in is reported.
+the training or inference path without a stand-in is reported.
 """
 import inspect
 import os
@@ -23,6 +27,7 @@ import sys
 
 import numpy as np
 import torch
+import torch.nn.functional as F
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for _p in (ROOT, os.path.join(ROOT, 'tests')):
@@ -41,10 +46,12 @@ OUTPUTS = {
     'upsample_bwd': ('gx',), 'warp_s2d_concat_hrflow': ('out',), 'warp_s2d_concat_bwd': ('d_hr_prev', 'd_hr_flow'),
     'maxpool2x2_bwd': ('gx',), 'upsample2x_bwd': ('gx',), 'flow_head_bwd': ('dz',), 'backward_warp': ('y',),
     'backward_warp_bwd': (), 'space_to_depth': ('y',), 'depth_to_space': (), 'GradScale': (),
+    'fused_tail': ('y', 'y_u8'), 'warp_s2d_concat_lrflow': ('out',), 'float_to_uint8_nhwc': ('y',),
 }
 ACCUMULATING = {('wgrad', 'dw'), ('wgrad', 'db'), ('bias_grad', 'db'), ('warp_s2d_concat_bwd', 'd_hr_prev')}
-EXACT = {'pack_pair', 'nchw_to_nhwc', 'space_to_depth', 'depth_to_space', 'grad_pack', 'maxpool2x2', 'GradScale'}
-WARPS = {'warp_s2d_concat_hrflow', 'warp_s2d_concat_bwd', 'backward_warp', 'backward_warp_bwd'}
+EXACT = {'pack_pair', 'nchw_to_nhwc', 'space_to_depth', 'depth_to_space', 'grad_pack', 'maxpool2x2', 'GradScale',
+         'float_to_uint8_nhwc'}
+WARPS = {'warp_s2d_concat_hrflow', 'warp_s2d_concat_lrflow', 'warp_s2d_concat_bwd', 'backward_warp', 'backward_warp_bwd'}
 
 
 def gamma(k):
@@ -82,11 +89,11 @@ def _overlaps(a, b):
 
 
 def _poison(t):
-    t.fill_(float('nan'))
+    t.fill_(77 if t.dtype == torch.uint8 else float('nan'))     # uint8 holds no NaN: a fixed byte instead
 
 
 class Recorder:
-    def __init__(self, ops, monkeypatch):
+    def __init__(self, ops, monkeypatch, names=FK.FAKED):
         self.ops = ops
         self.depth = 0
         self.params = {}            # id(layer object) -> (fp32 weight, fp32 bias or None) on the CPU
@@ -96,7 +103,7 @@ class Recorder:
         self.worst = {}             # op -> worst |err| / bound
         self.failures = []
         self.unfaked = []
-        for name in FK.FAKED:
+        for name in names:
             real = getattr(ops, name)
             wrapped = self._wrap_class(name, real) if inspect.isclass(real) else self._wrap_fn(name, real)
             monkeypatch.setattr(ops, name, wrapped)
@@ -183,6 +190,9 @@ class Recorder:
         ba.apply_defaults()
         args = dict(ba.arguments)
         args.pop('self', None)
+        for p in sig.parameters.values():       # a stand-in taking **kw: its keywords are arguments like the others
+            if p.kind == p.VAR_KEYWORD:
+                args.update(args.pop(p.name, {}))
         snap = {key: (v.detach().cpu().clone() if isinstance(v, torch.Tensor) else v) for key, v in args.items()}
         scale = args.get('scale')
         scale_ws = scale.ws.detach().cpu().clone() if scale is not None and hasattr(scale, 'ws') else None
@@ -204,7 +214,7 @@ class Recorder:
                 r[key] = v.abs() if absolute else v
             elif key == 'mul' and absolute:
                 r[key] = abs(v)
-            elif key == 'fwd':
+            elif key in ('fwd', 'up', 'outc'):
                 r[key] = self._fake_conv(v, absolute)
             elif key == 'scale' and hasattr(v, 'ws'):
                 r[key] = self._fake_scale(scale_ws)
@@ -242,49 +252,47 @@ class Recorder:
     def _check(self, name, obj, args, snap, scale_ws, out):
         got = {key: t.detach().cpu() for key, t in self._collect(name, out, args).items()}
         fn, ra = self._ref_args(name, obj, snap, scale_ws, False)
-        with _Mode():
-            rout = fn(**ra)
-        ref = {key: t for key, t in self._collect(name, rout, ra).items()}
+        bounds = None
+        if name == 'fused_tail':
+            ref, bounds = self._tail(ra)
+        else:
+            with _Mode():
+                rout = fn(**ra)
+            ref = {key: t for key, t in self._collect(name, rout, ra).items()}
         msgs = []
         if name in ('GradScale', 'flow_head_bwd'):
             ws_got = (obj if name == 'GradScale' else args['scale']).ws.detach().cpu().float()[:2]
             ws_ref = (rout if name == 'GradScale' else ra['scale']).ws.float()[:2]
             if not torch.equal(ws_got, ws_ref):
                 msgs.append(f'loss scale {ws_got.tolist()} != {ws_ref.tolist()}')
+        worst = 0.0
         if name in EXACT:
-            worst = 0.0
             for key, g in got.items():
                 r = ref[key].to(g.dtype)
-                ib = torch.int16 if g.dtype == torch.float16 else torch.int32
+                ib = {torch.float16: torch.int16, torch.uint8: torch.uint8}.get(g.dtype, torch.int32)
                 if g.shape != r.shape or not torch.equal(g.contiguous().view(ib), r.contiguous().view(ib)):
                     bad = int((g.double() != r.double()).sum()) if g.shape == r.shape else -1
                     msgs.append(f'{key}: not bit-exact ({bad} elements differ)')
                     worst = float('inf')
         else:
-            fa, aa = self._ref_args(name, obj, snap, scale_ws, True)
-            if name == 'flow_head_bwd':        # |terms| of g * (24 - f^2/24): |g| * 48, times the chosen scale
-                aa['flow'] = torch.zeros_like(aa['flow'])
-            with _Mode(absolute=True):
-                aout = fa(**aa)
-            absop = self._collect(name, aout, aa)
-            if name == 'flow_head_bwd':
-                s = float(ra['scale'].ws[0])
-                g = (ra['gflow'].abs() + (ra['gflow2'].abs() if ra['gflow2'] is not None else 0)) * 48 * s
-                key, = ref
-                a = torch.zeros(ref[key].shape, dtype=F64)
-                a[..., :2] = g.permute(0, 2, 3, 1)
-                absop = {key: a}
-            worst = 0.0
+            if bounds is None:
+                bounds = self._bounds(name, obj, args, snap, scale_ws, fn, ra, ref,
+                                      {key: g.dtype for key, g in got.items()})
             for key, g in got.items():
+                if name == 'fused_tail' and key == 'y_u8':
+                    # the uint8 frame is float32_to_uint8 of the kernel's OWN fp32 frame, bit for bit; how far that
+                    # frame is from the reference is the y check's business
+                    want = FK.float_to_uint8_nhwc(got['y'])
+                    if not torch.equal(g, want):
+                        msgs.append(f'y_u8: not float32_to_uint8(y) ({int((g != want).sum())} elements differ)')
+                        worst = float('inf')
+                    continue
                 r = ref[key]
                 gd = g.double()
                 if gd.shape != r.shape:
                     msgs.append(f'{key}: shape {tuple(gd.shape)} != {tuple(r.shape)}')
                     continue
-                bound = ulp(r, g.dtype) + gamma(self._k(name, key, obj, args)) * absop[key]
-                if name == 'PackedConv' and obj.epilogue == FK.EPI_FLOW_NCHW_F32:    # 24 * tanhf(pre-activation)
-                    bound = 4 * ulp(r, g.dtype) + 24 * gamma(self._k(name, key, obj, args)) * absop[key]
-                bound = bound + self._extra(name, key, ra, r, g.dtype)
+                bound = bounds[key]
                 err = (gd - r).abs()
                 err = torch.where(torch.isnan(gd), torch.full_like(err, float('inf')), err)
                 ratio = torch.where(bound > 0, err / bound, torch.where(err > 0, float('inf'), 0.0))
@@ -301,6 +309,81 @@ class Recorder:
             self.failures.append(f'{name} {shapes}: ' + '; '.join(msgs))
 
     # ------------------------------------------------------------------ bounds
+    def _bounds(self, name, obj, args, snap, scale_ws, fn, ra, ref, dtypes):
+        """{output: per-element bound} of an arithmetic op: ulp_out(ref) + gamma_K * (the op on |operands|)"""
+        fa, aa = self._ref_args(name, obj, snap, scale_ws, True)
+        if name == 'PackedConv' and args.get('pool'):
+            # pooled epilogue: the bound of the unpooled conv, max-pooled over the same 2x2 windows.  Each pooled
+            # output is max_i a_i (kernel) against max_i b_i (reference) over one window, and
+            # |max_i a_i - max_i b_i| <= max_i |a_i - b_i| <= max_i bound_i
+            key, = ref
+            ra, aa = dict(ra, pool=False, y=None), dict(aa, pool=False, y=None)
+            with _Mode():
+                r = fn(**ra)
+            with _Mode(absolute=True):
+                a = fa(**aa)
+            b = self._bound(name, key, obj, args, ra, r, a, dtypes[key])
+            return {key: F.max_pool2d(b.permute(0, 3, 1, 2), 2, 2).permute(0, 2, 3, 1)}
+        if name == 'flow_head_bwd':        # |terms| of g * (24 - f^2/24): |g| * 48, times the chosen scale
+            aa['flow'] = torch.zeros_like(aa['flow'])
+        with _Mode(absolute=True):
+            aout = fa(**aa)
+        absop = self._collect(name, aout, aa)
+        if name == 'flow_head_bwd':
+            s = float(ra['scale'].ws[0])
+            g = (ra['gflow'].abs() + (ra['gflow2'].abs() if ra['gflow2'] is not None else 0)) * 48 * s
+            key, = ref
+            a = torch.zeros(ref[key].shape, dtype=F64)
+            a[..., :2] = g.permute(0, 2, 3, 1)
+            absop = {key: a}
+        return {key: self._bound(name, key, obj, args, ra, r, absop[key], dtypes[key])
+                for key, r in ref.items() if key in dtypes}
+
+    def _bound(self, name, key, obj, args, ra, r, a, dtype):
+        k = gamma(self._k(name, key, obj, args))
+        if name == 'PackedConv' and obj.epilogue == FK.EPI_FLOW_NCHW_F32:    # 24 * tanhf(pre-activation)
+            return 4 * ulp(r, dtype) + 24 * k * a
+        return ulp(r, dtype) + k * a + self._extra(name, key, ra, r, dtype)
+
+    @staticmethod
+    def _tail(ra):
+        """fused_tail: the float64 reference of y and its bound, one image at a time (the 64-channel HR map of a
+        bench frame is 350 MB in float64).  With t = relu(convT(x) + b_up) >= 0 and r the residual (the pre-written y when
+        accumulating, else upsample_func(lr_curr)):
+          * the kernel sums convT in fp32 and keeps the 64-channel HR map in fp16:
+              |t_k - t| <= e_t = gamma(K1) A1 + ulp16(|t| + gamma(K1) A1),  A1 = |b_up| + convT(|x|, |w_up|),
+              K1 = 9 * 64 + 2 (relu is 1-Lipschitz);
+          * then conv_out(t_k) + b_out + r in fp32, rounded to the fp32 output:
+              |y_k - y| <= ulp32(y) + gamma(K2) A2 + conv_out(e_t, |w_out|),
+              A2 = |b_out| + conv_out(|t| + e_t, |w_out|) + |r|,  K2 = 9 * 64 + 2 + 20 (the in-kernel bicubic
+              residual is a 16-tap sum);
+            the last term is the fp16 rounding of the HR map pushed through |w_out|."""
+        up, outc, x, lr = ra['up'], ra['outc'], ra['x'], ra['lr_curr']
+        acc = ra['accumulate']
+        g1, g2 = gamma(9 * up.cin_real + 2), gamma(9 * outc.cin_real + 2 + 20)
+        ys, bounds = [], []
+        for i in range(x.shape[0]):
+            xi = x[i:i + 1]
+            lri = lr[i:i + 1] if lr is not None else None
+            with _Mode():
+                y = FK.fused_tail(up, outc, xi, lri, ra['lr_scale'], ra['up_mode'],
+                                  y=ra['y'][i:i + 1].clone() if acc else None, accumulate=acc)
+                xn = FK.to_nchw(xi, up.cin_real)
+                t = F.relu(F.conv_transpose2d(xn, up.w, up.b, 2, 1, output_padding=1))
+                a1 = F.conv_transpose2d(xn.abs(), up.w.abs(), up.b.abs(), 2, 1, output_padding=1)
+                e_t = g1 * a1 + ulp(t + g1 * a1, torch.float16)
+                wo = outc.w.abs()
+                a2 = F.conv2d(t + e_t, wo, outc.b.abs(), 1, 1)
+                if acc:
+                    a2 = a2 + ra['y'][i:i + 1].abs()
+                elif lri is not None:
+                    with _Mode(absolute=True):
+                        a2 = a2 + FK._up(lri.abs(), ra['lr_scale'], ra['up_mode'])
+                bounds.append(ulp(y, torch.float32) + g2 * a2 + F.conv2d(e_t, wo, None, 1, 1))
+            ys.append(y)
+        key = 'y' if ra['y'] is not None else 'ret'
+        return {key: torch.cat(ys)}, {key: torch.cat(bounds)}
+
     @staticmethod
     def _k(name, key, obj, args):
         """number of addends per output element (an upper bound)"""
@@ -332,12 +415,23 @@ class Recorder:
         """the bilinear warps: the kernels round the sample coordinate X + flow to fp32 (the stand-in does not)"""
         if name not in WARPS:
             return 0.0
-        flow = ra['hr_flow'] if 'hr_flow' in ra else ra['flow']
+        dflow = 0.0
+        if name == 'warp_s2d_concat_lrflow':
+            # the HR flow is itself computed in the kernel: scale * (an fp32 sum of <= 20 products) of the
+            # reflect-padded LR flow, off by at most scale * gamma(20) * upsample_func(|lr_flow|) -- one more
+            # coordinate error
+            s, hw = ra['scale'], tuple(ra['lr_curr'].shape[2:])
+            with _Mode():
+                flow = s * FK._up(FK._reflect_pad(ra['lr_flow'], hw), s, ra['up_mode'])
+            with _Mode(absolute=True):
+                dflow = s * gamma(20) * float(FK._up(FK._reflect_pad(ra['lr_flow'].abs(), hw), s, ra['up_mode']).max())
+        else:
+            flow = ra['hr_flow'] if 'hr_flow' in ra else ra['flow']
         x = ra['hr_prev'] if 'hr_prev' in ra else ra['x']
         H, W = flow.shape[2], flow.shape[3]
-        dc = 8 * U * (max(H, W) + float(flow.abs().max()))
+        dc = 8 * U * (max(H, W) + float(flow.abs().max())) + dflow
         xmax = float(x.abs().max())
-        if name in ('warp_s2d_concat_hrflow', 'backward_warp'):
+        if name in ('warp_s2d_concat_hrflow', 'warp_s2d_concat_lrflow', 'backward_warp'):
             return (gamma(8) + 2 * dc) * 4 * xmax
         g = _warp_grad_in(name, ra)                   # [n,C,H,W] gradient arriving at each HR sample
         if key in ('d_hr_flow', 'ret1'):
@@ -426,6 +520,71 @@ def scenarios(T, ops, dev):
     run_sequence(T, dev, 32, nb=10, n=1, t=3, h=32, w=32, flow_losses=False, loss_mul=1e-7)
     run_sequence(T, dev, 33, nb=1, n=1, t=3, h=16, w=24, degradation='BI', scale=2)
     run_module_ops(T, ops, dev, 34)
+
+
+# ---------------------------------------------------------------------------------------------- inference scenarios
+def inference_ops(tail, pool):
+    """the ops FRNet.step_into launches with ops.tail_mode() == tail and ops.pool_fused() == pool"""
+    names = {'pack_pair', 'PackedConv', 'upsample2x', 'warp_s2d_concat_lrflow'}
+    if not pool:
+        names.add('maxpool2x2')
+    if tail in ('acc', 'fused'):
+        names.add('fused_tail')
+    if tail != 'fused':
+        names |= {'upsample', 'float_to_uint8_nhwc'}
+    return names
+
+
+def run_frames(T, net, clips, dev):
+    """the recurrent eval step over clips [n,t,c,h,w] from zero state -- ClipEngine.run_frame without a CUDA graph on
+    a GPU (the step bench.py times), FRNet.step_into with a uint8 output on the CPU.  Returns the last (hr, u8)."""
+    n, t, c, h, w = clips.shape
+    s = net.scale
+    if torch.device(dev).type == 'cuda':
+        eng = T.ClipEngine(net, n, c, h, w, dev, use_graph=False)
+        eng.reset()
+        for i in range(t):
+            eng.lr[i & 1].copy_(clips[:, i].to(dev))
+            eng.run_frame(i & 1)
+        torch.cuda.synchronize()
+        return eng.hr[(t - 1) & 1], eng.u8[(t - 1) & 1]
+    lr_prev, hr_prev = torch.zeros(n, c, h, w), torch.zeros(n, c, s * h, s * w)
+    for i in range(t):
+        lr = clips[:, i].contiguous()
+        hr, u8 = torch.empty(n, c, s * h, s * w), torch.empty(n, s * h, s * w, c, dtype=torch.uint8)
+        net.step_into(lr, lr_prev, hr_prev, hr, out_u8=u8)
+        lr_prev, hr_prev = lr, hr
+    return hr, u8
+
+
+def run_inference(T, ops, dev, seed, nb, n, t, h, w, degradation='BD', scale=4, params=None, clips=None):
+    """t recurrent eval steps of n lock-stepped clips of h x w (O.make_clip, or `clips` [n,t,3,h,w]) through a net
+    with O.make_frnet_params(gain=1.5) (or `params`).  The net is built here, after the Recorder is installed:
+    layer objects made earlier would bypass its wrapped classes."""
+    from oracle import frnet_oracle as O
+    net = T.FRNet(3, 3, 64, nb, degradation, scale)
+    if params is None:
+        params = O.make_frnet_params(seed, nb=nb, scale=scale, degradation=degradation, gain=1.5)
+    net.load_state_dict(params, strict=True)
+    net = net.to(dev).eval()
+    if clips is None:
+        clips = torch.stack([O.make_clip(seed + 1 + k, t, 3, h, w) for k in range(n)])
+    return run_frames(T, net, clips, dev)
+
+
+def run_inference_module_ops(T, ops, dev, seed):
+    """the inference ops at edges the product step rarely reaches: warp_s2d_concat_lrflow on uniform-noise hr_prev
+    with LR flows of +-30 px (far past the borders) at sizes that are not multiples of 8 (reflect pad), bicubic x4
+    and bilinear x2; float_to_uint8_nhwc on values out of range and on exact rounding ties"""
+    for i, (scale, mode, h, w) in enumerate(((4, FK.UP_BICUBIC, 13, 22), (2, FK.UP_BILINEAR, 11, 19))):
+        s = seed + 10 * i
+        ops.warp_s2d_concat_lrflow(_rand(s, 2, 3, scale * h, scale * w, dev=dev),
+                                   _rand(s + 1, 2, 2, h // 8 * 8, w // 8 * 8, lo=-30, hi=30, dev=dev),
+                                   _rand(s + 2, 2, 3, h, w, dev=dev), scale, mode)
+    rng = np.random.default_rng(seed + 30)
+    ties = (rng.integers(-3, 259, size=(2, 3, 7, 11)) + 0.5) / 255.0
+    x = np.where(rng.random(ties.shape) < 0.5, ties, rng.uniform(-0.2, 1.2, size=ties.shape)).astype(np.float32)
+    ops.float_to_uint8_nhwc(torch.from_numpy(x).to(dev))
 
 
 def report(rec):
