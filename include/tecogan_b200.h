@@ -168,40 +168,6 @@ typedef struct tg_tail_desc {
 int tg_convT_convout_tcgen05(const tg_tail_desc* d, void* stream);
 
 /* ------------------------------------------------------------------------
- * A chain of 64->64 3x3 convolutions (SRNet conv_in + the residual blocks,
- * tecogan_nets.py:92-100, 111-116, 139-141) as ONE persistent cooperative launch: every CTA walks all
- * layers over its fixed set of 16x8 tiles; a tile of layer l starts as soon as the (up to 9)
- * tiles of layer l-1 under its 18x10 halo have been published (per-tile progress flags in
- * `sync_ws`), so there is no launch or whole-grid barrier between layers.  Bit-identical to
- * n_layers calls of tg_conv_tcgen05.
- *   layers[l].x / y / residual : NHWC fp16 [n,h,w,64]; y[l] is normally x[l+1].  y[l] may alias
- *       residual[l] (in place) or a buffer last READ by layer <= l-1; it must not alias x[l].
- *       At most 4 distinct x buffers per chain.
- *   sync_ws : device memory of tg_conv_chain_workspace_bytes(n,h,w) bytes, zeroed ONCE by the
- *       caller before first use, then owned by the library: word 0 = launch epoch, word 1 = count of
- *       finished CTAs, then one progress flag per tile, stamped with the epoch.  One chain launch in
- *       flight per workspace.
- * Needs every CTA co-resident (grid = min(#SM, tiles), 1 CTA/SM, cooperative launch: the driver
- * starts the grid only when all of its CTAs fit, or fails the launch): launch at most ONE chain at
- * a time per device and do not run it under an SM partition smaller than the device (waits are
- * bounded and trap instead of hanging).
- * ---------------------------------------------------------------------- */
-typedef struct tg_chain_layer {
-  const void* x;        /* NHWC fp16 [n,h,w,64]                          */
-  const void* weights;  /* tg_pack_conv3x3_weights(cout_pad=64, cin_pad=64) */
-  const float* bias;    /* fp32 [64]                                     */
-  const void* residual; /* NHWC fp16 [n,h,w,64] or NULL                  */
-  void* y;              /* NHWC fp16 [n,h,w,64]                          */
-  int32_t act;          /* TG_ACT_*                                      */
-  int32_t reserved;     /* must be 0                                     */
-} tg_chain_layer;
-#define TG_CHAIN_MAX_LAYERS 24
-
-size_t tg_conv_chain_workspace_bytes(int n, int h, int w);
-int tg_conv_chain_tcgen05(const tg_chain_layer* layers, int n_layers, int n, int h, int w,
-                          void* sync_ws, int max_ctas, void* stream);
-
-/* ------------------------------------------------------------------------
  * Fused  backward_warp + space_to_depth + concat  (HBM-bound).
  * Replaces net_utils.backward_warp (net_utils.py:50-82), space_to_depth
  * (:36-47) and torch.cat([lr_curr, hr_prev_tran]) (tecogan_nets.py:141).

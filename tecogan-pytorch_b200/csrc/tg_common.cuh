@@ -82,25 +82,6 @@ static inline cudaError_t tg_launch_cluster(void (*kernel)(KArgs...), dim3 grid,
   cfg.numAttrs = tg_pdl_enabled() ? 2 : 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
-
-// Cooperative launch: the driver schedules the grid only when EVERY CTA can be resident at once
-// (or fails the launch) -- required by kernels whose CTAs wait on each other (conv_chain_kernel).
-// Not combined with programmatic dependent launch: such a kernel starts after its predecessor.
-template <typename... KArgs, typename... Args>
-static inline cudaError_t tg_launch_cooperative(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
-                                                cudaStream_t stream, Args... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeCooperative;
-  attr[0].val.cooperative = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
 #endif
 
 // cudaFuncSetAttribute is per DEVICE: run `fn` once for every device this process launches on.

@@ -16,43 +16,42 @@
 //             consumer_splitk) or streamed per (tap, chunk) with cp.async.bulk (tap mode).
 //   D       : fp32 accumulators in the registers of the consumer warpgroup (64 per thread).
 //   roles   : warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers that take the
-//             CTA's tiles alternately, each with its own ring of smem stages: wgmma -> accumulators
-//             staged to a per-consumer fp32 smem tile -> one thread per pixel applies bias / act /
-//             residual (or the derivative, pool, pixel-shuffle and thin-head epilogues) and writes
-//             the pixel's 128-byte NHWC row.  On the forward halo and split-K paths the consumers take
-//             turns issuing their MMAs, so that one's epilogue runs under the other's MMAs.
+//             CTA's tiles alternately, each with its own ring of smem stages.  Data gradients, the
+//             stride-2 conv, the tap-mode kernels and the thin heads keep the pixels on M: wgmma ->
+//             accumulators staged to a per-consumer fp32 smem tile -> one thread per pixel applies bias /
+//             act / residual (or the derivative, pool, pixel-shuffle and thin-head epilogues) and writes
+//             the pixel's 128-byte NHWC row.
 //             The tap-mode transposed conv keeps 4 parity accumulators (1/2/2/4 taps), computed and
 //             stored one after the other; each stores its pixel's output of that parity (pixel shuffle).
 //
 // The forward halo conv and transposed conv with NHWC output (the SRNet body, the first SRNet
-// transposed conv and the FNet halo layers, pooled or not; see consumer_halo_pxn / consumer_convT_pxn)
-// swap the GEMM's roles: M = the 64 output channels (the packed weight tile is the K-major A operand),
-// N = the tile's 128 pixels (the halo view is the K-major B operand, 16 core groups of 8 pixels), so
-// each (tap, k-step) is ONE m64n128k16 that reads 6 KB of smem instead of two m64n64k16 that read 8 KB.
-// The epilogue works from registers: bias / act / residual -> fp16 -> stmatrix into a 16 KB tile in the
-// TMA box image -> one TMA tensor store per tile (per parity for the transposed conv, into a 5-D view
-// of its output); the residual arrives in that tile by one TMA load issued before the tile's MMAs.  With
-// the pool, the 2x2 max is taken in registers and a 4 KB pooled tile is stored.  Without the fp32
-// staging tiles each consumer's ring holds two halo stages or more.
+// transposed conv and the FNet halo layers, pooled or not; see consumer_halo_pxn / consumer_convT_pxn /
+// consumer_splitk) swap the GEMM's roles: M = the 64 output channels (the packed weight tile is the
+// K-major A operand), N = the tile's 128 pixels (the halo view is the K-major B operand, 16 core groups
+// of 8 pixels), so each (tap, k-step) is ONE m64n128k16 that reads 6 KB of smem instead of two m64n64k16
+// that read 8 KB.  The epilogue works from registers: bias / act / residual -> fp16 -> stmatrix into a
+// 16 KB tile in the TMA box image -> one TMA tensor store per tile (per parity for the transposed conv,
+// into a 5-D view of its output); the residual arrives in that tile by one TMA load issued before the
+// tile's MMAs.  With the pool, the 2x2 max is taken in registers and a 4 KB pooled tile is stored.
+// Without the fp32 staging tiles each consumer's ring holds two halo stages or more.  On the conv3x3 and
+// split-K paths the consumers take turns issuing their MMAs, so that one's epilogue runs under the
+// other's MMAs.  The mainloop and epilogue pieces (halo_pxn_mmas, convT_pxn_mmas, pxn_store_tile) are in
+// tg_wgmma.cuh; the fused SRNet tail (tg_tail.cu) uses the same ones.
 #include <cuda.h>
 
 #include <cstdlib>
-#include <mutex>
 
 #include "tg_common.cuh"
-#include "tg_epilogue.cuh"
 #include "tg_wgmma.cuh"
 
 namespace {
 
-constexpr int TH = 16, TW = 8;
 constexpr int kThreads = 384;             // producer warpgroup + 2 consumer warpgroups
 constexpr int kMaxRing = 4;               // smem stages per consumer ring
 constexpr int kBiasBar = 3;               // named barrier of both consumer warpgroups (1 + cw: one consumer's)
 constexpr uint32_t kHeaderBytes = 2048;   // barriers (first 1 KB) + bias (second 1 KB)
 constexpr uint32_t kTapABytes = TH * TW * 128;  // 16 KB
 constexpr uint32_t kPoolTileBytes = kTapABytes / 4;   // the pooled 8x4 px x 64 ch output tile
-constexpr uint32_t kSmemLimit = 232448;   // 227 KB opt-in limit per CTA
 // A-operand modes (template parameter MODE)
 constexpr int MODE_TAP = 0;    // one 16x8 box per (tap, chunk)
 constexpr int MODE_HALO = 1;   // one 18x10 halo box per (tile, chunk), taps = descriptor shifts
@@ -82,6 +81,23 @@ struct KParams {
   uint32_t off_b, off_stage, off_scratch;   // off_scratch: the consumers' fp32 staging or fp16 output tiles
   uint32_t epi_bytes;              // MODE_SPLITK: per-consumer receive buffer (the output tile overlaps it)
 };
+
+// The mbarriers of the header (8 bytes each), every slot named once; c = consumer 0 / 1.
+struct ConvBars {
+  uint32_t base;
+  enum { kFull = 0, kEmpty = 2 * kMaxRing, kWeights = 4 * kMaxRing, kRes, kRecv = kRes + 2, kFree = kRecv + 2,
+         kTurn = kFree + 2, kCount = kTurn + 2 };
+  __device__ uint32_t at(int slot) const { return base + 8u * (uint32_t)slot; }
+  // stage k of consumer c's ring: its TMA bytes have landed / its MMAs have read it (one arrival per consumer warp)
+  __device__ uint32_t full(int c, int k) const { return at(kFull + c * kMaxRing + k); }
+  __device__ uint32_t empty(int c, int k) const { return at(kEmpty + c * kMaxRing + k); }
+  __device__ uint32_t weights() const { return at(kWeights); }       // the resident weights have landed
+  __device__ uint32_t res(int c) const { return at(kRes + c); }      // consumer c's residual tile has landed
+  __device__ uint32_t recv(int c) const { return at(kRecv + c); }    // MODE_SPLITK: consumer c's partials received
+  __device__ uint32_t handback(int c) const { return at(kFree + c); }   // MODE_SPLITK: peers handed back their buffers
+  __device__ uint32_t turn(int c) const { return at(kTurn + c); }    // pixels-on-N conv3x3 / split-K: c may issue
+};
+static_assert(8 * ConvBars::kCount <= 1024, "the barriers take the first 1 KB of the header");
 
 // The forward halo conv / transposed conv with NHWC output (pooled or not) puts the roles of the GEMM the
 // other way round: D[cout][pixel] = W . X^T, the 64 output channels on M and the tile's 128 pixels on N.
@@ -216,23 +232,19 @@ __device__ __forceinline__ void epilogue_nhwc(const KParams& p, const TileCoord&
 //                        SBO 1024; B = the tap's shifted view of the halo stage, K-major, SBO = one box row)
 // then an epilogue from registers into a 16 KB tile in the TMA box image (16x8 px x 64 ch, 128B swizzle)
 // that one TMA tensor store writes out (clipped at the image edge).  The residual, if any, is TMA-loaded
-// into the same tile before the tile's MMAs and overwritten in place.  Thread t of the warpgroup holds
-// rows (couts) 16*(t/32) + (t%32)/4 + {0, 8} and pixel columns 8*j + 2*(t%4) + {0, 1}, j = 0..15.
-// POOL (MaxPool2d(2, 2) folded in): the 2x2 block (tile rows 2i, 2i+1; columns 2*(t%4), +1) of a cout lies in
-// four registers of one thread, so the pooled 8x4 px x 64 ch tile (4 KB) is formed without shuffles and
-// stored through the pooled tensor's map; clipping at that map's edge is the floor pooling.
+// into the same tile before the tile's MMAs and overwritten in place (pxn_store_tile).
+// POOL (MaxPool2d(2, 2) folded in, pxn_store_tile_pool2): the pooled 8x4 px x 64 ch tile (4 KB) is stored through
+// the pooled tensor's map; clipping at that map's edge is the floor pooling.
 template <bool POOL>
 __device__ __forceinline__ void consumer_halo_pxn(const TgMaps& maps, const KParams& p, uint32_t base,
                                                   const float* bias_s, int cw) {
   const tg_conv_desc& d = p.d;
   const int r = threadIdx.x - 128 * (1 + cw);
   const int q = r >> 5, lane = threadIdx.x & 31;
-  const uint32_t bar_full = base + 8u * (cw * kMaxRing), bar_empty = base + 16 * kMaxRing + 8u * (cw * kMaxRing);
-  const uint32_t bar_res = base + 32 * kMaxRing + 8 + 8u * cw;
+  const ConvBars bars{base};
+  const uint32_t bar_res = bars.res(cw);
   const uint32_t stage0 = base + p.off_stage + (uint32_t)(cw * p.ring) * p.stage_bytes;
   const uint32_t out_s = base + p.off_scratch + (uint32_t)cw * (POOL ? kPoolTileBytes : kTapABytes);
-  constexpr uint32_t kBoxW = TW + 2;
-  const uint64_t w_hi = gmma_desc_hi(1024u), x_hi = gmma_desc_hi(kBoxW * 128u);
   const uint32_t w16 = gmma_addr16(base + p.off_b), btb16 = p.b_stage_bytes >> 4;
   const bool has_res = !POOL && d.residual != nullptr;
   const int bar_id = 1 + cw;
@@ -246,15 +258,9 @@ __device__ __forceinline__ void consumer_halo_pxn(const TgMaps& maps, const KPar
   // whatever the tile counts of the two consumers (1 / 0, or unequal).  Waits and arrivals on a barrier
   // alternate (an arrival on turn[c] needs the wait that preceded the arriving consumer's own issue), so a parity
   // wait is never more than one phase behind; the arrival after a consumer's last tile has no waiter and is harmless.
-  const uint32_t turn_mine = base + 32 * kMaxRing + 56 + 8u * cw, turn_other = base + 32 * kMaxRing + 56 + 8u * (cw ^ 1);
+  const uint32_t turn_mine = bars.turn(cw), turn_other = bars.turn(cw ^ 1);
   uint32_t tphase = 0;
-  // stmatrix / ldmatrix: lane l addresses pixel row l%8 of 8x8 matrix m = l/8 = (tile row 2*jp + m/2,
-  // 8-channel chunk 2*q + m%2); the swizzled offset of (pixel px, chunk) is px*128 + ((chunk ^ px%8) << 4).
-  // POOL: matrix m = (pooled row pair 2*ip + m/2, chunk 2*q + m%2), its column 2*c + e = pooled pixel
-  // (row 2*(2*ip + m/2) + e, column c), i.e. lane l addresses tile pixel 8*(m/2) + kk, kk = 4*(l%2) + (l%8)/2.
-  const uint32_t kk = POOL ? 4u * (lane & 1) + ((lane & 7) >> 1) : (uint32_t)(lane & 7);
-  const uint32_t mat_off = (uint32_t)(8 * ((lane >> 3) >> 1) + kk) * 128u +
-                           ((uint32_t)((2 * q + ((lane >> 3) & 1)) ^ kk) << 4);
+  const uint32_t mat_off = pxn_mat_off(lane, q, 128u, /*swizzled=*/true, POOL);
   int stage = 0;
   uint32_t phase = 0, rphase = 0;
   float acc[64];
@@ -273,81 +279,29 @@ __device__ __forceinline__ void consumer_halo_pxn(const TgMaps& maps, const KPar
     int pend = -1;                       // stage whose MMAs may still be reading it
     for (int c = 0; c < p.chunks; ++c) {
       const int s = stage;
-      mbar_wait_mma(bar_full + 8 * s, phase);
+      mbar_wait_mma(bars.full(cw, s), phase);
       if (++stage == p.ring) { stage = 0; phase ^= 1u; }
       // take the turn only once the tile's first stage is here, so that it is never held while waiting on memory
       if (c == 0 && tile >= (int)gridDim.x) { mbar_wait_mma(turn_mine, tphase); tphase ^= 1u; }
       const uint32_t x16 = gmma_addr16(stage0 + (uint32_t)s * p.stage_bytes);
       wgmma_fence();
-#pragma unroll
-      for (int g = 0; g < 9; ++g) {
-        const TgGroup gr = tg_group(TG_CONV_3X3, g);
-        const uint32_t a16 = w16 + (uint32_t)(g * p.chunks + c) * btb16;
-        const uint32_t b16 = x16 + (uint32_t)((gr.dy + 1) * (int)kBoxW + (gr.dx + 1)) * 8u;
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          if (k < p.ksteps)
-            wgmma_n128(acc, w_hi | (uint64_t)(a16 + 2u * k), x_hi | (uint64_t)(b16 + 2u * k),
-                       (g == 0 && c == 0 && k == 0) ? 0u : 1u);
-      }
+      halo_pxn_mmas(acc, x16, w16, btb16, p.chunks, c, p.ksteps);
       wgmma_commit();
       if (c == p.chunks - 1) { __syncwarp(); if (lane == 0) mbar_arrive(turn_other); }   // pass the turn
       wgmma_wait<1>();
-      if (pend >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_empty + 8 * pend); }
+      if (pend >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bars.empty(cw, pend)); }
       pend = s;
     }
     wgmma_wait<0>();
     __syncwarp();
-    if (lane == 0) mbar_arrive(bar_empty + 8 * pend);
+    if (lane == 0) mbar_arrive(bars.empty(cw, pend));
 
     // the output tile is free once thread 0 saw the previous store read it (it issued the residual load after)
     if (has_res) { mbar_wait_mma(bar_res, rphase); rphase ^= 1u; }
     else named_bar_sync(bar_id, 128);
     const float b0 = bias_s[tc.nb * 64 + 16 * q + (lane >> 2)], b1 = bias_s[tc.nb * 64 + 16 * q + (lane >> 2) + 8];
-    if (POOL) {
-#pragma unroll
-      for (int ip = 0; ip < 2; ++ip) {
-        uint32_t ov[4];
-#pragma unroll
-        for (int m = 0; m < 4; ++m) {
-          const float bb = (m & 1) ? b1 : b0;
-          __half v[2];
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            // pooled row pr = tile rows 2*pr, 2*pr + 1; the same fp16 values the unpooled epilogue stores
-            const int pr = 2 * (2 * ip + (m >> 1)) + e;
-            const int i0 = 4 * (2 * pr) + 2 * (m & 1), i1 = i0 + 4;
-            const __half2 r0 = __floats2half2_rn(tg_epi_val(acc[i0], bb, d.act), tg_epi_val(acc[i0 + 1], bb, d.act));
-            const __half2 r1 = __floats2half2_rn(tg_epi_val(acc[i1], bb, d.act), tg_epi_val(acc[i1 + 1], bb, d.act));
-            const __half2 mx = __hmax2(r0, r1);
-            v[e] = __hmax(__low2half(mx), __high2half(mx));
-          }
-          const __half2 o = __halves2half2(v[0], v[1]);
-          ov[m] = *reinterpret_cast<const uint32_t*>(&o);
-        }
-        stmatrix_x4_trans(out_s + (uint32_t)ip * 2048u + mat_off, ov);
-      }
-    } else {
-#pragma unroll
-      for (int jp = 0; jp < 8; ++jp) {
-        const uint32_t addr = out_s + (uint32_t)jp * 2048u + mat_off;
-        uint32_t rv[4], ov[4];
-        if (has_res) ldmatrix_x4_trans(addr, rv);
-#pragma unroll
-        for (int m = 0; m < 4; ++m) {
-          const int i = 4 * (2 * jp + (m >> 1)) + 2 * (m & 1);
-          const float bb = (m & 1) ? b1 : b0;
-          float a0 = tg_epi_val(acc[i], bb, d.act), a1 = tg_epi_val(acc[i + 1], bb, d.act);
-          if (has_res) {
-            const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(&rv[m]));
-            a0 += rf.x; a1 += rf.y;
-          }
-          const __half2 o = __floats2half2_rn(a0, a1);
-          ov[m] = *reinterpret_cast<const uint32_t*>(&o);
-        }
-        stmatrix_x4_trans(addr, ov);
-      }
-    }
+    if (POOL) pxn_store_tile_pool2(acc, out_s, 128u, mat_off, b0, b1, d.act);
+    else pxn_store_tile(acc, out_s, 128u, mat_off, b0, b1, d.act, has_res);
     fence_proxy_async_smem();
     named_bar_sync(bar_id, 128);
     if (r == 0) {
@@ -389,12 +343,10 @@ __device__ __forceinline__ void consumer_splitk(const TgMaps& maps, const KParam
   const bool lead = r == rank * wpr * 32;  // first thread of the rank's first owned warp: stores, hand-backs
   const int sc = 64 / C;                   // output channels per rank
   const uint32_t sb = 2u * (uint32_t)sc;   // bytes per pixel of the rank's output slice tile
-  const uint32_t bar_full = base + 8u * (cw * kMaxRing), bar_empty = base + 16 * kMaxRing + 8u * (cw * kMaxRing);
-  const uint32_t bar_rfull = base + 32 * kMaxRing + 24 + 8u * cw, bar_free = base + 32 * kMaxRing + 40 + 8u * cw;
+  const ConvBars bars{base};
+  const uint32_t bar_rfull = bars.recv(cw), bar_free = bars.handback(cw);
   const uint32_t stage0 = base + p.off_stage + (uint32_t)(cw * p.ring) * p.stage_bytes;
   const uint32_t epi_s = base + p.off_scratch + (uint32_t)cw * p.epi_bytes;
-  constexpr uint32_t kBoxW = TW + 2;
-  const uint64_t w_hi = gmma_desc_hi(1024u), x_hi = gmma_desc_hi(kBoxW * 128u);
   const uint32_t w16 = gmma_addr16(base + p.off_b), btb16 = p.b_stage_bytes >> 4;
   const int bar_id = 1 + cw;
   // where this thread's partial goes in the owner's receive buffer (senders only)
@@ -403,15 +355,12 @@ __device__ __forceinline__ void consumer_splitk(const TgMaps& maps, const KParam
   const uint32_t peer_buf = mapa_shared(epi_s + send_off, (uint32_t)owner);
   const uint32_t peer_bar = mapa_shared(bar_rfull, (uint32_t)owner);
   const uint32_t recv_bytes = (uint32_t)((C - 1) * wpr) * 8192u;
-  // stmatrix: lane l addresses pixel row kk of matrix m = l/8 = (tile row pair, 8-channel chunk 2*q + m%2); in the
-  // rank's slice tile that chunk is local chunk 2*(q - rank*wpr) + m%2 (owners only)
-  const uint32_t kk = POOL ? 4u * (lane & 1) + ((lane & 7) >> 1) : (uint32_t)(lane & 7);
-  const uint32_t mat_off = (uint32_t)(8 * ((lane >> 3) >> 1) + kk) * sb +
-                           ((uint32_t)(2 * (q - rank * wpr) + ((lane >> 3) & 1)) << 4);
+  // in the rank's dense slice tile, warp q's chunks 2*q + m%2 are local chunks 2*(q - rank*wpr) + m%2 (owners only)
+  const uint32_t mat_off = pxn_mat_off(lane, q - rank * wpr, sb, /*swizzled=*/false, POOL);
   const int t0 = (int)cluster_id_x(), tstep = (int)cluster_count_x();
   // turns on the tensor pipe as in consumer_halo_pxn, over the CTA's tiles t0 + i * tstep; the waits for
   // peer CTAs (hand-back, partials) come after a tile's MMAs are issued, so the argument there holds here too
-  const uint32_t turn_mine = base + 32 * kMaxRing + 56 + 8u * cw, turn_other = base + 32 * kMaxRing + 56 + 8u * (cw ^ 1);
+  const uint32_t turn_mine = bars.turn(cw), turn_other = bars.turn(cw ^ 1);
   uint32_t tphase = 0;
   int stage = 0, it = 0;
   uint32_t phase = 0;
@@ -427,26 +376,18 @@ __device__ __forceinline__ void consumer_splitk(const TgMaps& maps, const KParam
       mbar_expect_tx(bar_rfull, recv_bytes);
     }
     const int s = stage;
-    mbar_wait_mma(bar_full + 8 * s, phase);
+    mbar_wait_mma(bars.full(cw, s), phase);
     if (++stage == p.ring) { stage = 0; phase ^= 1u; }
     if (tile >= tstep) { mbar_wait_mma(turn_mine, tphase); tphase ^= 1u; }
     const uint32_t x16 = gmma_addr16(stage0 + (uint32_t)s * p.stage_bytes);
     wgmma_fence();
-#pragma unroll
-    for (int g = 0; g < 9; ++g) {
-      const TgGroup gr = tg_group(TG_CONV_3X3, g);
-      const uint32_t a16 = w16 + (uint32_t)g * btb16;
-      const uint32_t b16 = x16 + (uint32_t)((gr.dy + 1) * (int)kBoxW + (gr.dx + 1)) * 8u;
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        wgmma_n128(acc, w_hi | (uint64_t)(a16 + 2u * k), x_hi | (uint64_t)(b16 + 2u * k), (g == 0 && k == 0) ? 0u : 1u);
-    }
+    halo_pxn_mmas(acc, x16, w16, btb16, 1, 0, 4);   // the rank's one chunk is resident: [tap][1]
     wgmma_commit();
     __syncwarp();
     if (lane == 0) mbar_arrive(turn_other);   // pass the turn
     wgmma_wait<0>();
     __syncwarp();
-    if (lane == 0) mbar_arrive(bar_empty + 8 * s);
+    if (lane == 0) mbar_arrive(bars.empty(cw, s));
 
     if (!own) {
       // the owner has handed back the buffer its previous tile's partials went to
@@ -477,42 +418,8 @@ __device__ __forceinline__ void consumer_splitk(const TgMaps& maps, const KParam
     named_bar_sync(bar_id, 128);         // the receive buffer is read: the output tile may overwrite it
     if (own) {
       const float b0 = bias_s[tc.nb * 64 + 16 * q + (lane >> 2)], b1 = bias_s[tc.nb * 64 + 16 * q + (lane >> 2) + 8];
-      if (POOL) {
-#pragma unroll
-        for (int ip = 0; ip < 2; ++ip) {
-          uint32_t ov[4];
-#pragma unroll
-          for (int m = 0; m < 4; ++m) {
-            const float bb = (m & 1) ? b1 : b0;
-            __half v[2];
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int pr = 2 * (2 * ip + (m >> 1)) + e;
-              const int i0 = 4 * (2 * pr) + 2 * (m & 1), i1 = i0 + 4;
-              const __half2 r0 = __floats2half2_rn(tg_epi_val(acc[i0], bb, d.act), tg_epi_val(acc[i0 + 1], bb, d.act));
-              const __half2 r1 = __floats2half2_rn(tg_epi_val(acc[i1], bb, d.act), tg_epi_val(acc[i1 + 1], bb, d.act));
-              const __half2 mx = __hmax2(r0, r1);
-              v[e] = __hmax(__low2half(mx), __high2half(mx));
-            }
-            const __half2 o = __halves2half2(v[0], v[1]);
-            ov[m] = *reinterpret_cast<const uint32_t*>(&o);
-          }
-          stmatrix_x4_trans(epi_s + (uint32_t)ip * 16u * sb + mat_off, ov);
-        }
-      } else {
-#pragma unroll
-        for (int jp = 0; jp < 8; ++jp) {
-          uint32_t ov[4];
-#pragma unroll
-          for (int m = 0; m < 4; ++m) {
-            const int i = 4 * (2 * jp + (m >> 1)) + 2 * (m & 1);
-            const float bb = (m & 1) ? b1 : b0;
-            const __half2 o = __floats2half2_rn(tg_epi_val(acc[i], bb, d.act), tg_epi_val(acc[i + 1], bb, d.act));
-            ov[m] = *reinterpret_cast<const uint32_t*>(&o);
-          }
-          stmatrix_x4_trans(epi_s + (uint32_t)jp * 16u * sb + mat_off, ov);
-        }
-      }
+      if (POOL) pxn_store_tile_pool2(acc, epi_s, sb, mat_off, b0, b1, d.act);
+      else pxn_store_tile(acc, epi_s, sb, mat_off, b0, b1, d.act, /*residual=*/false);
       fence_proxy_async_smem();
     }
     named_bar_sync(bar_id, 128);
@@ -535,14 +442,12 @@ __device__ __forceinline__ void consumer_convT_pxn(const TgMaps& maps, const KPa
   const tg_conv_desc& d = p.d;
   const int r = threadIdx.x - 128 * (1 + cw);
   const int q = r >> 5, lane = threadIdx.x & 31;
-  const uint32_t bar_full = base + 8u * (cw * kMaxRing), bar_empty = base + 16 * kMaxRing + 8u * (cw * kMaxRing);
+  const ConvBars bars{base};
   const uint32_t stage0 = base + p.off_stage + (uint32_t)(cw * p.ring) * p.stage_bytes;
   const uint32_t out0 = base + p.off_scratch + (uint32_t)cw * 2u * kTapABytes;
   const uint32_t w16 = gmma_addr16(base + p.off_b);
   const int bar_id = 1 + cw;
-  // as in consumer_halo_pxn: lane l addresses pixel row l%8 of matrix l/8 = (tile row 2*jp + m/2, chunk 2*q + m%2)
-  const uint32_t mat_off = (uint32_t)(8 * ((lane >> 3) >> 1) + (lane & 7)) * 128u +
-                           ((uint32_t)((2 * q + ((lane >> 3) & 1)) ^ (lane & 7)) << 4);
+  const uint32_t mat_off = pxn_mat_off(lane, q, 128u, /*swizzled=*/true, /*pool=*/false);
   int stage = 0;
   uint32_t phase = 0;
   float acc[64];
@@ -551,7 +456,7 @@ __device__ __forceinline__ void consumer_convT_pxn(const TgMaps& maps, const KPa
     const TileCoord tc = tile_coord(p, tile);
     const float b0 = bias_s[tc.nb * 64 + 16 * q + (lane >> 2)], b1 = bias_s[tc.nb * 64 + 16 * q + (lane >> 2) + 8];
     const int s = stage;
-    mbar_wait_mma(bar_full + 8 * s, phase);
+    mbar_wait_mma(bars.full(cw, s), phase);
     if (++stage == p.ring) { stage = 0; phase ^= 1u; }
     const uint32_t x16 = gmma_addr16(stage0 + (uint32_t)s * p.stage_bytes);
 #pragma unroll 1
@@ -563,20 +468,9 @@ __device__ __forceinline__ void consumer_convT_pxn(const TgMaps& maps, const KPa
       if (r == 0) bulk_wait_group_read1();
       named_bar_sync(bar_id, 128);
       wgmma_wait<0>();
-      if (a == 3) { __syncwarp(); if (lane == 0) mbar_arrive(bar_empty + 8 * s); }
+      if (a == 3) { __syncwarp(); if (lane == 0) mbar_arrive(bars.empty(cw, s)); }
       const uint32_t out_s = out0 + (uint32_t)(a & 1) * kTapABytes;
-#pragma unroll
-      for (int jp = 0; jp < 8; ++jp) {
-        uint32_t ov[4];
-#pragma unroll
-        for (int m = 0; m < 4; ++m) {
-          const int i = 4 * (2 * jp + (m >> 1)) + 2 * (m & 1);
-          const float bb = (m & 1) ? b1 : b0;
-          const __half2 o = __floats2half2_rn(tg_epi_val(acc[i], bb, d.act), tg_epi_val(acc[i + 1], bb, d.act));
-          ov[m] = *reinterpret_cast<const uint32_t*>(&o);
-        }
-        stmatrix_x4_trans(out_s + (uint32_t)jp * 2048u + mat_off, ov);
-      }
+      pxn_store_tile(acc, out_s, 128u, mat_off, b0, b1, d.act, /*residual=*/false);
       fence_proxy_async_smem();
       named_bar_sync(bar_id, 128);
       if (r == 0) {
@@ -606,14 +500,8 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
   const int warp = __shfl_sync(0xFFFFFFFFu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const tg_conv_desc& d = p.d;
 
-  // header: barriers, ring k of consumer c at index c * kMaxRing + k
-  const uint32_t bar_full = base;                          // [2 * kMaxRing]
-  const uint32_t bar_empty = base + 16 * kMaxRing;         // [2 * kMaxRing]
-  const uint32_t bar_b = base + 32 * kMaxRing;             // [1]
-  const uint32_t bar_res = bar_b + 8;                      // [2] residual tile of consumer c
-  const uint32_t bar_rfull = bar_b + 24;                   // [2] MODE_SPLITK: partials received, consumer c
-  const uint32_t bar_free = bar_b + 40;                    // [2] MODE_SPLITK: peers handed back their buffers
-  const uint32_t bar_turn = bar_b + 56;                    // [2] pixels-on-N conv3x3 / split-K: consumer c may issue
+  const ConvBars bars{base};
+  const uint32_t bar_b = bars.weights();
   float* bias_s = reinterpret_cast<float*>(sm + 1024);
   static_assert(!(KIND == TG_CONV_3X3_S2 && MODE != MODE_TAP), "the stride-2 conv runs in tap mode only");
   constexpr bool kPxN = pixels_on_n<KIND, MODE, BWD>();
@@ -627,22 +515,18 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
     if (kSplitK) tma_prefetch_desc(&maps.m[2]);
   }
   if (warp == 1 && lane == 0) {
-    for (int s = 0; s < 2 * kMaxRing; ++s) {
-      mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, 4);     // one arrival per consumer warp
-    }
     mbar_init(bar_b, 1);
-    mbar_init(bar_res, 1);
-    mbar_init(bar_res + 8, 1);
-    if (kSplitK) {
-      for (int c = 0; c < 2; ++c) {
-        mbar_init(bar_rfull + 8 * c, 1);             // the owner's expect_tx; the bytes come from the peers
-        mbar_init(bar_free + 8 * c, p.chunks - 1);   // one hand-back per peer
+    for (int c = 0; c < 2; ++c) {
+      for (int k = 0; k < kMaxRing; ++k) {
+        mbar_init(bars.full(c, k), 1);
+        mbar_init(bars.empty(c, k), 4);    // one arrival per consumer warp
       }
-    }
-    if (kSplitK || (kPxN && KIND == TG_CONV_3X3)) {
-      mbar_init(bar_turn, 4);              // one arrival per warp of the other consumer
-      mbar_init(bar_turn + 8, 4);
+      mbar_init(bars.res(c), 1);
+      if (kSplitK) {
+        mbar_init(bars.recv(c), 1);               // the owner's expect_tx; the bytes come from the peers
+        mbar_init(bars.handback(c), p.chunks - 1);    // one hand-back per peer
+      }
+      if (kSplitK || (kPxN && KIND == TG_CONV_3X3)) mbar_init(bars.turn(c), 4);   // one arrival per warp of the other consumer
     }
     fence_barrier_init();
   }
@@ -693,22 +577,22 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
         const TileCoord tc = tile_coord(p, tile);
         const int n_loads = MODE == MODE_TAP ? 9 * p.chunks : kSplitK ? 1 : p.chunks;
         for (int l = 0; l < n_loads; ++l) {
-          const int s = cw * kMaxRing + stage[cw];
-          mbar_wait_mma(bar_empty + 8 * s, phase[cw] ^ 1);
+          const uint32_t full = bars.full(cw, stage[cw]);
+          mbar_wait_mma(bars.empty(cw, stage[cw]), phase[cw] ^ 1);
           const uint32_t sa = smem_stage0 + (uint32_t)(cw * p.ring + stage[cw]) * p.stage_bytes;
           if (MODE != MODE_TAP) {
-            mbar_expect_tx(bar_full + 8 * s, p.a_bytes);
-            tma_load_4d(sa, &maps.m[0], bar_full + 8 * s, (l + k_rank) * 64, tc.x0 + p.org_x, tc.y0 + p.org_y, tc.n);
+            mbar_expect_tx(full, p.a_bytes);
+            tma_load_4d(sa, &maps.m[0], full, (l + k_rank) * 64, tc.x0 + p.org_x, tc.y0 + p.org_y, tc.n);
           } else {
             const int g = l / p.chunks, c = l - g * p.chunks;
             const TgGroup gr = tg_group(KIND, g);
-            mbar_expect_tx(bar_full + 8 * s, p.a_bytes + (p.b_resident ? 0u : p.b_stage_bytes));
-            tma_load_4d(sa, &maps.m[KIND == TG_CONV_3X3_S2 ? tg_s2_plane(g) : 0], bar_full + 8 * s, c * 64,
+            mbar_expect_tx(full, p.a_bytes + (p.b_resident ? 0u : p.b_stage_bytes));
+            tma_load_4d(sa, &maps.m[KIND == TG_CONV_3X3_S2 ? tg_s2_plane(g) : 0], full, c * 64,
                         tc.x0 + gr.dx, tc.y0 + gr.dy, tc.n);
             if (!p.b_resident)
               bulk_load(sa + kTapABytes,
                         wglob + (size_t)(g * p.chunks + c) * p.b_tile_bytes + (size_t)tc.nb * p.b_stage_bytes,
-                        p.b_stage_bytes, bar_full + 8 * s);
+                        p.b_stage_bytes, full);
           }
           if (++stage[cw] == p.ring) { stage[cw] = 0; phase[cw] ^= 1u; }
         }
@@ -759,11 +643,11 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
     };
     auto release = [&](int s) {
       __syncwarp();
-      if (lane == 0) mbar_arrive(bar_empty + 8 * (cw * kMaxRing + s));
+      if (lane == 0) mbar_arrive(bars.empty(cw, s));
     };
     auto next_stage = [&]() -> int {   // wait for the next stage of this consumer's ring; returns its index
       const int s = stage;
-      mbar_wait_mma(bar_full + 8 * (cw * kMaxRing + s), phase);
+      mbar_wait_mma(bars.full(cw, s), phase);
       if (++stage == p.ring) { stage = 0; phase ^= 1u; }
       return s;
     };
@@ -893,51 +777,6 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
 }
 
 // ------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                  const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  });
-  return fn;
-}
-
-// fp16 tensor of `rank` dims (dims[0] contiguous), element strides of dims 1.., 128B swizzle (or none)
-int encode_f16(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const size_t* elem_strides,
-               const cuuint32_t* box, bool swizzle = true) {
-  EncodeTiledFn fn = get_encode_fn();
-  TG_REQUIRE(fn != nullptr, TG_E_DRIVER, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t strides[4];
-  for (int i = 0; i + 1 < rank; ++i) strides[i] = (cuuint64_t)elem_strides[i] * 2;
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides, box,
-                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  TG_REQUIRE(r == CUDA_SUCCESS, TG_E_DRIVER,
-             "cuTensorMapEncodeTiled failed (%d) rank=%d dims=%llux%llux%llux%llu box=%ux%ux%u", (int)r, rank,
-             (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2],
-             (unsigned long long)dims[3], box[0], box[1], box[2]);
-  return TG_OK;
-}
-
-// NHWC fp16 tensor [n][h][w][c] with explicit element strides for w/h/n (parity views)
-int encode_nhwc(CUtensorMap* m, const void* ptr, int c, int w, int h, int n, size_t sw, size_t sh,
-                size_t sn, int box_c, int box_w, int box_h, bool swizzle = true) {
-  const cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
-  const size_t strides[3] = {sw, sh, sn};
-  const cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
-  return encode_f16(m, ptr, 4, dims, strides, box, swizzle);
-}
-
 // Output [n][2h][2w][c] of the transposed conv with input size h x w, as the 5-D tensor (2c, w, 2, h, n):
 // element (px*c + ch, x, py, y, n) is output pixel (2y + py, 2x + px).  Parity (py, px) of the 16x8 input
 // pixels at (y0, x0) is the box (64, 8, 1, 16, 1) at (px*c + nb*64, x0, py, y0, n); it clips at the right and

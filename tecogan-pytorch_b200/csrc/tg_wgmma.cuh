@@ -1,10 +1,18 @@
-// PTX wrappers shared by the tensor-core kernels of libtecogan_b200 (sm_90a): mbarriers, TMA
-// (tensor + bulk), wgmma with shared-memory descriptors.
+// Pieces shared by the tensor-core kernels of libtecogan_b200 (sm_90a): PTX wrappers (mbarriers, TMA tensor +
+// bulk, wgmma with shared-memory descriptors), the pixels-on-N mainloops and register epilogues, and the host-side
+// tensor-map encoder.
 #pragma once
 #include <cuda.h>
+
+#include <mutex>
+
 #include "tg_common.cuh"
+#include "tg_epilogue.cuh"
 
 namespace {
+
+constexpr int TH = 16, TW = 8;            // output tile of every tensor-core kernel: 16x8 pixels
+constexpr uint32_t kSmemLimit = 232448;   // 227 KB opt-in limit per CTA
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -277,6 +285,141 @@ __device__ __forceinline__ void convT_pxn_mmas(float (&acc)[64], uint32_t x16, u
     case 2: convT_pxn_parity<2>(acc, x16, w16); break;
     default: convT_pxn_parity<3>(acc, x16, w16); break;
   }
+}
+
+// 3x3 conv taps of 64-channel chunk c (of `chunks`) of one 16x8 tile, pixels on N:
+//   acc[64 cout][128 px] (+)= W[tap][c] (A: the packed [cout][64] tile, K-major, SBO 1024; the resident tiles at w16
+//                             are ordered [tap][chunk], tile16 = one tile's size / 16)
+//                             x the tap's shifted view of the 18x10 halo box (B: K-major, 16 core groups of 8
+//                             pixels, SBO = one box row of 10 x 128 B, origin -1, start += ((dy+1)*10+dx+1)*128 B)
+// one m64n128k16 per (tap, k-step < ksteps), taps outer and k-steps inner: that order is the accumulation order,
+// hence the output bits.  The first MMA of chunk 0 overwrites acc (scale-d = 0).
+__device__ __forceinline__ void halo_pxn_mmas(float (&acc)[64], uint32_t x16, uint32_t w16, uint32_t tile16, int chunks,
+                                              int c, int ksteps) {
+  constexpr uint32_t kBoxW = TW + 2;
+  const uint64_t w_hi = gmma_desc_hi(1024u), x_hi = gmma_desc_hi(kBoxW * 128u);
+#pragma unroll
+  for (int g = 0; g < 9; ++g) {
+    const TgGroup gr = tg_group(TG_CONV_3X3, g);
+    const uint32_t a16 = w16 + (uint32_t)(g * chunks + c) * tile16;
+    const uint32_t b16 = x16 + (uint32_t)((gr.dy + 1) * (int)kBoxW + (gr.dx + 1)) * 8u;
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (k < ksteps)
+        wgmma_n128(acc, w_hi | (uint64_t)(a16 + 2u * k), x_hi | (uint64_t)(b16 + 2u * k),
+                   (g == 0 && c == 0 && k == 0) ? 0u : 1u);
+  }
+}
+
+// ---- register epilogue of the pixels-on-N accumulators: acc[64 cout][128 px] -> fp16 -> stmatrix into an output
+// tile [pixel][channel], `pitch` bytes per pixel (128 B rows with the 128B swizzle = the TMA box image of a 64-channel
+// tile, or a dense unswizzled slice of fewer channels).  Thread t of the warpgroup holds couts 16*(t/32) + (t%32)/4
+// + {0, 8} and pixel columns 8*j + 2*(t%4) + {0, 1}, j = 0..15 (tile row j); one stmatrix.x4.trans writes two tile
+// rows x 16 couts of its warp.
+// Lane l addresses pixel row l%8 of 8x8 matrix m = l/8 = (tile row 2*jp + m/2, 8-channel chunk 2*q + m%2), q = the
+// warp's pair of chunks within the tile; the swizzled offset of (pixel px, chunk) is px*128 + ((chunk ^ px%8) << 4).
+// pool: matrix m = (pooled row pair 2*ip + m/2, chunk 2*q + m%2), its column 2*c + e = pooled pixel (row
+// 2*(2*ip + m/2) + e, column c), i.e. lane l addresses pooled-tile pixel 8*(m/2) + kk, kk = 4*(l%2) + (l%8)/2.
+__device__ __forceinline__ uint32_t pxn_mat_off(int lane, int q, uint32_t pitch, bool swizzled, bool pool) {
+  const uint32_t kk = pool ? 4u * (lane & 1) + ((lane & 7) >> 1) : (uint32_t)(lane & 7);
+  const uint32_t chunk = (uint32_t)(2 * q + ((lane >> 3) & 1));
+  return (uint32_t)(8 * ((lane >> 3) >> 1) + kk) * pitch + ((swizzled ? chunk ^ kk : chunk) << 4);
+}
+// act(acc + bias) [+ the residual already in the tile, overwritten in place] -> the 16x8 px tile at `tile`; b0 / b1 =
+// the bias of the thread's couts (t%32)/4 and + 8.
+__device__ __forceinline__ void pxn_store_tile(const float (&acc)[64], uint32_t tile, uint32_t pitch, uint32_t mat_off,
+                                               float b0, float b1, int act, bool residual) {
+#pragma unroll
+  for (int jp = 0; jp < 8; ++jp) {
+    const uint32_t addr = tile + (uint32_t)jp * 16u * pitch + mat_off;
+    uint32_t rv[4], ov[4];
+    if (residual) ldmatrix_x4_trans(addr, rv);
+#pragma unroll
+    for (int m = 0; m < 4; ++m) {
+      const int i = 4 * (2 * jp + (m >> 1)) + 2 * (m & 1);
+      const float bb = (m & 1) ? b1 : b0;
+      float a0 = tg_epi_val(acc[i], bb, act), a1 = tg_epi_val(acc[i + 1], bb, act);
+      if (residual) {
+        const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(&rv[m]));
+        a0 += rf.x; a1 += rf.y;
+      }
+      const __half2 o = __floats2half2_rn(a0, a1);
+      ov[m] = *reinterpret_cast<const uint32_t*>(&o);
+    }
+    stmatrix_x4_trans(addr, ov);
+  }
+}
+// MaxPool2d(2, 2) folded in: the 2x2 block (tile rows 2*pr, 2*pr + 1; columns 2*(t%4), + 1) of a cout lies in four
+// registers of one thread, so the pooled 8x4 px tile is formed without shuffles, from the same fp16 values the
+// unpooled epilogue stores.  mat_off from pxn_mat_off(pool = true).
+__device__ __forceinline__ void pxn_store_tile_pool2(const float (&acc)[64], uint32_t tile, uint32_t pitch,
+                                                     uint32_t mat_off, float b0, float b1, int act) {
+#pragma unroll
+  for (int ip = 0; ip < 2; ++ip) {
+    uint32_t ov[4];
+#pragma unroll
+    for (int m = 0; m < 4; ++m) {
+      const float bb = (m & 1) ? b1 : b0;
+      __half v[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int pr = 2 * (2 * ip + (m >> 1)) + e;
+        const int i0 = 4 * (2 * pr) + 2 * (m & 1), i1 = i0 + 4;
+        const __half2 r0 = __floats2half2_rn(tg_epi_val(acc[i0], bb, act), tg_epi_val(acc[i0 + 1], bb, act));
+        const __half2 r1 = __floats2half2_rn(tg_epi_val(acc[i1], bb, act), tg_epi_val(acc[i1 + 1], bb, act));
+        const __half2 mx = __hmax2(r0, r1);
+        v[e] = __hmax(__low2half(mx), __high2half(mx));
+      }
+      const __half2 o = __halves2half2(v[0], v[1]);
+      ov[m] = *reinterpret_cast<const uint32_t*>(&o);
+    }
+    stmatrix_x4_trans(tile + (uint32_t)ip * 16u * pitch + mat_off, ov);
+  }
+}
+
+// ---- host side: tensor maps
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+inline EncodeTiledFn get_encode_fn() {
+  static EncodeTiledFn fn = nullptr;
+  static std::once_flag once;
+  std::call_once(once, [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<EncodeTiledFn>(p);
+  });
+  return fn;
+}
+
+// fp16 tensor of `rank` dims (dims[0] contiguous), element strides of dims 1.., 128B swizzle (or none)
+inline int encode_f16(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const size_t* elem_strides,
+                      const cuuint32_t* box, bool swizzle = true) {
+  EncodeTiledFn fn = get_encode_fn();
+  TG_REQUIRE(fn != nullptr, TG_E_DRIVER, "cuTensorMapEncodeTiled not available from the driver");
+  cuuint64_t strides[4];
+  for (int i = 0; i + 1 < rank; ++i) strides[i] = (cuuint64_t)elem_strides[i] * 2;
+  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides, box,
+                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  TG_REQUIRE(r == CUDA_SUCCESS, TG_E_DRIVER,
+             "cuTensorMapEncodeTiled failed (%d) rank=%d dims=%llux%llux%llux%llu box=%ux%ux%u", (int)r, rank,
+             (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2],
+             (unsigned long long)dims[3], box[0], box[1], box[2]);
+  return TG_OK;
+}
+
+// NHWC fp16 tensor [n][h][w][c] with explicit element strides for w/h/n (parity views)
+inline int encode_nhwc(CUtensorMap* m, const void* ptr, int c, int w, int h, int n, size_t sw, size_t sh, size_t sn,
+                       int box_c, int box_w, int box_h, bool swizzle = true) {
+  const cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
+  const size_t strides[3] = {sw, sh, sn};
+  const cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+  return encode_f16(m, ptr, 4, dims, strides, box, swizzle);
 }
 
 }  // namespace

@@ -25,16 +25,13 @@
 #include <cuda.h>
 
 #include <cstdlib>
-#include <mutex>
 
 #include "tg_common.cuh"
 #include "tg_wgmma.cuh"
 
 namespace {
 
-constexpr int TH = 16, TW = 8;
 constexpr int kThreads = 512;            // warpgroup 0: TMA producer; warpgroups 1-3: taps 0-2, 3-5, 6-8
-constexpr uint32_t kSmemLimit = 232448;
 constexpr uint32_t kDzTileBytes = TH * TW * 128;   // 16 KB
 constexpr int kMaxStages = 6;
 
@@ -235,39 +232,6 @@ wgrad_simt_kernel(const __half* __restrict__ x, const __half* __restrict__ dz, f
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn wgrad_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, [] {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  });
-  return fn;
-}
-
-// NHWC fp16 [n][h][w][c] view with explicit element strides (parity planes of the convT output)
-int wgrad_encode(CUtensorMap* m, const void* ptr, int c, int w, int h, int n, size_t sw, size_t sh, size_t sn,
-                 int box_w, int box_h) {
-  EncodeTiledFn fn = wgrad_encode_fn();
-  TG_REQUIRE(fn != nullptr, TG_E_DRIVER, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
-  cuuint64_t strides[3] = {(cuuint64_t)sw * 2, (cuuint64_t)sh * 2, (cuuint64_t)sn * 2};
-  cuuint32_t box[4] = {64, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  TG_REQUIRE(r == CUDA_SUCCESS, TG_E_DRIVER, "wgrad: cuTensorMapEncodeTiled failed (%d) c=%d w=%d h=%d n=%d", (int)r, c,
-             w, h, n);
-  return TG_OK;
-}
-
 int wgrad_validate(const tg_wgrad_desc* d, const char* who) {
   TG_REQUIRE(d != nullptr, TG_E_INVALID, "%s: null descriptor", who);
   TG_REQUIRE(d->x && d->dz && d->dw, TG_E_INVALID, "%s: null pointer", who);
@@ -312,12 +276,12 @@ int tg_wgrad_tcgen05(const tg_wgrad_desc* d, void* stream) {
   TG_REQUIRE(stages >= 2, TG_E_UNSUPPORTED, "wgrad: shared memory budget");
   p.n_stages = stages;
 
-  rc = wgrad_encode(&p.map_x, d->x, d->cin, d->w, d->h, d->n, (size_t)d->cin, (size_t)d->w * d->cin,
-                    (size_t)d->h * d->w * d->cin, p.box_w, p.box_h);
+  rc = encode_nhwc(&p.map_x, d->x, d->cin, d->w, d->h, d->n, (size_t)d->cin, (size_t)d->w * d->cin,
+                   (size_t)d->h * d->w * d->cin, 64, p.box_w, p.box_h);
   if (rc != TG_OK) return rc;
   if (conv) {
-    rc = wgrad_encode(&p.map_dz[0], d->dz, d->cout, d->w, d->h, d->n, (size_t)d->cout, (size_t)d->w * d->cout,
-                      (size_t)d->h * d->w * d->cout, TW, TH);
+    rc = encode_nhwc(&p.map_dz[0], d->dz, d->cout, d->w, d->h, d->n, (size_t)d->cout, (size_t)d->w * d->cout,
+                     (size_t)d->h * d->w * d->cout, 64, TW, TH);
     if (rc != TG_OK) return rc;
     for (int i = 1; i < 4; ++i) p.map_dz[i] = p.map_dz[0];
   } else {
@@ -325,8 +289,8 @@ int tg_wgrad_tcgen05(const tg_wgrad_desc* d, void* stream) {
     const size_t W2 = (size_t)2 * d->w, C = (size_t)d->cout;
     for (int pl = 0; pl < 4; ++pl) {
       const __half* base = reinterpret_cast<const __half*>(d->dz) + ((size_t)(pl >> 1) * W2 + (pl & 1)) * C;
-      rc = wgrad_encode(&p.map_dz[pl], base, d->cout, d->w, d->h, d->n, 2 * C, 2 * W2 * C,
-                        (size_t)4 * d->h * d->w * C, TW, TH);
+      rc = encode_nhwc(&p.map_dz[pl], base, d->cout, d->w, d->h, d->n, 2 * C, 2 * W2 * C,
+                       (size_t)4 * d->h * d->w * C, 64, TW, TH);
       if (rc != TG_OK) return rc;
     }
   }

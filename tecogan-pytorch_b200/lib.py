@@ -38,14 +38,6 @@ class ConvDesc(ctypes.Structure):
     ]
 
 
-class ChainLayer(ctypes.Structure):
-    """struct tg_chain_layer"""
-    _fields_ = [
-        ('x', c_void_p), ('weights', c_void_p), ('bias', c_void_p), ('residual', c_void_p),
-        ('y', c_void_p), ('act', c_int32), ('reserved', c_int32),
-    ]
-
-
 class WgradDesc(ctypes.Structure):
     """struct tg_wgrad_desc"""
     _fields_ = [
@@ -78,8 +70,6 @@ class FarnebackParams(ctypes.Structure):
                 ('poly_n', c_int32), ('poly_sigma', c_double), ('flags', c_int32), ('reserved', c_int32)]
 
 
-CHAIN_MAX_LAYERS = 24
-
 _P = c_void_p
 _SIGNATURES = {
     'tg_version': (c_int, []),
@@ -93,8 +83,6 @@ _SIGNATURES = {
     'tg_conv_tcgen05': (c_int, [ctypes.POINTER(ConvDesc), _P]),
     'tg_conv_simt': (c_int, [ctypes.POINTER(ConvDesc), _P]),
     'tg_convT_convout_tcgen05': (c_int, [ctypes.POINTER(TailDesc), _P]),
-    'tg_conv_chain_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
-    'tg_conv_chain_tcgen05': (c_int, [ctypes.POINTER(ChainLayer), c_int, c_int, c_int, c_int, _P, c_int, _P]),
     'tg_warp_s2d_concat_hrflow': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_warp_s2d_concat_lrflow': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int,
                                           c_int, c_int, c_int, _P]),

@@ -160,7 +160,6 @@ class SRNet(nn.Module):
         self.conv_out = nn.Conv2d(nf, out_nc, 3, 1, 1, bias=True)
         self.upsample_func = upsample_func
         self._cache = _ConvCache()
-        self._chain = None
 
     def forward(self, lr_curr, hr_prev_tran):
         """lr_curr nchw, hr_prev_tran n(s*s*c)hw (both fp32) -> hr nchw fp32"""
@@ -177,21 +176,10 @@ class SRNet(nn.Module):
         for i, blk in enumerate(self.resblocks):
             body += [c.get(('r', i, 0), blk.conv[0], L.CONV_3X3, _RELU),
                      c.get(('r', i, 2), blk.conv[2], L.CONV_3X3, L.ACT_NONE)]
-        if (ops.chain_enabled() and ops.default_conv_impl() == 'tcgen05' and x.shape[-1] == 64
-                and ops.ConvChain.supported(body)):
-            # conv_in + all residual blocks in ONE persistent launch (TECOGAN_B200_CHAIN=1): buffers 0 = x (read only),
-            # 1 = block input/output (conv2 writes it in place over its own residual), 2 = conv1 output
-            if self._chain is None or [s[0] for s in self._chain.specs] != body:
-                specs = [(body[0], 0, 1, None)]
-                for i in range(len(self.resblocks)):
-                    specs += [(body[1 + 2 * i], 1, 2, None), (body[2 + 2 * i], 2, 1, 1)]
-                self._chain = ops.ConvChain(specs)
-            a = self._chain([x, torch.empty_like(x), torch.empty_like(x)])
-        else:
-            a = body[0](x)
-            for i in range(len(self.resblocks)):
-                t = body[1 + 2 * i](a)
-                a = body[2 + 2 * i](t, residual=a)
+        a = body[0](x)
+        for i in range(len(self.resblocks)):
+            t = body[1 + 2 * i](a)
+            a = body[2 + 2 * i](t, residual=a)
         ups = [c.get(('up', u), self.conv_up[u], L.CONVT_3X3_S2, _RELU) for u in range(0, len(self.conv_up), 2)]
         pc_out = c.get('out', self.conv_out, L.CONV_3X3, L.ACT_NONE, L.EPI_OUT_NCHW_F32)
         tail = ops.tail_mode()

@@ -146,55 +146,6 @@ class PackedConv:
         return y
 
 
-class ConvChain:
-    """A chain of 64->64 3x3 convs in ONE persistent launch (tg_conv_chain_tcgen05).
-
-    specs: list of (PackedConv, src, dst, res) where src/dst/res index into `buffers` (res may be
-    None).  buffers[0] is the chain input (never written)."""
-
-    def __init__(self, specs):
-        if not 1 <= len(specs) <= L.CHAIN_MAX_LAYERS:
-            raise L.TecoganB200Error(f'conv chain: {len(specs)} layers (1..{L.CHAIN_MAX_LAYERS})')
-        for pc, src, dst, res in specs:
-            if pc.kind != L.CONV_3X3 or pc.epilogue != L.EPI_NHWC_F16 or pc.cin != 64 or pc.cout != 64:
-                raise L.TecoganB200Error('conv chain: every layer must be a 64->64 3x3 conv (NHWC fp16)')
-            if src == dst or dst == 0:
-                raise L.TecoganB200Error('conv chain: a layer may not write its own input or the chain input')
-        self.specs = list(specs)
-        self._ws = {}
-
-    @staticmethod
-    def supported(pcs):
-        return all(pc.kind == L.CONV_3X3 and pc.epilogue == L.EPI_NHWC_F16 and pc.cin == 64 and pc.cout == 64
-                   for pc in pcs) and 1 <= len(pcs) <= L.CHAIN_MAX_LAYERS
-
-    def workspace(self, n, h, w, device):
-        key = (n, h, w, str(device))
-        ws = self._ws.get(key)
-        if ws is None:
-            nbytes = L.load().tg_conv_chain_workspace_bytes(n, h, w)
-            ws = self._ws[key] = torch.zeros(nbytes, dtype=torch.uint8, device=device)   # zeroed ONCE
-        return ws
-
-    def __call__(self, buffers, max_ctas=0):
-        x = buffers[0]
-        _req(x, torch.float16, 'chain input', 4)
-        n, h, w, c = x.shape
-        for t in buffers:
-            _req(t, torch.float16, 'chain buffer', 4)
-            if tuple(t.shape) != (n, h, w, 64):
-                raise L.TecoganB200Error(f'conv chain: buffer shape {tuple(t.shape)} != {(n, h, w, 64)}')
-        arr = (L.ChainLayer * len(self.specs))()
-        for i, (pc, src, dst, res) in enumerate(self.specs):
-            arr[i].x, arr[i].weights, arr[i].bias = buffers[src].data_ptr(), pc.packed.data_ptr(), pc.bias.data_ptr()
-            arr[i].residual = buffers[res].data_ptr() if res is not None else None
-            arr[i].y, arr[i].act, arr[i].reserved = buffers[dst].data_ptr(), pc.act, 0
-        ws = self.workspace(n, h, w, x.device)
-        L.check(L.load().tg_conv_chain_tcgen05(arr, len(self.specs), n, h, w, _ptr(ws), max_ctas, _stream()),
-                'tg_conv_chain_tcgen05')
-        return buffers[self.specs[-1][2]]
-
-
 def fused_tail(up, outc, x, lr_curr, lr_scale, up_mode, y=None, y_u8=None, max_ctas=0, accumulate=False):
     """SRNet tail in one launch (tg_convT_convout_tcgen05): y = conv_out(relu(convT(x))) + upsample_func(lr_curr)
     [, y_u8 = float32_to_uint8(y) as NHWC].  `up` / `outc` are the PackedConv objects of the last transposed
@@ -245,12 +196,8 @@ def pool_fused():
 
 
 def chain_enabled():
-    """TECOGAN_B200_CHAIN=1 runs SRNet's conv_in + residual blocks as one persistent tg_conv_chain_tcgen05 launch
-    instead of 21 PDL launches of tg_conv_tcgen05 (same products in the same order, with its own mainloop; held
-    to a 4e-3 relative tolerance against them).  Off by default: on an H100 the 21 launches measured faster
-    (the chain kernel keeps one halo stage per consumer and stalls on every layer's weight reload): 1205 us per
-    21-layer chain against 21 x 41.7 us of the previous per-layer kernel, bd4 shape."""
-    return os.environ.get('TECOGAN_B200_CHAIN', '0') == '1'
+    # bench.py asks; the persistent conv-chain kernel was removed (DESIGN.md)
+    return False
 
 
 def default_conv_impl():

@@ -366,7 +366,6 @@ def install(monkeypatch, pkg_ops, networks, net_utils, autograd):
     me = sys.modules[__name__]
     for name in FAKED + INFER_FAKED:
         monkeypatch.setattr(pkg_ops, name, getattr(me, name))
-    monkeypatch.setattr(pkg_ops, 'chain_enabled', lambda: False)
     monkeypatch.setattr(networks, '_cuda_f32', lambda t, name: t.detach().float().contiguous())
     monkeypatch.setattr(net_utils, '_chk', lambda t, name: t)
     monkeypatch.setattr(net_utils, '_f32', lambda t, name: t.detach().float().contiguous())

@@ -257,88 +257,6 @@ def check_conv_issue_variants(kind=None, cin_real=64, cout_real=64, h=61, w=45, 
     return {'bit_identical': True, 'rel_max_vs_simt': e}
 
 
-def check_conv_chain(n=2, h=37, w=29, blocks=2, max_ctas=0, repeats=1, seed=50):
-    """tg_conv_chain_tcgen05 (conv_in + `blocks` residual blocks in ONE persistent launch, tiles
-    gated by progress flags) vs the same layers as 1+2*blocks launches of tg_conv_tcgen05 on
-    identical packed weights: same MMAs in the same order, so the outputs are bit-identical (the
-    tolerance only guards against a future change of the issue order); `repeats` relaunches on
-    the same workspace exercise the epoch stamping of the flags.  The work buffers are poisoned
-    with NaN so a tile consumed before it was produced cannot go unnoticed."""
-    bound = 1.2 / np.sqrt(9 * 64)
-    pcs = []
-    for i in range(1 + 2 * blocks):
-        act = L.ACT_RELU if (i == 0 or i % 2 == 1) else L.ACT_NONE
-        pcs.append(ops.PackedConv(rand(seed + 3 * i, 64, 64, 3, 3, lo=-bound, hi=bound).to(DEV),
-                                  rand(seed + 3 * i + 1, 64, lo=-0.2, hi=0.2).to(DEV), L.CONV_3X3, act))
-    specs = [(pcs[0], 0, 1, None)]
-    for b in range(blocks):
-        specs += [(pcs[1 + 2 * b], 1, 2, None), (pcs[2 + 2 * b], 2, 1, 1)]
-    chain = ops.ConvChain(specs)
-    worst, frac = 0.0, 0.0
-    for rep in range(repeats):
-        x = nhwc(rand(seed + 100 + rep, n, 64, h, w, lo=-1, hi=1), 64)
-        a = pcs[0](x)
-        for b in range(blocks):
-            t = pcs[1 + 2 * b](a)
-            a = pcs[2 + 2 * b](t, residual=a)
-        # poison the chain's work buffers: stale data must never be read before it is produced
-        b1 = torch.full_like(x, float('nan'))
-        b2 = torch.full_like(x, float('nan'))
-        y = chain([x, b1, b2], max_ctas=max_ctas)
-        torch.cuda.synchronize()
-        assert torch.isfinite(y.float()).all(), f'chain output has non-finite values (rep {rep})'
-        d = (y.float() - a.float()).abs()
-        e = float(d.max() / a.float().abs().max())
-        worst = max(worst, e)
-        frac = max(frac, float((d > 0).float().mean()))
-        assert e <= 4e-3, f'conv chain vs per-layer launches: rel max {e} (rep {rep}, n={n} h={h} w={w} blocks={blocks})'
-    return {'rel_max': worst, 'frac_diff': frac}
-
-
-def check_conv_chain_plain(n=2, h=33, w=50, layers=24, seed=90):
-    """The longest chain the ABI takes (24 layers), no residuals, ping-pong over two work buffers,
-    LeakyReLU between layers -- vs the same layers launched one by one."""
-    bound = 1.4 / np.sqrt(9 * 64)
-    pcs = [ops.PackedConv(rand(seed + 2 * i, 64, 64, 3, 3, lo=-bound, hi=bound).to(DEV),
-                          rand(seed + 2 * i + 1, 64, lo=-0.1, hi=0.1).to(DEV), L.CONV_3X3, L.ACT_LRELU02)
-           for i in range(layers)]
-    specs = [(pcs[i], 0 if i == 0 else 1 + (i - 1) % 2, 1 + i % 2, None) for i in range(layers)]
-    x = nhwc(rand(seed + 200, n, 64, h, w, lo=-1, hi=1), 64)
-    a = x
-    for pc in pcs:
-        a = pc(a)
-    y = ops.ConvChain(specs)([x, torch.full_like(x, float('nan')), torch.full_like(x, float('nan'))])
-    torch.cuda.synchronize()
-    assert torch.isfinite(y.float()).all()
-    d = (y.float() - a.float()).abs()
-    e = float(d.max() / a.float().abs().max())
-    assert e <= 4e-3, f'24-layer chain vs per-layer launches: rel max {e}'
-    return {'rel_max': e, 'frac_diff': float((d > 0).float().mean())}
-
-
-def check_conv_chain_vs_reference(n=1, h=20, w=24, blocks=1, seed=70):
-    """conv chain vs the CPU fp32 reference of the same three layers (fp16-rounded between layers)."""
-    bound = 1.2 / np.sqrt(9 * 64)
-    ws = [rand(seed + 3 * i, 64, 64, 3, 3, lo=-bound, hi=bound) for i in range(1 + 2 * blocks)]
-    bs = [rand(seed + 3 * i + 1, 64, lo=-0.2, hi=0.2) for i in range(1 + 2 * blocks)]
-    acts = [L.ACT_RELU if (i == 0 or i % 2 == 1) else L.ACT_NONE for i in range(1 + 2 * blocks)]
-    pcs = [ops.PackedConv(ws[i].to(DEV), bs[i].to(DEV), L.CONV_3X3, acts[i]) for i in range(len(ws))]
-    specs = [(pcs[0], 0, 1, None)]
-    for b in range(blocks):
-        specs += [(pcs[1 + 2 * b], 1, 2, None), (pcs[2 + 2 * b], 2, 1, 1)]
-    x = rand(seed + 50, n, 64, h, w, lo=-1, hi=1)
-    xd = nhwc(x, 64)
-    y = ops.ConvChain(specs)([xd, torch.empty_like(xd), torch.empty_like(xd)])
-    torch.cuda.synchronize()
-    a = f16(_conv_ref(x, ws[0], bs[0], L.CONV_3X3, acts[0]))
-    for b in range(blocks):
-        t = f16(_conv_ref(a, ws[1 + 2 * b], bs[1 + 2 * b], L.CONV_3X3, acts[1 + 2 * b]))
-        a = f16(_conv_ref(t, ws[2 + 2 * b], bs[2 + 2 * b], L.CONV_3X3, acts[2 + 2 * b], a))
-    e = relmax(from_nhwc(y, 64).numpy(), a.numpy())
-    assert e <= 4e-3, f'conv chain vs CPU reference: rel max {e}'
-    return {'rel_max': e}
-
-
 def check_conv_epilogues(impl='tcgen05'):
     out = {}
     # flow head: 24*tanh(conv) -> NCHW fp32 [n,2,h,w]
@@ -1258,13 +1176,6 @@ CHECKS = {
     'conv_issue_variants_thin_6_32': lambda: check_conv_issue_variants(cin_real=6, cout_real=32),
     'conv_issue_variants_thin_32_64': lambda: check_conv_issue_variants(cin_real=32, cout_real=64, h=33, w=80),
     'conv_issue_variants_convT': lambda: check_conv_issue_variants(kind=L.CONVT_3X3_S2, h=24, w=40, n=2),
-    'conv_chain_vs_reference': check_conv_chain_vs_reference,
-    'conv_chain_1tile': lambda: check_conv_chain(n=1, h=16, w=8, blocks=1),
-    'conv_chain_ragged_repeat': lambda: check_conv_chain(n=2, h=37, w=29, blocks=2, repeats=3),
-    'conv_chain_few_ctas': lambda: check_conv_chain(n=3, h=50, w=44, blocks=3, max_ctas=5, repeats=2),
-    'conv_chain_full': lambda: check_conv_chain(n=4, h=134, w=320, blocks=10, repeats=2),
-    'conv_chain_24_layers': check_conv_chain_plain,
-    'conv_chain_two_tiles_per_cta': lambda: check_conv_chain(n=1, h=134, w=320, blocks=4, max_ctas=0, repeats=2, seed=120),
     'step_golden_g1': lambda: check_step_golden('g1'),
     'step_golden_g15': lambda: check_step_golden('g15'),
     'step_golden_g2_stress': lambda: check_step_golden('g2'),

@@ -66,26 +66,6 @@ def test_backward_entry_points_reject_bad_arguments_without_a_gpu():
     assert lib.tg_warp_s2d_concat_bwd(None, None, None, None, None, None, 1, 3, 8, 8, 4, 64, None) == -1
 
 
-def test_chain_layer_struct_and_argument_checks():
-    # struct tg_chain_layer: 5 pointers + 2 int32
-    assert ctypes.sizeof(L.ChainLayer) == 5 * 8 + 2 * 4
-    assert L.ChainLayer.act.offset == 40
-    lib = L.load()
-    # 16 uint32 of control words... + one progress flag per 16x8 tile
-    assert lib.tg_conv_chain_workspace_bytes(4, 134, 320) == (32 + 4 * 9 * 40) * 4
-    assert lib.tg_conv_chain_workspace_bytes(0, 134, 320) == 0
-    arr = (L.ChainLayer * 2)()
-    assert lib.tg_conv_chain_tcgen05(arr, 2, 1, 16, 8, None, 0, None) == -1          # null workspace
-    assert lib.tg_conv_chain_tcgen05(arr, 0, 1, 16, 8, ctypes.c_void_p(16), 0, None) == -2
-    assert lib.tg_conv_chain_tcgen05(arr, L.CHAIN_MAX_LAYERS + 1, 1, 16, 8, ctypes.c_void_p(16), 0, None) == -2
-    assert lib.tg_conv_chain_tcgen05(arr, 2, 1, 16, 8, ctypes.c_void_p(16), 0, None) == -1   # null layer pointers
-    assert b'layer 0' in lib.tg_last_error_string()
-    for a in arr:
-        a.x, a.weights, a.bias, a.y = 1024, 2048, 4096, 1024                         # y aliases x
-    assert lib.tg_conv_chain_tcgen05(arr, 2, 1, 16, 8, ctypes.c_void_p(16), 0, None) == -1
-    assert b'aliases' in lib.tg_last_error_string()
-
-
 def test_null_and_bad_arguments_are_rejected_without_a_gpu():
     lib = L.load()
     rc = lib.tg_maxpool2x2_nhwc_f16(None, None, 1, 4, 4, 64, None)

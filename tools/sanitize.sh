@@ -9,8 +9,8 @@
 set -u
 OUT=gpurun_out/sanitizer
 mkdir -p "$OUT"
-MEM=${SAN_MEMCHECK:-"warp_hrflow_s4 warp_lrflow_bd4 pool_upsample module_ops downsample_bd conv_tc_halo_64 conv_tc_tap_convT epilogues_tc conv_chain_1tile conv_chain_ragged_repeat step_golden_g1"}
-RACE=${SAN_RACECHECK:-"warp_lrflow_bd4 conv_tc_halo_64 conv_tc_tap_convT epilogues_tc conv_chain_ragged_repeat"}
+MEM=${SAN_MEMCHECK:-"warp_hrflow_s4 warp_lrflow_bd4 pool_upsample module_ops downsample_bd conv_tc_halo_64 conv_tc_tap_convT epilogues_tc step_golden_g1"}
+RACE=${SAN_RACECHECK:-"warp_lrflow_bd4 conv_tc_halo_64 conv_tc_tap_convT epilogues_tc"}
 TMO=${SAN_TIMEOUT:-600}
 for tool in memcheck racecheck; do
   if [ $tool = memcheck ]; then LIST=$MEM; else LIST=$RACE; fi
