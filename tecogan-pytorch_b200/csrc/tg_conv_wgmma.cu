@@ -16,7 +16,8 @@
 //             consumer_splitk) or streamed per (tap, chunk) with cp.async.bulk (tap mode).
 //   D       : fp32 accumulators in the registers of the consumer warpgroup (64 per thread).
 //   roles   : warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers that take the
-//             CTA's tiles alternately, each with its own ring of smem stages.  Data gradients, the
+//             CTA's tiles alternately, each with its own ring of smem stages (the forward pixels-on-N
+//             conv3x3 has three consumers on one shared ring, see below).  Data gradients, the
 //             stride-2 conv, the tap-mode kernels and the thin heads keep the pixels on M: wgmma ->
 //             accumulators staged to a per-consumer fp32 smem tile -> one thread per pixel applies bias /
 //             act / residual (or the derivative, pool, pixel-shuffle and thin-head epilogues) and writes
@@ -33,22 +34,25 @@
 // 16 KB tile in the TMA box image -> one TMA tensor store per tile (per parity for the transposed conv,
 // into a 5-D view of its output); the residual arrives in that tile by one TMA load issued before the
 // tile's MMAs.  With the pool, the 2x2 max is taken in registers and a 4 KB pooled tile is stored.
-// Without the fp32 staging tiles each consumer's ring holds two halo stages or more.  On the conv3x3 and
-// split-K paths the consumers take turns issuing their MMAs, so that one's epilogue runs under the
-// other's MMAs.  The mainloop and epilogue pieces (halo_pxn_mmas, convT_pxn_mmas, pxn_store_tile) are in
-// tg_wgmma.cuh; the fused SRNet tail (tg_tail.cu) uses the same ones.
+// On the conv3x3 and split-K paths the consumers take turns issuing their MMAs, so that one's epilogue
+// runs under the others' MMAs.  The conv3x3 (consumer_halo_pxn) runs three consumer warpgroups (512
+// threads) on one four-stage halo ring filled in tile order, so each epilogue has two other consumers'
+// MMA turns to hide under; a bottom tile row with at most 8 rows inside the image issues m64n64k16 over
+// its first 8 tile rows.  The transposed conv keeps two consumers with two halo stages each.  The
+// mainloop and epilogue pieces (halo_pxn_mmas, convT_pxn_mmas, pxn_store_tile) are in tg_wgmma.cuh; the
+// fused SRNet tail (tg_tail.cu) uses the same ones.
 #include <cuda.h>
 
 #include <cstdlib>
+#include <type_traits>
 
 #include "tg_common.cuh"
 #include "tg_wgmma.cuh"
 
 namespace {
 
-constexpr int kThreads = 384;             // producer warpgroup + 2 consumer warpgroups
-constexpr int kMaxRing = 4;               // smem stages per consumer ring
-constexpr int kBiasBar = 3;               // named barrier of both consumer warpgroups (1 + cw: one consumer's)
+constexpr int kMaxRing = 4;               // smem stages per ring
+constexpr int kBiasBar = 4;               // named barrier of all consumer warpgroups (1 + cw: one consumer's)
 constexpr uint32_t kHeaderBytes = 2048;   // barriers (first 1 KB) + bias (second 1 KB)
 constexpr uint32_t kTapABytes = TH * TW * 128;  // 16 KB
 constexpr uint32_t kPoolTileBytes = kTapABytes / 4;   // the pooled 8x4 px x 64 ch output tile
@@ -74,7 +78,7 @@ struct KParams {
   int halo, b_resident;
   int box_w, box_h, org_x, org_y;
   int step_y, step_x;              // output pixels a tile advances by (16x8; 14x6 for MODE_TAPN)
-  int ring;                        // smem stages per consumer
+  int ring;                        // smem stages per ring
   int ksteps;                      // wgmma k-steps (16 channels) per 64-channel chunk that can hold non-zero input (1..4)
   int n_split, bn;                 // output channels are split over n_split CTAs of bn columns
   uint32_t stage_bytes, a_bytes, b_tile_bytes, b_stage_bytes;
@@ -82,13 +86,14 @@ struct KParams {
   uint32_t epi_bytes;              // MODE_SPLITK: per-consumer receive buffer (the output tile overlaps it)
 };
 
-// The mbarriers of the header (8 bytes each), every slot named once; c = consumer 0 / 1.
+// The mbarriers of the header (8 bytes each), every slot named once; c = consumer 0 / 1 (0..2 for res and turn).
+// The three consumers of the pixels-on-N conv3x3 share ring 0.
 struct ConvBars {
   uint32_t base;
-  enum { kFull = 0, kEmpty = 2 * kMaxRing, kWeights = 4 * kMaxRing, kRes, kRecv = kRes + 2, kFree = kRecv + 2,
-         kTurn = kFree + 2, kCount = kTurn + 2 };
+  enum { kFull = 0, kEmpty = 2 * kMaxRing, kWeights = 4 * kMaxRing, kRes, kRecv = kRes + 3, kFree = kRecv + 2,
+         kTurn = kFree + 2, kCount = kTurn + 3 };
   __device__ uint32_t at(int slot) const { return base + 8u * (uint32_t)slot; }
-  // stage k of consumer c's ring: its TMA bytes have landed / its MMAs have read it (one arrival per consumer warp)
+  // stage k of ring c: its TMA bytes have landed / its MMAs have read it (one arrival per warp of the consumer)
   __device__ uint32_t full(int c, int k) const { return at(kFull + c * kMaxRing + k); }
   __device__ uint32_t empty(int c, int k) const { return at(kEmpty + c * kMaxRing + k); }
   __device__ uint32_t weights() const { return at(kWeights); }       // the resident weights have landed
@@ -104,6 +109,16 @@ static_assert(8 * ConvBars::kCount <= 1024, "the barriers take the first 1 KB of
 template <int KIND, int MODE, bool BWD>
 __host__ __device__ constexpr bool pixels_on_n() {
   return (KIND == TG_CONV_3X3 || KIND == TG_CONVT_3X3_S2) && MODE == MODE_HALO && !BWD;
+}
+// Consumer warpgroups: three for the forward pixels-on-N conv3x3 (consumer_halo_pxn, one shared ring of halo stages),
+// two, each with its own ring, for every other instantiation.  The producer warpgroup comes first.
+template <int KIND, int MODE, bool BWD>
+__host__ __device__ constexpr int conv_consumers() {
+  return KIND == TG_CONV_3X3 && pixels_on_n<KIND, MODE, BWD>() ? 3 : 2;
+}
+template <int KIND, int MODE, bool BWD>
+__host__ __device__ constexpr int conv_threads() {
+  return 128 * (1 + conv_consumers<KIND, MODE, BWD>());
 }
 
 struct TileCoord { int n, y0, x0, nb; };
@@ -227,7 +242,7 @@ __device__ __forceinline__ void epilogue_nhwc(const KParams& p, const TileCoord&
 }
 
 // ------------------------------------------------------------------ consumer of the pixels-on-N path
-// One consumer warpgroup (cw) of the forward 3x3 halo conv, NHWC fp16 output: for each of its tiles
+// One of the three consumer warpgroups (cw) of the forward 3x3 halo conv, NHWC fp16 output: for each of its tiles
 //   D[64 cout][128 px] = sum over (tap, chunk, k-step) of m64n128k16(A = resident weight tile, K-major,
 //                        SBO 1024; B = the tap's shifted view of the halo stage, K-major, SBO = one box row)
 // then an epilogue from registers into a 16 KB tile in the TMA box image (16x8 px x 64 ch, 128B swizzle)
@@ -235,66 +250,78 @@ __device__ __forceinline__ void epilogue_nhwc(const KParams& p, const TileCoord&
 // into the same tile before the tile's MMAs and overwritten in place (pxn_store_tile).
 // POOL (MaxPool2d(2, 2) folded in, pxn_store_tile_pool2): the pooled 8x4 px x 64 ch tile (4 KB) is stored through
 // the pooled tensor's map; clipping at that map's edge is the floor pooling.
+// The weights are one 64-channel chunk (cin = 64; wider inputs take the split-K path), so a tile is one halo stage.
 template <bool POOL>
 __device__ __forceinline__ void consumer_halo_pxn(const TgMaps& maps, const KParams& p, uint32_t base,
                                                   const float* bias_s, int cw) {
+  constexpr int kNC = conv_consumers<TG_CONV_3X3, MODE_HALO, false>();
   const tg_conv_desc& d = p.d;
   const int r = threadIdx.x - 128 * (1 + cw);
   const int q = r >> 5, lane = threadIdx.x & 31;
   const ConvBars bars{base};
   const uint32_t bar_res = bars.res(cw);
-  const uint32_t stage0 = base + p.off_stage + (uint32_t)(cw * p.ring) * p.stage_bytes;
+  const uint32_t stage0 = base + p.off_stage;
   const uint32_t out_s = base + p.off_scratch + (uint32_t)cw * (POOL ? kPoolTileBytes : kTapABytes);
   const uint32_t w16 = gmma_addr16(base + p.off_b), btb16 = p.b_stage_bytes >> 4;
   const bool has_res = !POOL && d.residual != nullptr;
   const int bar_id = 1 + cw;
-  // Turns on the tensor pipe.  The CTA's tiles blockIdx.x + i * gridDim.x, i = 0, 1, 2, ..., go to consumer i & 1.
-  // The owner of tile i > 0 issues its MMAs only after the other consumer has issued (and committed) tile i - 1:
-  // it waits on turn[cw], on which the other consumer's four warps arrive after each of their commits.  The
-  // tensor pipe then runs the two consumers' MMAs one tile after the other instead of sharing it, so one
-  // consumer's epilogue runs under the other's MMAs rather than both epilogues leaving the pipe idle together.
-  // No deadlock: every tile i > 0 has its tile i - 1 in the same CTA, and issuing tile i - 1 waits only for
-  // tile i - 2's issue and for memory (the stage, the store drain), never for anything of tile i or later,
-  // whatever the tile counts of the two consumers (1 / 0, or unequal).  Waits and arrivals on a barrier
+  // Turns on the tensor pipe.  The CTA's tiles blockIdx.x + i * gridDim.x, i = 0, 1, 2, ..., go to consumer i mod 3.
+  // The owner of tile i > 0 issues its MMAs only after the owner of tile i - 1 has issued (and committed) it: it
+  // waits on turn[cw], on which the previous consumer's four warps arrive after each of their commits.  The tensor
+  // pipe then runs the consumers' MMAs one tile after the other instead of sharing it, and each epilogue runs under
+  // the next two consumers' MMAs.  No deadlock: every tile i > 0 has its tile i - 1 in the same CTA, and issuing
+  // tile i - 1 waits only for tile i - 2's issue and for memory (the stage, the store drain), never for anything of
+  // tile i or later, whatever the consumers' tile counts (0, 1 or unequal).  Waits and arrivals on a barrier
   // alternate (an arrival on turn[c] needs the wait that preceded the arriving consumer's own issue), so a parity
   // wait is never more than one phase behind; the arrival after a consumer's last tile has no waiter and is harmless.
-  const uint32_t turn_mine = bars.turn(cw), turn_other = bars.turn(cw ^ 1);
+  // The shared ring: tile i is in stage i mod R with parity (i / R) & 1, filled by the producer in tile order.  A
+  // parity wait never mistakes an older fill of the stage for tile i's: the owner of tile j + 3 also owned tile j,
+  // and it issued tile j only after tile j - 1 had been issued, hence after tile j - 1's stage wait had returned.
+  // With R >= 4, tile j + 3 shares its stage with tile j + 3 - R, which is tile j - 1 or earlier, so that fill's
+  // phase has completed.  The invariant is ring depth >= consumers + 1 (the host requires R >= 4).
+  const uint32_t turn_mine = bars.turn(cw), turn_next = bars.turn(cw + 1 == kNC ? 0 : cw + 1);
   uint32_t tphase = 0;
   const uint32_t mat_off = pxn_mat_off(lane, q, 128u, /*swizzled=*/true, POOL);
-  int stage = 0;
-  uint32_t phase = 0, rphase = 0;
+  uint32_t rphase = 0;
   float acc[64];
 
-  for (int tile = blockIdx.x + cw * (int)gridDim.x; tile < p.num_tiles; tile += 2 * (int)gridDim.x) {
+  for (int i = cw;; i += kNC) {
+    const int tile = (int)blockIdx.x + i * (int)gridDim.x;
+    if (tile >= p.num_tiles) break;
     const TileCoord tc = tile_coord(p, tile);
     if (r == 0) {
-      bulk_wait_group_read0();           // the previous tile's store has left the output tile
+      bulk_wait_group_read0();           // the previous tile's store (three tiles back) has left the output tile
       if (has_res) {
         mbar_expect_tx(bar_res, kTapABytes);
         tma_load_4d(out_s, &maps.m[1], bar_res, tc.nb * 64, tc.x0, tc.y0, tc.n);
       }
     }
 #pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-    int pend = -1;                       // stage whose MMAs may still be reading it
-    for (int c = 0; c < p.chunks; ++c) {
-      const int s = stage;
-      mbar_wait_mma(bars.full(cw, s), phase);
-      if (++stage == p.ring) { stage = 0; phase ^= 1u; }
-      // take the turn only once the tile's first stage is here, so that it is never held while waiting on memory
-      if (c == 0 && tile >= (int)gridDim.x) { mbar_wait_mma(turn_mine, tphase); tphase ^= 1u; }
-      const uint32_t x16 = gmma_addr16(stage0 + (uint32_t)s * p.stage_bytes);
+    for (int k = 0; k < 64; ++k) acc[k] = 0.f;
+    const int s = i % p.ring;
+    mbar_wait_mma(bars.full(0, s), (uint32_t)(i / p.ring) & 1u);
+    // take the turn only once the tile's stage is here, so that it is never held while waiting on memory
+    if (i > 0) { mbar_wait_mma(turn_mine, tphase); tphase ^= 1u; }
+    const uint32_t x16 = gmma_addr16(stage0 + (uint32_t)s * p.stage_bytes);
+    auto mmas = [&](auto n, auto ks) {   // each path waits for its own MMAs (see halo_pxn_mmas)
       wgmma_fence();
-      halo_pxn_mmas(acc, x16, w16, btb16, p.chunks, c, p.ksteps);
+      halo_pxn_mmas<decltype(n)::value, decltype(ks)::value>(acc, x16, w16, btb16, 1, 0, p.ksteps);
       wgmma_commit();
-      if (c == p.chunks - 1) { __syncwarp(); if (lane == 0) mbar_arrive(turn_other); }   // pass the turn
-      wgmma_wait<1>();
-      if (pend >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bars.empty(cw, pend)); }
-      pend = s;
-    }
-    wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(turn_next);   // pass the turn
+      wgmma_wait<0>();
+    };
+    // A bottom tile row with at most 8 rows inside the image: m64n64k16 over rows 0-7 (rows 8-15 keep the zeros).
+    // Inputs with all 64 channels real (every layer but FNet's first) run 4 k-steps fixed at compile time.
+    using Rows16 = std::integral_constant<int, 128>;
+    using Rows8 = std::integral_constant<int, 64>;
+    using KSteps4 = std::integral_constant<int, 4>;
+    using KStepsRuntime = std::integral_constant<int, 0>;
+    const bool half = d.h - tc.y0 <= TH / 2;
+    if (p.ksteps == 4) half ? mmas(Rows8{}, KSteps4{}) : mmas(Rows16{}, KSteps4{});
+    else half ? mmas(Rows8{}, KStepsRuntime{}) : mmas(Rows16{}, KStepsRuntime{});
     __syncwarp();
-    if (lane == 0) mbar_arrive(bars.empty(cw, pend));
+    if (lane == 0) mbar_arrive(bars.empty(0, s));
 
     // the output tile is free once thread 0 saw the previous store read it (it issued the residual load after)
     if (has_res) { mbar_wait_mma(bar_res, rphase); rphase ^= 1u; }
@@ -488,8 +515,11 @@ __device__ __forceinline__ void consumer_convT_pxn(const TgMaps& maps, const KPa
 // POOL = TG_EPI_NHWC_F16_POOL2 instantiation: 2x2 max over the tile's pixels (tap mode: by warp shuffles,
 // one store per 2x2 block; halo mode: in registers, one TMA store of the pooled tile).
 template <int KIND, int MODE, bool BWD = false, bool POOL = false>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(conv_threads<KIND, MODE, BWD>(), 1)
 conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
+  constexpr int kThreads = conv_threads<KIND, MODE, BWD>();
+  constexpr int kConsumers = conv_consumers<KIND, MODE, BWD>();
+  constexpr bool kSharedRing = kConsumers == 3;   // one ring, filled in tile order (else one ring per consumer)
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;   // 128B swizzle atoms need 1024B alignment
@@ -516,17 +546,18 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
   }
   if (warp == 1 && lane == 0) {
     mbar_init(bar_b, 1);
-    for (int c = 0; c < 2; ++c) {
+    for (int c = 0; c < (kSharedRing ? 1 : 2); ++c)
       for (int k = 0; k < kMaxRing; ++k) {
         mbar_init(bars.full(c, k), 1);
-        mbar_init(bars.empty(c, k), 4);    // one arrival per consumer warp
+        mbar_init(bars.empty(c, k), 4);    // one arrival per warp of the consumer that read the stage
       }
+    for (int c = 0; c < kConsumers; ++c) {
       mbar_init(bars.res(c), 1);
       if (kSplitK) {
         mbar_init(bars.recv(c), 1);               // the owner's expect_tx; the bytes come from the peers
         mbar_init(bars.handback(c), p.chunks - 1);    // one hand-back per peer
       }
-      if (kSplitK || (kPxN && KIND == TG_CONV_3X3)) mbar_init(bars.turn(c), 4);   // one arrival per warp of the other consumer
+      if (kSplitK || kConsumers == 3) mbar_init(bars.turn(c), 4);   // one arrival per warp of the previous consumer
     }
     fence_barrier_init();
   }
@@ -573,7 +604,7 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
       uint32_t phase[2] = {0, 0};
       int it = 0;
       for (int tile = sched0; tile < p.num_tiles; tile += sched_step, ++it) {
-        const int cw = it & 1;
+        const int cw = kSharedRing ? 0 : it & 1;   // the ring the tile goes to
         const TileCoord tc = tile_coord(p, tile);
         const int n_loads = MODE == MODE_TAP ? 9 * p.chunks : kSplitK ? 1 : p.chunks;
         for (int l = 0; l < n_loads; ++l) {
@@ -795,6 +826,11 @@ cudaError_t set_smem_attr() {
                               (int)kSmemLimit);
 }
 
+template <int K, int M, bool B = false, bool P = false>
+cudaError_t launch_conv(dim3 grid, cudaStream_t st, const TgMaps& maps, const KParams& p) {
+  return tg_launch(conv_wgmma_kernel<K, M, B, P>, grid, dim3(conv_threads<K, M, B>()), kSmemLimit, st, maps, p);
+}
+
 // Clusters of `cluster` split-K CTAs (one per SM) that can be resident at once, per device; 0 if the query fails.
 template <bool P>
 int splitk_max_clusters(int cluster) {
@@ -805,7 +841,7 @@ int splitk_max_clusters(int cluster) {
   if (v == 0) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(cluster);
-    cfg.blockDim = dim3(kThreads);
+    cfg.blockDim = dim3(conv_threads<TG_CONV_3X3, MODE_SPLITK, false>());
     cfg.dynamicSmemBytes = kSmemLimit;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -947,18 +983,28 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
   // fp32 accumulator staging otherwise
   // Split-K: a receive buffer per consumer for the peers' partials of the couts this CTA owns ((C - 1) x 4/C
   // warps x 8 KB: 16 KB for C = 2, 24 KB for C = 4); the consumer's output slice tile overlaps it.
+  // The forward pixels-on-N conv3x3 has three consumers, one output tile each, and one ring shared in tile order: the
+  // ring must be at least consumers + 1 = 4 stages deep (consumer_halo_pxn), which the 72 KB weight slice of a cin = 64
+  // layer always leaves room for: 1024 + 2048 + 73,728 + 4 x 23,552 + 3 x 16,384 = 220,160 B.
   const bool pxn = p.halo && !bwd && !tapn && !splitk;
+  const bool three = pxn && !convT;
   p.epi_bytes = splitk ? (uint32_t)((p.chunks - 1) * (4 / p.chunks)) * 8192u : 0u;
-  const uint32_t epi_tiles = splitk ? 2u * p.epi_bytes
-                             : !pxn ? scratch : convT ? 4u * kTapABytes : pool ? 2u * kPoolTileBytes : 2u * kTapABytes;
+  const uint32_t epi_tiles = splitk  ? 2u * p.epi_bytes
+                             : !pxn  ? scratch
+                             : convT ? 4u * kTapABytes
+                                     : 3u * (pool ? kPoolTileBytes : kTapABytes);
   const uint32_t avail = kSmemLimit - 1024u - kHeaderBytes - epi_tiles - (p.b_resident ? b_total : 0u);
-  int ring = (int)(avail / p.stage_bytes) / 2;
+  const int rings = three ? 1 : 2;
+  int ring = (int)(avail / p.stage_bytes) / rings;
   if (ring > kMaxRing) ring = kMaxRing;
   TG_REQUIRE(ring >= 1, TG_E_UNSUPPORTED, "conv: shared memory budget (cin=%d cout=%d)", d->cin, d->cout);
+  TG_REQUIRE(!three || (ring >= 4 && p.chunks == 1), TG_E_UNSUPPORTED,
+             "conv: the three-consumer halo conv needs cin = 64 and 4 halo stages (cin=%d cout=%d: %d)", d->cin,
+             d->cout, ring);
   p.ring = ring;
   p.off_b = kHeaderBytes;
   p.off_stage = kHeaderBytes + (p.b_resident ? b_total : 0u);
-  p.off_scratch = p.off_stage + 2u * (uint32_t)ring * p.stage_bytes;   // consumer c's ring: stages [c*ring, (c+1)*ring)
+  p.off_scratch = p.off_stage + (uint32_t)(rings * ring) * p.stage_bytes;   // ring c: stages [c*ring, (c+1)*ring)
   const uint32_t smem_bytes = 1024u + p.off_scratch + epi_tiles;
   TG_REQUIRE(smem_bytes <= kSmemLimit, TG_E_UNSUPPORTED, "conv: smem %u > limit", smem_bytes);
 
@@ -1030,7 +1076,6 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
   rc = tg_device_sm_count(&sms);
   if (rc != TG_OK) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  const dim3 b(kThreads);
   cudaError_t lerr = cudaSuccess;
   if (splitk) {
     // clusters of C = cin/64 CTAs, as many as can be resident (max_ctas: at most that many CTAs); every
@@ -1042,7 +1087,7 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
     if (ncl > p.num_tiles) ncl = p.num_tiles;
     ncl -= ncl % p.n_split;
     if (ncl < p.n_split) ncl = p.n_split;
-    const dim3 g(ncl * C);
+    const dim3 g(ncl * C), b(conv_threads<TG_CONV_3X3, MODE_SPLITK, false>());
     lerr = pool ? tg_launch_cluster(conv_wgmma_kernel<TG_CONV_3X3, MODE_SPLITK, false, true>, g, b, kSmemLimit, st, C,
                                     map_a, p)
                 : tg_launch_cluster(conv_wgmma_kernel<TG_CONV_3X3, MODE_SPLITK, false, false>, g, b, kSmemLimit, st, C,
@@ -1057,23 +1102,23 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
   if (grid < p.n_split) grid = p.n_split;
   const dim3 g(grid);
   if (pool) {
-    lerr = p.halo ? tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_HALO, false, true>, g, b, kSmemLimit, st, map_a, p)
-                  : tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_TAP, false, true>, g, b, kSmemLimit, st, map_a, p);
+    lerr = p.halo ? launch_conv<TG_CONV_3X3, MODE_HALO, false, true>(g, st, map_a, p)
+                  : launch_conv<TG_CONV_3X3, MODE_TAP, false, true>(g, st, map_a, p);
   } else if (bwd) {
     if (d->kind == TG_CONV_3X3_S2)
-      lerr = tg_launch(conv_wgmma_kernel<TG_CONV_3X3_S2, MODE_TAP, true>, g, b, kSmemLimit, st, map_a, p);
+      lerr = launch_conv<TG_CONV_3X3_S2, MODE_TAP, true>(g, st, map_a, p);
     else if (p.halo)
-      lerr = tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_HALO, true>, g, b, kSmemLimit, st, map_a, p);
+      lerr = launch_conv<TG_CONV_3X3, MODE_HALO, true>(g, st, map_a, p);
     else
-      lerr = tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_TAP, true>, g, b, kSmemLimit, st, map_a, p);
+      lerr = launch_conv<TG_CONV_3X3, MODE_TAP, true>(g, st, map_a, p);
   } else if (tapn) {
-    lerr = tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_TAPN>, g, b, kSmemLimit, st, map_a, p);
+    lerr = launch_conv<TG_CONV_3X3, MODE_TAPN>(g, st, map_a, p);
   } else if (d->kind == TG_CONV_3X3) {
-    lerr = p.halo ? tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_HALO>, g, b, kSmemLimit, st, map_a, p)
-                  : tg_launch(conv_wgmma_kernel<TG_CONV_3X3, MODE_TAP>, g, b, kSmemLimit, st, map_a, p);
+    lerr = p.halo ? launch_conv<TG_CONV_3X3, MODE_HALO>(g, st, map_a, p)
+                  : launch_conv<TG_CONV_3X3, MODE_TAP>(g, st, map_a, p);
   } else {
-    lerr = p.halo ? tg_launch(conv_wgmma_kernel<TG_CONVT_3X3_S2, MODE_HALO>, g, b, kSmemLimit, st, map_a, p)
-                  : tg_launch(conv_wgmma_kernel<TG_CONVT_3X3_S2, MODE_TAP>, g, b, kSmemLimit, st, map_a, p);
+    lerr = p.halo ? launch_conv<TG_CONVT_3X3_S2, MODE_HALO>(g, st, map_a, p)
+                  : launch_conv<TG_CONVT_3X3_S2, MODE_TAP>(g, st, map_a, p);
   }
   TG_REQUIRE(lerr == cudaSuccess, (int)lerr, "conv: launch failed: %s", cudaGetErrorString(lerr));
   TG_CUDA_LAUNCH_CHECK("conv");

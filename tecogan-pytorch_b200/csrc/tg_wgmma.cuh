@@ -206,7 +206,10 @@ __device__ __forceinline__ void wgmma_wait() {
 // D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, fp16 in, fp32 accumulate, both operands K-major in smem.
 // Accumulator fragment of thread t of the warpgroup, register i (N/2 of them):
 //   row = 16*(t/32) + (t%32)/4 + 8*((i/2)%2),  col = 8*(i/4) + 2*(t%4) + i%2.
-__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+// The n64 fragment is therefore registers 0-31 of the n128 one; wgmma_n64 writes d[0..31] of a longer array.
+template <int L>
+__device__ __forceinline__ void wgmma_n64(float (&d)[L], uint64_t da, uint64_t db, uint32_t scale_d) {
+  static_assert(L >= 32, "m64n64 needs 32 accumulator registers");
   asm volatile(
       "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
@@ -294,8 +297,19 @@ __device__ __forceinline__ void convT_pxn_mmas(float (&acc)[64], uint32_t x16, u
 //                             pixels, SBO = one box row of 10 x 128 B, origin -1, start += ((dy+1)*10+dx+1)*128 B)
 // one m64n128k16 per (tap, k-step < ksteps), taps outer and k-steps inner: that order is the accumulation order,
 // hence the output bits.  The first MMA of chunk 0 overwrites acc (scale-d = 0).
+// N = 64 (a bottom tile row with at most 8 rows inside the image: rows 8-15 are clipped by the TMA store): each MMA is
+// an m64n64k16 over the first 8 core groups (tile rows 0-7), with the same descriptors.  Registers 0-31 of the n128
+// fragment are the n64 fragment, so rows 0-7 get the same products in the same order; acc[32..63] are not written and
+// keep what the caller left there.  A caller that picks N at run time must wait for the MMAs (wgmma_wait) inside each
+// branch: if the two paths join inside the wgmma pipeline stage, the register moves at the join make ptxas serialise
+// every wgmma of the kernel (C7515).
+// KS > 0 fixes the k-steps at compile time (ksteps_rt is then ignored).  With a run-time count each wgmma sits behind its
+// own `k < ksteps` branch, and ptxas fences every one of them (WARPGROUP.ARRIVE, info C7519).
+template <int N = 128, int KS = 0>
 __device__ __forceinline__ void halo_pxn_mmas(float (&acc)[64], uint32_t x16, uint32_t w16, uint32_t tile16, int chunks,
-                                              int c, int ksteps) {
+                                              int c, int ksteps_rt) {
+  static_assert(N == 128 || N == 64, "all 16 tile rows, or rows 0-7");
+  const int ksteps = KS > 0 ? KS : ksteps_rt;
   constexpr uint32_t kBoxW = TW + 2;
   const uint64_t w_hi = gmma_desc_hi(1024u), x_hi = gmma_desc_hi(kBoxW * 128u);
 #pragma unroll
@@ -305,9 +319,12 @@ __device__ __forceinline__ void halo_pxn_mmas(float (&acc)[64], uint32_t x16, ui
     const uint32_t b16 = x16 + (uint32_t)((gr.dy + 1) * (int)kBoxW + (gr.dx + 1)) * 8u;
 #pragma unroll
     for (int k = 0; k < 4; ++k)
-      if (k < ksteps)
-        wgmma_n128(acc, w_hi | (uint64_t)(a16 + 2u * k), x_hi | (uint64_t)(b16 + 2u * k),
-                   (g == 0 && c == 0 && k == 0) ? 0u : 1u);
+      if (k < ksteps) {
+        const uint64_t da = w_hi | (uint64_t)(a16 + 2u * k), db = x_hi | (uint64_t)(b16 + 2u * k);
+        const uint32_t sc = (g == 0 && c == 0 && k == 0) ? 0u : 1u;
+        if constexpr (N == 128) wgmma_n128(acc, da, db, sc);
+        else wgmma_n64(acc, da, db, sc);
+      }
   }
 }
 
