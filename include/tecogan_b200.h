@@ -34,6 +34,7 @@ extern "C" {
 #define TG_ABI_VERSION 2   /* 2: tg_conv_desc.mask, backward (training) entry points; tg_conv_desc.reserved became
                               cin_real (0 keeps the old meaning: all stored input channels are used) */
 #define TG_TAPN_ROWS 48   /* 9 taps x 4 output channels, padded to a multiple of 16 */
+#define TG_TAIL_OUT_ROWS 40   /* the fused tail's conv_out N: 5 x (2 taps x 4 output channels) */
 
 enum {
   TG_OK = 0,
@@ -150,7 +151,7 @@ typedef struct tg_tail_desc {
   const void* x;        /* input of the transposed conv, NHWC fp16 [n,h,w,64]                       */
   const void* w_up;     /* tg_pack_convT3x3s2_weights(cout_pad=64, cin_pad=64)                      */
   const float* b_up;    /* fp32 [64]                                                                */
-  const void* w_out;    /* tg_pack_conv3x3_weights_tapn(cin_pad=64)                                 */
+  const void* w_out;    /* tg_pack_tail_out_weights                                                 */
   const float* b_out;   /* fp32 [cout_real]                                                         */
   const float* lr;      /* lr_curr NCHW fp32 [n,cout_real,2h/lr_scale,2w/lr_scale] or NULL: the residual is
                            evaluated inside the kernel (16 gathers per pixel pair and channel)          */
@@ -166,6 +167,10 @@ typedef struct tg_tail_desc {
   int32_t reserved;     /* must be 0                                                                */
 } tg_tail_desc;
 int tg_convT_convout_tcgen05(const tg_tail_desc* d, void* stream);
+/* conv_out's weights (nn.Conv2d(cin <= 64, cout <= 3, 3, 1, 1).weight, fp32) as the tail reads them: one
+ * [TG_TAIL_OUT_ROWS rows][64 k] tile (TG_TAIL_OUT_ROWS * 128 bytes), tap t of output channel co in row
+ * 8*(t>>1) + 2*co + (t&1), so that one thread of the tail's conv_out holds all nine taps of one channel. */
+int tg_pack_tail_out_weights(const float* w_oihw, int cout, int cin, void* packed, void* stream);
 
 /* ------------------------------------------------------------------------
  * Fused  backward_warp + space_to_depth + concat  (HBM-bound).

@@ -6,9 +6,11 @@
 //   runs pixels-on-N (M = 64 couts, N = the 128 input pixels, one m64n128k16 per (tap group, k-step));
 //   its accumulators are written, +bias, ReLU, fp16, by stmatrix into one 128-pixel K-major 128B-swizzled
 //   operand block (pixels outside the image are zero = conv_out's zero padding); conv_out runs as
-//   "tap-major N" wgmmas (N = 48 = 9 taps x 4 couts) on that block; each thread adds the fp32 tap
-//   products that land on its 4 output pixels into registers.  The tile's 30x14 interior HR pixels are
-//   outputs (tiles advance by 15x7 input pixels, the transposed conv is recomputed on a one-pixel ring).
+//   m64n40 wgmmas on that block, N packed so that one thread holds all nine tap products of one cout
+//   for its pixels; the tap products are summed into the output pixels they land on in registers
+//   (x-neighbours by shuffle, y-neighbours in the thread's other row or, across warps, through a small
+//   edge buffer).  The tile's 30x14 interior HR pixels are outputs (tiles advance by 15x7 input pixels,
+//   the transposed conv is recomputed on a one-pixel ring).
 //   Warpgroup 0 runs the transposed conv with two accumulator sets, so parity a + 1's MMAs are in flight
 //   under parity a's epilogue; warpgroups 1 and 2 run conv_out, the summation and the global I/O of
 //   alternate tiles, each fed through its own two operand blocks.  The 64-channel HR map never reaches HBM.
@@ -23,29 +25,29 @@ constexpr uint32_t kWtBytes = 9 * 64 * 128;          // nine [64 cout][64 cin] f
 
 // warpgroup 0 (WG-T) runs the transposed conv and its epilogue; warpgroups 1 and 2 (WG-O 0 / 1) run conv_out and
 // the output of alternate tiles.  No producer warp: WG-T's thread 0 issues the halo TMAs.  WG-T holds two
-// 64-register accumulator sets, each WG-O the conv_out products and the 12 output sums.
+// 64-register accumulator sets, each WG-O the conv_out products and the 16 output sums.
 constexpr int kTailThreads = 384;
 constexpr int kStepY = 15, kStepX = 7;               // input pixels a tile advances by
 constexpr uint32_t kTailHalo = (TW + 1) * (TH + 1) * 128;            // 19584
 constexpr uint32_t kTailStage = (kTailHalo + 1023u) & ~1023u;        // 20480
 constexpr int kTailStages = 2;                       // halo ring: the tile in use + the next one loading
-constexpr uint32_t kWoBytes = TG_TAPN_ROWS * 128;                    // [48 rows = tap*4+co][64]
+constexpr uint32_t kWoBytes = TG_TAIL_OUT_ROWS * 128;                // [40 rows][64], see pack_tail_out_kernel
 constexpr uint32_t kHrBlock = 128 * 128;                             // one parity block: 128 px x 128 B
-constexpr int kD2Pitch = 27;                         // tap products kept per HR pixel: 9 taps x 3 couts (fp32)
-// the tap products of one parity block [128 px][27] fp32, + room for the shift-add's reads one block row and one
-// tap row past the end; its reads up to one block row before the start land in the weights placed before it
-constexpr uint32_t kD2Bytes = (((128 + 9) * kD2Pitch + 12) * 4 + 1023u) & ~1023u;   // 15360
-// layout: header | w_up | D2 of WG-O 0 | w_out | D2 of WG-O 1 | 2 halo stages | 2 operand blocks per WG-O (each D2
-// follows static weights, so the reads before its start never race with a write)
+// a WG-O's edge buffer: per parity (a & 1), per row pair w = 4 * m-block + warp (slots 1..8; slots 0 and 9 pad the
+// reads of the tile's first and last block rows, whose sums are never stored), per lane one tap row (3 of 4 floats)
+constexpr uint32_t kEdgeBytes = 2 * 10 * 32 * 16;                    // 10240
+// a WG-O's finished sums of one tile, [32 HR rows][16 HR columns][4] fp32 (3 couts + pad): they pass from the
+// threads that summed them (one cout, 16 pixels) to the threads that store them (one pixel, 3 couts)
+constexpr uint32_t kSumBytes = 32 * 16 * 16;                         // 8192
+// layout: header | w_up | w_out | edge buffers and sums of WG-O 0 and 1 | 2 halo stages | 2 operand blocks per WG-O
 constexpr uint32_t kTailOffWt = 2048;
-constexpr uint32_t kTailOffD2a = kTailOffWt + kWtBytes;              // 75776
-constexpr uint32_t kTailOffWo = kTailOffD2a + kD2Bytes;              // 91136
-constexpr uint32_t kTailOffD2b = kTailOffWo + kWoBytes;              // 97280
-constexpr uint32_t kTailOffHalo = kTailOffD2b + kD2Bytes;            // 112640
-constexpr uint32_t kTailOffBlk = kTailOffHalo + kTailStages * kTailStage;   // 153600
-constexpr uint32_t kTailSmem = 1024 + kTailOffBlk + 4 * kHrBlock;    // 220160
+constexpr uint32_t kTailOffWo = kTailOffWt + kWtBytes;               // 75776
+constexpr uint32_t kTailOffEdge = kTailOffWo + kWoBytes;             // 80896
+constexpr uint32_t kTailOffSum = kTailOffEdge + 2 * kEdgeBytes;      // 101376
+constexpr uint32_t kTailOffHalo = kTailOffSum + 2 * kSumBytes;       // 117760
+constexpr uint32_t kTailOffBlk = kTailOffHalo + kTailStages * kTailStage;   // 158720
+constexpr uint32_t kTailSmem = 1024 + kTailOffBlk + 4 * kHrBlock;    // 225280
 static_assert(kTailSmem <= kSmemLimit, "tail smem");
-static_assert(kWoBytes >= 9 * kD2Pitch * 4, "w_out must cover the reads before D2[1] (one block row + 1 pixel)");
 static_assert(kTailOffWo % 1024 == 0 && kTailOffHalo % 1024 == 0 && kTailOffBlk % 1024 == 0, "swizzle atoms");
 
 struct TailParams {
@@ -61,26 +63,62 @@ struct TailParams {
   int tiles_x, tiles_y, num_tiles;
 };
 
+// conv_out's weights as the tail reads them: one 128B-swizzled [40 rows][64 k] tile, tap t of cout co in row
+// 8 * (t >> 1) + 2 * co + (t & 1).  In an m64n40 accumulator fragment lane l holds columns 8j + 2 (l & 3) + e, so
+// lane quad position co holds all nine tap products of cout co (rows of co = 3 and of tap 9 are zero).
+__global__ void pack_tail_out_kernel(const float* __restrict__ w, __half* __restrict__ packed, int cout, int cin) {
+  tg_pdl_wait();
+  // no early trigger: the weights this kernel writes are loaded by the next tail BEFORE its PDL wait
+  for (int i = threadIdx.x; i < TG_TAIL_OUT_ROWS * 64; i += blockDim.x) {
+    const int k = i % 64, row = i / 64;
+    const int tap = 2 * (row >> 3) + (row & 1), co = (row >> 1) & 3;
+    float v = 0.f;
+    if (tap < 9 && co < cout && k < cin) v = w[(((size_t)co * cin + k) * 3 + tap / 3) * 3 + tap % 3];
+    *reinterpret_cast<__half*>(reinterpret_cast<unsigned char*>(packed) + tg_wtile_off(row, k)) = __float2half(v);
+  }
+}
+
+// fp16 pair of tg_act(v, TG_ACT_RELU) = fmaxf(v, v * 0).  For finite v that is v when v >= +0 and -0 when v < 0 or
+// v = -0; rounding to fp16 keeps the sign, so the pair is the rounded v with every half whose sign bit is set replaced
+// by -0 (0x8000): prmt replicates each half's sign bit over the half, lop3 selects.  Same bits, three integer
+// instructions per pair instead of two multiplies and two max.
+__device__ __forceinline__ uint32_t relu_f16x2(float v0, float v1) {
+  const __half2 hv = __floats2half2_rn(v0, v1);
+  const uint32_t h = *reinterpret_cast<const uint32_t*>(&hv);
+  uint32_t neg;
+  asm("prmt.b32 %0, %1, 0, 0xBB99;" : "=r"(neg) : "r"(h));
+  return (h & ~neg) | (neg & 0x80008000u);
+}
+
 // WG-T's epilogue of one parity: pxn_store_tile with ReLU, except that input pixels outside the image become zero
-// (conv_out's zero padding) -- a per-element predicate the conv kernels have no use for, so it is its own loop.
-__device__ __forceinline__ void tail_convT_epilogue(const float (&acc)[64], uint32_t blk, uint32_t mat_off, float b0,
-                                                    float b1, int y0, int x0, int lane, int h, int w) {
+// (conv_out's zero padding) -- a per-element predicate the conv kernels have no use for, so it is its own loop.  The
+// predicate is a mask per fp16 pair (the thread's two columns are fixed per tile, the row test is one compare); the
+// tiles whose 16x8 input pixels all lie in the image skip it.
+template <bool kEdge>
+__device__ __forceinline__ void tail_convT_store(const float (&acc)[64], uint32_t blk, uint32_t mat_off, float b0,
+                                                 float b1, int y0, int x0, int lane, int h, int w) {
+  const int ix = x0 + 2 * (lane & 3);
+  const uint32_t xmask = ((unsigned)ix < (unsigned)w ? 0x0000FFFFu : 0u) |
+                         ((unsigned)(ix + 1) < (unsigned)w ? 0xFFFF0000u : 0u);
 #pragma unroll
   for (int jp = 0; jp < 8; ++jp) {
     uint32_t ov[4];
 #pragma unroll
     for (int m = 0; m < 4; ++m) {
       const int i = 4 * (2 * jp + (m >> 1)) + 2 * (m & 1);
-      const int iy = y0 + 2 * jp + (m >> 1), ix = x0 + 2 * (lane & 3);
-      const bool rin = iy >= 0 && iy < h;
       const float bb = (m & 1) ? b1 : b0;
-      const float v0 = rin && ix >= 0 && ix < w ? tg_act(acc[i] + bb, TG_ACT_RELU) : 0.f;
-      const float v1 = rin && ix + 1 >= 0 && ix + 1 < w ? tg_act(acc[i + 1] + bb, TG_ACT_RELU) : 0.f;
-      const __half2 hv = __floats2half2_rn(v0, v1);
-      ov[m] = *reinterpret_cast<const uint32_t*>(&hv);
+      ov[m] = relu_f16x2(acc[i] + bb, acc[i + 1] + bb);
+      if (kEdge) ov[m] &= (unsigned)(y0 + 2 * jp + (m >> 1)) < (unsigned)h ? xmask : 0u;
     }
     stmatrix_x4_trans(blk + (uint32_t)jp * 2048u + mat_off, ov);
   }
+}
+__device__ __forceinline__ void tail_convT_epilogue(const float (&acc)[64], uint32_t blk, uint32_t mat_off, float b0,
+                                                    float b1, int y0, int x0, int lane, int h, int w) {
+  if (y0 >= 0 && y0 + 16 <= h && x0 >= 0 && x0 + 8 <= w)
+    tail_convT_store<false>(acc, blk, mat_off, b0, b1, y0, x0, lane, h, w);
+  else
+    tail_convT_store<true>(acc, blk, mat_off, b0, b1, y0, x0, lane, h, w);
 }
 
 __global__ void __launch_bounds__(kTailThreads, 1) convT_convout_kernel(const __grid_constant__ TailParams p) {
@@ -196,13 +234,20 @@ __global__ void __launch_bounds__(kTailThreads, 1) convT_convout_kernel(const __
       if (lane == 0) mbar_arrive(bar_full + 8 * b);
     }
   } else {
-    // ============================================================ WG-O c: conv_out, shift-add, output
+    // ============================================================ WG-O c: conv_out, register shift-add, output
     const int c = (warp >> 2) - 1;
     const uint32_t wo16 = gmma_addr16(base + kTailOffWo);
     const uint64_t k_hi = gmma_desc_hi(1024u);
-    float* D2 = reinterpret_cast<float*>(sm + (c ? kTailOffD2b : kTailOffD2a));
-    // this thread's HR pixels of the tile's 32x16: (Y0 + 8j, X), j = 0..3; the interior 30x14 are outputs
-    const int Y0 = r >> 4, X = r & 15;
+    // The thread's conv_out fragment: block pixels (row 8h + 2q + rb, column bx) for h, rb = 0, 1 (pixel row
+    // j = 2h + rb), all nine taps of cout cq (lane quad position 3 is padding).  The thread owns the HR outputs of
+    // those block pixels, (2 * row + ey, 2 * bx + ex) as o[j][e = 2ey + ex], of cout cq; the interior 30x14 of the
+    // tile's 32x16 are stored.
+    const int bx = lane >> 2, cq = lane & 3;
+    float4* edge = reinterpret_cast<float4*>(sm + kTailOffEdge + (uint32_t)c * kEdgeBytes);
+    float* sums = reinterpret_cast<float*>(sm + kTailOffSum + (uint32_t)c * kSumBytes);
+    // the pad slots feed only sums that are never stored; zero them once.  Every thread passes the first parity's
+    // named barrier after this store, before any read.
+    edge[(r >> 6) * 320 + ((r >> 5) & 1) * 288 + lane] = make_float4(0.f, 0.f, 0.f, 0.f);
     const int H = 2 * p.h, W = 2 * p.w;
     const int lh = H / p.lr_scale, lw = W / p.lr_scale;
     mbar_wait_mma(bar_w, 0);
@@ -210,69 +255,105 @@ __global__ void __launch_bounds__(kTailThreads, 1) convT_convout_kernel(const __
       const int img = tile / per_img, rr = tile - img * per_img;
       const int y0 = (rr / p.tiles_x) * kStepY - 1, x0 = (rr % p.tiles_x) * kStepX - 1;
       // the frame this tile adds onto is loaded into the output registers now; the loads complete under the MMAs
-      float o[4][3];
+      float o[4][4];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int Y = Y0 + 8 * j, gy = 2 * y0 + Y, gx = 2 * x0 + X;
-        const bool ok = Y >= 1 && Y <= 30 && X >= 1 && X <= 14 && gy >= 0 && gy < H && gx >= 0 && gx < W;
+      for (int j = 0; j < 4; ++j)
 #pragma unroll
-        for (int co = 0; co < 3; ++co) {
-          o[j][co] = 0.f;
-          if (p.accumulate && ok && co < p.cout_real)
-            o[j][co] = p.y[(((size_t)img * p.cout_real + co) * H + gy) * W + gx];
+        for (int e = 0; e < 4; ++e) {
+          const int Y = 2 * (8 * (j >> 1) + 2 * q + (j & 1)) + (e >> 1), X = 2 * bx + (e & 1);
+          const int gy = 2 * y0 + Y, gx = 2 * x0 + X;
+          const bool ok = Y >= 1 && Y <= 30 && X >= 1 && X <= 14 && gy >= 0 && gy < H && gx >= 0 && gx < W;
+          o[j][e] = 0.f;
+          if (p.accumulate && ok && cq < p.cout_real)
+            o[j][e] = p.y[(((size_t)img * p.cout_real + cq) * H + gy) * W + gx];
         }
-      }
       // parity a = (py, px) of the HR pixels: operand block -> conv_out tap products -> summed into the output
       // pixels they land on
-#pragma unroll 1
+#pragma unroll
       for (int a = 0; a < 4; ++a) {
+        const int py = a >> 1, px = a & 1;
         const uint32_t b = 2u * (uint32_t)c + ((uint32_t)a & 1u);
         const uint32_t blk16 = gmma_addr16(blk0 + b * kHrBlock);
-        mbar_wait_mma(bar_full + 8 * b, (uint32_t)(a >> 1) & 1u);
-        // conv_out as tap-major N (N = 48 = 9 taps x 4 couts) on the block
-        float d2[2][24];
+        mbar_wait_mma(bar_full + 8 * b, (uint32_t)py);
+        float d2[2][20];
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          wgmma_n48(d2[0], k_hi | (uint64_t)(blk16 + 2u * k), k_hi | (uint64_t)(wo16 + 2u * k), k > 0 ? 1u : 0u);
-          wgmma_n48(d2[1], k_hi | (uint64_t)(blk16 + 512u + 2u * k), k_hi | (uint64_t)(wo16 + 2u * k), k > 0 ? 1u : 0u);
+          wgmma_n40(d2[0], k_hi | (uint64_t)(blk16 + 2u * k), k_hi | (uint64_t)(wo16 + 2u * k), k > 0 ? 1u : 0u);
+          wgmma_n40(d2[1], k_hi | (uint64_t)(blk16 + 512u + 2u * k), k_hi | (uint64_t)(wo16 + 2u * k), k > 0 ? 1u : 0u);
         }
         wgmma_commit();
         wgmma_wait<0>();
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_empty + 8 * b);   // WG-T may write the block's next use
-        named_bar_sync(2 + c, 128);                      // every thread has read the previous parity's D2
+        // tap t of pixel row j
+        auto P = [&](int j, int t) { return d2[j >> 1][4 * (t >> 1) + 2 * (j & 1) + (t & 1)]; };
+        // HR pixel (Y, X) takes tap (ty, tx) from HR pixel (Y + ty - 1, X + tx - 1), which is in this parity block
+        // for ty = 1 if Y % 2 == py, else for ty = 0 and 2 (the same in x).  One of those two taps comes from the
+        // neighbouring block pixel: tap column txn from column bx + 1 (lane + 4) for px = 0, bx - 1 (lane - 4) for
+        // px = 1; tap row tyn from block row + dy.
+        const int dy = py ? -1 : 1, tyn = py ? 0 : 2, txn = px ? 0 : 2;
+        float xs[4][3];   // tap (ty, txn) of the x-neighbour
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+          for (int ty = 0; ty < 3; ++ty)
+            xs[j][ty] = px ? __shfl_up_sync(0xFFFFFFFFu, P(j, 3 * ty), 4)
+                           : __shfl_down_sync(0xFFFFFFFFu, P(j, 3 * ty + 2), 4);
+        // tap row tyn of pixel row j as the pixel row above / below it takes it (column txn from the x-neighbour)
+        auto nrow = [&](int j, int tx) { return tx == txn ? xs[j][tyn] : P(j, 3 * tyn + tx); };
+        // pixel row 2h + py is the y-neighbour of a row of another warp (or of the other m-block): it goes through
+        // the edge buffer of this parity, slot 1 + 4h + q; double-buffering by a & 1 lets one barrier per parity
+        // order both the writes after the last reads of the previous use and the reads after the writes
+        float4* eb = edge + (a & 1) * 320 + (1 + q) * 32 + lane;
 #pragma unroll
         for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int i = 0; i < 24; ++i) {
-            const int row = h * 64 + q * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
-            const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);   // = tap * 4 + co
-            if (col < 36 && (col & 3) < 3) D2[row * kD2Pitch + (col >> 2) * 3 + (col & 3)] = d2[h][i];
-          }
+          eb[h * 128] = make_float4(nrow(2 * h + py, 0), nrow(2 * h + py, 1), nrow(2 * h + py, 2), 0.f);
         named_bar_sync(2 + c, 128);
-        // HR pixel (Y, X) takes tap (ty, tx) from HR pixel (Y + ty - 1, X + tx - 1); that pixel has parity a for
-        // ty = ty0, ty0 + 2 (< 3) and tx = tx0, tx0 + 2 (< 3).  Only those slots are loaded (predicated, in slot
-        // order); the padding around D2 keeps the reads for the ring pixels inside shared memory.
-        const int ty0 = 1 - ((a >> 1) ^ (Y0 & 1)), tx0 = 1 - ((a & 1) ^ (X & 1));
+        float ny[4][3];   // tap row tyn of pixel row j's y-neighbour
 #pragma unroll
-        for (int sl = 0; sl < 4; ++sl) {
-          const int ty = ty0 + 2 * (sl >> 1), tx = tx0 + 2 * (sl & 1);
-          if (ty > 2 || tx > 2) continue;
-          const float* d = D2 + (((Y0 + ty - 1) >> 1) * 8 + ((X + tx - 1) >> 1)) * kD2Pitch + (ty * 3 + tx) * 3;
+        for (int h = 0; h < 2; ++h) {
+          const float4 v = eb[h * 128 + dy * 32];
+          ny[2 * h + 1 - py][0] = v.x;
+          ny[2 * h + 1 - py][1] = v.y;
+          ny[2 * h + 1 - py][2] = v.z;
 #pragma unroll
-          for (int j = 0; j < 4; ++j)        // HR row Y0 + 8j = block row ((Y0 + ty - 1) >> 1) + 4j
-#pragma unroll
-            for (int co = 0; co < 3; ++co) o[j][co] += d[j * 32 * kD2Pitch + co];
+          for (int tx = 0; tx < 3; ++tx) ny[2 * h + py][tx] = nrow(2 * h + 1 - py, tx);
         }
+        // each output adds its taps of this parity in slot order (ty, then tx), as the nine taps of a pixel are
+        // split over the four parities
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int ey = e >> 1, ex = e & 1;
+#pragma unroll
+            for (int sl = 0; sl < 4; ++sl) {
+              const int ty = (ey == py ? 1 : 0) + 2 * (sl >> 1), tx = (ex == px ? 1 : 0) + 2 * (sl & 1);
+              if (ty > 2 || tx > 2) continue;
+              const bool ynb = ey != py && ty == tyn, xnb = ex != px && tx == txn;
+              o[j][e] += ynb ? ny[j][tx] : xnb ? xs[j][ty] : P(j, 3 * ty + tx);
+            }
+            // the sums are done before the next parity's MMAs are issued: sinking them past those would keep
+            // this parity's tap products live next to the next one's accumulators
+            asm volatile("" : "+f"(o[j][e]));
+          }
       }
-      // + bias (+ upsample_func(lr)) -> fp32 NCHW (+ uint8 NHWC).  One pixel per iteration (the selects keep o in
-      // registers): the in-kernel upsample is inlined three times rather than twelve.
+      // the sums pass to one thread per HR pixel (Y0 + 8j, X) with all couts, as values, for the output stage.  The
+      // next tile writes them only after its parity barriers, which every thread passes after its reads here.
+      const int Y0 = r >> 4, X = r & 15;
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          if (cq < 3) sums[((2 * (8 * (j >> 1) + 2 * q + (j & 1)) + (e >> 1)) * 16 + 2 * bx + (e & 1)) * 4 + cq] = o[j][e];
+      named_bar_sync(2 + c, 128);
+      // + bias (+ upsample_func(lr)) -> fp32 NCHW (+ uint8 NHWC), one pixel per iteration: the in-kernel upsample is
+      // inlined three times rather than twelve.
 #pragma unroll 1
       for (int j = 0; j < 4; ++j) {
-        float oj[3];
-#pragma unroll
-        for (int co = 0; co < 3; ++co) oj[co] = j == 0 ? o[0][co] : j == 1 ? o[1][co] : j == 2 ? o[2][co] : o[3][co];
+        const float4 s = reinterpret_cast<const float4*>(sums)[(Y0 + 8 * j) * 16 + X];
+        const float oj[3] = {s.x, s.y, s.z};
         const int Y = Y0 + 8 * j, gy = 2 * y0 + Y, gx = 2 * x0 + X;
         if (Y < 1 || Y > 30 || X < 1 || X > 14 || gy < 0 || gy >= H || gx < 0 || gx >= W) continue;
         uint32_t q8[3] = {0u, 0u, 0u};
@@ -299,6 +380,15 @@ __global__ void __launch_bounds__(kTailThreads, 1) convT_convout_kernel(const __
 }  // namespace
 
 extern "C" {
+
+int tg_pack_tail_out_weights(const float* w_oihw, int cout, int cin, void* packed, void* stream) {
+  TG_REQUIRE(w_oihw && packed, TG_E_INVALID, "pack_tail_out: null pointer");
+  TG_REQUIRE(cout >= 1 && cout <= 3 && cin >= 1 && cin <= 64, TG_E_UNSUPPORTED,
+             "pack_tail_out: cout=%d (1..3) cin=%d (<= 64)", cout, cin);
+  tg_launch(pack_tail_out_kernel, dim3(1), dim3(256), 0, (cudaStream_t)stream, w_oihw, (__half*)packed, cout, cin);
+  TG_CUDA_LAUNCH_CHECK("pack_tail_out");
+  return TG_OK;
+}
 
 int tg_convT_convout_tcgen05(const tg_tail_desc* d, void* stream) {
   TG_REQUIRE(d != nullptr, TG_E_INVALID, "convT_convout: null descriptor");

@@ -22,6 +22,7 @@ YUV_NV12, YUV_I420, YUV_P010, YUV_I420_10 = 0, 1, 2, 3
 YUV_YUY2, YUV_UYVY, YUV_I444, YUV_I444_10 = 4, 5, 6, 8      # 7 is not a layout
 RESAMPLE_BICUBIC, RESAMPLE_LANCZOS3 = 0, 1
 SCENE_CUT_WORK_BYTES = 16            # TG_SCENE_CUT_WORK_BYTES: workspace of tg_scene_cut per slot
+TAIL_OUT_ROWS = 40                   # TG_TAIL_OUT_ROWS: rows of tg_pack_tail_out_weights' tile (128 bytes each)
 PSNR_NONE, PSNR_RGB, PSNR_Y = 0, 1, 2
 
 
@@ -83,6 +84,7 @@ _SIGNATURES = {
     'tg_conv_tcgen05': (c_int, [ctypes.POINTER(ConvDesc), _P]),
     'tg_conv_simt': (c_int, [ctypes.POINTER(ConvDesc), _P]),
     'tg_convT_convout_tcgen05': (c_int, [ctypes.POINTER(TailDesc), _P]),
+    'tg_pack_tail_out_weights': (c_int, [_P, c_int, c_int, _P, _P]),
     'tg_warp_s2d_concat_hrflow': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_warp_s2d_concat_lrflow': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int,
                                           c_int, c_int, c_int, _P]),

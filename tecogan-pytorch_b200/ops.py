@@ -65,6 +65,7 @@ class PackedConv:
         self.tapn = epilogue != L.EPI_NHWC_F16      # thin NCHW heads: tap-major N packing
         self.cout = pad64(self.cout_real) if not self.tapn else 48
         self.packed = None
+        self.tail_packed = None
         self.bias = None
         self._ver = None
         self.refresh(weight, bias)
@@ -94,6 +95,12 @@ class PackedConv:
             rc = lib.tg_pack_convT3x3s2_weights(_ptr(w), self.cin_real, self.cout_real,
                                                 _ptr(self.packed), self.cout, self.cin, _stream())
         L.check(rc, 'tg_pack_weights')
+        if self.epilogue == L.EPI_OUT_NCHW_F32 and self.cin == 64 and self.cout_real <= 3:
+            # conv_out: the fused SRNet tail (fused_tail) reads its own N packing of the same weights
+            if self.tail_packed is None:
+                self.tail_packed = torch.empty(L.TAIL_OUT_ROWS * 128, dtype=torch.uint8, device=w.device)
+            L.check(lib.tg_pack_tail_out_weights(_ptr(w), self.cout_real, self.cin_real, _ptr(self.tail_packed),
+                                                 _stream()), 'tg_pack_tail_out_weights')
         self.bias[:self.cout_real].copy_(bias.detach())
         self._ver = ver
 
@@ -149,11 +156,10 @@ class PackedConv:
 def fused_tail(up, outc, x, lr_curr, lr_scale, up_mode, y=None, y_u8=None, max_ctas=0, accumulate=False):
     """SRNet tail in one launch (tg_convT_convout_tcgen05): y = conv_out(relu(convT(x))) + upsample_func(lr_curr)
     [, y_u8 = float32_to_uint8(y) as NHWC].  `up` / `outc` are the PackedConv objects of the last transposed
-    conv and of conv_out (their packed weights are used as they are)."""
+    conv and of conv_out (the transposed conv's packed weights and conv_out's tail packing are used as they are)."""
     _req(x, torch.float16, 'tail input', 4)
     n, h, w, c = x.shape
-    if (up.kind != L.CONVT_3X3_S2 or up.cin != 64 or up.cout != 64 or c != 64 or not outc.tapn or outc.cin != 64
-            or outc.cout_real > 3):
+    if (up.kind != L.CONVT_3X3_S2 or up.cin != 64 or up.cout != 64 or c != 64 or outc.tail_packed is None):
         raise L.TecoganB200Error('fused tail: needs a 64->64 transposed conv and a 64->(<=3) conv_out')
     co = outc.cout_real
     if y is None:
@@ -163,7 +169,7 @@ def fused_tail(up, outc, x, lr_curr, lr_scale, up_mode, y=None, y_u8=None, max_c
         raise L.TecoganB200Error(f'fused tail: output shape {tuple(y.shape)}')
     d = L.TailDesc()
     d.x, d.w_up, d.b_up = x.data_ptr(), up.packed.data_ptr(), up.bias.data_ptr()
-    d.w_out, d.b_out, d.y = outc.packed.data_ptr(), outc.bias.data_ptr(), y.data_ptr()
+    d.w_out, d.b_out, d.y = outc.tail_packed.data_ptr(), outc.bias.data_ptr(), y.data_ptr()
     if lr_curr is not None:
         _req(lr_curr, torch.float32, 'lr_curr', 4)
         if tuple(lr_curr.shape) != (n, co, 2 * h // lr_scale, 2 * w // lr_scale):
