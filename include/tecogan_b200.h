@@ -219,6 +219,11 @@ int tg_nhwc_f16_to_nchw_f32(const void* x, float* y, int n, int c, int h, int w,
 /* float32_to_uint8 (data_utils.py:80-87) + CHW->HWC (tecogan_nets.py:281):
  * x NCHW fp32 [n,c,h,w] -> uint8 [n,h,w,c], round-half-even, clip [0,255] */
 int tg_float_to_uint8_nhwc(const float* x, uint8_t* y, int n, int c, int h, int w, void* stream);
+/* The same, written as the h x w picture at `win` of each uint8 HWC frame y [n, frame_h, frame_w, c]
+ * (struct tg_frame_window, declared with the stream's frame I/O below); nothing outside the picture is written. */
+struct tg_frame_window;
+int tg_float_to_uint8_nhwc_window(const float* x, uint8_t* y, const struct tg_frame_window* win, int n, int c, int h,
+                                  int w, void* stream);
 
 /* Frame input of one streamed step (codes/data/paired_folder_dataset.py:49, tecogan_nets.py:269-276).
  * in_u8 : uint8 [n,h,w,c] HWC frames, or NULL (lr_curr was filled by the caller)
@@ -289,6 +294,44 @@ int tg_rgb_to_yuv(const uint8_t* rgb_u8, const float* rgb_f32, void* out, const 
  * cBU cRV cGV cBV, decode CY CUB CUG CVG CVR, then the fraction bits and the luma offset. */
 int tg_yuv_coefficients(const tg_yuv_format* fmt, int32_t* out16);
 
+/* A picture inside a stored frame: the frames in memory are frame_h x frame_w pixels in their layout (a uint8 HWC
+ * frame [frame_h, frame_w, c], or that layout's YUV words of a frame_h x frame_w frame), and the picture is the
+ * h x w pixels at row `top`, column `left`.  The plain entry points are the window {h, w, 0, 0}.  Used on the input
+ * side (crop a letterboxed picture out of its frame; read a decoder surface of pitch P words and R rows as a frame
+ * of R x P) and on the output side (put the picture into a larger, black-padded delivery frame).  Only the picture
+ * is read or written.
+ * TG_E_INVALID: a NULL window, a frame of non-positive size, a picture outside the frame;
+ * TG_E_UNSUPPORTED: a window off the layout's chroma grid (4:2:0: frame_h, frame_w, top and left even; 4:2:2:
+ * frame_w and left even). */
+typedef struct tg_frame_window {
+  int32_t frame_h, frame_w;   /* the stored frame, in pixels */
+  int32_t top, left;          /* the picture's first row and column in it */
+} tg_frame_window;
+/* tg_stream_frame_in / tg_stream_frame_in_yuv reading the h x w picture at `win` of each stored frame (in_u8 / in
+ * point at the first frame; frames follow each other at the frame's size).  lr_curr, lr_prev, hr_prev, reset and the
+ * other arguments are those of the picture, as in the plain entry points. */
+int tg_stream_frame_in_window(const uint8_t* in_u8, const tg_frame_window* win, const int32_t* reset, float* lr_curr,
+                              float* lr_prev, float* hr_prev, int n, int c, int h, int w, int s, int bgr,
+                              void* stream);
+int tg_stream_frame_in_yuv_window(const void* in, const tg_yuv_format* fmt, const tg_frame_window* win,
+                                  const int32_t* reset, float* lr_curr, float* lr_prev, float* hr_prev, int n, int h,
+                                  int w, int s, void* stream);
+/* tg_rgb_to_yuv writing the encoded H x W picture at `win` of each output frame (out [n, frame words]).  The words
+ * outside the picture are not touched: fill them once with tg_fill_black. */
+int tg_rgb_to_yuv_window(const uint8_t* rgb_u8, const float* rgb_f32, void* out, const tg_yuv_format* fmt,
+                         const tg_frame_window* win, int n, int H, int W, void* stream);
+/* Every word of n frames of frame_h x frame_w set to the format's black: fmt NULL -> uint8 HWC [n,frame_h,frame_w,c]
+ * all 0; else the YUV layout's frames (c must be 3) with Y = the luma offset of the colour (16 << (depth - 8) for
+ * limited range, 0 for full) and U = V = 128 << (depth - 8), stored as the layout stores samples (P010: << 6).
+ * TG_E_INVALID: null pointers, non-positive sizes, misalignment; TG_E_UNSUPPORTED: sizes off the chroma grid. */
+int tg_fill_black(void* out, const tg_yuv_format* fmt, int n, int c, int frame_h, int frame_w, void* stream);
+/* Per-row and per-column sums of the 8-bit luma of n frames of h x w: Y for YUV frames (10-bit samples >> 2), and
+ * for uint8 HWC RGB frames (fmt NULL, c == 3; bgr != 0 for BGR order) the gray of tg_metrics_frames_in,
+ * (9798 R + 19235 G + 3735 B + 16384) >> 15.  rows uint64 [n,h], cols uint64 [n,w], zeroed by the call (memsets on
+ * the stream), 8-byte aligned.  Exact integers: the result does not depend on the grid.  detect_bars' input. */
+int tg_luma_line_sums(const void* in, const tg_yuv_format* fmt, int bgr, int n, int c, int h, int w,
+                      unsigned long long* rows, unsigned long long* cols, void* stream);
+
 /* Resize of the streamed output: Pillow's antialiased bicubic (a = -0.5, support 2) or Lanczos-3 (support 3)
  * filters, as Image.resize on 'F' images (oracle/resample.py restates them).  A downscale widens the filter by the
  * ratio.  Each axis needs in/4 <= out <= 2*in, so an axis has at most 17 (bicubic) or 25 (Lanczos) taps.
@@ -312,6 +355,12 @@ int tg_resample_table(int in, int out, int filter, int taps, int32_t* first, flo
 int tg_resample_nchw_f32(const float* x, int n, int c, int H, int W, const int32_t* row_first, const float* row_w,
                          int row_taps, const int32_t* col_first, const float* col_w, int col_taps, int Ho, int Wo,
                          uint8_t* y_u8, float* y_f32, void* stream);
+/* tg_resample_nchw_f32 with the uint8 output written as the Ho x Wo picture at `win` of each uint8 HWC frame
+ * y_u8 [n, frame_h, frame_w, c] (tg_frame_window above); nothing outside the picture is written. */
+int tg_resample_nchw_f32_window(const float* x, int n, int c, int H, int W, const int32_t* row_first,
+                                const float* row_w, int row_taps, const int32_t* col_first, const float* col_w,
+                                int col_taps, int Ho, int Wo, uint8_t* y_u8, const tg_frame_window* win,
+                                void* stream);
 
 /* Scene-cut detection of a streamed step (oracle/scene_cut.py is the specification).  Per slot k, with a = lr_curr[k]
  * and b = lr_prev[k] (fp32 [c,h,w], as the step sees them: decoded, and zeroed by a reset of this step):

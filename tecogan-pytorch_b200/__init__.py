@@ -10,6 +10,7 @@ from .data_utils import create_kernel, downsample_bd  # noqa: F401
 from .factory import define_generator  # noqa: F401
 from . import engine  # noqa: F401
 from .engine import infer_clips, ClipEngine, release_engines, StreamEngine, VideoStream  # noqa: F401
+from .engine import fit_size, detect_bars  # noqa: F401
 from .sharding import clips_for_rank  # noqa: F401
 from .autograd import st_discriminator_input  # noqa: F401
 from . import reducer  # noqa: F401

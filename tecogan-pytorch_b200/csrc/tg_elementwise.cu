@@ -455,8 +455,14 @@ upsample_nchw_kernel(const float* __restrict__ x, float* __restrict__ y, int hin
 __device__ __forceinline__ uint32_t tg_q8(float v) {
   return (uint32_t)fminf(fmaxf(rintf(v * 255.f), 0.f), 255.f);
 }
-__global__ void to_uint8_kernel(const float* __restrict__ x, uint8_t* __restrict__ y, int n, int c,
-                                int h, int w) {
+// pixel sp (< h*w, row-major) of image nn of an h x w picture -> its pixel in y's frames (tg_frame_window); the
+// whole-frame window {h, w, 0, 0} maps it to nn * h * w + sp
+__device__ __forceinline__ size_t tg_win_px(const tg_frame_window& win, int w, int nn, unsigned sp) {
+  const unsigned yy = sp / (unsigned)w, xx = sp - yy * (unsigned)w;
+  return ((size_t)nn * win.frame_h + win.top + yy) * win.frame_w + win.left + xx;
+}
+__global__ void to_uint8_kernel(const float* __restrict__ x, uint8_t* __restrict__ y, tg_frame_window win, int n,
+                                int c, int h, int w) {
   tg_pdl_wait();
   tg_pdl_trigger();
   const size_t hw = (size_t)h * w;
@@ -465,12 +471,14 @@ __global__ void to_uint8_kernel(const float* __restrict__ x, uint8_t* __restrict
        i += (size_t)gridDim.x * blockDim.x) {
     const int nn = (int)(i / hw);
     const size_t sp = i % hw;
-    for (int k = 0; k < c; ++k) y[i * c + k] = (uint8_t)tg_q8(__ldg(x + ((size_t)nn * c + k) * hw + sp));
+    uint8_t* o = y + tg_win_px(win, w, nn, (unsigned)sp) * c;
+    for (int k = 0; k < c; ++k) o[k] = (uint8_t)tg_q8(__ldg(x + ((size_t)nn * c + k) * hw + sp));
   }
 }
-// c == 3, hw % 4 == 0: one thread = 4 pixels = three float4 loads -> 12 bytes = three u32 stores
-__global__ void to_uint8_c3x4_kernel(const float4* __restrict__ x, uint32_t* __restrict__ y, int n,
-                                     size_t hw4) {
+// c == 3, hw % 4 == 0: one thread = 4 pixels = three float4 loads -> 12 bytes = three u32 stores.  A window other
+// than the whole frame needs w, frame_w and left to be multiples of 4 (four pixels of one row, 4-byte aligned).
+__global__ void to_uint8_c3x4_kernel(const float4* __restrict__ x, uint32_t* __restrict__ y, tg_frame_window win,
+                                     int n, int w, size_t hw4) {
   tg_pdl_wait();
   tg_pdl_trigger();
   const size_t total = (size_t)n * hw4;
@@ -484,7 +492,7 @@ __global__ void to_uint8_c3x4_kernel(const float4* __restrict__ x, uint32_t* __r
     const uint32_t w0 = tg_q8(r.x) | (tg_q8(g.x) << 8) | (tg_q8(b.x) << 16) | (tg_q8(r.y) << 24);
     const uint32_t w1 = tg_q8(g.y) | (tg_q8(b.y) << 8) | (tg_q8(r.z) << 16) | (tg_q8(g.z) << 24);
     const uint32_t w2 = tg_q8(b.z) | (tg_q8(r.w) << 8) | (tg_q8(g.w) << 16) | (tg_q8(b.w) << 24);
-    uint32_t* o = y + i * 3;
+    uint32_t* o = y + tg_win_px(win, w, (int)nn, (unsigned)(sp * 4)) / 4 * 3;
     o[0] = w0; o[1] = w1; o[2] = w2;
   }
 }
@@ -732,16 +740,36 @@ int tg_upsample_nchw_f32(const float* x, float* y, int n, int c, int hin, int wi
   return TG_OK;
 }
 
-int tg_float_to_uint8_nhwc(const float* x, uint8_t* y, int n, int c, int h, int w, void* stream) {
-  TG_REQUIRE(x && y, TG_E_INVALID, "float_to_uint8: null pointer");
-  TG_REQUIRE(n > 0 && c > 0 && h > 0 && w > 0, TG_E_INVALID, "float_to_uint8: bad shape");
+static int float_to_uint8(const char* name, const float* x, uint8_t* y, const tg_frame_window* win, int n, int c,
+                          int h, int w, void* stream) {
+  TG_REQUIRE(x && y, TG_E_INVALID, "%s: null pointer", name);
+  TG_REQUIRE(n > 0 && c > 0 && h > 0 && w > 0, TG_E_INVALID, "%s: bad shape", name);
+  const tg_frame_window whole = {h, w, 0, 0};
+  const bool is_whole = !win;
+  if (is_whole) win = &whole;
+  TG_REQUIRE(win->frame_h > 0 && win->frame_w > 0 && win->top >= 0 && win->left >= 0 &&
+                 (long long)win->top + h <= win->frame_h && (long long)win->left + w <= win->frame_w,
+             TG_E_INVALID, "%s: a %dx%d picture at (%d, %d) does not fit a %dx%d frame", name, h, w, win->top,
+             win->left, win->frame_h, win->frame_w);
+  TG_REQUIRE((size_t)h * w <= 0xffffffffu, TG_E_UNSUPPORTED, "%s: picture too large", name);
   const size_t total = (size_t)n * h * w;
-  if (c == 3 && ((size_t)h * w) % 4 == 0 && ((uintptr_t)x & 15) == 0 && ((uintptr_t)y & 3) == 0)
-    tg_launch(to_uint8_c3x4_kernel, dim3(grid_for(total / 4, 256)), dim3(256), 0, (cudaStream_t)stream, (const float4*)x, (uint32_t*)y, n, (size_t)h * w / 4);
+  const bool rows4 = is_whole || (w % 4 == 0 && win->frame_w % 4 == 0 && win->left % 4 == 0);
+  if (c == 3 && ((size_t)h * w) % 4 == 0 && rows4 && ((uintptr_t)x & 15) == 0 && ((uintptr_t)y & 3) == 0)
+    tg_launch(to_uint8_c3x4_kernel, dim3(grid_for(total / 4, 256)), dim3(256), 0, (cudaStream_t)stream, (const float4*)x, (uint32_t*)y, *win, n, w, (size_t)h * w / 4);
   else
-    tg_launch(to_uint8_kernel, dim3(grid_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, x, y, n, c, h, w);
-  TG_CUDA_LAUNCH_CHECK("float_to_uint8");
+    tg_launch(to_uint8_kernel, dim3(grid_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, x, y, *win, n, c, h, w);
+  TG_CUDA_LAUNCH_CHECK(name);
   return TG_OK;
+}
+
+int tg_float_to_uint8_nhwc(const float* x, uint8_t* y, int n, int c, int h, int w, void* stream) {
+  return float_to_uint8("float_to_uint8", x, y, nullptr, n, c, h, w, stream);
+}
+
+int tg_float_to_uint8_nhwc_window(const float* x, uint8_t* y, const tg_frame_window* win, int n, int c, int h, int w,
+                                  void* stream) {
+  TG_REQUIRE(win, TG_E_INVALID, "float_to_uint8_window: null window");
+  return float_to_uint8("float_to_uint8_window", x, y, win, n, c, h, w, stream);
 }
 
 }  // extern "C"

@@ -1,7 +1,8 @@
 // Antialiased bicubic / Lanczos-3 resize of the streamed HR frame (fp32 NCHW) to the output size, written as uint8
 // NHWC (quantised like float32_to_uint8) or fp32 NCHW (the source of the 10-bit encodes), and the host-side builder
 // of its per-axis tables.  The filters are Pillow's (Image.resize on 'F' images); oracle/resample.py specifies them.
-// Contract: include/tecogan_b200.h (tg_resample_taps, tg_resample_table, tg_resample_nchw_f32).
+// The uint8 output can be a picture window of larger frames (tg_frame_window).
+// Contract: include/tecogan_b200.h (tg_resample_taps, tg_resample_table, tg_resample_nchw_f32[_window]).
 #include <math.h>
 
 #include "tg_common.cuh"
@@ -31,7 +32,7 @@ __global__ void __launch_bounds__(kThreads)
 resample_kernel(const float* __restrict__ x, int c, int H, int W, const int32_t* __restrict__ row_first,
                 const float* __restrict__ row_w, int row_taps, const int32_t* __restrict__ col_first,
                 const float* __restrict__ col_w, int col_taps, int Ho, int Wo, int tiles_x, int tiles_y, int cap,
-                uint8_t* __restrict__ y_u8, float* __restrict__ y_f32) {
+                uint8_t* __restrict__ y_u8, tg_frame_window win, float* __restrict__ y_f32) {
   __shared__ float s_rw[kTY * kMaxTaps];
   __shared__ float s_cw[kTX * kMaxTaps];
   __shared__ int s_rf[kTY], s_cf[kTX];
@@ -42,6 +43,10 @@ resample_kernel(const float* __restrict__ x, int c, int H, int W, const int32_t*
   const int ty = rest % tiles_y, img = rest / tiles_y;
   const int ox0 = tx * kTX, oy0 = ty * kTY;
   const int nx = min(kTX, Wo - ox0), ny = min(kTY, Ho - oy0);
+  // uint8 output: pixel (y, x) of the picture is pixel (top + y, left + x) of its frame
+  const auto out_px = [&](int im, int y, int x) {
+    return ((size_t)im * win.frame_h + win.top + y) * win.frame_w + win.left + x;
+  };
   // the tables stay the same for the whole stream: staged before waiting on the previous kernel
   for (int i = t; i < ny * row_taps; i += kThreads) s_rw[i] = __ldg(row_w + (size_t)oy0 * row_taps + i);
   for (int i = t; i < nx * col_taps; i += kThreads) s_cw[i] = __ldg(col_w + (size_t)ox0 * col_taps + i);
@@ -95,7 +100,7 @@ resample_kernel(const float* __restrict__ x, int c, int H, int W, const int32_t*
       float acc = 0.f;
       for (int q = 0; q < col_taps; ++q) acc = fmaf(w[q], mid[min(max(off + q, 0), span - 1)], acc);
       if constexpr (kU8) {
-        const int lead = (int)((uintptr_t)(y_u8 + (((size_t)img * Ho + oy0 + r) * Wo + ox0) * c) & 15u);
+        const int lead = (int)((uintptr_t)(y_u8 + out_px(img, oy0 + r, ox0) * c) & 15u);
         s_out[r][lead + xo * c + k] = (uint8_t)fminf(fmaxf(rintf(acc * 255.f), 0.f), 255.f);
       } else {
         y_f32[(((size_t)img * c + k) * Ho + oy0 + r) * Wo + ox0 + xo] = acc;
@@ -109,7 +114,7 @@ resample_kernel(const float* __restrict__ x, int c, int H, int W, const int32_t*
     const int warp = t >> 5, lane = t & 31;
     const int bytes = nx * c;
     for (int r = warp; r < ny; r += kThreads / 32) {
-      uint8_t* dst = y_u8 + (((size_t)img * Ho + oy0 + r) * Wo + ox0) * c;
+      uint8_t* dst = y_u8 + out_px(img, oy0 + r, ox0) * c;
       const int lead = (int)((uintptr_t)dst & 15u);
       const int a0 = min(lead ? 16 - lead : 0, bytes);
       const int nv = (bytes - a0) / 16;
@@ -205,10 +210,11 @@ extern "C" int tg_resample_table(int in, int out, int filter, int taps, int32_t*
   return TG_OK;
 }
 
-extern "C" int tg_resample_nchw_f32(const float* x, int n, int c, int H, int W, const int32_t* row_first,
-                                    const float* row_w, int row_taps, const int32_t* col_first, const float* col_w,
-                                    int col_taps, int Ho, int Wo, uint8_t* y_u8, float* y_f32, void* stream) {
-  const char* name = "resample_nchw_f32";
+namespace {
+
+int resample(const char* name, const float* x, int n, int c, int H, int W, const int32_t* row_first,
+             const float* row_w, int row_taps, const int32_t* col_first, const float* col_w, int col_taps, int Ho,
+             int Wo, uint8_t* y_u8, const tg_frame_window* win, float* y_f32, void* stream) {
   TG_REQUIRE(x && row_first && row_w && col_first && col_w, TG_E_INVALID,
              "%s: null pointer (x / row_first / row_w / col_first / col_w)", name);
   TG_REQUIRE((y_u8 != nullptr) != (y_f32 != nullptr), TG_E_INVALID, "%s: exactly one of y_u8 / y_f32 is written",
@@ -224,6 +230,12 @@ extern "C" int tg_resample_nchw_f32(const float* x, int n, int c, int H, int W, 
              "%s: %dx%d -> %dx%d is outside the supported ratios (in/4 <= out <= 2*in per axis)", name, H, W, Ho, Wo);
   TG_REQUIRE(row_taps <= kMaxTaps && col_taps <= kMaxTaps, TG_E_UNSUPPORTED, "%s: taps %d / %d (at most %d)", name,
              row_taps, col_taps, kMaxTaps);
+  const tg_frame_window whole = {Ho, Wo, 0, 0};
+  if (!win) win = &whole;
+  TG_REQUIRE(win->frame_h > 0 && win->frame_w > 0 && win->top >= 0 && win->left >= 0 &&
+                 (long long)win->top + Ho <= win->frame_h && (long long)win->left + Wo <= win->frame_w,
+             TG_E_INVALID, "%s: a %dx%d picture at (%d, %d) does not fit a %dx%d frame", name, Ho, Wo, win->top,
+             win->left, win->frame_h, win->frame_w);
   const int tiles_x = tg_ceil_div(Wo, kTX), tiles_y = tg_ceil_div(Ho, kTY);
   const size_t ctas = (size_t)tiles_x * tiles_y * n;
   TG_REQUIRE(ctas <= 0x7fffffff, TG_E_UNSUPPORTED, "%s: grid too large", name);
@@ -237,7 +249,7 @@ extern "C" int tg_resample_nchw_f32(const float* x, int n, int c, int H, int W, 
     });
     TG_REQUIRE(e == cudaSuccess, (int)e, "%s: cudaFuncSetAttribute: %s", name, cudaGetErrorString(e));
     tg_launch(resample_kernel<true>, dim3((unsigned)ctas), dim3(kThreads), smem, st, x, c, H, W, row_first, row_w,
-              row_taps, col_first, col_w, col_taps, Ho, Wo, tiles_x, tiles_y, cap, y_u8, (float*)nullptr);
+              row_taps, col_first, col_w, col_taps, Ho, Wo, tiles_x, tiles_y, cap, y_u8, *win, (float*)nullptr);
   } else {
     static TgPerDeviceOnce attr_once;
     const cudaError_t e = attr_once.run([] {
@@ -245,8 +257,27 @@ extern "C" int tg_resample_nchw_f32(const float* x, int n, int c, int H, int W, 
     });
     TG_REQUIRE(e == cudaSuccess, (int)e, "%s: cudaFuncSetAttribute: %s", name, cudaGetErrorString(e));
     tg_launch(resample_kernel<false>, dim3((unsigned)ctas), dim3(kThreads), smem, st, x, c, H, W, row_first, row_w,
-              row_taps, col_first, col_w, col_taps, Ho, Wo, tiles_x, tiles_y, cap, (uint8_t*)nullptr, y_f32);
+              row_taps, col_first, col_w, col_taps, Ho, Wo, tiles_x, tiles_y, cap, (uint8_t*)nullptr, *win, y_f32);
   }
   TG_CUDA_LAUNCH_CHECK(name);
   return TG_OK;
+}
+
+}  // namespace
+
+extern "C" int tg_resample_nchw_f32(const float* x, int n, int c, int H, int W, const int32_t* row_first,
+                                    const float* row_w, int row_taps, const int32_t* col_first, const float* col_w,
+                                    int col_taps, int Ho, int Wo, uint8_t* y_u8, float* y_f32, void* stream) {
+  return resample("resample_nchw_f32", x, n, c, H, W, row_first, row_w, row_taps, col_first, col_w, col_taps, Ho, Wo,
+                  y_u8, nullptr, y_f32, stream);
+}
+
+extern "C" int tg_resample_nchw_f32_window(const float* x, int n, int c, int H, int W, const int32_t* row_first,
+                                           const float* row_w, int row_taps, const int32_t* col_first,
+                                           const float* col_w, int col_taps, int Ho, int Wo, uint8_t* y_u8,
+                                           const tg_frame_window* win, void* stream) {
+  TG_REQUIRE(win, TG_E_INVALID, "resample_nchw_f32_window: null window");
+  TG_REQUIRE(y_u8, TG_E_INVALID, "resample_nchw_f32_window: null pointer (y_u8)");
+  return resample("resample_nchw_f32_window", x, n, c, H, W, row_first, row_w, row_taps, col_first, col_w, col_taps,
+                  Ho, Wo, y_u8, win, nullptr, stream);
 }

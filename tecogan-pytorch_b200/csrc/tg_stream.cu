@@ -1,9 +1,11 @@
 // Frame I/O of one streamed inference step: uint8 HWC or YUV (4:2:0: NV12 / I420, 8 bit; P010 / I420_10, 10 bit;
 // packed 4:2:2: YUY2 / UYVY, 8 bit; planar 4:4:4: I444, 8 bit, I444_10) frames decoded on the device into the
 // step's fp32 NCHW lr_curr, the per-slot reset of the recurrent state, and the encode of the step's RGB output
-// (uint8 NHWC, or the fp32 NCHW HR frame for 10-bit output) into any of those YUV layouts.
-// Contract: include/tecogan_b200.h (tg_stream_frame_in, tg_stream_frame_in_yuv420, tg_rgb_u8_to_yuv420,
-// tg_stream_frame_in_yuv, tg_rgb_to_yuv, tg_yuv_coefficients).
+// (uint8 NHWC, or the fp32 NCHW HR frame for 10-bit output) into any of those YUV layouts; each of them reads or
+// writes a picture window of larger stored frames (tg_frame_window).  Also the fill of padded frames with a format's
+// black and the per-row / per-column luma sums of letterbox detection.
+// Contract: include/tecogan_b200.h (tg_stream_frame_in[_window], tg_stream_frame_in_yuv420, tg_rgb_u8_to_yuv420,
+// tg_stream_frame_in_yuv[_window], tg_rgb_to_yuv[_window], tg_yuv_coefficients, tg_fill_black, tg_luma_line_sums).
 #include <type_traits>
 
 #include "tg_common.cuh"
@@ -168,15 +170,19 @@ __device__ __forceinline__ void flush_bytes(uint8_t* __restrict__ dst, const uin
 
 __device__ __forceinline__ int lead_of(const void* p) { return (int)((uintptr_t)p & 15u); }
 
+// Every decode reads the h x w picture at (win.top, win.left) of frames of win.frame_h x win.frame_w pixels and
+// writes the h x w lr_curr; the encodes write their H x W picture there.  {h, w, 0, 0} is the whole frame.
+
 // decode CTA of HWC frames: kTilePx pixels of one image row
 __device__ __forceinline__ void decode_hwc(const uint8_t* __restrict__ in, float* __restrict__ lr_curr, int b, int t,
-                                           int c, int h, int w, int bgr, int x_tiles) {
+                                           int c, int h, int w, tg_frame_window win, int bgr, int x_tiles) {
   __shared__ __align__(16) uint8_t sb[kTilePx * kMaxC + 32];
   const int xt = b % x_tiles, r = b / x_tiles;
   const int y = r % h, img = r / h;
   const int x0 = xt * kTilePx;
   const int npx = min(kTilePx, w - x0);
-  const int lead = stage_bytes(sb, in + (((size_t)img * h + y) * w + x0) * c, npx * c, t);
+  const size_t src = ((size_t)img * win.frame_h + win.top + y) * win.frame_w + win.left + x0;
+  const int lead = stage_bytes(sb, in + src * c, npx * c, t);
   __syncthreads();
   if (t < npx) {
     float* dst = lr_curr + ((size_t)img * c * h + y) * w + x0 + t;
@@ -194,7 +200,7 @@ __device__ __forceinline__ void decode_hwc(const uint8_t* __restrict__ in, float
 // row `color` of the table; with the 8-bit bt601 row this is cv2 COLOR_YUV2RGB_NV12 / _I420 bit for bit.
 template <int kFmt>
 __device__ __forceinline__ void decode_yuv420(const uint8_t* __restrict__ in, float* __restrict__ lr_curr, int b,
-                                              int t, int h, int w, int x_tiles, int color) {
+                                              int t, int h, int w, tg_frame_window win, int x_tiles, int color) {
   using F = Yuv<kFmt>;
   using W = typename F::Word;
   constexpr int kB = (int)sizeof(W);
@@ -204,15 +210,17 @@ __device__ __forceinline__ void decode_yuv420(const uint8_t* __restrict__ in, fl
   const int hp = h >> 1, yp = r % hp, img = r / hp;
   const int x0 = xt * kTilePx;
   const int npx = min(kTilePx, w - x0);                      // even: w and x0 are
-  const W* frame = reinterpret_cast<const W*>(in) + (size_t)img * (3 * hp) * w;
-  const W* yrow = frame + (size_t)(2 * yp) * w + x0;
-  const W* crow = frame + (size_t)h * w;                     // chroma of the frame
+  const int fh = win.frame_h, fw = win.frame_w;              // even, as are top and left
+  const int fx = win.left + x0, fyp = (win.top >> 1) + yp;   // the tile's column and row pair in the frame
+  const W* frame = reinterpret_cast<const W*>(in) + (size_t)img * (3 * (fh >> 1)) * fw;
+  const W* yrow = frame + (size_t)(2 * fyp) * fw + fx;
+  const W* crow = frame + (size_t)fh * fw;                   // chroma of the frame
   const uint8_t* ysrc = reinterpret_cast<const uint8_t*>(yrow);
   const uint8_t* csrc = reinterpret_cast<const uint8_t*>(crow);
-  const uint8_t* c0 = csrc + (F::kInterleaved ? (size_t)yp * w + x0 : (size_t)yp * (w >> 1) + (x0 >> 1)) * kB;
-  const uint8_t* c1 = c0 + (size_t)hp * (w >> 1) * kB;        // I420 layout: the V sample of the same block
+  const uint8_t* c0 = csrc + (F::kInterleaved ? (size_t)fyp * fw + fx : (size_t)fyp * (fw >> 1) + (fx >> 1)) * kB;
+  const uint8_t* c1 = c0 + (size_t)(fh >> 1) * (fw >> 1) * kB;   // I420 layout: the V sample of the same block
   stage_bytes(sy[0], ysrc, npx * kB, t);
-  stage_bytes(sy[1], ysrc + (size_t)w * kB, npx * kB, t);
+  stage_bytes(sy[1], ysrc + (size_t)fw * kB, npx * kB, t);
   if (F::kInterleaved) {
     stage_bytes(sc[0], c0, npx * kB, t);
   } else {
@@ -222,7 +230,7 @@ __device__ __forceinline__ void decode_yuv420(const uint8_t* __restrict__ in, fl
   __syncthreads();
   if (t >= npx) return;
   // the staged words start at the sources' offsets within 16 bytes (cheaper to recompute than to keep live)
-  const int ly0 = lead_of(ysrc), ly1 = lead_of(ysrc + (size_t)w * kB), lc0 = lead_of(c0);
+  const int ly0 = lead_of(ysrc), ly1 = lead_of(ysrc + (size_t)fw * kB), lc0 = lead_of(c0);
   const int lc1 = F::kInterleaved ? 0 : lead_of(c1);
   // the leads are multiples of the word size: sources are word aligned
   const auto at = [](const uint8_t* sb, int lead, int j) { return F::sample(reinterpret_cast<const W*>(sb + lead)[j]); };
@@ -284,13 +292,15 @@ struct YuvDecode {
 // COLOR_YUV2RGB_YUY2 / _UYVY bit for bit.  The frames are 4-byte aligned (the launch checks).
 template <int kFmt>
 __device__ __forceinline__ void decode_yuv422(const uint8_t* __restrict__ in, float* __restrict__ lr_curr, int b,
-                                              int t, int h, int w, int x_tiles, int color) {
+                                              int t, int h, int w, tg_frame_window win, int x_tiles, int color) {
   using F = Yuv<kFmt>;
   const int xt = b % x_tiles, r = b / x_tiles;
   const int y = r % h, img = r / h;
   const int pair = xt * kTilePx + t;
   if (pair >= (w >> 1)) return;
-  const uint32_t g = __ldg(reinterpret_cast<const uint32_t*>(in) + ((size_t)img * h + y) * (w >> 1) + pair);
+  const size_t frow = (size_t)img * win.frame_h + win.top + y;   // frame_w and left are even
+  const uint32_t g =
+      __ldg(reinterpret_cast<const uint32_t*>(in) + frow * (win.frame_w >> 1) + (win.left >> 1) + pair);
   const auto byte = [g](int k) { return (int)((g >> (8 * k)) & 255u); };
   const YuvDecode<kFmt> d(byte(packed_u(kFmt)), byte(packed_u(kFmt) + 2), color);
   const size_t plane = (size_t)h * w;
@@ -303,16 +313,17 @@ __device__ __forceinline__ void decode_yuv422(const uint8_t* __restrict__ in, fl
 // sample of each plane per thread (coalesced word loads)
 template <int kFmt>
 __device__ __forceinline__ void decode_yuv444(const uint8_t* __restrict__ in, float* __restrict__ lr_curr, int b,
-                                              int t, int h, int w, int x_tiles, int color) {
+                                              int t, int h, int w, tg_frame_window win, int x_tiles, int color) {
   using F = Yuv<kFmt>;
   using W = typename F::Word;
   const int xt = b % x_tiles, r = b / x_tiles;
   const int y = r % h, img = r / h;
   const int x = xt * kTilePx + t;
   if (x >= w) return;
-  const size_t plane = (size_t)h * w;
-  const W* src = reinterpret_cast<const W*>(in) + (size_t)img * 3 * plane + (size_t)y * w + x;
-  const YuvDecode<kFmt> d(F::sample(__ldg(src + plane)), F::sample(__ldg(src + 2 * plane)), color);
+  const size_t plane = (size_t)h * w, fplane = (size_t)win.frame_h * win.frame_w;
+  const W* src = reinterpret_cast<const W*>(in) + (size_t)img * 3 * fplane + (size_t)(win.top + y) * win.frame_w +
+                 win.left + x;
+  const YuvDecode<kFmt> d(F::sample(__ldg(src + fplane)), F::sample(__ldg(src + 2 * fplane)), color);
   d.put(lr_curr + (size_t)img * 3 * plane + (size_t)y * w + x, plane, F::sample(__ldg(src)));
 }
 
@@ -323,7 +334,8 @@ template <int kFmt>
 __global__ void __launch_bounds__(kThreads)
 stream_frame_in_kernel(const uint8_t* __restrict__ in, const int32_t* __restrict__ reset,
                        float* __restrict__ lr_curr, float* __restrict__ lr_prev, float* __restrict__ hr_prev,
-                       int c, int h, int w, int s, int bgr, int x_tiles, int decode_ctas, int zpc, int color) {
+                       int c, int h, int w, tg_frame_window win, int s, int bgr, int x_tiles, int decode_ctas,
+                       int zpc, int color) {
   // lr_curr, lr_prev and hr_prev belong to the previous step until it has finished
   tg_pdl_wait();
   tg_pdl_trigger();
@@ -331,13 +343,13 @@ stream_frame_in_kernel(const uint8_t* __restrict__ in, const int32_t* __restrict
   const int b = blockIdx.x;
   if (b < decode_ctas) {
     if constexpr (kFmt == kHWC)
-      decode_hwc(in, lr_curr, b, t, c, h, w, bgr, x_tiles);
+      decode_hwc(in, lr_curr, b, t, c, h, w, win, bgr, x_tiles);
     else if constexpr (fmt_packed(kFmt))
-      decode_yuv422<kFmt>(in, lr_curr, b, t, h, w, x_tiles, color);
+      decode_yuv422<kFmt>(in, lr_curr, b, t, h, w, win, x_tiles, color);
     else if constexpr (fmt_444(kFmt))
-      decode_yuv444<kFmt>(in, lr_curr, b, t, h, w, x_tiles, color);
+      decode_yuv444<kFmt>(in, lr_curr, b, t, h, w, win, x_tiles, color);
     else
-      decode_yuv420<kFmt>(in, lr_curr, b, t, h, w, x_tiles, color);
+      decode_yuv420<kFmt>(in, lr_curr, b, t, h, w, win, x_tiles, color);
     return;
   }
   const int rb = b - decode_ctas;
@@ -349,9 +361,26 @@ stream_frame_in_kernel(const uint8_t* __restrict__ in, const int32_t* __restrict
   zero_range(hr_prev + slot * nhr, nhr, worker, workers);
 }
 
+// A window of an h x w picture in frames of layout kFmt: TG_E_INVALID outside the frame, TG_E_UNSUPPORTED off the
+// chroma grid (4:2:0: even frame size, top and left; 4:2:2: even frame width and left)
+template <int kFmt>
+int check_window(const char* name, const tg_frame_window* win, int h, int w) {
+  TG_REQUIRE(win, TG_E_INVALID, "%s: null window", name);
+  const long long fh = win->frame_h, fw = win->frame_w, top = win->top, left = win->left;
+  TG_REQUIRE(fh > 0 && fw > 0 && top >= 0 && left >= 0 && top + h <= fh && left + w <= fw, TG_E_INVALID,
+             "%s: a %dx%d picture at (%lld, %lld) does not fit a %lldx%lld frame", name, h, w, top, left, fh, fw);
+  TG_REQUIRE(!fmt_420(kFmt) || ((fh | fw | top | left) & 1) == 0, TG_E_UNSUPPORTED,
+             "%s: YUV 4:2:0 needs an even frame size, top and left, got %lldx%lld at (%lld, %lld)", name, fh, fw, top,
+             left);
+  TG_REQUIRE(!fmt_packed(kFmt) || ((fw | left) & 1) == 0, TG_E_UNSUPPORTED,
+             "%s: YUV 4:2:2 needs an even frame width and left, got width %lld at column %lld", name, fw, left);
+  return TG_OK;
+}
+
 template <int kFmt>
 int launch_frame_in(const char* name, const void* in, const int32_t* reset, float* lr_curr, float* lr_prev,
-                    float* hr_prev, int n, int c, int h, int w, int s, int bgr, int color, cudaStream_t stream) {
+                    float* hr_prev, int n, int c, int h, int w, const tg_frame_window* win, int s, int bgr, int color,
+                    cudaStream_t stream) {
   TG_REQUIRE(in || reset, TG_E_INVALID, "%s: in_u8 and reset are both NULL", name);
   TG_REQUIRE(lr_curr && lr_prev && hr_prev, TG_E_INVALID, "%s: null pointer (lr_curr / lr_prev / hr_prev)", name);
   TG_REQUIRE(n > 0 && c > 0 && h > 0 && w > 0, TG_E_INVALID, "%s: bad size n=%d c=%d h=%d w=%d", name, n, c, h, w);
@@ -368,6 +397,12 @@ int launch_frame_in(const char* name, const void* in, const int32_t* reset, floa
              "%s: 10-bit frames must be 2-byte aligned", name);
   TG_REQUIRE(!fmt_packed(kFmt) || ((uintptr_t)in & 3u) == 0, TG_E_INVALID,
              "%s: packed 4:2:2 frames must be 4-byte aligned", name);
+  const tg_frame_window whole = {h, w, 0, 0};
+  if (!win) win = &whole;
+  if (in) {
+    const int rc = check_window<kFmt>(name, win, h, w);
+    if (rc != TG_OK) return rc;
+  }
   const int x_tiles = tg_ceil_div(fmt_packed(kFmt) ? w / 2 : w, kTilePx);
   const size_t decode = in ? (size_t)x_tiles * (k420 ? h / 2 : h) * n : 0;
   const size_t hr4 = (size_t)c * s * h * s * w / 4;
@@ -375,8 +410,8 @@ int launch_frame_in(const char* name, const void* in, const int32_t* reset, floa
   const size_t ctas = decode + (size_t)zpc * n;
   TG_REQUIRE(ctas <= 0x7fffffff, TG_E_UNSUPPORTED, "%s: grid too large", name);
   tg_launch(stream_frame_in_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), 0, stream,
-            static_cast<const uint8_t*>(in), reset, lr_curr, lr_prev, hr_prev, c, h, w, s, bgr, x_tiles, (int)decode,
-            zpc, color);
+            static_cast<const uint8_t*>(in), reset, lr_curr, lr_prev, hr_prev, c, h, w, *win, s, bgr, x_tiles,
+            (int)decode, zpc, color);
   TG_CUDA_LAUNCH_CHECK(name);
   return TG_OK;
 }
@@ -387,8 +422,8 @@ int launch_frame_in(const char* name, const void* in, const int32_t* reset, floa
 // row reads of the three planes, q = clip(rint(x * 1023), 0, 1023)).  Colour row `color` of the table.
 template <int kFmt, bool kF32>
 __global__ void __launch_bounds__(kThreads)
-rgb_to_yuv420_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, int x_tiles,
-                     int color) {
+rgb_to_yuv420_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, tg_frame_window win,
+                     int x_tiles, int color) {
   using F = Yuv<kFmt>;
   using Wd = typename F::Word;
   static_assert(kF32 == F::k10, "8-bit output reads uint8 RGB, 10-bit output the fp32 frame");
@@ -410,17 +445,19 @@ rgb_to_yuv420_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, in
     li0 = stage_bytes(sin[0], src, npx * 3, t);
     li1 = stage_bytes(sin[1], src + (size_t)W * 3, npx * 3, t);
   }
-  Wd* frame = reinterpret_cast<Wd*>(out) + (size_t)img * (3 * hp) * W;
-  Wd* yrow = frame + (size_t)(2 * yp) * W + x0;
-  Wd* crow = frame + (size_t)H * W;
+  const int fh = win.frame_h, fw = win.frame_w;              // even, as are top and left
+  const int fx = win.left + x0, fyp = (win.top >> 1) + yp;   // the tile's column and row pair in the frame
+  Wd* frame = reinterpret_cast<Wd*>(out) + (size_t)img * (3 * (fh >> 1)) * fw;
+  Wd* yrow = frame + (size_t)(2 * fyp) * fw + fx;
+  Wd* crow = frame + (size_t)fh * fw;
   Wd *c0, *c1 = nullptr;
   if (F::kInterleaved) {
-    c0 = crow + (size_t)yp * W + x0;
+    c0 = crow + (size_t)fyp * fw + fx;
   } else {
-    c0 = crow + (size_t)yp * (W >> 1) + (x0 >> 1);
-    c1 = c0 + (size_t)hp * (W >> 1);
+    c0 = crow + (size_t)fyp * (fw >> 1) + (fx >> 1);
+    c1 = c0 + (size_t)(fh >> 1) * (fw >> 1);
   }
-  const int ly0 = lead_of(yrow), ly1 = lead_of(yrow + W), lc0 = lead_of(c0), lc1 = F::kInterleaved ? 0 : lead_of(c1);
+  const int ly0 = lead_of(yrow), ly1 = lead_of(yrow + fw), lc0 = lead_of(c0), lc1 = F::kInterleaved ? 0 : lead_of(c1);
   auto put = [](uint8_t* sb, int lead, int j, int v) { reinterpret_cast<Wd*>(sb + lead)[j] = F::word(v); };
   const int* k = c_yuv.v[F::k10][color];
   constexpr int kHalf = 1 << (F::kShift - 1);
@@ -462,7 +499,7 @@ rgb_to_yuv420_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, in
     flush_bytes(reinterpret_cast<uint8_t*>(dst), sb, words * kB, t);
   };
   flush(yrow, sy[0], npx);
-  flush(yrow + W, sy[1], npx);
+  flush(yrow + fw, sy[1], npx);
   if (F::kInterleaved) {
     flush(c0, sc[0], npx);
   } else {
@@ -475,8 +512,8 @@ rgb_to_yuv420_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, in
 // 4-byte YUY2 / UYVY group per pair: Y of each pixel, U and V of the pair's sum (c_yuv422 row `color`)
 template <int kFmt>
 __global__ void __launch_bounds__(kThreads)
-rgb_to_yuv422_kernel(const uint8_t* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, int x_tiles,
-                     int color) {
+rgb_to_yuv422_kernel(const uint8_t* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, tg_frame_window win,
+                     int x_tiles, int color) {
   using F = Yuv<kFmt>;
   static_assert(fmt_packed(kFmt) && !F::k10, "packed 4:2:2 is 8 bit");
   __shared__ __align__(16) uint8_t sin[kTilePx * 6 + 16];
@@ -504,7 +541,8 @@ rgb_to_yuv422_kernel(const uint8_t* __restrict__ rgb, uint8_t* __restrict__ out,
   const int sr = R0 + R1, sg = G0 + G1, sb = B0 + B1;
   const uint32_t u = q(k[3] * sr + k[4] * sg + k[5] * sb + co, sc);
   const uint32_t v = q(k[6] * sr + k[7] * sg + k[8] * sb + co, sc);
-  reinterpret_cast<uint32_t*>(out)[row * (W >> 1) + p0 + t] =
+  const size_t frow = (size_t)img * win.frame_h + win.top + y;   // frame_w and left are even
+  reinterpret_cast<uint32_t*>(out)[frow * (win.frame_w >> 1) + (win.left >> 1) + p0 + t] =
       y0 << (8 * packed_y0(kFmt)) | y1 << (8 * (packed_y0(kFmt) + 2)) | u << (8 * packed_u(kFmt)) |
       v << (8 * (packed_u(kFmt) + 2));
 }
@@ -514,8 +552,8 @@ rgb_to_yuv422_kernel(const uint8_t* __restrict__ rgb, uint8_t* __restrict__ out,
 // rgb_to_yuv420_kernel).  Colour row `color` of the table, per pixel.
 template <int kFmt, bool kF32>
 __global__ void __launch_bounds__(kThreads)
-rgb_to_yuv444_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, int x_tiles,
-                     int color) {
+rgb_to_yuv444_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, tg_frame_window win,
+                     int x_tiles, int color) {
   using F = Yuv<kFmt>;
   using Wd = typename F::Word;
   static_assert(fmt_444(kFmt) && kF32 == F::k10, "8-bit output reads uint8 RGB, 10-bit output the fp32 frame");
@@ -549,15 +587,17 @@ rgb_to_yuv444_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, in
   constexpr int kHalf = 1 << (F::kShift - 1);
   constexpr int coff = F::kCoff << F::kShift;
   auto q = [](int a) { return F::word(min(max(a >> F::kShift, 0), F::kTop)); };
-  Wd* dst = reinterpret_cast<Wd*>(out) + (size_t)img * 3 * plane + (size_t)y * W + x0 + t;
+  const size_t fplane = (size_t)win.frame_h * win.frame_w;
+  Wd* dst = reinterpret_cast<Wd*>(out) + (size_t)img * 3 * fplane + (size_t)(win.top + y) * win.frame_w + win.left +
+            x0 + t;
   dst[0] = q(k[0] * R + k[1] * G + k[2] * B + kHalf + (k[15] << F::kShift));
-  dst[plane] = q(k[3] * R + k[4] * G + k[5] * B + kHalf + coff);
-  dst[2 * plane] = q(k[6] * R + k[7] * G + k[8] * B + kHalf + coff);
+  dst[fplane] = q(k[3] * R + k[4] * G + k[5] * B + kHalf + coff);
+  dst[2 * fplane] = q(k[6] * R + k[7] * G + k[8] * B + kHalf + coff);
 }
 
 template <int kFmt>
-int launch_to_yuv(const char* name, const void* rgb, void* out, int n, int H, int W, int color,
-                  cudaStream_t stream) {
+int launch_to_yuv(const char* name, const void* rgb, void* out, int n, int H, int W, const tg_frame_window* win,
+                  int color, cudaStream_t stream) {
   using F = Yuv<kFmt>;
   TG_REQUIRE(n > 0 && H > 0 && W > 0, TG_E_INVALID, "%s: bad size n=%d H=%d W=%d", name, n, H, W);
   TG_REQUIRE(fmt_packed(kFmt) || fmt_444(kFmt) || (H % 2 == 0 && W % 2 == 0), TG_E_UNSUPPORTED,
@@ -565,21 +605,151 @@ int launch_to_yuv(const char* name, const void* rgb, void* out, int n, int H, in
   TG_REQUIRE(!fmt_packed(kFmt) || W % 2 == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name, W);
   TG_REQUIRE(!fmt_packed(kFmt) || ((uintptr_t)out & 3u) == 0, TG_E_INVALID,
              "%s: packed 4:2:2 output must be 4-byte aligned", name);
+  const tg_frame_window whole = {H, W, 0, 0};
+  if (!win) win = &whole;
+  const int rc = check_window<kFmt>(name, win, H, W);
+  if (rc != TG_OK) return rc;
   const int x_tiles = tg_ceil_div(fmt_packed(kFmt) ? W / 2 : W, kTilePx);
   const size_t ctas = (size_t)x_tiles * (fmt_packed(kFmt) || fmt_444(kFmt) ? H : H / 2) * n;
   TG_REQUIRE(ctas <= 0x7fffffff, TG_E_UNSUPPORTED, "%s: grid too large", name);
   uint8_t* o = static_cast<uint8_t*>(out);
   if constexpr (fmt_packed(kFmt))
     tg_launch(rgb_to_yuv422_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), 0, stream,
-              static_cast<const uint8_t*>(rgb), o, H, W, x_tiles, color);
+              static_cast<const uint8_t*>(rgb), o, H, W, *win, x_tiles, color);
   else if constexpr (fmt_444(kFmt))
     tg_launch(rgb_to_yuv444_kernel<kFmt, F::k10>, dim3((unsigned)ctas), dim3(kThreads), 0, stream, rgb, o, H, W,
-              x_tiles, color);
+              *win, x_tiles, color);
   else
     tg_launch(rgb_to_yuv420_kernel<kFmt, F::k10>, dim3((unsigned)ctas), dim3(kThreads), 0, stream, rgb, o, H, W,
-              x_tiles, color);
+              *win, x_tiles, color);
   TG_CUDA_LAUNCH_CHECK(name);
   return TG_OK;
+}
+
+// words of one fh x fw frame of layout kFmt (kHWC: c bytes a pixel)
+template <int kFmt>
+size_t frame_words(int c, int fh, int fw) {
+  const size_t px = (size_t)fh * fw;
+  return kFmt == kHWC ? px * c : fmt_packed(kFmt) ? 2 * px : fmt_444(kFmt) ? 3 * px : 3 * (px / 2);
+}
+
+// total words of n frames := the layout's black (Y: the colour's luma offset, U = V: kCoff; HWC: 0).  Grid-stride;
+// runs once per stream, when the padded output frames are allocated.
+template <int kFmt>
+__global__ void __launch_bounds__(kThreads)
+fill_black_kernel(uint8_t* __restrict__ out, size_t frame, size_t luma, size_t total, int color) {
+  using F = Yuv<kFmt>;
+  using Wd = typename F::Word;
+  tg_pdl_wait();
+  tg_pdl_trigger();
+  Wd* o = reinterpret_cast<Wd*>(out);
+  const int y = kFmt == kHWC ? 0 : c_yuv.v[F::k10][color][15];
+  for (size_t i = blockIdx.x * (size_t)kThreads + threadIdx.x; i < total; i += (size_t)gridDim.x * kThreads) {
+    const size_t j = i % frame;
+    // packed 4:2:2: Y is every other byte, starting at packed_y0; planar: the first fh * fw words
+    const bool is_y = fmt_packed(kFmt) ? (int)(j & 1) == packed_y0(kFmt) : j < luma;
+    o[i] = kFmt == kHWC ? (Wd)0 : F::word(is_y ? y : F::kCoff);
+  }
+}
+
+template <int kFmt>
+int launch_fill_black(const char* name, void* out, int n, int c, int fh, int fw, int color, cudaStream_t stream) {
+  TG_REQUIRE(out, TG_E_INVALID, "%s: null pointer (out)", name);
+  TG_REQUIRE(n > 0 && c > 0 && fh > 0 && fw > 0, TG_E_INVALID, "%s: bad size n=%d c=%d %dx%d", name, n, c, fh, fw);
+  TG_REQUIRE(kFmt == kHWC || c == 3, TG_E_INVALID, "%s: YUV frames carry 3 channels, got %d", name, c);
+  TG_REQUIRE(!fmt_10(kFmt) || ((uintptr_t)out & 1u) == 0, TG_E_INVALID, "%s: 10-bit frames must be 2-byte aligned",
+             name);
+  TG_REQUIRE(!fmt_420(kFmt) || ((fh | fw) & 1) == 0, TG_E_UNSUPPORTED,
+             "%s: YUV 4:2:0 needs an even height and width, got %dx%d", name, fh, fw);
+  TG_REQUIRE(!fmt_packed(kFmt) || (fw & 1) == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name,
+             fw);
+  const size_t frame = frame_words<kFmt>(c, fh, fw), total = frame * n;
+  const size_t need = (total + kThreads - 1) / kThreads, ctas = need < 4096 ? need : 4096;
+  tg_launch(fill_black_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), 0, stream, static_cast<uint8_t*>(out),
+            frame, (size_t)fh * fw, total, color);
+  TG_CUDA_LAUNCH_CHECK(name);
+  return TG_OK;
+}
+
+// One CTA: kTilePx pixels of one row of one frame -> their 8-bit luma (Y, 10-bit >> 2; RGB: cv2's gray) added to
+// cols[img][x] and, summed over the CTA, to rows[img][y].  Integer sums: the order does not matter.
+template <int kFmt>
+__global__ void __launch_bounds__(kThreads)
+luma_sums_kernel(const uint8_t* __restrict__ in, int c, int h, int w, int bgr, int x_tiles,
+                 unsigned long long* __restrict__ rows, unsigned long long* __restrict__ cols) {
+  using F = Yuv<kFmt>;
+  using Wd = typename F::Word;
+  __shared__ unsigned warp_sum[kThreads / 32];
+  tg_pdl_wait();
+  tg_pdl_trigger();
+  const int t = threadIdx.x;
+  const int xt = blockIdx.x % x_tiles, r = blockIdx.x / x_tiles;
+  const int y = r % h, img = r / h;
+  const int x = xt * kTilePx + t;
+  unsigned v = 0;
+  if (x < w) {
+    const size_t px = (size_t)h * w;
+    if constexpr (kFmt == kHWC) {
+      const uint8_t* p = in + (((size_t)img * h + y) * w + x) * c;
+      const unsigned R = __ldg(p + (bgr ? 2 : 0)), G = __ldg(p + 1), B = __ldg(p + (bgr ? 0 : 2));
+      v = (9798u * R + 19235u * G + 3735u * B + 16384u) >> 15;
+    } else if constexpr (fmt_packed(kFmt)) {
+      v = __ldg(in + ((size_t)img * h + y) * 2 * w + 2 * x + packed_y0(kFmt));   // Y of pixel x in its pair's group
+    } else {
+      const Wd* frame = reinterpret_cast<const Wd*>(in) + img * (fmt_444(kFmt) ? 3 * px : 3 * (px / 2));
+      v = (unsigned)F::sample(__ldg(frame + (size_t)y * w + x)) >> (F::k10 ? 2 : 0);
+    }
+    atomicAdd(cols + (size_t)img * w + x, (unsigned long long)v);
+  }
+  v = __reduce_add_sync(0xffffffffu, v);       // at most 32 * 255
+  if ((t & 31) == 0) warp_sum[t >> 5] = v;
+  __syncthreads();
+  if (t == 0) {
+    unsigned long long sum = 0;
+    for (int i = 0; i < kThreads / 32; ++i) sum += warp_sum[i];
+    atomicAdd(rows + (size_t)img * h + y, sum);
+  }
+}
+
+template <int kFmt>
+int launch_luma_sums(const char* name, const void* in, int bgr, int n, int c, int h, int w, unsigned long long* rows,
+                     unsigned long long* cols, cudaStream_t stream) {
+  TG_REQUIRE(in && rows && cols, TG_E_INVALID, "%s: null pointer (in / rows / cols)", name);
+  TG_REQUIRE(n > 0 && h > 0 && w > 0, TG_E_INVALID, "%s: bad size n=%d %dx%d", name, n, h, w);
+  TG_REQUIRE(c == 3, TG_E_INVALID, "%s: luma of 3-channel frames, got %d channels", name, c);
+  TG_REQUIRE((((uintptr_t)rows | (uintptr_t)cols) & 7u) == 0, TG_E_INVALID, "%s: rows and cols 8-byte aligned", name);
+  TG_REQUIRE(!fmt_10(kFmt) || ((uintptr_t)in & 1u) == 0, TG_E_INVALID, "%s: 10-bit frames must be 2-byte aligned",
+             name);
+  TG_REQUIRE(!fmt_420(kFmt) || ((h | w) & 1) == 0, TG_E_UNSUPPORTED,
+             "%s: YUV 4:2:0 needs an even height and width, got %dx%d", name, h, w);
+  TG_REQUIRE(!fmt_packed(kFmt) || (w & 1) == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name,
+             w);
+  const int x_tiles = tg_ceil_div(w, kTilePx);
+  const size_t ctas = (size_t)x_tiles * h * n;
+  TG_REQUIRE(ctas <= 0x7fffffff, TG_E_UNSUPPORTED, "%s: grid too large", name);
+  cudaError_t e = cudaMemsetAsync(rows, 0, (size_t)n * h * sizeof(unsigned long long), stream);
+  if (e == cudaSuccess) e = cudaMemsetAsync(cols, 0, (size_t)n * w * sizeof(unsigned long long), stream);
+  TG_REQUIRE(e == cudaSuccess, (int)e, "%s: cudaMemsetAsync: %s", name, cudaGetErrorString(e));
+  tg_launch(luma_sums_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), 0, stream, static_cast<const uint8_t*>(in),
+            c, h, w, bgr, x_tiles, rows, cols);
+  TG_CUDA_LAUNCH_CHECK(name);
+  return TG_OK;
+}
+
+// frame format kFmt -> fn(std::integral_constant<int, kFmt>)
+template <class Fn>
+int dispatch_format(int f, Fn&& fn) {
+  switch (f) {
+    case kHWC: return fn(std::integral_constant<int, kHWC>());
+    case kNV12: return fn(std::integral_constant<int, kNV12>());
+    case kI420: return fn(std::integral_constant<int, kI420>());
+    case kP010: return fn(std::integral_constant<int, kP010>());
+    case kI420_10: return fn(std::integral_constant<int, kI420_10>());
+    case kYUY2: return fn(std::integral_constant<int, kYUY2>());
+    case kUYVY: return fn(std::integral_constant<int, kUYVY>());
+    case kI444: return fn(std::integral_constant<int, kI444>());
+    default: return fn(std::integral_constant<int, kI444_10>());
+  }
 }
 
 // tg_yuv_format -> (frame format, colour row)
@@ -606,50 +776,23 @@ int parse_yuv_format(const char* name, const tg_yuv_format* f, int* fmt, int* co
 
 }  // namespace
 
-extern "C" int tg_stream_frame_in(const uint8_t* in_u8, const int32_t* reset, float* lr_curr, float* lr_prev,
-                                  float* hr_prev, int n, int c, int h, int w, int s, int bgr, void* stream) {
-  return launch_frame_in<kHWC>("stream_frame_in", in_u8, reset, lr_curr, lr_prev, hr_prev, n, c, h, w, s, bgr, 0,
-                               (cudaStream_t)stream);
-}
+namespace {
 
-extern "C" int tg_stream_frame_in_yuv420(const uint8_t* in, int nv12, const int32_t* reset, float* lr_curr,
-                                         float* lr_prev, float* hr_prev, int n, int h, int w, int s, void* stream) {
-  return nv12 ? launch_frame_in<kNV12>("stream_frame_in_yuv420", in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w,
-                                       s, 0, 0, (cudaStream_t)stream)
-              : launch_frame_in<kI420>("stream_frame_in_yuv420", in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w,
-                                       s, 0, 0, (cudaStream_t)stream);
-}
-
-extern "C" int tg_rgb_u8_to_yuv420(const uint8_t* rgb, uint8_t* out, int nv12, int n, int H, int W, void* stream) {
-  TG_REQUIRE(rgb && out, TG_E_INVALID, "rgb_u8_to_yuv420: null pointer (rgb / out)");
-  return nv12 ? launch_to_yuv<kNV12>("rgb_u8_to_yuv420", rgb, out, n, H, W, 0, (cudaStream_t)stream)
-              : launch_to_yuv<kI420>("rgb_u8_to_yuv420", rgb, out, n, H, W, 0, (cudaStream_t)stream);
-}
-
-extern "C" int tg_stream_frame_in_yuv(const void* in, const tg_yuv_format* fmt, const int32_t* reset, float* lr_curr,
-                                      float* lr_prev, float* hr_prev, int n, int h, int w, int s, void* stream) {
-  const char* name = "stream_frame_in_yuv";
+int frame_in_yuv(const char* name, const void* in, const tg_yuv_format* fmt, const tg_frame_window* win,
+                 const int32_t* reset, float* lr_curr, float* lr_prev, float* hr_prev, int n, int h, int w, int s,
+                 cudaStream_t st) {
   int f = 0, color = 0;
   const int rc = parse_yuv_format(name, fmt, &f, &color);
   if (rc != TG_OK) return rc;
-  const cudaStream_t st = (cudaStream_t)stream;
-  switch (f) {
-    case kNV12: return launch_frame_in<kNV12>(name, in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w, s, 0, color, st);
-    case kI420: return launch_frame_in<kI420>(name, in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w, s, 0, color, st);
-    case kP010: return launch_frame_in<kP010>(name, in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w, s, 0, color, st);
-    case kYUY2: return launch_frame_in<kYUY2>(name, in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w, s, 0, color, st);
-    case kUYVY: return launch_frame_in<kUYVY>(name, in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w, s, 0, color, st);
-    case kI444: return launch_frame_in<kI444>(name, in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w, s, 0, color, st);
-    case kI444_10:
-      return launch_frame_in<kI444_10>(name, in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w, s, 0, color, st);
-    default:
-      return launch_frame_in<kI420_10>(name, in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w, s, 0, color, st);
-  }
+  return dispatch_format(f, [&](auto k) {
+    constexpr int K = decltype(k)::value;
+    if constexpr (K == kHWC) return (int)TG_E_UNSUPPORTED;
+    else return launch_frame_in<K>(name, in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w, win, s, 0, color, st);
+  });
 }
 
-extern "C" int tg_rgb_to_yuv(const uint8_t* rgb_u8, const float* rgb_f32, void* out, const tg_yuv_format* fmt, int n,
-                             int H, int W, void* stream) {
-  const char* name = "rgb_to_yuv";
+int rgb_to_yuv(const char* name, const uint8_t* rgb_u8, const float* rgb_f32, void* out, const tg_yuv_format* fmt,
+               const tg_frame_window* win, int n, int H, int W, cudaStream_t st) {
   int f = 0, color = 0;
   const int rc = parse_yuv_format(name, fmt, &f, &color);
   if (rc != TG_OK) return rc;
@@ -660,17 +803,93 @@ extern "C" int tg_rgb_to_yuv(const uint8_t* rgb_u8, const float* rgb_f32, void* 
              ten ? "rgb_f32" : "rgb_u8");
   TG_REQUIRE(!ten || ((((uintptr_t)rgb_f32) & 3u) == 0 && (((uintptr_t)out) & 1u) == 0), TG_E_INVALID,
              "%s: rgb_f32 must be 4-byte and 10-bit output 2-byte aligned", name);
-  const cudaStream_t st = (cudaStream_t)stream;
-  switch (f) {
-    case kNV12: return launch_to_yuv<kNV12>(name, rgb_u8, out, n, H, W, color, st);
-    case kI420: return launch_to_yuv<kI420>(name, rgb_u8, out, n, H, W, color, st);
-    case kP010: return launch_to_yuv<kP010>(name, rgb_f32, out, n, H, W, color, st);
-    case kYUY2: return launch_to_yuv<kYUY2>(name, rgb_u8, out, n, H, W, color, st);
-    case kUYVY: return launch_to_yuv<kUYVY>(name, rgb_u8, out, n, H, W, color, st);
-    case kI444: return launch_to_yuv<kI444>(name, rgb_u8, out, n, H, W, color, st);
-    case kI444_10: return launch_to_yuv<kI444_10>(name, rgb_f32, out, n, H, W, color, st);
-    default: return launch_to_yuv<kI420_10>(name, rgb_f32, out, n, H, W, color, st);
+  const void* rgb = ten ? static_cast<const void*>(rgb_f32) : static_cast<const void*>(rgb_u8);
+  return dispatch_format(f, [&](auto k) {
+    constexpr int K = decltype(k)::value;
+    if constexpr (K == kHWC) return (int)TG_E_UNSUPPORTED;
+    else return launch_to_yuv<K>(name, rgb, out, n, H, W, win, color, st);
+  });
+}
+
+}  // namespace
+
+extern "C" int tg_stream_frame_in(const uint8_t* in_u8, const int32_t* reset, float* lr_curr, float* lr_prev,
+                                  float* hr_prev, int n, int c, int h, int w, int s, int bgr, void* stream) {
+  return launch_frame_in<kHWC>("stream_frame_in", in_u8, reset, lr_curr, lr_prev, hr_prev, n, c, h, w, nullptr, s,
+                               bgr, 0, (cudaStream_t)stream);
+}
+
+extern "C" int tg_stream_frame_in_window(const uint8_t* in_u8, const tg_frame_window* win, const int32_t* reset,
+                                         float* lr_curr, float* lr_prev, float* hr_prev, int n, int c, int h, int w,
+                                         int s, int bgr, void* stream) {
+  TG_REQUIRE(win, TG_E_INVALID, "stream_frame_in_window: null window");
+  return launch_frame_in<kHWC>("stream_frame_in_window", in_u8, reset, lr_curr, lr_prev, hr_prev, n, c, h, w, win, s,
+                               bgr, 0, (cudaStream_t)stream);
+}
+
+extern "C" int tg_stream_frame_in_yuv420(const uint8_t* in, int nv12, const int32_t* reset, float* lr_curr,
+                                         float* lr_prev, float* hr_prev, int n, int h, int w, int s, void* stream) {
+  return nv12 ? launch_frame_in<kNV12>("stream_frame_in_yuv420", in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w,
+                                       nullptr, s, 0, 0, (cudaStream_t)stream)
+              : launch_frame_in<kI420>("stream_frame_in_yuv420", in, reset, lr_curr, lr_prev, hr_prev, n, 3, h, w,
+                                       nullptr, s, 0, 0, (cudaStream_t)stream);
+}
+
+extern "C" int tg_rgb_u8_to_yuv420(const uint8_t* rgb, uint8_t* out, int nv12, int n, int H, int W, void* stream) {
+  TG_REQUIRE(rgb && out, TG_E_INVALID, "rgb_u8_to_yuv420: null pointer (rgb / out)");
+  return nv12 ? launch_to_yuv<kNV12>("rgb_u8_to_yuv420", rgb, out, n, H, W, nullptr, 0, (cudaStream_t)stream)
+              : launch_to_yuv<kI420>("rgb_u8_to_yuv420", rgb, out, n, H, W, nullptr, 0, (cudaStream_t)stream);
+}
+
+extern "C" int tg_stream_frame_in_yuv(const void* in, const tg_yuv_format* fmt, const int32_t* reset, float* lr_curr,
+                                      float* lr_prev, float* hr_prev, int n, int h, int w, int s, void* stream) {
+  return frame_in_yuv("stream_frame_in_yuv", in, fmt, nullptr, reset, lr_curr, lr_prev, hr_prev, n, h, w, s,
+                      (cudaStream_t)stream);
+}
+
+extern "C" int tg_stream_frame_in_yuv_window(const void* in, const tg_yuv_format* fmt, const tg_frame_window* win,
+                                             const int32_t* reset, float* lr_curr, float* lr_prev, float* hr_prev,
+                                             int n, int h, int w, int s, void* stream) {
+  TG_REQUIRE(win, TG_E_INVALID, "stream_frame_in_yuv_window: null window");
+  return frame_in_yuv("stream_frame_in_yuv_window", in, fmt, win, reset, lr_curr, lr_prev, hr_prev, n, h, w, s,
+                      (cudaStream_t)stream);
+}
+
+extern "C" int tg_rgb_to_yuv(const uint8_t* rgb_u8, const float* rgb_f32, void* out, const tg_yuv_format* fmt, int n,
+                             int H, int W, void* stream) {
+  return rgb_to_yuv("rgb_to_yuv", rgb_u8, rgb_f32, out, fmt, nullptr, n, H, W, (cudaStream_t)stream);
+}
+
+extern "C" int tg_rgb_to_yuv_window(const uint8_t* rgb_u8, const float* rgb_f32, void* out, const tg_yuv_format* fmt,
+                                    const tg_frame_window* win, int n, int H, int W, void* stream) {
+  TG_REQUIRE(win, TG_E_INVALID, "rgb_to_yuv_window: null window");
+  return rgb_to_yuv("rgb_to_yuv_window", rgb_u8, rgb_f32, out, fmt, win, n, H, W, (cudaStream_t)stream);
+}
+
+extern "C" int tg_fill_black(void* out, const tg_yuv_format* fmt, int n, int c, int frame_h, int frame_w,
+                             void* stream) {
+  const char* name = "fill_black";
+  int f = kHWC, color = 0;
+  if (fmt) {
+    const int rc = parse_yuv_format(name, fmt, &f, &color);
+    if (rc != TG_OK) return rc;
   }
+  return dispatch_format(f, [&](auto k) {
+    return launch_fill_black<decltype(k)::value>(name, out, n, c, frame_h, frame_w, color, (cudaStream_t)stream);
+  });
+}
+
+extern "C" int tg_luma_line_sums(const void* in, const tg_yuv_format* fmt, int bgr, int n, int c, int h, int w,
+                                 unsigned long long* rows, unsigned long long* cols, void* stream) {
+  const char* name = "luma_line_sums";
+  int f = kHWC, color = 0;
+  if (fmt) {
+    const int rc = parse_yuv_format(name, fmt, &f, &color);
+    if (rc != TG_OK) return rc;
+  }
+  return dispatch_format(f, [&](auto k) {
+    return launch_luma_sums<decltype(k)::value>(name, in, bgr, n, c, h, w, rows, cols, (cudaStream_t)stream);
+  });
 }
 
 extern "C" int tg_yuv_coefficients(const tg_yuv_format* fmt, int32_t* out16) {

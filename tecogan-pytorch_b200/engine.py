@@ -245,18 +245,29 @@ class StreamEngine(ClipEngine):
     and cut[p] (int32 [n]) are views of one int32 buffer rep[p] [3n], copied after each replay into the push's
     report [k,3n] (one device-to-device copy per frame).
 
+    Windows (tg_frame_window).  crop = (Hf, Wf, top, left): inp[p] holds whole Hf x Wf source frames and the frame input
+    reads the h x w picture at (top, left) out of them, in the same one launch (the net, FNet's flow and scene_cut see
+    the picture only).  out_frame = (Hf, Wf, y, x): the copies out read padded frames, pad[p] (uint8 RGB [n,Hf,Wf,c])
+    or yuv[p] (Hf x Wf YUV frames), whose bars are filled with the output format's black once, here, and never
+    written again; every step writes the picture at (y, x) -- the windowed uint8 writer in place of the step's own
+    uint8 output (the step then runs without it), the windowed resize, or the windowed encode.
+
     Copies overlap compute as in ClipEngine.run_clips.  uint8 input: inp[p] is itself the 2-deep staging ring (the
     step of parity p^1 never reads it), so the H2D of frame i+1 lands directly in the graph's input while frame i
     runs.  fp32 input: lr[p] is still read as lr_prev by frame i, so frames are staged as in run_clips."""
 
     def __init__(self, net, n, c, h, w, device, u8_input=True, bgr=False, yuv_in=None, yuv_out=None,
-                 in_color='bt601', out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None):
+                 in_color='bt601', out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None,
+                 crop=None, out_frame=None):
         dev = torch.device(device)
         self.u8_input, self.bgr = u8_input or yuv_in is not None, bgr
         self.yuv_in, self.yuv_out = yuv_in, yuv_out          # None or one of ops.YUV_LAYOUTS
         self.in_color, self.out_color = in_color, out_color
         self.mask = [torch.zeros(n, dtype=torch.int32, device=dev) for _ in range(2)]
-        frame = ops.yuv_frame_shape(yuv_in, h, w) if yuv_in else (h, w, c)
+        self.crop = tuple(crop) if crop else None            # (Hf, Wf, top, left) of the input frames
+        self.out_frame = tuple(out_frame) if out_frame else None   # (Hf, Wf, y, x) of the output frames
+        fh, fw = self.crop[:2] if self.crop else (h, w)
+        frame = ops.yuv_frame_shape(yuv_in, fh, fw) if yuv_in else (fh, fw, c)
         # 10-bit words: zeroed as int16, the same bits
         in_dtype = torch.int16 if yuv_in and ops.yuv_depth(yuv_in) == 10 else torch.uint8
         self.inp = ([torch.zeros(n, *frame, dtype=in_dtype, device=dev).view(_word_dtype(yuv_in)) for _ in range(2)]
@@ -271,9 +282,21 @@ class StreamEngine(ClipEngine):
             f32 = yuv_out is not None and ops.yuv_depth(yuv_out) == 10
             self.rs = [torch.empty((n, c, Ho, Wo) if f32 else (n, Ho, Wo, c),
                                    dtype=torch.float32 if f32 else torch.uint8, device=dev) for _ in range(2)]
-        self.yuv = ([torch.empty(n, *ops.yuv_frame_shape(yuv_out, Ho, Wo), dtype=_word_dtype(yuv_out), device=dev)
+        Yf, Xf = self.out_frame[:2] if self.out_frame else (Ho, Wo)
+        self.yuv = ([torch.empty(n, *ops.yuv_frame_shape(yuv_out, Yf, Xf), dtype=_word_dtype(yuv_out), device=dev)
                      for _ in range(2)]
                     if yuv_out else None)
+        self.pad = None
+        if self.out_frame:
+            # on dev's current stream, which the capture's warm-up stream waits for: the fill is ordered before every
+            # write of the picture
+            with torch.cuda.device(dev):
+                if yuv_out:
+                    for t in self.yuv:
+                        ops.fill_black(t, yuv_out, out_color)
+                else:
+                    self.pad = [ops.fill_black(torch.empty((n, Yf, Xf, c), dtype=torch.uint8, device=dev))
+                                for _ in range(2)]
         self.scene_cut = scene_cut
         self.prev_mafd = self.work = self.rep = self.score = self.cut = None
         self.report = None               # [k,3n] int32 of the last run: score[p] / cut[p] after each frame
@@ -295,41 +318,52 @@ class StreamEngine(ClipEngine):
 
     def close(self):
         super().close()
-        self.mask, self.inp, self.yuv = [], None, None
+        self.mask, self.inp, self.yuv, self.pad = [], None, None, None
         self.tables, self.rs = None, None
         self.prev_mafd = self.work = self.rep = self.score = self.cut = self.report = None
         self._report_dev = self._report_host = None
 
     def _enqueue(self, p):
-        if self.yuv_in in YUV420 and self.in_color == 'bt601':
+        crop = self.crop[2:] if self.crop else None          # (top, left)
+        pad = self.out_frame[2:] if self.out_frame else None  # (y, x)
+        if self.yuv_in in YUV420 and self.in_color == 'bt601' and crop is None:
             ops.stream_frame_in_yuv420(self.inp[p], self.yuv_in, self.mask[p], self.lr[p], self.lr[p ^ 1],
                                        self.hr[p ^ 1], self.net.scale)
         elif self.yuv_in:
+            # the windowed entry point has no BT.601-only twin: its bt601 row is the same cv2 conversion
             ops.stream_frame_in_yuv(self.inp[p], self.yuv_in, self.in_color, self.mask[p], self.lr[p],
-                                    self.lr[p ^ 1], self.hr[p ^ 1], self.net.scale)
+                                    self.lr[p ^ 1], self.hr[p ^ 1], self.net.scale, window=crop)
         else:
             ops.stream_frame_in(self.inp[p] if self.u8_input else None, self.mask[p], self.lr[p], self.lr[p ^ 1],
-                                self.hr[p ^ 1], self.net.scale, self.bgr)
+                                self.hr[p ^ 1], self.net.scale, self.bgr, window=crop if self.u8_input else None)
         if self.scene_cut is not None:
             ops.scene_cut(self.lr[p], self.lr[p ^ 1], self.mask[p], self.scene_cut, self.prev_mafd, self.work,
                           self.score[p], self.cut[p])
             # a detected cut restarts the slot: the reset-only frame input with cut[p] as its mask
             ops.stream_frame_in(None, self.cut[p], self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1], self.net.scale)
-        if self.out_size is None:
+        if self.out_size is None and self.pad is not None:
+            # the picture goes straight into the padded frame: the windowed writer replaces the step's uint8 output
+            self.net.step_into(self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1], self.hr[p], out_u8=None)
+            ops.float_to_uint8_nhwc_window(self.hr[p], self.pad[p], pad)
+        elif self.out_size is None:
             super()._enqueue(p)
             rgb_u8, rgb_f32 = self.u8[p], self.hr[p]
         else:
             self.net.step_into(self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1], self.hr[p], out_u8=None)
-            f32 = self.rs[p].dtype == torch.float32
-            ops.resample(self.hr[p], *self.tables, out_u8=None if f32 else self.rs[p], out_f32=self.rs[p] if f32 else None)
-            rgb_u8 = rgb_f32 = self.rs[p]
-        if self.yuv_out in YUV420 and self.out_color == 'bt601':
+            if self.pad is not None:
+                ops.resample(self.hr[p], *self.tables, out_u8=self.pad[p], window=pad)
+            else:
+                f32 = self.rs[p].dtype == torch.float32
+                ops.resample(self.hr[p], *self.tables, out_u8=None if f32 else self.rs[p],
+                             out_f32=self.rs[p] if f32 else None)
+                rgb_u8 = rgb_f32 = self.rs[p]
+        if self.yuv_out in YUV420 and self.out_color == 'bt601' and pad is None:
             ops.rgb_u8_to_yuv420(rgb_u8, self.yuv_out, out=self.yuv[p])
         elif self.yuv_out and ops.yuv_depth(self.yuv_out) == 8:
-            ops.rgb_to_yuv(self.yuv_out, self.out_color, rgb_u8=rgb_u8, out=self.yuv[p])
+            ops.rgb_to_yuv(self.yuv_out, self.out_color, rgb_u8=rgb_u8, out=self.yuv[p], window=pad)
         elif self.yuv_out:
             # 10 bit: from the step's fp32 HR frame (or its resize), two more bits than the uint8 output keeps
-            ops.rgb_to_yuv(self.yuv_out, self.out_color, rgb_f32=rgb_f32, out=self.yuv[p])
+            ops.rgb_to_yuv(self.yuv_out, self.out_color, rgb_f32=rgb_f32, out=self.yuv[p], window=pad)
 
     def _set_mask(self, p, slots):
         """On the main stream, before the replay of parity p: mask[p] = 1 for `slots`, 0 elsewhere."""
@@ -356,7 +390,7 @@ class StreamEngine(ClipEngine):
             for st in (self.main, self.h2d, self.d2h):
                 st.wait_stream(cur)
             # what the step graph leaves for the copy out
-            res = self.yuv if self.yuv_out else self.rs if self.out_size else self.u8
+            res = self.yuv if self.yuv_out else self.pad if self.pad else self.rs if self.out_size else self.u8
             shape = (n, k, *res[0].shape[1:])
             if out_host:
                 out = torch.empty(shape, dtype=res[0].dtype, pin_memory=True)
@@ -433,7 +467,8 @@ class VideoStream:
     Created by FRNet.stream(); see there."""
 
     def __init__(self, net, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb',
-                 in_color='bt601', out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None):
+                 in_color='bt601', out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None,
+                 crop=None, out_frame=None, out_origin=None):
         if scene_cut is not None:
             scene_cut = _check_scene_cut(scene_cut)
         if input not in ('uint8', 'float32', *YUV):
@@ -455,14 +490,28 @@ class VideoStream:
             raise ValueError(f'resize_filter must be one of {ops.RESIZE_FILTERS}, got {resize_filter!r}')
         if out_size is None and resize_filter != 'bicubic':
             raise ValueError(f'resize_filter={resize_filter!r} applies to a resized stream only (give out_size)')
+        if crop is not None:
+            if input == 'float32':
+                raise ValueError("crop applies to uint8 and YUV frames, not to input='float32'")
+            crop = _check_box('crop', crop, h, w, input)
+        ph, pw = crop[2:] if crop else (h, w)      # the picture the net runs on
         if out_size is not None:
-            out_size = _check_out_size(out_size, net.scale * h, net.scale * w, out_format)
+            out_size = _check_out_size(out_size, net.scale * ph, net.scale * pw, out_format)
         yuv = [f for f in (input, out_format) if f in YUV]
-        for f in yuv:
-            if f not in _YUV_422_444 and (h % 2 or w % 2):
-                raise ValueError(f'{f} frames are YUV 4:2:0: h and w must be even, got {h}x{w}')
-            if f in ops.YUV422_LAYOUTS and w % 2:
-                raise ValueError(f'{f} frames are YUV 4:2:2: w must be even, got {h}x{w}')
+        # the input layout holds the pushed h x w frames; the output layout's picture comes from the ph x pw picture
+        # the net runs on (the whole frame without crop)
+        for f, (a, b) in ((input, (h, w)), (out_format, (ph, pw))):
+            if f not in YUV:
+                continue
+            if f not in _YUV_422_444 and (a % 2 or b % 2):
+                raise ValueError(f'{f} frames are YUV 4:2:0: h and w must be even, got {a}x{b}')
+            if f in ops.YUV422_LAYOUTS and b % 2:
+                raise ValueError(f'{f} frames are YUV 4:2:2: w must be even, got {a}x{b}')
+        if out_frame is None and out_origin is not None:
+            raise ValueError('out_origin applies to a padded output only (give out_frame)')
+        if out_frame is not None:
+            Ho, Wo = out_size or (net.scale * ph, net.scale * pw)
+            out_frame, out_origin = _check_out_frame(out_frame, out_origin, Ho, Wo, out_format)
         if yuv and net.fnet.in_nc != 3:
             raise ValueError(f'{yuv[0]} frames carry 3 colour channels, the net takes {net.fnet.in_nc}')
         device = torch.device('cuda') if device is None else torch.device(device)
@@ -474,6 +523,7 @@ class VideoStream:
         self.in_color, self.out_color = in_color, out_color
         self.out_size, self.resize_filter = out_size, resize_filter
         self.scene_cut = scene_cut
+        self.crop, self.out_frame, self.out_origin = crop, out_frame, out_origin
         # the latest push's detected cuts (bool [n,k]) and scores (float64 [n,k]): NumPy after out='host', CUDA
         # tensors after out='device'; None before the first push and without scene_cut
         self.last_cuts = self.last_scores = None
@@ -608,10 +658,16 @@ class VideoStream:
         self.device = dev
         yuv_in = self.input if self.input in YUV else None
         yuv_out = self.out_format if self.out_format in YUV else None
-        return StreamEngine(self.net, self.n, self.c, self.h, self.w, dev, u8_input=self.input == 'uint8',
+        h, w, crop = self.h, self.w, None
+        if self.crop:
+            top, left, h, w = self.crop
+            crop = (self.h, self.w, top, left)
+        out_frame = (*self.out_frame, *self.out_origin) if self.out_frame else None
+        return StreamEngine(self.net, self.n, self.c, h, w, dev, u8_input=self.input == 'uint8',
                             bgr=self.channel_order == 'bgr', yuv_in=yuv_in, yuv_out=yuv_out,
                             in_color=self.in_color, out_color=self.out_color, out_size=self.out_size,
-                            resize_filter=self.resize_filter, scene_cut=self.scene_cut)
+                            resize_filter=self.resize_filter, scene_cut=self.scene_cut, crop=crop,
+                            out_frame=out_frame)
 
 
 def _check_scene_cut(threshold):
@@ -639,6 +695,131 @@ def _check_out_size(out_size, H, W, out_format):
     if out_format in ops.YUV422_LAYOUTS and Wo % 2:
         raise ValueError(f'{out_format} frames are YUV 4:2:2: the width of out_size must be even, got {Ho}x{Wo}')
     return Ho, Wo
+
+
+def _is_int(v):
+    return isinstance(v, numbers.Integral) and not isinstance(v, bool)
+
+
+def _grid(layout):
+    """(row, column) step of a layout's chroma grid: 4:2:0 (2, 2), 4:2:2 (1, 2), RGB / 4:4:4 (1, 1)."""
+    if layout in ops.YUV422_LAYOUTS:
+        return 1, 2
+    return (2, 2) if layout in YUV and layout not in _YUV_422_444 else (1, 1)
+
+
+def _check_box(arg, box, h, w, layout):
+    """box = (top, left, ch, cw) -> ints, or ValueError: a non-empty box inside the h x w frame, on the layout's
+    chroma grid (4:2:0: all four even; 4:2:2: left and cw even)."""
+    if not isinstance(box, (tuple, list)) or len(box) != 4 or not all(_is_int(v) for v in box):
+        raise ValueError(f'{arg} must be (top, left, ch, cw), four ints, got {box!r}')
+    top, left, ch, cw = (int(v) for v in box)
+    if top < 0 or left < 0 or ch <= 0 or cw <= 0 or top + ch > h or left + cw > w:
+        raise ValueError(f'{arg} {ch}x{cw} at ({top}, {left}) lies outside the {h}x{w} frame')
+    gy, gx = _grid(layout)
+    if top % gy or ch % gy or left % gx or cw % gx:
+        raise ValueError(f'{arg} ({top}, {left}, {ch}, {cw}) is off the {layout} chroma grid: rows in steps of {gy}, '
+                         f'columns in steps of {gx}')
+    return top, left, ch, cw
+
+
+def _check_out_frame(out_frame, out_origin, Ho, Wo, out_format):
+    """out_frame (Hf, Wf) and out_origin (y, x) or None -> ints, or ValueError: the Ho x Wo picture inside the frame,
+    frame and origin on the output layout's chroma grid.  The default origin centres the picture, rounded down to
+    the grid."""
+    if (not isinstance(out_frame, (tuple, list)) or len(out_frame) != 2
+            or not all(_is_int(v) and v > 0 for v in out_frame)):
+        raise ValueError(f'out_frame must be (Hf, Wf), two positive ints, got {out_frame!r}')
+    Hf, Wf = int(out_frame[0]), int(out_frame[1])
+    if Ho > Hf or Wo > Wf:
+        raise ValueError(f'the {Ho}x{Wo} output picture does not fit out_frame {Hf}x{Wf}')
+    gy, gx = _grid(out_format)
+    if Hf % gy or Wf % gx:
+        raise ValueError(f'out_frame {Hf}x{Wf} is off the {out_format} chroma grid')
+    if out_origin is None:
+        out_origin = ((Hf - Ho) // 2 // gy * gy, (Wf - Wo) // 2 // gx * gx)
+    if not isinstance(out_origin, (tuple, list)) or len(out_origin) != 2 or not all(_is_int(v) for v in out_origin):
+        raise ValueError(f'out_origin must be (y, x), two ints, got {out_origin!r}')
+    y, x = int(out_origin[0]), int(out_origin[1])
+    if y < 0 or x < 0 or y + Ho > Hf or x + Wo > Wf:
+        raise ValueError(f'the {Ho}x{Wo} output picture at out_origin ({y}, {x}) does not fit out_frame {Hf}x{Wf}')
+    if y % gy or x % gx:
+        raise ValueError(f'out_origin ({y}, {x}) is off the {out_format} chroma grid')
+    return (Hf, Wf), (y, x)
+
+
+def fit_size(picture, frame, sar=(1, 1), out_format='rgb'):
+    """The largest picture size (h, w) that shows a `picture` (ch, cw) of sample aspect ratio `sar` at its display
+    aspect inside `frame` (Hf, Wf) of square pixels: letterboxed or pillarboxed, each side on out_format's chroma grid
+    and within the resize's ratios (1/4 to 2 times the picture's side).  Host only.  Use it as out_size with
+    out_frame=frame: an anamorphic 720x480 DVD (sar 8:9 for 4:3, 32:27 for 16:9) becomes a pillarbox or letterbox of
+    a 1080p frame.  The ratio limits refer to the picture given here; pass the HR size (scale * crop) as `picture`
+    for a stream.  ValueError when no size on the grid fits."""
+    for arg, v in (('picture', picture), ('frame', frame), ('sar', sar)):
+        if not isinstance(v, (tuple, list)) or len(v) != 2 or not all(_is_int(x) and x > 0 for x in v):
+            raise ValueError(f'{arg} must be two positive ints, got {v!r}')
+    if out_format not in ('rgb', *YUV):
+        raise ValueError(f"out_format must be 'rgb' or one of {YUV}, got {out_format!r}")
+    ch, cw = (int(v) for v in picture)
+    Hf, Wf = (int(v) for v in frame)
+    gy, gx = _grid(out_format)
+    # display aspect num / den = (cw * sar_w) / (ch * sar_h), exact in integers
+    num, den = cw * int(sar[0]), ch * int(sar[1])
+    h, w = Hf, Hf * num // den
+    if w > Wf:
+        w, h = Wf, Wf * den // num
+    h, w = min(h // gy * gy, 2 * ch // gy * gy), min(w // gx * gx, 2 * cw // gx * gx)
+    # the side the ratio capped first keeps the display aspect of the other (rounded down to the grid)
+    if h * num > w * den:
+        h = w * den // num // gy * gy
+    elif w * den > h * num:
+        w = h * num // den // gx * gx
+    if h <= 0 or w <= 0 or not (ops.resample_ratio_ok(ch, h) and ops.resample_ratio_ok(cw, w)):
+        raise ValueError(f'no {out_format} picture size between 1/4 and 2 times {ch}x{cw} fits {Hf}x{Wf} at aspect '
+                         f'{num}:{den}')
+    return h, w
+
+
+def detect_bars(frames, input='uint8', channel_order='rgb', limit=24):
+    """The picture box (top, left, ch, cw) of letterboxed / pillarboxed frames, found on the device: a row or column
+    is picture when its mean 8-bit luma exceeds `limit` in any of the frames (24 is ffmpeg cropdetect's default
+    limit; the rule is oracle/frame_window.py's, not cropdetect's), and the box spans the first to the last picture
+    row and column, rounded inward to the input layout's chroma grid.  Luma is Y for YUV input (10-bit samples >> 2)
+    and cv2's gray of RGB ((9798 R + 19235 G + 3735 B + 16384) >> 15).  frames: a CUDA tensor [k,h,w,3] (uint8,
+    channel_order 'rgb' or 'bgr') or [k,*yuv_frame_shape(input, h, w)] for a YUV input.  Frames with no picture row
+    or column (all black) give the whole frame.  Pass crop=detect_bars(...) to FRNet.stream."""
+    if input not in ('uint8', *YUV):
+        raise ValueError(f"input must be 'uint8' or one of {YUV}, got {input!r}")
+    if channel_order not in ('rgb', 'bgr') or (input != 'uint8' and channel_order != 'rgb'):
+        raise ValueError(f'channel_order={channel_order!r} does not apply to input={input!r}')
+    if isinstance(limit, bool) or not isinstance(limit, numbers.Real) or not 0 <= limit < 255:
+        raise ValueError(f'limit must be a number in [0, 255), got {limit!r}')
+    if not isinstance(frames, torch.Tensor) or not frames.is_cuda:
+        raise ValueError('detect_bars: frames must be a CUDA tensor')
+    layout = input if input in YUV else None
+    with torch.cuda.device(frames.device):          # the memsets and the kernel go to the frames' device
+        rows, cols = ops.luma_line_sums(frames.contiguous(), layout, channel_order == 'bgr')
+    h, w = rows.shape[1], cols.shape[1]
+    # mean > limit <=> sum > limit * count: exact for integer limits, and for others compared in float64
+    pic_r = (rows.double() > float(limit) * w).any(0).cpu().numpy()
+    pic_c = (cols.double() > float(limit) * h).any(0).cpu().numpy()
+    return bars_box(pic_r, pic_c, input)
+
+
+def bars_box(pic_rows, pic_cols, layout):
+    """(top, left, ch, cw) from per-row / per-column picture flags, rounded inward to the layout's chroma grid; the
+    whole frame when no row or column is picture (or the rounded box is empty)."""
+    h, w = len(pic_rows), len(pic_cols)
+    gy, gx = _grid(layout)
+    if not pic_rows.any() or not pic_cols.any():
+        return 0, 0, h, w
+    r = np.flatnonzero(pic_rows)
+    c = np.flatnonzero(pic_cols)
+    top, bottom = -(-int(r[0]) // gy) * gy, (int(r[-1]) + 1) // gy * gy
+    left, right = -(-int(c[0]) // gx) * gx, (int(c[-1]) + 1) // gx * gx
+    if bottom <= top or right <= left:
+        return 0, 0, h, w
+    return top, left, bottom - top, right - left
 
 
 def _check_inference(net):

@@ -65,6 +65,11 @@ class YuvFormat(ctypes.Structure):
     _fields_ = [('layout', c_int32), ('matrix', c_int32), ('full_range', c_int32), ('reserved', c_int32)]
 
 
+class FrameWindow(ctypes.Structure):
+    """struct tg_frame_window"""
+    _fields_ = [('frame_h', c_int32), ('frame_w', c_int32), ('top', c_int32), ('left', c_int32)]
+
+
 class FarnebackParams(ctypes.Structure):
     """struct tg_farneback_params"""
     _fields_ = [('pyr_scale', c_double), ('levels', c_int32), ('winsize', c_int32), ('iterations', c_int32),
@@ -98,16 +103,27 @@ _SIGNATURES = {
     'tg_nchw_f32_to_nhwc_f16': (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_nhwc_f16_to_nchw_f32': (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_float_to_uint8_nhwc': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
+    'tg_float_to_uint8_nhwc_window': (c_int, [_P, _P, ctypes.POINTER(FrameWindow), c_int, c_int, c_int, c_int, _P]),
     'tg_stream_frame_in': (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_stream_frame_in_yuv420': (c_int, [_P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'tg_rgb_u8_to_yuv420': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     'tg_stream_frame_in_yuv': (c_int, [_P, ctypes.POINTER(YuvFormat), _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'tg_rgb_to_yuv': (c_int, [_P, _P, _P, ctypes.POINTER(YuvFormat), c_int, c_int, c_int, _P]),
     'tg_yuv_coefficients': (c_int, [ctypes.POINTER(YuvFormat), ctypes.POINTER(c_int32)]),
+    'tg_stream_frame_in_window': (c_int, [_P, ctypes.POINTER(FrameWindow), _P, _P, _P, _P, c_int, c_int, c_int, c_int,
+                                          c_int, c_int, _P]),
+    'tg_stream_frame_in_yuv_window': (c_int, [_P, ctypes.POINTER(YuvFormat), ctypes.POINTER(FrameWindow), _P, _P, _P,
+                                              _P, c_int, c_int, c_int, c_int, _P]),
+    'tg_rgb_to_yuv_window': (c_int, [_P, _P, _P, ctypes.POINTER(YuvFormat), ctypes.POINTER(FrameWindow), c_int, c_int,
+                                     c_int, _P]),
+    'tg_fill_black': (c_int, [_P, ctypes.POINTER(YuvFormat), c_int, c_int, c_int, c_int, _P]),
+    'tg_luma_line_sums': (c_int, [_P, ctypes.POINTER(YuvFormat), c_int, c_int, c_int, c_int, c_int, _P, _P, _P]),
     'tg_resample_taps': (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_int)]),
     'tg_resample_table': (c_int, [c_int, c_int, c_int, c_int, _P, _P]),
     'tg_resample_nchw_f32': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, _P, c_int, c_int, c_int,
                                      _P, _P, _P]),
+    'tg_resample_nchw_f32_window': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, _P, c_int, c_int, c_int,
+                                            _P, ctypes.POINTER(FrameWindow), _P]),
     'tg_scene_cut': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, c_double, _P, _P, _P, _P, _P]),
     'tg_metrics_frames_in': (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P, _P, _P]),
     'tg_farneback_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),

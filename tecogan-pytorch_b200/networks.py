@@ -344,7 +344,8 @@ class FRNet(BaseSequenceGenerator):
         return infer_clips(self, lr_data, device)
 
     def stream(self, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb', in_color='bt601',
-               out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None):
+               out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None, crop=None, out_frame=None,
+               out_origin=None):
         """A VideoStream of n lock-stepped slots of h x w LR frames: video pushed in chunks of any length, the
         recurrent state carried from one push to the next, and a slot restarted (reset=) when its video ends and
         the next one begins while the other slots keep running.
@@ -388,12 +389,25 @@ class FRNet(BaseSequenceGenerator):
         >= threshold restarts the slot at that frame exactly as reset= would have.  After each push the stream's
         last_cuts (bool [n,k]) and last_scores (float64 [n,k]) tell where, e.g. to ask the encoder for a keyframe.
         None (the default) turns detection off; any input and output format work with it.
+        Letterboxed / pillarboxed video: crop=(top, left, ch, cw) runs the net, FNet's flow and scene_cut on the
+        ch x cw picture at (top, left) of the h x w frames pushed (h x w stays the frame's size in the input layout's
+        shape); the output picture is s*ch x s*cw (or out_size, whose ratio limits then refer to the picture).  The
+        bars are never read.  A decoder surface of pitch P words and R rows (NVDEC NV12 / P010: the chroma plane at
+        P * R) is the frame h, w = R, P with crop=(0, 0, rows, cols) -- no copy into a packed frame.  tecogan_b200.
+        detect_bars(frames, input=...) finds the box on the device.  crop needs uint8 or YUV input and the input
+        layout's chroma grid (4:2:0: even top, left, ch, cw; 4:2:2: even left and cw).
+        out_frame=(Hf, Wf) returns Hf x Wf frames in out_format with the picture at out_origin=(y, x) (default: centred,
+        rounded down to the output layout's chroma grid) and everything else the format's exact black (RGB 0; Y 16 /
+        C 128 at 8-bit limited range, Y 0 full range, 64 / 512 and 0 / 512 at 10 bits, P010 words << 6).  The bars
+        are written once, when the stream is built; each step writes only the picture.  tecogan_b200.fit_size gives
+        the largest out_size of the picture's display aspect that fits the frame (pillarbox / letterbox).
+        A crop or picture that does not fit, or lies off the chroma grid, raises ValueError.
         Temporal padding (pad_sequence, base_model.py:230-251) stays the caller's job: for p reflect-padded
         frames, push frames[:, 1:1+p].flip(1) first and drop those p outputs.  The CUDA graphs are captured by the first push; the stream holds the
         net."""
         from .engine import VideoStream
         return VideoStream(self, n, h, w, device, input, channel_order, out_format, in_color, out_color, out_size,
-                           resize_filter, scene_cut)
+                           resize_filter, scene_cut, crop, out_frame, out_origin)
 
     def refresh_packed_weights(self, force=False):
         self.fnet._cache.refresh_all(force)

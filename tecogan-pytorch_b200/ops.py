@@ -364,10 +364,30 @@ def float_to_uint8_nhwc(x, y=None):
     return y
 
 
-def stream_frame_in(u8, reset, lr_curr, lr_prev, hr_prev, scale, bgr=False):
+def float_to_uint8_nhwc_window(x, y, window):
+    """tg_float_to_uint8_nhwc_window: float_to_uint8_nhwc of x fp32 NCHW [n,c,h,w] written as the h x w picture at
+    window = (top, left) of each uint8 NHWC frame of y [n,Hf,Wf,c]; nothing else of y is written."""
+    _req(x, torch.float32, 'x', 4)
+    n, c, h, w = x.shape
+    _req(y, torch.uint8, 'y', 4)
+    if y.shape[0] != n or y.shape[3] != c or y.device != x.device:
+        raise L.TecoganB200Error(f'float_to_uint8_nhwc: y {tuple(y.shape)} does not hold [n={n},Hf,Wf,c={c}] frames')
+    win = frame_window(y.shape[1], y.shape[2], *window)
+    L.check(L.load().tg_float_to_uint8_nhwc_window(_ptr(x), _ptr(y), ctypes.byref(win), n, c, h, w, _stream()),
+            'tg_float_to_uint8_nhwc_window')
+    return y
+
+
+def frame_window(frame_h, frame_w, top, left):
+    """struct tg_frame_window: the picture at (top, left) of a frame_h x frame_w stored frame."""
+    return L.FrameWindow(int(frame_h), int(frame_w), int(top), int(left))
+
+
+def stream_frame_in(u8, reset, lr_curr, lr_prev, hr_prev, scale, bgr=False, window=None):
     """Frame input of a streamed step (tg_stream_frame_in): u8 uint8 [n,h,w,c] (or None) -> lr_curr fp32
     [n,c,h,w] = u8 / 255, channels reversed when bgr; slots k with reset[k] != 0 (int32 [n] on the device,
-    or None) get lr_prev[k] = hr_prev[k] = 0 ([n,c,h,w] / [n,c,scale*h,scale*w] fp32)."""
+    or None) get lr_prev[k] = hr_prev[k] = 0 ([n,c,h,w] / [n,c,scale*h,scale*w] fp32).  With window = (top, left),
+    u8 is [n,Hf,Wf,c] and the h x w picture at (top, left) of each frame is read (tg_stream_frame_in_window)."""
     _req(lr_curr, torch.float32, 'lr_curr', 4)
     _req(lr_prev, torch.float32, 'lr_prev', 4)
     _req(hr_prev, torch.float32, 'hr_prev', 4)
@@ -376,7 +396,10 @@ def stream_frame_in(u8, reset, lr_curr, lr_prev, hr_prev, scale, bgr=False):
         raise L.TecoganB200Error('stream_frame_in: lr_prev / hr_prev shape mismatch')
     if u8 is not None:
         _req(u8, torch.uint8, 'frames', 4)
-        if tuple(u8.shape) != (n, h, w, c):
+        if window is not None:
+            if u8.shape[0] != n or u8.shape[3] != c:
+                raise L.TecoganB200Error(f'stream_frame_in: frames {tuple(u8.shape)} are not [n={n},Hf,Wf,c={c}]')
+        elif tuple(u8.shape) != (n, h, w, c):
             raise L.TecoganB200Error(f'stream_frame_in: frames {tuple(u8.shape)} != {(n, h, w, c)} (nhwc)')
     if reset is not None:
         _req(reset, torch.int32, 'reset', 1)
@@ -385,6 +408,12 @@ def stream_frame_in(u8, reset, lr_curr, lr_prev, hr_prev, scale, bgr=False):
     for t in (lr_prev, hr_prev, u8, reset):
         if t is not None and t.device != lr_curr.device:
             raise L.TecoganB200Error('stream_frame_in: tensors on different devices')
+    if window is not None:
+        win = frame_window(u8.shape[1], u8.shape[2], *window) if u8 is not None else frame_window(h, w, 0, 0)
+        L.check(L.load().tg_stream_frame_in_window(_ptr(u8), ctypes.byref(win), _ptr(reset), _ptr(lr_curr),
+                                                   _ptr(lr_prev), _ptr(hr_prev), n, c, h, w, scale, int(bool(bgr)),
+                                                   _stream()), 'tg_stream_frame_in_window')
+        return lr_curr
     L.check(L.load().tg_stream_frame_in(_ptr(u8), _ptr(reset), _ptr(lr_curr), _ptr(lr_prev), _ptr(hr_prev),
                                         n, c, h, w, scale, int(bool(bgr)), _stream()), 'tg_stream_frame_in')
     return lr_curr
@@ -499,12 +528,21 @@ def yuv_coefficients(layout, color):
     return list(out)
 
 
-def stream_frame_in_yuv(frames, layout, color, reset, lr_curr, lr_prev, hr_prev, scale):
+def yuv_frame_size(layout, shape):
+    """(h, w) of a frame whose words have the 2-d shape `shape` in a YUV layout (yuv_frame_shape's inverse)."""
+    a, b = shape
+    if layout in YUV422_LAYOUTS:
+        return a, b // 2
+    return (a // 3, b) if layout in YUV444_LAYOUTS else (2 * a // 3, b)
+
+
+def stream_frame_in_yuv(frames, layout, color, reset, lr_curr, lr_prev, hr_prev, scale, window=None):
     """tg_stream_frame_in_yuv: frames [n,*yuv_frame_shape(layout, h, w)] (uint8 for the 8-bit layouts, uint16 for
     'p010' / 'i420_10' / 'i444_10'; or None) in colour `color` -> lr_curr fp32 [n,3,h,w] = RGB / 255 (8 bit) or
     RGB / 1023 (10 bit), as oracle/yuv_color.py (4:2:0) and oracle/yuv_422_444.py (4:2:2, 4:4:4) specify; reset as
-    in stream_frame_in."""
-    name = 'stream_frame_in_yuv'
+    in stream_frame_in.  With window = (top, left), frames hold Hf x Wf frames (frames.shape[1:] ==
+    yuv_frame_shape(layout, Hf, Wf)) and the h x w picture at (top, left) is read (tg_stream_frame_in_yuv_window)."""
+    name = 'stream_frame_in_yuv' if window is None else 'stream_frame_in_yuv_window'
     fmt = yuv_format(layout, color, name)
     _req(lr_curr, torch.float32, 'lr_curr', 4)
     _req(lr_prev, torch.float32, 'lr_prev', 4)
@@ -519,9 +557,10 @@ def stream_frame_in_yuv(frames, layout, color, reset, lr_curr, lr_prev, hr_prev,
         raise L.TecoganB200Error(f'{name}: lr_prev / hr_prev shape mismatch')
     if frames is not None:
         _req(frames, torch.uint16 if yuv_depth(layout) == 10 else torch.uint8, 'frames', 3)
-        want = (n, *yuv_frame_shape(layout, h, w))
+        fh, fw = (h, w) if window is None else yuv_frame_size(layout, frames.shape[1:])
+        want = (n, *yuv_frame_shape(layout, fh, fw))
         if tuple(frames.shape) != want:
-            raise L.TecoganB200Error(f'{name}: frames {tuple(frames.shape)} != {want} ({layout} frames of {h}x{w})')
+            raise L.TecoganB200Error(f'{name}: frames {tuple(frames.shape)} != {want} ({layout} frames of {fh}x{fw})')
     if reset is not None:
         _req(reset, torch.int32, 'reset', 1)
         if reset.shape[0] != n:
@@ -529,17 +568,25 @@ def stream_frame_in_yuv(frames, layout, color, reset, lr_curr, lr_prev, hr_prev,
     for t in (lr_prev, hr_prev, frames, reset):
         if t is not None and t.device != lr_curr.device:
             raise L.TecoganB200Error(f'{name}: tensors on different devices')
+    if window is not None:
+        win = frame_window(fh, fw, *window) if frames is not None else frame_window(h, w, 0, 0)
+        L.check(L.load().tg_stream_frame_in_yuv_window(_ptr(frames), ctypes.byref(fmt), ctypes.byref(win),
+                                                       _ptr(reset), _ptr(lr_curr), _ptr(lr_prev), _ptr(hr_prev), n,
+                                                       h, w, scale, _stream()), 'tg_stream_frame_in_yuv_window')
+        return lr_curr
     L.check(L.load().tg_stream_frame_in_yuv(_ptr(frames), ctypes.byref(fmt), _ptr(reset), _ptr(lr_curr),
                                             _ptr(lr_prev), _ptr(hr_prev), n, h, w, scale, _stream()),
             'tg_stream_frame_in_yuv')
     return lr_curr
 
 
-def rgb_to_yuv(layout, color, rgb_u8=None, rgb_f32=None, out=None):
+def rgb_to_yuv(layout, color, rgb_u8=None, rgb_f32=None, out=None, window=None):
     """tg_rgb_to_yuv: 8-bit layouts encode rgb_u8 (uint8 NHWC [n,H,W,3]) into uint8 [n,*yuv_frame_shape]; 10-bit
     layouts encode rgb_f32 (fp32 NCHW [n,3,H,W], quantised as clip(rint(x * 1023), 0, 1023)) into uint16
-    [n,*yuv_frame_shape] ([n,3H/2,W] for 4:2:0, [n,H,2W] for 4:2:2, [n,3H,W] for 4:4:4)."""
-    name = 'rgb_to_yuv'
+    [n,*yuv_frame_shape] ([n,3H/2,W] for 4:2:0, [n,H,2W] for 4:2:2, [n,3H,W] for 4:4:4).  With window = (top, left),
+    out holds larger Hf x Wf frames and the H x W picture is written at (top, left) of each (tg_rgb_to_yuv_window);
+    the words around it are left as they are."""
+    name = 'rgb_to_yuv' if window is None else 'rgb_to_yuv_window'
     fmt = yuv_format(layout, color, name)
     ten = yuv_depth(layout) == 10
     if ten:
@@ -558,7 +605,10 @@ def rgb_to_yuv(layout, color, rgb_u8=None, rgb_f32=None, out=None):
     if err:
         raise L.TecoganB200Error(f'{name}: {err}')
     dtype = torch.uint16 if ten else torch.uint8
-    shape = (n, *yuv_frame_shape(layout, H, W))
+    if window is not None and out is None:
+        raise L.TecoganB200Error(f'{name}: a window needs the output frames (out)')
+    fh, fw = (H, W) if window is None else yuv_frame_size(layout, out.shape[1:])
+    shape = (n, *yuv_frame_shape(layout, fh, fw))
     if out is None:
         out = torch.empty(shape, dtype=dtype, device=src.device)
     _req(out, dtype, 'out', 3)
@@ -566,9 +616,53 @@ def rgb_to_yuv(layout, color, rgb_u8=None, rgb_f32=None, out=None):
         raise L.TecoganB200Error(f'{name}: out {tuple(out.shape)} != {shape}')
     if out.device != src.device:
         raise L.TecoganB200Error(f'{name}: tensors on different devices')
+    if window is not None:
+        win = frame_window(fh, fw, *window)
+        L.check(L.load().tg_rgb_to_yuv_window(_ptr(rgb_u8), _ptr(rgb_f32), _ptr(out), ctypes.byref(fmt),
+                                              ctypes.byref(win), n, H, W, _stream()), 'tg_rgb_to_yuv_window')
+        return out
     L.check(L.load().tg_rgb_to_yuv(_ptr(rgb_u8), _ptr(rgb_f32), _ptr(out), ctypes.byref(fmt), n, H, W, _stream()),
             'tg_rgb_to_yuv')
     return out
+
+
+def fill_black(out, layout=None, color='bt601'):
+    """tg_fill_black: every word of out := the format's black.  layout None: uint8 HWC [n,Hf,Wf,c], all 0; else the
+    YUV layout's frames [n,*yuv_frame_shape(layout, Hf, Wf)] with Y = the colour's black level (16 << (depth - 8)
+    limited range, 0 full) and U = V = 128 << (depth - 8), P010 words << 6."""
+    fmt = None
+    if layout is None:
+        _req(out, torch.uint8, 'out', 4)
+        n, fh, fw, c = out.shape
+    else:
+        fmt = yuv_format(layout, color, 'fill_black')
+        _req(out, torch.uint16 if yuv_depth(layout) == 10 else torch.uint8, 'out', 3)
+        (fh, fw), n, c = yuv_frame_size(layout, out.shape[1:]), out.shape[0], 3
+        if tuple(out.shape[1:]) != yuv_frame_shape(layout, fh, fw):
+            raise L.TecoganB200Error(f'fill_black: {tuple(out.shape)} is not a stack of {layout} frames')
+    L.check(L.load().tg_fill_black(_ptr(out), ctypes.byref(fmt) if fmt is not None else None, n, c, fh, fw,
+                                   _stream()), 'tg_fill_black')
+    return out
+
+
+def luma_line_sums(frames, layout=None, bgr=False):
+    """tg_luma_line_sums: the per-row and per-column sums of the 8-bit luma of frames (uint8 HWC RGB [n,h,w,3], or a
+    YUV layout's [n,*yuv_frame_shape]) as int64 tensors rows [n,h], cols [n,w] on the frames' device."""
+    fmt = None
+    if layout is None:
+        _req(frames, torch.uint8, 'frames', 4)
+        n, h, w, c = frames.shape
+    else:
+        fmt = yuv_format(layout, 'bt601', 'luma_line_sums')
+        _req(frames, torch.uint16 if yuv_depth(layout) == 10 else torch.uint8, 'frames', 3)
+        (h, w), n, c = yuv_frame_size(layout, frames.shape[1:]), frames.shape[0], 3
+        if tuple(frames.shape[1:]) != yuv_frame_shape(layout, h, w):
+            raise L.TecoganB200Error(f'luma_line_sums: {tuple(frames.shape)} is not a stack of {layout} frames')
+    rows = torch.empty((n, h), dtype=torch.int64, device=frames.device)
+    cols = torch.empty((n, w), dtype=torch.int64, device=frames.device)
+    L.check(L.load().tg_luma_line_sums(_ptr(frames), ctypes.byref(fmt) if fmt is not None else None, int(bool(bgr)),
+                                       n, c, h, w, _ptr(rows), _ptr(cols), _stream()), 'tg_luma_line_sums')
+    return rows, cols
 
 
 RESIZE_FILTERS = ('bicubic', 'lanczos')
@@ -595,10 +689,11 @@ def resample_table(n_in, n_out, filt='bicubic'):
     return first, weights
 
 
-def resample(x, rows, cols, out_u8=None, out_f32=None):
+def resample(x, rows, cols, out_u8=None, out_f32=None, window=None):
     """tg_resample_nchw_f32: x fp32 NCHW [n,c,H,W] resized with the device tables rows = (first [Ho], weights
     [Ho, taps]) and cols = (first [Wo], weights [Wo, taps]) into exactly one of out_u8 (uint8 NHWC [n,Ho,Wo,c],
-    float32_to_uint8 of the result) or out_f32 (fp32 NCHW [n,c,Ho,Wo]).  With neither given, a new uint8 tensor."""
+    float32_to_uint8 of the result) or out_f32 (fp32 NCHW [n,c,Ho,Wo]).  With neither given, a new uint8 tensor.
+    With window = (top, left), out_u8 is [n,Hf,Wf,c] and the picture is written at (top, left) of each frame."""
     name = 'resample'
     _req(x, torch.float32, 'x', 4)
     n, c, H, W = x.shape
@@ -619,8 +714,12 @@ def resample(x, rows, cols, out_u8=None, out_f32=None):
         raise L.TecoganB200Error(f'{name}: give out_u8 or out_f32, not both')
     if out_f32 is None and out_u8 is None:
         out_u8 = torch.empty((n, Ho, Wo, c), dtype=torch.uint8, device=x.device)
+    if window is not None and out_u8 is None:
+        raise L.TecoganB200Error(f'{name}: a window applies to the uint8 output (out_u8)')
     if out_u8 is not None:
         out, want = _req(out_u8, torch.uint8, 'out_u8', 4), (n, Ho, Wo, c)
+        if window is not None:
+            want = (n, out.shape[1], out.shape[2], c)
     else:
         out, want = _req(out_f32, torch.float32, 'out_f32', 4), (n, c, Ho, Wo)
     if tuple(out.shape) != want:
@@ -628,6 +727,12 @@ def resample(x, rows, cols, out_u8=None, out_f32=None):
     if out.device != x.device:
         raise L.TecoganB200Error(f'{name}: tensors on different devices')
     (rf, rw, rt), (cf, cw, ct) = tabs
+    if window is not None:
+        win = frame_window(out.shape[1], out.shape[2], *window)
+        L.check(L.load().tg_resample_nchw_f32_window(_ptr(x), n, c, H, W, _ptr(rf), _ptr(rw), rt, _ptr(cf), _ptr(cw),
+                                                     ct, Ho, Wo, _ptr(out_u8), ctypes.byref(win), _stream()),
+                'tg_resample_nchw_f32_window')
+        return out
     L.check(L.load().tg_resample_nchw_f32(_ptr(x), n, c, H, W, _ptr(rf), _ptr(rw), rt, _ptr(cf), _ptr(cw), ct, Ho, Wo,
                                           _ptr(out_u8), _ptr(out_f32), _stream()), 'tg_resample_nchw_f32')
     return out

@@ -49,7 +49,18 @@ frames of a device loop of FRNet.step over the frames P010 decodes to.  The resi
 oracle/resample.py's float64 resize of the fp32 HR frames of a device loop of FRNet.step (equal, or 1 apart where
 x * 255 is within 1e-3 of a rounding boundary), the resized NV12 output with the BT.709 encode of the resized RGB
 output.  The YUY2, UYVY and I444 outputs are compared with oracle/yuv_422_444.py's encode of the RGB output for the
-frames each input decodes to.  Card name and power limit are read in the same run.  Writes nothing."""
+frames each input decodes to.  Card name and power limit are read in the same run.  Writes nothing.
+
+    python tools/stream_bench.py --window [--frames 64] [--reps 3]
+
+measures letterboxed video instead (one JSON line, metric hr_frames_per_sec_4xBD_letterbox_134x320_in_180x320): the
+bd4 clips as a 2.39:1 134x320 picture at row 22 of black 180x320 (16:9) frames, uint8 RGB -> RGB and NV12 -> NV12,
+k = 16 pushes of pinned frames, three arms alternating in every rep:
+  uncropped       today's path: the whole 180x320 frame through the net (-> 720x1280)
+  crop_out_frame  crop=(22, 0, 134, 320), out_frame=(720, 1280): the picture through the net, placed in black
+  precropped      a plain 134x320 stream over frames cropped on the host (-> 536x1280)
+with crop_out_frame's output checked against precropped's placed into the black frame (oracle/frame_window.py), and
+the kernel times of the windowed frame input and output writers next to the plain ones (CUDA events over graphs)."""
 import argparse
 import json
 import os
@@ -75,9 +86,12 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--frames', type=int, default=64)
     ap.add_argument('--reps', type=int, default=3)
+    ap.add_argument('--window', action='store_true', help='the letterboxed-video arms instead')
     args = ap.parse_args()
     if args.frames < 60:
         ap.error('--frames must be >= 60')
+    if args.window:
+        return window_bench(args)
     import numpy as np
     import torch
     import bench
@@ -377,6 +391,112 @@ def main():
         'launches_per_step': {'infer_sequence': T.engine.get_engine(net, n, c, h, w, dev).launches_per_step,
                               'push': stream_launches, 'push_nv12': nv12_launches, 'push_p010': p010_launches,
                               'push_resize': resize_launches, 'push_scene': scene_launches},
+    }
+    print(json.dumps(line), flush=True)
+
+
+def window_bench(args):
+    import numpy as np
+    import torch
+    import bench
+    import tecogan_b200 as T
+    from oracle import frame_window as FW
+    from oracle import yuv_oracle as Y
+    ops = sys.modules['tecogan-pytorch_b200.ops']
+    assert torch.cuda.is_available(), 'stream_bench.py needs a GPU'
+    dev = torch.device('cuda', 0)
+    torch.cuda.set_device(dev)
+    bench.select_workload('bd4')
+    n, (c, h, w), s = bench.CLIPS_PER_GPU, bench.LR, bench.SCALE
+    t, chunk = args.frames, 16
+    Hf, top = 180, 22                      # 134 x 320 (2.39:1) at row 22 of 180 x 320 (16:9)
+    box = (top, 0, h, w)
+    net = T.FRNet(3, 3, 64, 10, 'BD', s)
+    net.load_state_dict(bench.make_params(), strict=True)
+    net = net.to(dev).eval()
+    clips = bench.synthetic_clips(n, t, seed=100).numpy()
+    pic = np.ascontiguousarray(np.rint(clips * 255.0).astype(np.uint8).transpose(0, 1, 3, 4, 2))   # [n,t,h,w,c]
+    full = np.zeros((n, t, Hf, w, c), np.uint8)
+    full[:, :, top:top + h] = pic
+    src = {'uint8': (full, pic), 'nv12': (Y.rgb_to_yuv420(full, 'nv12'), None)}
+    src['nv12'] = (src['nv12'][0], np.stack([np.stack([FW.crop_words(f, 'nv12', *box) for f in clip])
+                                             for clip in src['nv12'][0]]))
+    arms, opened, runs, outputs = {}, {}, {}, {}
+    for fmt, (whole, cropped) in src.items():
+        kw = dict(input=fmt, out_format='rgb' if fmt == 'uint8' else 'nv12')
+        pins = torch.from_numpy(whole).pin_memory(), torch.from_numpy(np.ascontiguousarray(cropped)).pin_memory()
+        arms[f'{fmt}_uncropped'] = (net.stream(n, Hf, w, device=dev, **kw), pins[0])
+        arms[f'{fmt}_crop_out_frame'] = (net.stream(n, Hf, w, device=dev, crop=box, out_frame=(s * Hf, s * w), **kw),
+                                         pins[0])
+        arms[f'{fmt}_precropped'] = (net.stream(n, h, w, device=dev, **kw), pins[1])
+    for k in arms:
+        runs[k] = []
+    for rep in range(args.reps + 1):                 # rep 0: untimed warm-up (graph capture, pinned blocks)
+        for k, (st, frames) in arms.items():
+            st.reset(range(n))
+            outputs[k] = None
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            outputs[k] = [st.push(frames[:, i:i + chunk]) for i in range(0, t, chunk)]
+            torch.cuda.synchronize()
+            if rep:
+                runs[k].append(n * t / (time.perf_counter() - t0))
+    identical = {}
+    for fmt in src:
+        got = np.concatenate(outputs[f'{fmt}_crop_out_frame'], 1)
+        ref = np.concatenate(outputs[f'{fmt}_precropped'], 1)
+        lay = 'rgb' if fmt == 'uint8' else 'nv12'
+        y, x = arms[f'{fmt}_crop_out_frame'][0].out_origin
+        identical[fmt] = all(np.array_equal(got[j, i], FW.place_words(ref[j, i], lay, 'bt601', s * Hf, s * w, y, x))
+                             for j in range(n) for i in range(t))
+    launches = {k: st._engine.launches_per_step for k, (st, _) in arms.items()}
+    for st, _ in arms.values():
+        st.close()
+
+    # the windowed kernels next to the plain ones: 8 rotating buffer sets, 60 launches per graph
+    nb, reps = 8, 60
+    H, W = s * h, s * w
+    lrs = [torch.empty(n, c, h, w, device=dev) for _ in range(nb)]
+    prev, hrp = torch.empty(n, c, h, w, device=dev), torch.empty(n, c, H, W, device=dev)
+    rgb_full = [torch.randint(0, 256, (n, Hf, w, c), dtype=torch.uint8, device=dev) for _ in range(nb)]
+    rgb_pic = [torch.randint(0, 256, (n, h, w, c), dtype=torch.uint8, device=dev) for _ in range(nb)]
+    nv_full = [torch.randint(0, 256, (n, 3 * Hf // 2, w), dtype=torch.uint8, device=dev) for _ in range(nb)]
+    nv_pic = [torch.randint(0, 256, (n, 3 * h // 2, w), dtype=torch.uint8, device=dev) for _ in range(nb)]
+    us = {}
+    timings = {
+        'decode_u8_plain': lambda i: ops.stream_frame_in(rgb_pic[i], None, lrs[i], prev, hrp, s),
+        'decode_u8_window': lambda i: ops.stream_frame_in(rgb_full[i], None, lrs[i], prev, hrp, s, window=(top, 0)),
+        'decode_nv12_plain': lambda i: ops.stream_frame_in_yuv420(nv_pic[i], 'nv12', None, lrs[i], prev, hrp, s),
+        'decode_nv12_window': lambda i: ops.stream_frame_in_yuv(nv_full[i], 'nv12', 'bt601', None, lrs[i], prev, hrp,
+                                                                s, window=(top, 0)),
+    }
+    for k, fn in timings.items():
+        us[k] = bench._time_graph(fn, nb, reps, torch) * 1e6
+    del rgb_full, rgb_pic, nv_full, nv_pic
+    hrs = [torch.rand(n, c, H, W, device=dev) for _ in range(nb)]
+    u8s = [torch.empty(n, H, W, c, dtype=torch.uint8, device=dev) for _ in range(nb)]
+    pads = [torch.empty(n, s * Hf, W, c, dtype=torch.uint8, device=dev) for _ in range(nb)]
+    nvs = [torch.empty(n, 3 * H // 2, W, dtype=torch.uint8, device=dev) for _ in range(nb)]
+    nv_pads = [torch.empty(n, 3 * s * Hf // 2, W, dtype=torch.uint8, device=dev) for _ in range(nb)]
+    y0 = (s * Hf - H) // 2 // 2 * 2
+    timings = {
+        'to_uint8_plain': lambda i: ops.float_to_uint8_nhwc(hrs[i], u8s[i]),
+        'to_uint8_window': lambda i: ops.float_to_uint8_nhwc_window(hrs[i], pads[i], (y0, 0)),
+        'encode_nv12_plain': lambda i: ops.rgb_u8_to_yuv420(u8s[i], 'nv12', out=nvs[i]),
+        'encode_nv12_window': lambda i: ops.rgb_to_yuv('nv12', 'bt601', rgb_u8=u8s[i], out=nv_pads[i],
+                                                       window=(y0, 0)),
+    }
+    for k, fn in timings.items():
+        us[k] = bench._time_graph(fn, nb, reps, torch) * 1e6
+    line = {
+        'metric': 'hr_frames_per_sec_4xBD_letterbox_134x320_in_180x320', 'unit': 'frames/s',
+        'device': torch.cuda.get_device_name(0), 'power_limit_w': power_limit_w(),
+        'clips': n, 'frames_per_clip': t, 'chunk': chunk, 'reps': args.reps,
+        'results': {k: {'median': statistics.median(v), 'min': min(v), 'max': max(v), 'runs': v}
+                    for k, v in runs.items()},
+        'crop_out_frame_identical_to_precropped_placed': identical,
+        'launches_per_step': launches,
+        'kernel_us': us,
     }
     print(json.dumps(line), flush=True)
 
