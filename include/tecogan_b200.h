@@ -236,6 +236,25 @@ int tg_float_to_uint8_nhwc_window(const float* x, uint8_t* y, const struct tg_fr
  * on the device, so one captured launch serves every pattern of resets. */
 int tg_stream_frame_in(const uint8_t* in_u8, const int32_t* reset, float* lr_curr, float* lr_prev,
                        float* hr_prev, int n, int c, int h, int w, int s, int bgr, void* stream);
+/* Step input of a temporally padded stream, assembled from a ring of decoded frames (FRNet.stream(pad_front=p)).
+ * ring   : fp32 [depth, n, c, h, w], frames decoded ahead of the step (tg_stream_frame_in into ring positions)
+ * table  : int32 [3n] in device memory, read on the device (one captured launch serves every schedule):
+ *          cur[k] = table[k], mode[k] = table[n + k], prev[k] = table[2n + k]
+ *   cur[k] in [0, depth): lr_curr[k] = ring[cur[k]][k]; any other value leaves lr_curr[k] untouched
+ *   mode[k] == TG_GATHER_ZERO: lr_prev[k] = hr_prev[k] = 0 (tg_stream_frame_in's reset)
+ *   mode[k] == TG_GATHER_LOAD: lr_prev[k] = ring[prev[k]][k] (0 when prev[k] lies outside [0, depth)) and
+ *                              hr_prev[k] = warm_hr[k]; with warm_hr NULL the slot is kept
+ *   any other mode (TG_GATHER_KEEP): lr_prev[k] and hr_prev[k] are not touched (one read of mode[k])
+ * warm_hr: fp32 [n, c, s*h, s*w] (the warm-up steps' HR state), or NULL.  The outputs must not overlap the ring or
+ * warm_hr.  Exact copies: no arithmetic, so the result does not depend on the grid.  Pointers 4-byte aligned; 16-byte
+ * vectors wherever source and destination share their alignment.
+ * TG_E_INVALID: null pointers (warm_hr aside), non-positive sizes, misalignment; TG_E_UNSUPPORTED: s not 2 or 4, a
+ * grid too large. */
+#define TG_GATHER_KEEP 0
+#define TG_GATHER_ZERO 1
+#define TG_GATHER_LOAD 2
+int tg_stream_gather(const float* ring, int depth, const int32_t* table, const float* warm_hr, float* lr_curr,
+                     float* lr_prev, float* hr_prev, int n, int c, int h, int w, int s, void* stream);
 /* The same step input from YUV 4:2:0 frames, as video decoders produce them (BT.601 limited range).
  * in    : uint8 [n, 3h/2, w], each frame the h x w Y plane followed by the interleaved (h/2) x w UV plane
  *         (nv12 != 0) or by the (h/2) x (w/2) U and V planes (nv12 == 0: I420 / yuv420p), or NULL

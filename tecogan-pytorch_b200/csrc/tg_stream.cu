@@ -811,7 +811,89 @@ int rgb_to_yuv(const char* name, const uint8_t* rgb_u8, const float* rgb_f32, vo
   });
 }
 
+// copy floats [0, count) of src to dst (4-byte aligned, not overlapping): 16-byte vectors over the interior when
+// both share their alignment mod 16, else one float at a time.  `worker` of `workers` threads.
+__device__ __forceinline__ void copy_range(float* __restrict__ dst, const float* __restrict__ src, size_t count,
+                                           size_t worker, size_t workers) {
+  if ((((uintptr_t)dst ^ (uintptr_t)src) & 15u) != 0) {
+    for (size_t i = worker; i < count; i += workers) dst[i] = __ldg(src + i);
+    return;
+  }
+  size_t head = ((16u - ((uintptr_t)dst & 15u)) & 15u) / 4u;
+  if (head > count) head = count;
+  const size_t n4 = (count - head) / 4;
+  const size_t tail0 = head + n4 * 4;
+  const float4* s4 = reinterpret_cast<const float4*>(src + head);
+  float4* d4 = reinterpret_cast<float4*>(dst + head);
+  for (size_t i = worker; i < n4; i += workers) d4[i] = __ldg(s4 + i);
+  if (worker < head) dst[worker] = __ldg(src + worker);
+  if (worker < count - tail0) dst[tail0 + worker] = __ldg(src + tail0 + worker);
+}
+
+// blockIdx.x < n * cpc: cpc CTAs per slot copy a strided share of its current frame out of the ring; the rest: zpc
+// CTAs per slot apply its state mode (a keep-slot's CTAs read mode[k] and return)
+__global__ void __launch_bounds__(kThreads)
+stream_gather_kernel(const float* __restrict__ ring, int depth, const int32_t* __restrict__ table,
+                     const float* __restrict__ warm_hr, float* __restrict__ lr_curr, float* __restrict__ lr_prev,
+                     float* __restrict__ hr_prev, int n, size_t nlr, size_t nhr, int cpc, int zpc) {
+  // the table is written, and lr_curr / lr_prev / hr_prev read, by work ordered before this launch
+  tg_pdl_wait();
+  tg_pdl_trigger();
+  const int t = threadIdx.x, b = blockIdx.x;
+  const size_t frame = (size_t)n * nlr;          // one ring position
+  if (b < n * cpc) {
+    const int slot = b / cpc, part = b - slot * cpc;
+    const int cur = __ldg(table + slot);
+    if (cur < 0 || cur >= depth) return;
+    copy_range(lr_curr + slot * nlr, ring + cur * frame + slot * nlr, nlr, (size_t)part * kThreads + t,
+               (size_t)cpc * kThreads);
+    return;
+  }
+  const int rb = b - n * cpc;
+  const int slot = rb / zpc, part = rb - slot * zpc;
+  const int mode = __ldg(table + n + slot);
+  if (mode != TG_GATHER_ZERO && (mode != TG_GATHER_LOAD || warm_hr == nullptr)) return;
+  const size_t worker = (size_t)part * kThreads + t, workers = (size_t)zpc * kThreads;
+  const int prev = mode == TG_GATHER_LOAD ? __ldg(table + 2 * n + slot) : -1;
+  if (prev < 0 || prev >= depth)
+    zero_range(lr_prev + slot * nlr, nlr, worker, workers);
+  else
+    copy_range(lr_prev + slot * nlr, ring + prev * frame + slot * nlr, nlr, worker, workers);
+  if (mode == TG_GATHER_ZERO)
+    zero_range(hr_prev + slot * nhr, nhr, worker, workers);
+  else
+    copy_range(hr_prev + slot * nhr, warm_hr + slot * nhr, nhr, worker, workers);
+}
+
+// CTAs per slot for `count` floats: one per 8 float4 vectors of each thread, at most 64
+inline int ctas_per_slot(size_t count) {
+  const size_t v = count / 4 / (kThreads * 8) + 1;
+  return (int)(v < 64 ? v : 64);
+}
+
 }  // namespace
+
+extern "C" int tg_stream_gather(const float* ring, int depth, const int32_t* table, const float* warm_hr,
+                                float* lr_curr, float* lr_prev, float* hr_prev, int n, int c, int h, int w, int s,
+                                void* stream) {
+  const char* name = "stream_gather";
+  TG_REQUIRE(ring && table && lr_curr && lr_prev && hr_prev, TG_E_INVALID,
+             "%s: null pointer (ring / table / lr_curr / lr_prev / hr_prev)", name);
+  TG_REQUIRE(depth > 0 && n > 0 && c > 0 && h > 0 && w > 0, TG_E_INVALID, "%s: bad size depth=%d n=%d c=%d h=%d w=%d",
+             name, depth, n, c, h, w);
+  TG_REQUIRE(s == 2 || s == 4, TG_E_UNSUPPORTED, "%s: scale %d (2 or 4)", name, s);
+  TG_REQUIRE((((uintptr_t)ring | (uintptr_t)table | (uintptr_t)warm_hr | (uintptr_t)lr_curr | (uintptr_t)lr_prev |
+               (uintptr_t)hr_prev) & 3u) == 0,
+             TG_E_INVALID, "%s: buffers must be 4-byte aligned", name);
+  const size_t nlr = (size_t)c * h * w, nhr = nlr * s * s;
+  const int cpc = ctas_per_slot(nlr), zpc = ctas_per_slot(nhr);
+  const size_t ctas = (size_t)(cpc + zpc) * n;
+  TG_REQUIRE(ctas <= 0x7fffffff, TG_E_UNSUPPORTED, "%s: grid too large", name);
+  tg_launch(stream_gather_kernel, dim3((unsigned)ctas), dim3(kThreads), 0, (cudaStream_t)stream, ring, depth, table,
+            warm_hr, lr_curr, lr_prev, hr_prev, n, nlr, nhr, cpc, zpc);
+  TG_CUDA_LAUNCH_CHECK(name);
+  return TG_OK;
+}
 
 extern "C" int tg_stream_frame_in(const uint8_t* in_u8, const int32_t* reset, float* lr_curr, float* lr_prev,
                                   float* hr_prev, int n, int c, int h, int w, int s, int bgr, void* stream) {

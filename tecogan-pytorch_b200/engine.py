@@ -324,23 +324,30 @@ class StreamEngine(ClipEngine):
         self._report_dev = self._report_host = None
 
     def _enqueue(self, p):
-        crop = self.crop[2:] if self.crop else None          # (top, left)
-        pad = self.out_frame[2:] if self.out_frame else None  # (y, x)
-        if self.yuv_in in YUV420 and self.in_color == 'bt601' and crop is None:
-            ops.stream_frame_in_yuv420(self.inp[p], self.yuv_in, self.mask[p], self.lr[p], self.lr[p ^ 1],
-                                       self.hr[p ^ 1], self.net.scale)
-        elif self.yuv_in:
-            # the windowed entry point has no BT.601-only twin: its bt601 row is the same cv2 conversion
-            ops.stream_frame_in_yuv(self.inp[p], self.yuv_in, self.in_color, self.mask[p], self.lr[p],
-                                    self.lr[p ^ 1], self.hr[p ^ 1], self.net.scale, window=crop)
-        else:
-            ops.stream_frame_in(self.inp[p] if self.u8_input else None, self.mask[p], self.lr[p], self.lr[p ^ 1],
-                                self.hr[p ^ 1], self.net.scale, self.bgr, window=crop if self.u8_input else None)
+        self._decode(self.inp[p] if self.u8_input else None, self.mask[p], self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1])
         if self.scene_cut is not None:
             ops.scene_cut(self.lr[p], self.lr[p ^ 1], self.mask[p], self.scene_cut, self.prev_mafd, self.work,
                           self.score[p], self.cut[p])
             # a detected cut restarts the slot: the reset-only frame input with cut[p] as its mask
             ops.stream_frame_in(None, self.cut[p], self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1], self.net.scale)
+        self._step_out(p)
+
+    def _decode(self, inp, mask, lr_curr, lr_prev, hr_prev):
+        """The frame input launch: inp (None for fp32 input) decoded into lr_curr, the slots of mask reset."""
+        crop = self.crop[2:] if self.crop else None          # (top, left)
+        if self.yuv_in in YUV420 and self.in_color == 'bt601' and crop is None:
+            ops.stream_frame_in_yuv420(inp, self.yuv_in, mask, lr_curr, lr_prev, hr_prev, self.net.scale)
+        elif self.yuv_in:
+            # the windowed entry point has no BT.601-only twin: its bt601 row is the same cv2 conversion
+            ops.stream_frame_in_yuv(inp, self.yuv_in, self.in_color, mask, lr_curr, lr_prev, hr_prev, self.net.scale,
+                                    window=crop)
+        else:
+            ops.stream_frame_in(inp, mask, lr_curr, lr_prev, hr_prev, self.net.scale, self.bgr,
+                                window=crop if self.u8_input else None)
+
+    def _step_out(self, p):
+        """The step of parity p on lr[p], lr[p ^ 1], hr[p ^ 1] and the writes of its output frame."""
+        pad = self.out_frame[2:] if self.out_frame else None  # (y, x)
         if self.out_size is None and self.pad is not None:
             # the picture goes straight into the padded frame: the windowed writer replaces the step's uint8 output
             self.net.step_into(self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1], self.hr[p], out_u8=None)
@@ -376,32 +383,42 @@ class StreamEngine(ClipEngine):
             self.mask[p].zero_()
             self.mask_set[p] = False
 
-    def run(self, frames, reset_slots, out_host):
+    def _res(self):
+        """What the step graph leaves for the copy out, per parity."""
+        return self.yuv if self.yuv_out else self.pad if self.pad else self.rs if self.out_size else self.u8
+
+    def _outputs(self, k, out_host):
+        """The k frames a call returns (pinned host or device) and the [k,3n] report rows (scene_cut) or None."""
+        n, res = self.n, self._res()
+        shape = (n, k, *res[0].shape[1:])
+        if out_host:
+            out = torch.empty(shape, dtype=res[0].dtype, pin_memory=True)
+        else:
+            out = torch.empty(shape, dtype=res[0].dtype, device=self.device)
+        report = None
+        if self.scene_cut is not None:
+            # kept between pushes (read on the current stream, which the next push's streams wait for)
+            if self._report_dev is None or self._report_dev.shape[0] < k:
+                self._report_dev = torch.empty((max(k, 16), 3 * n), dtype=torch.int32, device=self.device)
+            report = self._report_dev[:k]
+        return out, report
+
+    def run(self, frames, reset_slots, out_host, flush=False):
         """frames: uint8 [n,k,h,w,c] (u8_input), uint8 / uint16 [n,k,*yuv_frame_shape] (yuv_in) or fp32
         [n,k,c,h,w], each
-        frame contiguous, pinned host or on this device.
+        frame contiguous, pinned host or on this device; None for no frames.
         Slots in `reset_slots` start a new video at frame 0.  Returns uint8 [n,k,H,W,c] (or [n,k,3H/2,W] words with
         yuv_out; Ho, Wo instead of H, W with out_size): a pinned host tensor (out_host; one synchronisation, at the end) or a new tensor on the device,
-        ordered on the current stream (no synchronisation)."""
-        n, k = self.n, frames.shape[1]
+        ordered on the current stream (no synchronisation).  flush: the videos end here (this engine holds no
+        frames, so it changes nothing)."""
+        n, k = self.n, 0 if frames is None else frames.shape[1]
         with torch.cuda.device(self.device):
             cur = torch.cuda.current_stream()
             self.net.refresh_packed_weights()        # a load_state_dict between pushes takes effect
             for st in (self.main, self.h2d, self.d2h):
                 st.wait_stream(cur)
-            # what the step graph leaves for the copy out
-            res = self.yuv if self.yuv_out else self.pad if self.pad else self.rs if self.out_size else self.u8
-            shape = (n, k, *res[0].shape[1:])
-            if out_host:
-                out = torch.empty(shape, dtype=res[0].dtype, pin_memory=True)
-            else:
-                out = torch.empty(shape, dtype=res[0].dtype, device=self.device)
-            report = None
-            if self.scene_cut is not None:
-                # kept between pushes (read on the current stream, which the next push's streams wait for)
-                if self._report_dev is None or self._report_dev.shape[0] < k:
-                    self._report_dev = torch.empty((max(k, 16), 3 * n), dtype=torch.int32, device=self.device)
-                report = self._report_dev[:k]
+            res = self._res()
+            out, report = self._outputs(k, out_host)
             if not self.u8_input and self.stage is None:
                 self.stage = [torch.empty_like(self.lr[0]) for _ in range(2)]
             dst = self.inp if self.u8_input else self.stage
@@ -437,19 +454,323 @@ class StreamEngine(ClipEngine):
                         self.out_copied[p] = torch.cuda.Event()
                         self.out_copied[p].record(self.d2h)
                 self.parity ^= 1
-            if out_host:
-                if report is not None:       # the D2H stream has waited on the last replay's event
-                    if self._report_host is None or self._report_host.shape[0] < k:
-                        self._report_host = torch.empty(self._report_dev.shape, dtype=torch.int32, pin_memory=True)
-                    with torch.cuda.stream(self.d2h):
-                        self._report_host[:k].copy_(report, non_blocking=True)
-                    report = self._report_host[:k]
-                self.d2h.synchronize()   # after every replay (D2H waited on each) and so after every H2D
-            else:
-                cur.wait_stream(self.main)
-                cur.wait_stream(self.h2d)    # a device input may be freed once the call returns
+            report = self._finish(cur, report, k, out_host)
         self.report = report
         return out
+
+    def _finish(self, cur, report, k, out_host):
+        """End of a call: host output -> the report copied to the host and one synchronisation; device output -> the
+        current stream waits for the work of the call.  Returns the report as the caller reads it."""
+        if out_host:
+            if report is not None:       # the D2H stream has waited on the last replay's event
+                if self._report_host is None or self._report_host.shape[0] < k:
+                    self._report_host = torch.empty(self._report_dev.shape, dtype=torch.int32, pin_memory=True)
+                with torch.cuda.stream(self.d2h):
+                    self.d2h.wait_stream(self.main)
+                    self._report_host[:k].copy_(report, non_blocking=True)
+                report = self._report_host[:k]
+            self.d2h.synchronize()   # after every replay (D2H waited on each) and so after every H2D
+        else:
+            cur.wait_stream(self.main)
+            cur.wait_stream(self.h2d)    # a device input may be freed once the call returns
+        return report
+
+
+# ------------------------------------------------------------------------------------------ temporal padding
+PAD_MODES = ('reflect', 'replicate')
+MAX_PAD_FRONT = 32                # bounds the ring: pad_front + 2 decoded LR frames per slot
+KEEP, ZERO, LOAD = ops.L.GATHER_KEEP, ops.L.GATHER_ZERO, ops.L.GATHER_LOAD
+
+
+def pad_count(p, mode, length):
+    """Pad frames in front of a shot of `length` frames: reflect min(p, length - 1) (the reference asserts
+    p < length; the stream pads with the longest reflection the shot has), replicate p."""
+    return min(p, length - 1) if mode == 'reflect' else p
+
+
+def shot_lengths(j, starts, end, p):
+    """Per slot: None when frame j continues a shot, else the length of the shot that starts at j, capped at p + 1.
+    starts: per slot the set of frames that start a shot, known up to j + p; end: the frame count when the videos
+    end before j + p + 1 (a flush), else None."""
+    out = []
+    for b in starts:
+        if j not in b:
+            out.append(None)
+            continue
+        length = p + 1
+        for i in range(1, p + 1):
+            if j + i in b or (end is not None and j + i >= end):
+                length = i
+                break
+        out.append(length)
+    return out
+
+
+def plan_step(j, lengths, p, mode):
+    """The warm-up steps and the main step that produce lock-stepped frame j of a stream padded as
+    BaseModel.pad_sequence pads each shot (base_model.py:230-251).  lengths: shot_lengths(j, ...).
+    -> (warm, main):
+      warm: the warm-up steps in order, each a per-slot list of (cur, mode): cur the frame read as lr_curr (None:
+            nothing is read), mode ZERO at the slot's first warm-up step (zero state, as frame 0 of infer_sequence),
+            else KEEP.  A shot with q pad frames runs q steps over its pad frames (reflect: j+q, ..., j+1; replicate:
+            j, ..., j), ending on the last step of the list: slots that start a shot at j share the steps.
+      main: per slot (j, mode, prev): KEEP continues the shot; ZERO starts it cold (no pad frame); LOAD starts it from
+            the warm-up: hr_prev is the warm-up's last HR frame and lr_prev is frame prev (its last pad frame)."""
+    qs = [None if length is None else pad_count(p, mode, length) for length in lengths]
+    qmax = max([q for q in qs if q] or [0])
+    warm = [[(None, KEEP)] * len(qs) for _ in range(qmax)]
+    main = []
+    for k, q in enumerate(qs):
+        if q is None:
+            main.append((j, KEEP, None))
+        elif q == 0:
+            main.append((j, ZERO, None))
+        else:
+            for m in range(q):
+                warm[qmax - q + m][k] = (j + q - m if mode == 'reflect' else j, ZERO if m == 0 else KEEP)
+            main.append((j, LOAD, j + 1 if mode == 'reflect' else j))
+    return warm, main
+
+
+def plan(starts, frames, p, mode):
+    """The whole schedule of `frames` lock-stepped frames whose shots start at `starts` (per slot, a set of frames;
+    frame 0 starts every slot's first shot) and end with the stream: [plan_step(j, ...) for j in range(frames)]."""
+    starts = [set(b) | {0} for b in starts]
+    return [plan_step(j, shot_lengths(j, starts, frames, p), p, mode) for j in range(frames)]
+
+
+class PadSchedule:
+    """The host's plan of a padded stream of n lock-stepped slots: the shot starts seen so far, the next frame to
+    ingest (t_in) and to produce (t_out).  Pure Python; PaddedStreamEngine calls, per push: start(reset slots), then
+    per frame ingest(cut slots) and next() while ready(); per flush: next(flush=True) while ready(flush=True), then
+    restart()."""
+
+    def __init__(self, n, p, mode):
+        self.n, self.p, self.mode = n, p, mode
+        self.lag = p if mode == 'reflect' else 0
+        self.t_in = self.t_out = 0
+        self.starts = [set() for _ in range(n)]      # per slot, the frames not yet produced that start a shot
+
+    def start(self, slots):
+        """`slots` start a new video at the next frame ingested (the caller's resets)."""
+        for k in slots:
+            self.starts[k].add(self.t_in)
+
+    def ingest(self, cut_slots=()):
+        """Frame t_in is in the ring; `cut_slots` detected a scene cut at it."""
+        self.start(cut_slots)
+        self.t_in += 1
+
+    def ready(self, flush=False):
+        """Frame t_out can be produced: frames up to t_out + lag are ingested, or the videos end (flush)."""
+        return self.t_out < self.t_in - (0 if flush else self.lag)
+
+    def next(self, flush=False):
+        """-> (j, warm, main) of frame j = t_out (plan_step), which the caller then produces."""
+        j = self.t_out
+        warm, main = plan_step(j, shot_lengths(j, self.starts, self.t_in if flush else None, self.p), self.p,
+                               self.mode)
+        self.t_out += 1
+        for b in self.starts:                          # frames before t_out never start a planned shot again
+            b.discard(j)
+        return j, warm, main
+
+    def restart(self):
+        """After a flush: every slot starts a new video at the next frame."""
+        assert self.t_out == self.t_in
+        self.start(range(self.n))
+
+
+class PaddedStreamEngine(StreamEngine):
+    """StreamEngine for a stream padded at every shot start (FRNet.stream(pad_front=p)).
+
+    Ingest: each pushed frame t is decoded (the frame-input launch, no reset) into ring[t % depth], a device ring of
+    depth = p + 2 fp32 LR frames [depth,n,c,h,w], and with scene_cut scored against ring[(t-1) % depth] on the ingest
+    stream; the cut flags go to pinned host memory, and the host reads them from there.  The caller's resets and
+    the cuts are the shot starts of each slot.
+
+    Frame j is produced once frames up to j + lag (lag = p for 'reflect', 0 for 'replicate') are ingested, or the
+    videos end (flush): plan_step gives its warm-up steps -- batch-n graphs on their own state wlr / whr, each starting
+    with tg_stream_gather of the table wtab[q] -- and its main step, the main graph of parity p: tg_stream_gather of
+    mtab[p] (lr[p] = ring[j % depth]; per slot keep, zero, or load lr_prev from the ring and hr_prev from whr[0]), the
+    unchanged net.step_into and the output writes of StreamEngine.  The tables are int32 [3n] in device memory,
+    written by one H2D copy before each replay, so the four captured graphs serve every schedule."""
+
+    def __init__(self, net, n, c, h, w, device, pad_front, padding_mode, **kw):
+        dev = torch.device(device)
+        self.sched = PadSchedule(n, pad_front, padding_mode)
+        self.depth = pad_front + 2
+        H, W = net.scale * h, net.scale * w
+        self.ring = torch.zeros((self.depth, n, c, h, w), device=dev)
+        self.wlr = [torch.zeros(n, c, h, w, device=dev) for _ in range(2)]
+        self.whr = [torch.zeros(n, c, H, W, device=dev) for _ in range(2)]
+        idle = torch.tensor([-1] * n + [KEEP] * n + [-1] * n, dtype=torch.int32)
+        self.mtab = [idle.to(dev) for _ in range(2)]
+        self.wtab = [idle.to(dev) for _ in range(2)]
+        self.warm_graphs = [None, None]
+        self.ingest = torch.cuda.Stream(device=dev)
+        self.ring_free = [None] * self.depth         # event: the main step that last read ring[r] finished
+        self.ingested = None                         # event: the latest ingest finished
+        self.rep_ring = self.cut_host = self.in_mask = None
+        if kw.get('scene_cut') is not None:
+            # per ring position the frame's report: [0,2n) the float64 scores, [2n,3n) the cut flags; rows of 4n words
+            # keep every row's scores 8-byte aligned
+            self.rep_ring = torch.zeros((self.depth, 4 * n), dtype=torch.int32, device=dev)
+            self.cut_host = torch.zeros((self.depth, n), dtype=torch.int32, pin_memory=True)
+            self.in_mask = torch.zeros(n, dtype=torch.int32, device=dev)
+        super().__init__(net, n, c, h, w, dev, **kw)
+
+    def close(self):
+        super().close()
+        self.ring = self.rep_ring = self.cut_host = self.in_mask = None
+        self.wlr = self.whr = self.mtab = self.wtab = []
+        self.warm_graphs = [None, None]
+
+    def _enqueue(self, p):
+        ops.stream_gather(self.ring, self.mtab[p], self.whr[0], self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1],
+                          self.net.scale)
+        self._step_out(p)
+
+    def _enqueue_warm(self, q):
+        ops.stream_gather(self.ring, self.wtab[q], None, self.wlr[q], self.wlr[q ^ 1], self.whr[q ^ 1], self.net.scale)
+        self.net.step_into(self.wlr[q], self.wlr[q ^ 1], self.whr[q ^ 1], self.whr[q], out_u8=None)
+
+    def _capture(self):
+        super()._capture()
+        with torch.cuda.device(self.device):
+            warm = torch.cuda.Stream(device=self.device)
+            warm.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(warm):
+                for q in (0, 1):
+                    self._enqueue_warm(q)
+            torch.cuda.current_stream().wait_stream(warm)
+            torch.cuda.synchronize(self.device)
+            for q in (0, 1):
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g, pool=self.graphs[1].pool()):
+                    self._enqueue_warm(q)
+                self.warm_graphs[q] = g
+
+    def run_warm(self, q):
+        if self.warm_graphs[q] is not None:
+            self.warm_graphs[q].replay()
+        else:
+            self._enqueue_warm(q)
+
+    def _load_table(self, tab, rows):
+        """On the current stream: tab = cur + mode + prev of rows [(cur, mode, prev)] (frames -> ring positions)."""
+        pos = lambda f: -1 if f is None else f % self.depth          # noqa: E731
+        vals = [pos(r[0]) for r in rows] + [r[1] for r in rows] + [pos(r[2] if len(r) > 2 else None) for r in rows]
+        tab.copy_(torch.tensor(vals, dtype=torch.int32).pin_memory(), non_blocking=True)
+
+    def run(self, frames, reset_slots, out_host, flush=False):
+        """StreamEngine.run with padding: returns the frames that are complete after this call's frames are ingested,
+        [n,k_out,...], k_out = the frames up to lag behind the last ingested one (flush: all of them); the report
+        rows (scene_cut) are those of the returned frames."""
+        sched, k = self.sched, 0 if frames is None else frames.shape[1]
+        end = sched.t_in + k
+        k_out = max(0, (end if flush else end - sched.lag) - sched.t_out)
+        with torch.cuda.device(self.device):
+            cur = torch.cuda.current_stream()
+            self.net.refresh_packed_weights()
+            for st in (self.main, self.h2d, self.d2h, self.ingest):
+                st.wait_stream(cur)
+            out, report = self._outputs(k_out, out_host)
+            sched.start(reset_slots)
+            row = 0
+            for i in range(k):
+                self._ingest(frames, i, reset_slots if i == 0 else ())
+                while sched.ready():
+                    self._emit(row, out, report, out_host, *sched.next())
+                    row += 1
+            while flush and sched.ready(flush=True):
+                self._emit(row, out, report, out_host, *sched.next(flush=True))
+                row += 1
+            if flush:
+                sched.restart()
+            assert row == k_out
+            if out_host:
+                self.ingest.synchronize()              # the H2D of the frames held for later steps too
+            else:
+                cur.wait_stream(self.ingest)
+            report = self._finish(cur, report, k_out, out_host)
+        self.report = report
+        return out
+
+    def _ingest(self, frames, i, reset_slots):
+        t, n = self.sched.t_in, self.n
+        r = t % self.depth
+        q = t & 1                                      # staging buffer of uint8 / YUV input
+        with torch.cuda.stream(self.h2d):
+            if self.u8_input:
+                if self.in_free[q] is not None:
+                    self.h2d.wait_event(self.in_free[q])
+                dst = self.inp[q]
+            else:                                      # fp32 frames land in the ring directly
+                if self.ring_free[r] is not None:
+                    self.h2d.wait_event(self.ring_free[r])
+                dst = self.ring[r]
+            for j in range(n):
+                dst[j].copy_(frames[j, i], non_blocking=True)
+            staged = torch.cuda.Event()
+            staged.record(self.h2d)
+        with torch.cuda.stream(self.ingest):
+            self.ingest.wait_event(staged)
+            if self.ring_free[r] is not None:
+                self.ingest.wait_event(self.ring_free[r])
+            if self.u8_input:
+                # no reset: lr_prev / hr_prev are not touched
+                self._decode(self.inp[q], None, self.ring[r], self.lr[0], self.hr[0])
+                self.in_free[q] = torch.cuda.Event()
+                self.in_free[q].record(self.ingest)
+            if self.scene_cut is not None:
+                mask = None
+                if reset_slots:
+                    m = torch.zeros(n, dtype=torch.int32)
+                    m[list(reset_slots)] = 1
+                    self.in_mask.copy_(m.pin_memory(), non_blocking=True)
+                    mask = self.in_mask
+                rep = self.rep_ring[r]
+                ops.scene_cut(self.ring[r], self.ring[(t - 1) % self.depth], mask, self.scene_cut, self.prev_mafd,
+                              self.work, rep[:2 * n].view(torch.float64), rep[2 * n:3 * n])
+                self.cut_host[r].copy_(rep[2 * n:3 * n], non_blocking=True)
+            self.ingested = torch.cuda.Event()
+            self.ingested.record(self.ingest)
+        cuts = ()
+        if self.scene_cut is not None:
+            self.ingested.synchronize()                # the ingest only: decode, score and the flag copy
+            cuts = [int(k) for k in np.flatnonzero(self.cut_host[r].numpy())]
+        self.sched.ingest(cuts)
+
+    def _emit(self, row, out, report, out_host, j, warm, main):
+        """Warm-ups and main step of frame j, its output into out[:, row] and its report into report[row]."""
+        res = self._res()
+        with torch.cuda.stream(self.main):
+            self.main.wait_event(self.ingested)       # frames up to t_in - 1 are in the ring
+            for i, step in enumerate(warm):
+                q = (len(warm) - 1 - i) & 1             # the last warm-up writes whr[0], which the main step loads
+                self._load_table(self.wtab[q], step)
+                self.run_warm(q)
+            p = self.parity
+            self._load_table(self.mtab[p], main)
+            if out_host and self.out_copied[p] is not None:
+                self.main.wait_event(self.out_copied[p])
+            self.run_frame(p)
+            if report is not None:
+                report[row].copy_(self.rep_ring[j % self.depth, :3 * self.n], non_blocking=True)
+            done = torch.cuda.Event()
+            done.record(self.main)
+            self.ring_free[j % self.depth] = done
+            if not out_host:
+                out[:, row].copy_(res[p], non_blocking=True)
+        if out_host:
+            with torch.cuda.stream(self.d2h):
+                self.d2h.wait_event(done)
+                for k in range(self.n):
+                    out[k, row].copy_(res[p][k], non_blocking=True)
+                self.out_copied[p] = torch.cuda.Event()
+                self.out_copied[p].record(self.d2h)
+        self.parity ^= 1
 
 
 YUV420 = ops.YUV420_LAYOUTS       # 'nv12', 'i420'
@@ -468,7 +789,11 @@ class VideoStream:
 
     def __init__(self, net, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb',
                  in_color='bt601', out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None,
-                 crop=None, out_frame=None, out_origin=None):
+                 crop=None, out_frame=None, out_origin=None, pad_front=0, padding_mode='reflect'):
+        if not _is_int(pad_front) or not 0 <= pad_front <= MAX_PAD_FRONT:
+            raise ValueError(f'pad_front must be an int in [0, {MAX_PAD_FRONT}], got {pad_front!r}')
+        if not isinstance(padding_mode, str) or padding_mode not in PAD_MODES:
+            raise ValueError(f'padding_mode must be one of {PAD_MODES}, got {padding_mode!r}')
         if scene_cut is not None:
             scene_cut = _check_scene_cut(scene_cut)
         if input not in ('uint8', 'float32', *YUV):
@@ -524,6 +849,7 @@ class VideoStream:
         self.out_size, self.resize_filter = out_size, resize_filter
         self.scene_cut = scene_cut
         self.crop, self.out_frame, self.out_origin = crop, out_frame, out_origin
+        self.pad_front, self.padding_mode = int(pad_front), padding_mode
         # the latest push's detected cuts (bool [n,k]) and scores (float64 [n,k]): NumPy after out='host', CUDA
         # tensors after out='device'; None before the first push and without scene_cut
         self.last_cuts = self.last_scores = None
@@ -590,6 +916,25 @@ class VideoStream:
             frames = torch.empty(frames.shape, dtype=frames.dtype, pin_memory=True).copy_(frames)
         res = self._engine.run(frames, [k for k in range(self.n) if slots[k]], out == 'host')
         self._pending = [False] * self.n
+        return self._result(res, out)
+
+    def flush(self, out='host'):
+        """End every slot's video: returns the frames the stream still holds, [n,k_held,...] as push returns them
+        (k_held <= pad_front with padding_mode='reflect', 0 otherwise), each made with the padding its shot gets
+        now that the shot's end is known; last_cuts / last_scores describe them.  Every slot then starts a new video
+        at the next push, as in a new stream."""
+        if self._engine is False:
+            raise ops.L.TecoganB200Error('VideoStream.flush: the stream is closed')
+        if out not in ('host', 'device'):
+            raise ValueError(f"out must be 'host' or 'device', got {out!r}")
+        _check_inference(self.net)
+        if self._engine is None:
+            self._engine = self._build()
+        res = self._engine.run(None, [], out == 'host', flush=True)
+        self._pending = [True] * self.n
+        return self._result(res, out)
+
+    def _result(self, res, out):
         rep = self._engine.report
         if rep is not None:
             # [k,3n] int32: words [0,2n) the n float64 scores, [2n,3n) the n cut flags.  rep is the engine's report
@@ -663,11 +1008,14 @@ class VideoStream:
             top, left, h, w = self.crop
             crop = (self.h, self.w, top, left)
         out_frame = (*self.out_frame, *self.out_origin) if self.out_frame else None
-        return StreamEngine(self.net, self.n, self.c, h, w, dev, u8_input=self.input == 'uint8',
+        engine, pad = StreamEngine, {}
+        if self.pad_front:
+            engine, pad = PaddedStreamEngine, dict(pad_front=self.pad_front, padding_mode=self.padding_mode)
+        return engine(self.net, self.n, self.c, h, w, dev, u8_input=self.input == 'uint8',
                             bgr=self.channel_order == 'bgr', yuv_in=yuv_in, yuv_out=yuv_out,
                             in_color=self.in_color, out_color=self.out_color, out_size=self.out_size,
                             resize_filter=self.resize_filter, scene_cut=self.scene_cut, crop=crop,
-                            out_frame=out_frame)
+                            out_frame=out_frame, **pad)
 
 
 def _check_scene_cut(threshold):

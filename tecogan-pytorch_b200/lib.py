@@ -24,6 +24,7 @@ RESAMPLE_BICUBIC, RESAMPLE_LANCZOS3 = 0, 1
 SCENE_CUT_WORK_BYTES = 16            # TG_SCENE_CUT_WORK_BYTES: workspace of tg_scene_cut per slot
 TAIL_OUT_ROWS = 40                   # TG_TAIL_OUT_ROWS: rows of tg_pack_tail_out_weights' tile (128 bytes each)
 PSNR_NONE, PSNR_RGB, PSNR_Y = 0, 1, 2
+GATHER_KEEP, GATHER_ZERO, GATHER_LOAD = 0, 1, 2    # TG_GATHER_*: per-slot state modes of tg_stream_gather
 
 
 class ConvDesc(ctypes.Structure):
@@ -105,6 +106,7 @@ _SIGNATURES = {
     'tg_float_to_uint8_nhwc': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     'tg_float_to_uint8_nhwc_window': (c_int, [_P, _P, ctypes.POINTER(FrameWindow), c_int, c_int, c_int, c_int, _P]),
     'tg_stream_frame_in': (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    'tg_stream_gather': (c_int, [_P, c_int, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_stream_frame_in_yuv420': (c_int, [_P, c_int, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),
     'tg_rgb_u8_to_yuv420': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     'tg_stream_frame_in_yuv': (c_int, [_P, ctypes.POINTER(YuvFormat), _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P]),

@@ -345,7 +345,7 @@ class FRNet(BaseSequenceGenerator):
 
     def stream(self, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb', in_color='bt601',
                out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None, crop=None, out_frame=None,
-               out_origin=None):
+               out_origin=None, pad_front=0, padding_mode='reflect'):
         """A VideoStream of n lock-stepped slots of h x w LR frames: video pushed in chunks of any length, the
         recurrent state carried from one push to the next, and a slot restarted (reset=) when its video ends and
         the next one begins while the other slots keep running.
@@ -402,12 +402,24 @@ class FRNet(BaseSequenceGenerator):
         are written once, when the stream is built; each step writes only the picture.  tecogan_b200.fit_size gives
         the largest out_size of the picture's display aspect that fits the frame (pillarbox / letterbox).
         A crop or picture that does not fit, or lies off the chroma grid, raises ValueError.
-        Temporal padding (pad_sequence, base_model.py:230-251) stays the caller's job: for p reflect-padded
-        frames, push frames[:, 1:1+p].flip(1) first and drop those p outputs.  The CUDA graphs are captured by the first push; the stream holds the
-        net."""
+        Temporal padding, as the reference's test pipeline pads (VSRModel.infer -> BaseModel.pad_sequence,
+        base_model.py:230-251; test.yml's num_pad_front / padding_mode): pad_front=p (an int in [0, 32]) and
+        padding_mode='reflect' or 'replicate' warm each slot's recurrent state on p pad frames at every shot start --
+        frame 0, a reset= and a detected scene_cut -- so the frames of a shot of L frames are byte-identical to
+        infer_sequence(pad_sequence(shot, q))[q:], with q = min(p, L - 1) for 'reflect' (the reference asserts p < L;
+        a shorter shot gets the longest reflection it has) and q = p for 'replicate'.  'reflect' reads the p frames
+        after a shot start before it can produce that start, so push() returns every slot's frames p frames behind
+        its input: [n,k_out,...] with k_out < k only while the first p frames fill the stream.  flush() ends every
+        slot's video and returns the held frames (then every slot starts anew at the next push); close() drops them.
+        A reset= ends the slot's previous video with the previous push, and its held tail comes out, padded for that
+        end, in the rows of this push.  last_cuts / last_scores stay those of the unpadded stream (pad frames are
+        never scored) and row j describes returned frame j.  The warm-up steps run on state of their own before the
+        main step of the shot's first frame, batch-n and shared by the slots starting a shot at the same frame.
+        pad_front=0 (the default) is the stream without padding, launch for launch.
+        The CUDA graphs are captured by the first push; the stream holds the net."""
         from .engine import VideoStream
         return VideoStream(self, n, h, w, device, input, channel_order, out_format, in_color, out_color, out_size,
-                           resize_filter, scene_cut, crop, out_frame, out_origin)
+                           resize_filter, scene_cut, crop, out_frame, out_origin, pad_front, padding_mode)
 
     def refresh_packed_weights(self, force=False):
         self.fnet._cache.refresh_all(force)

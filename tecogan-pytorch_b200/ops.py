@@ -419,6 +419,34 @@ def stream_frame_in(u8, reset, lr_curr, lr_prev, hr_prev, scale, bgr=False, wind
     return lr_curr
 
 
+def stream_gather(ring, table, warm_hr, lr_curr, lr_prev, hr_prev, scale):
+    """Step input of a padded stream from the ring of decoded frames (tg_stream_gather): ring fp32 [depth,n,c,h,w],
+    table int32 [3n] on the device (cur, mode, prev per slot; modes L.GATHER_KEEP / _ZERO / _LOAD), warm_hr fp32
+    [n,c,scale*h,scale*w] or None -> lr_curr[k] = ring[cur[k]][k]; zero: lr_prev[k] = hr_prev[k] = 0; load:
+    lr_prev[k] = ring[prev[k]][k] (0 for prev[k] < 0), hr_prev[k] = warm_hr[k]."""
+    name = 'stream_gather'
+    _req(ring, torch.float32, 'ring', 5)
+    for t, nm in ((lr_curr, 'lr_curr'), (lr_prev, 'lr_prev'), (hr_prev, 'hr_prev')):
+        _req(t, torch.float32, nm, 4)
+    depth, n, c, h, w = ring.shape
+    H, W = scale * h, scale * w
+    if tuple(lr_curr.shape) != (n, c, h, w) or tuple(lr_prev.shape) != (n, c, h, w):
+        raise L.TecoganB200Error(f'{name}: lr_curr / lr_prev are not [n={n},c={c},h={h},w={w}]')
+    if tuple(hr_prev.shape) != (n, c, H, W) or (warm_hr is not None and tuple(warm_hr.shape) != (n, c, H, W)):
+        raise L.TecoganB200Error(f'{name}: hr_prev / warm_hr are not [n={n},c={c},{H},{W}]')
+    if warm_hr is not None:
+        _req(warm_hr, torch.float32, 'warm_hr', 4)
+    _req(table, torch.int32, 'table', 1)
+    if table.shape[0] != 3 * n:
+        raise L.TecoganB200Error(f'{name}: table has {table.shape[0]} entries, expected {3 * n}')
+    for t in (table, warm_hr, lr_curr, lr_prev, hr_prev):
+        if t is not None and t.device != ring.device:
+            raise L.TecoganB200Error(f'{name}: tensors on different devices')
+    L.check(L.load().tg_stream_gather(_ptr(ring), depth, _ptr(table), _ptr(warm_hr), _ptr(lr_curr), _ptr(lr_prev),
+                                      _ptr(hr_prev), n, c, h, w, scale, _stream()), 'tg_stream_gather')
+    return lr_curr
+
+
 YUV420_LAYOUTS = ('nv12', 'i420')
 
 

@@ -60,7 +60,17 @@ k = 16 pushes of pinned frames, three arms alternating in every rep:
   crop_out_frame  crop=(22, 0, 134, 320), out_frame=(720, 1280): the picture through the net, placed in black
   precropped      a plain 134x320 stream over frames cropped on the host (-> 536x1280)
 with crop_out_frame's output checked against precropped's placed into the black frame (oracle/frame_window.py), and
-the kernel times of the windowed frame input and output writers next to the plain ones (CUDA events over graphs)."""
+the kernel times of the windowed frame input and output writers next to the plain ones (CUDA events over graphs).
+
+    python tools/stream_bench.py --pad [--frames 64] [--reps 3]
+
+measures temporally padded streams instead (one JSON line, metric hr_frames_per_sec_4xBD_pad5): the bd4 clips, uint8
+RGB -> RGB, k = 16 pushes of pinned frames and a flush, four arms alternating in every rep:
+  plain / pad5            pad_front=0 and pad_front=5 reflect, clips without cuts
+  plain_cuts32 / pad5_cuts32  the same with scene_cut=10 on clips that change shot every 32 frames in every slot
+(reported cuts counted, so the cut arms must find n * (frames / 32 - 1) of them), then with CUDA events: one batch-n
+warm-up step of the padded stream and one of a batch-1 padded stream (the cost of a warm start is p such steps), and
+tg_stream_gather per step with all slots kept (the current frame copied) and all slots loaded, with its bytes."""
 import argparse
 import json
 import os
@@ -87,11 +97,14 @@ def main():
     ap.add_argument('--frames', type=int, default=64)
     ap.add_argument('--reps', type=int, default=3)
     ap.add_argument('--window', action='store_true', help='the letterboxed-video arms instead')
+    ap.add_argument('--pad', action='store_true', help='the temporally padded arms instead')
     args = ap.parse_args()
     if args.frames < 60:
         ap.error('--frames must be >= 60')
     if args.window:
         return window_bench(args)
+    if args.pad:
+        return pad_bench(args)
     import numpy as np
     import torch
     import bench
@@ -499,6 +512,101 @@ def window_bench(args):
         'kernel_us': us,
     }
     print(json.dumps(line), flush=True)
+
+
+def _graph_us(fn, launches=20, reps=50):
+    """Mean time of fn (enqueues on the current stream) over `reps` replays of a graph of `launches` calls."""
+    import torch
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        fn()
+    torch.cuda.current_stream().wait_stream(side)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        for _ in range(launches):
+            fn()
+    g.replay()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(reps):
+        g.replay()
+    b.record()
+    torch.cuda.synchronize()
+    return a.elapsed_time(b) * 1e3 / (reps * launches)
+
+
+def pad_bench(args):
+    import numpy as np
+    import torch
+    import bench
+    import tecogan_b200 as T
+    ops = sys.modules['tecogan-pytorch_b200.ops']
+    L = sys.modules['tecogan-pytorch_b200.lib']
+    assert torch.cuda.is_available(), 'stream_bench.py needs a GPU'
+    dev = torch.device('cuda', 0)
+    torch.cuda.set_device(dev)
+    bench.select_workload('bd4')
+    n, (c, h, w), s = bench.CLIPS_PER_GPU, bench.LR, bench.SCALE
+    t, p = args.frames, 5
+    net = T.FRNet(3, 3, 64, 10, 'BD', s)
+    net.load_state_dict(bench.make_params(), strict=True)
+    net = net.to(dev).eval()
+    to_u8 = lambda x: np.ascontiguousarray(np.rint(x * 255.0).astype(np.uint8).transpose(0, 1, 3, 4, 2))   # noqa
+    u8 = torch.from_numpy(to_u8(bench.synthetic_clips(n, t, seed=100).numpy())).pin_memory()
+    shots = [bench.synthetic_clips(n, 32, seed=200 + i).numpy() for i in range(-(-t // 32))]
+    cut_u8 = torch.from_numpy(to_u8(np.concatenate(shots, axis=1)[:, :t])).pin_memory()
+    arms = {'plain': (u8, {}), 'pad5': (u8, dict(pad_front=p)),
+            'plain_cuts32': (cut_u8, dict(scene_cut=10.0)), 'pad5_cuts32': (cut_u8, dict(scene_cut=10.0, pad_front=p))}
+    opened = {k: net.stream(n, h, w, device=dev, **kw) for k, (_, kw) in arms.items()}
+    runs = {k: [] for k in arms}
+    cuts = {k: 0 for k in arms}
+    for rep in range(args.reps + 1):                   # rep 0: untimed warm-up (graph capture)
+        for k, (src, _) in arms.items():
+            st = opened[k]
+            found = 0
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            for i in range(0, t, 16):
+                st.push(src[:, i:i + 16])
+                if st.scene_cut is not None:
+                    found += int(st.last_cuts.sum())
+            st.flush()
+            if st.scene_cut is not None:
+                found += int(st.last_cuts.sum())
+            torch.cuda.synchronize()
+            fps = n * t / (time.perf_counter() - t0)
+            if rep:
+                runs[k].append(fps)
+                cuts[k] = found
+    eng = opened['pad5']._engine
+    warm_n = _graph_us(lambda: eng._enqueue_warm(0), launches=1)
+    one = net.stream(1, h, w, device=dev, pad_front=p)
+    one.push(u8[:1, :1])
+    e1 = one._engine
+    warm_1 = _graph_us(lambda: e1._enqueue_warm(0), launches=1)
+    ring = eng.ring
+    lr, prev, hr, wh = eng.lr[0].clone(), eng.lr[1].clone(), eng.hr[1].clone(), eng.whr[0].clone()
+    tabs = {'keep': [0] * n + [L.GATHER_KEEP] * n + [-1] * n, 'load': [0] * n + [L.GATHER_LOAD] * n + [1] * n}
+    gather = {}
+    nlr, nhr = n * c * h * w * 4, n * c * h * w * s * s * 4
+    for k, v in tabs.items():
+        tab = torch.tensor(v, dtype=torch.int32, device=dev)
+        us = _graph_us(lambda: ops.stream_gather(ring, tab, wh, lr, prev, hr, s))
+        nbytes = 2 * nlr if k == 'keep' else 4 * nlr + 2 * nhr
+        gather[k] = dict(us=round(us, 2), bytes=nbytes, tb_per_s=round(nbytes / us / 1e6, 3))
+    for st in list(opened.values()) + [one]:
+        st.close()
+    med = {k: round(statistics.median(v), 1) for k, v in runs.items()}
+    print(json.dumps({
+        'metric': 'hr_frames_per_sec_4xBD_pad5', 'gpu': torch.cuda.get_device_name(dev), 'power_limit_w': power_limit_w(),
+        'frames': t, 'reps': args.reps, 'push': 16, 'median': med,
+        'runs': {k: [round(x, 1) for x in v] for k, v in runs.items()}, 'cuts_reported': cuts,
+        'cuts_expected': n * (-(-t // 32) - 1),
+        'warm_step_us': {'batch_n': round(warm_n, 1), 'batch_1': round(warm_1, 1)},
+        'warm_start_us': {'batch_n': round(p * warm_n, 1), 'batch_1': round(p * warm_1, 1)},
+        'gather_per_step': gather}))
+
 
 
 if __name__ == '__main__':
