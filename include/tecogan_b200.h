@@ -380,6 +380,27 @@ int tg_resample_nchw_f32_window(const float* x, int n, int c, int H, int W, cons
                                 const float* row_w, int row_taps, const int32_t* col_first, const float* col_w,
                                 int col_taps, int Ho, int Wo, uint8_t* y_u8, const tg_frame_window* win,
                                 void* stream);
+/* Frame input of a streamed step at another LR size: the h x w source picture resized to hn x wn in one launch.
+ * in    : the source frames, uint8 HWC [n, frame_h, frame_w, c] (fmt NULL; bgr != 0 reverses the channel order) or
+ *         any tg_yuv_format layout and colour (c must be 3, bgr 0), read through `win` as tg_stream_frame_in_window /
+ *         tg_stream_frame_in_yuv_window read them (NULL: the whole h x w frame)
+ *      -> lr_curr fp32 NCHW [n,c,hn,wn] = the resize (tg_resample_nchw_f32, fp32 output) of the fp32 picture those
+ *         entry points would write, with the row tables (h -> hn) and the column tables (w -> wn) of
+ *         tg_resample_table, bit for bit: the same decode per source pixel and the same fmaf sums in tap order.
+ *         Nothing is re-quantised, and no source-size fp32 frame exists.
+ * reset : int32 [n] in device memory, or NULL: lr_prev[k] ([c,hn,wn]) and hr_prev[k] ([c,s*hn,s*wn]) of the flagged
+ *         slots are zeroed in the same launch, as tg_stream_frame_in does.
+ * Each axis needs in/4 <= out <= 2*in, and its table's taps must be the bicubic or the Lanczos-3 count of that axis
+ * (tg_resample_taps).  Tables in device memory, 4-byte aligned like the fp32 buffers.
+ * TG_E_INVALID: null pointers (reset aside; in too), non-positive sizes, misalignment, c != 3 or bgr with a YUV
+ * format, a non-zero reserved, a picture outside its frame, tap counts that do not belong to the sizes;
+ * TG_E_UNSUPPORTED: c > 4, s not 2 or 4, odd sizes or windows off the layout's chroma grid, an unknown layout or
+ * matrix, a ratio outside [1/4, 2], a grid too large. */
+int tg_stream_frame_in_resample(const void* in, const tg_yuv_format* fmt, int bgr, const tg_frame_window* win, int h,
+                                int w, const int32_t* row_first, const float* row_w, int row_taps,
+                                const int32_t* col_first, const float* col_w, int col_taps, const int32_t* reset,
+                                float* lr_curr, float* lr_prev, float* hr_prev, int n, int c, int hn, int wn, int s,
+                                void* stream);
 
 /* Scene-cut detection of a streamed step (oracle/scene_cut.py is the specification).  Per slot k, with a = lr_curr[k]
  * and b = lr_prev[k] (fp32 [c,h,w], as the step sees them: decoded, and zeroed by a reset of this step):

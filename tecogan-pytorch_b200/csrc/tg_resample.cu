@@ -1,18 +1,20 @@
 // Antialiased bicubic / Lanczos-3 resize of the streamed HR frame (fp32 NCHW) to the output size, written as uint8
 // NHWC (quantised like float32_to_uint8) or fp32 NCHW (the source of the 10-bit encodes), and the host-side builder
 // of its per-axis tables.  The filters are Pillow's (Image.resize on 'F' images); oracle/resample.py specifies them.
-// The uint8 output can be a picture window of larger frames (tg_frame_window).
-// Contract: include/tecogan_b200.h (tg_resample_taps, tg_resample_table, tg_resample_nchw_f32[_window]).
+// The uint8 output can be a picture window of larger frames (tg_frame_window).  The same tiles resize the streamed
+// input: the frame-input launch's decode of the source picture (tg_frame_decode.cuh) read in place of the fp32 frame,
+// fp32 LR frame out, with the per-slot reset of tg_stream_frame_in in the same launch.
+// Contract: include/tecogan_b200.h (tg_resample_taps, tg_resample_table, tg_resample_nchw_f32[_window],
+// tg_stream_frame_in_resample).
 #include <math.h>
 
 #include "tg_common.cuh"
+#include "tg_frame_decode.cuh"     // also kThreads (256) and kMaxC (4)
 
 namespace {
 
-constexpr int kThreads = 256;
 constexpr int kTY = 16, kTX = 64;            // output tile of one CTA: kTY rows x kTX columns, every channel
 constexpr int kMaxTaps = 25;                 // lanczos at a 1/4 downscale: 2 * ceil(3 * 4) + 1
-constexpr int kMaxC = 4;
 constexpr int kOutRow = kTX * kMaxC + 16;    // staged uint8 row: the destination's 16-byte lead, then the pixels
 // the vertical pass's columns of one tile: first[last] - first[0] + taps <= ceil((kTX - 1) * in / out) + 1 + taps
 constexpr int kMaxSpan = (kTX - 1) * 4 + 2 + kMaxTaps;
@@ -20,26 +22,60 @@ constexpr int kMaxMidBytes = kMaxC * kTY * kMaxSpan * (int)sizeof(float);
 
 int span_cap(int in, int out, int taps) { return (int)(((long long)(kTX - 1) * in + out - 1) / out) + 2 + taps; }
 
-// One CTA: output rows [oy0, oy0 + kTY) x columns [ox0, ox0 + kTX) of image `img`, all c channels.
+// Sources of the vertical pass.  An item of the pass is one column of one output row for kC channels: col() names
+// the column (channel group k, source column xc, already clamped), read() gives its kC values at source row y.
+// fp32 NCHW x [n,c,H,W] (the streamed HR frame): one channel per item.
+struct NchwSource {
+  // kC channels per item, kItems items per thread and iteration, the vertical pass's taps unrolled kUnroll times
+  static constexpr int kC = 1, kItems = 2, kUnroll = 4;
+  using Col = const float*;
+  const float* x;
+  int c, H, W;
+  __device__ __forceinline__ Col col(int img, int k, int xc) const { return x + ((size_t)img * c + k) * H * W + xc; }
+  __device__ __forceinline__ void read(Col p, int y, float* v) const { v[0] = __ldg(p + (size_t)y * W); }
+};
+
+// The H x W picture at `win` of stored frames of layout kFmt, decoded as the frame input decodes it (decode_pixel):
+// every channel of a pixel per item, so a source pixel is decoded once per tap, not once per channel.
+template <int kFmt>
+struct FrameSource {
+  static constexpr int kC = kMaxC, kItems = 1, kUnroll = 1;   // no spills around the decode's divisions
+  struct Col {
+    int img, x;
+  };
+  const uint8_t* in;
+  tg_frame_window win;
+  int c, bgr, color;
+  __device__ __forceinline__ Col col(int img, int, int xc) const { return Col{img, xc}; }
+  __device__ __forceinline__ void read(Col p, int y, float* v) const {
+    decode_pixel<kFmt>(in, win, c, bgr, color, p.img, y, p.x, v);
+  }
+};
+
+// One CTA (b of the resize's CTAs): output rows [oy0, oy0 + kTY) x columns [ox0, ox0 + kTX) of image `img`, all c
+// channels.
 //  1. vertical pass: for every input column the tile's horizontal windows cover ([base, base + span)), every channel
 //     and every output row, mid = sum_q row_w[q] * x[row_first + q][col] -- coalesced row reads (L1 / L2 serve the
 //     rows neighbouring outputs share), fp32 results in shared memory;
 //  2. horizontal pass: y = sum_q col_w[q] * mid[col_first + q - base] from shared memory.
-// Both sums run in tap order with fmaf, so an output's value does not depend on the grid.  Every row and column
-// index is clamped into the image (padding taps have weight 0) and into the staged span.
-template <bool kU8>
-__global__ void __launch_bounds__(kThreads)
-resample_kernel(const float* __restrict__ x, int c, int H, int W, const int32_t* __restrict__ row_first,
-                const float* __restrict__ row_w, int row_taps, const int32_t* __restrict__ col_first,
-                const float* __restrict__ col_w, int col_taps, int Ho, int Wo, int tiles_x, int tiles_y, int cap,
-                uint8_t* __restrict__ y_u8, tg_frame_window win, float* __restrict__ y_f32) {
+// Both sums run in tap order with fmaf, so an output's value does not depend on the grid or on the source (an fp32
+// frame, or the decode that would have written it).  Every row and column index is clamped into the image (padding
+// taps have weight 0) and into the staged span.
+template <bool kU8, class Src>
+__device__ __forceinline__ void resample_tile(const Src& src, int b, int c, int H, int W,
+                                              const int32_t* __restrict__ row_first, const float* __restrict__ row_w,
+                                              int row_taps, const int32_t* __restrict__ col_first,
+                                              const float* __restrict__ col_w, int col_taps, int Ho, int Wo,
+                                              int tiles_x, int tiles_y, int cap, uint8_t* __restrict__ y_u8,
+                                              tg_frame_window win, float* __restrict__ y_f32) {
+  constexpr int kC = Src::kC;
   __shared__ float s_rw[kTY * kMaxTaps];
   __shared__ float s_cw[kTX * kMaxTaps];
   __shared__ int s_rf[kTY], s_cf[kTX];
   __shared__ __align__(16) uint8_t s_out[kU8 ? kTY : 1][kU8 ? kOutRow : 16];
   extern __shared__ float s_mid[];           // [c][kTY][cap]
   const int t = threadIdx.x;
-  const int tx = blockIdx.x % tiles_x, rest = blockIdx.x / tiles_x;
+  const int tx = b % tiles_x, rest = b / tiles_x;
   const int ty = rest % tiles_y, img = rest / tiles_y;
   const int ox0 = tx * kTX, oy0 = ty * kTY;
   const int nx = min(kTX, Wo - ox0), ny = min(kTY, Ho - oy0);
@@ -59,35 +95,46 @@ resample_kernel(const float* __restrict__ x, int c, int H, int W, const int32_t*
   const int base = min(max(s_cf[0], 0), W - 1);
   const int span = max(min(s_cf[nx - 1] - base + col_taps, cap), 1);
 
-  const size_t plane = (size_t)H * W;
-  const float* src = x + (size_t)img * c * plane;
-  // items (channel, output row, column), columns fastest: consecutive threads read consecutive addresses.  Two
-  // items per thread and iteration, so that both windows' loads are in flight together.
-  const int items = c * ny * span;
-  for (int i0 = t; i0 < items; i0 += 2 * kThreads) {
-    const int i1 = min(i0 + kThreads, items - 1);
-    const float *p[2], *w[2];
-    int f[2], dst[2];
+  // items (channel group, output row, column), columns fastest: consecutive threads read consecutive addresses.
+  // kI items per thread and iteration, so that their windows' loads are in flight together.
+  constexpr int kI = Src::kItems;
+  const int items = (kC == 1 ? c : 1) * ny * span;
+  for (int i0 = t; i0 < items; i0 += kI * kThreads) {
+    typename Src::Col p[kI];
+    const float* w[kI];
+    int f[kI], dst[kI];
 #pragma unroll
-    for (int u = 0; u < 2; ++u) {
-      const int i = u ? i1 : i0;
+    for (int u = 0; u < kI; ++u) {
+      const int i = u ? min(i0 + u * kThreads, items - 1) : i0;
       const int kr = i / span, j = i - kr * span;
       const int k = kr / ny, r = kr - k * ny;
-      p[u] = src + k * plane + min(base + j, W - 1);
+      p[u] = src.col(img, k, min(base + j, W - 1));
       w[u] = s_rw + r * row_taps;
       f[u] = s_rf[r];
       dst[u] = (k * kTY + r) * cap + j;
     }
-    float acc0 = 0.f, acc1 = 0.f;
-#pragma unroll 4
+    float acc[kI][kC];
+#pragma unroll
+    for (int u = 0; u < kI; ++u)
+#pragma unroll
+      for (int k = 0; k < kC; ++k) acc[u][k] = 0.f;
+#pragma unroll Src::kUnroll
     for (int q = 0; q < row_taps; ++q) {
-      const float x0 = __ldg(p[0] + (size_t)min(max(f[0] + q, 0), H - 1) * W);
-      const float x1 = __ldg(p[1] + (size_t)min(max(f[1] + q, 0), H - 1) * W);
-      acc0 = fmaf(w[0][q], x0, acc0);
-      acc1 = fmaf(w[1][q], x1, acc1);
+      float x[kI][kC] = {};
+#pragma unroll
+      for (int u = 0; u < kI; ++u) src.read(p[u], min(max(f[u] + q, 0), H - 1), x[u]);
+#pragma unroll
+      for (int u = 0; u < kI; ++u)
+#pragma unroll
+        for (int k = 0; k < kC; ++k) acc[u][k] = fmaf(w[u][q], x[u][k], acc[u][k]);
     }
-    s_mid[dst[0]] = acc0;
-    if (i0 + kThreads < items) s_mid[dst[1]] = acc1;
+#pragma unroll
+    for (int k = 0; k < kC; ++k) {
+      if (k >= c) break;
+#pragma unroll
+      for (int u = 0; u < kI; ++u)
+        if (u == 0 || i0 + u * kThreads < items) s_mid[dst[u] + k * kTY * cap] = acc[u][k];
+    }
   }
   __syncthreads();
 
@@ -126,6 +173,45 @@ resample_kernel(const float* __restrict__ x, int c, int H, int W, const int32_t*
       if (tail0 + lane < bytes) dst[tail0 + lane] = sb[tail0 + lane];
     }
   }
+}
+
+// the output resize: one CTA per tile of the fp32 NCHW frame x
+template <bool kU8>
+__global__ void __launch_bounds__(kThreads)
+resample_kernel(const float* __restrict__ x, int c, int H, int W, const int32_t* __restrict__ row_first,
+                const float* __restrict__ row_w, int row_taps, const int32_t* __restrict__ col_first,
+                const float* __restrict__ col_w, int col_taps, int Ho, int Wo, int tiles_x, int tiles_y, int cap,
+                uint8_t* __restrict__ y_u8, tg_frame_window win, float* __restrict__ y_f32) {
+  resample_tile<kU8>(NchwSource{x, c, H, W}, blockIdx.x, c, H, W, row_first, row_w, row_taps, col_first, col_w,
+                     col_taps, Ho, Wo, tiles_x, tiles_y, cap, y_u8, win, y_f32);
+}
+
+// The resizing frame input.  blockIdx.x < resize_ctas: a tile of lr_curr [n,c,Ho,Wo] resized from the decoded source
+// picture; the rest: zpc CTAs per slot, each zeroing a strided share of that slot's lr_prev and hr_prev when flagged
+// (stream_frame_in_kernel's reset).
+template <int kFmt>
+__global__ void __launch_bounds__(kThreads)
+frame_in_resample_kernel(FrameSource<kFmt> src, int H, int W, const int32_t* __restrict__ row_first,
+                         const float* __restrict__ row_w, int row_taps, const int32_t* __restrict__ col_first,
+                         const float* __restrict__ col_w, int col_taps, int Ho, int Wo, int tiles_x, int tiles_y,
+                         int cap, float* __restrict__ lr_curr, const int32_t* __restrict__ reset,
+                         float* __restrict__ lr_prev, float* __restrict__ hr_prev, int s, int resize_ctas, int zpc) {
+  const int b = blockIdx.x, c = src.c;
+  if (b < resize_ctas) {
+    resample_tile<false>(src, b, c, H, W, row_first, row_w, row_taps, col_first, col_w, col_taps, Ho, Wo, tiles_x,
+                         tiles_y, cap, nullptr, tg_frame_window{Ho, Wo, 0, 0}, lr_curr);
+    return;
+  }
+  // lr_prev and hr_prev belong to the previous step until it has finished
+  tg_pdl_wait();
+  tg_pdl_trigger();
+  const int rb = b - resize_ctas;
+  const int slot = rb / zpc, part = rb - slot * zpc;
+  if (__ldg(reset + slot) == 0) return;
+  const size_t nlr = (size_t)c * Ho * Wo, nhr = nlr * s * s;
+  const size_t worker = (size_t)part * kThreads + threadIdx.x, workers = (size_t)zpc * kThreads;
+  zero_range(lr_prev + slot * nlr, nlr, worker, workers);
+  zero_range(hr_prev + slot * nhr, nhr, worker, workers);
 }
 
 // ---------------------------------------------------------------- host: Pillow's filters and window placement
@@ -263,7 +349,91 @@ int resample(const char* name, const float* x, int n, int c, int H, int W, const
   return TG_OK;
 }
 
+// one axis of the input resize: `in` -> `out` within the ratios, `taps` the bicubic or the Lanczos table's width
+int check_input_axis(const char* name, const char* axis, int in, int out, int taps) {
+  TG_REQUIRE(4ll * out >= in && out <= 2ll * in, TG_E_UNSUPPORTED,
+             "%s: %s %d -> %d is outside the supported ratios (in/4 <= out <= 2*in)", name, axis, in, out);
+  const int bicubic = taps_of(in, out, TG_RESAMPLE_BICUBIC), lanczos = taps_of(in, out, TG_RESAMPLE_LANCZOS3);
+  TG_REQUIRE(taps == bicubic || taps == lanczos, TG_E_INVALID,
+             "%s: %s table of %d taps, %d -> %d takes %d (bicubic) or %d (lanczos)", name, axis, taps, in, out,
+             bicubic, lanczos);
+  return TG_OK;
+}
+
+template <int kFmt>
+int launch_frame_in_resample(const char* name, const void* in, const tg_frame_window* win, int bgr, int color, int h,
+                             int w, const int32_t* row_first, const float* row_w, int row_taps,
+                             const int32_t* col_first, const float* col_w, int col_taps, const int32_t* reset,
+                             float* lr_curr, float* lr_prev, float* hr_prev, int n, int c, int hn, int wn, int s,
+                             cudaStream_t stream) {
+  TG_REQUIRE(in, TG_E_INVALID, "%s: null pointer (in)", name);
+  TG_REQUIRE(lr_curr && lr_prev && hr_prev, TG_E_INVALID, "%s: null pointer (lr_curr / lr_prev / hr_prev)", name);
+  TG_REQUIRE(row_first && row_w && col_first && col_w, TG_E_INVALID,
+             "%s: null pointer (row_first / row_w / col_first / col_w)", name);
+  TG_REQUIRE(n > 0 && c > 0 && h > 0 && w > 0 && hn > 0 && wn > 0, TG_E_INVALID,
+             "%s: bad size n=%d c=%d %dx%d -> %dx%d", name, n, c, h, w, hn, wn);
+  TG_REQUIRE(c <= kMaxC, TG_E_UNSUPPORTED, "%s: %d channels (at most %d)", name, c, kMaxC);
+  TG_REQUIRE(!fmt_420(kFmt) || (h % 2 == 0 && w % 2 == 0), TG_E_UNSUPPORTED,
+             "%s: YUV 4:2:0 needs an even height and width, got %dx%d", name, h, w);
+  TG_REQUIRE(!fmt_packed(kFmt) || w % 2 == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name, w);
+  TG_REQUIRE(s == 2 || s == 4, TG_E_UNSUPPORTED, "%s: scale %d (2 or 4)", name, s);
+  TG_REQUIRE((((uintptr_t)lr_curr | (uintptr_t)lr_prev | (uintptr_t)hr_prev | (uintptr_t)row_first |
+               (uintptr_t)row_w | (uintptr_t)col_first | (uintptr_t)col_w) & 3u) == 0,
+             TG_E_INVALID, "%s: fp32 buffers and the tables must be 4-byte aligned", name);
+  TG_REQUIRE(!fmt_10(kFmt) || ((uintptr_t)in & 1u) == 0, TG_E_INVALID, "%s: 10-bit frames must be 2-byte aligned",
+             name);
+  TG_REQUIRE(!fmt_packed(kFmt) || ((uintptr_t)in & 3u) == 0, TG_E_INVALID,
+             "%s: packed 4:2:2 frames must be 4-byte aligned", name);
+  const tg_frame_window whole = {h, w, 0, 0};
+  if (!win) win = &whole;
+  int rc = check_window<kFmt>(name, win, h, w);
+  if (rc == TG_OK) rc = check_input_axis(name, "rows", h, hn, row_taps);
+  if (rc == TG_OK) rc = check_input_axis(name, "columns", w, wn, col_taps);
+  if (rc != TG_OK) return rc;
+  const int tiles_x = tg_ceil_div(wn, kTX), tiles_y = tg_ceil_div(hn, kTY);
+  const size_t resize = (size_t)tiles_x * tiles_y * n;
+  const size_t hr4 = (size_t)c * s * hn * s * wn / 4;
+  const int zpc = reset ? (int)(hr4 / (kThreads * 8) + 1 < 64 ? hr4 / (kThreads * 8) + 1 : 64) : 0;
+  const size_t ctas = resize + (size_t)zpc * n;
+  TG_REQUIRE(ctas <= 0x7fffffff, TG_E_UNSUPPORTED, "%s: grid too large", name);
+  const int cap = span_cap(w, wn, col_taps);
+  const size_t smem = (size_t)c * kTY * cap * sizeof(float);
+  static TgPerDeviceOnce attr_once;
+  const cudaError_t e = attr_once.run([] {
+    return cudaFuncSetAttribute(frame_in_resample_kernel<kFmt>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                kMaxMidBytes);
+  });
+  TG_REQUIRE(e == cudaSuccess, (int)e, "%s: cudaFuncSetAttribute: %s", name, cudaGetErrorString(e));
+  const FrameSource<kFmt> src{static_cast<const uint8_t*>(in), *win, c, bgr, color};
+  tg_launch(frame_in_resample_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), smem, stream, src, h, w, row_first,
+            row_w, row_taps, col_first, col_w, col_taps, hn, wn, tiles_x, tiles_y, cap, lr_curr, reset, lr_prev,
+            hr_prev, s, (int)resize, zpc);
+  TG_CUDA_LAUNCH_CHECK(name);
+  return TG_OK;
+}
+
 }  // namespace
+
+extern "C" int tg_stream_frame_in_resample(const void* in, const tg_yuv_format* fmt, int bgr,
+                                           const tg_frame_window* win, int h, int w, const int32_t* row_first,
+                                           const float* row_w, int row_taps, const int32_t* col_first,
+                                           const float* col_w, int col_taps, const int32_t* reset, float* lr_curr,
+                                           float* lr_prev, float* hr_prev, int n, int c, int hn, int wn, int s,
+                                           void* stream) {
+  const char* name = "stream_frame_in_resample";
+  int f = kHWC, color = 0;
+  if (fmt) {
+    const int rc = parse_yuv_format(name, fmt, &f, &color);
+    if (rc != TG_OK) return rc;
+    TG_REQUIRE(c == 3, TG_E_INVALID, "%s: YUV frames decode to 3 channels, got c=%d", name, c);
+    TG_REQUIRE(bgr == 0, TG_E_INVALID, "%s: bgr applies to uint8 HWC frames only", name);
+  }
+  return dispatch_format(f, [&](auto k) {
+    return launch_frame_in_resample<decltype(k)::value>(name, in, win, bgr, color, h, w, row_first, row_w, row_taps,
+                                                        col_first, col_w, col_taps, reset, lr_curr, lr_prev, hr_prev,
+                                                        n, c, hn, wn, s, (cudaStream_t)stream);
+  });
+}
 
 extern "C" int tg_resample_nchw_f32(const float* x, int n, int c, int H, int W, const int32_t* row_first,
                                     const float* row_w, int row_taps, const int32_t* col_first, const float* col_w,

@@ -245,6 +245,11 @@ class StreamEngine(ClipEngine):
     and cut[p] (int32 [n]) are views of one int32 buffer rep[p] [3n], copied after each replay into the push's
     report [k,3n] (one device-to-device copy per frame).
 
+    Resized input (in_picture = (ph, pw)): the source picture is ph x pw and the net runs at h x w; the frame input is
+    tg_stream_frame_in_resample instead, the same decode resized with the per-axis tables in_tables (rows, columns;
+    built once) into lr[p] in the same one launch, with the same reset.  Everything after it sees the h x w frame:
+    scene_cut scores the resized frames, and a padded stream's ring holds them.
+
     Windows (tg_frame_window).  crop = (Hf, Wf, top, left): inp[p] holds whole Hf x Wf source frames and the frame input
     reads the h x w picture at (top, left) out of them, in the same one launch (the net, FNet's flow and scene_cut see
     the picture only).  out_frame = (Hf, Wf, y, x): the copies out read padded frames, pad[p] (uint8 RGB [n,Hf,Wf,c])
@@ -258,7 +263,7 @@ class StreamEngine(ClipEngine):
 
     def __init__(self, net, n, c, h, w, device, u8_input=True, bgr=False, yuv_in=None, yuv_out=None,
                  in_color='bt601', out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None,
-                 crop=None, out_frame=None):
+                 crop=None, out_frame=None, in_picture=None, in_filter='bicubic'):
         dev = torch.device(device)
         self.u8_input, self.bgr = u8_input or yuv_in is not None, bgr
         self.yuv_in, self.yuv_out = yuv_in, yuv_out          # None or one of ops.YUV_LAYOUTS
@@ -266,12 +271,17 @@ class StreamEngine(ClipEngine):
         self.mask = [torch.zeros(n, dtype=torch.int32, device=dev) for _ in range(2)]
         self.crop = tuple(crop) if crop else None            # (Hf, Wf, top, left) of the input frames
         self.out_frame = tuple(out_frame) if out_frame else None   # (Hf, Wf, y, x) of the output frames
-        fh, fw = self.crop[:2] if self.crop else (h, w)
+        self.in_picture = tuple(in_picture) if in_picture else None   # (ph, pw) of the source picture
+        fh, fw = self.crop[:2] if self.crop else self.in_picture or (h, w)
         frame = ops.yuv_frame_shape(yuv_in, fh, fw) if yuv_in else (fh, fw, c)
         # 10-bit words: zeroed as int16, the same bits
         in_dtype = torch.int16 if yuv_in and ops.yuv_depth(yuv_in) == 10 else torch.uint8
         self.inp = ([torch.zeros(n, *frame, dtype=in_dtype, device=dev).view(_word_dtype(yuv_in)) for _ in range(2)]
                     if self.u8_input else None)
+        self.in_tables = None
+        if self.in_picture:
+            self.in_tables = [tuple(t.to(dev) for t in ops.resample_table(a, b, in_filter))
+                              for a, b in zip(self.in_picture, (h, w))]
         H, W = net.scale * h, net.scale * w
         self.out_size = tuple(out_size) if out_size else None
         Ho, Wo = self.out_size or (H, W)
@@ -319,7 +329,7 @@ class StreamEngine(ClipEngine):
     def close(self):
         super().close()
         self.mask, self.inp, self.yuv, self.pad = [], None, None, None
-        self.tables, self.rs = None, None
+        self.tables, self.rs, self.in_tables = None, None, None
         self.prev_mafd = self.work = self.rep = self.score = self.cut = self.report = None
         self._report_dev = self._report_host = None
 
@@ -335,7 +345,10 @@ class StreamEngine(ClipEngine):
     def _decode(self, inp, mask, lr_curr, lr_prev, hr_prev):
         """The frame input launch: inp (None for fp32 input) decoded into lr_curr, the slots of mask reset."""
         crop = self.crop[2:] if self.crop else None          # (top, left)
-        if self.yuv_in in YUV420 and self.in_color == 'bt601' and crop is None:
+        if self.in_tables is not None:
+            ops.stream_frame_in_resample(inp, self.yuv_in, self.in_color, mask, lr_curr, lr_prev, hr_prev,
+                                         self.net.scale, *self.in_tables, self.in_picture, bgr=self.bgr, window=crop)
+        elif self.yuv_in in YUV420 and self.in_color == 'bt601' and crop is None:
             ops.stream_frame_in_yuv420(inp, self.yuv_in, mask, lr_curr, lr_prev, hr_prev, self.net.scale)
         elif self.yuv_in:
             # the windowed entry point has no BT.601-only twin: its bt601 row is the same cv2 conversion
@@ -789,7 +802,8 @@ class VideoStream:
 
     def __init__(self, net, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb',
                  in_color='bt601', out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None,
-                 crop=None, out_frame=None, out_origin=None, pad_front=0, padding_mode='reflect'):
+                 crop=None, out_frame=None, out_origin=None, pad_front=0, padding_mode='reflect', in_size=None,
+                 in_filter='bicubic'):
         if not _is_int(pad_front) or not 0 <= pad_front <= MAX_PAD_FRONT:
             raise ValueError(f'pad_front must be an int in [0, {MAX_PAD_FRONT}], got {pad_front!r}')
         if not isinstance(padding_mode, str) or padding_mode not in PAD_MODES:
@@ -815,11 +829,20 @@ class VideoStream:
             raise ValueError(f'resize_filter must be one of {ops.RESIZE_FILTERS}, got {resize_filter!r}')
         if out_size is None and resize_filter != 'bicubic':
             raise ValueError(f'resize_filter={resize_filter!r} applies to a resized stream only (give out_size)')
+        if not isinstance(in_filter, str) or in_filter not in ops.RESIZE_FILTERS:
+            raise ValueError(f'in_filter must be one of {ops.RESIZE_FILTERS}, got {in_filter!r}')
+        if in_size is None and in_filter != 'bicubic':
+            raise ValueError(f'in_filter={in_filter!r} applies to a resized input only (give in_size)')
+        if in_size is not None and input == 'float32':
+            raise ValueError("in_size applies to uint8 and YUV frames, not to input='float32'")
         if crop is not None:
             if input == 'float32':
                 raise ValueError("crop applies to uint8 and YUV frames, not to input='float32'")
             crop = _check_box('crop', crop, h, w, input)
-        ph, pw = crop[2:] if crop else (h, w)      # the picture the net runs on
+        ph, pw = crop[2:] if crop else (h, w)      # the source picture
+        if in_size is not None:
+            in_size = _check_in_size(in_size, ph, pw)
+        ph, pw = in_size or (ph, pw)               # the picture the net runs on
         if out_size is not None:
             out_size = _check_out_size(out_size, net.scale * ph, net.scale * pw, out_format)
         yuv = [f for f in (input, out_format) if f in YUV]
@@ -850,6 +873,7 @@ class VideoStream:
         self.scene_cut = scene_cut
         self.crop, self.out_frame, self.out_origin = crop, out_frame, out_origin
         self.pad_front, self.padding_mode = int(pad_front), padding_mode
+        self.in_size, self.in_filter = in_size, in_filter
         # the latest push's detected cuts (bool [n,k]) and scores (float64 [n,k]): NumPy after out='host', CUDA
         # tensors after out='device'; None before the first push and without scene_cut
         self.last_cuts = self.last_scores = None
@@ -1001,6 +1025,11 @@ class VideoStream:
             raise ops.L.TecoganB200Error(f'VideoStream: the net\'s parameters are on {pdev}, the stream runs on '
                                          f'{dev}; move the net first (net.to(device))')
         self.device = dev
+        engine, args, kw = self._engine_args()
+        return engine(*args, **kw)
+
+    def _engine_args(self):
+        """(engine class, positional arguments, keyword arguments) of the stream's engine."""
         yuv_in = self.input if self.input in YUV else None
         yuv_out = self.out_format if self.out_format in YUV else None
         h, w, crop = self.h, self.w, None
@@ -1008,14 +1037,17 @@ class VideoStream:
             top, left, h, w = self.crop
             crop = (self.h, self.w, top, left)
         out_frame = (*self.out_frame, *self.out_origin) if self.out_frame else None
-        engine, pad = StreamEngine, {}
+        engine, kw = StreamEngine, {}
         if self.pad_front:
-            engine, pad = PaddedStreamEngine, dict(pad_front=self.pad_front, padding_mode=self.padding_mode)
-        return engine(self.net, self.n, self.c, h, w, dev, u8_input=self.input == 'uint8',
-                            bgr=self.channel_order == 'bgr', yuv_in=yuv_in, yuv_out=yuv_out,
-                            in_color=self.in_color, out_color=self.out_color, out_size=self.out_size,
-                            resize_filter=self.resize_filter, scene_cut=self.scene_cut, crop=crop,
-                            out_frame=out_frame, **pad)
+            engine, kw = PaddedStreamEngine, dict(pad_front=self.pad_front, padding_mode=self.padding_mode)
+        if self.in_size is not None and self.in_size != (h, w):
+            # the net runs at in_size; an in_size equal to the picture is the stream without it
+            kw.update(in_picture=(h, w), in_filter=self.in_filter)
+            h, w = self.in_size
+        return engine, (self.net, self.n, self.c, h, w, self.device), dict(
+            u8_input=self.input == 'uint8', bgr=self.channel_order == 'bgr', yuv_in=yuv_in, yuv_out=yuv_out,
+            in_color=self.in_color, out_color=self.out_color, out_size=self.out_size,
+            resize_filter=self.resize_filter, scene_cut=self.scene_cut, crop=crop, out_frame=out_frame, **kw)
 
 
 def _check_scene_cut(threshold):
@@ -1026,6 +1058,19 @@ def _check_scene_cut(threshold):
     if not (math.isfinite(t) and ops.scene_cut_threshold_ok(t)):
         raise ValueError(f'scene_cut threshold must be finite and in (0, 100], got {threshold!r}')
     return t
+
+
+def _check_in_size(in_size, h, w):
+    """in_size -> (hn, wn) ints, or ValueError: two positive ints within the resize's ratios (1/4 to 2 times) of the
+    h x w source picture."""
+    if (not isinstance(in_size, (tuple, list)) or len(in_size) != 2
+            or not all(_is_int(v) and v > 0 for v in in_size)):
+        raise ValueError(f'in_size must be (hn, wn), two positive ints, got {in_size!r}')
+    hn, wn = int(in_size[0]), int(in_size[1])
+    if not (ops.resample_ratio_ok(h, hn) and ops.resample_ratio_ok(w, wn)):
+        raise ValueError(f'in_size {hn}x{wn} from a {h}x{w} picture: each axis must be within 1/4 to 2 times the '
+                         f'picture size')
+    return hn, wn
 
 
 def _check_out_size(out_size, H, W, out_format):

@@ -126,6 +126,9 @@ _SIGNATURES = {
                                      _P, _P, _P]),
     'tg_resample_nchw_f32_window': (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, _P, c_int, c_int, c_int,
                                             _P, ctypes.POINTER(FrameWindow), _P]),
+    'tg_stream_frame_in_resample': (c_int, [_P, ctypes.POINTER(YuvFormat), c_int, ctypes.POINTER(FrameWindow), c_int,
+                                            c_int, _P, _P, c_int, _P, _P, c_int, _P, _P, _P, _P, c_int, c_int, c_int,
+                                            c_int, c_int, _P]),
     'tg_scene_cut': (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P, c_double, _P, _P, _P, _P, _P]),
     'tg_metrics_frames_in': (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_int, c_int, _P, _P, _P]),
     'tg_farneback_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),

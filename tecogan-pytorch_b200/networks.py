@@ -345,7 +345,7 @@ class FRNet(BaseSequenceGenerator):
 
     def stream(self, n, h, w, device=None, input='uint8', channel_order='rgb', out_format='rgb', in_color='bt601',
                out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None, crop=None, out_frame=None,
-               out_origin=None, pad_front=0, padding_mode='reflect'):
+               out_origin=None, pad_front=0, padding_mode='reflect', in_size=None, in_filter='bicubic'):
         """A VideoStream of n lock-stepped slots of h x w LR frames: video pushed in chunks of any length, the
         recurrent state carried from one push to the next, and a slot restarted (reset=) when its video ends and
         the next one begins while the other slots keep running.
@@ -416,10 +416,20 @@ class FRNet(BaseSequenceGenerator):
         never scored) and row j describes returned frame j.  The warm-up steps run on state of their own before the
         main step of the shot's first frame, batch-n and shared by the slots starting a shot at the same frame.
         pad_front=0 (the default) is the stream without padding, launch for launch.
+        Any input resolution: in_size=(hn, wn) resizes the picture (the whole frame, or the crop box) on the device to
+        hn x wn, inside the frame-input launch, and the net runs at that size: the output is s*hn x s*wn (out_size,
+        out_frame and out_origin refer to it).  in_filter is 'bicubic' (the default) or 'lanczos', Pillow's
+        antialiased filters as for out_size.  The net's LR frame is oracle/resample.resize(decode(picture), (hn, wn),
+        in_filter), kept in fp32 and not re-quantised to 8 bits, where decode is what the frame input computes
+        without in_size (uint8 / 255, or the YUV conversion; 10 bit / 1023).  scene_cut scores these resized frames.
+        Each axis needs picture/4 <= in_size <= 2*picture; uint8 and YUV input only.  in_size equal to the picture
+        (every source already at the LR size) is the stream without it, launch for launch and byte for byte.  E.g. a
+        1080p NV12 source through a x4 net: h, w = 1080, 1920, in_size=(540, 960), NV12 2160x3840 out.
         The CUDA graphs are captured by the first push; the stream holds the net."""
         from .engine import VideoStream
         return VideoStream(self, n, h, w, device, input, channel_order, out_format, in_color, out_color, out_size,
-                           resize_filter, scene_cut, crop, out_frame, out_origin, pad_front, padding_mode)
+                           resize_filter, scene_cut, crop, out_frame, out_origin, pad_front, padding_mode, in_size,
+                           in_filter)
 
     def refresh_packed_weights(self, force=False):
         self.fnet._cache.refresh_all(force)

@@ -766,6 +766,65 @@ def resample(x, rows, cols, out_u8=None, out_f32=None, window=None):
     return out
 
 
+def stream_frame_in_resample(frames, layout, color, reset, lr_curr, lr_prev, hr_prev, scale, rows, cols, size,
+                             bgr=False, window=None):
+    """tg_stream_frame_in_resample: the frame input (stream_frame_in / stream_frame_in_yuv) of the size = (h, w)
+    source picture, resized on the device with the device tables rows = (first [hn], weights [hn, taps]) (h -> hn)
+    and cols = (first [wn], weights [wn, taps]) (w -> wn) into lr_curr fp32 [n,c,hn,wn], in one launch; bit for bit
+    the frame input at h x w followed by resample(..., out_f32=lr_curr).  frames: uint8 HWC [n,Hf,Wf,c] (layout None,
+    channels reversed when bgr) or a YUV layout's [n,*yuv_frame_shape(layout, Hf, Wf)] in colour `color`; the picture
+    is the whole frame, or the h x w one at window = (top, left).  reset as in stream_frame_in (lr_prev
+    [n,c,hn,wn], hr_prev [n,c,scale*hn,scale*wn])."""
+    name = 'stream_frame_in_resample'
+    for t, nm in ((lr_curr, 'lr_curr'), (lr_prev, 'lr_prev'), (hr_prev, 'hr_prev')):
+        _req(t, torch.float32, nm, 4)
+    n, c, hn, wn = lr_curr.shape
+    h, w = (int(v) for v in size)
+    if tuple(lr_prev.shape) != (n, c, hn, wn) or tuple(hr_prev.shape) != (n, c, scale * hn, scale * wn):
+        raise L.TecoganB200Error(f'{name}: lr_prev / hr_prev shape mismatch')
+    fmt = None
+    if layout is None:
+        _req(frames, torch.uint8, 'frames', 4)
+        fh, fw = frames.shape[1:3]
+        if frames.shape[0] != n or frames.shape[3] != c:
+            raise L.TecoganB200Error(f'{name}: frames {tuple(frames.shape)} are not [n={n},Hf,Wf,c={c}]')
+    else:
+        fmt = yuv_format(layout, color, name)
+        if c != 3:
+            raise L.TecoganB200Error(f'{name}: lr_curr has {c} channels, YUV frames decode to 3')
+        _req(frames, torch.uint16 if yuv_depth(layout) == 10 else torch.uint8, 'frames', 3)
+        fh, fw = yuv_frame_size(layout, frames.shape[1:])
+        if tuple(frames.shape) != (n, *yuv_frame_shape(layout, fh, fw)):
+            raise L.TecoganB200Error(f'{name}: frames {tuple(frames.shape)} are not n={n} {layout} frames')
+    if window is None and (fh, fw) != (h, w):
+        raise L.TecoganB200Error(f'{name}: frames of {fh}x{fw} for a {h}x{w} picture need a window')
+    tabs = []
+    for axis, (first, weights), n_in, n_out in (('rows', rows, h, hn), ('cols', cols, w, wn)):
+        _req(first, torch.int32, f'{axis} first', 1)
+        _req(weights, torch.float32, f'{axis} weights', 2)
+        if first.shape[0] != n_out or weights.shape[0] != n_out:
+            raise L.TecoganB200Error(f'{name}: {axis} tables {tuple(first.shape)} / {tuple(weights.shape)} do not '
+                                     f'give {n_out} outputs')
+        if not resample_ratio_ok(n_in, n_out):
+            raise L.TecoganB200Error(f'{name}: {axis} {n_in} -> {n_out} outside in/4 <= out <= 2*in')
+        tabs.append((first, weights, weights.shape[1]))
+    if reset is not None:
+        _req(reset, torch.int32, 'reset', 1)
+        if reset.shape[0] != n:
+            raise L.TecoganB200Error(f'{name}: reset has {reset.shape[0]} entries, expected {n}')
+    for t in (lr_prev, hr_prev, frames, reset, *rows, *cols):
+        if t is not None and t.device != lr_curr.device:
+            raise L.TecoganB200Error(f'{name}: tensors on different devices')
+    win = frame_window(fh, fw, *(window or (0, 0)))
+    (rf, rw, rt), (cf, cw, ct) = tabs
+    L.check(L.load().tg_stream_frame_in_resample(_ptr(frames), ctypes.byref(fmt) if fmt is not None else None,
+                                                 int(bool(bgr)), ctypes.byref(win), h, w, _ptr(rf), _ptr(rw), rt,
+                                                 _ptr(cf), _ptr(cw), ct, _ptr(reset), _ptr(lr_curr), _ptr(lr_prev),
+                                                 _ptr(hr_prev), n, c, hn, wn, scale, _stream()),
+            'tg_stream_frame_in_resample')
+    return lr_curr
+
+
 def scene_cut_threshold_ok(threshold):
     """tg_scene_cut takes a finite threshold in (0, 100]."""
     return 0.0 < threshold <= 100.0

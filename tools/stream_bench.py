@@ -70,7 +70,17 @@ RGB -> RGB, k = 16 pushes of pinned frames and a flush, four arms alternating in
   plain_cuts32 / pad5_cuts32  the same with scene_cut=10 on clips that change shot every 32 frames in every slot
 (reported cuts counted, so the cut arms must find n * (frames / 32 - 1) of them), then with CUDA events: one batch-n
 warm-up step of the padded stream and one of a batch-1 padded stream (the cost of a warm start is p such steps), and
-tg_stream_gather per step with all slots kept (the current frame copied) and all slots loaded, with its bytes."""
+tg_stream_gather per step with all slots kept (the current frame copied) and all slots loaded, with its bytes.
+
+    python tools/stream_bench.py --insize [--frames 64] [--reps 3]
+
+measures a resized input instead (one JSON line, metric hr_frames_per_sec_4xBD_nv12_1080p_insize_540x960): the bd4
+net (10 blocks, bench weights) on 1920x1080 NV12 sources with in_size=(540, 960), NV12 2160x3840 out, against the
+same stream fed 960x540 NV12 frames directly, at n = 1 and n = 2 slots; k = 16 pushes of pinned frames (16 distinct
+frames per slot, pushed again for every chunk) with out='device', the four arms alternating in every rep.  Then, in a
+separate torch.profiler run of 16 frames of each stream, the frame-input kernel's time per step with its algorithmic
+bytes (the NV12 frames read, lr_curr written) and TB/s.  The launch count per step of both streams is reported; it
+must be the same."""
 import argparse
 import json
 import os
@@ -98,6 +108,7 @@ def main():
     ap.add_argument('--reps', type=int, default=3)
     ap.add_argument('--window', action='store_true', help='the letterboxed-video arms instead')
     ap.add_argument('--pad', action='store_true', help='the temporally padded arms instead')
+    ap.add_argument('--insize', action='store_true', help='the resized-input arms instead')
     args = ap.parse_args()
     if args.frames < 60:
         ap.error('--frames must be >= 60')
@@ -105,6 +116,8 @@ def main():
         return window_bench(args)
     if args.pad:
         return pad_bench(args)
+    if args.insize:
+        return insize_bench(args)
     import numpy as np
     import torch
     import bench
@@ -607,6 +620,74 @@ def pad_bench(args):
         'warm_start_us': {'batch_n': round(p * warm_n, 1), 'batch_1': round(p * warm_1, 1)},
         'gather_per_step': gather}))
 
+
+def insize_bench(args):
+    import numpy as np
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    import bench
+    import tecogan_b200 as T
+    from oracle import yuv_oracle as Y
+    assert torch.cuda.is_available(), 'stream_bench.py needs a GPU'
+    dev = torch.device('cuda', 0)
+    torch.cuda.set_device(dev)
+    bench.select_workload('bd4')
+    t, k = args.frames, 16
+    net = T.FRNet(3, 3, 64, 10, 'BD', bench.SCALE)
+    net.load_state_dict(bench.make_params(), strict=True)
+    net = net.to(dev).eval()
+    rng = np.random.default_rng(7)
+
+    def source(n, h, w):
+        """n x k smooth RGB frames (noise upsampled 8x, shifted a pixel a frame) as pinned NV12 [n,k,3h/2,w]."""
+        base = rng.integers(0, 256, (n, h // 8 + 1, w // 8 + 2, 3)).astype(np.uint8)
+        big = np.repeat(np.repeat(base, 8, 1), 8, 2)
+        rgb = np.stack([big[:, :h, i:i + w] for i in range(k)], 1)
+        return torch.from_numpy(Y.rgb_to_yuv420(np.ascontiguousarray(rgb), 'nv12')).pin_memory()
+
+    arms, opened, frames = {}, {}, {}
+    for n in (1, 2):
+        frames[n] = (source(n, 1080, 1920), source(n, 540, 960))
+        arms[f'insize_1080p_n{n}'] = (n, 0, dict(in_size=(540, 960)))
+        arms[f'direct_540p_n{n}'] = (n, 1, {})
+    for name, (n, i, kw) in arms.items():
+        h, w = (1080, 1920) if i == 0 else (540, 960)
+        opened[name] = net.stream(n, h, w, device=dev, input='nv12', out_format='nv12', **kw)
+    runs = {name: [] for name in arms}
+    for rep in range(args.reps + 1):                   # rep 0: untimed warm-up (graph capture)
+        for name, (n, i, _) in arms.items():
+            st, src = opened[name], frames[n][i]
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            for _ in range(0, t, k):
+                out = st.push(src, out='device')
+            torch.cuda.synchronize()
+            fps = n * t / (time.perf_counter() - t0)
+            assert tuple(out.shape) == (n, k, 3240, 3840)
+            if rep:
+                runs[name].append(fps)
+    launches = {name: st._engine.launches_per_step for name, st in opened.items()}
+    frame_in = {}
+    for name, (n, i, _) in arms.items():
+        st, src = opened[name], frames[n][i]
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            st.push(src, out='device')
+            torch.cuda.synchronize()
+        kern = 'frame_in_resample_kernel' if i == 0 else 'stream_frame_in_kernel'
+        evs = [e for e in prof.events() if e.device_type.name == 'CUDA' and kern in e.name]
+        us = sum(e.time_range.elapsed_us() for e in evs) / len(evs) if evs else float("nan")
+        h, w = (1080, 1920) if i == 0 else (540, 960)
+        nbytes = n * (h * w * 3 // 2 + 3 * 540 * 960 * 4)
+        frame_in[name] = dict(kernel=kern, launches=len(evs), us=round(us, 2), bytes=nbytes,
+                              tb_per_s=round(nbytes / us / 1e6, 3))
+    for st in opened.values():
+        st.close()
+    print(json.dumps({
+        'metric': 'hr_frames_per_sec_4xBD_nv12_1080p_insize_540x960', 'gpu': torch.cuda.get_device_name(dev),
+        'power_limit_w': power_limit_w(), 'frames': t, 'reps': args.reps, 'push': k,
+        'median': {name: round(statistics.median(v), 1) for name, v in runs.items()},
+        'runs': {name: [round(x, 1) for x in v] for name, v in runs.items()}, 'launches_per_step': launches,
+        'frame_in_per_step': frame_in}))
 
 
 if __name__ == '__main__':
