@@ -7,6 +7,7 @@ uint8 conversion per frame; here a frame is one graph replay, the uint8/HWC conv
 kernel (tg_float_to_uint8_nhwc) and the copies overlap compute on side streams.
 """
 import collections
+import functools
 import math
 import numbers
 import os
@@ -20,6 +21,19 @@ from . import ops
 
 def _use_graph():
     return os.environ.get('TECOGAN_B200_GRAPH', '1') != '0'
+
+
+def _record(stream):
+    """A new event recorded on `stream`."""
+    e = torch.cuda.Event()
+    e.record(stream)
+    return e
+
+
+def _wait(stream, event):
+    """`stream` waits for `event`; None: nothing to wait for."""
+    if event is not None:
+        stream.wait_event(event)
 
 
 class ClipEngine:
@@ -42,6 +56,8 @@ class ClipEngine:
             self.d2h = torch.cuda.Stream(device=dev)
             self.launches_per_step = None
             self.stage = None
+            self.in_free = [None, None]      # event: the staging buffer of parity p is free for the next H2D
+            self.out_copied = [None, None]   # event: the D2H of parity p's output finished
             if self.use_graph:
                 self._capture()
 
@@ -114,37 +130,72 @@ class ClipEngine:
             self.main.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(self.main):
                 self.reset()
-            staged = [None, None]          # H2D into stage[q] finished
-            consumed = [None, None]        # stage[q] copied into lr[] (free for the next H2D)
-            out_copied = [None, None]      # D2H of u8[p] finished
+            self.in_free = [None, None]
+            self.out_copied = [None, None]
             self.h2d.wait_stream(self.main)
             for i in range(t):
-                p = q = i & 1
-                with torch.cuda.stream(self.h2d):
-                    if consumed[q] is not None:
-                        self.h2d.wait_event(consumed[q])
-                    for k in range(self.n):
-                        self.stage[q][k].copy_(lr_host[k, i], non_blocking=True)
-                    staged[q] = torch.cuda.Event()
-                    staged[q].record(self.h2d)
+                p = i & 1
+                staged = self._stage(self.stage[p], lr_host[:, i], self.in_free[p])
                 with torch.cuda.stream(self.main):
-                    self.main.wait_event(staged[q])
-                    self.lr[p].copy_(self.stage[q], non_blocking=True)
-                    consumed[q] = torch.cuda.Event()
-                    consumed[q].record(self.main)
-                    if out_copied[p] is not None:
-                        self.main.wait_event(out_copied[p])    # u8[p] free to overwrite
-                    self.run_frame(p)
-                    done = torch.cuda.Event()
-                    done.record(self.main)
-                with torch.cuda.stream(self.d2h):
-                    self.d2h.wait_event(done)
-                    out_host[i].copy_(self.u8[p], non_blocking=True)
-                    out_copied[p] = torch.cuda.Event()
-                    out_copied[p].record(self.d2h)
-            self.d2h.synchronize()
-            self.main.synchronize()
+                    self.main.wait_event(staged)
+                    self.lr[p].copy_(self.stage[p], non_blocking=True)
+                    self.in_free[p] = _record(self.main)
+                    done = self._step(p, True)
+                self._drain(p, done, out_host[i], self.u8[p], True, per_slot=False)
+            self._finish(None, True)
         return out_host
+
+    # the copy pipeline of run_clips and the streams: H2D stream -> main stream -> D2H stream, one event per hand-over
+    def _stage(self, dst, src, free):
+        """On the H2D stream, once the event `free` (None: at once) has passed: dst[k] := src[k] for every slot.
+        Returns the event of the copies."""
+        with torch.cuda.stream(self.h2d):
+            _wait(self.h2d, free)
+            for k in range(self.n):
+                dst[k].copy_(src[k], non_blocking=True)
+            return _record(self.h2d)
+
+    def _step(self, p, out_host, report=None):
+        """On the current (main) stream: the step of parity p, after the D2H of its last output (host output), then the
+        copy report = (dst, src) if given.  Returns the event of the step."""
+        if out_host:
+            _wait(self.main, self.out_copied[p])      # the output buffer is free to overwrite
+        self.run_frame(p)
+        if report is not None:
+            report[0].copy_(report[1], non_blocking=True)
+        return _record(self.main)
+
+    def _drain(self, p, done, dst, src, out_host, per_slot=True):
+        """dst := src, the output of the step of parity p whose event is `done`: host output on the D2H stream, one copy
+        per slot (per_slot) or one, then out_copied[p]; device output on the main stream, one copy."""
+        if not out_host:
+            with torch.cuda.stream(self.main):
+                dst.copy_(src, non_blocking=True)
+            return
+        with torch.cuda.stream(self.d2h):
+            self.d2h.wait_event(done)
+            for d, s in zip(dst, src) if per_slot else ((dst, src),):
+                d.copy_(s, non_blocking=True)
+            self.out_copied[p] = _record(self.d2h)
+
+    def _finish(self, cur, out_host, report=None):
+        """End of a call: host output -> the report [k,...] (if any) copied to pinned host memory and one
+        synchronisation; device output -> the current stream `cur` waits for the work of the call.  Returns the report
+        as the caller reads it."""
+        if out_host:
+            if report is not None:       # the D2H stream has waited on the last replay's event
+                k = report.shape[0]
+                if self._report_host is None or self._report_host.shape[0] < k:
+                    self._report_host = torch.empty(self._report_dev.shape, dtype=torch.int32, pin_memory=True)
+                with torch.cuda.stream(self.d2h):
+                    self.d2h.wait_stream(self.main)
+                    self._report_host[:k].copy_(report, non_blocking=True)
+                report = self._report_host[:k]
+            self.d2h.synchronize()   # after every step (D2H waited on each) and so after every H2D
+        else:
+            cur.wait_stream(self.main)
+            cur.wait_stream(self.h2d)    # a device input may be freed once the call returns
+        return report
 
 
 # Engines are cached per net (weakly: deleting the net frees its engines) and per clip geometry,
@@ -264,10 +315,10 @@ class StreamEngine(ClipEngine):
     def __init__(self, net, n, c, h, w, device, u8_input=True, bgr=False, yuv_in=None, yuv_out=None,
                  in_color='bt601', out_color='bt601', out_size=None, resize_filter='bicubic', scene_cut=None,
                  crop=None, out_frame=None, in_picture=None, in_filter='bicubic'):
-        dev = torch.device(device)
-        self.u8_input, self.bgr = u8_input or yuv_in is not None, bgr
-        self.yuv_in, self.yuv_out = yuv_in, yuv_out          # None or one of ops.YUV_LAYOUTS
-        self.in_color, self.out_color = in_color, out_color
+        # lr / hr / u8 and the streams; the graphs are captured at the end, once the buffers below exist
+        super().__init__(net, n, c, h, w, device, use_graph=False)
+        dev, s = self.device, net.scale
+        self.u8_input = u8_input or yuv_in is not None
         self.mask = [torch.zeros(n, dtype=torch.int32, device=dev) for _ in range(2)]
         self.crop = tuple(crop) if crop else None            # (Hf, Wf, top, left) of the input frames
         self.out_frame = tuple(out_frame) if out_frame else None   # (Hf, Wf, y, x) of the output frames
@@ -278,37 +329,68 @@ class StreamEngine(ClipEngine):
         in_dtype = torch.int16 if yuv_in and ops.yuv_depth(yuv_in) == 10 else torch.uint8
         self.inp = ([torch.zeros(n, *frame, dtype=in_dtype, device=dev).view(_word_dtype(yuv_in)) for _ in range(2)]
                     if self.u8_input else None)
+        # the frame input, called as frame_in(frames, reset=, lr_curr=, lr_prev=, hr_prev=)
+        in_window = self.crop[2:] if self.crop else None       # (top, left) of the picture in the input frames
         self.in_tables = None
         if self.in_picture:
             self.in_tables = [tuple(t.to(dev) for t in ops.resample_table(a, b, in_filter))
                               for a, b in zip(self.in_picture, (h, w))]
-        H, W = net.scale * h, net.scale * w
+            self.frame_in = functools.partial(ops.stream_frame_in_resample, layout=yuv_in, color=in_color, scale=s,
+                                              rows=self.in_tables[0], cols=self.in_tables[1], size=self.in_picture,
+                                              bgr=bgr, window=in_window)
+        elif yuv_in in YUV420 and in_color == 'bt601' and in_window is None:
+            self.frame_in = functools.partial(ops.stream_frame_in_yuv420, layout=yuv_in, scale=s)
+        elif yuv_in:
+            # the windowed entry point has no BT.601-only twin: its bt601 row is the same cv2 conversion
+            self.frame_in = functools.partial(ops.stream_frame_in_yuv, layout=yuv_in, color=in_color, scale=s,
+                                              window=in_window)
+        else:
+            self.frame_in = functools.partial(ops.stream_frame_in, scale=s, bgr=bgr, window=in_window)
+        # the output: per parity the step's own uint8 output step_u8[p] (or None), the calls after the step writes[p]
+        # and the frames the copies out read res[p]
+        H, W = self.H, self.W
         self.out_size = tuple(out_size) if out_size else None
         Ho, Wo = self.out_size or (H, W)
-        self.tables, self.rs = None, None
-        if self.out_size:
-            self.tables = [tuple(t.to(dev) for t in ops.resample_table(a, b, resize_filter))
-                           for a, b in ((H, Ho), (W, Wo))]
-            f32 = yuv_out is not None and ops.yuv_depth(yuv_out) == 10
-            self.rs = [torch.empty((n, c, Ho, Wo) if f32 else (n, Ho, Wo, c),
-                                   dtype=torch.float32 if f32 else torch.uint8, device=dev) for _ in range(2)]
+        out_window = self.out_frame[2:] if self.out_frame else None     # (y, x) of the picture in the output frames
         Yf, Xf = self.out_frame[:2] if self.out_frame else (Ho, Wo)
-        self.yuv = ([torch.empty(n, *ops.yuv_frame_shape(yuv_out, Yf, Xf), dtype=_word_dtype(yuv_out), device=dev)
-                     for _ in range(2)]
-                    if yuv_out else None)
-        self.pad = None
+        ten = yuv_out is not None and ops.yuv_depth(yuv_out) == 10
+        self.yuv = self.pad = self.rs = self.tables = None
+        if yuv_out:
+            self.yuv = [torch.empty(n, *ops.yuv_frame_shape(yuv_out, Yf, Xf), dtype=_word_dtype(yuv_out), device=dev)
+                        for _ in range(2)]
+        elif self.out_frame:
+            self.pad = [torch.empty((n, Yf, Xf, c), dtype=torch.uint8, device=dev) for _ in range(2)]
         if self.out_frame:
             # on dev's current stream, which the capture's warm-up stream waits for: the fill is ordered before every
             # write of the picture
             with torch.cuda.device(dev):
-                if yuv_out:
-                    for t in self.yuv:
-                        ops.fill_black(t, yuv_out, out_color)
-                else:
-                    self.pad = [ops.fill_black(torch.empty((n, Yf, Xf, c), dtype=torch.uint8, device=dev))
-                                for _ in range(2)]
+                for t in self.yuv or self.pad:
+                    ops.fill_black(t, yuv_out, out_color)
+        if self.out_size:
+            self.tables = [tuple(t.to(dev) for t in ops.resample_table(a, b, resize_filter))
+                           for a, b in ((H, Ho), (W, Wo))]
+            if not self.pad:      # uint8 [n,Ho,Wo,c], or fp32 [n,c,Ho,Wo] when a 10-bit encode follows
+                self.rs = [torch.empty((n, c, Ho, Wo) if ten else (n, Ho, Wo, c),
+                                       dtype=torch.float32 if ten else torch.uint8, device=dev) for _ in range(2)]
+        src = self.rs or (self.hr if ten else self.u8)          # what an encode reads
+        self.step_u8 = self.u8 if not self.out_size and not self.pad else [None, None]
+        self.writes = [[], []]
+        for p, calls in enumerate(self.writes):
+            if self.out_size:
+                dst = (dict(out_u8=self.pad[p], window=out_window) if self.pad else
+                       {'out_f32' if ten else 'out_u8': self.rs[p]})
+                calls.append(functools.partial(ops.resample, self.hr[p], *self.tables, **dst))
+            elif self.pad:
+                # the picture goes straight into the padded frame: the windowed writer replaces the step's uint8 output
+                calls.append(functools.partial(ops.float_to_uint8_nhwc_window, self.hr[p], self.pad[p], out_window))
+            if yuv_out in YUV420 and out_color == 'bt601' and out_window is None:
+                calls.append(functools.partial(ops.rgb_u8_to_yuv420, src[p], yuv_out, out=self.yuv[p]))
+            elif yuv_out:
+                # 10 bit: from the step's fp32 HR frame (or its resize), two more bits than the uint8 output keeps
+                calls.append(functools.partial(ops.rgb_to_yuv, yuv_out, out_color, out=self.yuv[p], window=out_window,
+                                               **{'rgb_f32' if ten else 'rgb_u8': src[p]}))
+        self.res = self.yuv or self.pad or self.rs or self.u8
         self.scene_cut = scene_cut
-        self.prev_mafd = self.work = self.rep = self.score = self.cut = None
         self.report = None               # [k,3n] int32 of the last run: score[p] / cut[p] after each frame
         self._report_dev = self._report_host = None
         if scene_cut is not None:
@@ -320,21 +402,15 @@ class StreamEngine(ClipEngine):
         self.sig = _param_signature(net)
         self.parity = 0                  # parity of the next frame
         self.mask_set = [False, False]   # mask[p] holds a reset pattern (cleared before the next replay)
-        self.in_free = [None, None]      # event: the replay that last read inp[p] / stage[p] finished
-        self.out_copied = [None, None]   # event: the D2H of u8[p] (yuv[p]) finished
         # the capture's warm-up steps update prev_mafd; that state is never read, because the first push resets every
         # slot (VideoStream._pending) and a reset sets prev_mafd := -1 without reading it
-        super().__init__(net, n, c, h, w, dev)     # lr / hr / u8, streams, the two graphs of _enqueue below
-
-    def close(self):
-        super().close()
-        self.mask, self.inp, self.yuv, self.pad = [], None, None, None
-        self.tables, self.rs, self.in_tables = None, None, None
-        self.prev_mafd = self.work = self.rep = self.score = self.cut = self.report = None
-        self._report_dev = self._report_host = None
+        self.use_graph = _use_graph()
+        if self.use_graph:
+            self._capture()
 
     def _enqueue(self, p):
-        self._decode(self.inp[p] if self.u8_input else None, self.mask[p], self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1])
+        self.frame_in(self.inp[p] if self.inp else None, reset=self.mask[p], lr_curr=self.lr[p],
+                      lr_prev=self.lr[p ^ 1], hr_prev=self.hr[p ^ 1])
         if self.scene_cut is not None:
             ops.scene_cut(self.lr[p], self.lr[p ^ 1], self.mask[p], self.scene_cut, self.prev_mafd, self.work,
                           self.score[p], self.cut[p])
@@ -342,48 +418,11 @@ class StreamEngine(ClipEngine):
             ops.stream_frame_in(None, self.cut[p], self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1], self.net.scale)
         self._step_out(p)
 
-    def _decode(self, inp, mask, lr_curr, lr_prev, hr_prev):
-        """The frame input launch: inp (None for fp32 input) decoded into lr_curr, the slots of mask reset."""
-        crop = self.crop[2:] if self.crop else None          # (top, left)
-        if self.in_tables is not None:
-            ops.stream_frame_in_resample(inp, self.yuv_in, self.in_color, mask, lr_curr, lr_prev, hr_prev,
-                                         self.net.scale, *self.in_tables, self.in_picture, bgr=self.bgr, window=crop)
-        elif self.yuv_in in YUV420 and self.in_color == 'bt601' and crop is None:
-            ops.stream_frame_in_yuv420(inp, self.yuv_in, mask, lr_curr, lr_prev, hr_prev, self.net.scale)
-        elif self.yuv_in:
-            # the windowed entry point has no BT.601-only twin: its bt601 row is the same cv2 conversion
-            ops.stream_frame_in_yuv(inp, self.yuv_in, self.in_color, mask, lr_curr, lr_prev, hr_prev, self.net.scale,
-                                    window=crop)
-        else:
-            ops.stream_frame_in(inp, mask, lr_curr, lr_prev, hr_prev, self.net.scale, self.bgr,
-                                window=crop if self.u8_input else None)
-
     def _step_out(self, p):
         """The step of parity p on lr[p], lr[p ^ 1], hr[p ^ 1] and the writes of its output frame."""
-        pad = self.out_frame[2:] if self.out_frame else None  # (y, x)
-        if self.out_size is None and self.pad is not None:
-            # the picture goes straight into the padded frame: the windowed writer replaces the step's uint8 output
-            self.net.step_into(self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1], self.hr[p], out_u8=None)
-            ops.float_to_uint8_nhwc_window(self.hr[p], self.pad[p], pad)
-        elif self.out_size is None:
-            super()._enqueue(p)
-            rgb_u8, rgb_f32 = self.u8[p], self.hr[p]
-        else:
-            self.net.step_into(self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1], self.hr[p], out_u8=None)
-            if self.pad is not None:
-                ops.resample(self.hr[p], *self.tables, out_u8=self.pad[p], window=pad)
-            else:
-                f32 = self.rs[p].dtype == torch.float32
-                ops.resample(self.hr[p], *self.tables, out_u8=None if f32 else self.rs[p],
-                             out_f32=self.rs[p] if f32 else None)
-                rgb_u8 = rgb_f32 = self.rs[p]
-        if self.yuv_out in YUV420 and self.out_color == 'bt601' and pad is None:
-            ops.rgb_u8_to_yuv420(rgb_u8, self.yuv_out, out=self.yuv[p])
-        elif self.yuv_out and ops.yuv_depth(self.yuv_out) == 8:
-            ops.rgb_to_yuv(self.yuv_out, self.out_color, rgb_u8=rgb_u8, out=self.yuv[p], window=pad)
-        elif self.yuv_out:
-            # 10 bit: from the step's fp32 HR frame (or its resize), two more bits than the uint8 output keeps
-            ops.rgb_to_yuv(self.yuv_out, self.out_color, rgb_f32=rgb_f32, out=self.yuv[p], window=pad)
+        self.net.step_into(self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1], self.hr[p], out_u8=self.step_u8[p])
+        for write in self.writes[p]:
+            write()
 
     def _set_mask(self, p, slots):
         """On the main stream, before the replay of parity p: mask[p] = 1 for `slots`, 0 elsewhere."""
@@ -396,13 +435,9 @@ class StreamEngine(ClipEngine):
             self.mask[p].zero_()
             self.mask_set[p] = False
 
-    def _res(self):
-        """What the step graph leaves for the copy out, per parity."""
-        return self.yuv if self.yuv_out else self.pad if self.pad else self.rs if self.out_size else self.u8
-
     def _outputs(self, k, out_host):
         """The k frames a call returns (pinned host or device) and the [k,3n] report rows (scene_cut) or None."""
-        n, res = self.n, self._res()
+        n, res = self.n, self.res
         shape = (n, k, *res[0].shape[1:])
         if out_host:
             out = torch.empty(shape, dtype=res[0].dtype, pin_memory=True)
@@ -424,69 +459,30 @@ class StreamEngine(ClipEngine):
         yuv_out; Ho, Wo instead of H, W with out_size): a pinned host tensor (out_host; one synchronisation, at the end) or a new tensor on the device,
         ordered on the current stream (no synchronisation).  flush: the videos end here (this engine holds no
         frames, so it changes nothing)."""
-        n, k = self.n, 0 if frames is None else frames.shape[1]
+        k = 0 if frames is None else frames.shape[1]
         with torch.cuda.device(self.device):
             cur = torch.cuda.current_stream()
             self.net.refresh_packed_weights()        # a load_state_dict between pushes takes effect
             for st in (self.main, self.h2d, self.d2h):
                 st.wait_stream(cur)
-            res = self._res()
             out, report = self._outputs(k, out_host)
             if not self.u8_input and self.stage is None:
                 self.stage = [torch.empty_like(self.lr[0]) for _ in range(2)]
             dst = self.inp if self.u8_input else self.stage
             for i in range(k):
                 p = self.parity
-                with torch.cuda.stream(self.h2d):
-                    if self.in_free[p] is not None:
-                        self.h2d.wait_event(self.in_free[p])
-                    for j in range(n):
-                        dst[p][j].copy_(frames[j, i], non_blocking=True)
-                    staged = torch.cuda.Event()
-                    staged.record(self.h2d)
+                staged = self._stage(dst[p], frames[:, i], self.in_free[p])
                 with torch.cuda.stream(self.main):
                     self.main.wait_event(staged)
                     if not self.u8_input:
                         self.lr[p].copy_(self.stage[p], non_blocking=True)
                     self._set_mask(p, reset_slots if i == 0 else None)
-                    if out_host and self.out_copied[p] is not None:
-                        self.main.wait_event(self.out_copied[p])     # res[p] free to overwrite
-                    self.run_frame(p)
-                    if report is not None:
-                        report[i].copy_(self.rep[p], non_blocking=True)
-                    done = torch.cuda.Event()
-                    done.record(self.main)
-                    self.in_free[p] = done
-                    if not out_host:
-                        out[:, i].copy_(res[p], non_blocking=True)
-                if out_host:
-                    with torch.cuda.stream(self.d2h):
-                        self.d2h.wait_event(done)
-                        for j in range(n):
-                            out[j, i].copy_(res[p][j], non_blocking=True)
-                        self.out_copied[p] = torch.cuda.Event()
-                        self.out_copied[p].record(self.d2h)
+                    copy = None if report is None else (report[i], self.rep[p])
+                    self.in_free[p] = done = self._step(p, out_host, copy)
+                self._drain(p, done, out[:, i], self.res[p], out_host)
                 self.parity ^= 1
-            report = self._finish(cur, report, k, out_host)
-        self.report = report
+            self.report = self._finish(cur, out_host, report)
         return out
-
-    def _finish(self, cur, report, k, out_host):
-        """End of a call: host output -> the report copied to the host and one synchronisation; device output -> the
-        current stream waits for the work of the call.  Returns the report as the caller reads it."""
-        if out_host:
-            if report is not None:       # the D2H stream has waited on the last replay's event
-                if self._report_host is None or self._report_host.shape[0] < k:
-                    self._report_host = torch.empty(self._report_dev.shape, dtype=torch.int32, pin_memory=True)
-                with torch.cuda.stream(self.d2h):
-                    self.d2h.wait_stream(self.main)
-                    self._report_host[:k].copy_(report, non_blocking=True)
-                report = self._report_host[:k]
-            self.d2h.synchronize()   # after every replay (D2H waited on each) and so after every H2D
-        else:
-            cur.wait_stream(self.main)
-            cur.wait_stream(self.h2d)    # a device input may be freed once the call returns
-        return report
 
 
 # ------------------------------------------------------------------------------------------ temporal padding
@@ -633,12 +629,6 @@ class PaddedStreamEngine(StreamEngine):
             self.in_mask = torch.zeros(n, dtype=torch.int32, device=dev)
         super().__init__(net, n, c, h, w, dev, **kw)
 
-    def close(self):
-        super().close()
-        self.ring = self.rep_ring = self.cut_host = self.in_mask = None
-        self.wlr = self.whr = self.mtab = self.wtab = []
-        self.warm_graphs = [None, None]
-
     def _enqueue(self, p):
         ops.stream_gather(self.ring, self.mtab[p], self.whr[0], self.lr[p], self.lr[p ^ 1], self.hr[p ^ 1],
                           self.net.scale)
@@ -706,36 +696,24 @@ class PaddedStreamEngine(StreamEngine):
                 self.ingest.synchronize()              # the H2D of the frames held for later steps too
             else:
                 cur.wait_stream(self.ingest)
-            report = self._finish(cur, report, k_out, out_host)
-        self.report = report
+            self.report = self._finish(cur, out_host, report)
         return out
 
     def _ingest(self, frames, i, reset_slots):
         t, n = self.sched.t_in, self.n
         r = t % self.depth
         q = t & 1                                      # staging buffer of uint8 / YUV input
-        with torch.cuda.stream(self.h2d):
-            if self.u8_input:
-                if self.in_free[q] is not None:
-                    self.h2d.wait_event(self.in_free[q])
-                dst = self.inp[q]
-            else:                                      # fp32 frames land in the ring directly
-                if self.ring_free[r] is not None:
-                    self.h2d.wait_event(self.ring_free[r])
-                dst = self.ring[r]
-            for j in range(n):
-                dst[j].copy_(frames[j, i], non_blocking=True)
-            staged = torch.cuda.Event()
-            staged.record(self.h2d)
+        if self.u8_input:
+            staged = self._stage(self.inp[q], frames[:, i], self.in_free[q])
+        else:                                          # fp32 frames land in the ring directly
+            staged = self._stage(self.ring[r], frames[:, i], self.ring_free[r])
         with torch.cuda.stream(self.ingest):
             self.ingest.wait_event(staged)
-            if self.ring_free[r] is not None:
-                self.ingest.wait_event(self.ring_free[r])
+            _wait(self.ingest, self.ring_free[r])
             if self.u8_input:
                 # no reset: lr_prev / hr_prev are not touched
-                self._decode(self.inp[q], None, self.ring[r], self.lr[0], self.hr[0])
-                self.in_free[q] = torch.cuda.Event()
-                self.in_free[q].record(self.ingest)
+                self.frame_in(self.inp[q], reset=None, lr_curr=self.ring[r], lr_prev=self.lr[0], hr_prev=self.hr[0])
+                self.in_free[q] = _record(self.ingest)
             if self.scene_cut is not None:
                 mask = None
                 if reset_slots:
@@ -747,8 +725,7 @@ class PaddedStreamEngine(StreamEngine):
                 ops.scene_cut(self.ring[r], self.ring[(t - 1) % self.depth], mask, self.scene_cut, self.prev_mafd,
                               self.work, rep[:2 * n].view(torch.float64), rep[2 * n:3 * n])
                 self.cut_host[r].copy_(rep[2 * n:3 * n], non_blocking=True)
-            self.ingested = torch.cuda.Event()
-            self.ingested.record(self.ingest)
+            self.ingested = _record(self.ingest)
         cuts = ()
         if self.scene_cut is not None:
             self.ingested.synchronize()                # the ingest only: decode, score and the flag copy
@@ -757,7 +734,7 @@ class PaddedStreamEngine(StreamEngine):
 
     def _emit(self, row, out, report, out_host, j, warm, main):
         """Warm-ups and main step of frame j, its output into out[:, row] and its report into report[row]."""
-        res = self._res()
+        r = j % self.depth
         with torch.cuda.stream(self.main):
             self.main.wait_event(self.ingested)       # frames up to t_in - 1 are in the ring
             for i, step in enumerate(warm):
@@ -766,23 +743,9 @@ class PaddedStreamEngine(StreamEngine):
                 self.run_warm(q)
             p = self.parity
             self._load_table(self.mtab[p], main)
-            if out_host and self.out_copied[p] is not None:
-                self.main.wait_event(self.out_copied[p])
-            self.run_frame(p)
-            if report is not None:
-                report[row].copy_(self.rep_ring[j % self.depth, :3 * self.n], non_blocking=True)
-            done = torch.cuda.Event()
-            done.record(self.main)
-            self.ring_free[j % self.depth] = done
-            if not out_host:
-                out[:, row].copy_(res[p], non_blocking=True)
-        if out_host:
-            with torch.cuda.stream(self.d2h):
-                self.d2h.wait_event(done)
-                for k in range(self.n):
-                    out[k, row].copy_(res[p][k], non_blocking=True)
-                self.out_copied[p] = torch.cuda.Event()
-                self.out_copied[p].record(self.d2h)
+            copy = None if report is None else (report[row], self.rep_ring[r, :3 * self.n])
+            self.ring_free[r] = done = self._step(p, out_host, copy)
+        self._drain(p, done, out[:, row], self.res[p], out_host)
         self.parity ^= 1
 
 
@@ -849,12 +812,9 @@ class VideoStream:
         # the input layout holds the pushed h x w frames; the output layout's picture comes from the ph x pw picture
         # the net runs on (the whole frame without crop)
         for f, (a, b) in ((input, (h, w)), (out_format, (ph, pw))):
-            if f not in YUV:
-                continue
-            if f not in _YUV_422_444 and (a % 2 or b % 2):
-                raise ValueError(f'{f} frames are YUV 4:2:0: h and w must be even, got {a}x{b}')
-            if f in ops.YUV422_LAYOUTS and b % 2:
-                raise ValueError(f'{f} frames are YUV 4:2:2: w must be even, got {a}x{b}')
+            err = f in YUV and ops.yuv_size_error(f, a, b)
+            if err:
+                raise ValueError(f'{f} frames: {err}')
         if out_frame is None and out_origin is not None:
             raise ValueError('out_origin applies to a padded output only (give out_frame)')
         if out_frame is not None:
@@ -1083,10 +1043,9 @@ def _check_out_size(out_size, H, W, out_format):
     if not (ops.resample_ratio_ok(H, Ho) and ops.resample_ratio_ok(W, Wo)):
         raise ValueError(f'out_size {Ho}x{Wo} from a {H}x{W} output: each axis must be within 1/4 to 2 times the '
                          f'output size')
-    if out_format in YUV and out_format not in _YUV_422_444 and (Ho % 2 or Wo % 2):
-        raise ValueError(f'{out_format} frames are YUV 4:2:0: out_size must be even, got {Ho}x{Wo}')
-    if out_format in ops.YUV422_LAYOUTS and Wo % 2:
-        raise ValueError(f'{out_format} frames are YUV 4:2:2: the width of out_size must be even, got {Ho}x{Wo}')
+    err = out_format in YUV and ops.yuv_size_error(out_format, Ho, Wo)
+    if err:
+        raise ValueError(f'{out_format} frames: out_size {Ho}x{Wo}: {err}')
     return Ho, Wo
 
 

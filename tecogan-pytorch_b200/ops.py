@@ -383,33 +383,64 @@ def frame_window(frame_h, frame_w, top, left):
     return L.FrameWindow(int(frame_h), int(frame_w), int(top), int(left))
 
 
+def _step_state(name, reset, lr_curr, lr_prev, hr_prev, scale):
+    """Checks the step state a frame input writes: lr_curr / lr_prev fp32 [n,c,h,w], hr_prev fp32 [n,c,scale*h,scale*w]
+    and reset int32 [n] or None.  -> (n, c, h, w)"""
+    for t, nm in ((lr_curr, 'lr_curr'), (lr_prev, 'lr_prev'), (hr_prev, 'hr_prev')):
+        _req(t, torch.float32, nm, 4)
+    n, c, h, w = lr_curr.shape
+    if tuple(lr_prev.shape) != (n, c, h, w) or tuple(hr_prev.shape) != (n, c, scale * h, scale * w):
+        raise L.TecoganB200Error(f'{name}: lr_prev / hr_prev shape mismatch')
+    if reset is not None:
+        _req(reset, torch.int32, 'reset', 1)
+        if reset.shape[0] != n:
+            raise L.TecoganB200Error(f'{name}: reset has {reset.shape[0]} entries, expected {n}')
+    return n, c, h, w
+
+
+def _frames(name, frames, layout, n, c, h, w, window):
+    """Checks the frames an h x w picture of n slots is read from: uint8 HWC [n,Hf,Wf,c] (layout None) or a YUV
+    layout's words [n,*yuv_frame_shape(layout, Hf, Wf)] (uint16 for the 10-bit layouts), or None (no frames).  Hf x Wf
+    is h x w, or any size when the picture is read at window = (top, left).  -> (Hf, Wf)"""
+    if layout is not None:
+        if c != 3:
+            raise L.TecoganB200Error(f'{name}: lr_curr has {c} channels, YUV frames decode to 3')
+        err = yuv_size_error(layout, h, w)
+        if err:
+            raise L.TecoganB200Error(f'{name}: {err}')
+    if frames is None:
+        return h, w
+    if layout is None:
+        _req(frames, torch.uint8, 'frames', 4)
+        fh, fw = (h, w) if window is None else frames.shape[1:3]
+        want = (n, fh, fw, c)
+    else:
+        _req(frames, torch.uint16 if yuv_depth(layout) == 10 else torch.uint8, 'frames', 3)
+        fh, fw = (h, w) if window is None else yuv_frame_size(layout, frames.shape[1:])
+        want = (n, *yuv_frame_shape(layout, fh, fw))
+    if tuple(frames.shape) != want:
+        raise L.TecoganB200Error(f'{name}: frames {tuple(frames.shape)} != {want} ({layout or "uint8 HWC"} frames of '
+                                 f'{fh}x{fw})')
+    return fh, fw
+
+
+def _same_device(name, x, *tensors):
+    for t in tensors:
+        if t is not None and t.device != x.device:
+            raise L.TecoganB200Error(f'{name}: tensors on different devices')
+
+
 def stream_frame_in(u8, reset, lr_curr, lr_prev, hr_prev, scale, bgr=False, window=None):
     """Frame input of a streamed step (tg_stream_frame_in): u8 uint8 [n,h,w,c] (or None) -> lr_curr fp32
     [n,c,h,w] = u8 / 255, channels reversed when bgr; slots k with reset[k] != 0 (int32 [n] on the device,
     or None) get lr_prev[k] = hr_prev[k] = 0 ([n,c,h,w] / [n,c,scale*h,scale*w] fp32).  With window = (top, left),
     u8 is [n,Hf,Wf,c] and the h x w picture at (top, left) of each frame is read (tg_stream_frame_in_window)."""
-    _req(lr_curr, torch.float32, 'lr_curr', 4)
-    _req(lr_prev, torch.float32, 'lr_prev', 4)
-    _req(hr_prev, torch.float32, 'hr_prev', 4)
-    n, c, h, w = lr_curr.shape
-    if tuple(lr_prev.shape) != (n, c, h, w) or tuple(hr_prev.shape) != (n, c, scale * h, scale * w):
-        raise L.TecoganB200Error('stream_frame_in: lr_prev / hr_prev shape mismatch')
-    if u8 is not None:
-        _req(u8, torch.uint8, 'frames', 4)
-        if window is not None:
-            if u8.shape[0] != n or u8.shape[3] != c:
-                raise L.TecoganB200Error(f'stream_frame_in: frames {tuple(u8.shape)} are not [n={n},Hf,Wf,c={c}]')
-        elif tuple(u8.shape) != (n, h, w, c):
-            raise L.TecoganB200Error(f'stream_frame_in: frames {tuple(u8.shape)} != {(n, h, w, c)} (nhwc)')
-    if reset is not None:
-        _req(reset, torch.int32, 'reset', 1)
-        if reset.shape[0] != n:
-            raise L.TecoganB200Error(f'stream_frame_in: reset has {reset.shape[0]} entries, expected {n}')
-    for t in (lr_prev, hr_prev, u8, reset):
-        if t is not None and t.device != lr_curr.device:
-            raise L.TecoganB200Error('stream_frame_in: tensors on different devices')
+    name = 'stream_frame_in'
+    n, c, h, w = _step_state(name, reset, lr_curr, lr_prev, hr_prev, scale)
+    fh, fw = _frames(name, u8, None, n, c, h, w, window)
+    _same_device(name, lr_curr, lr_prev, hr_prev, u8, reset)
     if window is not None:
-        win = frame_window(u8.shape[1], u8.shape[2], *window) if u8 is not None else frame_window(h, w, 0, 0)
+        win = frame_window(fh, fw, *window) if u8 is not None else frame_window(h, w, 0, 0)
         L.check(L.load().tg_stream_frame_in_window(_ptr(u8), ctypes.byref(win), _ptr(reset), _ptr(lr_curr),
                                                    _ptr(lr_prev), _ptr(hr_prev), n, c, h, w, scale, int(bool(bgr)),
                                                    _stream()), 'tg_stream_frame_in_window')
@@ -426,22 +457,18 @@ def stream_gather(ring, table, warm_hr, lr_curr, lr_prev, hr_prev, scale):
     lr_prev[k] = ring[prev[k]][k] (0 for prev[k] < 0), hr_prev[k] = warm_hr[k]."""
     name = 'stream_gather'
     _req(ring, torch.float32, 'ring', 5)
-    for t, nm in ((lr_curr, 'lr_curr'), (lr_prev, 'lr_prev'), (hr_prev, 'hr_prev')):
-        _req(t, torch.float32, nm, 4)
     depth, n, c, h, w = ring.shape
-    H, W = scale * h, scale * w
-    if tuple(lr_curr.shape) != (n, c, h, w) or tuple(lr_prev.shape) != (n, c, h, w):
-        raise L.TecoganB200Error(f'{name}: lr_curr / lr_prev are not [n={n},c={c},h={h},w={w}]')
-    if tuple(hr_prev.shape) != (n, c, H, W) or (warm_hr is not None and tuple(warm_hr.shape) != (n, c, H, W)):
-        raise L.TecoganB200Error(f'{name}: hr_prev / warm_hr are not [n={n},c={c},{H},{W}]')
+    _step_state(name, None, lr_curr, lr_prev, hr_prev, scale)
+    if tuple(lr_curr.shape) != (n, c, h, w):
+        raise L.TecoganB200Error(f'{name}: lr_curr {tuple(lr_curr.shape)} is not [n={n},c={c},h={h},w={w}]')
     if warm_hr is not None:
         _req(warm_hr, torch.float32, 'warm_hr', 4)
+        if warm_hr.shape != hr_prev.shape:
+            raise L.TecoganB200Error(f'{name}: warm_hr {tuple(warm_hr.shape)} != hr_prev {tuple(hr_prev.shape)}')
     _req(table, torch.int32, 'table', 1)
     if table.shape[0] != 3 * n:
         raise L.TecoganB200Error(f'{name}: table has {table.shape[0]} entries, expected {3 * n}')
-    for t in (table, warm_hr, lr_curr, lr_prev, hr_prev):
-        if t is not None and t.device != ring.device:
-            raise L.TecoganB200Error(f'{name}: tensors on different devices')
+    _same_device(name, ring, table, warm_hr, lr_curr, lr_prev, hr_prev)
     L.check(L.load().tg_stream_gather(_ptr(ring), depth, _ptr(table), _ptr(warm_hr), _ptr(lr_curr), _ptr(lr_prev),
                                       _ptr(hr_prev), n, c, h, w, scale, _stream()), 'tg_stream_gather')
     return lr_curr
@@ -460,27 +487,11 @@ def stream_frame_in_yuv420(yuv, layout, reset, lr_curr, lr_prev, hr_prev, scale)
     """stream_frame_in from YUV 4:2:0 frames (tg_stream_frame_in_yuv420): yuv uint8 [n,3h/2,w] in layout 'nv12' or
     'i420' (or None) -> lr_curr fp32 [n,3,h,w] = cv2.cvtColor(frame, COLOR_YUV2RGB_<layout>) / 255; reset as in
     stream_frame_in."""
-    nv12 = _yuv_layout(layout, 'stream_frame_in_yuv420')
-    _req(lr_curr, torch.float32, 'lr_curr', 4)
-    _req(lr_prev, torch.float32, 'lr_prev', 4)
-    _req(hr_prev, torch.float32, 'hr_prev', 4)
-    n, c, h, w = lr_curr.shape
-    if c != 3:
-        raise L.TecoganB200Error(f'stream_frame_in_yuv420: lr_curr has {c} channels, YUV frames decode to 3')
-    if tuple(lr_prev.shape) != (n, c, h, w) or tuple(hr_prev.shape) != (n, c, scale * h, scale * w):
-        raise L.TecoganB200Error('stream_frame_in_yuv420: lr_prev / hr_prev shape mismatch')
-    if yuv is not None:
-        _req(yuv, torch.uint8, 'frames', 3)
-        if tuple(yuv.shape) != (n, 3 * h // 2, w) or h % 2:
-            raise L.TecoganB200Error(f'stream_frame_in_yuv420: frames {tuple(yuv.shape)} != '
-                                     f'{(n, 3 * h // 2, w)} ([n,3h/2,w], h even)')
-    if reset is not None:
-        _req(reset, torch.int32, 'reset', 1)
-        if reset.shape[0] != n:
-            raise L.TecoganB200Error(f'stream_frame_in_yuv420: reset has {reset.shape[0]} entries, expected {n}')
-    for t in (lr_prev, hr_prev, yuv, reset):
-        if t is not None and t.device != lr_curr.device:
-            raise L.TecoganB200Error('stream_frame_in_yuv420: tensors on different devices')
+    name = 'stream_frame_in_yuv420'
+    nv12 = _yuv_layout(layout, name)
+    n, c, h, w = _step_state(name, reset, lr_curr, lr_prev, hr_prev, scale)
+    _frames(name, yuv, layout, n, c, h, w, None)
+    _same_device(name, lr_curr, lr_prev, hr_prev, yuv, reset)
     L.check(L.load().tg_stream_frame_in_yuv420(_ptr(yuv), nv12, _ptr(reset), _ptr(lr_curr), _ptr(lr_prev),
                                                _ptr(hr_prev), n, h, w, scale, _stream()), 'tg_stream_frame_in_yuv420')
     return lr_curr
@@ -572,30 +583,9 @@ def stream_frame_in_yuv(frames, layout, color, reset, lr_curr, lr_prev, hr_prev,
     yuv_frame_shape(layout, Hf, Wf)) and the h x w picture at (top, left) is read (tg_stream_frame_in_yuv_window)."""
     name = 'stream_frame_in_yuv' if window is None else 'stream_frame_in_yuv_window'
     fmt = yuv_format(layout, color, name)
-    _req(lr_curr, torch.float32, 'lr_curr', 4)
-    _req(lr_prev, torch.float32, 'lr_prev', 4)
-    _req(hr_prev, torch.float32, 'hr_prev', 4)
-    n, c, h, w = lr_curr.shape
-    if c != 3:
-        raise L.TecoganB200Error(f'{name}: lr_curr has {c} channels, YUV frames decode to 3')
-    err = yuv_size_error(layout, h, w)
-    if err:
-        raise L.TecoganB200Error(f'{name}: {err}')
-    if tuple(lr_prev.shape) != (n, c, h, w) or tuple(hr_prev.shape) != (n, c, scale * h, scale * w):
-        raise L.TecoganB200Error(f'{name}: lr_prev / hr_prev shape mismatch')
-    if frames is not None:
-        _req(frames, torch.uint16 if yuv_depth(layout) == 10 else torch.uint8, 'frames', 3)
-        fh, fw = (h, w) if window is None else yuv_frame_size(layout, frames.shape[1:])
-        want = (n, *yuv_frame_shape(layout, fh, fw))
-        if tuple(frames.shape) != want:
-            raise L.TecoganB200Error(f'{name}: frames {tuple(frames.shape)} != {want} ({layout} frames of {fh}x{fw})')
-    if reset is not None:
-        _req(reset, torch.int32, 'reset', 1)
-        if reset.shape[0] != n:
-            raise L.TecoganB200Error(f'{name}: reset has {reset.shape[0]} entries, expected {n}')
-    for t in (lr_prev, hr_prev, frames, reset):
-        if t is not None and t.device != lr_curr.device:
-            raise L.TecoganB200Error(f'{name}: tensors on different devices')
+    n, c, h, w = _step_state(name, reset, lr_curr, lr_prev, hr_prev, scale)
+    fh, fw = _frames(name, frames, layout, n, c, h, w, window)
+    _same_device(name, lr_curr, lr_prev, hr_prev, frames, reset)
     if window is not None:
         win = frame_window(fh, fw, *window) if frames is not None else frame_window(h, w, 0, 0)
         L.check(L.load().tg_stream_frame_in_yuv_window(_ptr(frames), ctypes.byref(fmt), ctypes.byref(win),
@@ -776,28 +766,10 @@ def stream_frame_in_resample(frames, layout, color, reset, lr_curr, lr_prev, hr_
     is the whole frame, or the h x w one at window = (top, left).  reset as in stream_frame_in (lr_prev
     [n,c,hn,wn], hr_prev [n,c,scale*hn,scale*wn])."""
     name = 'stream_frame_in_resample'
-    for t, nm in ((lr_curr, 'lr_curr'), (lr_prev, 'lr_prev'), (hr_prev, 'hr_prev')):
-        _req(t, torch.float32, nm, 4)
-    n, c, hn, wn = lr_curr.shape
+    fmt = None if layout is None else yuv_format(layout, color, name)
+    n, c, hn, wn = _step_state(name, reset, lr_curr, lr_prev, hr_prev, scale)
     h, w = (int(v) for v in size)
-    if tuple(lr_prev.shape) != (n, c, hn, wn) or tuple(hr_prev.shape) != (n, c, scale * hn, scale * wn):
-        raise L.TecoganB200Error(f'{name}: lr_prev / hr_prev shape mismatch')
-    fmt = None
-    if layout is None:
-        _req(frames, torch.uint8, 'frames', 4)
-        fh, fw = frames.shape[1:3]
-        if frames.shape[0] != n or frames.shape[3] != c:
-            raise L.TecoganB200Error(f'{name}: frames {tuple(frames.shape)} are not [n={n},Hf,Wf,c={c}]')
-    else:
-        fmt = yuv_format(layout, color, name)
-        if c != 3:
-            raise L.TecoganB200Error(f'{name}: lr_curr has {c} channels, YUV frames decode to 3')
-        _req(frames, torch.uint16 if yuv_depth(layout) == 10 else torch.uint8, 'frames', 3)
-        fh, fw = yuv_frame_size(layout, frames.shape[1:])
-        if tuple(frames.shape) != (n, *yuv_frame_shape(layout, fh, fw)):
-            raise L.TecoganB200Error(f'{name}: frames {tuple(frames.shape)} are not n={n} {layout} frames')
-    if window is None and (fh, fw) != (h, w):
-        raise L.TecoganB200Error(f'{name}: frames of {fh}x{fw} for a {h}x{w} picture need a window')
+    fh, fw = _frames(name, frames, layout, n, c, h, w, window)
     tabs = []
     for axis, (first, weights), n_in, n_out in (('rows', rows, h, hn), ('cols', cols, w, wn)):
         _req(first, torch.int32, f'{axis} first', 1)
@@ -808,13 +780,7 @@ def stream_frame_in_resample(frames, layout, color, reset, lr_curr, lr_prev, hr_
         if not resample_ratio_ok(n_in, n_out):
             raise L.TecoganB200Error(f'{name}: {axis} {n_in} -> {n_out} outside in/4 <= out <= 2*in')
         tabs.append((first, weights, weights.shape[1]))
-    if reset is not None:
-        _req(reset, torch.int32, 'reset', 1)
-        if reset.shape[0] != n:
-            raise L.TecoganB200Error(f'{name}: reset has {reset.shape[0]} entries, expected {n}')
-    for t in (lr_prev, hr_prev, frames, reset, *rows, *cols):
-        if t is not None and t.device != lr_curr.device:
-            raise L.TecoganB200Error(f'{name}: tensors on different devices')
+    _same_device(name, lr_curr, lr_prev, hr_prev, frames, reset, *rows, *cols)
     win = frame_window(fh, fw, *(window or (0, 0)))
     (rf, rw, rt), (cf, cw, ct) = tabs
     L.check(L.load().tg_stream_frame_in_resample(_ptr(frames), ctypes.byref(fmt) if fmt is not None else None,
@@ -855,9 +821,7 @@ def scene_cut(lr_curr, lr_prev, reset, threshold, prev_mafd, work, score, cut):
     _req(work, torch.int64, 'work', 1)
     if work.numel() * 8 != n * L.SCENE_CUT_WORK_BYTES:
         raise L.TecoganB200Error(f'{name}: work has {work.numel() * 8} bytes, expected {n * L.SCENE_CUT_WORK_BYTES}')
-    for t in (lr_prev, reset, prev_mafd, work, score, cut):
-        if t is not None and t.device != lr_curr.device:
-            raise L.TecoganB200Error(f'{name}: tensors on different devices')
+    _same_device(name, lr_curr, lr_prev, reset, prev_mafd, work, score, cut)
     L.check(L.load().tg_scene_cut(_ptr(lr_curr), _ptr(lr_prev), n, c, h, w, _ptr(reset), float(threshold),
                                   _ptr(prev_mafd), _ptr(work), _ptr(score), _ptr(cut), _stream()), 'tg_scene_cut')
     return score, cut
