@@ -470,6 +470,37 @@ int tg_farneback(const uint8_t* gray, int groups, int t, int h, int w, const tg_
  * in float64; sums is zeroed by the call.  a, b and sums 8-byte aligned.  TG_E_INVALID: null pointers, non-positive
  * sizes, misalignment; TG_E_UNSUPPORTED: n > 65535. */
 int tg_flow_epe_sum(const float* a, const float* b, int n, int h, int w, double* sums, void* stream);
+/* Bytes of tg_flow_epe_sum_window's workspace for n pairs and a window of hc rows (0 for bad sizes). */
+size_t tg_flow_epe_sum_window_workspace_bytes(int n, int hc);
+/* tg_flow_epe_sum over the window rows y0 .. y0+hc-1, columns x0 .. x0+wc-1 of the h x w flows, with the per-CTA
+ * sums added in a fixed order through the workspace (work 8-byte aligned, work_bytes >=
+ * tg_flow_epe_sum_window_workspace_bytes): the same inputs give the same bits.  tg_flow_epe_sum is the same kernel
+ * over the whole frame with float64 atomics in place of the workspace.  TG_E_INVALID also for a window outside the
+ * flows, a null or short workspace. */
+int tg_flow_epe_sum_window(const float* a, const float* b, int n, int h, int w, int y0, int x0, int hc, int wc,
+                           double* sums, void* work, size_t work_bytes, void* stream);
+
+/* The official metric script (codes/official_metrics/metrics.py, oracle/official_metrics.py) scores the Y of
+ * _rgb2ycbcr, Y = float64 r*T0 + g*T1 + b*T2 + 16 left to right without FMA and without rounding, over the window
+ * rows y0 .. y0+hc-1, columns x0 .. x0+wc-1 of t pairs of uint8 RGB frames true_u8 [t,ht,wt,3] / pred_u8
+ * [t,hp,wp,3].  The window lies in the common size min(ht, hp) x min(wt, wp) (the frames' top-left corner).
+ * Sums are reduced in a fixed order through the caller's workspace: the same inputs give the same bits.
+ * TG_E_INVALID: null or misaligned (8 bytes) pointers, non-positive sizes, a window outside the common size, a short
+ * workspace; TG_E_UNSUPPORTED: t > 65535.  Two launches each. */
+size_t tg_official_frames_stats_workspace_bytes(int t, int hc, int wc);
+/* stats [t,3] float64 = {sum over the window of (Yt - Yp)^2, min Yp, max Yp} per frame. */
+int tg_official_frames_stats(const uint8_t* true_u8, int ht, int wt, const uint8_t* pred_u8, int hp, int wp, int t,
+                             int y0, int x0, int hc, int wc, double* stats, void* work, size_t work_bytes,
+                             void* stream);
+/* Bytes of tg_ssim_y's workspace (0 for bad sizes or a window below 7 x 7). */
+size_t tg_ssim_y_workspace_bytes(int t, int hc, int wc);
+/* ssim [t] float64 = skimage.measure.compare_ssim(Yt, Yp, data_range=R) of the window: 7x7 box means of Yt, Yp,
+ * Yt^2, Yp^2, Yt Yp, covariances scaled by 49/48, C1 = (0.01 R)^2, C2 = (0.03 R)^2, and the mean of the SSIM map
+ * over the (hc-6) x (wc-6) windows inside the crop.  R = stats[3f+2] - stats[3f+1] (tg_official_frames_stats's
+ * output, read on the device).  Plain IEEE division: R = 0 gives numpy's nan where a 7x7 window is flat in both
+ * frames.  TG_E_INVALID also for a window below 7 x 7. */
+int tg_ssim_y(const uint8_t* true_u8, int ht, int wt, const uint8_t* pred_u8, int hp, int wp, int t, int y0, int x0,
+              int hc, int wc, const double* stats, double* ssim, void* work, size_t work_bytes, void* stream);
 
 /* BD degradation of the data side (codes/utils/data_utils.py:30-53, called on GT frames by
  * base_model.py:75,115): optional reflect pad by (k-1)/2 | k-1-(k-1)/2, then a depthwise valid

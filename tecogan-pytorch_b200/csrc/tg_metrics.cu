@@ -1,7 +1,10 @@
 // Video quality metrics on the device: the frame input of PSNR / tOF scoring (gray planes and per-frame integer
 // SSE in one read of the uint8 frames) and Farneback dense optical flow (cv2.calcOpticalFlowFarneback, flags=0),
-// batched over many frame pairs per launch, and the per-pair sum of the end-point error between two flow sets.
-// Specification: oracle/farneback.py and oracle/metrics_oracle.py.  Contract: include/tecogan_b200.h.
+// batched over many frame pairs per launch, and the per-pair sum of the end-point error between two flow sets over
+// a window.  For the official metric script: the unrounded Y's squared-difference sum and the predicted Y's range
+// over a window, and SSIM (skimage compare_ssim) of the Y over that window.
+// Specification: oracle/farneback.py, oracle/metrics_oracle.py and oracle/official_metrics.py.
+// Contract: include/tecogan_b200.h.
 #include <math.h>
 
 #include "tg_common.cuh"
@@ -17,14 +20,20 @@ constexpr int kTileW = 32, kTileH = 16;    // flow-update tile (outputs)
 
 // ---- frame input ---------------------------------------------------------------------------------------------------
 
-// BT.601 studio-swing Y of data_utils.rgb_to_ycbcr: float64 r*T0 + g*T1 + b*T2 + 16, left to right, no FMA,
-// rounded half to even.  For three colours numpy's matmul rounds its sum to the other side of a .5 tie; the
-// reference's Y of those is one lower (the rule is checked over all 2^24 colours in tests/test_metrics_cpu.py).
-__device__ __forceinline__ int y_of(int r, int g, int b) {
+// BT.601 studio-swing Y before rounding: float64 r*T0 + g*T1 + b*T2 + 16, left to right, no FMA.  This is the
+// official metric script's _rgb2ycbcr Y (maxVal=255), which it never rounds.
+__device__ __forceinline__ double y_f64(int r, int g, int b) {
   double s = __dmul_rn((double)r, 0.256788235294118);
   s = __dadd_rn(s, __dmul_rn((double)g, 0.504129411764706));
   s = __dadd_rn(s, __dmul_rn((double)b, 0.097905882352941));
-  s = __dadd_rn(s, 16.0);
+  return __dadd_rn(s, 16.0);
+}
+
+// Y of data_utils.rgb_to_ycbcr: y_f64 rounded half to even.  For three colours numpy's matmul rounds its sum to the
+// other side of a .5 tie; the reference's Y of those is one lower (the rule is checked over all 2^24 colours in
+// tests/test_metrics_cpu.py).
+__device__ __forceinline__ int y_of(int r, int g, int b) {
+  const double s = y_f64(r, g, b);
   int y = (int)rint(fmin(fmax(s, 0.0), 255.0));
   const int c = (r << 16) | (g << 8) | b;
   if (c == 0x01ade1 || c == 0x0caebf || c == 0x182e49) y -= 1;   // (1,173,225) (12,174,191) (24,46,73)
@@ -71,6 +80,181 @@ frames_in_kernel(const uint8_t* __restrict__ tru, int ht, int wt, const uint8_t*
 #pragma unroll
   for (int k = 0; k < kThreads / 32; ++k) s += warp_sum[k];
   atomicAdd(sse + f, s);
+}
+
+// ---- official metric script: Y statistics and SSIM over a window ---------------------------------------------------
+// Every sum is reduced in a fixed order (per-CTA partials in the caller's workspace, then one CTA per frame), so the
+// same inputs give the same bits on every run and for every chunking of the frames.
+
+constexpr int kStatsMaxBlocks = 128;       // per frame
+constexpr int kSsimTW = 32, kSsimTH = 16;  // SSIM outputs per CTA
+constexpr int kSsimR = 3;                  // 7x7 window
+
+// sum, min and max of a CTA, in a fixed order; the result is valid in thread 0
+__device__ __forceinline__ void block_sum_min_max(double& s, double& mn, double& mx) {
+  __shared__ double red[3][kThreads / 32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    s = __dadd_rn(s, __shfl_down_sync(0xffffffffu, s, o));
+    mn = fmin(mn, __shfl_down_sync(0xffffffffu, mn, o));
+    mx = fmax(mx, __shfl_down_sync(0xffffffffu, mx, o));
+  }
+  const int warp = threadIdx.x >> 5;
+  if ((threadIdx.x & 31) == 0) {
+    red[0][warp] = s;
+    red[1][warp] = mn;
+    red[2][warp] = mx;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    s = red[0][0];
+    mn = red[1][0];
+    mx = red[2][0];
+#pragma unroll
+    for (int k = 1; k < kThreads / 32; ++k) {
+      s = __dadd_rn(s, red[0][k]);
+      mn = fmin(mn, red[1][k]);
+      mx = fmax(mx, red[2][k]);
+    }
+  }
+}
+
+// part [t, gridDim.x, 3]: per CTA {sum (Yt - Yp)^2, min Yp, max Yp} over its rows of the window
+__global__ void __launch_bounds__(kThreads)
+official_stats_kernel(const uint8_t* __restrict__ tru, int ht, int wt, const uint8_t* __restrict__ pred, int hp,
+                      int wp, int y0, int x0, int hc, int wc, double* __restrict__ part) {
+  tg_pdl_wait();
+  tg_pdl_trigger();
+  const int f = blockIdx.y;
+  const uint8_t* a = tru + (size_t)f * ht * wt * 3;
+  const uint8_t* b = pred + (size_t)f * hp * wp * 3;
+  double s = 0.0, mn = INFINITY, mx = -INFINITY;
+  for (int r = blockIdx.x; r < hc; r += gridDim.x) {          // CTA k: rows k, k + gridDim.x, ...
+    const uint8_t* ra = a + ((size_t)(y0 + r) * wt + x0) * 3;
+    const uint8_t* rb = b + ((size_t)(y0 + r) * wp + x0) * 3;
+    for (int c = threadIdx.x; c < wc; c += kThreads) {
+      const double yp = y_f64(rb[3 * c], rb[3 * c + 1], rb[3 * c + 2]);
+      const double d = __dadd_rn(y_f64(ra[3 * c], ra[3 * c + 1], ra[3 * c + 2]), -yp);
+      s = __dadd_rn(s, __dmul_rn(d, d));
+      mn = fmin(mn, yp);
+      mx = fmax(mx, yp);
+    }
+  }
+  block_sum_min_max(s, mn, mx);
+  if (threadIdx.x == 0) {
+    double* o = part + ((size_t)f * gridDim.x + blockIdx.x) * 3;
+    o[0] = s;
+    o[1] = mn;
+    o[2] = mx;
+  }
+}
+
+// stats [t, 3] from part [t, nb, 3]: one CTA per frame
+__global__ void __launch_bounds__(kThreads)
+official_stats_final_kernel(const double* __restrict__ part, int nb, double* __restrict__ stats) {
+  tg_pdl_wait();
+  tg_pdl_trigger();
+  const int f = blockIdx.x;
+  const double* p = part + (size_t)f * nb * 3;
+  double s = 0.0, mn = INFINITY, mx = -INFINITY;
+  for (int k = threadIdx.x; k < nb; k += kThreads) {
+    s = __dadd_rn(s, p[3 * k]);
+    mn = fmin(mn, p[3 * k + 1]);
+    mx = fmax(mx, p[3 * k + 2]);
+  }
+  block_sum_min_max(s, mn, mx);
+  if (threadIdx.x == 0) {
+    stats[3 * f] = s;
+    stats[3 * f + 1] = mn;
+    stats[3 * f + 2] = mx;
+  }
+}
+
+// SSIM map of skimage's compare_ssim (7x7 uniform window, sample covariance) on a kSsimTW x kSsimTH tile of the
+// window's interior, with data_range = max Yp - min Yp from stats [t, 3].  Interior pixel (i, j) of the window
+// (3 <= i < hc - 3, 3 <= j < wc - 3) is tile output (i - 3, j - 3).  part [t, tiles]: the tile's sum of S.
+__global__ void __launch_bounds__(kThreads)
+ssim_tile_kernel(const uint8_t* __restrict__ tru, int ht, int wt, const uint8_t* __restrict__ pred, int hp, int wp,
+                 int y0, int x0, int hc, int wc, const double* __restrict__ stats, double* __restrict__ part) {
+  constexpr int LW = kSsimTW + 2 * kSsimR, LH = kSsimTH + 2 * kSsimR;
+  __shared__ double ys[2][LH][LW];            // Yt, Yp with a 3-pixel halo
+  __shared__ double hs[5][LH][kSsimTW];       // 7-tap row sums of x, y, x x, y y, x y
+  tg_pdl_wait();
+  tg_pdl_trigger();
+  const int f = blockIdx.z;
+  const int oy = blockIdx.y * kSsimTH, ox = blockIdx.x * kSsimTW;   // tile origin in window coordinates
+  const uint8_t* a = tru + (size_t)f * ht * wt * 3;
+  const uint8_t* b = pred + (size_t)f * hp * wp * 3;
+  for (int i = threadIdx.x; i < LH * LW; i += kThreads) {
+    const int r = i / LW, c = i % LW;
+    // rows / columns past the window only feed outputs past the interior, which are not kept
+    const int y = y0 + min(oy + r, hc - 1), x = x0 + min(ox + c, wc - 1);
+    const uint8_t* pa = a + ((size_t)y * wt + x) * 3;
+    const uint8_t* pb = b + ((size_t)y * wp + x) * 3;
+    ys[0][r][c] = y_f64(pa[0], pa[1], pa[2]);
+    ys[1][r][c] = y_f64(pb[0], pb[1], pb[2]);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < LH * kSsimTW; i += kThreads) {
+    const int r = i / kSsimTW, c = i % kSsimTW;
+    double sx = 0.0, sy = 0.0, sxx = 0.0, syy = 0.0, sxy = 0.0;
+#pragma unroll
+    for (int k = 0; k <= 2 * kSsimR; ++k) {
+      const double x = ys[0][r][c + k], y = ys[1][r][c + k];
+      sx = __dadd_rn(sx, x);
+      sy = __dadd_rn(sy, y);
+      sxx = __dadd_rn(sxx, __dmul_rn(x, x));
+      syy = __dadd_rn(syy, __dmul_rn(y, y));
+      sxy = __dadd_rn(sxy, __dmul_rn(x, y));
+    }
+    hs[0][r][c] = sx;
+    hs[1][r][c] = sy;
+    hs[2][r][c] = sxx;
+    hs[3][r][c] = syy;
+    hs[4][r][c] = sxy;
+  }
+  __syncthreads();
+  const double R = __dadd_rn(stats[3 * f + 2], -stats[3 * f + 1]);
+  const double k1r = __dmul_rn(0.01, R), k2r = __dmul_rn(0.03, R);
+  const double C1 = __dmul_rn(k1r, k1r), C2 = __dmul_rn(k2r, k2r);
+  const double cov_norm = 49.0 / 48.0;
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < kSsimTW * kSsimTH; i += kThreads) {
+    const int r = i / kSsimTW, c = i % kSsimTW;
+    if (oy + r >= hc - 2 * kSsimR || ox + c >= wc - 2 * kSsimR) continue;
+    double m[5];
+#pragma unroll
+    for (int q = 0; q < 5; ++q) {
+      double v = 0.0;
+#pragma unroll
+      for (int k = 0; k <= 2 * kSsimR; ++k) v = __dadd_rn(v, hs[q][r + k][c]);
+      m[q] = v / 49.0;
+    }
+    const double ux = m[0], uy = m[1];
+    const double vx = __dmul_rn(cov_norm, __dadd_rn(m[2], -__dmul_rn(ux, ux)));
+    const double vy = __dmul_rn(cov_norm, __dadd_rn(m[3], -__dmul_rn(uy, uy)));
+    const double vxy = __dmul_rn(cov_norm, __dadd_rn(m[4], -__dmul_rn(ux, uy)));
+    const double A1 = __dadd_rn(__dmul_rn(__dmul_rn(2.0, ux), uy), C1);
+    const double A2 = __dadd_rn(__dmul_rn(2.0, vxy), C2);
+    const double B1 = __dadd_rn(__dadd_rn(__dmul_rn(ux, ux), __dmul_rn(uy, uy)), C1);
+    const double B2 = __dadd_rn(__dadd_rn(vx, vy), C2);
+    acc = __dadd_rn(acc, __dmul_rn(A1, A2) / __dmul_rn(B1, B2));
+  }
+  double mn = 0.0, mx = 0.0;
+  block_sum_min_max(acc, mn, mx);
+  if (threadIdx.x == 0) part[((size_t)f * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = acc;
+}
+
+// ssim[f] = sum of part[f, 0..nb) / count: one CTA per frame
+__global__ void __launch_bounds__(kThreads)
+ssim_final_kernel(const double* __restrict__ part, int nb, double count, double* __restrict__ ssim) {
+  tg_pdl_wait();
+  tg_pdl_trigger();
+  const int f = blockIdx.x;
+  double s = 0.0, mn = 0.0, mx = 0.0;
+  for (int k = threadIdx.x; k < nb; k += kThreads) s = __dadd_rn(s, part[(size_t)f * nb + k]);
+  block_sum_min_max(s, mn, mx);
+  if (threadIdx.x == 0) ssim[f] = s / count;
 }
 
 // ---- pyramid level: Gaussian blur at full size + INTER_LINEAR resize, both separable -------------------------------
@@ -345,30 +529,57 @@ flow_iter_kernel(const float* __restrict__ M_in, const float* __restrict__ R, fl
   }
 }
 
-// sums[q] += sum over pixels of |a[q] - b[q]| (Euclidean, per pixel), in float64
+constexpr int kEpeMaxBlocks = 512;        // CTAs per pair
+
+// The sum over the window (y0, x0, hc, wc) of |a[q] - b[q]| (Euclidean, per pixel), in float64.  With part, CTA k of
+// pair q takes rows k, k + gridDim.x, ... and writes its sum to part[q, k] (epe_final_kernel adds them in a fixed
+// order: the same bits on every run).  Without, the window is the whole frame, read as one grid-strided range, and
+// each CTA adds its sum to sums[q] with a float64 atomic.
 __global__ void __launch_bounds__(kThreads)
-epe_kernel(const float2* __restrict__ a, const float2* __restrict__ b, size_t hw, double* __restrict__ sums) {
+epe_kernel(const float2* __restrict__ a, const float2* __restrict__ b, int h, int w, int y0, int x0, int hc, int wc,
+           double* __restrict__ sums, double* __restrict__ part) {
   tg_pdl_wait();
   tg_pdl_trigger();
   const int q = blockIdx.y;
-  const float2* pa = a + (size_t)q * hw;
-  const float2* pb = b + (size_t)q * hw;
+  const size_t base = (size_t)q * h * w + (size_t)y0 * w + x0;
+  const float2* pa = a + base;
+  const float2* pb = b + base;
   double acc = 0.0;
-  for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < hw; i += (size_t)gridDim.x * kThreads) {
-    const float2 u = __ldg(pa + i), v = __ldg(pb + i);
-    const float ex = u.x - v.x, ey = u.y - v.y;
-    acc += (double)sqrtf(ex * ex + ey * ey);
+  if (!part) {                                 // the whole frame (tg_flow_epe_sum): one flat range
+    const size_t n = (size_t)hc * wc;
+    for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += (size_t)gridDim.x * kThreads) {
+      const float2 u = __ldg(pa + i), v = __ldg(pb + i);
+      const float ex = u.x - v.x, ey = u.y - v.y;
+      acc += (double)sqrtf(ex * ex + ey * ey);
+    }
+  } else {
+    for (int r = blockIdx.x; r < hc; r += gridDim.x) {
+      for (int c = threadIdx.x; c < wc; c += kThreads) {
+        const float2 u = __ldg(pa + (size_t)r * w + c), v = __ldg(pb + (size_t)r * w + c);
+        const float ex = u.x - v.x, ey = u.y - v.y;
+        acc += (double)sqrtf(ex * ex + ey * ey);
+      }
+    }
   }
-  __shared__ double warp_sum[kThreads / 32];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_down_sync(0xffffffffu, acc, o);
-  if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = acc;
-  __syncthreads();
+  double mn = 0.0, mx = 0.0;
+  block_sum_min_max(acc, mn, mx);
   if (threadIdx.x != 0) return;
-  double s = 0.0;
-#pragma unroll
-  for (int k = 0; k < kThreads / 32; ++k) s += warp_sum[k];
-  atomicAdd(sums + q, s);
+  if (part)
+    part[(size_t)q * gridDim.x + blockIdx.x] = acc;
+  else
+    atomicAdd(sums + q, acc);
+}
+
+// sums[q] = the sum of part[q, 0..nb) in a fixed order: one CTA per pair
+__global__ void __launch_bounds__(kThreads)
+epe_final_kernel(const double* __restrict__ part, int nb, double* __restrict__ sums) {
+  tg_pdl_wait();
+  tg_pdl_trigger();
+  const int q = blockIdx.x;
+  double s = 0.0, mn = 0.0, mx = 0.0;
+  for (int k = threadIdx.x; k < nb; k += kThreads) s = __dadd_rn(s, part[(size_t)q * nb + k]);
+  block_sum_min_max(s, mn, mx);
+  if (threadIdx.x == 0) sums[q] = s;
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------
@@ -503,6 +714,31 @@ inline dim3 row_grid(int w, int rows, int z) {
   return dim3((unsigned)(bx < 8 ? bx : 8), (unsigned)rows, (unsigned)z);
 }
 
+bool window_inside(int y0, int x0, int hc, int wc, int h, int w) {
+  return y0 >= 0 && x0 >= 0 && hc > 0 && wc > 0 && (long long)y0 + hc <= h && (long long)x0 + wc <= w;
+}
+
+int stats_blocks(int hc, int wc) {
+  (void)wc;
+  return hc < kStatsMaxBlocks ? hc : kStatsMaxBlocks;
+}
+
+// CTAs of ssim_tile_kernel over the (hc - 6) x (wc - 6) interior of the window
+dim3 ssim_tiles(int hc, int wc) {
+  return dim3((unsigned)((wc - 2 * kSsimR + kSsimTW - 1) / kSsimTW),
+              (unsigned)((hc - 2 * kSsimR + kSsimTH - 1) / kSsimTH));
+}
+
+// the frame and window arguments of tg_official_frames_stats / tg_ssim_y; the window lies in the common size
+const char* check_official_args(const uint8_t* tru, int ht, int wt, const uint8_t* pred, int hp, int wp, int t,
+                                int y0, int x0, int hc, int wc, int min_side) {
+  if (!tru || !pred) return "null frames";
+  if (t <= 0 || ht <= 0 || wt <= 0 || hp <= 0 || wp <= 0) return "non-positive size";
+  if (!window_inside(y0, x0, hc, wc, ht < hp ? ht : hp, wt < wp ? wt : wp)) return "window outside the common size";
+  if (hc < min_side || wc < min_side) return "window smaller than the 7x7 SSIM window";
+  return nullptr;
+}
+
 }  // namespace
 
 extern "C" int tg_metrics_frames_in(const uint8_t* true_u8, int ht, int wt, const uint8_t* pred_u8, int hp, int wp,
@@ -622,21 +858,111 @@ extern "C" int tg_farneback(const uint8_t* gray, int groups, int t, int h, int w
   return TG_OK;
 }
 
-extern "C" int tg_flow_epe_sum(const float* a, const float* b, int n, int h, int w, double* sums, void* stream) {
-  const char* name = "flow_epe_sum";
+namespace {
+
+int epe_blocks(int hc) { return hc < kEpeMaxBlocks ? hc : kEpeMaxBlocks; }
+
+// work == nullptr: per-CTA float64 atomics into sums (zeroed first); else the fixed-order two-pass sum
+int epe_sum(const char* name, const float* a, const float* b, int n, int h, int w, int y0, int x0, int hc, int wc,
+            double* sums, void* work, size_t work_bytes, void* stream) {
   TG_REQUIRE(a && b && sums, TG_E_INVALID, "%s: null pointer (a / b / sums)", name);
   TG_REQUIRE(n > 0 && h > 0 && w > 0, TG_E_INVALID, "%s: bad size n=%d h=%d w=%d", name, n, h, w);
-  TG_REQUIRE(((((uintptr_t)a) | ((uintptr_t)b)) & 7u) == 0 && (((uintptr_t)sums) & 7u) == 0, TG_E_INVALID,
-             "%s: a / b / sums must be 8-byte aligned", name);
+  TG_REQUIRE(window_inside(y0, x0, hc, wc, h, w), TG_E_INVALID, "%s: window (%d, %d, %d, %d) outside %dx%d", name,
+             y0, x0, hc, wc, h, w);
+  TG_REQUIRE(((((uintptr_t)a) | ((uintptr_t)b) | ((uintptr_t)sums) | ((uintptr_t)work)) & 7u) == 0, TG_E_INVALID,
+             "%s: a / b / sums / work must be 8-byte aligned", name);
   TG_REQUIRE(n <= 65535, TG_E_UNSUPPORTED, "%s: %d pairs per launch (at most 65535)", name, n);
+  double* part = static_cast<double*>(work);
+  size_t flat = ((size_t)hc * wc + kThreads * 8 - 1) / (kThreads * 8);
+  const int nb = part ? epe_blocks(hc) : (int)(flat < kEpeMaxBlocks ? flat : kEpeMaxBlocks);
   cudaStream_t s = (cudaStream_t)stream;
-  cudaError_t e = cudaMemsetAsync(sums, 0, (size_t)n * sizeof(double), s);
-  TG_REQUIRE(e == cudaSuccess, (int)e, "%s: memset: %s", name, cudaGetErrorString(e));
-  const size_t hw = (size_t)h * w;
-  size_t bx = (hw + kThreads * 8 - 1) / (kThreads * 8);
-  if (bx > 512) bx = 512;
-  tg_launch(epe_kernel, dim3((unsigned)bx, (unsigned)n), dim3(kThreads), 0, s, reinterpret_cast<const float2*>(a),
-            reinterpret_cast<const float2*>(b), hw, sums);
+  if (part) {
+    const size_t need = (size_t)n * nb * sizeof(double);
+    TG_REQUIRE(work_bytes >= need, TG_E_INVALID, "%s: workspace of %zu bytes, %zu needed", name, work_bytes, need);
+  } else {
+    cudaError_t e = cudaMemsetAsync(sums, 0, (size_t)n * sizeof(double), s);
+    TG_REQUIRE(e == cudaSuccess, (int)e, "%s: memset: %s", name, cudaGetErrorString(e));
+  }
+  tg_launch(epe_kernel, dim3((unsigned)nb, (unsigned)n), dim3(kThreads), 0, s, reinterpret_cast<const float2*>(a),
+            reinterpret_cast<const float2*>(b), h, w, y0, x0, hc, wc, sums, part);
+  TG_CUDA_LAUNCH_CHECK(name);
+  if (part) {
+    tg_launch(epe_final_kernel, dim3((unsigned)n), dim3(kThreads), 0, s, (const double*)part, nb, sums);
+    TG_CUDA_LAUNCH_CHECK(name);
+  }
+  return TG_OK;
+}
+
+}  // namespace
+
+extern "C" size_t tg_flow_epe_sum_window_workspace_bytes(int n, int hc) {
+  if (n <= 0 || hc <= 0) return 0;
+  return (size_t)n * epe_blocks(hc) * sizeof(double);
+}
+
+extern "C" int tg_flow_epe_sum_window(const float* a, const float* b, int n, int h, int w, int y0, int x0, int hc,
+                                      int wc, double* sums, void* work, size_t work_bytes, void* stream) {
+  TG_REQUIRE(work != nullptr, TG_E_INVALID, "flow_epe_sum_window: null workspace");
+  return epe_sum("flow_epe_sum_window", a, b, n, h, w, y0, x0, hc, wc, sums, work, work_bytes, stream);
+}
+
+extern "C" int tg_flow_epe_sum(const float* a, const float* b, int n, int h, int w, double* sums, void* stream) {
+  return epe_sum("flow_epe_sum", a, b, n, h, w, 0, 0, h, w, sums, nullptr, 0, stream);
+}
+
+extern "C" size_t tg_official_frames_stats_workspace_bytes(int t, int hc, int wc) {
+  if (t <= 0 || hc <= 0 || wc <= 0) return 0;
+  return (size_t)t * stats_blocks(hc, wc) * 3 * sizeof(double);
+}
+
+extern "C" int tg_official_frames_stats(const uint8_t* true_u8, int ht, int wt, const uint8_t* pred_u8, int hp,
+                                        int wp, int t, int y0, int x0, int hc, int wc, double* stats, void* work,
+                                        size_t work_bytes, void* stream) {
+  const char* name = "official_frames_stats";
+  const char* bad = check_official_args(true_u8, ht, wt, pred_u8, hp, wp, t, y0, x0, hc, wc, 1);
+  TG_REQUIRE(bad == nullptr, TG_E_INVALID, "%s: %s", name, bad);
+  TG_REQUIRE(stats && work, TG_E_INVALID, "%s: null pointer (stats / work)", name);
+  TG_REQUIRE(((((uintptr_t)stats) | ((uintptr_t)work)) & 7u) == 0, TG_E_INVALID,
+             "%s: stats and work must be 8-byte aligned", name);
+  const size_t need = tg_official_frames_stats_workspace_bytes(t, hc, wc);
+  TG_REQUIRE(work_bytes >= need, TG_E_INVALID, "%s: workspace of %zu bytes, %zu needed", name, work_bytes, need);
+  TG_REQUIRE(t <= 65535, TG_E_UNSUPPORTED, "%s: %d frames per launch (at most 65535)", name, t);
+  cudaStream_t s = (cudaStream_t)stream;
+  const int nb = stats_blocks(hc, wc);
+  double* part = static_cast<double*>(work);
+  tg_launch(official_stats_kernel, dim3((unsigned)nb, (unsigned)t), dim3(kThreads), 0, s, true_u8, ht, wt, pred_u8,
+            hp, wp, y0, x0, hc, wc, part);
+  TG_CUDA_LAUNCH_CHECK(name);
+  tg_launch(official_stats_final_kernel, dim3((unsigned)t), dim3(kThreads), 0, s, (const double*)part, nb, stats);
+  TG_CUDA_LAUNCH_CHECK(name);
+  return TG_OK;
+}
+
+extern "C" size_t tg_ssim_y_workspace_bytes(int t, int hc, int wc) {
+  if (t <= 0 || hc < 2 * kSsimR + 1 || wc < 2 * kSsimR + 1) return 0;
+  return (size_t)t * ssim_tiles(hc, wc).x * ssim_tiles(hc, wc).y * sizeof(double);
+}
+
+extern "C" int tg_ssim_y(const uint8_t* true_u8, int ht, int wt, const uint8_t* pred_u8, int hp, int wp, int t,
+                         int y0, int x0, int hc, int wc, const double* stats, double* ssim, void* work,
+                         size_t work_bytes, void* stream) {
+  const char* name = "ssim_y";
+  const char* bad = check_official_args(true_u8, ht, wt, pred_u8, hp, wp, t, y0, x0, hc, wc, 2 * kSsimR + 1);
+  TG_REQUIRE(bad == nullptr, TG_E_INVALID, "%s: %s", name, bad);
+  TG_REQUIRE(stats && ssim && work, TG_E_INVALID, "%s: null pointer (stats / ssim / work)", name);
+  TG_REQUIRE(((((uintptr_t)stats) | ((uintptr_t)ssim) | ((uintptr_t)work)) & 7u) == 0, TG_E_INVALID,
+             "%s: stats, ssim and work must be 8-byte aligned", name);
+  const size_t need = tg_ssim_y_workspace_bytes(t, hc, wc);
+  TG_REQUIRE(work_bytes >= need, TG_E_INVALID, "%s: workspace of %zu bytes, %zu needed", name, work_bytes, need);
+  TG_REQUIRE(t <= 65535, TG_E_UNSUPPORTED, "%s: %d frames per launch (at most 65535)", name, t);
+  cudaStream_t s = (cudaStream_t)stream;
+  const dim3 tiles = ssim_tiles(hc, wc);
+  double* part = static_cast<double*>(work);
+  tg_launch(ssim_tile_kernel, dim3(tiles.x, tiles.y, (unsigned)t), dim3(kThreads), 0, s, true_u8, ht, wt, pred_u8,
+            hp, wp, y0, x0, hc, wc, stats, part);
+  TG_CUDA_LAUNCH_CHECK(name);
+  tg_launch(ssim_final_kernel, dim3((unsigned)t), dim3(kThreads), 0, s, (const double*)part, (int)(tiles.x * tiles.y),
+            (double)(hc - 2 * kSsimR) * (wc - 2 * kSsimR), ssim);
   TG_CUDA_LAUNCH_CHECK(name);
   return TG_OK;
 }

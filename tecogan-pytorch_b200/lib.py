@@ -134,6 +134,14 @@ _SIGNATURES = {
     'tg_farneback_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
     'tg_farneback': (c_int, [_P, c_int, c_int, c_int, c_int, ctypes.POINTER(FarnebackParams), _P, _P, c_size_t, _P]),
     'tg_flow_epe_sum': (c_int, [_P, _P, c_int, c_int, c_int, _P, _P]),
+    'tg_flow_epe_sum_window_workspace_bytes': (c_size_t, [c_int, c_int]),
+    'tg_flow_epe_sum_window': (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, c_size_t, _P]),
+    'tg_official_frames_stats_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
+    'tg_official_frames_stats': (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P,
+                                         _P, c_size_t, _P]),
+    'tg_ssim_y_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
+    'tg_ssim_y': (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, c_size_t,
+                          _P]),
     'tg_downsample_bd_nchw_f32': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_debug_set_conv_timers': (c_int, [_P]),
     # ---- training (generator backward)

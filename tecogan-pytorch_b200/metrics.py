@@ -180,3 +180,140 @@ def sequence_metrics(true_seq, pred_seq, psnr='y', tof=True, max_workspace_bytes
     if tof:
         out['tOF'] = (torch.cat(epe_parts).cpu().numpy() / hw) if epe_parts else np.zeros(0)
     return out
+
+
+# ---- the official metric script (codes/official_metrics/metrics.py) -------------------------------------------------
+
+OFFICIAL_KEYS = ('PSNR', 'SSIM', 'tOF')
+OFFICIAL_MIN_SIDE = 48                     # the smallest side whose crop_8x8 is not empty
+
+
+def crop_8x8(n):
+    """(offset, size) of the official script's crop_8x8 along a side of n >= 48 pixels: the largest multiple of 32
+    that is <= n - 16, centred at (n - size) // 2"""
+    size = (n // 32) * 32
+    while size > n - 16:
+        size -= 32
+    return (n - size) // 2, size
+
+
+def official_sequence_metrics(true_seq, pred_seq, cutfr=2, keys=OFFICIAL_KEYS,
+                              max_workspace_bytes=DEFAULT_MAX_WORKSPACE_BYTES):
+    """PSNR, SSIM and tOF of a predicted sequence as TecoGAN's official metric script (the one behind the paper's
+    tables) computes them frame by frame, on the device.
+
+    true_seq, pred_seq: uint8 RGB frames [T, H, W, 3], host numpy arrays or CUDA tensors, as sequence_metrics takes
+    them.  Both are cropped to their common top-left size (h, w), which must be at least 48 x 48; crop_8x8 of it is
+    the scored window.  Frames cutfr .. T - cutfr - 1 are scored:
+      PSNR  20 log10(255 / RMSE) of the unrounded float64 Y of _rgb2ycbcr over the window (inf on equal frames)
+      SSIM  skimage compare_ssim of those Y (7x7 uniform window), data_range = max - min of the predicted Y
+      tOF   from frame cutfr + 1 on: the mean end-point error over the window of the Farneback flows of the full
+            common-size gray frames (flow of frame i - 1 -> i, ground truth against prediction)
+    keys: the metrics to compute, a subset of OFFICIAL_KEYS.  max_workspace_bytes bounds the device memory of the
+    pass; a longer sequence is scored in chunks of consecutive frames that overlap by one frame.
+
+    Returns {key: float64 numpy array} in the order of OFFICIAL_KEYS: PSNR and SSIM of T - 2 cutfr frames, tOF of
+    T - 2 cutfr - 1 (empty arrays when there are too few frames)."""
+    true_seq, pred_seq = _frames(true_seq, 'true_seq'), _frames(pred_seq, 'pred_seq')
+    if isinstance(keys, str) or not all(isinstance(k, str) and k in OFFICIAL_KEYS for k in keys):
+        raise ValueError(f'keys must be a subset of {OFFICIAL_KEYS}, got {keys!r}')
+    if not isinstance(cutfr, (int, np.integer)) or isinstance(cutfr, bool) or cutfr < 0:
+        raise ValueError(f'cutfr must be a non-negative integer, got {cutfr!r}')
+    T = true_seq.shape[0]
+    if pred_seq.shape[0] != T:
+        raise ValueError(f'true_seq has {T} frames, pred_seq {pred_seq.shape[0]}')
+    h, w = min(true_seq.shape[1], pred_seq.shape[1]), min(true_seq.shape[2], pred_seq.shape[2])
+    if h < OFFICIAL_MIN_SIDE or w < OFFICIAL_MIN_SIDE:
+        raise ValueError(f'the common frame size {h}x{w} is below {OFFICIAL_MIN_SIDE}x{OFFICIAL_MIN_SIDE}: its '
+                         f'crop_8x8 is empty')
+    keys = [k for k in OFFICIAL_KEYS if k in keys]
+    tof = 'tOF' in keys
+    stats_wanted = 'PSNR' in keys or 'SSIM' in keys
+    (y0, hc), (x0, wc) = crop_8x8(h), crop_8x8(w)
+    window = (y0, x0, hc, wc)
+    n_s = max(T - 2 * cutfr, 0)
+    if n_s == 0 or not keys:
+        return {k: np.zeros(0) for k in keys}
+    true_seq, pred_seq = true_seq[cutfr:T - cutfr], pred_seq[cutfr:T - cutfr]
+    device = next((x.device for x in (true_seq, pred_seq) if isinstance(x, torch.Tensor)),
+                  torch.device('cuda', torch.cuda.current_device()))
+    hw = h * w
+    frame_bytes = 3 * (true_seq.shape[1] * true_seq.shape[2] + pred_seq.shape[1] * pred_seq.shape[2])
+
+    def chunk_bytes(n):
+        b = n * frame_bytes                                            # the uint8 frames of the chunk, full size
+        if stats_wanted:
+            b += n * 3 * 8 + ops.official_frames_stats_workspace_bytes(n, hc, wc)
+        if 'SSIM' in keys:
+            b += n * 8 + ops.ssim_y_workspace_bytes(n, hc, wc)
+        if tof and n >= 2:
+            b += ops.farneback_workspace_bytes(2, n, h, w) + 2 * n * hw + 2 * (n - 1) * hw * 8
+            b += (n - 1) * 8 + int(L.load().tg_flow_epe_sum_window_workspace_bytes(n - 1, hc))
+        return b
+    n, n_min = n_s, min(n_s, 2 if tof else 1)     # chunks overlap by one frame with tOF, so they need two
+    while n > n_min and chunk_bytes(n) > max_workspace_bytes:
+        n -= 1
+    if chunk_bytes(n) > max_workspace_bytes:
+        raise ValueError(f'max_workspace_bytes={max_workspace_bytes} is below the {chunk_bytes(n)} bytes that '
+                         f'{n} frames of {h}x{w} need')
+    params = _check_farneback_args(0.5, 3, 15, 3, 5, 1.2, 0) if tof else None
+    stats_parts, ssim_parts, epe_parts = [], [], []
+    with torch.cuda.device(device):
+        s = 0
+        while True:
+            e = min(s + n, n_s)
+            tc, pc = _chunk(true_seq, s, e, device), _chunk(pred_seq, s, e, device)
+            m = e - s
+            # with tOF a chunk's first frame is the last one's last frame, whose PSNR / SSIM are already kept
+            new = slice(1 if s > 0 and tof else 0, None)
+            if stats_wanted:
+                stats = ops.official_frames_stats(tc, pc, window)
+                stats_parts.append(stats[new])
+                if 'SSIM' in keys:
+                    ssim_parts.append(ops.ssim_y(tc, pc, window, stats)[new])
+            if tof and m >= 2:
+                gray = torch.empty(2, m, h, w, dtype=torch.uint8, device=device)
+                ops.metrics_frames_in(tc, pc, L.PSNR_NONE, gray)
+                flow = ops.farneback(gray.view(2 * m, h, w), 2, params)
+                epe_parts.append(ops.flow_epe_sum(flow[:m - 1], flow[m - 1:], window))
+            if e == n_s:
+                break
+            s = e - 1 if tof else e
+    out = {}
+    if 'PSNR' in keys:
+        sse = torch.cat(stats_parts)[:, 0].cpu().numpy()
+        with np.errstate(divide='ignore'):
+            out['PSNR'] = 20 * np.log10(255.0 / np.sqrt(sse / (hc * wc)))
+    if 'SSIM' in keys:
+        out['SSIM'] = torch.cat(ssim_parts).cpu().numpy()
+    if tof:
+        out['tOF'] = (torch.cat(epe_parts).cpu().numpy() / (hc * wc)) if epe_parts else np.zeros(0)
+    return out
+
+
+def official_averages(per_sequence):
+    """The totals the official metric script prints and writes for a list of sequences (its folders), each a dict of
+    per-frame arrays as official_sequence_metrics returns them.  Like the script, each sequence's list is cast to
+    float32 first.  Returns {'FrameAvg_<key>': the mean over all frames, 'FolderAvg_<key>': the mean of the
+    per-sequence means, 'Avg_<key>': float32 [sequences] of the per-sequence means} for every key of the dicts."""
+    if not per_sequence:
+        raise ValueError('official_averages needs at least one sequence')
+    keys = [k for k in per_sequence[0]]
+    if any(list(d) != keys for d in per_sequence):
+        raise ValueError('every sequence must have the same keys')
+    sums, lens, folder, avg = dict.fromkeys(keys, 0), dict.fromkeys(keys, 0), dict.fromkeys(keys, 0), {}
+    for d in per_sequence:
+        for k in keys:
+            cur = np.float32(d[k])
+            s = cur.sum()
+            mean = s / cur.shape[0]
+            avg.setdefault(k, []).append(mean)
+            sums[k] += s
+            lens[k] += cur.shape[0]
+            folder[k] += mean
+    out = {}
+    for k in keys:
+        out['FrameAvg_' + k] = sums[k] / lens[k]
+        out['FolderAvg_' + k] = folder[k] / len(per_sequence)
+        out['Avg_' + k] = np.float32(avg[k])
+    return out

@@ -885,16 +885,70 @@ def farneback(gray, groups, params, work=None):
     return flow
 
 
-def flow_epe_sum(a, b):
-    """tg_flow_epe_sum: fp32 flows a, b [n,h,w,2] -> float64 [n], the per-pair sum of |a - b| over the pixels"""
+def flow_epe_sum(a, b, window=None):
+    """tg_flow_epe_sum: fp32 flows a, b [n,h,w,2] -> float64 [n], the per-pair sum of |a - b| over the pixels, or
+    (tg_flow_epe_sum_window) over the window (y0, x0, hc, wc) of them, summed in a fixed order"""
     _req(a, torch.float32, 'a', 4)
     _req(b, torch.float32, 'b', 4)
     if a.shape != b.shape or a.shape[3] != 2:
         raise L.TecoganB200Error(f'flow_epe_sum: shapes {tuple(a.shape)} / {tuple(b.shape)}')
     n, h, w, _ = a.shape
     sums = torch.empty(n, dtype=torch.float64, device=a.device)
-    L.check(L.load().tg_flow_epe_sum(_ptr(a), _ptr(b), n, h, w, _ptr(sums), _stream()), 'tg_flow_epe_sum')
+    if window is None:
+        L.check(L.load().tg_flow_epe_sum(_ptr(a), _ptr(b), n, h, w, _ptr(sums), _stream()), 'tg_flow_epe_sum')
+    else:
+        need = int(L.load().tg_flow_epe_sum_window_workspace_bytes(n, window[2]))
+        work = torch.empty(max(need, 8) // 8, dtype=torch.float64, device=a.device)
+        L.check(L.load().tg_flow_epe_sum_window(_ptr(a), _ptr(b), n, h, w, *window, _ptr(sums), _ptr(work), need,
+                                                _stream()), 'tg_flow_epe_sum_window')
     return sums
+
+
+def _official_frames(name, true_u8, pred_u8):
+    _req(true_u8, torch.uint8, 'true_u8', 4)
+    _req(pred_u8, torch.uint8, 'pred_u8', 4)
+    if true_u8.shape[0] != pred_u8.shape[0] or true_u8.shape[3] != 3 or pred_u8.shape[3] != 3:
+        raise L.TecoganB200Error(f'{name}: expected RGB frames [t,h,w,3] of one length, got {tuple(true_u8.shape)} / '
+                                 f'{tuple(pred_u8.shape)}')
+    _same_device(name, true_u8, pred_u8)
+    t, ht, wt, _ = true_u8.shape
+    return (t, ht, wt) + tuple(pred_u8.shape[1:3])
+
+
+def official_frames_stats_workspace_bytes(t, hc, wc):
+    return int(L.load().tg_official_frames_stats_workspace_bytes(t, hc, wc))
+
+
+def ssim_y_workspace_bytes(t, hc, wc):
+    return int(L.load().tg_ssim_y_workspace_bytes(t, hc, wc))
+
+
+def official_frames_stats(true_u8, pred_u8, window):
+    """tg_official_frames_stats: uint8 RGB true_u8 [t,ht,wt,3] / pred_u8 [t,hp,wp,3], window (y0, x0, hc, wc) of the
+    common size -> float64 [t, 3]: {sum (Yt - Yp)^2, min Yp, max Yp} per frame"""
+    t, ht, wt, hp, wp = _official_frames('official_frames_stats', true_u8, pred_u8)
+    stats = torch.empty(t, 3, dtype=torch.float64, device=true_u8.device)
+    need = official_frames_stats_workspace_bytes(t, *window[2:])
+    work = torch.empty(max(need, 8) // 8, dtype=torch.float64, device=true_u8.device)
+    L.check(L.load().tg_official_frames_stats(_ptr(true_u8), ht, wt, _ptr(pred_u8), hp, wp, t, *window, _ptr(stats),
+                                              _ptr(work), need, _stream()), 'tg_official_frames_stats')
+    return stats
+
+
+def ssim_y(true_u8, pred_u8, window, stats):
+    """tg_ssim_y: SSIM of the Y over the window (y0, x0, hc, wc) -> float64 [t], with data_range from stats
+    (official_frames_stats's output, float64 [t, 3] on the device)"""
+    t, ht, wt, hp, wp = _official_frames('ssim_y', true_u8, pred_u8)
+    _req(stats, torch.float64, 'stats', 2)
+    if tuple(stats.shape) != (t, 3):
+        raise L.TecoganB200Error(f'ssim_y: stats {tuple(stats.shape)}, expected {(t, 3)}')
+    _same_device('ssim_y', true_u8, stats)
+    out = torch.empty(t, dtype=torch.float64, device=true_u8.device)
+    need = ssim_y_workspace_bytes(t, *window[2:])
+    work = torch.empty(max(need, 8) // 8, dtype=torch.float64, device=true_u8.device)
+    L.check(L.load().tg_ssim_y(_ptr(true_u8), ht, wt, _ptr(pred_u8), hp, wp, t, *window, _ptr(stats), _ptr(out),
+                               _ptr(work), need, _stream()), 'tg_ssim_y')
+    return out
 
 
 # ============================================================================ training (backward) ops

@@ -4,6 +4,10 @@ each phase must move (from shapes) and their share of the H100 SXM's 3.35 TB/s, 
 (cv2 Farneback + numpy PSNR, as MetricCalculator runs them) on the host cores for comparison.
 
     python tools/metrics_bench.py [--seqs 4] [--ref-frames 4] [--out metrics_bench.json]
+
+--official measures official_sequence_metrics (the official metric script's PSNR, SSIM and tOF on the crop_8x8
+window, frames 2 .. T-3) instead: scored frames/s end to end, per-kernel times from CUDA events, the algorithmic
+bytes and TB/s of the Y statistics and SSIM kernels, and oracle/official_metrics.py (cv2 + scipy) on the host cores.
 """
 import argparse
 import json
@@ -101,13 +105,91 @@ def reference_rate(true, pred, frames):
     return frames / (time.perf_counter() - t0), cv2.getNumThreads()
 
 
+def official_kernel_times(true, pred, cutfr=2, reps=5):
+    """CUDA-event times (ms, median of reps) of the kernels of one official_sequence_metrics pass over the T - 2 cutfr
+    scored frames of a sequence, and the algorithmic bytes of the Y statistics and SSIM kernels"""
+    dev = torch.device('cuda:0')
+    tc = torch.from_numpy(true[cutfr:len(true) - cutfr]).to(dev)
+    pc = torch.from_numpy(pred[cutfr:len(pred) - cutfr]).to(dev)
+    n, h, w = tc.shape[:3]
+    (y0, hc), (x0, wc) = M.crop_8x8(h), M.crop_8x8(w)
+    win = (y0, x0, hc, wc)
+    gray = torch.empty(2, n, h, w, dtype=torch.uint8, device=dev)
+    params = ops.farneback_params(0.5, 3, 15, 3, 5, 1.2, 0)
+    work = torch.empty(ops.farneback_workspace_bytes(2, n, h, w), dtype=torch.uint8, device=dev)
+    times = {k: [] for k in ('stats', 'ssim', 'gray', 'farneback', 'epe')}
+    for _ in range(reps + 1):
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(6)]
+        ev[0].record()
+        stats = ops.official_frames_stats(tc, pc, win)
+        ev[1].record()
+        ops.ssim_y(tc, pc, win, stats)
+        ev[2].record()
+        ops.metrics_frames_in(tc, pc, L.PSNR_NONE, gray)
+        ev[3].record()
+        flow = ops.farneback(gray.view(2 * n, h, w), 2, params, work)
+        ev[4].record()
+        ops.flow_epe_sum(flow[:n - 1], flow[n - 1:], win)
+        ev[5].record()
+        torch.cuda.synchronize()
+        for i, k in enumerate(times):
+            times[k].append(ev[i].elapsed_time(ev[i + 1]))
+    ms = {k: float(np.median(v[1:])) for k, v in times.items()}     # the first pass is a warm-up
+    # each kernel reads the window of both uint8 RGB frames once; the outputs are a few doubles per frame
+    moved = {'stats': n * 2 * hc * wc * 3 + n * 24, 'ssim': n * 2 * hc * wc * 3 + n * 32}
+    return ms, moved, [n, h, w], win
+
+
+def official_host_rate(true, pred, frames):
+    import cv2
+    from oracle import official_metrics as OM
+    t0 = time.perf_counter()
+    OM.sequence_metrics(true[:frames + 1], pred[:frames + 1], cutfr=0)
+    return (frames + 1) / (time.perf_counter() - t0), cv2.getNumThreads(), os.cpu_count()
+
+
+def main_official(a):
+    seqs = [sequence(s) for s in range(a.seqs)]
+    T_, h, w = seqs[0][0].shape[:3]
+    M.official_sequence_metrics(*seqs[0])
+    torch.cuda.synchronize()
+    rates = []
+    for _ in range(3):
+        t0 = time.perf_counter()
+        for t, p in seqs:
+            M.official_sequence_metrics(t, p)
+        torch.cuda.synchronize()
+        rates.append(len(seqs) * (T_ - 4) / (time.perf_counter() - t0))
+    ms, moved, shape, win = official_kernel_times(*seqs[0])
+    total = sum(ms.values())
+    host = official_host_rate(*seqs[0], a.ref_frames) if a.ref_frames else (None, None, None)
+    res = {
+        'card': card(),
+        'shape': [T_, h, w], 'scored_frames_per_sequence': T_ - 4, 'window': win,
+        'scored_frames_per_s_host_to_host': rates,
+        'kernel_ms_per_sequence': ms,
+        'farneback_share_of_kernel_time': (ms['gray'] + ms['farneback'] + ms['epe']) / total,
+        'algorithmic_bytes_per_sequence': moved,
+        'TBps': {k: moved[k] / (ms[k] * 1e-3) / 1e12 for k in moved},
+        'oracle_host_frames_per_s': host[0], 'oracle_cv2_threads': host[1], 'host_cpus': host[2],
+    }
+    print(json.dumps(res))
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, 'w') as f:
+            json.dump(res, f, indent=1)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--seqs', type=int, default=4)
     ap.add_argument('--ref-frames', type=int, default=4)
+    ap.add_argument('--official', action='store_true', help='measure official_sequence_metrics')
     ap.add_argument('--out', default=None)
     a = ap.parse_args()
     assert torch.cuda.is_available(), 'metrics_bench needs a GPU'
+    if a.official:
+        return main_official(a)
     seqs = [sequence(s) for s in range(a.seqs)]
     T_, h, w = seqs[0][0].shape[:3]
     M.sequence_metrics(*seqs[0])               # warm-up: module load, allocations
