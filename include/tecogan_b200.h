@@ -120,7 +120,7 @@ typedef struct tg_conv_desc {
   void* y;              /* see epilogue; convT writes [n,2h,2w,cout]                     */
   int32_t n, h, w;      /* batch and the height / width the kernel tiles over: the input's (= the
                            output's for conv3x3; convT writes 2h x 2w), the OUTPUT's for TG_CONV_3X3_S2 */
-  int32_t cin, cout;    /* stored channel counts: cin in {64,128,256}; cout in {64,128,256}
+  int32_t cin, cout;    /* stored channel counts: cin in {64,128,192,256,384}; cout in {64,128,192,256,384}
                            for TG_EPI_NHWC_F16, 48 (= TG_TAPN_ROWS, tap-major N packing)
                            for the two NCHW epilogues                                    */
   int32_t cout_real;    /* NCHW epilogues: channels actually written (2 resp. 3)         */
@@ -501,6 +501,55 @@ size_t tg_ssim_y_workspace_bytes(int t, int hc, int wc);
  * frames.  TG_E_INVALID also for a window below 7 x 7. */
 int tg_ssim_y(const uint8_t* true_u8, int ht, int wt, const uint8_t* pred_u8, int hp, int wp, int t, int y0, int x0,
               int hc, int wc, const double* stats, double* ssim, void* work, size_t work_bytes, void* stream);
+
+/* ------------------------------------------------------------------------
+ * LPIPS (net-lin, AlexNet, v0.1) as both of TecoGAN's copies compute it (codes/metrics/LPIPS,
+ * codes/official_metrics/LPIPSmodels; oracle/lpips.py is the specification of every layout below).  AlexNet's five
+ * convs run on tg_conv_tcgen05 as pad-1 3x3 convs:
+ *   conv1 (11x11, stride 4, pad 2, 3 -> 64): a 3x3 conv over the space-to-depth(4) picture, zero-padded by 2 at the
+ *         top and left, on an (oh+2) x (ow+2) grid (oh = (h-7)/4 + 1, ow likewise) with cin = 64, cin_real = 48
+ *         (channel (py*4 + px)*3 + c) and the 11x11 kernel zero-padded to 12x12 and split the same way; its output
+ *         is the grid's interior at (1, 1).
+ *   conv2 (5x5, pad 2, 64 -> 192): a 3x3 conv over four copies of the pooled map (cin = 256, copy b = (by, bx)
+ *         shifted by (3by - 1, 3bx - 1), zero fill) with the kernel padded to 6x6 and split into four 3x3 blocks, on
+ *         a (ph+2) x (pw+2) grid; its output is the interior at (1, 1).
+ *   conv3 .. conv5 (192 -> 384 -> 256 -> 256): plain pad-1 3x3 convs.
+ * Each layer's feature (after its ReLU) feeds a head; a picture needs at least TG_LPIPS_MIN_SIDE pixels per side.
+ * ---------------------------------------------------------------------- */
+#define TG_LPIPS_MIN_SIDE 31   /* below it the second pool is empty */
+enum { TG_LPIPS_NORM_CALC = 0,      /* MetricCalculator: float32 x * 2 / 255 - 1 */
+       TG_LPIPS_NORM_OFFICIAL = 1   /* the official script's util.im2tensor: float64 x / 127.5 - 1, then float32 */ };
+/* t uint8 RGB frames [t, frame_h, frame_w, 3] read through `win` (the h x w picture at (top, left)) -> out fp16 NHWC
+ * [t, oh+2, ow+2, 64] in conv1's layout: channel (py*4 + px)*3 + c of grid pixel (Y, X) holds the normalised
+ * (norm: TG_LPIPS_NORM_*) and scaled ((v - shift[c]) / scale[c], PNetLin's ScalingLayer, fp32) value of picture pixel
+ * (4Y + py - 2, 4X + px - 2), 0 outside the picture; channels 48..63 are 0.  One read of the frames.
+ * TG_E_INVALID: null pointers, non-positive sizes, a picture outside its frame, a bad norm, out not 16-byte aligned;
+ * TG_E_UNSUPPORTED: h or w below TG_LPIPS_MIN_SIDE. */
+int tg_lpips_frames_in(const uint8_t* frames, const tg_frame_window* win, int t, int h, int w, int norm, void* out,
+                       void* stream);
+/* MaxPool2d(3, 2) (floor) of the h x w interior at (y0, x0) of x fp16 NHWC [n, xh, xw, c] (c a multiple of 8), with
+ * ph = (h-3)/2 + 1, pw = (w-3)/2 + 1:
+ *   shifts == 0: y [n, ph, pw, c]
+ *   shifts != 0: conv2's input, y [n, ph+2, pw+2, 4c]: channel block b = by*2 + bx of pixel (i, j) holds the pooled
+ *                pixel (i + 3by - 2, j + 3bx - 2), 0 outside the pooled map.
+ * Every output element is written.  TG_E_INVALID: null or misaligned (16 bytes) pointers, bad sizes, an interior below
+ * 3x3 or outside x. */
+int tg_maxpool3x3s2_nhwc_f16(const void* x, int n, int xh, int xw, int c, int y0, int x0, int h, int w, void* y,
+                             int shifts, void* stream);
+/* Bytes of tg_lpips_head's workspace for npairs pairs and an h x w interior (0 for bad sizes). */
+size_t tg_lpips_head_workspace_bytes(int npairs, int h, int w);
+/* One LPIPS layer for npairs pairs of images of a batch of features feat fp16 NHWC [n, xh, xw, c] (c <= 512, a
+ * multiple of 8), over the h x w interior at (y0, x0): pair k = (pairs[2k], pairs[2k+1]) (int32, device memory; an
+ * index outside [0, n) scores NaN) gives
+ *   d = mean over the interior of sum_c weights[c] (f0_c / (|f0| + 1e-10) - f1_c / (|f1| + 1e-10))^2,
+ * |f| the pixel's channel norm.  Per pixel in fp32; the pixels are summed in float64 per CTA and the CTA sums per pair
+ * in a fixed order through the workspace, so the same inputs give the same bits.  out [npairs] float64: out = d, or
+ * out += d with accumulate != 0 (the five layers of LPIPS summed in layer order).  weights fp32 [c].
+ * TG_E_INVALID: null or misaligned pointers (feat 16 bytes, pairs / weights 4, out / work 8), bad sizes, an interior
+ * outside the map, a short workspace; TG_E_UNSUPPORTED: c, more than 65535 pairs.  Two launches. */
+int tg_lpips_head(const void* feat, int n, int xh, int xw, int c, int y0, int x0, int h, int w, const int32_t* pairs,
+                  int npairs, const float* weights, int accumulate, double* out, void* work, size_t work_bytes,
+                  void* stream);
 
 /* BD degradation of the data side (codes/utils/data_utils.py:30-53, called on GT frames by
  * base_model.py:75,115): optional reflect pad by (k-1)/2 | k-1-(k-1)/2, then a depthwise valid

@@ -115,3 +115,19 @@ def make_clip(seed, t, c, h, w, shift=1):
     big = np.clip(_smooth_upsample(base, 4), 0.0, 1.0)
     frames = [big[0, :, 2:2 + h, 2 + shift * i:2 + shift * i + w] for i in range(t)]
     return _t(np.stack(frames).astype(np.float32))
+
+
+def make_lpips_params(seed=0):
+    """Seeded weights of LPIPS net-lin AlexNet v0.1 (numpy float32), under torchvision's keys features.{0,3,6,8,10}.*
+    and the heads lin{0..4}.model.1.weight.  Convs at the scale of PyTorch's default Conv2d init (uniform in
+    +-1/sqrt(fan_in)); heads non-negative, as the published ones are."""
+    rng = np.random.default_rng(seed)
+    shapes = ((64, 3, 11, 11), (192, 64, 5, 5), (384, 192, 3, 3), (256, 384, 3, 3), (256, 256, 3, 3))
+    p = OrderedDict()
+    for idx, shape in zip((0, 3, 6, 8, 10), shapes):
+        bound = 1.0 / np.sqrt(np.prod(shape[1:]))
+        p[f'features.{idx}.weight'] = rng.uniform(-bound, bound, shape).astype(np.float32)
+        p[f'features.{idx}.bias'] = rng.uniform(-bound, bound, shape[0]).astype(np.float32)
+    for l, shape in enumerate(shapes):
+        p[f'lin{l}.model.1.weight'] = rng.uniform(0, 0.5, (1, shape[0], 1, 1)).astype(np.float32)
+    return p

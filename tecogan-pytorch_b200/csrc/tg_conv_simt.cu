@@ -128,8 +128,8 @@ static int pack_common(const float* w, int kind, int cout, int cin, void* packed
   TG_REQUIRE(w && packed, TG_E_INVALID, "pack_weights: null pointer");
   TG_REQUIRE(cout > 0 && cin > 0 && cout <= cout_pad && cin <= cin_pad, TG_E_INVALID,
              "pack_weights: cout=%d cin=%d exceed pads %d/%d", cout, cin, cout_pad, cin_pad);
-  TG_REQUIRE(cin_pad % 64 == 0 && cout_pad % 16 == 0 && cout_pad <= 256, TG_E_UNSUPPORTED,
-             "pack_weights: cin_pad %% 64, cout_pad %% 16, cout_pad <= 256 required");
+  TG_REQUIRE(cin_pad % 64 == 0 && cout_pad % 16 == 0 && cout_pad <= 384, TG_E_UNSUPPORTED,
+             "pack_weights: cin_pad %% 64, cout_pad %% 16, cout_pad <= 384 required");
   const size_t total = (size_t)9 * cin_pad * cout_pad;
   int grid = (int)((total + 255) / 256);
   if (grid > tg_sms() * 16) grid = tg_sms() * 16;

@@ -3,7 +3,7 @@
 //
 //   M tile  = 128 output pixels = a 16x8 patch of one image (row m <-> pixel (m>>3, m&7)), issued as
 //             two m64 wgmmas (tile rows 0-7 and 8-15)
-//   N       = 64 output channels per CTA (layers with 128 / 256 are split over 2 / 4 CTAs); 48 for
+//   N       = 64 output channels per CTA (layers with 128 ... 384 are split over 2 ... 6 CTAs); 48 for
 //             the thin heads (MODE_TAPN: 9 taps x 4 couts in N, 3x3 shift-add in the epilogue)
 //   K       = 64-channel chunks x 9 taps; wgmma K = 16 -> 4 k-steps per (tap, chunk)
 //   A       : NHWC fp16 activations, fetched by TMA (4-D tiled map, 128B swizzle, OOB zero fill =
@@ -53,7 +53,7 @@ namespace {
 
 constexpr int kMaxRing = 4;               // smem stages per ring
 constexpr int kBiasBar = 4;               // named barrier of all consumer warpgroups (1 + cw: one consumer's)
-constexpr uint32_t kHeaderBytes = 2048;   // barriers (first 1 KB) + bias (second 1 KB)
+constexpr uint32_t kHeaderBytes = 2048;   // barriers (first 1 KB) + bias (second 1 KB; 2 KB for cout = 384)
 constexpr uint32_t kTapABytes = TH * TW * 128;  // 16 KB
 constexpr uint32_t kPoolTileBytes = kTapABytes / 4;   // the pooled 8x4 px x 64 ch output tile
 // A-operand modes (template parameter MODE)
@@ -883,14 +883,14 @@ int tg_conv_validate(const tg_conv_desc* d, const char* who) {
              TG_E_UNSUPPORTED, "%s: derivative epilogues need NHWC output and a conv3x3 / conv3x3s2 layer", who);
   TG_REQUIRE(!(d->kind == TG_CONV_3X3_S2 && d->epilogue != TG_EPI_NHWC_F16), TG_E_UNSUPPORTED,
              "%s: conv3x3s2 needs the NHWC epilogue", who);
-  TG_REQUIRE(d->cin == 64 || d->cin == 128 || d->cin == 256, TG_E_UNSUPPORTED,
-             "%s: cin=%d (stored channels must be 64, 128 or 256)", who, d->cin);
+  TG_REQUIRE(d->cin == 64 || d->cin == 128 || d->cin == 192 || d->cin == 256 || d->cin == 384, TG_E_UNSUPPORTED,
+             "%s: cin=%d (stored channels must be 64, 128, 192, 256 or 384)", who, d->cin);
   if (d->epilogue == TG_EPI_NHWC_F16_POOL2)
     TG_REQUIRE(d->kind == TG_CONV_3X3 && d->residual == nullptr && d->act <= TG_ACT_LRELU02 && d->h >= 2 && d->w >= 2,
                TG_E_UNSUPPORTED, "%s: the pooled epilogue needs a conv3x3 without residual / derivative epilogue", who);
   if (d->epilogue == TG_EPI_NHWC_F16 || d->epilogue == TG_EPI_NHWC_F16_POOL2) {
-    TG_REQUIRE(d->cout == 64 || d->cout == 128 || d->cout == 256, TG_E_UNSUPPORTED,
-               "%s: cout=%d (64, 128 or 256 for the NHWC epilogue)", who, d->cout);
+    TG_REQUIRE(d->cout == 64 || d->cout == 128 || d->cout == 192 || d->cout == 256 || d->cout == 384,
+               TG_E_UNSUPPORTED, "%s: cout=%d (64, 128, 192, 256 or 384 for the NHWC epilogue)", who, d->cout);
     TG_REQUIRE(!(d->residual && d->kind == TG_CONVT_3X3_S2), TG_E_UNSUPPORTED, "%s: residual with convT", who);
     TG_REQUIRE(!(d->kind == TG_CONVT_3X3_S2 && d->cout != 64), TG_E_UNSUPPORTED,
                "%s: convT needs cout == 64 (4 parity accumulators per tile)", who);
@@ -936,15 +936,19 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
   const bool convT = d->kind == TG_CONVT_3X3_S2;
   // Forward 3x3 convs with 128 / 256 input channels (NHWC output, pooled or not) split K over a cluster of
   // cin/64 CTAs (MODE_SPLITK), each with one chunk's weights resident; TG_AMODE_TAP keeps the tap kernel.
-  const bool splitk = d->a_mode == TG_AMODE_AUTO && d->kind == TG_CONV_3X3 && !bwd && !tapn && p.chunks >= 2 &&
-                      d->residual == nullptr;
+  // consumer_splitk partitions the four 16-cout warps among the ranks, so 192 / 384 input channels (3 / 6 chunks)
+  // stream their weights in tap mode.
+  const bool splitk = d->a_mode == TG_AMODE_AUTO && d->kind == TG_CONV_3X3 && !bwd && !tapn &&
+                      (p.chunks == 2 || p.chunks == 4) && d->residual == nullptr;
+  // the bias follows the barriers: 1 KB holds 256 output channels, 384 take a second KB
+  const uint32_t header = kHeaderBytes + (d->cout > 256 ? 1024u : 0u);
   const uint32_t b_total = (tapn ? 1u : 9u) * (splitk ? 1u : (uint32_t)p.chunks) * p.b_stage_bytes;   // resident slice per CTA
   const int hbox_w = d->kind != TG_CONVT_3X3_S2 ? TW + 2 : TW + 1;
   const int hbox_h = d->kind != TG_CONVT_3X3_S2 ? TH + 2 : TH + 1;
   const uint32_t halo_bytes = (uint32_t)hbox_w * hbox_h * 128u;
   const uint32_t halo_stage = (halo_bytes + 1023u) & ~1023u;
   const uint32_t scratch = 2u * scratch_bytes(tapn ? MODE_TAPN : MODE_TAP);
-  const uint32_t fixed = 1024u /*align slack*/ + kHeaderBytes + scratch;
+  const uint32_t fixed = 1024u /*align slack*/ + header + scratch;
 
   // every consumer needs at least one stage of its own
   const bool can_resident_halo = fixed + b_total + 2u * halo_stage <= kSmemLimit &&
@@ -993,7 +997,7 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
                              : !pxn  ? scratch
                              : convT ? 4u * kTapABytes
                                      : 3u * (pool ? kPoolTileBytes : kTapABytes);
-  const uint32_t avail = kSmemLimit - 1024u - kHeaderBytes - epi_tiles - (p.b_resident ? b_total : 0u);
+  const uint32_t avail = kSmemLimit - 1024u - header - epi_tiles - (p.b_resident ? b_total : 0u);
   const int rings = three ? 1 : 2;
   int ring = (int)(avail / p.stage_bytes) / rings;
   if (ring > kMaxRing) ring = kMaxRing;
@@ -1002,8 +1006,8 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
              "conv: the three-consumer halo conv needs cin = 64 and 4 halo stages (cin=%d cout=%d: %d)", d->cin,
              d->cout, ring);
   p.ring = ring;
-  p.off_b = kHeaderBytes;
-  p.off_stage = kHeaderBytes + (p.b_resident ? b_total : 0u);
+  p.off_b = header;
+  p.off_stage = header + (p.b_resident ? b_total : 0u);
   p.off_scratch = p.off_stage + (uint32_t)(rings * ring) * p.stage_bytes;   // ring c: stages [c*ring, (c+1)*ring)
   const uint32_t smem_bytes = 1024u + p.off_scratch + epi_tiles;
   TG_REQUIRE(smem_bytes <= kSmemLimit, TG_E_UNSUPPORTED, "conv: smem %u > limit", smem_bytes);

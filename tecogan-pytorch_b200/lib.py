@@ -25,6 +25,8 @@ SCENE_CUT_WORK_BYTES = 16            # TG_SCENE_CUT_WORK_BYTES: workspace of tg_
 TAIL_OUT_ROWS = 40                   # TG_TAIL_OUT_ROWS: rows of tg_pack_tail_out_weights' tile (128 bytes each)
 PSNR_NONE, PSNR_RGB, PSNR_Y = 0, 1, 2
 GATHER_KEEP, GATHER_ZERO, GATHER_LOAD = 0, 1, 2    # TG_GATHER_*: per-slot state modes of tg_stream_gather
+LPIPS_NORM_CALC, LPIPS_NORM_OFFICIAL = 0, 1          # TG_LPIPS_NORM_*: the input normalisation of tg_lpips_frames_in
+LPIPS_MIN_SIDE = 31                                  # TG_LPIPS_MIN_SIDE
 
 
 class ConvDesc(ctypes.Structure):
@@ -142,6 +144,11 @@ _SIGNATURES = {
     'tg_ssim_y_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'tg_ssim_y': (c_int, [_P, c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, c_size_t,
                           _P]),
+    'tg_lpips_frames_in': (c_int, [_P, ctypes.POINTER(FrameWindow), c_int, c_int, c_int, c_int, _P, _P]),
+    'tg_maxpool3x3s2_nhwc_f16': (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, _P]),
+    'tg_lpips_head_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
+    'tg_lpips_head': (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int, _P, c_int, _P, _P,
+                              c_size_t, _P]),
     'tg_downsample_bd_nchw_f32': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_debug_set_conv_timers': (c_int, [_P]),
     # ---- training (generator backward)

@@ -52,7 +52,7 @@ class PackedConv:
     """One 3x3 conv / stride-2 transposed conv of the path with device-packed fp16 weights.
 
     weight: nn.Conv2d layout [cout,cin,3,3] or nn.ConvTranspose2d layout [cin,cout,3,3] (fp32).
-    Stored channel counts are padded to multiples of 64 (cin) and to 64/128/256 or 16 (cout).
+    Stored channel counts are padded to multiples of 64 (cin) and to 64/128/192/256/384 or 16 (cout).
     """
 
     def __init__(self, weight, bias, kind=L.CONV_3X3, act=L.ACT_NONE, epilogue=L.EPI_NHWC_F16):
@@ -948,6 +948,66 @@ def ssim_y(true_u8, pred_u8, window, stats):
     work = torch.empty(max(need, 8) // 8, dtype=torch.float64, device=true_u8.device)
     L.check(L.load().tg_ssim_y(_ptr(true_u8), ht, wt, _ptr(pred_u8), hp, wp, t, *window, _ptr(stats), _ptr(out),
                                _ptr(work), need, _stream()), 'tg_ssim_y')
+    return out
+
+
+def lpips_frames_in(frames, window, norm, out):
+    """tg_lpips_frames_in: uint8 RGB frames [t, H, W, 3], window (y0, x0, h, w) of them, norm L.LPIPS_NORM_* ->
+    out fp16 [t, (h-7)//4 + 3, (w-7)//4 + 3, 64], conv1's space-to-depth input"""
+    _req(frames, torch.uint8, 'frames', 4)
+    t, fh, fw, c = frames.shape
+    y0, x0, h, w = window
+    _req(out, torch.float16, 'out', 4)
+    if c != 3 or tuple(out.shape) != (t, (h - 7) // 4 + 3, (w - 7) // 4 + 3, 64):
+        raise L.TecoganB200Error(f'lpips_frames_in: frames {tuple(frames.shape)}, out {tuple(out.shape)}')
+    _same_device('lpips_frames_in', frames, out)
+    win = L.FrameWindow(fh, fw, y0, x0)
+    L.check(L.load().tg_lpips_frames_in(_ptr(frames), ctypes.byref(win), t, h, w, norm, _ptr(out), _stream()),
+            'tg_lpips_frames_in')
+    return out
+
+
+def maxpool3x3s2(x, interior, shifts, y=None):
+    """tg_maxpool3x3s2_nhwc_f16: MaxPool2d(3, 2) of the interior (y0, x0, h, w) of x fp16 [n, xh, xw, c] -> y
+    [n, ph, pw, c], or with shifts conv2's four-shift input [n, ph+2, pw+2, 4c]"""
+    _req(x, torch.float16, 'maxpool3x3s2 input', 4)
+    n, xh, xw, c = x.shape
+    y0, x0, h, w = interior
+    ph, pw = (h - 3) // 2 + 1, (w - 3) // 2 + 1
+    shape = (n, ph + 2, pw + 2, 4 * c) if shifts else (n, ph, pw, c)
+    if y is None:
+        y = torch.empty(shape, dtype=torch.float16, device=x.device)
+    _req(y, torch.float16, 'maxpool3x3s2 output', 4)
+    if tuple(y.shape) != shape:
+        raise L.TecoganB200Error(f'maxpool3x3s2: output {tuple(y.shape)}, expected {shape}')
+    _same_device('maxpool3x3s2', x, y)
+    L.check(L.load().tg_maxpool3x3s2_nhwc_f16(_ptr(x), n, xh, xw, c, y0, x0, h, w, _ptr(y), 1 if shifts else 0,
+                                             _stream()), 'tg_maxpool3x3s2_nhwc_f16')
+    return y
+
+
+def lpips_head_workspace_bytes(npairs, h, w):
+    return int(L.load().tg_lpips_head_workspace_bytes(npairs, h, w))
+
+
+def lpips_head(feat, interior, pairs, weights, out, accumulate):
+    """tg_lpips_head: one LPIPS layer of the image pairs `pairs` (int32 [P, 2] on the device) of the features feat
+    fp16 [n, xh, xw, c] over their interior (y0, x0, h, w), with the head weights fp32 [c]; out float64 [P] = (or +=,
+    with accumulate) the layer's distance"""
+    _req(feat, torch.float16, 'feat', 4)
+    _req(pairs, torch.int32, 'pairs', 2)
+    _req(weights, torch.float32, 'weights', 1)
+    _req(out, torch.float64, 'out', 1)
+    n, xh, xw, c = feat.shape
+    P = pairs.shape[0]
+    if pairs.shape[1] != 2 or out.shape[0] != P or weights.shape[0] != c:
+        raise L.TecoganB200Error(f'lpips_head: pairs {tuple(pairs.shape)}, out {tuple(out.shape)}, weights '
+                                 f'{tuple(weights.shape)} for {c} channels')
+    _same_device('lpips_head', feat, pairs, weights, out)
+    need = lpips_head_workspace_bytes(P, *interior[2:])
+    work = torch.empty(max(need, 8) // 8, dtype=torch.float64, device=feat.device)
+    L.check(L.load().tg_lpips_head(_ptr(feat), n, xh, xw, c, *interior, _ptr(pairs), P, _ptr(weights),
+                                   1 if accumulate else 0, _ptr(out), _ptr(work), need, _stream()), 'tg_lpips_head')
     return out
 
 

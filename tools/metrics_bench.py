@@ -8,6 +8,12 @@ each phase must move (from shapes) and their share of the H100 SXM's 3.35 TB/s, 
 --official measures official_sequence_metrics (the official metric script's PSNR, SSIM and tOF on the crop_8x8
 window, frames 2 .. T-3) instead: scored frames/s end to end, per-kernel times from CUDA events, the algorithmic
 bytes and TB/s of the Y statistics and SSIM kernels, and oracle/official_metrics.py (cv2 + scipy) on the host cores.
+
+--lpips measures all five official keys (PSNR, SSIM, LPIPS, tOF, tLP100) with seeded AlexNet weights
+(synthetic.make_lpips_params): scored frames/s end to end, per-kernel times of one LPIPS pass over a chunk's frames
+from CUDA events, the AlexNet convs' TFLOP/s (by the reference counter's convention, 2 x MACs of the unpadded convs,
+and as executed on the padded layouts) against the 989 TFLOP/s of dense FP16, and the reference's PNetLin (from
+oracle/_ref) on the same frames with cuDNN at PyTorch's defaults.
 """
 import argparse
 import json
@@ -180,14 +186,150 @@ def main_official(a):
             json.dump(res, f, indent=1)
 
 
+def lpips_flops(h, w):
+    """(reference-convention, executed) FLOP of one h x w picture's five AlexNet convs: 2 x MACs of the direct convs,
+    and 2 x the MACs the device runs on its padded layouts (full grids; conv1 skips its k-steps past 48 channels)"""
+    sz = M.lpips_sizes(h, w)
+    (g1, i1), (g2, i2), (m3, _) = sz[0], sz[1], sz[2]
+    px1, px2, px3 = i1[2] * i1[3], i2[2] * i2[3], m3[0] * m3[1]
+    ref = 2 * (px1 * 64 * 3 * 121 + px2 * 192 * 64 * 25 + px3 * 9 * (384 * 192 + 256 * 384 + 256 * 256))
+    exe = 2 * 9 * (g1[0] * g1[1] * 48 * 64 + g2[0] * g2[1] * 192 * 256 + px3 * (384 * 192 + 256 * 384 + 256 * 256))
+    return ref, exe
+
+
+def reference_pnetlin(params):
+    """the reference's PNetLin (codes/metrics/LPIPS of oracle/_ref, unmodified) with the seeded weights, on cuda:0"""
+    from oracle.gen_lpips_golden import install_stubs
+    codes = os.path.join(ROOT, 'oracle', '_ref', 'codes')
+    if not os.path.isdir(os.path.join(codes, 'metrics', 'LPIPS')):
+        return None
+    install_stubs(codes)
+    from metrics.LPIPS.models import networks_basic as nb
+    net = nb.PNetLin(pnet_rand=True, pnet_tune=False, pnet_type='alex', use_dropout=True, spatial=False,
+                     version='0.1', lpips=True)
+    sd = {}
+    for l, fi in enumerate(M._ALEX_CONVS):
+        for k in ('weight', 'bias'):
+            sd[f'net.slice{l + 1}.{fi}.{k}'] = torch.from_numpy(params[f'features.{fi}.{k}'])
+        sd[f'lin{l}.model.1.weight'] = torch.from_numpy(params[f'lin{l}.model.1.weight'])
+    net.load_state_dict(sd, strict=False)
+    return net.cuda().eval()
+
+
+def main_lpips(a):
+    params = synthetic.make_lpips_params(7)
+    lp = M.LPIPS(params, torch.device('cuda', 0))
+    seqs = [sequence(s) for s in range(a.seqs)]
+    T_, h, w = seqs[0][0].shape[:3]
+    keys = ('PSNR', 'SSIM', 'LPIPS', 'tOF', 'tLP100')
+    M.official_sequence_metrics(*seqs[0], keys=keys, lpips=lp)
+    torch.cuda.synchronize()
+    rates = []
+    for _ in range(3):
+        t0 = time.perf_counter()
+        for t, p in seqs:
+            M.official_sequence_metrics(t, p, keys=keys, lpips=lp)
+        torch.cuda.synchronize()
+        rates.append(len(seqs) * (T_ - 4) / (time.perf_counter() - t0))
+    # one LPIPS pass over the scored frames of a sequence (true and pred), kernel by kernel
+    (y0, hc), (x0, wc) = M.crop_8x8(h), M.crop_8x8(w)
+    t, p = seqs[0]
+    frames = torch.from_numpy(np.concatenate([t[2:T_ - 2, y0:y0 + hc, x0:x0 + wc],
+                                              p[2:T_ - 2, y0:y0 + hc, x0:x0 + wc]])).cuda().contiguous()
+    n, m = frames.shape[0], frames.shape[0] // 2
+    sz = M.lpips_sizes(hc, wc)
+    pairs = torch.tensor([(i, m + i) for i in range(m)] + [(i - 1, i) for i in range(1, m)] +
+                         [(m + i - 1, m + i) for i in range(1, m)], dtype=torch.int32).cuda()
+    out = torch.empty(pairs.shape[0], dtype=torch.float64, device='cuda')
+    x = torch.empty(n, *sz[0][0], 64, dtype=torch.float16, device='cuda')
+    steps = {}
+
+    def run():
+        def ev(name, fn):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            r = fn()
+            e1.record()
+            steps.setdefault(name, []).append((e0, e1))
+            return r
+        ev('frames_in', lambda: ops.lpips_frames_in(frames, (0, 0, hc, wc), L.LPIPS_NORM_OFFICIAL, x))
+        f1 = ev('conv1', lambda: lp.convs[0](x))
+        q1 = ev('pool1', lambda: ops.maxpool3x3s2(f1, sz[0][1], True))
+        f2 = ev('conv2', lambda: lp.convs[1](q1))
+        q2 = ev('pool2', lambda: ops.maxpool3x3s2(f2, sz[1][1], False))
+        f3 = ev('conv3', lambda: lp.convs[2](q2))
+        f4 = ev('conv4', lambda: lp.convs[3](f3))
+        f5 = ev('conv5', lambda: lp.convs[4](f4))
+        ev('heads', lambda: [ops.lpips_head(f, sz[l][1], pairs, lp.heads[l], out, l > 0)
+                             for l, f in enumerate((f1, f2, f3, f4, f5))])
+    for _ in range(3):
+        run()
+    steps.clear()
+    for _ in range(10):
+        run()
+    torch.cuda.synchronize()
+    ms = {k: float(np.median([e0.elapsed_time(e1) for e0, e1 in v])) for k, v in steps.items()}
+    conv_ms = sum(ms[f'conv{i}'] for i in range(1, 6))
+    ref_f, exe_f = lpips_flops(hc, wc)
+    res = {'card': card(), 'shape': [T_, h, w], 'crop': [hc, wc], 'keys': list(keys),
+           'scored_frames_per_sequence': T_ - 4,
+           'scored_frames_per_s_host_to_host': rates,
+           'lpips_pass_images': n, 'lpips_pass_pairs': int(pairs.shape[0]),
+           'kernel_ms_per_pass': ms, 'conv_ms_per_pass': conv_ms,
+           'gflop_per_image_reference_counter': ref_f / 1e9, 'gflop_per_image_executed': exe_f / 1e9,
+           'conv_tflops_reference_counter': n * ref_f / (conv_ms * 1e-3) / 1e12,
+           'conv_tflops_executed': n * exe_f / (conv_ms * 1e-3) / 1e12, 'peak_fp16_dense_tflops': 989}
+    net = reference_pnetlin(params)
+    if net is not None:
+        scale = torch.float32
+        a0 = (frames[:m].permute(0, 3, 1, 2).to(scale) / 127.5 - 1)
+        a1 = (frames[m:].permute(0, 3, 1, 2).to(scale) / 127.5 - 1)
+        with torch.no_grad():
+            for _ in range(2):
+                net.forward(a0, a1)
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(5):
+                d_ref = net.forward(a0, a1)
+            e1.record()
+            torch.cuda.synchronize()
+            ref_ms = e0.elapsed_time(e1) / 5
+            # the same pairs through the device kernels, against float64
+            mine = lp.distances(frames, (0, 0, hc, wc), L.LPIPS_NORM_OFFICIAL, [(i, m + i) for i in range(m)])
+        from oracle import lpips as O
+        # float64 reference of all m pairs (on the GPU: cuDNN's float64 convs), 4 pairs at a time
+        fr = frames.cpu().numpy()
+        want = np.concatenate([O.lpips(params, fr[i:min(i + 4, m)], fr[m + i:m + min(i + 4, m)], 'official', 'cuda')
+                               for i in range(0, m, 4)])
+
+        def errs(d):
+            r = np.abs(np.asarray(d, np.float64) - want) / want
+            return {'max': float(r.max()), 'median': float(np.median(r))}
+        res['reference_pnetlin'] = {
+            'tf32_matmul': torch.backends.cuda.matmul.allow_tf32, 'tf32_cudnn': torch.backends.cudnn.allow_tf32,
+            'ms_per_pass_of_pairs': ref_ms, 'pairs': m,
+            'rel_err_vs_float64_all_pairs': errs(d_ref.flatten().double().cpu().numpy()),
+        }
+        res['device_rel_err_vs_float64_all_pairs'] = errs(mine.cpu().numpy())
+    print(json.dumps(res))
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, 'w') as f:
+            json.dump(res, f, indent=1)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--seqs', type=int, default=4)
     ap.add_argument('--ref-frames', type=int, default=4)
     ap.add_argument('--official', action='store_true', help='measure official_sequence_metrics')
+    ap.add_argument('--lpips', action='store_true', help='measure official_sequence_metrics with all five keys')
     ap.add_argument('--out', default=None)
     a = ap.parse_args()
     assert torch.cuda.is_available(), 'metrics_bench needs a GPU'
+    if a.lpips:
+        return main_lpips(a)
     if a.official:
         return main_official(a)
     seqs = [sequence(s) for s in range(a.seqs)]
