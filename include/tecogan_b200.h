@@ -66,6 +66,10 @@ enum {
                                conv3x3 only, no residual); the full-resolution map is never written */
 };
 enum { TG_AMODE_AUTO = 0, TG_AMODE_HALO = 1, TG_AMODE_TAP = 2 };
+/* Flag OR'd into tg_conv_desc.a_mode (wgmma kernel only): walk the tiles last to first.  The output bits do not
+ * depend on the walk.  A launch that reads a map the previous launch wrote then starts on the tiles written last,
+ * which are the ones still in L2; networks.py alternates the direction along each chain of convs. */
+#define TG_AMODE_REVERSE 0x100
 
 int tg_version(void);
 const char* tg_last_error_string(void);
@@ -127,7 +131,7 @@ typedef struct tg_conv_desc {
   int32_t kind;         /* TG_CONV_3X3 | TG_CONVT_3X3_S2                                 */
   int32_t act;          /* TG_ACT_*                                                      */
   int32_t epilogue;     /* TG_EPI_*                                                      */
-  int32_t a_mode;       /* TG_AMODE_* (wgmma kernel only; AUTO = fastest validated)      */
+  int32_t a_mode;       /* TG_AMODE_* (wgmma kernel only; AUTO = fastest validated), | TG_AMODE_REVERSE */
   int32_t max_ctas;     /* 0 = one persistent CTA per SM                                 */
   int32_t cin_real;     /* input channels that can be non-zero (0 = cin): for cin = 64 the wgmma kernel skips the
                            k-steps of 16 channels at or beyond it -- the packed weights are zero there, so the

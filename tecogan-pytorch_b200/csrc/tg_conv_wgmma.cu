@@ -84,6 +84,7 @@ struct KParams {
   uint32_t stage_bytes, a_bytes, b_tile_bytes, b_stage_bytes;
   uint32_t off_b, off_stage, off_scratch;   // off_scratch: the consumers' fp32 staging or fp16 output tiles
   uint32_t epi_bytes;              // MODE_SPLITK: per-consumer receive buffer (the output tile overlaps it)
+  int reverse;                     // schedule index t works on tile num_tiles - 1 - t (TG_AMODE_REVERSE)
 };
 
 // The mbarriers of the header (8 bytes each), every slot named once; c = consumer 0 / 1 (0..2 for res and turn).
@@ -122,8 +123,10 @@ __host__ __device__ constexpr int conv_threads() {
 }
 
 struct TileCoord { int n, y0, x0, nb; };
+// Every role maps its schedule index to a tile here, so the walk direction is applied once for all of them.
 __device__ __forceinline__ TileCoord tile_coord(const KParams& p, int tile) {
   TileCoord t;
+  if (p.reverse) tile = p.num_tiles - 1 - tile;
   const int per_img = p.tiles_x * p.tiles_y;
   const int sp = tile / p.n_split;          // CTAs that share an A tile are adjacent (L2 reuse)
   t.nb = tile - sp * p.n_split;
@@ -579,8 +582,8 @@ conv_wgmma_kernel(const __grid_constant__ TgMaps maps, const KParams p) {
   // separates tg_pack_* from the conv by a bias copy): start their load, then join the
   // programmatic-dependent-launch wait.  The previous kernel's OUTPUT is only read after tg_pdl_wait().
   if (warp == 0 && lane == 0 && p.b_resident) {
-    // fixed per CTA: the number of CTAs (clusters for split-K) is a multiple of n_split
-    const uint32_t nb = (uint32_t)sched0 % (uint32_t)p.n_split;
+    // fixed per CTA: the number of CTAs (clusters for split-K) and num_tiles are multiples of n_split
+    const uint32_t nb = (uint32_t)tile_coord(p, sched0).nb;
     mbar_expect_tx(bar_b, (uint32_t)n_tiles_w * p.b_stage_bytes);
     for (int t = 0; t < n_tiles_w; ++t) {
       const int src = kSplitK ? t * p.chunks + k_rank : t;   // split-K: the 9 taps of chunk k_rank
@@ -907,12 +910,15 @@ int tg_conv_validate(const tg_conv_desc* d, const char* who) {
 int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
   int rc = tg_conv_validate(d, "conv");
   if (rc != TG_OK) return rc;
-  TG_REQUIRE(d->a_mode >= TG_AMODE_AUTO && d->a_mode <= TG_AMODE_TAP, TG_E_INVALID, "conv: a_mode");
+  const int a_mode = d->a_mode & ~TG_AMODE_REVERSE;
+  TG_REQUIRE(a_mode >= TG_AMODE_AUTO && a_mode <= TG_AMODE_TAP, TG_E_INVALID, "conv: a_mode");
   TG_REQUIRE(((uintptr_t)d->x & 15) == 0 && ((uintptr_t)d->weights & 15) == 0 && ((uintptr_t)d->y & 15) == 0,
              TG_E_INVALID, "conv: pointers must be 16-byte aligned");
 
   KParams p;
   p.d = *d;
+  p.d.a_mode = a_mode;
+  p.reverse = (d->a_mode & TG_AMODE_REVERSE) != 0;
   const bool tapn = d->epilogue == TG_EPI_FLOW_NCHW_F32 || d->epilogue == TG_EPI_OUT_NCHW_F32;
   const bool pool = d->epilogue == TG_EPI_NHWC_F16_POOL2;
   p.step_y = tapn ? kTapnStepY : TH;
@@ -938,7 +944,7 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
   // cin/64 CTAs (MODE_SPLITK), each with one chunk's weights resident; TG_AMODE_TAP keeps the tap kernel.
   // consumer_splitk partitions the four 16-cout warps among the ranks, so 192 / 384 input channels (3 / 6 chunks)
   // stream their weights in tap mode.
-  const bool splitk = d->a_mode == TG_AMODE_AUTO && d->kind == TG_CONV_3X3 && !bwd && !tapn &&
+  const bool splitk = a_mode == TG_AMODE_AUTO && d->kind == TG_CONV_3X3 && !bwd && !tapn &&
                       (p.chunks == 2 || p.chunks == 4) && d->residual == nullptr;
   // the bias follows the barriers: 1 KB holds 256 output channels, 384 take a second KB
   const uint32_t header = kHeaderBytes + (d->cout > 256 ? 1024u : 0u);
@@ -954,7 +960,7 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
   const bool can_resident_halo = fixed + b_total + 2u * halo_stage <= kSmemLimit &&
                                  !(d->kind == TG_CONVT_3X3_S2 && p.chunks != 1);
   const bool can_resident_tap = fixed + b_total + 2u * kTapABytes <= kSmemLimit;
-  int mode = d->a_mode;
+  int mode = a_mode;
   TG_REQUIRE(!(d->kind == TG_CONV_3X3_S2 && mode == TG_AMODE_HALO), TG_E_UNSUPPORTED,
              "conv: conv3x3s2 runs in tap mode (a stride-2 view is not a wgmma descriptor)");
   if (d->kind == TG_CONV_3X3_S2 || tapn) mode = TG_AMODE_TAP;   // thin heads run MODE_TAPN below

@@ -263,7 +263,9 @@ upsample2x_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int n, int
   tg_pdl_trigger();
   const int total = n * h * w * c8;
   const int wo = 2 * w;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+  // last element first: the conv that reads the output walks its tiles forward (networks.FNet.CHAIN)
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < total; j += gridDim.x * blockDim.x) {
+    const int i = total - 1 - j;
     const int cv = i % c8;
     int p = i / c8;
     const int xi = p % w; p /= w;
@@ -300,7 +302,9 @@ pack_pair_c64_kernel(const float* __restrict__ x1, const float* __restrict__ x2,
   tg_pdl_wait();
   tg_pdl_trigger();
   const int total = n * hw;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+  // last pixel first: FNet's first conv walks its tiles forward (networks.FNet.CHAIN)
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < total; j += gridDim.x * blockDim.x) {
+    const int i = total - 1 - j;
     const int nn = i / hw, sp = i - nn * hw;
     __align__(16) __half vals[8];
 #pragma unroll
@@ -482,8 +486,11 @@ __global__ void to_uint8_c3x4_kernel(const float4* __restrict__ x, uint32_t* __r
   tg_pdl_wait();
   tg_pdl_trigger();
   const size_t total = (size_t)n * hw4;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total;
-       i += (size_t)gridDim.x * blockDim.x) {
+  // last pixels first: the fused SRNet tail, which writes x just before, walks its tiles forward, so its last
+  // tiles are the ones still in L2
+  for (size_t j = blockIdx.x * (size_t)blockDim.x + threadIdx.x; j < total;
+       j += (size_t)gridDim.x * blockDim.x) {
+    const size_t i = total - 1 - j;
     const size_t nn = i / hw4, sp = i % hw4;
     const float4 r = __ldg(x + (nn * 3 + 0) * hw4 + sp);
     const float4 g = __ldg(x + (nn * 3 + 1) * hw4 + sp);

@@ -18,6 +18,7 @@ CONV_3X3, CONVT_3X3_S2, CONV_3X3_S2 = 0, 1, 2
 UP_BICUBIC, UP_BILINEAR = 0, 1
 EPI_NHWC_F16, EPI_FLOW_NCHW_F32, EPI_OUT_NCHW_F32, EPI_NHWC_F16_POOL2 = 0, 1, 2, 3
 AMODE_AUTO, AMODE_HALO, AMODE_TAP = 0, 1, 2
+AMODE_REVERSE = 0x100               # TG_AMODE_REVERSE: flag, walk the conv's tiles last to first
 YUV_NV12, YUV_I420, YUV_P010, YUV_I420_10 = 0, 1, 2, 3
 YUV_YUY2, YUV_UYVY, YUV_I444, YUV_I444_10 = 4, 5, 6, 8      # 7 is not a layout
 RESAMPLE_BICUBIC, RESAMPLE_LANCZOS3 = 0, 1

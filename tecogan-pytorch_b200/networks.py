@@ -81,6 +81,11 @@ class FNet(nn.Module):
 
     ENC = (('encoder1', None, 32), ('encoder2', 32, 64), ('encoder3', 64, 128))
     DEC = (('decoder1', 128, 256), ('decoder2', 256, 128), ('decoder3', 128, 64))
+    # Position of each conv from the input to the flow head.  The convs alternate their tile walk along it, odd
+    # positions walking last to first (PackedConv.reverse), so that each starts on the tiles its producer wrote
+    # last, which are still in L2.  pack_pair and upsample2x walk last to first, so encoder1[0] and flow[0], which
+    # read their full-resolution maps, walk forward.
+    CHAIN = {k: i for i, k in enumerate([(b, j) for b, _, _ in ENC + DEC for j in (0, 2)] + [('flow', 0), ('flow', 2)])}
 
     def __init__(self, in_nc):
         super().__init__()
@@ -94,7 +99,9 @@ class FNet(nn.Module):
         self._cache = _ConvCache()
 
     def _conv(self, block, idx, act, epilogue=L.EPI_NHWC_F16):
-        return self._cache.get((block, idx), getattr(self, block)[idx], L.CONV_3X3, act, epilogue)
+        pc = self._cache.get((block, idx), getattr(self, block)[idx], L.CONV_3X3, act, epilogue)
+        pc.reverse = self.CHAIN[(block, idx)] % 2 == 1
+        return pc
 
     def forward(self, x1, x2):
         """flow from x1 to x2, NCHW fp32 [n,2,8*(h//8),8*(w//8)]"""
@@ -176,11 +183,17 @@ class SRNet(nn.Module):
         for i, blk in enumerate(self.resblocks):
             body += [c.get(('r', i, 0), blk.conv[0], L.CONV_3X3, _RELU),
                      c.get(('r', i, 2), blk.conv[2], L.CONV_3X3, L.ACT_NONE)]
+        ups = [c.get(('up', u), self.conv_up[u], L.CONVT_3X3_S2, _RELU) for u in range(0, len(self.conv_up), 2)]
+        # Each conv walks its tiles opposite to the launch that wrote its input, so it starts on the tiles that are
+        # still in L2: conv_in last to first against warp_s2d_concat's forward walk, then alternating down the body
+        # to the first transposed conv.  A residual conv also reads `a` right after the plain conv read it the
+        # other way round.
+        for i, pc in enumerate(body + ups):
+            pc.reverse = i % 2 == 0
         a = body[0](x)
         for i in range(len(self.resblocks)):
             t = body[1 + 2 * i](a)
             a = body[2 + 2 * i](t, residual=a)
-        ups = [c.get(('up', u), self.conv_up[u], L.CONVT_3X3_S2, _RELU) for u in range(0, len(self.conv_up), 2)]
         pc_out = c.get('out', self.conv_out, L.CONV_3X3, L.ACT_NONE, L.EPI_OUT_NCHW_F32)
         tail = ops.tail_mode()
         if (tail and ops.default_conv_impl() == 'tcgen05' and ups[-1].cin == 64 and ups[-1].cout == 64

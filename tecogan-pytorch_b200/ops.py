@@ -64,6 +64,9 @@ class PackedConv:
         self.cin = pad64(self.cin_real)
         self.tapn = epilogue != L.EPI_NHWC_F16      # thin NCHW heads: tap-major N packing
         self.cout = pad64(self.cout_real) if not self.tapn else 48
+        # Walk the tiles last to first (TG_AMODE_REVERSE); same output bits.  The networks set it so that each conv
+        # walks opposite to the launch that wrote its input and starts on what is still in L2.
+        self.reverse = False
         self.packed = None
         self.tail_packed = None
         self.bias = None
@@ -139,7 +142,7 @@ class PackedConv:
         d.y = y.data_ptr()
         d.n, d.h, d.w, d.cin, d.cout, d.cout_real = n, h, w, self.cin, self.cout, self.cout_real
         d.kind, d.act, d.epilogue = self.kind, self.act, (L.EPI_NHWC_F16_POOL2 if pool else self.epilogue)
-        d.a_mode = default_a_mode() if a_mode is None else a_mode
+        d.a_mode = (default_a_mode() if a_mode is None else a_mode) | (L.AMODE_REVERSE if self.reverse else 0)
         d.max_ctas = max_ctas
         d.cin_real = self.cin_real
         impl = impl or default_conv_impl()
