@@ -124,7 +124,7 @@ typedef struct tg_conv_desc {
   void* y;              /* see epilogue; convT writes [n,2h,2w,cout]                     */
   int32_t n, h, w;      /* batch and the height / width the kernel tiles over: the input's (= the
                            output's for conv3x3; convT writes 2h x 2w), the OUTPUT's for TG_CONV_3X3_S2 */
-  int32_t cin, cout;    /* stored channel counts: cin in {64,128,192,256,384}; cout in {64,128,192,256,384}
+  int32_t cin, cout;    /* stored channel counts: cin in {64,128,192,256,384,512}; cout in {64,...,384,512}
                            for TG_EPI_NHWC_F16, 48 (= TG_TAPN_ROWS, tap-major N packing)
                            for the two NCHW epilogues                                    */
   int32_t cout_real;    /* NCHW epilogues: channels actually written (2 resp. 3)         */
@@ -583,6 +583,23 @@ int tg_grad_pack_nhwc_f16(const float* a, const float* b, const float* scale, vo
 /* channels [c_offset, c_offset+c) of NHWC fp16 -> NCHW fp32 * 1/scale ; accumulate != 0 adds into y */
 int tg_grad_unpack_nchw_f32(const void* x, const float* scale, float* y, int n, int c, int h, int w, int cpad,
                             int c_offset, int accumulate, void* stream);
+/* The amax step of tg_grad_scale_from_amax alone: folds max |a| into the workspace, so that the next
+ * tg_grad_scale_from_amax on the same ws chooses one scale for several tensors (the VGG extractor's taps). */
+int tg_grad_amax_f32(const float* a, size_t na, void* ws, void* stream);
+/* tg_grad_pack_nhwc_f16 of one tensor a, with each of these steps where its operand is non-NULL, in this order:
+ *   v = (a - sub[ch]) / div[ch]     per-channel normalisation in fp32 (sub and div fp32 [c], given together)
+ *   v = v * scale                   (scale NULL: 1)
+ *   v = v + add                     add NHWC fp16 [n,h,w,cpad], every channel
+ *   v = v * act'(mask)              mask NHWC fp16 [n,h,w,cpad], the stored forward output; act TG_ACT_DRELU /
+ *                                   TG_ACT_DLRELU02 with a mask, TG_ACT_NONE without
+ * -> NHWC fp16 y [n,h,w,cpad] (channels >= c of a count as 0).  VGG19 perceptual loss: the input normalisation
+ * (vgg_nets.py:30) and each feature tap's loss gradient joined to the running gradient.  y, add, mask 16-byte aligned. */
+int tg_grad_pack_ex_nhwc_f16(const float* a, const float* sub, const float* div, const float* scale, const void* add,
+                             const void* mask, int act, void* y, int n, int c, int h, int w, int cpad, void* stream);
+/* tg_grad_unpack_nchw_f32 with a per-channel divisor: y = x * 1/scale / div[ch] (div fp32 [c], non-NULL; the input
+ * gradient of the VGG extractor through its normalisation (x - mean) / std) */
+int tg_grad_unpack_ex_nchw_f32(const void* x, const float* scale, const float* div, float* y, int n, int c, int h,
+                               int w, int cpad, int c_offset, int accumulate, void* stream);
 /* db[ch] += 1/scale * sum_pixels dz[p][ch], ch < c_real  (bias gradient of any conv layer) */
 int tg_bias_grad_nhwc_f16(const void* dz, size_t npix, int c, int c_real, const float* scale, float* db,
                           void* stream);

@@ -16,8 +16,9 @@ from .autograd import st_discriminator_input  # noqa: F401
 from . import reducer  # noqa: F401
 from . import metrics  # noqa: F401
 from .reducer import FlatGradientReducer  # noqa: F401
+from .vgg import VGGFeatureExtractor  # noqa: F401
 
 __all__ = ['FRNet', 'FNet', 'SRNet', 'define_generator', 'space_to_depth', 'backward_warp',
            'get_upsampling_func', 'BicubicUpsampler', 'infer_clips', 'ClipEngine', 'VideoStream',
            'clips_for_rank', 'st_discriminator_input', 'FlatGradientReducer', 'load_library', 'TecoganB200Error', 'create_kernel', 'downsample_bd',
-           'metrics']
+           'metrics', 'VGGFeatureExtractor']

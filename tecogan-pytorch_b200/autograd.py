@@ -346,3 +346,67 @@ def st_discriminator_input(data, bi_data, hr_flow_merge, spatial_size, crop_bord
     csize = int(spatial_size * crop_border_ratio)
     pad = (spatial_size - csize) // 2
     return StDiscInputFunction.apply(data, bi_data[:, :data.shape[1]], hr_flow_merge.detach(), t, pad, csize)
+
+
+# ================================================================================ VGG19 perceptual loss
+def vgg_forward(vgg, x, keep):
+    """VGGFeatureExtractor.forward on the kernels: x NCHW fp32 [N,3,H,W] -> (features NCHW fp32, tape).  keep=True
+    keeps every conv's NHWC fp16 output (the ReLU' masks and max-pool routes of the backward) in the tape; keep=False
+    keeps nothing, and each map is freed once the next layer has read it."""
+    layers = vgg.packed_layers()
+    a = ops.grad_pack_ex(x, sub=vgg.mean.view(3), div=vgg.std.view(3))     # (x - mean) / std, 64 channels
+    outs, feats = [], {}
+    for u, ((fwd, _), (_, _, pool)) in enumerate(zip(layers, vgg._units)):
+        a = fwd(a)
+        if u in vgg._taps:
+            feats[u] = ops.nhwc_to_nchw(a, fwd.cout_real)
+        if keep:
+            outs.append(a)
+        if pool and u + 1 < len(layers):
+            a = ops.maxpool2x2(a)
+    return [feats[u] for u in vgg._taps], outs
+
+
+def vgg_backward(vgg, outs, grads):
+    """input gradient of the extractor: grads[k] = d loss / d feature k (NCHW fp32) -> d loss / d x (NCHW fp32).
+
+    Walks the units from the deepest tap to conv1_1 with dz = d loss / d (pre-ReLU output of the unit), loss-scaled
+    NHWC fp16 under ONE scale chosen from the amax over all the taps' gradients.  A tap on a unit followed by a conv
+    joins as the dgrad epilogue's residual, (dgrad + tap) * ReLU'; a tap on a unit followed by a max-pool joins after
+    the pool's backward, (route + tap) * ReLU' (tg_grad_pack_ex_nhwc_f16)."""
+    layers = vgg.packed_layers()
+    tap_of = {u: k for k, u in enumerate(vgg._taps)}
+    sc = ops.GradScale(outs[0].device).from_amax_of(grads)
+    last = len(layers) - 1
+    dz = ops.grad_pack_ex(grads[tap_of[last]], scale=sc, mask=outs[last], mask_act=_RELU, cpad=outs[last].shape[-1])
+    for u in range(last, 0, -1):
+        dg = layers[u][1]
+        prev, pool = outs[u - 1], vgg._units[u - 1][2]
+        k = tap_of.get(u - 1)
+        if not pool:
+            res = ops.grad_pack(grads[k], scale=sc, cpad=prev.shape[-1]) if k is not None else None
+            dz = dg(dz, residual=res, mask=prev, mask_act=_RELU)
+        elif k is None:
+            dz = ops.maxpool2x2_bwd(prev, dg(dz), _RELU)
+        else:
+            route = ops.maxpool2x2_bwd(prev, dg(dz), _NONE)
+            dz = ops.grad_pack_ex(grads[k], scale=sc, add=route, mask=prev, mask_act=_RELU, cpad=prev.shape[-1])
+    g = layers[0][1](dz)                                                 # d loss / d normalised input, 64 channels
+    return ops.grad_unpack_ex(g, 3, vgg.std.view(3), scale=sc)
+
+
+class VGGFeaturesFunction(torch.autograd.Function):
+    """VGGFeatureExtractor.forward under autograd: outputs the features; the gradient flows to the input only."""
+
+    @staticmethod
+    def forward(ctx, vgg, x):
+        feats, outs = vgg_forward(vgg, _f32c(x), keep=True)
+        ctx.vgg, ctx.outs = vgg, outs
+        return tuple(feats)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, *g):
+        gx = vgg_backward(ctx.vgg, ctx.outs, [_f32c(t) for t in g])
+        ctx.outs = None
+        return None, gx

@@ -56,9 +56,14 @@ __global__ void scale_from_amax_kernel(unsigned int* __restrict__ amax_bits, flo
 }
 
 // ------------------------------------------------------------------ gradient packing
-// g = (a [+ b]) * scale : NCHW fp32 [n,c,h,w] -> NHWC fp16 [n,h,w,cpad] (pad channels zero)
+// g = (a [+ b]) * scale : NCHW fp32 [n,c,h,w] -> NHWC fp16 [n,h,w,cpad] (pad channels zero).
+// The VGG path (tg_grad_pack_ex_nhwc_f16) adds, each step only where its operand is given:
+//   v = (v - sub[ch]) / div[ch]  (per channel, before the scale),  v += add (NHWC fp16, every channel),
+//   v *= act'(mask) (NHWC fp16, the stored forward output; act TG_ACT_DRELU / TG_ACT_DLRELU02).
 __global__ void grad_pack_kernel(const float* __restrict__ a, const float* __restrict__ b,
-                                 const float* __restrict__ scale, uint4* __restrict__ y, int n, int c, int hw, int c8) {
+                                 const float* __restrict__ scale, uint4* __restrict__ y, int n, int c, int hw, int c8,
+                                 const float* __restrict__ sub, const float* __restrict__ div,
+                                 const uint4* __restrict__ add, const uint4* __restrict__ mask, int act) {
   tg_pdl_wait();
   tg_pdl_trigger();
   const float s = scale ? __ldg(scale) : 1.f;
@@ -68,6 +73,9 @@ __global__ void grad_pack_kernel(const float* __restrict__ a, const float* __res
     const int cv = (int)(i / ((size_t)n * hw));
     const int nn = (int)(px / hw);
     const size_t sp = px % hw;
+    uint4 av = make_uint4(0u, 0u, 0u, 0u), mv = av;
+    if (add != nullptr) av = __ldg(add + px * c8 + cv);
+    if (mask != nullptr) mv = __ldg(mask + px * c8 + cv);
     __align__(16) __half vals[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
@@ -77,16 +85,21 @@ __global__ void grad_pack_kernel(const float* __restrict__ a, const float* __res
         const size_t off = ((size_t)nn * c + ch) * hw + sp;
         v = __ldg(a + off);
         if (b != nullptr) v += __ldg(b + off);
+        if (div != nullptr) v = (v - __ldg(sub + ch)) / __ldg(div + ch);
       }
-      vals[k] = __float2half(v * s);
+      v *= s;
+      if (add != nullptr) v += __half2float(reinterpret_cast<const __half*>(&av)[k]);
+      if (mask != nullptr) v *= tg_dact(__half2float(reinterpret_cast<const __half*>(&mv)[k]), act);
+      vals[k] = __float2half(v);
     }
     y[px * c8 + cv] = *reinterpret_cast<const uint4*>(vals);
   }
 }
 
-// NHWC fp16 [n,h,w,cpad] channels [c0, c0+c) -> NCHW fp32 [n,c,h,w], times inv_scale (accumulate opt.)
+// NHWC fp16 [n,h,w,cpad] channels [c0, c0+c) -> NCHW fp32 [n,c,h,w], times inv_scale [/ div[ch]] (accumulate opt.)
 __global__ void grad_unpack_kernel(const __half* __restrict__ x, const float* __restrict__ scale,
-                                   float* __restrict__ y, int n, int c, int hw, int cpad, int c0, int accumulate) {
+                                   float* __restrict__ y, int n, int c, int hw, int cpad, int c0, int accumulate,
+                                   const float* __restrict__ div) {
   tg_pdl_wait();
   tg_pdl_trigger();
   const float inv = scale ? __ldg(scale + 1) : 1.f;
@@ -95,7 +108,8 @@ __global__ void grad_unpack_kernel(const __half* __restrict__ x, const float* __
     const size_t sp = i % hw;
     const int ch = (int)((i / hw) % c);
     const int nn = (int)(i / ((size_t)hw * c));
-    const float v = __half2float(x[((size_t)nn * hw + sp) * cpad + c0 + ch]) * inv;
+    float v = __half2float(x[((size_t)nn * hw + sp) * cpad + c0 + ch]) * inv;
+    if (div != nullptr) v /= __ldg(div + ch);
     y[i] = accumulate ? y[i] + v : v;
   }
 }
@@ -528,27 +542,65 @@ int tg_grad_scale_from_amax(const float* a, size_t na, const float* b, size_t nb
   return TG_OK;
 }
 
+int tg_grad_amax_f32(const float* a, size_t na, void* ws, void* stream) {
+  TG_REQUIRE(a && ws && na > 0, TG_E_INVALID, "grad_amax: null pointer / empty tensor");
+  TG_REQUIRE(((uintptr_t)ws & 15) == 0, TG_E_INVALID, "grad_amax: workspace must be 16-byte aligned");
+  tg_launch(amax_kernel, dim3(bgrid(na, 256)), dim3(256), 0, (cudaStream_t)stream, a, na, (const float*)nullptr,
+            (size_t)0, reinterpret_cast<unsigned int*>(ws) + 2);
+  TG_CUDA_LAUNCH_CHECK("grad_amax");
+  return TG_OK;
+}
+
 int tg_grad_pack_nhwc_f16(const float* a, const float* b, const float* scale, void* y, int n, int c, int h, int w,
                           int cpad, void* stream) {
   TG_REQUIRE(a && y, TG_E_INVALID, "grad_pack: null pointer");
   TG_REQUIRE(n > 0 && c > 0 && h > 0 && w > 0 && cpad % 8 == 0 && c <= cpad, TG_E_INVALID, "grad_pack: bad shape");
   const size_t total = (size_t)n * h * w * (cpad / 8);
   tg_launch(grad_pack_kernel, dim3(bgrid(total, 256)), dim3(256), 0, (cudaStream_t)stream, a, b, scale, (uint4*)y, n,
-            c, h * w, cpad / 8);
+            c, h * w, cpad / 8, (const float*)nullptr, (const float*)nullptr, (const uint4*)nullptr,
+            (const uint4*)nullptr, (int)TG_ACT_NONE);
   TG_CUDA_LAUNCH_CHECK("grad_pack");
   return TG_OK;
 }
 
-int tg_grad_unpack_nchw_f32(const void* x, const float* scale, float* y, int n, int c, int h, int w, int cpad,
-                            int c_offset, int accumulate, void* stream) {
+int tg_grad_pack_ex_nhwc_f16(const float* a, const float* sub, const float* div, const float* scale, const void* add,
+                             const void* mask, int act, void* y, int n, int c, int h, int w, int cpad, void* stream) {
+  TG_REQUIRE(a && y, TG_E_INVALID, "grad_pack_ex: null pointer");
+  TG_REQUIRE(n > 0 && c > 0 && h > 0 && w > 0 && cpad % 8 == 0 && c <= cpad, TG_E_INVALID, "grad_pack_ex: bad shape");
+  TG_REQUIRE((sub == nullptr) == (div == nullptr), TG_E_INVALID, "grad_pack_ex: sub and div go together");
+  TG_REQUIRE((mask != nullptr) == (act == TG_ACT_DRELU || act == TG_ACT_DLRELU02) &&
+                 (mask != nullptr || act == TG_ACT_NONE),
+             TG_E_INVALID, "grad_pack_ex: mask goes with act TG_ACT_DRELU / TG_ACT_DLRELU02, no mask with TG_ACT_NONE");
+  TG_REQUIRE(((uintptr_t)y & 15) == 0 && ((uintptr_t)add & 15) == 0 && ((uintptr_t)mask & 15) == 0, TG_E_INVALID,
+             "grad_pack_ex: y, add and mask must be 16-byte aligned");
+  const size_t total = (size_t)n * h * w * (cpad / 8);
+  tg_launch(grad_pack_kernel, dim3(bgrid(total, 256)), dim3(256), 0, (cudaStream_t)stream, a, (const float*)nullptr,
+            scale, (uint4*)y, n, c, h * w, cpad / 8, sub, div, (const uint4*)add, (const uint4*)mask, act);
+  TG_CUDA_LAUNCH_CHECK("grad_pack_ex");
+  return TG_OK;
+}
+
+static int grad_unpack(const void* x, const float* scale, const float* div, float* y, int n, int c, int h, int w,
+                       int cpad, int c_offset, int accumulate, void* stream) {
   TG_REQUIRE(x && y, TG_E_INVALID, "grad_unpack: null pointer");
   TG_REQUIRE(n > 0 && c > 0 && h > 0 && w > 0 && c_offset >= 0 && c_offset + c <= cpad, TG_E_INVALID,
              "grad_unpack: bad shape");
   const size_t total = (size_t)n * c * h * w;
   tg_launch(grad_unpack_kernel, dim3(bgrid(total, 256)), dim3(256), 0, (cudaStream_t)stream, (const __half*)x, scale, y,
-            n, c, h * w, cpad, c_offset, accumulate);
+            n, c, h * w, cpad, c_offset, accumulate, div);
   TG_CUDA_LAUNCH_CHECK("grad_unpack");
   return TG_OK;
+}
+
+int tg_grad_unpack_nchw_f32(const void* x, const float* scale, float* y, int n, int c, int h, int w, int cpad,
+                            int c_offset, int accumulate, void* stream) {
+  return grad_unpack(x, scale, nullptr, y, n, c, h, w, cpad, c_offset, accumulate, stream);
+}
+
+int tg_grad_unpack_ex_nchw_f32(const void* x, const float* scale, const float* div, float* y, int n, int c, int h,
+                               int w, int cpad, int c_offset, int accumulate, void* stream) {
+  TG_REQUIRE(div != nullptr, TG_E_INVALID, "grad_unpack_ex: null divisor");
+  return grad_unpack(x, scale, div, y, n, c, h, w, cpad, c_offset, accumulate, stream);
 }
 
 int tg_bias_grad_nhwc_f16(const void* dz, size_t npix, int c, int c_real, const float* scale, float* db,

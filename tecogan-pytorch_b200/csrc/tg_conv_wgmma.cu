@@ -53,7 +53,7 @@ namespace {
 
 constexpr int kMaxRing = 4;               // smem stages per ring
 constexpr int kBiasBar = 4;               // named barrier of all consumer warpgroups (1 + cw: one consumer's)
-constexpr uint32_t kHeaderBytes = 2048;   // barriers (first 1 KB) + bias (second 1 KB; 2 KB for cout = 384)
+constexpr uint32_t kHeaderBytes = 2048;   // barriers (first 1 KB) + bias (second 1 KB; 2 KB for cout = 384, 512)
 constexpr uint32_t kTapABytes = TH * TW * 128;  // 16 KB
 constexpr uint32_t kPoolTileBytes = kTapABytes / 4;   // the pooled 8x4 px x 64 ch output tile
 // A-operand modes (template parameter MODE)
@@ -886,14 +886,15 @@ int tg_conv_validate(const tg_conv_desc* d, const char* who) {
              TG_E_UNSUPPORTED, "%s: derivative epilogues need NHWC output and a conv3x3 / conv3x3s2 layer", who);
   TG_REQUIRE(!(d->kind == TG_CONV_3X3_S2 && d->epilogue != TG_EPI_NHWC_F16), TG_E_UNSUPPORTED,
              "%s: conv3x3s2 needs the NHWC epilogue", who);
-  TG_REQUIRE(d->cin == 64 || d->cin == 128 || d->cin == 192 || d->cin == 256 || d->cin == 384, TG_E_UNSUPPORTED,
-             "%s: cin=%d (stored channels must be 64, 128, 192, 256 or 384)", who, d->cin);
+  TG_REQUIRE(d->cin == 64 || d->cin == 128 || d->cin == 192 || d->cin == 256 || d->cin == 384 || d->cin == 512,
+             TG_E_UNSUPPORTED, "%s: cin=%d (stored channels must be 64, 128, 192, 256, 384 or 512)", who, d->cin);
   if (d->epilogue == TG_EPI_NHWC_F16_POOL2)
     TG_REQUIRE(d->kind == TG_CONV_3X3 && d->residual == nullptr && d->act <= TG_ACT_LRELU02 && d->h >= 2 && d->w >= 2,
                TG_E_UNSUPPORTED, "%s: the pooled epilogue needs a conv3x3 without residual / derivative epilogue", who);
   if (d->epilogue == TG_EPI_NHWC_F16 || d->epilogue == TG_EPI_NHWC_F16_POOL2) {
-    TG_REQUIRE(d->cout == 64 || d->cout == 128 || d->cout == 192 || d->cout == 256 || d->cout == 384,
-               TG_E_UNSUPPORTED, "%s: cout=%d (64, 128, 192, 256 or 384 for the NHWC epilogue)", who, d->cout);
+    TG_REQUIRE(d->cout == 64 || d->cout == 128 || d->cout == 192 || d->cout == 256 || d->cout == 384 ||
+                   d->cout == 512,
+               TG_E_UNSUPPORTED, "%s: cout=%d (64, 128, 192, 256, 384 or 512 for the NHWC epilogue)", who, d->cout);
     TG_REQUIRE(!(d->residual && d->kind == TG_CONVT_3X3_S2), TG_E_UNSUPPORTED, "%s: residual with convT", who);
     TG_REQUIRE(!(d->kind == TG_CONVT_3X3_S2 && d->cout != 64), TG_E_UNSUPPORTED,
                "%s: convT needs cout == 64 (4 parity accumulators per tile)", who);
@@ -946,7 +947,7 @@ int tg_conv_tcgen05(const tg_conv_desc* d, void* stream) {
   // stream their weights in tap mode.
   const bool splitk = a_mode == TG_AMODE_AUTO && d->kind == TG_CONV_3X3 && !bwd && !tapn &&
                       (p.chunks == 2 || p.chunks == 4) && d->residual == nullptr;
-  // the bias follows the barriers: 1 KB holds 256 output channels, 384 take a second KB
+  // the bias follows the barriers: 1 KB holds 256 output channels, 384 and 512 take a second KB
   const uint32_t header = kHeaderBytes + (d->cout > 256 ? 1024u : 0u);
   const uint32_t b_total = (tapn ? 1u : 9u) * (splitk ? 1u : (uint32_t)p.chunks) * p.b_stage_bytes;   // resident slice per CTA
   const int hbox_w = d->kind != TG_CONVT_3X3_S2 ? TW + 2 : TW + 1;

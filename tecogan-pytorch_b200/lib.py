@@ -159,6 +159,9 @@ _SIGNATURES = {
     'tg_grad_scale_from_amax': (c_int, [_P, c_size_t, _P, c_size_t, c_float, _P, _P]),
     'tg_grad_pack_nhwc_f16': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_grad_unpack_nchw_f32': (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    'tg_grad_amax_f32': (c_int, [_P, c_size_t, _P, _P]),
+    'tg_grad_pack_ex_nhwc_f16': (c_int, [_P, _P, _P, _P, _P, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int, _P]),
+    'tg_grad_unpack_ex_nchw_f32': (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'tg_bias_grad_nhwc_f16': (c_int, [_P, c_size_t, c_int, c_int, _P, _P, _P]),
     'tg_wgrad_tcgen05': (c_int, [ctypes.POINTER(WgradDesc), _P]),
     'tg_wgrad_simt': (c_int, [ctypes.POINTER(WgradDesc), _P]),

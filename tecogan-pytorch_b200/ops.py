@@ -1035,6 +1035,13 @@ class GradScale:
         LAUNCH_COUNT += 1            # two kernels per call
         return self
 
+    def from_amax_of(self, tensors, target=None):
+        """one scale for several fp32 tensors: from the amax over all of them"""
+        for t in tensors[:-1]:
+            _req(t, torch.float32, 'grad')
+            L.check(L.load().tg_grad_amax_f32(_ptr(t), t.numel(), _ptr(self.ws), _stream()), 'tg_grad_amax')
+        return self.from_amax(tensors[-1], target=target)
+
     @property
     def ptr(self):
         return ctypes.c_void_p(self.ws.data_ptr())
@@ -1187,6 +1194,49 @@ def grad_unpack(x, c, scale=None, c_offset=0, y=None, accumulate=False):
         y = torch.empty((n, c, h, w), dtype=torch.float32, device=x.device)
     L.check(L.load().tg_grad_unpack_nchw_f32(_ptr(x), _scale_ptr(scale), _ptr(y), n, c, h, w, cpad, c_offset,
                                              int(accumulate), _stream()), 'tg_grad_unpack')
+    return y
+
+
+def grad_pack_ex(a, sub=None, div=None, scale=None, add=None, mask=None, mask_act=L.ACT_NONE, cpad=64, y=None):
+    """NCHW fp32 a -> NHWC fp16 y (cpad channels): ((a - sub[c]) / div[c] * scale + add) * act'(mask), each step only
+    where its operand is given (tg_grad_pack_ex_nhwc_f16).  mask_act: the activation (RELU / LRELU02) whose stored
+    output is `mask`."""
+    _req(a, torch.float32, 'grad', 4)
+    n, c, h, w = a.shape
+    if (sub is None) != (div is None):
+        raise L.TecoganB200Error('grad_pack_ex: sub and div go together')
+    for t, nm in ((sub, 'sub'), (div, 'div')):
+        if t is not None:
+            _req(t, torch.float32, nm)
+            if t.numel() != c:
+                raise L.TecoganB200Error(f'grad_pack_ex: {nm} must have {c} elements')
+    if y is None:
+        y = torch.empty((n, h, w, cpad), dtype=torch.float16, device=a.device)
+    for t, nm in ((y, 'y'), (add, 'add'), (mask, 'mask')):
+        if t is not None:
+            _req(t, torch.float16, nm, 4)
+            if tuple(t.shape) != (n, h, w, cpad):
+                raise L.TecoganB200Error(f'grad_pack_ex: {nm} shape {tuple(t.shape)} != {(n, h, w, cpad)}')
+    if (mask is not None) != (mask_act in (L.ACT_RELU, L.ACT_LRELU02)):
+        raise L.TecoganB200Error('grad_pack_ex: mask and mask_act (RELU / LRELU02) go together')
+    act = {L.ACT_NONE: L.ACT_NONE, L.ACT_RELU: L.ACT_DRELU, L.ACT_LRELU02: L.ACT_DLRELU02}[mask_act]
+    L.check(L.load().tg_grad_pack_ex_nhwc_f16(_ptr(a), _ptr(sub), _ptr(div), _scale_ptr(scale), _ptr(add), _ptr(mask),
+                                              act, _ptr(y), n, c, h, w, cpad, _stream()), 'tg_grad_pack_ex')
+    return y
+
+
+def grad_unpack_ex(x, c, div, scale=None, y=None):
+    """channels [0, c) of NHWC fp16 -> NCHW fp32 / scale / div[ch] (tg_grad_unpack_ex_nchw_f32)"""
+    _req(x, torch.float16, 'x', 4)
+    _req(div, torch.float32, 'div')
+    if div.numel() != c:
+        raise L.TecoganB200Error(f'grad_unpack_ex: div must have {c} elements')
+    n, h, w, cpad = x.shape
+    if y is None:
+        y = torch.empty((n, c, h, w), dtype=torch.float32, device=x.device)
+    _req(y, torch.float32, 'y', 4)
+    L.check(L.load().tg_grad_unpack_ex_nchw_f32(_ptr(x), _scale_ptr(scale), _ptr(div), _ptr(y), n, c, h, w, cpad, 0, 0,
+                                                _stream()), 'tg_grad_unpack_ex')
     return y
 
 
