@@ -119,6 +119,19 @@ __device__ __forceinline__ void block_sum_min_max(double& s, double& mn, double&
   }
 }
 
+// out[q] = the sum of part[q, 0..nb) in a fixed order, / div: one CTA per row of part.  SSIM's mean divides by the
+// interior's pixel count; the end-point error sums pass div = 1, and x / 1 is x exactly.
+__global__ void __launch_bounds__(kThreads)
+sum_parts_kernel(const double* __restrict__ part, int nb, double div, double* __restrict__ out) {
+  tg_pdl_wait();
+  tg_pdl_trigger();
+  const int q = blockIdx.x;
+  double s = 0.0, mn = 0.0, mx = 0.0;
+  for (int k = threadIdx.x; k < nb; k += kThreads) s = __dadd_rn(s, part[(size_t)q * nb + k]);
+  block_sum_min_max(s, mn, mx);
+  if (threadIdx.x == 0) out[q] = s / div;
+}
+
 // part [t, gridDim.x, 3]: per CTA {sum (Yt - Yp)^2, min Yp, max Yp} over its rows of the window
 __global__ void __launch_bounds__(kThreads)
 official_stats_kernel(const uint8_t* __restrict__ tru, int ht, int wt, const uint8_t* __restrict__ pred, int hp,
@@ -243,18 +256,6 @@ ssim_tile_kernel(const uint8_t* __restrict__ tru, int ht, int wt, const uint8_t*
   double mn = 0.0, mx = 0.0;
   block_sum_min_max(acc, mn, mx);
   if (threadIdx.x == 0) part[((size_t)f * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = acc;
-}
-
-// ssim[f] = sum of part[f, 0..nb) / count: one CTA per frame
-__global__ void __launch_bounds__(kThreads)
-ssim_final_kernel(const double* __restrict__ part, int nb, double count, double* __restrict__ ssim) {
-  tg_pdl_wait();
-  tg_pdl_trigger();
-  const int f = blockIdx.x;
-  double s = 0.0, mn = 0.0, mx = 0.0;
-  for (int k = threadIdx.x; k < nb; k += kThreads) s = __dadd_rn(s, part[(size_t)f * nb + k]);
-  block_sum_min_max(s, mn, mx);
-  if (threadIdx.x == 0) ssim[f] = s / count;
 }
 
 // ---- pyramid level: Gaussian blur at full size + INTER_LINEAR resize, both separable -------------------------------
@@ -532,7 +533,7 @@ flow_iter_kernel(const float* __restrict__ M_in, const float* __restrict__ R, fl
 constexpr int kEpeMaxBlocks = 512;        // CTAs per pair
 
 // The sum over the window (y0, x0, hc, wc) of |a[q] - b[q]| (Euclidean, per pixel), in float64.  With part, CTA k of
-// pair q takes rows k, k + gridDim.x, ... and writes its sum to part[q, k] (epe_final_kernel adds them in a fixed
+// pair q takes rows k, k + gridDim.x, ... and writes its sum to part[q, k] (sum_parts_kernel adds them in a fixed
 // order: the same bits on every run).  Without, the window is the whole frame, read as one grid-strided range, and
 // each CTA adds its sum to sums[q] with a float64 atomic.
 __global__ void __launch_bounds__(kThreads)
@@ -568,18 +569,6 @@ epe_kernel(const float2* __restrict__ a, const float2* __restrict__ b, int h, in
     part[(size_t)q * gridDim.x + blockIdx.x] = acc;
   else
     atomicAdd(sums + q, acc);
-}
-
-// sums[q] = the sum of part[q, 0..nb) in a fixed order: one CTA per pair
-__global__ void __launch_bounds__(kThreads)
-epe_final_kernel(const double* __restrict__ part, int nb, double* __restrict__ sums) {
-  tg_pdl_wait();
-  tg_pdl_trigger();
-  const int q = blockIdx.x;
-  double s = 0.0, mn = 0.0, mx = 0.0;
-  for (int k = threadIdx.x; k < nb; k += kThreads) s = __dadd_rn(s, part[(size_t)q * nb + k]);
-  block_sum_min_max(s, mn, mx);
-  if (threadIdx.x == 0) sums[q] = s;
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------
@@ -887,7 +876,7 @@ int epe_sum(const char* name, const float* a, const float* b, int n, int h, int 
             reinterpret_cast<const float2*>(b), h, w, y0, x0, hc, wc, sums, part);
   TG_CUDA_LAUNCH_CHECK(name);
   if (part) {
-    tg_launch(epe_final_kernel, dim3((unsigned)n), dim3(kThreads), 0, s, (const double*)part, nb, sums);
+    tg_launch(sum_parts_kernel, dim3((unsigned)n), dim3(kThreads), 0, s, (const double*)part, nb, 1.0, sums);
     TG_CUDA_LAUNCH_CHECK(name);
   }
   return TG_OK;
@@ -961,7 +950,7 @@ extern "C" int tg_ssim_y(const uint8_t* true_u8, int ht, int wt, const uint8_t* 
   tg_launch(ssim_tile_kernel, dim3(tiles.x, tiles.y, (unsigned)t), dim3(kThreads), 0, s, true_u8, ht, wt, pred_u8,
             hp, wp, y0, x0, hc, wc, stats, part);
   TG_CUDA_LAUNCH_CHECK(name);
-  tg_launch(ssim_final_kernel, dim3((unsigned)t), dim3(kThreads), 0, s, (const double*)part, (int)(tiles.x * tiles.y),
+  tg_launch(sum_parts_kernel, dim3((unsigned)t), dim3(kThreads), 0, s, (const double*)part, (int)(tiles.x * tiles.y),
             (double)(hc - 2 * kSsimR) * (wc - 2 * kSsimR), ssim);
   TG_CUDA_LAUNCH_CHECK(name);
   return TG_OK;

@@ -96,10 +96,55 @@ def _frames(x, nm):
     return x
 
 
+def _pair_frames(true, pred, names):
+    """(true, pred, T, h, w): both checked by _frames (names: theirs in the messages), their common frame count and
+    their common top-left size"""
+    true, pred = _frames(true, names[0]), _frames(pred, names[1])
+    if pred.shape[0] != true.shape[0]:
+        raise ValueError(f'{names[0]} has {true.shape[0]} frames, {names[1]} {pred.shape[0]}')
+    return true, pred, true.shape[0], min(true.shape[1], pred.shape[1]), min(true.shape[2], pred.shape[2])
+
+
+def _device(true, pred, lpips):
+    """the device of a CUDA input, else the LPIPS weights', else the current CUDA device"""
+    return next((x.device for x in (true, pred) if isinstance(x, torch.Tensor)),
+                lpips.device if lpips is not None else torch.device('cuda', torch.cuda.current_device()))
+
+
+def _chunk_len(total, n_min, chunk_bytes, max_workspace_bytes, need):
+    """the longest chunk, of n_min .. total frames, whose chunk_bytes fit; else ValueError naming need(n_min)"""
+    n = total
+    while n > n_min and chunk_bytes(n) > max_workspace_bytes:
+        n -= 1
+    if chunk_bytes(n) > max_workspace_bytes:
+        raise ValueError(f'max_workspace_bytes={max_workspace_bytes} is below the {need(n)}')
+    return n
+
+
+def _chunks(total, n, overlap):
+    """(s, e, first) of the chunks [s, e) of n frames that cover `total`.  With overlap, each chunk after the first
+    starts at the last frame of the one before, whose per-frame results are kept already: first = 1 skips it."""
+    if n < (2 if overlap else 1) and n < total:
+        raise ValueError(f'chunks of {n} frames (overlap={overlap}) never cover {total} frames')
+    s = 0
+    while True:
+        e = min(s + n, total)
+        yield s, e, int(overlap and s > 0)
+        if e == total:
+            return
+        s = e - 1 if overlap else e
+
+
 def _chunk(x, s, e, device):
     if isinstance(x, np.ndarray):
         return torch.from_numpy(np.ascontiguousarray(x[s:e])).to(device, non_blocking=False)
     return x[s:e].contiguous()
+
+
+def _lpips_batch(tc, pc, window):
+    """the window (y0, x0, h, w) of a chunk's true and pred frames as one uint8 CUDA batch [2m, h, w, 3], true first"""
+    y0, x0, h, w = window
+    return torch.cat([tc[:, y0:y0 + h, x0:x0 + w], pc[:, y0:y0 + h, x0:x0 + w]]).contiguous()
 
 
 # ---- LPIPS (net-lin, AlexNet, v0.1) ----------------------------------------------------------------------------------
@@ -214,33 +259,24 @@ class LPIPS:
         return out
 
     def __call__(self, true, pred, max_workspace_bytes=DEFAULT_MAX_WORKSPACE_BYTES):
-        true, pred = _frames(true, 'true'), _frames(pred, 'pred')
-        N = true.shape[0]
-        if pred.shape[0] != N:
-            raise ValueError(f'true has {N} frames, pred {pred.shape[0]}')
-        h, w = min(true.shape[1], pred.shape[1]), min(true.shape[2], pred.shape[2])
+        true, pred, N, h, w = _pair_frames(true, pred, ('true', 'pred'))
         if h < L.LPIPS_MIN_SIDE or w < L.LPIPS_MIN_SIDE:
             raise ValueError(f'LPIPS needs at least {L.LPIPS_MIN_SIDE}x{L.LPIPS_MIN_SIDE} pixels, got {h}x{w}')
         if N == 0:
             return np.zeros(0)
         full = true.shape[1] * true.shape[2] * 3 + pred.shape[1] * pred.shape[2] * 3
+        window = (0, 0, h, w)
 
         def chunk_bytes(n):      # the uint8 frames as given and cropped, the features, the distances, the heads' work
             return (n * full + 2 * n * h * w * 3 + 2 * n * self.image_bytes(h, w) + n * 8
                     + 5 * ops.lpips_head_workspace_bytes(n, h, w))
-        n = N
-        while n > 1 and chunk_bytes(n) > max_workspace_bytes:
-            n -= 1
-        if chunk_bytes(n) > max_workspace_bytes:
-            raise ValueError(f'max_workspace_bytes={max_workspace_bytes} is below the {chunk_bytes(1)} bytes that one '
-                             f'pair of {h}x{w} frames needs')
+        n = _chunk_len(N, 1, chunk_bytes, max_workspace_bytes,
+                       lambda n: f'{chunk_bytes(1)} bytes that one pair of {h}x{w} frames needs')
         parts = []
         with torch.cuda.device(self.device):
-            for s in range(0, N, n):
-                e = min(s + n, N)
-                batch = _lpips_batch(_chunk(true, s, e, self.device), _chunk(pred, s, e, self.device), h, w)
-                parts.append(self.distances(batch, (0, 0, h, w), L.LPIPS_NORM_CALC,
-                                            [(i, e - s + i) for i in range(e - s)]))
+            for s, e, _ in _chunks(N, n, False):
+                batch = _lpips_batch(_chunk(true, s, e, self.device), _chunk(pred, s, e, self.device), window)
+                parts.append(self.distances(batch, window, L.LPIPS_NORM_CALC, [(i, e - s + i) for i in range(e - s)]))
             return torch.cat(parts).cpu().numpy()
 
 
@@ -250,11 +286,6 @@ def _check_lpips(lpips, true_seq, pred_seq):
     for x in (true_seq, pred_seq):
         if isinstance(x, torch.Tensor) and x.device != lpips.device:
             raise ValueError(f'frames on {x.device}, LPIPS weights on {lpips.device}')
-
-
-def _lpips_batch(tc, pc, h, w):
-    """the chunk's true and pred frames cropped to (h, w), as one uint8 CUDA batch [2m, h, w, 3] (true first)"""
-    return torch.cat([tc[:, :h, :w], pc[:, :h, :w]]).contiguous()
 
 
 def psnr_from_sse(sse, count):
@@ -282,71 +313,52 @@ def sequence_metrics(true_seq, pred_seq, psnr='y', tof=True, max_workspace_bytes
     lpips: an LPIPS (its weights' device must be the frames'), or None for no LPIPS.
 
     Returns {'PSNR': float64 [T]}, {'LPIPS': float64 [T]} and / or {'tOF': float64 [T - 1]} (numpy), in that order."""
-    true_seq, pred_seq = _frames(true_seq, 'true_seq'), _frames(pred_seq, 'pred_seq')
+    true_seq, pred_seq, T, h, w = _pair_frames(true_seq, pred_seq, ('true_seq', 'pred_seq'))
     if psnr not in ('y', 'rgb', None):
         raise ValueError(f"psnr must be 'y', 'rgb' or None, got {psnr!r}")
     if not isinstance(tof, bool):
         raise ValueError(f'tof must be a bool, got {tof!r}')
-    T = true_seq.shape[0]
-    if pred_seq.shape[0] != T:
-        raise ValueError(f'true_seq has {T} frames, pred_seq {pred_seq.shape[0]}')
-    h, w = min(true_seq.shape[1], pred_seq.shape[1]), min(true_seq.shape[2], pred_seq.shape[2])
     if lpips is not None:
         _check_lpips(lpips, true_seq, pred_seq)
         if h < L.LPIPS_MIN_SIDE or w < L.LPIPS_MIN_SIDE:
             raise ValueError(f'LPIPS needs at least {L.LPIPS_MIN_SIDE}x{L.LPIPS_MIN_SIDE} pixels, got {h}x{w}')
-    out = {}
-    if T == 0 or (psnr is None and not tof and lpips is None):
-        if psnr is not None:
-            out['PSNR'] = np.zeros(0)
-        if lpips is not None:
-            out['LPIPS'] = np.zeros(0)
-        if tof:
-            out['tOF'] = np.zeros(0)
-        return out
-    device = next((x.device for x in (true_seq, pred_seq) if isinstance(x, torch.Tensor)),
-                  lpips.device if lpips is not None else torch.device('cuda', torch.cuda.current_device()))
+    keys = [k for k, on in (('PSNR', psnr is not None), ('LPIPS', lpips is not None), ('tOF', tof)) if on]
+    if T == 0 or not keys:
+        return {k: np.zeros(0) for k in keys}
+    device = _device(true_seq, pred_seq, lpips)
     mode = {'y': L.PSNR_Y, 'rgb': L.PSNR_RGB, None: L.PSNR_NONE}[psnr]
     hw = h * w
+    window = (0, 0, h, w)
+
+    def chunk_bytes(n):
+        b = 0
+        if tof:
+            b += ops.farneback_workspace_bytes(2, n, h, w) + 2 * n * hw + 2 * (n - 1) * hw * 8 + 2 * n * hw * 3 * 2
+        if lpips is not None:
+            b += 2 * n * hw * 3 * 2 + 2 * n * LPIPS.image_bytes(h, w) + n * 8
+            b += 5 * ops.lpips_head_workspace_bytes(n, h, w)
+        return b
+    n = T                                      # without flows or LPIPS there is no workspace to bound
     if (tof and T >= 2) or lpips is not None:
-        def chunk_bytes(n):
-            b = 0
-            if tof:
-                b += (ops.farneback_workspace_bytes(2, n, h, w) + 2 * n * hw + 2 * (n - 1) * hw * 8
-                      + 2 * n * hw * 3 * 2)
-            if lpips is not None:
-                b += 2 * n * hw * 3 * 2 + 2 * n * LPIPS.image_bytes(h, w) + n * 8
-                b += 5 * ops.lpips_head_workspace_bytes(n, h, w)
-            return b
-        n, n_min = T, (2 if tof and T >= 2 else 1)
-        while n > n_min and chunk_bytes(n) > max_workspace_bytes:
-            n -= 1
-        if chunk_bytes(n) > max_workspace_bytes:
-            raise ValueError(f'max_workspace_bytes={max_workspace_bytes} is below the {chunk_bytes(n)} bytes that '
-                             f'{n} frames of {h}x{w} need')
-    else:
-        n = T
+        n = _chunk_len(T, 2 if tof and T >= 2 else 1, chunk_bytes, max_workspace_bytes,
+                       lambda n: f'{chunk_bytes(n)} bytes that {n} frames of {h}x{w} need')
+    params = _check_farneback_args(0.5, 3, 15, 3, 5, 1.2, 0) if tof else None
     sse_parts, epe_parts, lp_parts = [], [], []
     with torch.cuda.device(device):
-        s = 0
-        while True:
-            e = min(s + n, T)
+        for s, e, first in _chunks(T, n, tof):
             tc, pc = _chunk(true_seq, s, e, device), _chunk(pred_seq, s, e, device)
             m = e - s
             gray = torch.empty(2, m, h, w, dtype=torch.uint8, device=device) if tof else None
             sse = ops.metrics_frames_in(tc, pc, mode, gray)
             if sse is not None:
-                sse_parts.append(sse if s == 0 or not tof else sse[1:])
+                sse_parts.append(sse[first:])
             if lpips is not None:
-                k0 = 1 if s > 0 and tof else 0
-                lp_parts.append(lpips.distances(_lpips_batch(tc, pc, h, w), (0, 0, h, w), L.LPIPS_NORM_CALC,
-                                                [(i, m + i) for i in range(k0, m)]))
+                lp_parts.append(lpips.distances(_lpips_batch(tc, pc, window), window, L.LPIPS_NORM_CALC,
+                                                [(i, m + i) for i in range(first, m)]))
             if tof and m >= 2:
-                flow = ops.farneback(gray.view(2 * m, h, w), 2, _check_farneback_args(0.5, 3, 15, 3, 5, 1.2, 0))
+                flow = ops.farneback(gray.view(2 * m, h, w), 2, params)
                 epe_parts.append(ops.flow_epe_sum(flow[:m - 1], flow[m - 1:]))
-            if e == T:
-                break
-            s = e - 1 if tof else e
+    out = {}
     if psnr is not None:
         sse = torch.cat(sse_parts).cpu().numpy().view(np.uint64)
         out['PSNR'] = psnr_from_sse(sse, hw * (3 if psnr == 'rgb' else 1))
@@ -394,7 +406,7 @@ def official_sequence_metrics(true_seq, pred_seq, cutfr=2, keys=OFFICIAL_KEYS,
 
     Returns {key: float64 numpy array} in the order of OFFICIAL_LPIPS_KEYS: PSNR, SSIM and LPIPS of T - 2 cutfr
     frames, tOF and tLP100 of T - 2 cutfr - 1 (empty arrays when there are too few frames)."""
-    true_seq, pred_seq = _frames(true_seq, 'true_seq'), _frames(pred_seq, 'pred_seq')
+    true_seq, pred_seq, T, h, w = _pair_frames(true_seq, pred_seq, ('true_seq', 'pred_seq'))
     allowed = OFFICIAL_KEYS if lpips is None else OFFICIAL_LPIPS_KEYS
     if isinstance(keys, str) or not all(isinstance(k, str) and k in allowed for k in keys):
         raise ValueError(f'keys must be a subset of {allowed}' +
@@ -404,10 +416,6 @@ def official_sequence_metrics(true_seq, pred_seq, cutfr=2, keys=OFFICIAL_KEYS,
         _check_lpips(lpips, true_seq, pred_seq)
     if not isinstance(cutfr, (int, np.integer)) or isinstance(cutfr, bool) or cutfr < 0:
         raise ValueError(f'cutfr must be a non-negative integer, got {cutfr!r}')
-    T = true_seq.shape[0]
-    if pred_seq.shape[0] != T:
-        raise ValueError(f'true_seq has {T} frames, pred_seq {pred_seq.shape[0]}')
-    h, w = min(true_seq.shape[1], pred_seq.shape[1]), min(true_seq.shape[2], pred_seq.shape[2])
     if h < OFFICIAL_MIN_SIDE or w < OFFICIAL_MIN_SIDE:
         raise ValueError(f'the common frame size {h}x{w} is below {OFFICIAL_MIN_SIDE}x{OFFICIAL_MIN_SIDE}: its '
                          f'crop_8x8 is empty')
@@ -423,8 +431,7 @@ def official_sequence_metrics(true_seq, pred_seq, cutfr=2, keys=OFFICIAL_KEYS,
     if n_s == 0 or not keys:
         return {k: np.zeros(0) for k in keys}
     true_seq, pred_seq = true_seq[cutfr:T - cutfr], pred_seq[cutfr:T - cutfr]
-    device = next((x.device for x in (true_seq, pred_seq) if isinstance(x, torch.Tensor)),
-                  lpips.device if lpips is not None else torch.device('cuda', torch.cuda.current_device()))
+    device = _device(true_seq, pred_seq, lpips)
     hw = h * w
     frame_bytes = 3 * (true_seq.shape[1] * true_seq.shape[2] + pred_seq.shape[1] * pred_seq.shape[2])
 
@@ -441,27 +448,20 @@ def official_sequence_metrics(true_seq, pred_seq, cutfr=2, keys=OFFICIAL_KEYS,
             b += 2 * n * hc * wc * 3 + 2 * n * LPIPS.image_bytes(hc, wc) + 3 * n * (8 + 8)
             b += 5 * ops.lpips_head_workspace_bytes(3 * n, hc, wc)
         return b
-    n, n_min = n_s, min(n_s, 2 if overlap else 1)     # overlapping chunks need two frames
-    while n > n_min and chunk_bytes(n) > max_workspace_bytes:
-        n -= 1
-    if chunk_bytes(n) > max_workspace_bytes:
-        raise ValueError(f'max_workspace_bytes={max_workspace_bytes} is below the {chunk_bytes(n)} bytes that '
-                         f'{n} frames of {h}x{w} need')
+    n = _chunk_len(n_s, min(n_s, 2 if overlap else 1), chunk_bytes, max_workspace_bytes,  # overlapping chunks: >= 2
+                   lambda n: f'{chunk_bytes(n)} bytes that {n} frames of {h}x{w} need')
     params = _check_farneback_args(0.5, 3, 15, 3, 5, 1.2, 0) if tof else None
     stats_parts, ssim_parts, epe_parts, lp_parts, tlp_parts = [], [], [], [], []
     with torch.cuda.device(device):
-        s = 0
-        while True:
-            e = min(s + n, n_s)
+        # with tOF / tLP100 a chunk's first frame is the last one's last frame, whose PSNR / SSIM / LPIPS are kept
+        for s, e, first in _chunks(n_s, n, overlap):
             tc, pc = _chunk(true_seq, s, e, device), _chunk(pred_seq, s, e, device)
             m = e - s
-            # with tOF / tLP100 a chunk's first frame is the last one's last frame, whose PSNR / SSIM / LPIPS are kept
-            new = slice(1 if s > 0 and overlap else 0, None)
             if stats_wanted:
                 stats = ops.official_frames_stats(tc, pc, window)
-                stats_parts.append(stats[new])
+                stats_parts.append(stats[first:])
                 if 'SSIM' in keys:
-                    ssim_parts.append(ops.ssim_y(tc, pc, window, stats)[new])
+                    ssim_parts.append(ops.ssim_y(tc, pc, window, stats)[first:])
             if tof and m >= 2:
                 gray = torch.empty(2, m, h, w, dtype=torch.uint8, device=device)
                 ops.metrics_frames_in(tc, pc, L.PSNR_NONE, gray)
@@ -470,21 +470,17 @@ def official_sequence_metrics(true_seq, pred_seq, cutfr=2, keys=OFFICIAL_KEYS,
             if lp_wanted:
                 # true frames 0 .. m-1, pred frames m .. 2m-1 of the batch: (true_i, pred_i) for LPIPS, then the
                 # consecutive (true_{i-1}, true_i) and (pred_{i-1}, pred_i) for tLP100; each frame's features once
-                first = new.start
                 pairs = [(i, m + i) for i in range(first, m)] if 'LPIPS' in keys else []
                 if tlp:
                     pairs += [(i - 1, i) for i in range(1, m)] + [(m + i - 1, m + i) for i in range(1, m)]
                 if pairs:
-                    batch = torch.cat([tc[:, y0:y0 + hc, x0:x0 + wc], pc[:, y0:y0 + hc, x0:x0 + wc]]).contiguous()
-                    d = lpips.distances(batch, (0, 0, hc, wc), L.LPIPS_NORM_OFFICIAL, pairs).cpu().numpy()
+                    d = lpips.distances(_lpips_batch(tc, pc, window), (0, 0, hc, wc), L.LPIPS_NORM_OFFICIAL,
+                                        pairs).cpu().numpy()
                     k = m - first if 'LPIPS' in keys else 0
                     if 'LPIPS' in keys:
                         lp_parts.append(d[:k])
                     if tlp:
                         tlp_parts.append((d[k:k + m - 1], d[k + m - 1:]))
-            if e == n_s:
-                break
-            s = e - 1 if overlap else e
     out = {}
     if 'PSNR' in keys:
         sse = torch.cat(stats_parts)[:, 0].cpu().numpy()
