@@ -292,9 +292,28 @@ int tg_rgb_u8_to_yuv420(const uint8_t* rgb, uint8_t* out, int nv12, int n, int H
  * rounded half up: C = (c . (rgb0 + rgb1) + 2^(s-1) + (128 << s)) >> s with the table row's coefficients and
  * s = 21, except for 601 / limited, where it is cv2's COLOR_RGB2YUV_YUY2 / _UYVY bit for bit, luma included:
  * Y = ((4211 R + 8258 G + 1606 B + 8192) >> 14) + 16, U = ((-1212 SR - 2384 SG + 3596 SB + 8192) >> 14) + 128,
- * V = ((3596 SR - 3015 SG - 582 SB + 8192) >> 14) + 128 with SR = R0 + R1 and so on. */
+ * V = ((3596 SR - 3015 SG - 582 SB + 8192) >> 14) + 128 with SR = R0 + R1 and so on.
+ *
+ * 10-bit 4:2:2 (h of any parity, w even; oracle/yuv_422_10.py specifies these three):
+ *          TG_YUV_P210: uint16 frames [n, 2h, w], the h x w Y plane then a full-height interleaved UV plane
+ *            (U0 V0 U1 V1 ... per row, one (U, V) per pixel pair), each sample in the high 10 bits (v << 6), as P010.
+ *          TG_YUV_I422_10: uint16 frames [n, 2h, w], the Y plane then the U and V planes of h x w/2, each sample in
+ *            the low 10 bits, read as min(v, 1023) (ffmpeg yuv422p10le).
+ *          TG_YUV_V210: uint8 frames [n, h, S], S = 128 * ceil(w / 48) bytes a row (SDI capture / playout, ffmpeg
+ *            v210).  Each 16-byte group holds 6 pixels as four little-endian 32-bit words
+ *              Cb0 Y0 Cr0 | Y1 Cb2 Y2 | Cr2 Y3 Cb4 | Y4 Cr4 Y5
+ *            with the 10-bit fields at bits 0, 10 and 20 and bits 30-31 zero.  Row r starts at byte r * S; the
+ *            ceil(w / 6) groups of a row hold its pixels, the fields past pixel w - 1 of a partial last group and
+ *            the row padding up to S are 0 in encoded frames (ignored on decode).  Frames and output 16-byte aligned.
+ *            A v210 window's picture starts on a group (left % 6 == 0) and ends on one unless it reaches the frame's
+ *            right edge; a windowed encode writes its picture's groups only, a whole-frame encode every byte of
+ *            each row.  The frame width is not implied by S: every call passes it (w or frame_w).
+ *          Decode: the 10-bit row per pixel, nearest chroma.  Encode from rgb_f32 (10 bit): Y per pixel as
+ *          I444_10, C = clip((c . (q0 + q1) + 2^18 + (512 << 19)) >> 19) from the pair's sum of 10-bit codes (the
+ *          10-bit row's coefficients, one more fraction bit). */
 enum { TG_YUV_NV12 = 0, TG_YUV_I420 = 1, TG_YUV_P010 = 2, TG_YUV_I420_10 = 3, TG_YUV_YUY2 = 4, TG_YUV_UYVY = 5,
        TG_YUV_I444 = 6, TG_YUV_I444_10 = 8 };
+enum { TG_YUV_P210 = 9, TG_YUV_I422_10 = 10, TG_YUV_V210 = 11 };
 typedef struct tg_yuv_format {
   int32_t layout;       /* TG_YUV_*                   */
   int32_t matrix;       /* 601 or 709                 */
@@ -308,7 +327,8 @@ int tg_stream_frame_in_yuv(const void* in, const tg_yuv_format* fmt, const int32
 /* Encode of the streamed output into any format.  8-bit layouts read rgb_u8 (uint8 NHWC [n,H,W,3], the step's
  * out_u8; rgb_f32 must be NULL), 10-bit layouts read rgb_f32 (fp32 NCHW [n,3,H,W], the step's HR frame, quantised as
  * clip(rint(x * 1023), 0, 1023); rgb_u8 must be NULL).  4:2:0: chroma of each 2x2 block from its top-left pixel;
- * 4:2:2: of each pixel pair's mean (above); 4:4:4: per pixel.  Output [n, 3H/2, W], [n, H, 2W] or [n, 3H, W] words.
+ * 4:2:2: of each pixel pair's mean (above); 4:4:4: per pixel.  Output [n, 3H/2, W], [n, H, 2W] or [n, 3H, W] words;
+ * P210 / I422_10 [n, 2H, W] uint16 and v210 [n, H, 128 * ceil(W / 48)] bytes, all three from rgb_f32.
  * TG_E_INVALID: null pointers, the wrong source for the bit depth, a non-zero reserved, misaligned buffers;
  * TG_E_UNSUPPORTED: odd sizes (H and W for 4:2:0, W for 4:2:2), unknown layout or matrix. */
 int tg_rgb_to_yuv(const uint8_t* rgb_u8, const float* rgb_f32, void* out, const tg_yuv_format* fmt, int n, int H,
@@ -325,7 +345,7 @@ int tg_yuv_coefficients(const tg_yuv_format* fmt, int32_t* out16);
  * is read or written.
  * TG_E_INVALID: a NULL window, a frame of non-positive size, a picture outside the frame;
  * TG_E_UNSUPPORTED: a window off the layout's chroma grid (4:2:0: frame_h, frame_w, top and left even; 4:2:2:
- * frame_w and left even). */
+ * frame_w and left even; v210 in addition left % 6 == 0 and left + w % 6 == 0 or left + w == frame_w). */
 typedef struct tg_frame_window {
   int32_t frame_h, frame_w;   /* the stored frame, in pixels */
   int32_t top, left;          /* the picture's first row and column in it */

@@ -1,6 +1,6 @@
 // The per-pixel decode of streamed frames, shared by the frame-input launches of tg_stream.cu and the resizing frame
 // input of tg_resample.cu: the frame layouts (uint8 HWC; YUV 4:2:0 NV12 / I420 / P010 / I420_10, packed 4:2:2 YUY2 /
-// UYVY, planar 4:4:4 I444 / I444_10), the fixed-point colour table, the row decoders of the frame-input CTAs and the
+// UYVY, planar 4:4:4 I444 / I444_10, 10-bit 4:2:2 P210 / I422_10 / v210), the fixed-point colour table, the row decoders of the frame-input CTAs and the
 // per-pixel sample fetch of any layout, the picture-window check and the format dispatch.  Every decoder computes the
 // same fp32 value of a pixel: float(code) / 255 (8 bit) or / 1023 (10 bit) by IEEE division.
 // Contract: include/tecogan_b200.h (tg_yuv_format, tg_frame_window, tg_stream_frame_in*).
@@ -16,12 +16,16 @@ constexpr int kTilePx = 256;            // decode / encode CTA: kTilePx pixels o
 constexpr int kMaxC = 4;
 
 enum FrameFormat { kHWC = 0, kNV12 = 1, kI420 = 2, kP010 = 3, kI420_10 = 4, kYUY2 = 5, kUYVY = 6, kI444 = 7,
-                   kI444_10 = 8 };
+                   kI444_10 = 8, kP210 = 9, kI422_10 = 10, kV210 = 11 };
 
-constexpr bool fmt_10(int f) { return f == kP010 || f == kI420_10 || f == kI444_10; }
+constexpr bool fmt_10(int f) {
+  return f == kP010 || f == kI420_10 || f == kI444_10 || f == kP210 || f == kI422_10 || f == kV210;
+}
 constexpr bool fmt_packed(int f) { return f == kYUY2 || f == kUYVY; }     // 4:2:2, one 4-byte group per pair
 constexpr bool fmt_444(int f) { return f == kI444 || f == kI444_10; }     // three full-size planes
-constexpr bool fmt_420(int f) { return f != kHWC && !fmt_packed(f) && !fmt_444(f); }
+constexpr bool fmt_p422(int f) { return f == kP210 || f == kI422_10; }    // 10-bit 4:2:2, [2h, w] uint16 words
+constexpr bool fmt_422(int f) { return fmt_packed(f) || fmt_p422(f) || f == kV210; }   // needs an even width
+constexpr bool fmt_420(int f) { return f != kHWC && !fmt_422(f) && !fmt_444(f); }
 // byte of Y0 (Y1 two bytes later) and of U (V two bytes later) in a packed group: YUY2 is Y0 U Y1 V, UYVY U Y0 V Y1
 constexpr int packed_y0(int f) { return f == kUYVY ? 1 : 0; }
 constexpr int packed_u(int f) { return f == kUYVY ? 0 : 1; }
@@ -30,16 +34,19 @@ template <int kFmt>
 struct Yuv {
   static constexpr bool kInterleaved = kFmt == kNV12 || kFmt == kP010;     // NV12 plane layout
   static constexpr bool k10 = fmt_10(kFmt);
-  using Word = typename std::conditional<k10, uint16_t, uint8_t>::type;
+  // v210 packs its 10-bit samples into the 32-bit words of 16-byte groups: its frames are addressed in bytes
+  using Word = typename std::conditional<k10 && kFmt != kV210, uint16_t, uint8_t>::type;
   static constexpr int kShift = k10 ? 18 : 20;                              // fraction bits of the table row
   static constexpr int kTop = k10 ? 1023 : 255;
   static constexpr int kCoff = k10 ? 512 : 128;
-  // the sample of a stored word: P010 keeps it in the high 10 bits, I420_10 / I444_10 in the low 10 (larger
-  // words clamp)
+  static constexpr bool kHigh = kFmt == kP010 || kFmt == kP210;           // sample in the high 10 bits
+  // the sample of a stored word: P010 / P210 keep it in the high 10 bits, I420_10 / I444_10 / I422_10 in the low 10
+  // (larger words clamp)
   static __device__ __forceinline__ int sample(Word v) {
-    return kFmt == kP010 ? (int)(v >> 6) : (kFmt == kI420_10 || kFmt == kI444_10) ? min((int)v, 1023) : (int)v;
+    return kHigh ? (int)(v >> 6) : (kFmt == kI420_10 || kFmt == kI444_10 || kFmt == kI422_10) ? min((int)v, 1023)
+                                                                                             : (int)v;
   }
-  static __device__ __forceinline__ Word word(int v) { return (Word)(kFmt == kP010 ? v << 6 : v); }
+  static __device__ __forceinline__ Word word(int v) { return (Word)(kHigh ? v << 6 : v); }
 };
 
 // The colour table (oracle/yuv_color.py derives the same numbers): [depth 8 / 10][colour][16] with colour
@@ -100,6 +107,16 @@ static_assert(Yuv<kYUY2>::kTop == 255 && Yuv<kUYVY>::kCoff == 128 && Yuv<kI444>:
               "4:2:2 is 8 bit only, I444_10 is the 10-bit table row");
 static_assert(!Yuv<kYUY2>::kInterleaved && !Yuv<kUYVY>::kInterleaved && !Yuv<kI444>::kInterleaved &&
                   !Yuv<kI444_10>::kInterleaved, "4:2:2 and 4:4:4 frames have no NV12 chroma plane");
+static_assert(Yuv<kP210>::kShift == 18 && Yuv<kI422_10>::kTop == 1023 && Yuv<kV210>::kCoff == 512 &&
+                  sizeof(Yuv<kP210>::Word) == 2 && sizeof(Yuv<kV210>::Word) == 1 && !Yuv<kP210>::kInterleaved,
+              "10-bit 4:2:2 is the 10-bit table row; v210 frames are bytes");
+
+// v210: a row of a frame_w-pixel frame is 128 * ceil(frame_w / 48) bytes, ceil(frame_w / 6) 16-byte groups of 6
+// pixels used.  The 12 fields of a group, f = 3 * word + k at bits 10k of word f / 3, are
+//   Cb0 Y0 Cr0 Y1 Cb2 Y2 Cr2 Y3 Cb4 Y4 Cr4 Y5:
+// Y of pixel j at field 2j + 1, Cb / Cr of pair p (pixels 2p, 2p + 1) at fields 4p / 4p + 2.
+__host__ __device__ constexpr size_t v210_stride(int fw) { return (size_t)128 * ((fw + 47) / 48); }
+__device__ __forceinline__ int v210_field(const uint32_t* g, int f) { return (int)((g[f / 3] >> (10 * (f % 3))) & 1023u); }
 
 // zero floats [0, count) of p (4-byte aligned): 16-byte stores over the aligned interior, at most three
 // scalar stores at each end.  `worker` of `workers` threads; writes nothing outside the range.
@@ -275,6 +292,26 @@ __device__ __forceinline__ void yuv_samples(const uint8_t* __restrict__ in, tg_f
     Y = byte(packed_y0(kFmt) + 2 * (x & 1));
     U = byte(packed_u(kFmt));
     V = byte(packed_u(kFmt) + 2);
+  } else if constexpr (kFmt == kV210) {
+    const uint32_t* g = reinterpret_cast<const uint32_t*>(in + ((size_t)img * fh + y) * v210_stride(fw)) + 4 * (x / 6);
+    const int j = x % 6, p = j >> 1;
+    const auto field = [g](int f) { return (int)((__ldg(g + f / 3) >> (10 * (f % 3))) & 1023u); };
+    Y = field(2 * j + 1);
+    U = field(4 * p);
+    V = field(4 * p + 2);
+  } else if constexpr (fmt_p422(kFmt)) {
+    const size_t fplane = (size_t)fh * fw;
+    const W* frame = reinterpret_cast<const W*>(in) + (size_t)img * 2 * fplane;
+    Y = F::sample(__ldg(frame + (size_t)y * fw + x));
+    if (kFmt == kP210) {
+      const W* c = frame + fplane + (size_t)y * fw + (x & ~1);
+      U = F::sample(__ldg(c));
+      V = F::sample(__ldg(c + 1));
+    } else {
+      const W* c = frame + fplane + (size_t)y * (fw >> 1) + (x >> 1);
+      U = F::sample(__ldg(c));
+      V = F::sample(__ldg(c + fplane / 2));
+    }
   } else if constexpr (fmt_444(kFmt)) {
     const size_t fplane = (size_t)fh * fw;
     const W* src = reinterpret_cast<const W*>(in) + (size_t)img * 3 * fplane + (size_t)y * fw + x;
@@ -356,8 +393,66 @@ __device__ __forceinline__ void decode_yuv444(const uint8_t* __restrict__ in, fl
   d.put(lr_curr + (size_t)img * 3 * plane + (size_t)y * w + x, plane, F::sample(__ldg(src)));
 }
 
+// decode CTA of planar 10-bit 4:2:2 frames ([2h, w] uint16 words each: the Y plane, then P210's interleaved UV plane
+// of h x w or I422_10's U and V planes of h x w/2): kTilePx pixel pairs of one row, one pair per thread; both
+// pixels take the pair's U and V (nearest chroma)
+template <int kFmt>
+__device__ __forceinline__ void decode_yuv422_10(const uint8_t* __restrict__ in, float* __restrict__ lr_curr, int b,
+                                                 int t, int h, int w, tg_frame_window win, int x_tiles, int color) {
+  using F = Yuv<kFmt>;
+  using W = typename F::Word;
+  const int xt = b % x_tiles, r = b / x_tiles;
+  const int y = r % h, img = r / h;
+  const int pair = xt * kTilePx + t;
+  if (pair >= (w >> 1)) return;
+  const int fw = win.frame_w, fy = win.top + y, fx = win.left + 2 * pair;   // frame_w and left are even
+  const size_t fplane = (size_t)win.frame_h * fw;
+  const W* frame = reinterpret_cast<const W*>(in) + (size_t)img * 2 * fplane;
+  const W* ys = frame + (size_t)fy * fw + fx;
+  int u, v;
+  if (kFmt == kP210) {
+    const W* c = frame + fplane + (size_t)fy * fw + fx;
+    u = F::sample(__ldg(c));
+    v = F::sample(__ldg(c + 1));
+  } else {
+    const W* c = frame + fplane + (size_t)fy * (fw >> 1) + (fx >> 1);
+    u = F::sample(__ldg(c));
+    v = F::sample(__ldg(c + fplane / 2));
+  }
+  const YuvDecode<kFmt> d(u, v, color);
+  const size_t plane = (size_t)h * w;
+  float* dst = lr_curr + (size_t)img * 3 * plane + (size_t)y * w + 2 * pair;
+  d.put(dst, plane, F::sample(__ldg(ys)));
+  d.put(dst + 1, plane, F::sample(__ldg(ys + 1)));
+}
+
+// decode CTA of v210 frames ([h, v210_stride(frame_w)] bytes each): kTilePx 16-byte groups of one row, one group
+// (6 pixels, 3 pairs) per thread with one 16-byte load; the pixels past w of a partial last group are not written.
+// The frames are 16-byte aligned and the picture starts on a group (the launch checks).
+__device__ __forceinline__ void decode_v210(const uint8_t* __restrict__ in, float* __restrict__ lr_curr, int b, int t,
+                                            int h, int w, tg_frame_window win, int x_tiles, int color) {
+  const int xt = b % x_tiles, r = b / x_tiles;
+  const int y = r % h, img = r / h;
+  const int grp = xt * kTilePx + t;
+  const int x0 = 6 * grp;
+  if (x0 >= w) return;
+  const size_t frow = (size_t)img * win.frame_h + win.top + y;
+  const uint4 q = __ldg(reinterpret_cast<const uint4*>(in + frow * v210_stride(win.frame_w)) + win.left / 6 + grp);
+  const uint32_t g[4] = {q.x, q.y, q.z, q.w};
+  const size_t plane = (size_t)h * w;
+  float* dst = lr_curr + (size_t)img * 3 * plane + (size_t)y * w + x0;
+#pragma unroll
+  for (int p = 0; p < 3; ++p) {
+    if (x0 + 2 * p >= w) break;                      // w is even: a pair is whole or absent
+    const YuvDecode<kV210> d(v210_field(g, 4 * p), v210_field(g, 4 * p + 2), color);
+    d.put(dst + 2 * p, plane, v210_field(g, 4 * p + 1));
+    d.put(dst + 2 * p + 1, plane, v210_field(g, 4 * p + 3));
+  }
+}
+
 // A window of an h x w picture in frames of layout kFmt: TG_E_INVALID outside the frame, TG_E_UNSUPPORTED off the
-// chroma grid (4:2:0: even frame size, top and left; 4:2:2: even frame width and left)
+// chroma grid (4:2:0: even frame size, top and left; 4:2:2: even frame width and left; v210: the picture starts on
+// a 6-pixel group and ends on one or at the frame's right edge)
 template <int kFmt>
 int check_window(const char* name, const tg_frame_window* win, int h, int w) {
   TG_REQUIRE(win, TG_E_INVALID, "%s: null window", name);
@@ -367,8 +462,11 @@ int check_window(const char* name, const tg_frame_window* win, int h, int w) {
   TG_REQUIRE(!fmt_420(kFmt) || ((fh | fw | top | left) & 1) == 0, TG_E_UNSUPPORTED,
              "%s: YUV 4:2:0 needs an even frame size, top and left, got %lldx%lld at (%lld, %lld)", name, fh, fw, top,
              left);
-  TG_REQUIRE(!fmt_packed(kFmt) || ((fw | left) & 1) == 0, TG_E_UNSUPPORTED,
+  TG_REQUIRE(!fmt_422(kFmt) || ((fw | left) & 1) == 0, TG_E_UNSUPPORTED,
              "%s: YUV 4:2:2 needs an even frame width and left, got width %lld at column %lld", name, fw, left);
+  TG_REQUIRE(kFmt != kV210 || (left % 6 == 0 && ((left + w) % 6 == 0 || left + w == fw)), TG_E_UNSUPPORTED,
+             "%s: a v210 picture of width %d at column %lld of a %lld-wide frame must start on a 6-pixel group and "
+             "end on one or at the frame's right edge", name, w, left, fw);
   return TG_OK;
 }
 
@@ -384,6 +482,9 @@ int dispatch_format(int f, Fn&& fn) {
     case kYUY2: return fn(std::integral_constant<int, kYUY2>());
     case kUYVY: return fn(std::integral_constant<int, kUYVY>());
     case kI444: return fn(std::integral_constant<int, kI444>());
+    case kP210: return fn(std::integral_constant<int, kP210>());
+    case kI422_10: return fn(std::integral_constant<int, kI422_10>());
+    case kV210: return fn(std::integral_constant<int, kV210>());
     default: return fn(std::integral_constant<int, kI444_10>());
   }
 }
@@ -404,6 +505,9 @@ int parse_yuv_format(const char* name, const tg_yuv_format* f, int* fmt, int* co
     case TG_YUV_UYVY: *fmt = kUYVY; break;
     case TG_YUV_I444: *fmt = kI444; break;
     case TG_YUV_I444_10: *fmt = kI444_10; break;
+    case TG_YUV_P210: *fmt = kP210; break;
+    case TG_YUV_I422_10: *fmt = kI422_10; break;
+    case TG_YUV_V210: *fmt = kV210; break;
     default: TG_REQUIRE(false, TG_E_UNSUPPORTED, "%s: unknown layout %d", name, f->layout);
   }
   *color = (f->matrix == 709 ? 1 : 0) + 2 * f->full_range;

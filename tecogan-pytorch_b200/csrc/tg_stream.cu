@@ -1,5 +1,5 @@
 // Frame I/O of one streamed inference step: uint8 HWC or YUV (4:2:0: NV12 / I420, 8 bit; P010 / I420_10, 10 bit;
-// packed 4:2:2: YUY2 / UYVY, 8 bit; planar 4:4:4: I444, 8 bit, I444_10) frames decoded on the device into the
+// packed 4:2:2: YUY2 / UYVY, 8 bit; planar 4:4:4: I444, 8 bit, I444_10; 10-bit 4:2:2: P210, I422_10, v210) frames decoded on the device into the
 // step's fp32 NCHW lr_curr, the per-slot reset of the recurrent state, and the encode of the step's RGB output
 // (uint8 NHWC, or the fp32 NCHW HR frame for 10-bit output) into any of those YUV layouts; each of them reads or
 // writes a picture window of larger stored frames (tg_frame_window).  Also the fill of padded frames with a format's
@@ -72,6 +72,10 @@ stream_frame_in_kernel(const uint8_t* __restrict__ in, const int32_t* __restrict
       decode_yuv422<kFmt>(in, lr_curr, b, t, h, w, win, x_tiles, color);
     else if constexpr (fmt_444(kFmt))
       decode_yuv444<kFmt>(in, lr_curr, b, t, h, w, win, x_tiles, color);
+    else if constexpr (fmt_p422(kFmt))
+      decode_yuv422_10<kFmt>(in, lr_curr, b, t, h, w, win, x_tiles, color);
+    else if constexpr (kFmt == kV210)
+      decode_v210(in, lr_curr, b, t, h, w, win, x_tiles, color);
     else
       decode_yuv420<kFmt>(in, lr_curr, b, t, h, w, win, x_tiles, color);
     return;
@@ -97,7 +101,7 @@ int launch_frame_in(const char* name, const void* in, const int32_t* reset, floa
   constexpr bool k420 = fmt_420(kFmt);
   TG_REQUIRE(!k420 || (h % 2 == 0 && w % 2 == 0), TG_E_UNSUPPORTED,
              "%s: YUV 4:2:0 needs an even height and width, got %dx%d", name, h, w);
-  TG_REQUIRE(!fmt_packed(kFmt) || w % 2 == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name,
+  TG_REQUIRE(!fmt_422(kFmt) || w % 2 == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name,
              w);
   TG_REQUIRE(s == 2 || s == 4, TG_E_UNSUPPORTED, "%s: scale %d (2 or 4)", name, s);
   TG_REQUIRE((((uintptr_t)lr_curr | (uintptr_t)lr_prev | (uintptr_t)hr_prev) & 3u) == 0, TG_E_INVALID,
@@ -106,13 +110,16 @@ int launch_frame_in(const char* name, const void* in, const int32_t* reset, floa
              "%s: 10-bit frames must be 2-byte aligned", name);
   TG_REQUIRE(!fmt_packed(kFmt) || ((uintptr_t)in & 3u) == 0, TG_E_INVALID,
              "%s: packed 4:2:2 frames must be 4-byte aligned", name);
+  TG_REQUIRE(kFmt != kV210 || ((uintptr_t)in & 15u) == 0, TG_E_INVALID, "%s: v210 frames must be 16-byte aligned",
+             name);
   const tg_frame_window whole = {h, w, 0, 0};
   if (!win) win = &whole;
   if (in) {
     const int rc = check_window<kFmt>(name, win, h, w);
     if (rc != TG_OK) return rc;
   }
-  const int x_tiles = tg_ceil_div(fmt_packed(kFmt) ? w / 2 : w, kTilePx);
+  // threads per row: a pixel, a pair (4:2:2) or a 6-pixel group (v210)
+  const int x_tiles = tg_ceil_div(kFmt == kV210 ? tg_ceil_div(w, 6) : fmt_422(kFmt) ? w / 2 : w, kTilePx);
   const size_t decode = in ? (size_t)x_tiles * (k420 ? h / 2 : h) * n : 0;
   const size_t hr4 = (size_t)c * s * h * s * w / 4;
   const int zpc = reset ? (int)(hr4 / (kThreads * 8) + 1 < 64 ? hr4 / (kThreads * 8) + 1 : 64) : 0;
@@ -304,25 +311,124 @@ rgb_to_yuv444_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, in
   dst[2 * fplane] = q(k[6] * R + k[7] * G + k[8] * B + kHalf + coff);
 }
 
+// 10-bit 4:2:2 encode of one pixel pair from the fp32 NCHW HR frame: q = clip(rint(x * 1023), 0, 1023) per channel;
+// Y of each pixel with the 10-bit table row (as the I444_10 encode), U and V from the pair's sums q0 + q1 with one
+// more fraction bit (19), rounded half up -- the 8-bit derived rows' 4:2:2 rule at 10 bits
+struct Pair10 {
+  int y0, y1, u, v;
+};
+
+__device__ __forceinline__ Pair10 encode_pair10(const float* p, size_t plane, int color) {
+  auto q10 = [](float x) { return (int)fminf(fmaxf(rintf(x * 1023.f), 0.f), 1023.f); };
+  const int R0 = q10(__ldg(p)), G0 = q10(__ldg(p + plane)), B0 = q10(__ldg(p + 2 * plane));
+  const int R1 = q10(__ldg(p + 1)), G1 = q10(__ldg(p + plane + 1)), B1 = q10(__ldg(p + 2 * plane + 1));
+  const int* k = c_yuv.v[1][color];
+  constexpr int sy = 18, sc = 19;
+  const int yo = (k[15] << sy) + (1 << (sy - 1));
+  constexpr int co = (512 << sc) + (1 << (sc - 1));
+  auto q = [](int a, int s) { return min(max(a >> s, 0), 1023); };
+  const int sr = R0 + R1, sg = G0 + G1, sb = B0 + B1;
+  return {q(k[0] * R0 + k[1] * G0 + k[2] * B0 + yo, sy), q(k[0] * R1 + k[1] * G1 + k[2] * B1 + yo, sy),
+          q(k[3] * sr + k[4] * sg + k[5] * sb + co, sc), q(k[6] * sr + k[7] * sg + k[8] * sb + co, sc)};
+}
+
+// one CTA: kTilePx pixel pairs of one row of the fp32 NCHW HR frame -> their words in a P210 / I422_10 frame
+// ([2h, w] uint16: Y plane, then the interleaved UV plane or the U and V planes of h x w/2)
+template <int kFmt>
+__global__ void __launch_bounds__(kThreads)
+rgb_to_yuv422_10_kernel(const float* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, tg_frame_window win,
+                        int x_tiles, int color) {
+  using F = Yuv<kFmt>;
+  using Wd = typename F::Word;
+  static_assert(fmt_p422(kFmt), "P210 / I422_10");
+  tg_pdl_wait();
+  tg_pdl_trigger();
+  const int t = threadIdx.x;
+  const int xt = blockIdx.x % x_tiles, r = blockIdx.x / x_tiles;
+  const int y = r % H, img = r / H;
+  const int pair = xt * kTilePx + t;
+  if (pair >= (W >> 1)) return;
+  const size_t plane = (size_t)H * W;
+  const Pair10 e = encode_pair10(rgb + (size_t)img * 3 * plane + (size_t)y * W + 2 * pair, plane, color);
+  const int fw = win.frame_w, fy = win.top + y, fx = win.left + 2 * pair;   // frame_w and left are even
+  const size_t fplane = (size_t)win.frame_h * fw;
+  Wd* frame = reinterpret_cast<Wd*>(out) + (size_t)img * 2 * fplane;
+  Wd* ys = frame + (size_t)fy * fw + fx;
+  ys[0] = F::word(e.y0);
+  ys[1] = F::word(e.y1);
+  if (kFmt == kP210) {
+    Wd* c = frame + fplane + (size_t)fy * fw + fx;
+    c[0] = F::word(e.u);
+    c[1] = F::word(e.v);
+  } else {
+    Wd* c = frame + fplane + (size_t)fy * (fw >> 1) + (fx >> 1);
+    c[0] = F::word(e.u);
+    c[fplane / 2] = F::word(e.v);
+  }
+}
+
+// one CTA: kTilePx 16-byte v210 groups of one row of the fp32 NCHW HR frame, one group (6 pixels) per thread packed
+// into one 16-byte store; the fields past pixel W - 1 of a partial last group are 0.  Groups [0, groups) of the
+// picture are written; a whole-frame encode (groups = the row's S / 16) also writes the row padding as 0.
+__global__ void __launch_bounds__(kThreads)
+rgb_to_v210_kernel(const float* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, tg_frame_window win,
+                   int x_tiles, int groups, int color) {
+  tg_pdl_wait();
+  tg_pdl_trigger();
+  const int t = threadIdx.x;
+  const int xt = blockIdx.x % x_tiles, r = blockIdx.x / x_tiles;
+  const int y = r % H, img = r / H;
+  const int grp = xt * kTilePx + t;
+  if (grp >= groups) return;
+  const int x0 = 6 * grp;
+  uint32_t g[4] = {0u, 0u, 0u, 0u};
+  const size_t plane = (size_t)H * W;
+  const float* src = rgb + (size_t)img * 3 * plane + (size_t)y * W + x0;
+  auto put = [&g](int f, int v) { g[f / 3] |= (uint32_t)v << (10 * (f % 3)); };
+#pragma unroll
+  for (int p = 0; p < 3; ++p) {
+    if (x0 + 2 * p >= W) break;                      // W is even: a pair is whole or absent
+    const Pair10 e = encode_pair10(src + 2 * p, plane, color);
+    put(4 * p, e.u);
+    put(4 * p + 1, e.y0);
+    put(4 * p + 2, e.v);
+    put(4 * p + 3, e.y1);
+  }
+  const size_t frow = (size_t)img * win.frame_h + win.top + y;
+  reinterpret_cast<uint4*>(out + frow * v210_stride(win.frame_w))[win.left / 6 + grp] =
+      make_uint4(g[0], g[1], g[2], g[3]);
+}
+
 template <int kFmt>
 int launch_to_yuv(const char* name, const void* rgb, void* out, int n, int H, int W, const tg_frame_window* win,
                   int color, cudaStream_t stream) {
   using F = Yuv<kFmt>;
   TG_REQUIRE(n > 0 && H > 0 && W > 0, TG_E_INVALID, "%s: bad size n=%d H=%d W=%d", name, n, H, W);
-  TG_REQUIRE(fmt_packed(kFmt) || fmt_444(kFmt) || (H % 2 == 0 && W % 2 == 0), TG_E_UNSUPPORTED,
+  TG_REQUIRE(!fmt_420(kFmt) || (H % 2 == 0 && W % 2 == 0), TG_E_UNSUPPORTED,
              "%s: YUV 4:2:0 needs an even height and width, got %dx%d", name, H, W);
-  TG_REQUIRE(!fmt_packed(kFmt) || W % 2 == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name, W);
+  TG_REQUIRE(!fmt_422(kFmt) || W % 2 == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name, W);
   TG_REQUIRE(!fmt_packed(kFmt) || ((uintptr_t)out & 3u) == 0, TG_E_INVALID,
              "%s: packed 4:2:2 output must be 4-byte aligned", name);
+  TG_REQUIRE(kFmt != kV210 || ((uintptr_t)out & 15u) == 0, TG_E_INVALID, "%s: v210 output must be 16-byte aligned",
+             name);
+  const bool whole_frame = win == nullptr;
   const tg_frame_window whole = {H, W, 0, 0};
   if (!win) win = &whole;
   const int rc = check_window<kFmt>(name, win, H, W);
   if (rc != TG_OK) return rc;
-  const int x_tiles = tg_ceil_div(fmt_packed(kFmt) ? W / 2 : W, kTilePx);
-  const size_t ctas = (size_t)x_tiles * (fmt_packed(kFmt) || fmt_444(kFmt) ? H : H / 2) * n;
+  // v210: the picture's groups, or every group of the row up to its stride for a whole-frame encode
+  const int groups = kFmt != kV210 ? 0 : whole_frame ? (int)(v210_stride(W) / 16) : tg_ceil_div(W, 6);
+  const int x_tiles = tg_ceil_div(kFmt == kV210 ? groups : fmt_422(kFmt) ? W / 2 : W, kTilePx);
+  const size_t ctas = (size_t)x_tiles * (fmt_420(kFmt) ? H / 2 : H) * n;
   TG_REQUIRE(ctas <= 0x7fffffff, TG_E_UNSUPPORTED, "%s: grid too large", name);
   uint8_t* o = static_cast<uint8_t*>(out);
-  if constexpr (fmt_packed(kFmt))
+  if constexpr (kFmt == kV210)
+    tg_launch(rgb_to_v210_kernel, dim3((unsigned)ctas), dim3(kThreads), 0, stream, static_cast<const float*>(rgb), o,
+              H, W, *win, x_tiles, groups, color);
+  else if constexpr (fmt_p422(kFmt))
+    tg_launch(rgb_to_yuv422_10_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), 0, stream,
+              static_cast<const float*>(rgb), o, H, W, *win, x_tiles, color);
+  else if constexpr (fmt_packed(kFmt))
     tg_launch(rgb_to_yuv422_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), 0, stream,
               static_cast<const uint8_t*>(rgb), o, H, W, *win, x_tiles, color);
   else if constexpr (fmt_444(kFmt))
@@ -339,25 +445,43 @@ int launch_to_yuv(const char* name, const void* rgb, void* out, int n, int H, in
 template <int kFmt>
 size_t frame_words(int c, int fh, int fw) {
   const size_t px = (size_t)fh * fw;
-  return kFmt == kHWC ? px * c : fmt_packed(kFmt) ? 2 * px : fmt_444(kFmt) ? 3 * px : 3 * (px / 2);
+  if (kFmt == kV210) return (size_t)fh * v210_stride(fw);    // bytes
+  return kFmt == kHWC ? px * c : fmt_packed(kFmt) || fmt_p422(kFmt) ? 2 * px : fmt_444(kFmt) ? 3 * px : 3 * (px / 2);
 }
 
 // total words of n frames := the layout's black (Y: the colour's luma offset, U = V: kCoff; HWC: 0).  Grid-stride;
-// runs once per stream, when the padded output frames are allocated.
+// runs once per stream, when the padded output frames are allocated.  v210 (frame_w fw): the fields of each row's
+// ceil(fw / 6) groups that hold a pixel, 0 in the rest of a partial last group and in the row padding.
 template <int kFmt>
 __global__ void __launch_bounds__(kThreads)
-fill_black_kernel(uint8_t* __restrict__ out, size_t frame, size_t luma, size_t total, int color) {
+fill_black_kernel(uint8_t* __restrict__ out, size_t frame, size_t luma, size_t total, int color, int fw) {
   using F = Yuv<kFmt>;
   using Wd = typename F::Word;
   tg_pdl_wait();
   tg_pdl_trigger();
   Wd* o = reinterpret_cast<Wd*>(out);
   const int y = kFmt == kHWC ? 0 : c_yuv.v[F::k10][color][15];
-  for (size_t i = blockIdx.x * (size_t)kThreads + threadIdx.x; i < total; i += (size_t)gridDim.x * kThreads) {
-    const size_t j = i % frame;
-    // packed 4:2:2: Y is every other byte, starting at packed_y0; planar: the first fh * fw words
-    const bool is_y = fmt_packed(kFmt) ? (int)(j & 1) == packed_y0(kFmt) : j < luma;
-    o[i] = kFmt == kHWC ? (Wd)0 : F::word(is_y ? y : F::kCoff);
+  if constexpr (kFmt == kV210) {
+    const size_t row_words = v210_stride(fw) / 4;
+    uint32_t* o32 = reinterpret_cast<uint32_t*>(out);
+    for (size_t i = blockIdx.x * (size_t)kThreads + threadIdx.x; i < total / 4; i += (size_t)gridDim.x * kThreads) {
+      const int wi = (int)(i % row_words), x0 = 6 * (wi >> 2);
+      uint32_t word = 0;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const int f = 3 * (wi & 3) + k;              // Y of pixel (f - 1) / 2 when f is odd, else chroma of pair f / 4
+        const int x = x0 + ((f & 1) ? (f - 1) / 2 : 2 * (f / 4));
+        if (x < fw) word |= (uint32_t)((f & 1) ? y : F::kCoff) << (10 * k);
+      }
+      o32[i] = word;
+    }
+  } else {
+    for (size_t i = blockIdx.x * (size_t)kThreads + threadIdx.x; i < total; i += (size_t)gridDim.x * kThreads) {
+      const size_t j = i % frame;
+      // packed 4:2:2: Y is every other byte, starting at packed_y0; planar: the first fh * fw words
+      const bool is_y = fmt_packed(kFmt) ? (int)(j & 1) == packed_y0(kFmt) : j < luma;
+      o[i] = kFmt == kHWC ? (Wd)0 : F::word(is_y ? y : F::kCoff);
+    }
   }
 }
 
@@ -370,12 +494,14 @@ int launch_fill_black(const char* name, void* out, int n, int c, int fh, int fw,
              name);
   TG_REQUIRE(!fmt_420(kFmt) || ((fh | fw) & 1) == 0, TG_E_UNSUPPORTED,
              "%s: YUV 4:2:0 needs an even height and width, got %dx%d", name, fh, fw);
-  TG_REQUIRE(!fmt_packed(kFmt) || (fw & 1) == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name,
+  TG_REQUIRE(!fmt_422(kFmt) || (fw & 1) == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name,
              fw);
+  TG_REQUIRE(kFmt != kV210 || ((uintptr_t)out & 15u) == 0, TG_E_INVALID, "%s: v210 frames must be 16-byte aligned",
+             name);
   const size_t frame = frame_words<kFmt>(c, fh, fw), total = frame * n;
   const size_t need = (total + kThreads - 1) / kThreads, ctas = need < 4096 ? need : 4096;
   tg_launch(fill_black_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), 0, stream, static_cast<uint8_t*>(out),
-            frame, (size_t)fh * fw, total, color);
+            frame, (size_t)fh * fw, total, color, fw);
   TG_CUDA_LAUNCH_CHECK(name);
   return TG_OK;
 }
@@ -404,8 +530,13 @@ luma_sums_kernel(const uint8_t* __restrict__ in, int c, int h, int w, int bgr, i
       v = (9798u * R + 19235u * G + 3735u * B + 16384u) >> 15;
     } else if constexpr (fmt_packed(kFmt)) {
       v = __ldg(in + ((size_t)img * h + y) * 2 * w + 2 * x + packed_y0(kFmt));   // Y of pixel x in its pair's group
+    } else if constexpr (kFmt == kV210) {
+      const int f = 2 * (x % 6) + 1;                                           // Y of pixel x in its group
+      const uint32_t* g = reinterpret_cast<const uint32_t*>(in + ((size_t)img * h + y) * v210_stride(w)) + 4 * (x / 6);
+      v = ((__ldg(g + f / 3) >> (10 * (f % 3))) & 1023u) >> 2;
     } else {
-      const Wd* frame = reinterpret_cast<const Wd*>(in) + img * (fmt_444(kFmt) ? 3 * px : 3 * (px / 2));
+      const Wd* frame = reinterpret_cast<const Wd*>(in) +
+                        img * (fmt_444(kFmt) ? 3 * px : fmt_p422(kFmt) ? 2 * px : 3 * (px / 2));
       v = (unsigned)F::sample(__ldg(frame + (size_t)y * w + x)) >> (F::k10 ? 2 : 0);
     }
     atomicAdd(cols + (size_t)img * w + x, (unsigned long long)v);
@@ -431,8 +562,9 @@ int launch_luma_sums(const char* name, const void* in, int bgr, int n, int c, in
              name);
   TG_REQUIRE(!fmt_420(kFmt) || ((h | w) & 1) == 0, TG_E_UNSUPPORTED,
              "%s: YUV 4:2:0 needs an even height and width, got %dx%d", name, h, w);
-  TG_REQUIRE(!fmt_packed(kFmt) || (w & 1) == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name,
+  TG_REQUIRE(!fmt_422(kFmt) || (w & 1) == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name,
              w);
+  TG_REQUIRE(kFmt != kV210 || ((uintptr_t)in & 3u) == 0, TG_E_INVALID, "%s: v210 frames must be 4-byte aligned", name);
   const int x_tiles = tg_ceil_div(w, kTilePx);
   const size_t ctas = (size_t)x_tiles * h * n;
   TG_REQUIRE(ctas <= 0x7fffffff, TG_E_UNSUPPORTED, "%s: grid too large", name);
@@ -468,7 +600,7 @@ int rgb_to_yuv(const char* name, const uint8_t* rgb_u8, const float* rgb_f32, vo
   int f = 0, color = 0;
   const int rc = parse_yuv_format(name, fmt, &f, &color);
   if (rc != TG_OK) return rc;
-  const bool ten = f == kP010 || f == kI420_10 || f == kI444_10;
+  const bool ten = fmt_10(f);
   TG_REQUIRE(out, TG_E_INVALID, "%s: null pointer (out)", name);
   TG_REQUIRE(ten ? (rgb_f32 && !rgb_u8) : (rgb_u8 && !rgb_f32), TG_E_INVALID,
              "%s: %s output is encoded from %s (and only that source)", name, ten ? "10-bit" : "8-bit",
@@ -651,7 +783,7 @@ extern "C" int tg_yuv_coefficients(const tg_yuv_format* fmt, int32_t* out16) {
   const int rc = parse_yuv_format("yuv_coefficients", fmt, &f, &color);
   if (rc != TG_OK) return rc;
   TG_REQUIRE(out16, TG_E_INVALID, "yuv_coefficients: null pointer (out16)");
-  const int* r = kYuvTable.v[(f == kP010 || f == kI420_10 || f == kI444_10) ? 1 : 0][color];
+  const int* r = kYuvTable.v[fmt_10(f) ? 1 : 0][color];
   for (int k = 0; k < 16; ++k) out16[k] = r[k];
   return TG_OK;
 }

@@ -276,9 +276,9 @@ class StreamEngine(ClipEngine):
     pattern of resets.  The step itself is the unchanged net.step_into.
 
     YUV input (yuv_in = 'nv12' / 'i420' / 'p010' / 'i420_10', or the 4:2:2 / 4:4:4 'yuy2' / 'uyvy' / 'i444' /
-    'i444_10'): inp[p] holds [n,3h/2,w] frames ([n,h,2w] for 4:2:2, [n,3h,w] for 4:4:4; uint16 for the 10-bit
-    layouts) and the first launch is tg_stream_frame_in_yuv420 (8 bit, BT.601 limited range: cv2's
-    conversion) or tg_stream_frame_in_yuv (any other layout or colour) instead, with the same reset.  YUV output
+    'i444_10', or the 10-bit 4:2:2 'p210' / 'i422_10' / 'v210'): inp[p] holds [n,3h/2,w] frames ([n,h,2w] for 4:2:2,
+    [n,3h,w] for 4:4:4, [n,2h,w] for P210 / I422_10, [n,h,v210_stride(w)] for v210; ops.yuv_word_dtype words) and
+    the first launch is tg_stream_frame_in_yuv420 (8 bit, BT.601 limited range: cv2's conversion) or tg_stream_frame_in_yuv (any other layout or colour) instead, with the same reset.  YUV output
     (yuv_out): each graph ends with the encode into yuv[p] [n,3H/2,W] (or that layout's shape) --
     tg_rgb_u8_to_yuv420 of u8[p] (8 bit,
     BT.601 limited range), tg_rgb_to_yuv of u8[p] (8 bit, other colours) or tg_rgb_to_yuv of the fp32 HR frame
@@ -326,11 +326,13 @@ class StreamEngine(ClipEngine):
         fh, fw = self.crop[:2] if self.crop else self.in_picture or (h, w)
         frame = ops.yuv_frame_shape(yuv_in, fh, fw) if yuv_in else (fh, fw, c)
         # 10-bit words: zeroed as int16, the same bits
-        in_dtype = torch.int16 if yuv_in and ops.yuv_depth(yuv_in) == 10 else torch.uint8
+        in_dtype = torch.int16 if _word_dtype(yuv_in) == torch.uint16 else torch.uint8
         self.inp = ([torch.zeros(n, *frame, dtype=in_dtype, device=dev).view(_word_dtype(yuv_in)) for _ in range(2)]
                     if self.u8_input else None)
         # the frame input, called as frame_in(frames, reset=, lr_curr=, lr_prev=, hr_prev=)
         in_window = self.crop[2:] if self.crop else None       # (top, left) of the picture in the input frames
+        if in_window and yuv_in == 'v210':
+            in_window = (*in_window, fw)                       # v210 rows do not give the frame's width: name it
         self.in_tables = None
         if self.in_picture:
             self.in_tables = [tuple(t.to(dev) for t in ops.resample_table(a, b, in_filter))
@@ -353,6 +355,7 @@ class StreamEngine(ClipEngine):
         Ho, Wo = self.out_size or (H, W)
         out_window = self.out_frame[2:] if self.out_frame else None     # (y, x) of the picture in the output frames
         Yf, Xf = self.out_frame[:2] if self.out_frame else (Ho, Wo)
+        enc_window = (*out_window, Xf) if out_window and yuv_out == 'v210' else out_window
         ten = yuv_out is not None and ops.yuv_depth(yuv_out) == 10
         self.yuv = self.pad = self.rs = self.tables = None
         if yuv_out:
@@ -365,7 +368,10 @@ class StreamEngine(ClipEngine):
             # write of the picture
             with torch.cuda.device(dev):
                 for t in self.yuv or self.pad:
-                    ops.fill_black(t, yuv_out, out_color)
+                    if yuv_out == 'v210':
+                        ops.fill_black_v210(t, out_color, Xf)
+                    else:
+                        ops.fill_black(t, yuv_out, out_color)
         if self.out_size:
             self.tables = [tuple(t.to(dev) for t in ops.resample_table(a, b, resize_filter))
                            for a, b in ((H, Ho), (W, Wo))]
@@ -387,7 +393,7 @@ class StreamEngine(ClipEngine):
                 calls.append(functools.partial(ops.rgb_u8_to_yuv420, src[p], yuv_out, out=self.yuv[p]))
             elif yuv_out:
                 # 10 bit: from the step's fp32 HR frame (or its resize), two more bits than the uint8 output keeps
-                calls.append(functools.partial(ops.rgb_to_yuv, yuv_out, out_color, out=self.yuv[p], window=out_window,
+                calls.append(functools.partial(ops.rgb_to_yuv, yuv_out, out_color, out=self.yuv[p], window=enc_window,
                                                **{'rgb_f32' if ten else 'rgb_u8': src[p]}))
         self.res = self.yuv or self.pad or self.rs or self.u8
         self.scene_cut = scene_cut
@@ -750,13 +756,14 @@ class PaddedStreamEngine(StreamEngine):
 
 
 YUV420 = ops.YUV420_LAYOUTS       # 'nv12', 'i420'
-YUV = ops.YUV_LAYOUTS             # those, the 10-bit 'p010', 'i420_10', 4:2:2 'yuy2', 'uyvy', 4:4:4 'i444', 'i444_10'
+YUV = ops.YUV_LAYOUTS             # those, the 10-bit 'p010', 'i420_10', 4:2:2 'yuy2', 'uyvy', 4:4:4 'i444', 'i444_10',
+                                  # 10-bit 4:2:2 'p210', 'i422_10', 'v210'
 _YUV_422_444 = ops.YUV422_LAYOUTS + ops.YUV444_LAYOUTS
 COLORS = ops.YUV_COLORS           # 'bt601' (the default, cv2's conversion), 'bt709', 'bt601-full', 'bt709-full'
 
 
 def _word_dtype(layout):
-    return torch.uint16 if layout and ops.yuv_depth(layout) == 10 else torch.uint8
+    return ops.yuv_word_dtype(layout) if layout else torch.uint8
 
 
 class VideoStream:
@@ -872,7 +879,8 @@ class VideoStream:
         10-bit input ('p010', 'i420_10') takes uint16 frames [n,k,3h/2,w] ([k,3h/2,w] when n == 1), torch.uint16 or
         NumPy uint16; uint8 frames into a 10-bit stream raise, and so do uint16 frames into an 8-bit one.
         4:2:2 and 4:4:4, in and out: 'yuy2' / 'uyvy' frames are uint8 [n,k,h,2w], 'i444' uint8 [n,k,3h,w] and
-        'i444_10' uint16 [n,k,3h,w] (H, W or Ho, Wo on the output side).
+        'i444_10' uint16 [n,k,3h,w] (H, W or Ho, Wo on the output side).  10-bit 4:2:2: 'p210' / 'i422_10' uint16
+        [n,k,2h,w] and 'v210' uint8 [n,k,h,S] with S = 128 * ceil(w / 48) bytes a row.
         A stream opened with scene_cut=threshold restarts a slot at every detected cut, as reset= would have, and
         sets last_cuts (bool [n,k]) and last_scores (float64 [n,k]) for this push: NumPy with out='host', CUDA
         tensors ordered on the current stream with out='device'.  A reset requested by the caller scores 0 and is
@@ -956,7 +964,9 @@ class VideoStream:
         if frame is None:
             frame = ops.yuv_frame_shape(self.input, self.h, self.w)
             layout = ('n,k,h,2w' if self.input in ops.YUV422_LAYOUTS else
-                      'n,k,3h,w' if self.input in ops.YUV444_LAYOUTS else 'n,k,3h/2,w')
+                      'n,k,3h,w' if self.input in ops.YUV444_LAYOUTS else
+                      'n,k,2h,w' if self.input in ('p210', 'i422_10') else
+                      'n,k,h,128*ceil(w/48)' if self.input == 'v210' else 'n,k,3h/2,w')
         if frames.dim() == len(frame) + 1 and self.n == 1:
             frames = frames.unsqueeze(0)
         if (frames.dim() != len(frame) + 2 or frames.shape[0] != self.n or frames.shape[1] < 1
@@ -1054,31 +1064,52 @@ def _is_int(v):
 
 
 def _grid(layout):
-    """(row, column) step of a layout's chroma grid: 4:2:0 (2, 2), 4:2:2 (1, 2), RGB / 4:4:4 (1, 1)."""
-    if layout in ops.YUV422_LAYOUTS:
+    """(row, column) step of a layout's chroma grid: 4:2:0 (2, 2), 4:2:2 (1, 2), RGB / 4:4:4 (1, 1); v210 (1, 6),
+    its 6-pixel groups, where a picture starts."""
+    if layout == 'v210':
+        return 1, 6
+    if layout in ops.YUV422_LAYOUTS or layout in ops.YUV422_10_LAYOUTS:
         return 1, 2
     return (2, 2) if layout in YUV and layout not in _YUV_422_444 else (1, 1)
 
 
+def _size_grid(layout):
+    """(row, column) step of a layout's frame and picture sizes: _grid's, except v210's even width (a picture that
+    reaches the frame's right edge may end inside a group)."""
+    return (1, 2) if layout == 'v210' else _grid(layout)
+
+
+def _group_end(layout, right, w):
+    """A picture ending at column `right` of a w-wide frame ends on the layout's grid: always, except in v210, whose
+    pictures end on a 6-pixel group or at the frame's right edge."""
+    return layout != 'v210' or right % 6 == 0 or right == w
+
+
 def _check_box(arg, box, h, w, layout):
     """box = (top, left, ch, cw) -> ints, or ValueError: a non-empty box inside the h x w frame, on the layout's
-    chroma grid (4:2:0: all four even; 4:2:2: left and cw even)."""
+    chroma grid (4:2:0: all four even; 4:2:2: left and cw even; v210: left on a 6-pixel group, cw even and the box
+    ending on a group or at the frame's right edge)."""
     if not isinstance(box, (tuple, list)) or len(box) != 4 or not all(_is_int(v) for v in box):
         raise ValueError(f'{arg} must be (top, left, ch, cw), four ints, got {box!r}')
     top, left, ch, cw = (int(v) for v in box)
     if top < 0 or left < 0 or ch <= 0 or cw <= 0 or top + ch > h or left + cw > w:
         raise ValueError(f'{arg} {ch}x{cw} at ({top}, {left}) lies outside the {h}x{w} frame')
     gy, gx = _grid(layout)
-    if top % gy or ch % gy or left % gx or cw % gx:
+    sy, sx = _size_grid(layout)
+    if top % gy or ch % sy or left % gx or cw % sx or not _group_end(layout, left + cw, w):
         raise ValueError(f'{arg} ({top}, {left}, {ch}, {cw}) is off the {layout} chroma grid: rows in steps of {gy}, '
-                         f'columns in steps of {gx}')
+                         f'columns in steps of {gx}' + _V210_RULE * (layout == 'v210'))
     return top, left, ch, cw
+
+
+_V210_RULE = ' (a v210 picture starts on a 6-pixel group and ends on one or at the frame\'s right edge)'
 
 
 def _check_out_frame(out_frame, out_origin, Ho, Wo, out_format):
     """out_frame (Hf, Wf) and out_origin (y, x) or None -> ints, or ValueError: the Ho x Wo picture inside the frame,
     frame and origin on the output layout's chroma grid.  The default origin centres the picture, rounded down to
-    the grid."""
+    the grid; a v210 picture that would then not end on a 6-pixel group goes to the frame's right edge instead, the
+    only place it can end inside a group."""
     if (not isinstance(out_frame, (tuple, list)) or len(out_frame) != 2
             or not all(_is_int(v) and v > 0 for v in out_frame)):
         raise ValueError(f'out_frame must be (Hf, Wf), two positive ints, got {out_frame!r}')
@@ -1086,17 +1117,26 @@ def _check_out_frame(out_frame, out_origin, Ho, Wo, out_format):
     if Ho > Hf or Wo > Wf:
         raise ValueError(f'the {Ho}x{Wo} output picture does not fit out_frame {Hf}x{Wf}')
     gy, gx = _grid(out_format)
-    if Hf % gy or Wf % gx:
+    sy, sx = _size_grid(out_format)
+    if Hf % sy or Wf % sx:
         raise ValueError(f'out_frame {Hf}x{Wf} is off the {out_format} chroma grid')
     if out_origin is None:
-        out_origin = ((Hf - Ho) // 2 // gy * gy, (Wf - Wo) // 2 // gx * gx)
+        x = (Wf - Wo) // 2 // gx * gx
+        if not _group_end(out_format, x + Wo, Wf):
+            if (Wf - Wo) % gx:
+                raise ValueError(f'no out_origin puts a {Wo}-wide v210 picture into out_frame {Hf}x{Wf}: it starts on '
+                                 f'a 6-pixel group and ends on one or at the frame\'s right edge, so Wo or Wf - Wo '
+                                 f'must be a multiple of 6')
+            x = Wf - Wo
+        out_origin = ((Hf - Ho) // 2 // gy * gy, x)
     if not isinstance(out_origin, (tuple, list)) or len(out_origin) != 2 or not all(_is_int(v) for v in out_origin):
         raise ValueError(f'out_origin must be (y, x), two ints, got {out_origin!r}')
     y, x = int(out_origin[0]), int(out_origin[1])
     if y < 0 or x < 0 or y + Ho > Hf or x + Wo > Wf:
         raise ValueError(f'the {Ho}x{Wo} output picture at out_origin ({y}, {x}) does not fit out_frame {Hf}x{Wf}')
-    if y % gy or x % gx:
-        raise ValueError(f'out_origin ({y}, {x}) is off the {out_format} chroma grid')
+    if y % gy or x % gx or not _group_end(out_format, x + Wo, Wf):
+        raise ValueError(f'out_origin ({y}, {x}) is off the {out_format} chroma grid' +
+                         _V210_RULE * (out_format == 'v210'))
     return (Hf, Wf), (y, x)
 
 
@@ -1132,25 +1172,29 @@ def fit_size(picture, frame, sar=(1, 1), out_format='rgb'):
     return h, w
 
 
-def detect_bars(frames, input='uint8', channel_order='rgb', limit=24):
+def detect_bars(frames, input='uint8', channel_order='rgb', limit=24, width=None):
     """The picture box (top, left, ch, cw) of letterboxed / pillarboxed frames, found on the device: a row or column
     is picture when its mean 8-bit luma exceeds `limit` in any of the frames (24 is ffmpeg cropdetect's default
     limit; the rule is oracle/frame_window.py's, not cropdetect's), and the box spans the first to the last picture
     row and column, rounded inward to the input layout's chroma grid.  Luma is Y for YUV input (10-bit samples >> 2)
     and cv2's gray of RGB ((9798 R + 19235 G + 3735 B + 16384) >> 15).  frames: a CUDA tensor [k,h,w,3] (uint8,
     channel_order 'rgb' or 'bgr') or [k,*yuv_frame_shape(input, h, w)] for a YUV input.  Frames with no picture row
-    or column (all black) give the whole frame.  Pass crop=detect_bars(...) to FRNet.stream."""
+    or column (all black) give the whole frame.  v210 frames [k,h,128*ceil(w/48)] need their width w (`width`), which
+    their padded rows do not give; their box starts on a 6-pixel group and ends on one or at the frame's right edge.
+    Pass crop=detect_bars(...) to FRNet.stream."""
     if input not in ('uint8', *YUV):
         raise ValueError(f"input must be 'uint8' or one of {YUV}, got {input!r}")
     if channel_order not in ('rgb', 'bgr') or (input != 'uint8' and channel_order != 'rgb'):
         raise ValueError(f'channel_order={channel_order!r} does not apply to input={input!r}')
     if isinstance(limit, bool) or not isinstance(limit, numbers.Real) or not 0 <= limit < 255:
         raise ValueError(f'limit must be a number in [0, 255), got {limit!r}')
+    if (width is None) != (input != 'v210'):
+        raise ValueError(f'width applies to, and is needed by, v210 frames only (input={input!r}, width={width!r})')
     if not isinstance(frames, torch.Tensor) or not frames.is_cuda:
         raise ValueError('detect_bars: frames must be a CUDA tensor')
     layout = input if input in YUV else None
     with torch.cuda.device(frames.device):          # the memsets and the kernel go to the frames' device
-        rows, cols = ops.luma_line_sums(frames.contiguous(), layout, channel_order == 'bgr')
+        rows, cols = ops.luma_line_sums(frames.contiguous(), layout, channel_order == 'bgr', frame_w=width)
     h, w = rows.shape[1], cols.shape[1]
     # mean > limit <=> sum > limit * count: exact for integer limits, and for others compared in float64
     pic_r = (rows.double() > float(limit) * w).any(0).cpu().numpy()
@@ -1169,6 +1213,8 @@ def bars_box(pic_rows, pic_cols, layout):
     c = np.flatnonzero(pic_cols)
     top, bottom = -(-int(r[0]) // gy) * gy, (int(r[-1]) + 1) // gy * gy
     left, right = -(-int(c[0]) // gx) * gx, (int(c[-1]) + 1) // gx * gx
+    if layout == 'v210' and int(c[-1]) + 1 == w:
+        right = w                                    # a v210 picture may end inside the frame's last group
     if bottom <= top or right <= left:
         return 0, 0, h, w
     return top, left, bottom - top, right - left

@@ -21,6 +21,7 @@ AMODE_AUTO, AMODE_HALO, AMODE_TAP = 0, 1, 2
 AMODE_REVERSE = 0x100               # TG_AMODE_REVERSE: flag, walk the conv's tiles last to first
 YUV_NV12, YUV_I420, YUV_P010, YUV_I420_10 = 0, 1, 2, 3
 YUV_YUY2, YUV_UYVY, YUV_I444, YUV_I444_10 = 4, 5, 6, 8      # 7 is not a layout
+YUV_P210, YUV_I422_10, YUV_V210 = 9, 10, 11                 # 10-bit 4:2:2
 RESAMPLE_BICUBIC, RESAMPLE_LANCZOS3 = 0, 1
 SCENE_CUT_WORK_BYTES = 16            # TG_SCENE_CUT_WORK_BYTES: workspace of tg_scene_cut per slot
 TAIL_OUT_ROWS = 40                   # TG_TAIL_OUT_ROWS: rows of tg_pack_tail_out_weights' tile (128 bytes each)

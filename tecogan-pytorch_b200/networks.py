@@ -384,6 +384,14 @@ class FRNet(BaseSequenceGenerator):
         COLOR_YUV2RGB_YUY2 / _UYVY and COLOR_RGB2YUV_YUY2 / _UYVY (chroma of each pair's mean); 'i444' (uint8) and
         'i444_10' (uint16, sample in the low 10 bits) are planar [n,k,3h,w] frames with a chroma sample per pixel.
         Neither needs an even h.
+        10-bit 4:2:2 video (professional and broadcast), as input or out_format, w even, any h: 'p210' (uint16
+        [n,k,2h,w]: the Y plane, then a full-height interleaved UV plane, samples in the high 10 bits; GPU video
+        engines), 'i422_10' (uint16 [n,k,2h,w]: the Y plane, then U and V planes of h x w/2, samples in the low 10
+        bits; ffmpeg yuv422p10le, what ProRes 422 and DNxHR decode into) and 'v210' (uint8 [n,k,h,S] with
+        S = 128 * ceil(w / 48): 6 pixels per 16-byte group, rows padded to 128 bytes; SDI capture and playout).
+        Decode is the 10-bit row with nearest chroma; the encode takes the fp32 HR frame, Y per pixel and U, V from
+        each pair's sum.  A v210 crop or out_origin starts on a 6-pixel group and ends on one or at the frame's right
+        edge.
         in_color / out_color pick the YUV side's colour: 'bt601' (the default, limited range; for 8-bit frames
         exactly cv2's conversion), 'bt709', 'bt601-full', 'bt709-full' (ITU-T H.273 quantisation, integer fixed
         point as oracle/yuv_color.py specifies).  Take in_color from the decoder (ffprobe's color_space /

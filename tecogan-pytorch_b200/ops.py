@@ -401,10 +401,24 @@ def _step_state(name, reset, lr_curr, lr_prev, hr_prev, scale):
     return n, c, h, w
 
 
-def _frames(name, frames, layout, n, c, h, w, window):
+def _split_window(name, layout, window):
+    """window -> ((top, left) or None, the frame width it names or None).  A v210 frame's padded rows do not give its
+    width, so a v210 window is (top, left, frame_w); every other window is (top, left)."""
+    if window is None:
+        return None, None
+    window = tuple(window)
+    if layout == 'v210':
+        if len(window) != 3:
+            raise L.TecoganB200Error(f'{name}: a v210 window is (top, left, frame_w), got {window!r}')
+        return window[:2], window[2]
+    return window, None
+
+
+def _frames(name, frames, layout, n, c, h, w, window, frame_w=None):
     """Checks the frames an h x w picture of n slots is read from: uint8 HWC [n,Hf,Wf,c] (layout None) or a YUV
-    layout's words [n,*yuv_frame_shape(layout, Hf, Wf)] (uint16 for the 10-bit layouts), or None (no frames).  Hf x Wf
-    is h x w, or any size when the picture is read at window = (top, left).  -> (Hf, Wf)"""
+    layout's words [n,*yuv_frame_shape(layout, Hf, Wf)] (yuv_word_dtype), or None (no frames).  Hf x Wf is h x w, or
+    any size when the picture is read at window = (top, left); a windowed v210 frame's width Wf is frame_w, which its
+    padded rows do not give.  -> (Hf, Wf)"""
     if layout is not None:
         if c != 3:
             raise L.TecoganB200Error(f'{name}: lr_curr has {c} channels, YUV frames decode to 3')
@@ -418,8 +432,8 @@ def _frames(name, frames, layout, n, c, h, w, window):
         fh, fw = (h, w) if window is None else frames.shape[1:3]
         want = (n, fh, fw, c)
     else:
-        _req(frames, torch.uint16 if yuv_depth(layout) == 10 else torch.uint8, 'frames', 3)
-        fh, fw = (h, w) if window is None else yuv_frame_size(layout, frames.shape[1:])
+        _req(frames, yuv_word_dtype(layout), 'frames', 3)
+        fh, fw = (h, w) if window is None else yuv_frame_size(layout, frames.shape[1:], frame_w)
         want = (n, *yuv_frame_shape(layout, fh, fw))
     if tuple(frames.shape) != want:
         raise L.TecoganB200Error(f'{name}: frames {tuple(frames.shape)} != {want} ({layout or "uint8 HWC"} frames of '
@@ -523,20 +537,41 @@ def rgb_u8_to_yuv420(rgb, layout, out=None):
 
 YUV422_LAYOUTS = ('yuy2', 'uyvy')                     # packed 4:2:2, uint8
 YUV444_LAYOUTS = ('i444', 'i444_10')                  # planar 4:4:4, uint8 / uint16
-# 4:2:0, then 4:2:2 and 4:4:4; 8-bit uint8 words; 10-bit uint16 words
-YUV_LAYOUTS = ('nv12', 'i420', 'p010', 'i420_10') + YUV422_LAYOUTS + YUV444_LAYOUTS
+# 10-bit 4:2:2: 'p210' / 'i422_10' uint16 [2h, w] (Y plane, then the interleaved UV plane / the U and V planes of
+# h x w/2), 'v210' uint8 [h, v210_stride(w)] (6 pixels per 16-byte group, rows padded to 128 bytes)
+YUV422_10_LAYOUTS = ('p210', 'i422_10', 'v210')
+# 4:2:0, then 4:2:2 and 4:4:4, then 10-bit 4:2:2; 8-bit uint8 words; 10-bit uint16 words, v210 uint8
+YUV_LAYOUTS = ('nv12', 'i420', 'p010', 'i420_10') + YUV422_LAYOUTS + YUV444_LAYOUTS + YUV422_10_LAYOUTS
 YUV_COLORS = ('bt601', 'bt709', 'bt601-full', 'bt709-full')
 _LAYOUT_CODE = {'nv12': L.YUV_NV12, 'i420': L.YUV_I420, 'p010': L.YUV_P010, 'i420_10': L.YUV_I420_10,
-                'yuy2': L.YUV_YUY2, 'uyvy': L.YUV_UYVY, 'i444': L.YUV_I444, 'i444_10': L.YUV_I444_10}
+                'yuy2': L.YUV_YUY2, 'uyvy': L.YUV_UYVY, 'i444': L.YUV_I444, 'i444_10': L.YUV_I444_10,
+                'p210': L.YUV_P210, 'i422_10': L.YUV_I422_10, 'v210': L.YUV_V210}
 
 
 def yuv_depth(layout):
-    """Bit depth of a YUV layout: 8 (uint8 frames) or 10 (uint16 frames)."""
-    return 10 if layout in ('p010', 'i420_10', 'i444_10') else 8
+    """Bit depth of a YUV layout: 8 or 10."""
+    return 10 if layout in ('p010', 'i420_10', 'i444_10') + YUV422_10_LAYOUTS else 8
+
+
+def yuv_word_dtype(layout):
+    """The dtype of a YUV layout's frames: uint16 for the 10-bit layouts, uint8 for the 8-bit ones and for v210,
+    whose 10-bit samples are packed into bytes."""
+    return torch.uint16 if yuv_depth(layout) == 10 and layout != 'v210' else torch.uint8
+
+
+def v210_stride(w):
+    """Bytes per row of a v210 frame w pixels wide: 128 * ceil(w / 48) (ceil(w / 6) 16-byte groups of 6 pixels,
+    padded to 128 bytes)."""
+    return 128 * (-(-w // 48))
 
 
 def yuv_frame_shape(layout, h, w):
-    """The words of one h x w frame: (3h/2, w) for 4:2:0, (h, 2w) for packed 4:2:2, (3h, w) for planar 4:4:4."""
+    """The words of one h x w frame: (3h/2, w) for 4:2:0, (h, 2w) for packed 4:2:2, (3h, w) for planar 4:4:4,
+    (2h, w) for P210 / I422_10 and (h, v210_stride(w)) bytes for v210."""
+    if layout == 'v210':
+        return (h, v210_stride(w))
+    if layout in ('p210', 'i422_10'):
+        return (2 * h, w)
     if layout in YUV422_LAYOUTS:
         return (h, 2 * w)
     return (3 * h, w) if layout in YUV444_LAYOUTS else (3 * h // 2, w)
@@ -545,7 +580,7 @@ def yuv_frame_shape(layout, h, w):
 def yuv_size_error(layout, h, w):
     """None if an h x w frame fits the layout's chroma subsampling, else why not: 4:2:0 needs an even height and
     width, 4:2:2 an even width, 4:4:4 any size."""
-    if layout in YUV422_LAYOUTS:
+    if layout in YUV422_LAYOUTS + YUV422_10_LAYOUTS:
         return None if w % 2 == 0 else f'YUV 4:2:2 needs an even width, got {w}'
     if layout in YUV444_LAYOUTS:
         return None
@@ -570,12 +605,25 @@ def yuv_coefficients(layout, color):
     return list(out)
 
 
-def yuv_frame_size(layout, shape):
-    """(h, w) of a frame whose words have the 2-d shape `shape` in a YUV layout (yuv_frame_shape's inverse)."""
+def yuv_frame_size(layout, shape, w=None):
+    """(h, w) of a frame whose words have the 2-d shape `shape` in a YUV layout (yuv_frame_shape's inverse).  A v210
+    row's bytes do not give its width (rows are padded to 128 bytes): w must be given; for the other layouts a w
+    that is given must be the shape's."""
     a, b = shape
-    if layout in YUV422_LAYOUTS:
-        return a, b // 2
-    return (a // 3, b) if layout in YUV444_LAYOUTS else (2 * a // 3, b)
+    if layout == 'v210':
+        if w is None:
+            raise L.TecoganB200Error('v210 frames do not give their width (rows are padded to 128 bytes): pass it '
+                                     '(frame_w)')
+        return a, int(w)
+    if layout in ('p210', 'i422_10'):
+        hw = (a // 2, b)
+    elif layout in YUV422_LAYOUTS:
+        hw = (a, b // 2)
+    else:
+        hw = (a // 3, b) if layout in YUV444_LAYOUTS else (2 * a // 3, b)
+    if w is not None and int(w) != hw[1]:
+        raise L.TecoganB200Error(f'{layout} frames of shape {tuple(shape)} are {hw[1]} wide, not {w}')
+    return hw
 
 
 def stream_frame_in_yuv(frames, layout, color, reset, lr_curr, lr_prev, hr_prev, scale, window=None):
@@ -583,11 +631,13 @@ def stream_frame_in_yuv(frames, layout, color, reset, lr_curr, lr_prev, hr_prev,
     'p010' / 'i420_10' / 'i444_10'; or None) in colour `color` -> lr_curr fp32 [n,3,h,w] = RGB / 255 (8 bit) or
     RGB / 1023 (10 bit), as oracle/yuv_color.py (4:2:0) and oracle/yuv_422_444.py (4:2:2, 4:4:4) specify; reset as
     in stream_frame_in.  With window = (top, left), frames hold Hf x Wf frames (frames.shape[1:] ==
-    yuv_frame_shape(layout, Hf, Wf)) and the h x w picture at (top, left) is read (tg_stream_frame_in_yuv_window)."""
+    yuv_frame_shape(layout, Hf, Wf)) and the h x w picture at (top, left) is read (tg_stream_frame_in_yuv_window);
+    a v210 window is (top, left, Wf): its frames' rows do not give Wf."""
     name = 'stream_frame_in_yuv' if window is None else 'stream_frame_in_yuv_window'
     fmt = yuv_format(layout, color, name)
+    window, frame_w = _split_window(name, layout, window)
     n, c, h, w = _step_state(name, reset, lr_curr, lr_prev, hr_prev, scale)
-    fh, fw = _frames(name, frames, layout, n, c, h, w, window)
+    fh, fw = _frames(name, frames, layout, n, c, h, w, window, frame_w)
     _same_device(name, lr_curr, lr_prev, hr_prev, frames, reset)
     if window is not None:
         win = frame_window(fh, fw, *window) if frames is not None else frame_window(h, w, 0, 0)
@@ -606,9 +656,12 @@ def rgb_to_yuv(layout, color, rgb_u8=None, rgb_f32=None, out=None, window=None):
     layouts encode rgb_f32 (fp32 NCHW [n,3,H,W], quantised as clip(rint(x * 1023), 0, 1023)) into uint16
     [n,*yuv_frame_shape] ([n,3H/2,W] for 4:2:0, [n,H,2W] for 4:2:2, [n,3H,W] for 4:4:4).  With window = (top, left),
     out holds larger Hf x Wf frames and the H x W picture is written at (top, left) of each (tg_rgb_to_yuv_window);
-    the words around it are left as they are."""
+    the words around it are left as they are.  'p210' / 'i422_10' are [n,2H,W] uint16 and 'v210' [n,H,v210_stride(W)]
+    uint8, all three 10-bit (from rgb_f32); a v210 window is (top, left, Wf).  A whole-frame v210 encode writes every
+    byte of each row (the fields past the last pixel and the row padding 0), a windowed one the picture's groups."""
     name = 'rgb_to_yuv' if window is None else 'rgb_to_yuv_window'
     fmt = yuv_format(layout, color, name)
+    window, frame_w = _split_window(name, layout, window)
     ten = yuv_depth(layout) == 10
     if ten:
         if rgb_f32 is None or rgb_u8 is not None:
@@ -625,10 +678,10 @@ def rgb_to_yuv(layout, color, rgb_u8=None, rgb_f32=None, out=None, window=None):
     err = yuv_size_error(layout, H, W)
     if err:
         raise L.TecoganB200Error(f'{name}: {err}')
-    dtype = torch.uint16 if ten else torch.uint8
+    dtype = yuv_word_dtype(layout)
     if window is not None and out is None:
         raise L.TecoganB200Error(f'{name}: a window needs the output frames (out)')
-    fh, fw = (H, W) if window is None else yuv_frame_size(layout, out.shape[1:])
+    fh, fw = (H, W) if window is None else yuv_frame_size(layout, out.shape[1:], frame_w)
     shape = (n, *yuv_frame_shape(layout, fh, fw))
     if out is None:
         out = torch.empty(shape, dtype=dtype, device=src.device)
@@ -650,15 +703,29 @@ def rgb_to_yuv(layout, color, rgb_u8=None, rgb_f32=None, out=None, window=None):
 def fill_black(out, layout=None, color='bt601'):
     """tg_fill_black: every word of out := the format's black.  layout None: uint8 HWC [n,Hf,Wf,c], all 0; else the
     YUV layout's frames [n,*yuv_frame_shape(layout, Hf, Wf)] with Y = the colour's black level (16 << (depth - 8)
-    limited range, 0 full) and U = V = 128 << (depth - 8), P010 words << 6."""
+    limited range, 0 full) and U = V = 128 << (depth - 8), P010 / P210 words << 6.  v210: fill_black_v210."""
+    if layout == 'v210':
+        raise L.TecoganB200Error('fill_black: v210 frames do not give their width: use fill_black_v210(out, color, '
+                                 'frame_w)')
+    return _fill_black(out, layout, color, None)
+
+
+def fill_black_v210(out, color, frame_w):
+    """tg_fill_black of v210 frames out [n,Hf,v210_stride(frame_w)] (uint8), whose rows do not give their width:
+    Y = the colour's black level (64 limited range, 0 full) and U = V = 512 in the fields of the frame_w pixels, 0 in
+    the rest of each row."""
+    return _fill_black(out, 'v210', color, frame_w)
+
+
+def _fill_black(out, layout, color, frame_w):
     fmt = None
     if layout is None:
         _req(out, torch.uint8, 'out', 4)
         n, fh, fw, c = out.shape
     else:
         fmt = yuv_format(layout, color, 'fill_black')
-        _req(out, torch.uint16 if yuv_depth(layout) == 10 else torch.uint8, 'out', 3)
-        (fh, fw), n, c = yuv_frame_size(layout, out.shape[1:]), out.shape[0], 3
+        _req(out, yuv_word_dtype(layout), 'out', 3)
+        (fh, fw), n, c = yuv_frame_size(layout, out.shape[1:], frame_w), out.shape[0], 3
         if tuple(out.shape[1:]) != yuv_frame_shape(layout, fh, fw):
             raise L.TecoganB200Error(f'fill_black: {tuple(out.shape)} is not a stack of {layout} frames')
     L.check(L.load().tg_fill_black(_ptr(out), ctypes.byref(fmt) if fmt is not None else None, n, c, fh, fw,
@@ -666,17 +733,18 @@ def fill_black(out, layout=None, color='bt601'):
     return out
 
 
-def luma_line_sums(frames, layout=None, bgr=False):
+def luma_line_sums(frames, layout=None, bgr=False, frame_w=None):
     """tg_luma_line_sums: the per-row and per-column sums of the 8-bit luma of frames (uint8 HWC RGB [n,h,w,3], or a
-    YUV layout's [n,*yuv_frame_shape]) as int64 tensors rows [n,h], cols [n,w] on the frames' device."""
+    YUV layout's [n,*yuv_frame_shape]; v210 frames are frame_w wide) as int64 tensors rows [n,h], cols [n,w] on the
+    frames' device."""
     fmt = None
     if layout is None:
         _req(frames, torch.uint8, 'frames', 4)
         n, h, w, c = frames.shape
     else:
         fmt = yuv_format(layout, 'bt601', 'luma_line_sums')
-        _req(frames, torch.uint16 if yuv_depth(layout) == 10 else torch.uint8, 'frames', 3)
-        (h, w), n, c = yuv_frame_size(layout, frames.shape[1:]), frames.shape[0], 3
+        _req(frames, yuv_word_dtype(layout), 'frames', 3)
+        (h, w), n, c = yuv_frame_size(layout, frames.shape[1:], frame_w), frames.shape[0], 3
         if tuple(frames.shape[1:]) != yuv_frame_shape(layout, h, w):
             raise L.TecoganB200Error(f'luma_line_sums: {tuple(frames.shape)} is not a stack of {layout} frames')
     rows = torch.empty((n, h), dtype=torch.int64, device=frames.device)
@@ -766,13 +834,14 @@ def stream_frame_in_resample(frames, layout, color, reset, lr_curr, lr_prev, hr_
     and cols = (first [wn], weights [wn, taps]) (w -> wn) into lr_curr fp32 [n,c,hn,wn], in one launch; bit for bit
     the frame input at h x w followed by resample(..., out_f32=lr_curr).  frames: uint8 HWC [n,Hf,Wf,c] (layout None,
     channels reversed when bgr) or a YUV layout's [n,*yuv_frame_shape(layout, Hf, Wf)] in colour `color`; the picture
-    is the whole frame, or the h x w one at window = (top, left).  reset as in stream_frame_in (lr_prev
-    [n,c,hn,wn], hr_prev [n,c,scale*hn,scale*wn])."""
+    is the whole frame, or the h x w one at window = (top, left) ((top, left, Wf) for v210).  reset as in
+    stream_frame_in (lr_prev [n,c,hn,wn], hr_prev [n,c,scale*hn,scale*wn])."""
     name = 'stream_frame_in_resample'
     fmt = None if layout is None else yuv_format(layout, color, name)
     n, c, hn, wn = _step_state(name, reset, lr_curr, lr_prev, hr_prev, scale)
     h, w = (int(v) for v in size)
-    fh, fw = _frames(name, frames, layout, n, c, h, w, window)
+    window, frame_w = _split_window(name, layout, window)
+    fh, fw = _frames(name, frames, layout, n, c, h, w, window, frame_w)
     tabs = []
     for axis, (first, weights), n_in, n_out in (('rows', rows, h, hn), ('cols', cols, w, wn)):
         _req(first, torch.int32, f'{axis} first', 1)

@@ -51,6 +51,17 @@ x * 255 is within 1e-3 of a rounding boundary), the resized NV12 output with the
 output.  The YUY2, UYVY and I444 outputs are compared with oracle/yuv_422_444.py's encode of the RGB output for the
 frames each input decodes to.  Card name and power limit are read in the same run.  Writes nothing.
 
+    python tools/stream_bench.py --yuv422-10 [--frames 64] [--reps 3]
+
+measures 10-bit 4:2:2 video instead (one JSON line, metric hr_frames_per_sec_4xBD_3x134x320_streamed_yuv422_10):
+VideoStream.push of pinned frames, k = 16, out='host', in and out of one format -- rgb (uint8), p010_709, p210_709,
+i422_10_709 and v210_709 (BT.709 limited range) -- the arms alternating in every rep, with the median, min, max and
+runs of each; identical: P210's output frame by frame against oracle/yuv_422_10.py's encode of the fp32 HR frames of a
+device loop of FRNet.step over its decode, I422_10's and v210's samples against P210's.  decode_us / encode_us:
+tg_stream_frame_in_yuv and tg_rgb_to_yuv (from the fp32 HR frame) per step for P010 and the three layouts, CUDA events
+over a graph of launches on 8 rotating buffer sets, with their algorithmic bytes (frames read or written, lr_curr or
+the fp32 HR frame) and TB/s.  The card, its power limit and SM clocks (current, max) are read in the same run.
+
     python tools/stream_bench.py --window [--frames 64] [--reps 3]
 
 measures letterboxed video instead (one JSON line, metric hr_frames_per_sec_4xBD_letterbox_134x320_in_180x320): the
@@ -109,6 +120,7 @@ def main():
     ap.add_argument('--window', action='store_true', help='the letterboxed-video arms instead')
     ap.add_argument('--pad', action='store_true', help='the temporally padded arms instead')
     ap.add_argument('--insize', action='store_true', help='the resized-input arms instead')
+    ap.add_argument('--yuv422-10', action='store_true', help='the 10-bit 4:2:2 (P210, I422_10, v210) arms instead')
     args = ap.parse_args()
     if args.frames < 60:
         ap.error('--frames must be >= 60')
@@ -118,6 +130,8 @@ def main():
         return pad_bench(args)
     if args.insize:
         return insize_bench(args)
+    if args.yuv422_10:
+        return yuv422_10_bench(args)
     import numpy as np
     import torch
     import bench
@@ -688,6 +702,123 @@ def insize_bench(args):
         'median': {name: round(statistics.median(v), 1) for name, v in runs.items()},
         'runs': {name: [round(x, 1) for x in v] for name, v in runs.items()}, 'launches_per_step': launches,
         'frame_in_per_step': frame_in}))
+
+
+
+
+def yuv422_10_bench(args):
+    """The 10-bit 4:2:2 arms at bench.py's bd4 shape: k = 16 pushes of pinned frames, in and out of one layout, next to
+    RGB and P010 (BT.709) in the same run, the arms alternating in every rep (rep 0 an untimed warm-up); then each
+    layout's frame-input decode and fp32 encode alone, CUDA-graph timed over 8 rotating buffer sets."""
+    import numpy as np
+    import torch
+    import bench
+    import tecogan_b200 as T
+    from oracle import yuv_color as C
+    from oracle import yuv_422_10 as V
+    ops = sys.modules['tecogan-pytorch_b200.ops']
+    assert torch.cuda.is_available(), 'stream_bench.py needs a GPU'
+    dev = torch.device('cuda', 0)
+    torch.cuda.set_device(dev)
+    bench.select_workload('bd4')
+    n, (c, h, w), s = bench.CLIPS_PER_GPU, bench.LR, bench.SCALE
+    t, H, W = args.frames, s * h, s * w
+    net = T.FRNet(3, 3, 64, 10, 'BD', s)
+    net.load_state_dict(bench.make_params(), strict=True)
+    net = net.to(dev).eval()
+    clips = bench.synthetic_clips(n, t, seed=100).numpy().transpose(0, 1, 3, 4, 2)     # [n,t,h,w,c] in [0,1]
+    u8 = np.ascontiguousarray(np.rint(clips * 255.0).astype(np.uint8))
+    rgb10 = V.quantize10(clips)
+    samples = V.encode_samples(rgb10, 'bt709')
+    sources = {'rgb': (u8, {}),
+               'p010_709': (C.rgb_to_yuv(rgb10, 'p010', 'bt709'), dict(input='p010', out_format='p010'))}
+    for lay in V.LAYOUTS:
+        sources[f'{lay}_709'] = (V.join_planes(*samples, lay), dict(input=lay, out_format=lay))
+    pins = {k: torch.from_numpy(f).pin_memory() for k, (f, _) in sources.items()}
+    opened = {k: net.stream(n, h, w, device=dev, **kw, **({'in_color': 'bt709', 'out_color': 'bt709'} if kw else {}))
+              for k, (_, kw) in sources.items()}
+    runs = {k: [] for k in sources}
+    outputs = {}
+    for rep in range(args.reps + 1):
+        for k in sources:
+            opened[k].reset(range(n))
+            outputs[k] = None
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            outputs[k] = [opened[k].push(pins[k][:, i:i + 16]) for i in range(0, t, 16)]
+            torch.cuda.synchronize()
+            if rep:
+                runs[k].append(n * t / (time.perf_counter() - t0))
+    launches = {k: st._engine.launches_per_step for k, st in opened.items()}
+    for st in opened.values():
+        st.close()
+    got = {k: np.concatenate(v, axis=1) for k, v in outputs.items()}
+    # P210: frame by frame the oracle's encode of the fp32 HR frames of a device loop of FRNet.step over its decode;
+    # I422_10 and v210: the same samples as P210
+    identical = {}
+    lr = torch.from_numpy(V.yuv_to_rgb(sources['p210_709'][0], 'p210', 'bt709').astype(np.float32) / np.float32(1023))
+    lr = lr.permute(0, 1, 4, 2, 3).contiguous()
+    ok = got['p210_709'].shape == (n, t, 2 * H, W)
+    lr_prev, hr_prev = torch.zeros(n, c, h, w, device=dev), torch.zeros(n, c, H, W, device=dev)
+    with torch.no_grad():
+        for i in range(t):
+            if not ok:
+                break
+            cur = lr[:, i].to(dev)
+            hr_prev = net.step(cur, lr_prev, hr_prev)
+            lr_prev = cur
+            ok = np.array_equal(got['p210_709'][:, i], V.rgb_f32_to_yuv(hr_prev.permute(0, 2, 3, 1).cpu().numpy(),
+                                                                        'p210', 'bt709'))
+    identical['p210_709'] = bool(ok)
+    ref = V.split_planes(got['p210_709'], 'p210')
+    for lay in ('i422_10', 'v210'):
+        identical[f'{lay}_709'] = all(np.array_equal(a, b) for a, b in zip(V.split_planes(got[f'{lay}_709'], lay, W),
+                                                                           ref))
+    del got, outputs
+    # the kernels alone: 8 rotating sets of 4 frames
+    nb, reps = 8, 60
+    lrs = [torch.empty(n, c, h, w, device=dev) for _ in range(nb)]
+    prev, hrp = torch.empty(n, c, h, w, device=dev), torch.empty(n, c, H, W, device=dev)
+    hrs = [torch.rand(n, c, H, W, device=dev) for _ in range(nb)]
+    decode, encode, decode_bytes, encode_bytes = {}, {}, {}, {}
+    for lay in ('p010',) + V.LAYOUTS:
+        shape = (n, *((3 * h // 2, w) if lay == 'p010' else V.frame_shape(lay, h, w)))
+        dt = ops.yuv_word_dtype(lay)
+        src = [torch.randint(0, 256, shape, dtype=torch.uint8, device=dev) if dt == torch.uint8 else
+               torch.randint(0, 1 << 15, shape, dtype=torch.int16, device=dev).view(torch.uint16) for _ in range(nb)]
+        sec = bench._time_graph(lambda i: ops.stream_frame_in_yuv(src[i], lay, 'bt709', None, lrs[i], prev, hrp, s),
+                                nb, reps, torch)
+        decode[lay] = sec * 1e6
+        decode_bytes[lay] = src[0].numel() * src[0].element_size() + n * c * h * w * 4
+        oshape = (n, *((3 * H // 2, W) if lay == 'p010' else V.frame_shape(lay, H, W)))
+        outs = [torch.empty(oshape, dtype=dt, device=dev) for _ in range(nb)]
+        sec = bench._time_graph(lambda i: ops.rgb_to_yuv(lay, 'bt709', rgb_f32=hrs[i], out=outs[i]), nb, reps, torch)
+        encode[lay] = sec * 1e6
+        encode_bytes[lay] = n * c * H * W * 4 + outs[0].numel() * outs[0].element_size()
+        del src, outs
+    line = {
+        'metric': 'hr_frames_per_sec_4xBD_3x134x320_streamed_yuv422_10', 'unit': 'frames/s',
+        'device': torch.cuda.get_device_name(0), 'power_limit_w': power_limit_w(), 'sm_clock_mhz': sm_clock_mhz(),
+        'clips': n, 'frames_per_clip': t, 'reps': args.reps, 'chunk': 16,
+        'results': {k: {'median': statistics.median(v), 'min': min(v), 'max': max(v), 'runs': v}
+                    for k, v in runs.items()},
+        'identical': identical,
+        'launches_per_step': launches,
+        'decode_us': decode, 'decode_bytes_per_step': decode_bytes,
+        'decode_tb_per_s': {k: decode_bytes[k] / v * 1e-6 for k, v in decode.items()},
+        'encode_us': encode, 'encode_bytes_per_step': encode_bytes,
+        'encode_tb_per_s': {k: encode_bytes[k] / v * 1e-6 for k, v in encode.items()},
+    }
+    print(json.dumps(line), flush=True)
+
+
+def sm_clock_mhz():
+    try:
+        r = subprocess.run(['nvidia-smi', '-i', '0', '--query-gpu=clocks.sm,clocks.max.sm', '--format=csv,noheader,nounits'],
+                           capture_output=True, text=True, timeout=20)
+        return [float(v) for v in r.stdout.strip().splitlines()[0].split(',')]
+    except Exception:
+        return None
 
 
 if __name__ == '__main__':
