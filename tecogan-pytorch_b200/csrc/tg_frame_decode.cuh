@@ -1,7 +1,8 @@
 // The per-pixel decode of streamed frames, shared by the frame-input launches of tg_stream.cu and the resizing frame
 // input of tg_resample.cu: the frame layouts (uint8 HWC; YUV 4:2:0 NV12 / I420 / P010 / I420_10, packed 4:2:2 YUY2 /
-// UYVY, planar 4:4:4 I444 / I444_10, 10-bit 4:2:2 P210 / I422_10 / v210), the fixed-point colour table, the row decoders of the frame-input CTAs and the
-// per-pixel sample fetch of any layout, the picture-window check and the format dispatch.  Every decoder computes the
+// UYVY, planar 4:4:4 I444 / I444_10, 10-bit 4:2:2 P210 / I422_10 / v210) and what each of them is (Yuv), the
+// fixed-point colour table, the row decoders of the frame-input CTAs and the per-pixel sample fetch of any layout,
+// the frame and picture-window check and the format dispatch.  Every decoder computes the
 // same fp32 value of a pixel: float(code) / 255 (8 bit) or / 1023 (10 bit) by IEEE division.
 // Contract: include/tecogan_b200.h (tg_yuv_format, tg_frame_window, tg_stream_frame_in*).
 #pragma once
@@ -12,7 +13,7 @@
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kTilePx = 256;            // decode / encode CTA: kTilePx pixels of a row, one per thread
+constexpr int kTilePx = 256;            // decode / encode CTA: kTilePx pixels (or units) of a row, one per thread
 constexpr int kMaxC = 4;
 
 enum FrameFormat { kHWC = 0, kNV12 = 1, kI420 = 2, kP010 = 3, kI420_10 = 4, kYUY2 = 5, kUYVY = 6, kI444 = 7,
@@ -26,16 +27,31 @@ constexpr bool fmt_444(int f) { return f == kI444 || f == kI444_10; }     // thr
 constexpr bool fmt_p422(int f) { return f == kP210 || f == kI422_10; }    // 10-bit 4:2:2, [2h, w] uint16 words
 constexpr bool fmt_422(int f) { return fmt_packed(f) || fmt_p422(f) || f == kV210; }   // needs an even width
 constexpr bool fmt_420(int f) { return f != kHWC && !fmt_422(f) && !fmt_444(f); }
-// byte of Y0 (Y1 two bytes later) and of U (V two bytes later) in a packed group: YUY2 is Y0 U Y1 V, UYVY U Y0 V Y1
-constexpr int packed_y0(int f) { return f == kUYVY ? 1 : 0; }
-constexpr int packed_u(int f) { return f == kUYVY ? 0 : 1; }
 
+// v210: a row of a frame_w-pixel frame is 128 * ceil(frame_w / 48) bytes, ceil(frame_w / 6) 16-byte groups of 6
+// pixels used.  The 12 fields of a group, f = 3 * word + k at bits 10k of word f / 3, are
+//   Cb0 Y0 Cr0 Y1 Cb2 Y2 Cr2 Y3 Cb4 Y4 Cr4 Y5:
+// Y of pixel j at field 2j + 1, Cb / Cr of pair p (pixels 2p, 2p + 1) at fields 4p / 4p + 2.
+__host__ __device__ constexpr size_t v210_stride(int fw) { return (size_t)128 * ((fw + 47) / 48); }
+
+// What a frame layout is: its words, chroma grid, alignment and where the Y, U and V samples of a pixel live.  The
+// layout predicates above are read here only.
 template <int kFmt>
 struct Yuv {
-  static constexpr bool kInterleaved = kFmt == kNV12 || kFmt == kP010;     // NV12 plane layout
-  static constexpr bool k10 = fmt_10(kFmt);
+  static constexpr bool k420 = fmt_420(kFmt), k422 = fmt_422(kFmt), k10 = fmt_10(kFmt);
+  // packed 4:2:2 and v210 store a row as aligned groups of 32-bit words (a pair in 4 bytes, 6 pixels in 16); the
+  // planar layouts store a Y plane and the chroma of the grid, U and V interleaved (kSemi) or in two planes
+  static constexpr bool kGrouped = fmt_packed(kFmt) || kFmt == kV210;
+  static constexpr bool kSemi = kFmt == kNV12 || kFmt == kP010 || kFmt == kP210;
+  // the chroma grid: pixels that share one U, V sample (v210: the 6 pixels of a group, 3 pairs), and the pixels of
+  // a row one thread of the row kernels owns (4:2:0: one pixel of each of two rows; else a pixel, a pair or a group)
+  static constexpr int kGy = k420 ? 2 : 1;
+  static constexpr int kGx = kFmt == kV210 ? 6 : k420 || k422 ? 2 : 1;
+  static constexpr int kUnitPx = k420 || kFmt == kHWC ? 1 : kGx;
   // v210 packs its 10-bit samples into the 32-bit words of 16-byte groups: its frames are addressed in bytes
   using Word = typename std::conditional<k10 && kFmt != kV210, uint16_t, uint8_t>::type;
+  // the widest access of a frame's unit: the group (packed 4:2:2, v210) or a word
+  static constexpr int kAlign = kFmt == kV210 ? 16 : fmt_packed(kFmt) ? 4 : (int)sizeof(Word);
   static constexpr int kShift = k10 ? 18 : 20;                              // fraction bits of the table row
   static constexpr int kTop = k10 ? 1023 : 255;
   static constexpr int kCoff = k10 ? 512 : 128;
@@ -47,6 +63,43 @@ struct Yuv {
                                                                                              : (int)v;
   }
   static __device__ __forceinline__ Word word(int v) { return (Word)(kHigh ? v << 6 : v); }
+
+  // words of one fh x fw frame (kHWC: c bytes a pixel)
+  static __host__ __device__ size_t frame_words(int c, int fh, int fw) {
+    if (kFmt == kHWC) return (size_t)fh * fw * c;
+    if (kGrouped) return (size_t)fh * row_bytes(fw);
+    return (size_t)fh * fw + 2 * (size_t)(fh / kGy) * (fw / kGx);
+  }
+  // planar: word offsets in its frame of pixel (y, x)'s Y, and of the U and V it takes (nearest chroma): the offset
+  // of its chroma sample in a chroma plane (chroma_at) plus that of the U or V plane (u_plane / v_plane, the same
+  // for every pixel of a frame)
+  static __device__ __forceinline__ size_t y_at(int fw, int y, int x) { return (size_t)y * fw + x; }
+  static __device__ __forceinline__ size_t chroma_at(int fw, int y, int x) {
+    const unsigned cy = (unsigned)y / kGy, cx = (unsigned)x / kGx;   // coordinates are non-negative
+    return kSemi ? (size_t)cy * fw + 2 * cx : (size_t)cy * ((unsigned)fw / kGx) + cx;
+  }
+  static __host__ __device__ size_t u_plane(int fh, int fw) { return (size_t)fh * fw; }
+  static __host__ __device__ size_t v_plane(int fh, int fw) {
+    return u_plane(fh, fw) + (kSemi ? 1 : (size_t)((unsigned)fh / kGy) * ((unsigned)fw / kGx));
+  }
+  // grouped: bytes of a row, the byte offset of the group holding pixel (y, x) of frame img, and the fields of a
+  // group: Y of its pixel j, U and V of its pair p.  A field is byte f of the group (packed: YUY2 is Y0 U Y1 V, UYVY
+  // U Y0 V Y1) or the 10-bit field f (v210)
+  static __host__ __device__ size_t row_bytes(int fw) { return kFmt == kV210 ? v210_stride(fw) : (size_t)2 * fw; }
+  static __device__ __forceinline__ size_t group_at(int fh, int fw, int img, int y, int x) {
+    return ((size_t)img * fh + y) * row_bytes(fw) + (size_t)(x / kGx) * kAlign;
+  }
+  static constexpr int kFieldBits = kFmt == kV210 ? 10 : 8, kFieldsPerWord = kFmt == kV210 ? 3 : 4;
+  static constexpr int y_field(int j) { return kFmt == kV210 ? 2 * j + 1 : (kFmt == kUYVY ? 1 : 0) + 2 * j; }
+  static constexpr int u_field(int p) { return kFmt == kV210 ? 4 * p : kFmt == kUYVY ? 0 : 1; }
+  static constexpr int v_field(int p) { return u_field(p) + 2; }
+  // field f of a group whose word f / kFieldsPerWord is w, and the bits of value v at field f
+  static __device__ __forceinline__ int field(uint32_t w, int f) {
+    return (int)((w >> (kFieldBits * (f % kFieldsPerWord))) & ((1u << kFieldBits) - 1));
+  }
+  static __device__ __forceinline__ uint32_t field_bits(int f, int v) {
+    return (uint32_t)v << (kFieldBits * (f % kFieldsPerWord));
+  }
 };
 
 // The colour table (oracle/yuv_color.py derives the same numbers): [depth 8 / 10][colour][16] with colour
@@ -105,18 +158,9 @@ static_assert(kYuvTable.v[0][0][14] == Yuv<kYUY2>::kShift && kYuvTable.v[0][3][1
 static_assert(Yuv<kYUY2>::kTop == 255 && Yuv<kUYVY>::kCoff == 128 && Yuv<kI444>::kTop == 255 &&
                   Yuv<kI444_10>::kTop == 1023 && Yuv<kI444_10>::kCoff == 512 && Yuv<kI444_10>::k10,
               "4:2:2 is 8 bit only, I444_10 is the 10-bit table row");
-static_assert(!Yuv<kYUY2>::kInterleaved && !Yuv<kUYVY>::kInterleaved && !Yuv<kI444>::kInterleaved &&
-                  !Yuv<kI444_10>::kInterleaved, "4:2:2 and 4:4:4 frames have no NV12 chroma plane");
 static_assert(Yuv<kP210>::kShift == 18 && Yuv<kI422_10>::kTop == 1023 && Yuv<kV210>::kCoff == 512 &&
-                  sizeof(Yuv<kP210>::Word) == 2 && sizeof(Yuv<kV210>::Word) == 1 && !Yuv<kP210>::kInterleaved,
+                  sizeof(Yuv<kP210>::Word) == 2 && sizeof(Yuv<kV210>::Word) == 1,
               "10-bit 4:2:2 is the 10-bit table row; v210 frames are bytes");
-
-// v210: a row of a frame_w-pixel frame is 128 * ceil(frame_w / 48) bytes, ceil(frame_w / 6) 16-byte groups of 6
-// pixels used.  The 12 fields of a group, f = 3 * word + k at bits 10k of word f / 3, are
-//   Cb0 Y0 Cr0 Y1 Cb2 Y2 Cr2 Y3 Cb4 Y4 Cr4 Y5:
-// Y of pixel j at field 2j + 1, Cb / Cr of pair p (pixels 2p, 2p + 1) at fields 4p / 4p + 2.
-__host__ __device__ constexpr size_t v210_stride(int fw) { return (size_t)128 * ((fw + 47) / 48); }
-__device__ __forceinline__ int v210_field(const uint32_t* g, int f) { return (int)((g[f / 3] >> (10 * (f % 3))) & 1023u); }
 
 // zero floats [0, count) of p (4-byte aligned): 16-byte stores over the aligned interior, at most three
 // scalar stores at each end.  `worker` of `workers` threads; writes nothing outside the range.
@@ -176,71 +220,8 @@ __device__ __forceinline__ void decode_hwc(const uint8_t* __restrict__ in, float
   }
 }
 
-// decode CTA of YUV 4:2:0 frames ([3h/2, w] words each): kTilePx pixels of the luma rows 2*yp and 2*yp + 1 and
-// the chroma samples they share (nearest chroma), written as RGB / 255 (8 bit) or RGB / 1023 (10 bit).  Colour
-// row `color` of the table; with the 8-bit bt601 row this is cv2 COLOR_YUV2RGB_NV12 / _I420 bit for bit.
-template <int kFmt>
-__device__ __forceinline__ void decode_yuv420(const uint8_t* __restrict__ in, float* __restrict__ lr_curr, int b,
-                                              int t, int h, int w, tg_frame_window win, int x_tiles, int color) {
-  using F = Yuv<kFmt>;
-  using W = typename F::Word;
-  constexpr int kB = (int)sizeof(W);
-  __shared__ __align__(16) uint8_t sy[2][kTilePx * kB + 16];
-  __shared__ __align__(16) uint8_t sc[2][kTilePx * kB + 16];   // NV12 layout: sc[0] = U V U V ...; I420: U, V
-  const int xt = b % x_tiles, r = b / x_tiles;
-  const int hp = h >> 1, yp = r % hp, img = r / hp;
-  const int x0 = xt * kTilePx;
-  const int npx = min(kTilePx, w - x0);                      // even: w and x0 are
-  const int fh = win.frame_h, fw = win.frame_w;              // even, as are top and left
-  const int fx = win.left + x0, fyp = (win.top >> 1) + yp;   // the tile's column and row pair in the frame
-  const W* frame = reinterpret_cast<const W*>(in) + (size_t)img * (3 * (fh >> 1)) * fw;
-  const W* yrow = frame + (size_t)(2 * fyp) * fw + fx;
-  const W* crow = frame + (size_t)fh * fw;                   // chroma of the frame
-  const uint8_t* ysrc = reinterpret_cast<const uint8_t*>(yrow);
-  const uint8_t* csrc = reinterpret_cast<const uint8_t*>(crow);
-  const uint8_t* c0 = csrc + (F::kInterleaved ? (size_t)fyp * fw + fx : (size_t)fyp * (fw >> 1) + (fx >> 1)) * kB;
-  const uint8_t* c1 = c0 + (size_t)(fh >> 1) * (fw >> 1) * kB;   // I420 layout: the V sample of the same block
-  stage_bytes(sy[0], ysrc, npx * kB, t);
-  stage_bytes(sy[1], ysrc + (size_t)fw * kB, npx * kB, t);
-  if (F::kInterleaved) {
-    stage_bytes(sc[0], c0, npx * kB, t);
-  } else {
-    stage_bytes(sc[0], c0, (npx >> 1) * kB, t);
-    stage_bytes(sc[1], c1, (npx >> 1) * kB, t);
-  }
-  __syncthreads();
-  if (t >= npx) return;
-  // the staged words start at the sources' offsets within 16 bytes (cheaper to recompute than to keep live)
-  const int ly0 = lead_of(ysrc), ly1 = lead_of(ysrc + (size_t)fw * kB), lc0 = lead_of(c0);
-  const int lc1 = F::kInterleaved ? 0 : lead_of(c1);
-  // the leads are multiples of the word size: sources are word aligned
-  const auto at = [](const uint8_t* sb, int lead, int j) { return F::sample(reinterpret_cast<const W*>(sb + lead)[j]); };
-  const int j = t >> 1;
-  const int u = F::kInterleaved ? at(sc[0], lc0, 2 * j) : at(sc[0], lc0, j);
-  const int v = F::kInterleaved ? at(sc[0], lc0, 2 * j + 1) : at(sc[1], lc1, j);
-  const int* k = c_yuv.v[F::k10][color];
-  constexpr int kHalf = 1 << (F::kShift - 1);
-  const int ruv = kHalf + k[13] * (v - F::kCoff);
-  const int guv = kHalf + k[12] * (v - F::kCoff) + k[11] * (u - F::kCoff);
-  const int buv = kHalf + k[10] * (u - F::kCoff);
-  const int cy = k[9], yoff = k[15];
-  const bool cv2_clamp = !F::k10 && color == 0;              // cv2: max(Y - 16, 0) before the multiply
-  constexpr float kScale = F::k10 ? 1023.f : 255.f;
-  auto rgb = [](int a) { return __fdiv_rn((float)min(max(a >> F::kShift, 0), F::kTop), kScale); };
-  const size_t plane = (size_t)h * w;
-  float* dst = lr_curr + (size_t)img * 3 * plane + (size_t)(2 * yp) * w + x0 + t;
-#pragma unroll
-  for (int dy = 0; dy < 2; ++dy) {
-    int yv = at(sy[dy], dy ? ly1 : ly0, t) - yoff;
-    if (cv2_clamp) yv = max(yv, 0);
-    const int yy = yv * cy;
-    dst[dy * w] = rgb(yy + ruv);
-    dst[dy * w + plane] = rgb(yy + guv);
-    dst[dy * w + 2 * plane] = rgb(yy + buv);
-  }
-}
-
-// one pixel's RGB from its Y and the (U, V) it takes, colour row `color`: the per-pixel rule of decode_yuv420
+// one pixel's RGB from its Y and the (U, V) it takes, colour row `color` of the table.  With the 8-bit bt601 row
+// this is cv2's COLOR_YUV2RGB_* bit for bit.
 template <int kFmt>
 struct YuvDecode {
   using F = Yuv<kFmt>;
@@ -277,60 +258,144 @@ struct YuvDecode {
   }
 };
 
+// decode CTA of YUV 4:2:0 frames ([3h/2, w] words each): kTilePx pixels of the luma rows 2*yp and 2*yp + 1 and
+// the chroma samples they share (nearest chroma), written as RGB / 255 (8 bit) or RGB / 1023 (10 bit).  Colour
+// row `color` of the table; with the 8-bit bt601 row this is cv2 COLOR_YUV2RGB_NV12 / _I420 bit for bit.
+template <int kFmt>
+__device__ __forceinline__ void decode_yuv420(const uint8_t* __restrict__ in, float* __restrict__ lr_curr, int b,
+                                              int t, int h, int w, tg_frame_window win, int x_tiles, int color) {
+  using F = Yuv<kFmt>;
+  using W = typename F::Word;
+  constexpr int kB = (int)sizeof(W);
+  __shared__ __align__(16) uint8_t sy[2][kTilePx * kB + 16];
+  __shared__ __align__(16) uint8_t sc[2][kTilePx * kB + 16];   // NV12 layout: sc[0] = U V U V ...; I420: U, V
+  const int xt = b % x_tiles, r = b / x_tiles;
+  const int hp = h >> 1, yp = r % hp, img = r / hp;
+  const int x0 = xt * kTilePx;
+  const int npx = min(kTilePx, w - x0);                      // even: w and x0 are
+  const int fh = win.frame_h, fw = win.frame_w;              // even, as are top and left
+  const int fx = win.left + x0, fy = win.top + 2 * yp;       // the tile's column and first row in the frame
+  const W* frame = reinterpret_cast<const W*>(in) + (size_t)img * F::frame_words(3, fh, fw);
+  const uint8_t* ysrc = reinterpret_cast<const uint8_t*>(frame + F::y_at(fw, fy, fx));
+  const W* chroma = frame + F::chroma_at(fw, fy, fx);
+  const uint8_t* c0 = reinterpret_cast<const uint8_t*>(chroma + F::u_plane(fh, fw));
+  const uint8_t* c1 = reinterpret_cast<const uint8_t*>(chroma + F::v_plane(fh, fw));   // I420 layout
+  stage_bytes(sy[0], ysrc, npx * kB, t);
+  stage_bytes(sy[1], ysrc + (size_t)fw * kB, npx * kB, t);
+  if (F::kSemi) {
+    stage_bytes(sc[0], c0, npx * kB, t);
+  } else {
+    stage_bytes(sc[0], c0, (npx >> 1) * kB, t);
+    stage_bytes(sc[1], c1, (npx >> 1) * kB, t);
+  }
+  __syncthreads();
+  if (t >= npx) return;
+  // the staged words start at the sources' offsets within 16 bytes (cheaper to recompute than to keep live)
+  const int ly0 = lead_of(ysrc), ly1 = lead_of(ysrc + (size_t)fw * kB), lc0 = lead_of(c0);
+  const int lc1 = F::kSemi ? 0 : lead_of(c1);
+  // the leads are multiples of the word size: sources are word aligned
+  const auto at = [](const uint8_t* sb, int lead, int j) { return F::sample(reinterpret_cast<const W*>(sb + lead)[j]); };
+  const int j = t >> 1;
+  const int u = F::kSemi ? at(sc[0], lc0, 2 * j) : at(sc[0], lc0, j);
+  const int v = F::kSemi ? at(sc[0], lc0, 2 * j + 1) : at(sc[1], lc1, j);
+  const YuvDecode<kFmt> d(u, v, color);
+  const size_t plane = (size_t)h * w;
+  float* dst = lr_curr + (size_t)img * 3 * plane + (size_t)(2 * yp) * w + x0 + t;
+#pragma unroll
+  for (int dy = 0; dy < 2; ++dy) d.put(dst + dy * w, plane, at(sy[dy], dy ? ly1 : ly0, t));
+}
+
+// The samples of the kUnitPx pixels of a row one thread of the per-unit row kernels owns (packed 4:2:2 and
+// P210 / I422_10: a pair; 4:4:4: a pixel; v210: a 6-pixel group): Y of each pixel, U and V of each pair (4:4:4: of
+// the pixel).  Grouped layouts keep the group's 32-bit words (fields never set are 0), planar ones the samples.
+template <int kFmt>
+struct Unit {
+  using F = Yuv<kFmt>;
+  static constexpr int kPx = F::kUnitPx, kC = kPx > 1 ? kPx / 2 : 1;
+  uint32_t w[F::kGrouped ? F::kAlign / 4 : kPx + 2] = {};
+  __device__ __forceinline__ int get(int f, int i) const {
+    return F::kGrouped ? F::field(w[f / F::kFieldsPerWord], f) : (int)w[i];
+  }
+  __device__ __forceinline__ void set(int f, int i, int v) {
+    if (F::kGrouped) w[f / F::kFieldsPerWord] |= F::field_bits(f, v);
+    else w[i] = (uint32_t)v;
+  }
+  __device__ __forceinline__ int y(int j) const { return get(F::y_field(j), j); }
+  __device__ __forceinline__ int u(int p) const { return get(F::u_field(p), kPx); }
+  __device__ __forceinline__ int v(int p) const { return get(F::v_field(p), kPx + 1); }
+  __device__ __forceinline__ void set_y(int j, int v) { set(F::y_field(j), j, v); }
+  __device__ __forceinline__ void set_uv(int p, int u, int v) {
+    set(F::u_field(p), kPx, u);
+    set(F::v_field(p), kPx + 1, v);
+  }
+};
+
+// the unit whose first pixel is (y, x) of frame img (fh x fw pixels): one 4-byte (packed 4:2:2) or 16-byte (v210)
+// load of its group, or one word of each plane per sample
+template <int kFmt>
+__device__ __forceinline__ Unit<kFmt> load_unit(const uint8_t* __restrict__ in, int fh, int fw, int img, int y, int x) {
+  using F = Yuv<kFmt>;
+  Unit<kFmt> q;
+  if constexpr (kFmt == kV210) {
+    const uint4 a = __ldg(reinterpret_cast<const uint4*>(in + F::group_at(fh, fw, img, y, x)));
+    q.w[0] = a.x, q.w[1] = a.y, q.w[2] = a.z, q.w[3] = a.w;
+  } else if constexpr (F::kGrouped) {
+    q.w[0] = __ldg(reinterpret_cast<const uint32_t*>(in + F::group_at(fh, fw, img, y, x)));
+  } else {
+    const typename F::Word* f = reinterpret_cast<const typename F::Word*>(in) + (size_t)img * F::frame_words(3, fh, fw);
+#pragma unroll
+    for (int j = 0; j < q.kPx; ++j) q.set_y(j, F::sample(__ldg(f + F::y_at(fw, y, x + j))));
+    const typename F::Word* c = f + F::chroma_at(fw, y, x);
+    q.set_uv(0, F::sample(__ldg(c + F::u_plane(fh, fw))), F::sample(__ldg(c + F::v_plane(fh, fw))));
+  }
+  return q;
+}
+
+// decode CTA of the per-unit layouts (packed 4:2:2, 4:4:4, 10-bit 4:2:2): kTilePx units of one row, one per thread;
+// every pixel takes its pair's U and V (nearest chroma).  The pixels past w of a partial last v210 group are not
+// written.  The frames are aligned to their group and the picture starts on one (the launch checks).
+template <int kFmt>
+__device__ __forceinline__ void decode_units(const uint8_t* __restrict__ in, float* __restrict__ lr_curr, int b, int t,
+                                             int h, int w, tg_frame_window win, int x_tiles, int color) {
+  using U = Unit<kFmt>;
+  const int xt = b % x_tiles, r = b / x_tiles;
+  const int y = r % h, img = r / h;
+  const int x0 = (xt * kTilePx + t) * U::kPx;
+  if (x0 >= w) return;
+  const U q = load_unit<kFmt>(in, win.frame_h, win.frame_w, img, win.top + y, win.left + x0);
+  const size_t plane = (size_t)h * w;
+  float* dst = lr_curr + (size_t)img * 3 * plane + (size_t)y * w + x0;
+#pragma unroll
+  for (int p = 0; p < U::kC; ++p) {
+    if (x0 + 2 * p >= w) break;                      // w is even: a pair is whole or absent
+    const YuvDecode<kFmt> d(q.u(p), q.v(p), color);
+#pragma unroll
+    for (int j = 0; j < U::kPx / U::kC; ++j) d.put(dst + 2 * p + j, plane, q.y(2 * p + j));
+  }
+}
+
 // The samples (Y, U, V) of pixel (y, x) of frame `img` of n stored frames of layout kFmt (YUV), win.frame_h x
-// win.frame_w pixels each; y and x count in the frame (the picture's offset added).  Nearest chroma: the sample of
-// the 2x2 block (4:2:0) or of the pixel pair (4:2:2) the pixel lies in, as the row decoders above take it.
+// win.frame_w pixels each; y and x count in the frame (the picture's offset added).  Nearest chroma, as the row
+// decoders above take it.
 template <int kFmt>
 __device__ __forceinline__ void yuv_samples(const uint8_t* __restrict__ in, tg_frame_window win, int img, int y, int x,
                                             int& Y, int& U, int& V) {
   using F = Yuv<kFmt>;
-  using W = typename F::Word;
   const int fh = win.frame_h, fw = win.frame_w;
-  if constexpr (fmt_packed(kFmt)) {
-    const uint32_t g = __ldg(reinterpret_cast<const uint32_t*>(in) + ((size_t)img * fh + y) * (fw >> 1) + (x >> 1));
-    const auto byte = [g](int k) { return (int)((g >> (8 * k)) & 255u); };
-    Y = byte(packed_y0(kFmt) + 2 * (x & 1));
-    U = byte(packed_u(kFmt));
-    V = byte(packed_u(kFmt) + 2);
-  } else if constexpr (kFmt == kV210) {
-    const uint32_t* g = reinterpret_cast<const uint32_t*>(in + ((size_t)img * fh + y) * v210_stride(fw)) + 4 * (x / 6);
-    const int j = x % 6, p = j >> 1;
-    const auto field = [g](int f) { return (int)((__ldg(g + f / 3) >> (10 * (f % 3))) & 1023u); };
-    Y = field(2 * j + 1);
-    U = field(4 * p);
-    V = field(4 * p + 2);
-  } else if constexpr (fmt_p422(kFmt)) {
-    const size_t fplane = (size_t)fh * fw;
-    const W* frame = reinterpret_cast<const W*>(in) + (size_t)img * 2 * fplane;
-    Y = F::sample(__ldg(frame + (size_t)y * fw + x));
-    if (kFmt == kP210) {
-      const W* c = frame + fplane + (size_t)y * fw + (x & ~1);
-      U = F::sample(__ldg(c));
-      V = F::sample(__ldg(c + 1));
-    } else {
-      const W* c = frame + fplane + (size_t)y * (fw >> 1) + (x >> 1);
-      U = F::sample(__ldg(c));
-      V = F::sample(__ldg(c + fplane / 2));
-    }
-  } else if constexpr (fmt_444(kFmt)) {
-    const size_t fplane = (size_t)fh * fw;
-    const W* src = reinterpret_cast<const W*>(in) + (size_t)img * 3 * fplane + (size_t)y * fw + x;
-    Y = F::sample(__ldg(src));
-    U = F::sample(__ldg(src + fplane));
-    V = F::sample(__ldg(src + 2 * fplane));
+  if constexpr (F::kGrouped) {
+    // one load of a packed group; the words of a v210 group that hold the three fields
+    const uint32_t* g = reinterpret_cast<const uint32_t*>(in + F::group_at(fh, fw, img, y, x));
+    const int j = x % F::kGx;
+    const auto get = [g](int f) { return F::field(__ldg(g + f / F::kFieldsPerWord), f); };
+    Y = get(F::y_field(j));
+    U = get(F::u_field(j >> 1));
+    V = get(F::v_field(j >> 1));
   } else {
-    const W* frame = reinterpret_cast<const W*>(in) + (size_t)img * (3 * (fh >> 1)) * fw;
-    const W* chroma = frame + (size_t)fh * fw;
-    Y = F::sample(__ldg(frame + (size_t)y * fw + x));
-    if (F::kInterleaved) {
-      const W* c = chroma + (size_t)(y >> 1) * fw + (x & ~1);
-      U = F::sample(__ldg(c));
-      V = F::sample(__ldg(c + 1));
-    } else {
-      const W* c = chroma + (size_t)(y >> 1) * (fw >> 1) + (x >> 1);
-      U = F::sample(__ldg(c));
-      V = F::sample(__ldg(c + (size_t)(fh >> 1) * (fw >> 1)));
-    }
+    const typename F::Word* f = reinterpret_cast<const typename F::Word*>(in) + (size_t)img * F::frame_words(3, fh, fw);
+    Y = F::sample(__ldg(f + F::y_at(fw, y, x)));
+    const typename F::Word* c = f + F::chroma_at(fw, y, x);
+    U = F::sample(__ldg(c + F::u_plane(fh, fw)));
+    V = F::sample(__ldg(c + F::v_plane(fh, fw)));
   }
 }
 
@@ -353,116 +418,31 @@ __device__ __forceinline__ void decode_pixel(const uint8_t* __restrict__ in, tg_
   }
 }
 
-// decode CTA of packed 4:2:2 frames ([h, 2w] bytes each): kTilePx pixel pairs of one row, one 4-byte group per
-// thread; both pixels of a pair take its U and V (nearest chroma).  With the 8-bit bt601 row this is cv2
-// COLOR_YUV2RGB_YUY2 / _UYVY bit for bit.  The frames are 4-byte aligned (the launch checks).
+// The frames an h x w picture of layout kFmt is read from or written to, at `win` (nullptr: the whole frame), by a
+// kernel whose widest access of the frames at p is `align` bytes: TG_E_UNSUPPORTED for a picture off the chroma
+// grid (4:2:0: even height and width; 4:2:2: even width), TG_E_INVALID for misaligned frames, and for a window
+// (checked when p is given) TG_E_INVALID outside the frame, TG_E_UNSUPPORTED off the chroma grid (4:2:0: even frame
+// size, top and left; 4:2:2: even frame width and left; v210: the picture starts on a 6-pixel group and ends on
+// one or at the frame's right edge).  `what` names the frames in the messages.
 template <int kFmt>
-__device__ __forceinline__ void decode_yuv422(const uint8_t* __restrict__ in, float* __restrict__ lr_curr, int b,
-                                              int t, int h, int w, tg_frame_window win, int x_tiles, int color) {
+int check_frames(const char* name, const void* p, int h, int w, const tg_frame_window* win, int align,
+                 const char* what = "frames") {
   using F = Yuv<kFmt>;
-  const int xt = b % x_tiles, r = b / x_tiles;
-  const int y = r % h, img = r / h;
-  const int pair = xt * kTilePx + t;
-  if (pair >= (w >> 1)) return;
-  const size_t frow = (size_t)img * win.frame_h + win.top + y;   // frame_w and left are even
-  const uint32_t g =
-      __ldg(reinterpret_cast<const uint32_t*>(in) + frow * (win.frame_w >> 1) + (win.left >> 1) + pair);
-  const auto byte = [g](int k) { return (int)((g >> (8 * k)) & 255u); };
-  const YuvDecode<kFmt> d(byte(packed_u(kFmt)), byte(packed_u(kFmt) + 2), color);
-  const size_t plane = (size_t)h * w;
-  float* dst = lr_curr + (size_t)img * 3 * plane + (size_t)y * w + 2 * pair;
-  d.put(dst, plane, byte(packed_y0(kFmt)));
-  d.put(dst + 1, plane, byte(packed_y0(kFmt) + 2));
-}
-
-// decode CTA of planar 4:4:4 frames ([3h, w] words each: the Y, U and V planes): kTilePx pixels of one row, one
-// sample of each plane per thread (coalesced word loads)
-template <int kFmt>
-__device__ __forceinline__ void decode_yuv444(const uint8_t* __restrict__ in, float* __restrict__ lr_curr, int b,
-                                              int t, int h, int w, tg_frame_window win, int x_tiles, int color) {
-  using F = Yuv<kFmt>;
-  using W = typename F::Word;
-  const int xt = b % x_tiles, r = b / x_tiles;
-  const int y = r % h, img = r / h;
-  const int x = xt * kTilePx + t;
-  if (x >= w) return;
-  const size_t plane = (size_t)h * w, fplane = (size_t)win.frame_h * win.frame_w;
-  const W* src = reinterpret_cast<const W*>(in) + (size_t)img * 3 * fplane + (size_t)(win.top + y) * win.frame_w +
-                 win.left + x;
-  const YuvDecode<kFmt> d(F::sample(__ldg(src + fplane)), F::sample(__ldg(src + 2 * fplane)), color);
-  d.put(lr_curr + (size_t)img * 3 * plane + (size_t)y * w + x, plane, F::sample(__ldg(src)));
-}
-
-// decode CTA of planar 10-bit 4:2:2 frames ([2h, w] uint16 words each: the Y plane, then P210's interleaved UV plane
-// of h x w or I422_10's U and V planes of h x w/2): kTilePx pixel pairs of one row, one pair per thread; both
-// pixels take the pair's U and V (nearest chroma)
-template <int kFmt>
-__device__ __forceinline__ void decode_yuv422_10(const uint8_t* __restrict__ in, float* __restrict__ lr_curr, int b,
-                                                 int t, int h, int w, tg_frame_window win, int x_tiles, int color) {
-  using F = Yuv<kFmt>;
-  using W = typename F::Word;
-  const int xt = b % x_tiles, r = b / x_tiles;
-  const int y = r % h, img = r / h;
-  const int pair = xt * kTilePx + t;
-  if (pair >= (w >> 1)) return;
-  const int fw = win.frame_w, fy = win.top + y, fx = win.left + 2 * pair;   // frame_w and left are even
-  const size_t fplane = (size_t)win.frame_h * fw;
-  const W* frame = reinterpret_cast<const W*>(in) + (size_t)img * 2 * fplane;
-  const W* ys = frame + (size_t)fy * fw + fx;
-  int u, v;
-  if (kFmt == kP210) {
-    const W* c = frame + fplane + (size_t)fy * fw + fx;
-    u = F::sample(__ldg(c));
-    v = F::sample(__ldg(c + 1));
-  } else {
-    const W* c = frame + fplane + (size_t)fy * (fw >> 1) + (fx >> 1);
-    u = F::sample(__ldg(c));
-    v = F::sample(__ldg(c + fplane / 2));
-  }
-  const YuvDecode<kFmt> d(u, v, color);
-  const size_t plane = (size_t)h * w;
-  float* dst = lr_curr + (size_t)img * 3 * plane + (size_t)y * w + 2 * pair;
-  d.put(dst, plane, F::sample(__ldg(ys)));
-  d.put(dst + 1, plane, F::sample(__ldg(ys + 1)));
-}
-
-// decode CTA of v210 frames ([h, v210_stride(frame_w)] bytes each): kTilePx 16-byte groups of one row, one group
-// (6 pixels, 3 pairs) per thread with one 16-byte load; the pixels past w of a partial last group are not written.
-// The frames are 16-byte aligned and the picture starts on a group (the launch checks).
-__device__ __forceinline__ void decode_v210(const uint8_t* __restrict__ in, float* __restrict__ lr_curr, int b, int t,
-                                            int h, int w, tg_frame_window win, int x_tiles, int color) {
-  const int xt = b % x_tiles, r = b / x_tiles;
-  const int y = r % h, img = r / h;
-  const int grp = xt * kTilePx + t;
-  const int x0 = 6 * grp;
-  if (x0 >= w) return;
-  const size_t frow = (size_t)img * win.frame_h + win.top + y;
-  const uint4 q = __ldg(reinterpret_cast<const uint4*>(in + frow * v210_stride(win.frame_w)) + win.left / 6 + grp);
-  const uint32_t g[4] = {q.x, q.y, q.z, q.w};
-  const size_t plane = (size_t)h * w;
-  float* dst = lr_curr + (size_t)img * 3 * plane + (size_t)y * w + x0;
-#pragma unroll
-  for (int p = 0; p < 3; ++p) {
-    if (x0 + 2 * p >= w) break;                      // w is even: a pair is whole or absent
-    const YuvDecode<kV210> d(v210_field(g, 4 * p), v210_field(g, 4 * p + 2), color);
-    d.put(dst + 2 * p, plane, v210_field(g, 4 * p + 1));
-    d.put(dst + 2 * p + 1, plane, v210_field(g, 4 * p + 3));
-  }
-}
-
-// A window of an h x w picture in frames of layout kFmt: TG_E_INVALID outside the frame, TG_E_UNSUPPORTED off the
-// chroma grid (4:2:0: even frame size, top and left; 4:2:2: even frame width and left; v210: the picture starts on
-// a 6-pixel group and ends on one or at the frame's right edge)
-template <int kFmt>
-int check_window(const char* name, const tg_frame_window* win, int h, int w) {
-  TG_REQUIRE(win, TG_E_INVALID, "%s: null window", name);
+  TG_REQUIRE(!F::k420 || (h % 2 == 0 && w % 2 == 0), TG_E_UNSUPPORTED,
+             "%s: YUV 4:2:0 needs an even height and width, got %dx%d", name, h, w);
+  TG_REQUIRE(!F::k422 || w % 2 == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name, w);
+  const uintptr_t a = (uintptr_t)p;
+  TG_REQUIRE(!F::k10 || (a & 1u) == 0, TG_E_INVALID, "%s: 10-bit %s must be 2-byte aligned", name, what);
+  TG_REQUIRE(!F::kGrouped || (a & (uintptr_t)(align - 1)) == 0, TG_E_INVALID, "%s: %s %s must be %d-byte aligned",
+             name, kFmt == kV210 ? "v210" : "packed 4:2:2", what, align);
+  if (!p || !win) return TG_OK;
   const long long fh = win->frame_h, fw = win->frame_w, top = win->top, left = win->left;
   TG_REQUIRE(fh > 0 && fw > 0 && top >= 0 && left >= 0 && top + h <= fh && left + w <= fw, TG_E_INVALID,
              "%s: a %dx%d picture at (%lld, %lld) does not fit a %lldx%lld frame", name, h, w, top, left, fh, fw);
-  TG_REQUIRE(!fmt_420(kFmt) || ((fh | fw | top | left) & 1) == 0, TG_E_UNSUPPORTED,
+  TG_REQUIRE(!F::k420 || ((fh | fw | top | left) & 1) == 0, TG_E_UNSUPPORTED,
              "%s: YUV 4:2:0 needs an even frame size, top and left, got %lldx%lld at (%lld, %lld)", name, fh, fw, top,
              left);
-  TG_REQUIRE(!fmt_422(kFmt) || ((fw | left) & 1) == 0, TG_E_UNSUPPORTED,
+  TG_REQUIRE(!F::k422 || ((fw | left) & 1) == 0, TG_E_UNSUPPORTED,
              "%s: YUV 4:2:2 needs an even frame width and left, got width %lld at column %lld", name, fw, left);
   TG_REQUIRE(kFmt != kV210 || (left % 6 == 0 && ((left + w) % 6 == 0 || left + w == fw)), TG_E_UNSUPPORTED,
              "%s: a v210 picture of width %d at column %lld of a %lld-wide frame must start on a 6-pixel group and "

@@ -373,22 +373,13 @@ int launch_frame_in_resample(const char* name, const void* in, const tg_frame_wi
   TG_REQUIRE(n > 0 && c > 0 && h > 0 && w > 0 && hn > 0 && wn > 0, TG_E_INVALID,
              "%s: bad size n=%d c=%d %dx%d -> %dx%d", name, n, c, h, w, hn, wn);
   TG_REQUIRE(c <= kMaxC, TG_E_UNSUPPORTED, "%s: %d channels (at most %d)", name, c, kMaxC);
-  TG_REQUIRE(!fmt_420(kFmt) || (h % 2 == 0 && w % 2 == 0), TG_E_UNSUPPORTED,
-             "%s: YUV 4:2:0 needs an even height and width, got %dx%d", name, h, w);
-  TG_REQUIRE(!fmt_422(kFmt) || w % 2 == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name, w);
   TG_REQUIRE(s == 2 || s == 4, TG_E_UNSUPPORTED, "%s: scale %d (2 or 4)", name, s);
   TG_REQUIRE((((uintptr_t)lr_curr | (uintptr_t)lr_prev | (uintptr_t)hr_prev | (uintptr_t)row_first |
                (uintptr_t)row_w | (uintptr_t)col_first | (uintptr_t)col_w) & 3u) == 0,
              TG_E_INVALID, "%s: fp32 buffers and the tables must be 4-byte aligned", name);
-  TG_REQUIRE(!fmt_10(kFmt) || ((uintptr_t)in & 1u) == 0, TG_E_INVALID, "%s: 10-bit frames must be 2-byte aligned",
-             name);
-  TG_REQUIRE(!fmt_packed(kFmt) || ((uintptr_t)in & 3u) == 0, TG_E_INVALID,
-             "%s: packed 4:2:2 frames must be 4-byte aligned", name);
-  TG_REQUIRE(kFmt != kV210 || ((uintptr_t)in & 15u) == 0, TG_E_INVALID, "%s: v210 frames must be 16-byte aligned",
-             name);
+  int rc = check_frames<kFmt>(name, in, h, w, win, Yuv<kFmt>::kAlign);
   const tg_frame_window whole = {h, w, 0, 0};
   if (!win) win = &whole;
-  int rc = check_window<kFmt>(name, win, h, w);
   if (rc == TG_OK) rc = check_input_axis(name, "rows", h, hn, row_taps);
   if (rc == TG_OK) rc = check_input_axis(name, "columns", w, wn, col_taps);
   if (rc != TG_OK) return rc;

@@ -13,30 +13,90 @@
 
 namespace {
 
-// Encode rows of 4:2:2 (8 bit): Y per pixel, U and V from the sum of the pair's two pixels,
+// Encode rows of 4:2:2: Y per pixel, U and V from the sum of the pair's two pixels,
 //   Y = clip((kY . rgb + 2^(sy-1) + (yoff << sy)) >> sy)
-//   C = clip((kC . (rgb0 + rgb1) + 2^(sc-1) + (128 << sc)) >> sc)
-// i.e. the chroma of the pair's mean, rounded half up.  [colour][kRY kGY kBY kRU kGU kBU kRV kGV kBV sy sc].  The
-// bt601 row is cv2's COLOR_RGB2YUV_YUY2 / _UYVY (14-bit constants of its own, luma included, with the chroma
-// constants halved for the sum); the derived rows are the table's encode rows with sy = 20 and sc = 21.
-// oracle/yuv_422_444.py specifies the same rule.
+//   C = clip((kC . (rgb0 + rgb1) + 2^(sc-1) + (coff << sc)) >> sc)
+// i.e. the chroma of the pair's mean, rounded half up.  [depth 8 / 10][colour][kRY kGY kBY kRU kGU kBU kRV kGV kBV
+// sy sc].  The 8-bit bt601 row is cv2's COLOR_RGB2YUV_YUY2 / _UYVY (14-bit constants of its own, luma included,
+// with the chroma constants halved for the sum); the other rows are the table's encode rows with sy its shift (20
+// at 8 bits, 18 at 10) and sc = sy + 1.  oracle/yuv_422_444.py and oracle/yuv_422_10.py specify the same rule.
 struct Yuv422Enc {
-  int v[4][11];
+  int v[2][4][11];
 };
 
 constexpr Yuv422Enc make_yuv422_enc() {
   Yuv422Enc e{};
   const int cv2[11] = {4211, 8258, 1606, -1212, -2384, 3596, 3596, -3015, -582, 14, 14};
-  for (int k = 0; k < 11; ++k) e.v[0][k] = cv2[k];
-  for (int ci = 1; ci < 4; ++ci) {
-    for (int k = 0; k < 9; ++k) e.v[ci][k] = kYuvTable.v[0][ci][k];
-    e.v[ci][9] = kYuvTable.v[0][ci][14];
-    e.v[ci][10] = kYuvTable.v[0][ci][14] + 1;
+  for (int di = 0; di < 2; ++di) {
+    for (int ci = 0; ci < 4; ++ci) {
+      int* r = e.v[di][ci];
+      if (di == 0 && ci == 0) {
+        for (int k = 0; k < 11; ++k) r[k] = cv2[k];
+        continue;
+      }
+      for (int k = 0; k < 9; ++k) r[k] = kYuvTable.v[di][ci][k];
+      r[9] = kYuvTable.v[di][ci][14];
+      r[10] = kYuvTable.v[di][ci][14] + 1;
+    }
   }
   return e;
 }
 
 __constant__ Yuv422Enc c_yuv422 = make_yuv422_enc();
+
+// The encode of RGB codes into the samples of layout kFmt, colour row `color`:
+//   Y = clip((kY . rgb + 2^(sy-1) + (yoff << sy)) >> sy),  C = clip((kC . rgb + 2^(sc-1) + (coff << sc)) >> sc)
+// 4:2:0 and 4:4:4 with the table row (sy = sc = its shift), U and V of one pixel (4:2:0: a block's top-left, as cv2
+// COLOR_RGB2YUV_I420); 4:2:2 with the c_yuv422 row, U and V of the sums of a pair's two pixels.
+template <int kFmt>
+struct YuvEncode {
+  using F = Yuv<kFmt>;
+  static constexpr bool kPairSum = F::k422;
+  const int* k;
+  int sy, sc, yo, co;
+  __device__ __forceinline__ explicit YuvEncode(int color) {
+    k = kPairSum ? c_yuv422.v[F::k10][color] : c_yuv.v[F::k10][color];
+    sy = kPairSum ? k[9] : F::kShift;
+    sc = kPairSum ? k[10] : F::kShift;
+    yo = (c_yuv.v[F::k10][color][15] << sy) + (1 << (sy - 1));
+    co = (F::kCoff << sc) + (1 << (sc - 1));
+  }
+  static __device__ __forceinline__ int q(int a, int s) { return min(max(a >> s, 0), F::kTop); }
+  __device__ __forceinline__ int y(int R, int G, int B) const { return q(k[0] * R + k[1] * G + k[2] * B + yo, sy); }
+  __device__ __forceinline__ int u(int R, int G, int B) const { return q(k[3] * R + k[4] * G + k[5] * B + co, sc); }
+  __device__ __forceinline__ int v(int R, int G, int B) const { return q(k[6] * R + k[7] * G + k[8] * B + co, sc); }
+};
+
+// The RGB codes of a row's pixels [x0, x0 + npx) of the encode's source: the step's uint8 NHWC RGB (8-bit output),
+// staged into sb with 16-byte loads (the caller synchronises before reading), or its fp32 NCHW HR frame (kF32,
+// 10-bit output), read per pixel with coalesced row reads of the three planes, q = clip(rint(x * 1023), 0, 1023).
+template <bool kF32>
+struct RgbRow {
+  const void* rgb;
+  const uint8_t* sb;
+  int H, W, img, y, x0, lead = 0;
+  __device__ __forceinline__ RgbRow(const void* rgb_, const uint8_t* sb_, int H_, int W_, int img_, int y_, int x0_)
+      : rgb(rgb_), sb(sb_), H(H_), W(W_), img(img_), y(y_), x0(x0_) {}
+  // stages the uint8 row's npx pixels into sb (thread t of kThreads; the caller synchronises before reading)
+  __device__ __forceinline__ RgbRow(const void* rgb_, uint8_t* sb_, int H_, int W_, int img_, int y_, int x0_, int npx,
+                                    int t)
+      : RgbRow(rgb_, sb_, H_, W_, img_, y_, x0_) {
+    if constexpr (!kF32)
+      lead = stage_bytes(sb_, static_cast<const uint8_t*>(rgb) + (((size_t)img * H + y) * W + x0) * 3, npx * 3, t);
+  }
+  // R, G, B of pixel x0 + j (recomputed per call: cheaper than keeping a row pointer live)
+  __device__ __forceinline__ void operator()(int j, int& R, int& G, int& B) const {
+    if constexpr (kF32) {
+      const size_t plane = (size_t)H * W;
+      const float* f = static_cast<const float*>(rgb) + (size_t)img * 3 * plane + (size_t)y * W + x0 + j;
+      auto q10 = [](float x) { return (int)fminf(fmaxf(rintf(x * 1023.f), 0.f), 1023.f); };
+      R = q10(__ldg(f)), G = q10(__ldg(f + plane)), B = q10(__ldg(f + 2 * plane));
+    } else {
+      const uint8_t* b = sb + lead + 3 * j;
+      R = b[0], G = b[1], B = b[2];
+    }
+  }
+};
 
 // the store counterpart: dst[j] = sb[lead + j] for j < bytes with lead = dst % 16 (the caller placed the bytes
 // there); 16-byte stores over the aligned interior, single bytes at the ends, nothing outside [dst, dst + bytes)
@@ -68,16 +128,10 @@ stream_frame_in_kernel(const uint8_t* __restrict__ in, const int32_t* __restrict
   if (b < decode_ctas) {
     if constexpr (kFmt == kHWC)
       decode_hwc(in, lr_curr, b, t, c, h, w, win, bgr, x_tiles);
-    else if constexpr (fmt_packed(kFmt))
-      decode_yuv422<kFmt>(in, lr_curr, b, t, h, w, win, x_tiles, color);
-    else if constexpr (fmt_444(kFmt))
-      decode_yuv444<kFmt>(in, lr_curr, b, t, h, w, win, x_tiles, color);
-    else if constexpr (fmt_p422(kFmt))
-      decode_yuv422_10<kFmt>(in, lr_curr, b, t, h, w, win, x_tiles, color);
-    else if constexpr (kFmt == kV210)
-      decode_v210(in, lr_curr, b, t, h, w, win, x_tiles, color);
-    else
+    else if constexpr (Yuv<kFmt>::k420)
       decode_yuv420<kFmt>(in, lr_curr, b, t, h, w, win, x_tiles, color);
+    else
+      decode_units<kFmt>(in, lr_curr, b, t, h, w, win, x_tiles, color);
     return;
   }
   const int rb = b - decode_ctas;
@@ -94,33 +148,20 @@ template <int kFmt>
 int launch_frame_in(const char* name, const void* in, const int32_t* reset, float* lr_curr, float* lr_prev,
                     float* hr_prev, int n, int c, int h, int w, const tg_frame_window* win, int s, int bgr, int color,
                     cudaStream_t stream) {
+  using F = Yuv<kFmt>;
   TG_REQUIRE(in || reset, TG_E_INVALID, "%s: in_u8 and reset are both NULL", name);
   TG_REQUIRE(lr_curr && lr_prev && hr_prev, TG_E_INVALID, "%s: null pointer (lr_curr / lr_prev / hr_prev)", name);
   TG_REQUIRE(n > 0 && c > 0 && h > 0 && w > 0, TG_E_INVALID, "%s: bad size n=%d c=%d h=%d w=%d", name, n, c, h, w);
   TG_REQUIRE(c <= kMaxC, TG_E_UNSUPPORTED, "%s: %d channels (at most %d)", name, c, kMaxC);
-  constexpr bool k420 = fmt_420(kFmt);
-  TG_REQUIRE(!k420 || (h % 2 == 0 && w % 2 == 0), TG_E_UNSUPPORTED,
-             "%s: YUV 4:2:0 needs an even height and width, got %dx%d", name, h, w);
-  TG_REQUIRE(!fmt_422(kFmt) || w % 2 == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name,
-             w);
   TG_REQUIRE(s == 2 || s == 4, TG_E_UNSUPPORTED, "%s: scale %d (2 or 4)", name, s);
   TG_REQUIRE((((uintptr_t)lr_curr | (uintptr_t)lr_prev | (uintptr_t)hr_prev) & 3u) == 0, TG_E_INVALID,
              "%s: fp32 buffers must be 4-byte aligned", name);
-  TG_REQUIRE(!fmt_10(kFmt) || ((uintptr_t)in & 1u) == 0, TG_E_INVALID,
-             "%s: 10-bit frames must be 2-byte aligned", name);
-  TG_REQUIRE(!fmt_packed(kFmt) || ((uintptr_t)in & 3u) == 0, TG_E_INVALID,
-             "%s: packed 4:2:2 frames must be 4-byte aligned", name);
-  TG_REQUIRE(kFmt != kV210 || ((uintptr_t)in & 15u) == 0, TG_E_INVALID, "%s: v210 frames must be 16-byte aligned",
-             name);
+  const int rc = check_frames<kFmt>(name, in, h, w, win, F::kAlign);
+  if (rc != TG_OK) return rc;
   const tg_frame_window whole = {h, w, 0, 0};
   if (!win) win = &whole;
-  if (in) {
-    const int rc = check_window<kFmt>(name, win, h, w);
-    if (rc != TG_OK) return rc;
-  }
-  // threads per row: a pixel, a pair (4:2:2) or a 6-pixel group (v210)
-  const int x_tiles = tg_ceil_div(kFmt == kV210 ? tg_ceil_div(w, 6) : fmt_422(kFmt) ? w / 2 : w, kTilePx);
-  const size_t decode = in ? (size_t)x_tiles * (k420 ? h / 2 : h) * n : 0;
+  const int x_tiles = tg_ceil_div(tg_ceil_div(w, F::kUnitPx), kTilePx);
+  const size_t decode = in ? (size_t)x_tiles * (h / F::kGy) * n : 0;
   const size_t hr4 = (size_t)c * s * h * s * w / 4;
   const int zpc = reset ? (int)(hr4 / (kThreads * 8) + 1 < 64 ? hr4 / (kThreads * 8) + 1 : 64) : 0;
   const size_t ctas = decode + (size_t)zpc * n;
@@ -133,16 +174,14 @@ int launch_frame_in(const char* name, const void* in, const int32_t* reset, floa
 }
 
 // one CTA: kTilePx pixels of the RGB rows 2*yp and 2*yp + 1 -> their Y words and the chroma words of the pair
-// (U and V of a 2x2 block from its top-left pixel, as cv2 COLOR_RGB2YUV_I420).  The source is the step's uint8
-// NHWC RGB (8-bit output; staged with 16-byte loads) or its fp32 NCHW HR frame (kF32, 10-bit output: coalesced
-// row reads of the three planes, q = clip(rint(x * 1023), 0, 1023)).  Colour row `color` of the table.
-template <int kFmt, bool kF32>
+// (U and V of a 2x2 block from its top-left pixel), staged in shared memory and written with 16-byte stores.
+template <int kFmt>
 __global__ void __launch_bounds__(kThreads)
 rgb_to_yuv420_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, tg_frame_window win,
                      int x_tiles, int color) {
   using F = Yuv<kFmt>;
   using Wd = typename F::Word;
-  static_assert(kF32 == F::k10, "8-bit output reads uint8 RGB, 10-bit output the fp32 frame");
+  constexpr bool kF32 = F::k10;                              // 8-bit output reads uint8 RGB, 10-bit the fp32 frame
   constexpr int kB = (int)sizeof(Wd);
   __shared__ __align__(16) uint8_t sin[2][kF32 ? 16 : kTilePx * 3 + 16];
   __shared__ __align__(16) uint8_t sy[2][kTilePx * kB + 16];
@@ -155,52 +194,28 @@ rgb_to_yuv420_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, in
   const int hp = H >> 1, yp = r % hp, img = r / hp;
   const int x0 = xt * kTilePx;
   const int npx = min(kTilePx, W - x0);                      // even
-  int li0 = 0, li1 = 0;
-  if constexpr (!kF32) {
-    const uint8_t* src = static_cast<const uint8_t*>(rgb) + (((size_t)img * H + 2 * yp) * W + x0) * 3;
-    li0 = stage_bytes(sin[0], src, npx * 3, t);
-    li1 = stage_bytes(sin[1], src + (size_t)W * 3, npx * 3, t);
-  }
+  const RgbRow<kF32> src0(rgb, sin[0], H, W, img, 2 * yp, x0, npx, t), src1(rgb, sin[1], H, W, img, 2 * yp + 1, x0,
+                                                                          npx, t);
   const int fh = win.frame_h, fw = win.frame_w;              // even, as are top and left
-  const int fx = win.left + x0, fyp = (win.top >> 1) + yp;   // the tile's column and row pair in the frame
-  Wd* frame = reinterpret_cast<Wd*>(out) + (size_t)img * (3 * (fh >> 1)) * fw;
-  Wd* yrow = frame + (size_t)(2 * fyp) * fw + fx;
-  Wd* crow = frame + (size_t)fh * fw;
-  Wd *c0, *c1 = nullptr;
-  if (F::kInterleaved) {
-    c0 = crow + (size_t)fyp * fw + fx;
-  } else {
-    c0 = crow + (size_t)fyp * (fw >> 1) + (fx >> 1);
-    c1 = c0 + (size_t)(fh >> 1) * (fw >> 1);
-  }
-  const int ly0 = lead_of(yrow), ly1 = lead_of(yrow + fw), lc0 = lead_of(c0), lc1 = F::kInterleaved ? 0 : lead_of(c1);
+  const int fx = win.left + x0, fy = win.top + 2 * yp;       // the tile's column and first row in the frame
+  Wd* frame = reinterpret_cast<Wd*>(out) + (size_t)img * F::frame_words(3, fh, fw);
+  Wd* yrow = frame + F::y_at(fw, fy, fx);
+  Wd* c0 = frame + F::chroma_at(fw, fy, fx) + F::u_plane(fh, fw);
+  Wd* c1 = frame + F::chroma_at(fw, fy, fx) + F::v_plane(fh, fw);   // I420 layout
+  const int ly0 = lead_of(yrow), ly1 = lead_of(yrow + fw), lc0 = lead_of(c0), lc1 = F::kSemi ? 0 : lead_of(c1);
   auto put = [](uint8_t* sb, int lead, int j, int v) { reinterpret_cast<Wd*>(sb + lead)[j] = F::word(v); };
-  const int* k = c_yuv.v[F::k10][color];
-  constexpr int kHalf = 1 << (F::kShift - 1);
-  const int yoff = k[15] << F::kShift;
-  constexpr int coff = F::kCoff << F::kShift;
-  auto q = [](int a) { return min(max(a >> F::kShift, 0), F::kTop); };
   if constexpr (!kF32) __syncthreads();
   if (t < npx) {
+    const YuvEncode<kFmt> e(color);
 #pragma unroll
     for (int dy = 0; dy < 2; ++dy) {
       int R, G, B;
-      if constexpr (kF32) {
-        const size_t plane = (size_t)H * W;
-        const float* p = static_cast<const float*>(rgb) + (size_t)img * 3 * plane + (size_t)(2 * yp + dy) * W + x0 + t;
-        auto q10 = [](float x) { return (int)fminf(fmaxf(rintf(x * 1023.f), 0.f), 1023.f); };
-        R = q10(__ldg(p));
-        G = q10(__ldg(p + plane));
-        B = q10(__ldg(p + 2 * plane));
-      } else {
-        const uint8_t* p = sin[dy] + (dy ? li1 : li0) + 3 * t;
-        R = p[0], G = p[1], B = p[2];
-      }
-      put(sy[dy], dy ? ly1 : ly0, t, q(k[0] * R + k[1] * G + k[2] * B + kHalf + yoff));
+      if (dy) src1(t, R, G, B);
+      else src0(t, R, G, B);
+      put(sy[dy], dy ? ly1 : ly0, t, e.y(R, G, B));
       if (dy == 0 && (t & 1) == 0) {
-        const int u = q(k[3] * R + k[4] * G + k[5] * B + kHalf + coff);
-        const int v = q(k[6] * R + k[7] * G + k[8] * B + kHalf + coff);
-        if (F::kInterleaved) {
+        const int u = e.u(R, G, B), v = e.v(R, G, B);
+        if (F::kSemi) {
           put(sc[0], lc0, t, u);
           put(sc[0], lc0, t + 1, v);
         } else {
@@ -216,7 +231,7 @@ rgb_to_yuv420_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, in
   };
   flush(yrow, sy[0], npx);
   flush(yrow + fw, sy[1], npx);
-  if (F::kInterleaved) {
+  if (F::kSemi) {
     flush(c0, sc[0], npx);
   } else {
     flush(c0, sc[0], npx >> 1);
@@ -224,179 +239,68 @@ rgb_to_yuv420_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, in
   }
 }
 
-// one CTA: kTilePx pixel pairs of one uint8 NHWC RGB row (6 bytes a pair, staged with 16-byte loads) -> one
-// 4-byte YUY2 / UYVY group per pair: Y of each pixel, U and V of the pair's sum (c_yuv422 row `color`)
+// q into the unit whose first pixel is (y, x) of frame img (fh x fw pixels): one 4-byte (packed 4:2:2) or 16-byte
+// (v210) store of its group, or one word of each plane per sample
+template <int kFmt>
+__device__ __forceinline__ void store_unit(uint8_t* __restrict__ out, int fh, int fw, int img, int y, int x,
+                                           const Unit<kFmt>& q) {
+  using F = Yuv<kFmt>;
+  if constexpr (kFmt == kV210) {
+    *reinterpret_cast<uint4*>(out + F::group_at(fh, fw, img, y, x)) = make_uint4(q.w[0], q.w[1], q.w[2], q.w[3]);
+  } else if constexpr (F::kGrouped) {
+    *reinterpret_cast<uint32_t*>(out + F::group_at(fh, fw, img, y, x)) = q.w[0];
+  } else {
+    typename F::Word* f = reinterpret_cast<typename F::Word*>(out) + (size_t)img * F::frame_words(3, fh, fw);
+#pragma unroll
+    for (int j = 0; j < q.kPx; ++j) f[F::y_at(fw, y, x + j)] = F::word(q.y(j));
+    typename F::Word* c = f + F::chroma_at(fw, y, x);
+    c[F::u_plane(fh, fw)] = F::word(q.u(0));
+    c[F::v_plane(fh, fw)] = F::word(q.v(0));
+  }
+}
+
+// one CTA: kTilePx units of one row of the per-unit layouts (packed 4:2:2, 4:4:4, 10-bit 4:2:2), one per thread:
+// Y of each pixel, U and V of each pixel (4:4:4) or of each pair's sum (4:2:2).  Units [0, units) of the picture are
+// written; the fields past pixel W - 1 of a partial last v210 group are 0, and a whole-frame v210 encode (units = the
+// row's S / 16 groups) also writes the row padding as 0.
 template <int kFmt>
 __global__ void __launch_bounds__(kThreads)
-rgb_to_yuv422_kernel(const uint8_t* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, tg_frame_window win,
-                     int x_tiles, int color) {
-  using F = Yuv<kFmt>;
-  static_assert(fmt_packed(kFmt) && !F::k10, "packed 4:2:2 is 8 bit");
-  __shared__ __align__(16) uint8_t sin[kTilePx * 6 + 16];
+rgb_to_yuv_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, tg_frame_window win,
+                  int x_tiles, int units, int color) {
+  using U = Unit<kFmt>;
+  constexpr bool kF32 = Yuv<kFmt>::k10;                      // 8-bit output reads uint8 RGB, 10-bit the fp32 frame
+  __shared__ __align__(16) uint8_t sin[kF32 ? 16 : kTilePx * U::kPx * 3 + 16];
   // rgb is the previous kernel's output; out may still be read by the copy of an earlier step
   tg_pdl_wait();
   tg_pdl_trigger();
   const int t = threadIdx.x;
   const int xt = blockIdx.x % x_tiles, r = blockIdx.x / x_tiles;
   const int y = r % H, img = r / H;
-  const int p0 = xt * kTilePx;
-  const int npair = min(kTilePx, (W >> 1) - p0);
-  const size_t row = (size_t)img * H + y;
-  const int li = stage_bytes(sin, rgb + (row * W + 2 * p0) * 3, npair * 6, t);
-  __syncthreads();
-  if (t >= npair) return;
-  const uint8_t* p = sin + li + 6 * t;
-  const int R0 = p[0], G0 = p[1], B0 = p[2], R1 = p[3], G1 = p[4], B1 = p[5];
-  const int* k = c_yuv422.v[color];
-  const int sy = k[9], sc = k[10];
-  const int yo = (c_yuv.v[0][color][15] << sy) + (1 << (sy - 1));
-  const int co = (F::kCoff << sc) + (1 << (sc - 1));
-  auto q = [](int a, int s) { return (uint32_t)min(max(a >> s, 0), 255); };
-  const uint32_t y0 = q(k[0] * R0 + k[1] * G0 + k[2] * B0 + yo, sy);
-  const uint32_t y1 = q(k[0] * R1 + k[1] * G1 + k[2] * B1 + yo, sy);
-  const int sr = R0 + R1, sg = G0 + G1, sb = B0 + B1;
-  const uint32_t u = q(k[3] * sr + k[4] * sg + k[5] * sb + co, sc);
-  const uint32_t v = q(k[6] * sr + k[7] * sg + k[8] * sb + co, sc);
-  const size_t frow = (size_t)img * win.frame_h + win.top + y;   // frame_w and left are even
-  reinterpret_cast<uint32_t*>(out)[frow * (win.frame_w >> 1) + (win.left >> 1) + p0 + t] =
-      y0 << (8 * packed_y0(kFmt)) | y1 << (8 * (packed_y0(kFmt) + 2)) | u << (8 * packed_u(kFmt)) |
-      v << (8 * (packed_u(kFmt) + 2));
-}
-
-// one CTA: kTilePx pixels of one row -> their Y, U and V words in the three planes of a 4:4:4 frame.  The source is
-// the uint8 NHWC RGB (8 bit, staged with 16-byte loads) or the fp32 NCHW HR frame (kF32, 10 bit, quantised as in
-// rgb_to_yuv420_kernel).  Colour row `color` of the table, per pixel.
-template <int kFmt, bool kF32>
-__global__ void __launch_bounds__(kThreads)
-rgb_to_yuv444_kernel(const void* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, tg_frame_window win,
-                     int x_tiles, int color) {
-  using F = Yuv<kFmt>;
-  using Wd = typename F::Word;
-  static_assert(fmt_444(kFmt) && kF32 == F::k10, "8-bit output reads uint8 RGB, 10-bit output the fp32 frame");
-  __shared__ __align__(16) uint8_t sin[kF32 ? 16 : kTilePx * 3 + 16];
-  tg_pdl_wait();
-  tg_pdl_trigger();
-  const int t = threadIdx.x;
-  const int xt = blockIdx.x % x_tiles, r = blockIdx.x / x_tiles;
-  const int y = r % H, img = r / H;
-  const int x0 = xt * kTilePx;
-  const int npx = min(kTilePx, W - x0);
-  const size_t plane = (size_t)H * W;
-  int li = 0;
-  if constexpr (!kF32) {
-    li = stage_bytes(sin, static_cast<const uint8_t*>(rgb) + (((size_t)img * H + y) * W + x0) * 3, npx * 3, t);
-    __syncthreads();
-  }
-  if (t >= npx) return;
-  int R, G, B;
-  if constexpr (kF32) {
-    const float* p = static_cast<const float*>(rgb) + (size_t)img * 3 * plane + (size_t)y * W + x0 + t;
-    auto q10 = [](float x) { return (int)fminf(fmaxf(rintf(x * 1023.f), 0.f), 1023.f); };
-    R = q10(__ldg(p));
-    G = q10(__ldg(p + plane));
-    B = q10(__ldg(p + 2 * plane));
-  } else {
-    const uint8_t* p = sin + li + 3 * t;
-    R = p[0], G = p[1], B = p[2];
-  }
-  const int* k = c_yuv.v[F::k10][color];
-  constexpr int kHalf = 1 << (F::kShift - 1);
-  constexpr int coff = F::kCoff << F::kShift;
-  auto q = [](int a) { return F::word(min(max(a >> F::kShift, 0), F::kTop)); };
-  const size_t fplane = (size_t)win.frame_h * win.frame_w;
-  Wd* dst = reinterpret_cast<Wd*>(out) + (size_t)img * 3 * fplane + (size_t)(win.top + y) * win.frame_w + win.left +
-            x0 + t;
-  dst[0] = q(k[0] * R + k[1] * G + k[2] * B + kHalf + (k[15] << F::kShift));
-  dst[fplane] = q(k[3] * R + k[4] * G + k[5] * B + kHalf + coff);
-  dst[2 * fplane] = q(k[6] * R + k[7] * G + k[8] * B + kHalf + coff);
-}
-
-// 10-bit 4:2:2 encode of one pixel pair from the fp32 NCHW HR frame: q = clip(rint(x * 1023), 0, 1023) per channel;
-// Y of each pixel with the 10-bit table row (as the I444_10 encode), U and V from the pair's sums q0 + q1 with one
-// more fraction bit (19), rounded half up -- the 8-bit derived rows' 4:2:2 rule at 10 bits
-struct Pair10 {
-  int y0, y1, u, v;
-};
-
-__device__ __forceinline__ Pair10 encode_pair10(const float* p, size_t plane, int color) {
-  auto q10 = [](float x) { return (int)fminf(fmaxf(rintf(x * 1023.f), 0.f), 1023.f); };
-  const int R0 = q10(__ldg(p)), G0 = q10(__ldg(p + plane)), B0 = q10(__ldg(p + 2 * plane));
-  const int R1 = q10(__ldg(p + 1)), G1 = q10(__ldg(p + plane + 1)), B1 = q10(__ldg(p + 2 * plane + 1));
-  const int* k = c_yuv.v[1][color];
-  constexpr int sy = 18, sc = 19;
-  const int yo = (k[15] << sy) + (1 << (sy - 1));
-  constexpr int co = (512 << sc) + (1 << (sc - 1));
-  auto q = [](int a, int s) { return min(max(a >> s, 0), 1023); };
-  const int sr = R0 + R1, sg = G0 + G1, sb = B0 + B1;
-  return {q(k[0] * R0 + k[1] * G0 + k[2] * B0 + yo, sy), q(k[0] * R1 + k[1] * G1 + k[2] * B1 + yo, sy),
-          q(k[3] * sr + k[4] * sg + k[5] * sb + co, sc), q(k[6] * sr + k[7] * sg + k[8] * sb + co, sc)};
-}
-
-// one CTA: kTilePx pixel pairs of one row of the fp32 NCHW HR frame -> their words in a P210 / I422_10 frame
-// ([2h, w] uint16: Y plane, then the interleaved UV plane or the U and V planes of h x w/2)
-template <int kFmt>
-__global__ void __launch_bounds__(kThreads)
-rgb_to_yuv422_10_kernel(const float* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, tg_frame_window win,
-                        int x_tiles, int color) {
-  using F = Yuv<kFmt>;
-  using Wd = typename F::Word;
-  static_assert(fmt_p422(kFmt), "P210 / I422_10");
-  tg_pdl_wait();
-  tg_pdl_trigger();
-  const int t = threadIdx.x;
-  const int xt = blockIdx.x % x_tiles, r = blockIdx.x / x_tiles;
-  const int y = r % H, img = r / H;
-  const int pair = xt * kTilePx + t;
-  if (pair >= (W >> 1)) return;
-  const size_t plane = (size_t)H * W;
-  const Pair10 e = encode_pair10(rgb + (size_t)img * 3 * plane + (size_t)y * W + 2 * pair, plane, color);
-  const int fw = win.frame_w, fy = win.top + y, fx = win.left + 2 * pair;   // frame_w and left are even
-  const size_t fplane = (size_t)win.frame_h * fw;
-  Wd* frame = reinterpret_cast<Wd*>(out) + (size_t)img * 2 * fplane;
-  Wd* ys = frame + (size_t)fy * fw + fx;
-  ys[0] = F::word(e.y0);
-  ys[1] = F::word(e.y1);
-  if (kFmt == kP210) {
-    Wd* c = frame + fplane + (size_t)fy * fw + fx;
-    c[0] = F::word(e.u);
-    c[1] = F::word(e.v);
-  } else {
-    Wd* c = frame + fplane + (size_t)fy * (fw >> 1) + (fx >> 1);
-    c[0] = F::word(e.u);
-    c[fplane / 2] = F::word(e.v);
-  }
-}
-
-// one CTA: kTilePx 16-byte v210 groups of one row of the fp32 NCHW HR frame, one group (6 pixels) per thread packed
-// into one 16-byte store; the fields past pixel W - 1 of a partial last group are 0.  Groups [0, groups) of the
-// picture are written; a whole-frame encode (groups = the row's S / 16) also writes the row padding as 0.
-__global__ void __launch_bounds__(kThreads)
-rgb_to_v210_kernel(const float* __restrict__ rgb, uint8_t* __restrict__ out, int H, int W, tg_frame_window win,
-                   int x_tiles, int groups, int color) {
-  tg_pdl_wait();
-  tg_pdl_trigger();
-  const int t = threadIdx.x;
-  const int xt = blockIdx.x % x_tiles, r = blockIdx.x / x_tiles;
-  const int y = r % H, img = r / H;
-  const int grp = xt * kTilePx + t;
-  if (grp >= groups) return;
-  const int x0 = 6 * grp;
-  uint32_t g[4] = {0u, 0u, 0u, 0u};
-  const size_t plane = (size_t)H * W;
-  const float* src = rgb + (size_t)img * 3 * plane + (size_t)y * W + x0;
-  auto put = [&g](int f, int v) { g[f / 3] |= (uint32_t)v << (10 * (f % 3)); };
+  const int tx0 = xt * kTilePx * U::kPx;                     // the tile's first pixel
+  const RgbRow<kF32> src(rgb, sin, H, W, img, y, tx0, min(kTilePx * U::kPx, W - tx0), t);
+  if constexpr (!kF32) __syncthreads();
+  const int unit = xt * kTilePx + t;
+  if (unit >= units) return;
+  const YuvEncode<kFmt> e(color);
+  U q;
 #pragma unroll
-  for (int p = 0; p < 3; ++p) {
-    if (x0 + 2 * p >= W) break;                      // W is even: a pair is whole or absent
-    const Pair10 e = encode_pair10(src + 2 * p, plane, color);
-    put(4 * p, e.u);
-    put(4 * p + 1, e.y0);
-    put(4 * p + 2, e.v);
-    put(4 * p + 3, e.y1);
+  for (int p = 0; p < U::kC; ++p) {
+    const int j = t * U::kPx + 2 * p;                        // the pair's (4:4:4: the pixel's) column in the tile
+    if (tx0 + j >= W) break;                                 // W is even: a pair is whole or absent
+    int R0, G0, B0;
+    src(j, R0, G0, B0);
+    if constexpr (U::kPx == 1) {
+      q.set_y(0, e.y(R0, G0, B0));
+      q.set_uv(0, e.u(R0, G0, B0), e.v(R0, G0, B0));
+    } else {
+      int R1, G1, B1;
+      src(j + 1, R1, G1, B1);
+      q.set_y(2 * p, e.y(R0, G0, B0));
+      q.set_y(2 * p + 1, e.y(R1, G1, B1));
+      q.set_uv(p, e.u(R0 + R1, G0 + G1, B0 + B1), e.v(R0 + R1, G0 + G1, B0 + B1));
+    }
   }
-  const size_t frow = (size_t)img * win.frame_h + win.top + y;
-  reinterpret_cast<uint4*>(out + frow * v210_stride(win.frame_w))[win.left / 6 + grp] =
-      make_uint4(g[0], g[1], g[2], g[3]);
+  store_unit<kFmt>(out, win.frame_h, win.frame_w, img, win.top + y, win.left + unit * U::kPx, q);
 }
 
 template <int kFmt>
@@ -404,49 +308,25 @@ int launch_to_yuv(const char* name, const void* rgb, void* out, int n, int H, in
                   int color, cudaStream_t stream) {
   using F = Yuv<kFmt>;
   TG_REQUIRE(n > 0 && H > 0 && W > 0, TG_E_INVALID, "%s: bad size n=%d H=%d W=%d", name, n, H, W);
-  TG_REQUIRE(!fmt_420(kFmt) || (H % 2 == 0 && W % 2 == 0), TG_E_UNSUPPORTED,
-             "%s: YUV 4:2:0 needs an even height and width, got %dx%d", name, H, W);
-  TG_REQUIRE(!fmt_422(kFmt) || W % 2 == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name, W);
-  TG_REQUIRE(!fmt_packed(kFmt) || ((uintptr_t)out & 3u) == 0, TG_E_INVALID,
-             "%s: packed 4:2:2 output must be 4-byte aligned", name);
-  TG_REQUIRE(kFmt != kV210 || ((uintptr_t)out & 15u) == 0, TG_E_INVALID, "%s: v210 output must be 16-byte aligned",
-             name);
+  const int rc = check_frames<kFmt>(name, out, H, W, win, F::kAlign, "output");
+  if (rc != TG_OK) return rc;
   const bool whole_frame = win == nullptr;
   const tg_frame_window whole = {H, W, 0, 0};
   if (!win) win = &whole;
-  const int rc = check_window<kFmt>(name, win, H, W);
-  if (rc != TG_OK) return rc;
-  // v210: the picture's groups, or every group of the row up to its stride for a whole-frame encode
-  const int groups = kFmt != kV210 ? 0 : whole_frame ? (int)(v210_stride(W) / 16) : tg_ceil_div(W, 6);
-  const int x_tiles = tg_ceil_div(kFmt == kV210 ? groups : fmt_422(kFmt) ? W / 2 : W, kTilePx);
-  const size_t ctas = (size_t)x_tiles * (fmt_420(kFmt) ? H / 2 : H) * n;
+  // the picture's units, or every v210 group of the row up to its stride for a whole-frame encode
+  const int units = kFmt == kV210 && whole_frame ? (int)(v210_stride(W) / 16) : tg_ceil_div(W, F::kUnitPx);
+  const int x_tiles = tg_ceil_div(units, kTilePx);
+  const size_t ctas = (size_t)x_tiles * (H / F::kGy) * n;
   TG_REQUIRE(ctas <= 0x7fffffff, TG_E_UNSUPPORTED, "%s: grid too large", name);
   uint8_t* o = static_cast<uint8_t*>(out);
-  if constexpr (kFmt == kV210)
-    tg_launch(rgb_to_v210_kernel, dim3((unsigned)ctas), dim3(kThreads), 0, stream, static_cast<const float*>(rgb), o,
-              H, W, *win, x_tiles, groups, color);
-  else if constexpr (fmt_p422(kFmt))
-    tg_launch(rgb_to_yuv422_10_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), 0, stream,
-              static_cast<const float*>(rgb), o, H, W, *win, x_tiles, color);
-  else if constexpr (fmt_packed(kFmt))
-    tg_launch(rgb_to_yuv422_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), 0, stream,
-              static_cast<const uint8_t*>(rgb), o, H, W, *win, x_tiles, color);
-  else if constexpr (fmt_444(kFmt))
-    tg_launch(rgb_to_yuv444_kernel<kFmt, F::k10>, dim3((unsigned)ctas), dim3(kThreads), 0, stream, rgb, o, H, W,
-              *win, x_tiles, color);
+  if constexpr (F::k420)
+    tg_launch(rgb_to_yuv420_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), 0, stream, rgb, o, H, W, *win,
+              x_tiles, color);
   else
-    tg_launch(rgb_to_yuv420_kernel<kFmt, F::k10>, dim3((unsigned)ctas), dim3(kThreads), 0, stream, rgb, o, H, W,
-              *win, x_tiles, color);
+    tg_launch(rgb_to_yuv_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), 0, stream, rgb, o, H, W, *win, x_tiles,
+              units, color);
   TG_CUDA_LAUNCH_CHECK(name);
   return TG_OK;
-}
-
-// words of one fh x fw frame of layout kFmt (kHWC: c bytes a pixel)
-template <int kFmt>
-size_t frame_words(int c, int fh, int fw) {
-  const size_t px = (size_t)fh * fw;
-  if (kFmt == kV210) return (size_t)fh * v210_stride(fw);    // bytes
-  return kFmt == kHWC ? px * c : fmt_packed(kFmt) || fmt_p422(kFmt) ? 2 * px : fmt_444(kFmt) ? 3 * px : 3 * (px / 2);
 }
 
 // total words of n frames := the layout's black (Y: the colour's luma offset, U = V: kCoff; HWC: 0).  Grid-stride;
@@ -478,8 +358,8 @@ fill_black_kernel(uint8_t* __restrict__ out, size_t frame, size_t luma, size_t t
   } else {
     for (size_t i = blockIdx.x * (size_t)kThreads + threadIdx.x; i < total; i += (size_t)gridDim.x * kThreads) {
       const size_t j = i % frame;
-      // packed 4:2:2: Y is every other byte, starting at packed_y0; planar: the first fh * fw words
-      const bool is_y = fmt_packed(kFmt) ? (int)(j & 1) == packed_y0(kFmt) : j < luma;
+      // packed 4:2:2: Y is every other byte, starting at Y0's; planar: the first fh * fw words
+      const bool is_y = F::kGrouped ? (int)(j & 1) == F::y_field(0) : j < luma;
       o[i] = kFmt == kHWC ? (Wd)0 : F::word(is_y ? y : F::kCoff);
     }
   }
@@ -487,18 +367,15 @@ fill_black_kernel(uint8_t* __restrict__ out, size_t frame, size_t luma, size_t t
 
 template <int kFmt>
 int launch_fill_black(const char* name, void* out, int n, int c, int fh, int fw, int color, cudaStream_t stream) {
+  using F = Yuv<kFmt>;
   TG_REQUIRE(out, TG_E_INVALID, "%s: null pointer (out)", name);
   TG_REQUIRE(n > 0 && c > 0 && fh > 0 && fw > 0, TG_E_INVALID, "%s: bad size n=%d c=%d %dx%d", name, n, c, fh, fw);
   TG_REQUIRE(kFmt == kHWC || c == 3, TG_E_INVALID, "%s: YUV frames carry 3 channels, got %d", name, c);
-  TG_REQUIRE(!fmt_10(kFmt) || ((uintptr_t)out & 1u) == 0, TG_E_INVALID, "%s: 10-bit frames must be 2-byte aligned",
-             name);
-  TG_REQUIRE(!fmt_420(kFmt) || ((fh | fw) & 1) == 0, TG_E_UNSUPPORTED,
-             "%s: YUV 4:2:0 needs an even height and width, got %dx%d", name, fh, fw);
-  TG_REQUIRE(!fmt_422(kFmt) || (fw & 1) == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name,
-             fw);
-  TG_REQUIRE(kFmt != kV210 || ((uintptr_t)out & 15u) == 0, TG_E_INVALID, "%s: v210 frames must be 16-byte aligned",
-             name);
-  const size_t frame = frame_words<kFmt>(c, fh, fw), total = frame * n;
+  // words, one at a time; v210 frames are whole groups
+  const int rc =
+      check_frames<kFmt>(name, out, fh, fw, nullptr, kFmt == kV210 ? F::kAlign : (int)sizeof(typename F::Word));
+  if (rc != TG_OK) return rc;
+  const size_t frame = F::frame_words(c, fh, fw), total = frame * n;
   const size_t need = (total + kThreads - 1) / kThreads, ctas = need < 4096 ? need : 4096;
   tg_launch(fill_black_kernel<kFmt>, dim3((unsigned)ctas), dim3(kThreads), 0, stream, static_cast<uint8_t*>(out),
             frame, (size_t)fh * fw, total, color, fw);
@@ -513,7 +390,6 @@ __global__ void __launch_bounds__(kThreads)
 luma_sums_kernel(const uint8_t* __restrict__ in, int c, int h, int w, int bgr, int x_tiles,
                  unsigned long long* __restrict__ rows, unsigned long long* __restrict__ cols) {
   using F = Yuv<kFmt>;
-  using Wd = typename F::Word;
   __shared__ unsigned warp_sum[kThreads / 32];
   tg_pdl_wait();
   tg_pdl_trigger();
@@ -523,21 +399,19 @@ luma_sums_kernel(const uint8_t* __restrict__ in, int c, int h, int w, int bgr, i
   const int x = xt * kTilePx + t;
   unsigned v = 0;
   if (x < w) {
-    const size_t px = (size_t)h * w;
     if constexpr (kFmt == kHWC) {
       const uint8_t* p = in + (((size_t)img * h + y) * w + x) * c;
       const unsigned R = __ldg(p + (bgr ? 2 : 0)), G = __ldg(p + 1), B = __ldg(p + (bgr ? 0 : 2));
       v = (9798u * R + 19235u * G + 3735u * B + 16384u) >> 15;
-    } else if constexpr (fmt_packed(kFmt)) {
-      v = __ldg(in + ((size_t)img * h + y) * 2 * w + 2 * x + packed_y0(kFmt));   // Y of pixel x in its pair's group
     } else if constexpr (kFmt == kV210) {
-      const int f = 2 * (x % 6) + 1;                                           // Y of pixel x in its group
-      const uint32_t* g = reinterpret_cast<const uint32_t*>(in + ((size_t)img * h + y) * v210_stride(w)) + 4 * (x / 6);
-      v = ((__ldg(g + f / 3) >> (10 * (f % 3))) & 1023u) >> 2;
+      const uint32_t* g = reinterpret_cast<const uint32_t*>(in + F::group_at(h, w, img, y, x));
+      const int f = F::y_field(x % 6);
+      v = (unsigned)F::field(__ldg(g + f / F::kFieldsPerWord), f) >> 2;
+    } else if constexpr (F::kGrouped) {
+      v = __ldg(in + F::group_at(h, w, img, y, x) + F::y_field(x & 1));   // a packed field is a byte of the group
     } else {
-      const Wd* frame = reinterpret_cast<const Wd*>(in) +
-                        img * (fmt_444(kFmt) ? 3 * px : fmt_p422(kFmt) ? 2 * px : 3 * (px / 2));
-      v = (unsigned)F::sample(__ldg(frame + (size_t)y * w + x)) >> (F::k10 ? 2 : 0);
+      const typename F::Word* frame = reinterpret_cast<const typename F::Word*>(in) + img * F::frame_words(3, h, w);
+      v = (unsigned)F::sample(__ldg(frame + F::y_at(w, y, x))) >> (F::k10 ? 2 : 0);
     }
     atomicAdd(cols + (size_t)img * w + x, (unsigned long long)v);
   }
@@ -558,13 +432,9 @@ int launch_luma_sums(const char* name, const void* in, int bgr, int n, int c, in
   TG_REQUIRE(n > 0 && h > 0 && w > 0, TG_E_INVALID, "%s: bad size n=%d %dx%d", name, n, h, w);
   TG_REQUIRE(c == 3, TG_E_INVALID, "%s: luma of 3-channel frames, got %d channels", name, c);
   TG_REQUIRE((((uintptr_t)rows | (uintptr_t)cols) & 7u) == 0, TG_E_INVALID, "%s: rows and cols 8-byte aligned", name);
-  TG_REQUIRE(!fmt_10(kFmt) || ((uintptr_t)in & 1u) == 0, TG_E_INVALID, "%s: 10-bit frames must be 2-byte aligned",
-             name);
-  TG_REQUIRE(!fmt_420(kFmt) || ((h | w) & 1) == 0, TG_E_UNSUPPORTED,
-             "%s: YUV 4:2:0 needs an even height and width, got %dx%d", name, h, w);
-  TG_REQUIRE(!fmt_422(kFmt) || (w & 1) == 0, TG_E_UNSUPPORTED, "%s: YUV 4:2:2 needs an even width, got %d", name,
-             w);
-  TG_REQUIRE(kFmt != kV210 || ((uintptr_t)in & 3u) == 0, TG_E_INVALID, "%s: v210 frames must be 4-byte aligned", name);
+  // Y alone: a byte of a packed group, a 4-byte word of a v210 group, a planar word
+  const int rc = check_frames<kFmt>(name, in, h, w, nullptr, kFmt == kV210 ? 4 : (int)sizeof(typename Yuv<kFmt>::Word));
+  if (rc != TG_OK) return rc;
   const int x_tiles = tg_ceil_div(w, kTilePx);
   const size_t ctas = (size_t)x_tiles * h * n;
   TG_REQUIRE(ctas <= 0x7fffffff, TG_E_UNSUPPORTED, "%s: grid too large", name);

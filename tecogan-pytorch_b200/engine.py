@@ -326,8 +326,9 @@ class StreamEngine(ClipEngine):
         fh, fw = self.crop[:2] if self.crop else self.in_picture or (h, w)
         frame = ops.yuv_frame_shape(yuv_in, fh, fw) if yuv_in else (fh, fw, c)
         # 10-bit words: zeroed as int16, the same bits
-        in_dtype = torch.int16 if _word_dtype(yuv_in) == torch.uint16 else torch.uint8
-        self.inp = ([torch.zeros(n, *frame, dtype=in_dtype, device=dev).view(_word_dtype(yuv_in)) for _ in range(2)]
+        word = ops.yuv_word_dtype(yuv_in) if yuv_in else torch.uint8
+        in_dtype = torch.int16 if word == torch.uint16 else torch.uint8
+        self.inp = ([torch.zeros(n, *frame, dtype=in_dtype, device=dev).view(word) for _ in range(2)]
                     if self.u8_input else None)
         # the frame input, called as frame_in(frames, reset=, lr_curr=, lr_prev=, hr_prev=)
         in_window = self.crop[2:] if self.crop else None       # (top, left) of the picture in the input frames
@@ -359,8 +360,8 @@ class StreamEngine(ClipEngine):
         ten = yuv_out is not None and ops.yuv_depth(yuv_out) == 10
         self.yuv = self.pad = self.rs = self.tables = None
         if yuv_out:
-            self.yuv = [torch.empty(n, *ops.yuv_frame_shape(yuv_out, Yf, Xf), dtype=_word_dtype(yuv_out), device=dev)
-                        for _ in range(2)]
+            self.yuv = [torch.empty(n, *ops.yuv_frame_shape(yuv_out, Yf, Xf), dtype=ops.yuv_word_dtype(yuv_out),
+                                    device=dev) for _ in range(2)]
         elif self.out_frame:
             self.pad = [torch.empty((n, Yf, Xf, c), dtype=torch.uint8, device=dev) for _ in range(2)]
         if self.out_frame:
@@ -758,12 +759,7 @@ class PaddedStreamEngine(StreamEngine):
 YUV420 = ops.YUV420_LAYOUTS       # 'nv12', 'i420'
 YUV = ops.YUV_LAYOUTS             # those, the 10-bit 'p010', 'i420_10', 4:2:2 'yuy2', 'uyvy', 4:4:4 'i444', 'i444_10',
                                   # 10-bit 4:2:2 'p210', 'i422_10', 'v210'
-_YUV_422_444 = ops.YUV422_LAYOUTS + ops.YUV444_LAYOUTS
 COLORS = ops.YUV_COLORS           # 'bt601' (the default, cv2's conversion), 'bt709', 'bt601-full', 'bt709-full'
-
-
-def _word_dtype(layout):
-    return ops.yuv_word_dtype(layout) if layout else torch.uint8
 
 
 class VideoStream:
@@ -954,7 +950,8 @@ class VideoStream:
             frames = torch.from_numpy(frames)
         if not isinstance(frames, torch.Tensor):
             raise TypeError(f'VideoStream.push: frames must be a tensor or ndarray, got {type(frames).__name__}')
-        dtype = torch.float32 if self.input == 'float32' else _word_dtype(self.input if self.input in YUV else None)
+        dtype = (torch.float32 if self.input == 'float32' else
+                 ops.yuv_word_dtype(self.input) if self.input in YUV else torch.uint8)
         if frames.dtype != dtype:
             raise L.TecoganB200Error(f'VideoStream.push: {self.input} stream expects {dtype} frames, got '
                                      f'{frames.dtype}')
@@ -963,10 +960,7 @@ class VideoStream:
                              self.input, (None, None))
         if frame is None:
             frame = ops.yuv_frame_shape(self.input, self.h, self.w)
-            layout = ('n,k,h,2w' if self.input in ops.YUV422_LAYOUTS else
-                      'n,k,3h,w' if self.input in ops.YUV444_LAYOUTS else
-                      'n,k,2h,w' if self.input in ('p210', 'i422_10') else
-                      'n,k,h,128*ceil(w/48)' if self.input == 'v210' else 'n,k,3h/2,w')
+            layout = 'n,k,' + ops.YUV_LAYOUT_TABLE[self.input].text
         if frames.dim() == len(frame) + 1 and self.n == 1:
             frames = frames.unsqueeze(0)
         if (frames.dim() != len(frame) + 2 or frames.shape[0] != self.n or frames.shape[1] < 1
@@ -1063,20 +1057,14 @@ def _is_int(v):
     return isinstance(v, numbers.Integral) and not isinstance(v, bool)
 
 
-def _grid(layout):
-    """(row, column) step of a layout's chroma grid: 4:2:0 (2, 2), 4:2:2 (1, 2), RGB / 4:4:4 (1, 1); v210 (1, 6),
-    its 6-pixel groups, where a picture starts."""
-    if layout == 'v210':
-        return 1, 6
-    if layout in ops.YUV422_LAYOUTS or layout in ops.YUV422_10_LAYOUTS:
-        return 1, 2
-    return (2, 2) if layout in YUV and layout not in _YUV_422_444 else (1, 1)
-
-
-def _size_grid(layout):
-    """(row, column) step of a layout's frame and picture sizes: _grid's, except v210's even width (a picture that
-    reaches the frame's right edge may end inside a group)."""
-    return (1, 2) if layout == 'v210' else _grid(layout)
+def _grids(layout):
+    """(row, column) steps of a layout's chroma grid, where a picture starts (4:2:0 (2, 2), 4:2:2 (1, 2), RGB / 4:4:4
+    (1, 1); v210 (1, 6), its 6-pixel groups), and of its frame and picture sizes (the same, except v210's even width:
+    a picture that reaches the frame's right edge may end inside a group)."""
+    if layout not in YUV:
+        return (1, 1), (1, 1)
+    lay = ops.YUV_LAYOUT_TABLE[layout]
+    return lay.grid, lay.size_grid
 
 
 def _group_end(layout, right, w):
@@ -1094,8 +1082,7 @@ def _check_box(arg, box, h, w, layout):
     top, left, ch, cw = (int(v) for v in box)
     if top < 0 or left < 0 or ch <= 0 or cw <= 0 or top + ch > h or left + cw > w:
         raise ValueError(f'{arg} {ch}x{cw} at ({top}, {left}) lies outside the {h}x{w} frame')
-    gy, gx = _grid(layout)
-    sy, sx = _size_grid(layout)
+    (gy, gx), (sy, sx) = _grids(layout)
     if top % gy or ch % sy or left % gx or cw % sx or not _group_end(layout, left + cw, w):
         raise ValueError(f'{arg} ({top}, {left}, {ch}, {cw}) is off the {layout} chroma grid: rows in steps of {gy}, '
                          f'columns in steps of {gx}' + _V210_RULE * (layout == 'v210'))
@@ -1116,8 +1103,7 @@ def _check_out_frame(out_frame, out_origin, Ho, Wo, out_format):
     Hf, Wf = int(out_frame[0]), int(out_frame[1])
     if Ho > Hf or Wo > Wf:
         raise ValueError(f'the {Ho}x{Wo} output picture does not fit out_frame {Hf}x{Wf}')
-    gy, gx = _grid(out_format)
-    sy, sx = _size_grid(out_format)
+    (gy, gx), (sy, sx) = _grids(out_format)
     if Hf % sy or Wf % sx:
         raise ValueError(f'out_frame {Hf}x{Wf} is off the {out_format} chroma grid')
     if out_origin is None:
@@ -1154,7 +1140,7 @@ def fit_size(picture, frame, sar=(1, 1), out_format='rgb'):
         raise ValueError(f"out_format must be 'rgb' or one of {YUV}, got {out_format!r}")
     ch, cw = (int(v) for v in picture)
     Hf, Wf = (int(v) for v in frame)
-    gy, gx = _grid(out_format)
+    gy, gx = _grids(out_format)[0]
     # display aspect num / den = (cw * sar_w) / (ch * sar_h), exact in integers
     num, den = cw * int(sar[0]), ch * int(sar[1])
     h, w = Hf, Hf * num // den
@@ -1206,7 +1192,7 @@ def bars_box(pic_rows, pic_cols, layout):
     """(top, left, ch, cw) from per-row / per-column picture flags, rounded inward to the layout's chroma grid; the
     whole frame when no row or column is picture (or the rounded box is empty)."""
     h, w = len(pic_rows), len(pic_cols)
-    gy, gx = _grid(layout)
+    gy, gx = _grids(layout)[0]
     if not pic_rows.any() or not pic_cols.any():
         return 0, 0, h, w
     r = np.flatnonzero(pic_rows)

@@ -4,6 +4,7 @@ PyTorch is plumbing here: it owns device memory and the CUDA stream; every opera
 one call into libtecogan_b200.so on ``torch.cuda.current_stream()``.  No op has a torch/CPU
 fallback -- a tensor that is not on a CUDA device is an error.
 """
+import collections
 import ctypes
 import os
 
@@ -407,9 +408,9 @@ def _split_window(name, layout, window):
     if window is None:
         return None, None
     window = tuple(window)
-    if layout == 'v210':
+    if layout is not None and YUV_LAYOUT_TABLE[layout].needs_width:
         if len(window) != 3:
-            raise L.TecoganB200Error(f'{name}: a v210 window is (top, left, frame_w), got {window!r}')
+            raise L.TecoganB200Error(f'{name}: a {layout} window is (top, left, frame_w), got {window!r}')
         return window[:2], window[2]
     return window, None
 
@@ -491,9 +492,6 @@ def stream_gather(ring, table, warm_hr, lr_curr, lr_prev, hr_prev, scale):
     return lr_curr
 
 
-YUV420_LAYOUTS = ('nv12', 'i420')
-
-
 def _yuv_layout(layout, name):
     if layout not in YUV420_LAYOUTS:
         raise L.TecoganB200Error(f'{name}: layout must be one of {YUV420_LAYOUTS}, got {layout!r}')
@@ -535,56 +533,71 @@ def rgb_u8_to_yuv420(rgb, layout, out=None):
     return out
 
 
-YUV422_LAYOUTS = ('yuy2', 'uyvy')                     # packed 4:2:2, uint8
-YUV444_LAYOUTS = ('i444', 'i444_10')                  # planar 4:4:4, uint8 / uint16
-# 10-bit 4:2:2: 'p210' / 'i422_10' uint16 [2h, w] (Y plane, then the interleaved UV plane / the U and V planes of
-# h x w/2), 'v210' uint8 [h, v210_stride(w)] (6 pixels per 16-byte group, rows padded to 128 bytes)
-YUV422_10_LAYOUTS = ('p210', 'i422_10', 'v210')
-# 4:2:0, then 4:2:2 and 4:4:4, then 10-bit 4:2:2; 8-bit uint8 words; 10-bit uint16 words, v210 uint8
-YUV_LAYOUTS = ('nv12', 'i420', 'p010', 'i420_10') + YUV422_LAYOUTS + YUV444_LAYOUTS + YUV422_10_LAYOUTS
-YUV_COLORS = ('bt601', 'bt709', 'bt601-full', 'bt709-full')
-_LAYOUT_CODE = {'nv12': L.YUV_NV12, 'i420': L.YUV_I420, 'p010': L.YUV_P010, 'i420_10': L.YUV_I420_10,
-                'yuy2': L.YUV_YUY2, 'uyvy': L.YUV_UYVY, 'i444': L.YUV_I444, 'i444_10': L.YUV_I444_10,
-                'p210': L.YUV_P210, 'i422_10': L.YUV_I422_10, 'v210': L.YUV_V210}
-
-
-def yuv_depth(layout):
-    """Bit depth of a YUV layout: 8 or 10."""
-    return 10 if layout in ('p010', 'i420_10', 'i444_10') + YUV422_10_LAYOUTS else 8
-
-
-def yuv_word_dtype(layout):
-    """The dtype of a YUV layout's frames: uint16 for the 10-bit layouts, uint8 for the 8-bit ones and for v210,
-    whose 10-bit samples are packed into bytes."""
-    return torch.uint16 if yuv_depth(layout) == 10 and layout != 'v210' else torch.uint8
-
-
 def v210_stride(w):
     """Bytes per row of a v210 frame w pixels wide: 128 * ceil(w / 48) (ceil(w / 6) 16-byte groups of 6 pixels,
     padded to 128 bytes)."""
     return 128 * (-(-w // 48))
 
 
+# What a YUV layout is, on the host: C code, bit depth, word dtype, the words (a, b) of an h x w frame (shape) and
+# its inverse (size; v210 rows do not give w, which needs_width says must be passed), the (row, column) steps of a
+# picture's origin (grid) and size (size_grid), and the shape text of a stack of its frames.
+_Layout = collections.namedtuple('_Layout', 'code depth dtype shape size grid size_grid needs_width text')
+_420, _422, _444 = (2, 2), (1, 2), (1, 1)
+_P420 = (lambda h, w: (3 * h // 2, w), lambda a, b: (2 * a // 3, b), _420, _420, False, '3h/2,w')
+_PACKED422 = (lambda h, w: (h, 2 * w), lambda a, b: (a, b // 2), _422, _422, False, 'h,2w')
+_P444 = (lambda h, w: (3 * h, w), lambda a, b: (a // 3, b), _444, _444, False, '3h,w')
+_P422 = (lambda h, w: (2 * h, w), lambda a, b: (a // 2, b), _422, _422, False, '2h,w')
+# a v210 picture starts on a 6-pixel group and has an even width; it ends on a group or at the frame's right edge
+_V210 = (lambda h, w: (h, v210_stride(w)), None, (1, 6), _422, True, 'h,128*ceil(w/48)')
+YUV_LAYOUT_TABLE = {
+    'nv12': _Layout(L.YUV_NV12, 8, torch.uint8, *_P420),
+    'i420': _Layout(L.YUV_I420, 8, torch.uint8, *_P420),
+    'p010': _Layout(L.YUV_P010, 10, torch.uint16, *_P420),
+    'i420_10': _Layout(L.YUV_I420_10, 10, torch.uint16, *_P420),
+    'yuy2': _Layout(L.YUV_YUY2, 8, torch.uint8, *_PACKED422),
+    'uyvy': _Layout(L.YUV_UYVY, 8, torch.uint8, *_PACKED422),
+    'i444': _Layout(L.YUV_I444, 8, torch.uint8, *_P444),
+    'i444_10': _Layout(L.YUV_I444_10, 10, torch.uint16, *_P444),
+    # P210 / I422_10: the Y plane, then the interleaved UV plane / the U and V planes of h x w/2; v210: 6 pixels
+    # per 16-byte group, rows padded to 128 bytes
+    'p210': _Layout(L.YUV_P210, 10, torch.uint16, *_P422),
+    'i422_10': _Layout(L.YUV_I422_10, 10, torch.uint16, *_P422),
+    'v210': _Layout(L.YUV_V210, 10, torch.uint8, *_V210),
+}
+YUV_LAYOUTS = tuple(YUV_LAYOUT_TABLE)          # 4:2:0, then 4:2:2 and 4:4:4, then 10-bit 4:2:2
+_LAYOUT_CODE = {k: v.code for k, v in YUV_LAYOUT_TABLE.items()}
+YUV420_LAYOUTS = tuple(k for k, v in YUV_LAYOUT_TABLE.items() if v.grid == _420 and v.depth == 8)
+YUV422_LAYOUTS = tuple(k for k, v in YUV_LAYOUT_TABLE.items() if v.grid == _422 and v.depth == 8)   # packed
+YUV444_LAYOUTS = tuple(k for k, v in YUV_LAYOUT_TABLE.items() if v.grid == _444)
+YUV422_10_LAYOUTS = tuple(k for k, v in YUV_LAYOUT_TABLE.items() if v.size_grid == _422 and v.depth == 10)
+YUV_COLORS = ('bt601', 'bt709', 'bt601-full', 'bt709-full')
+
+
+def yuv_depth(layout):
+    """Bit depth of a YUV layout: 8 or 10."""
+    return YUV_LAYOUT_TABLE[layout].depth
+
+
+def yuv_word_dtype(layout):
+    """The dtype of a YUV layout's frames: uint16 for the 10-bit layouts, uint8 for the 8-bit ones and for v210,
+    whose 10-bit samples are packed into bytes."""
+    return YUV_LAYOUT_TABLE[layout].dtype
+
+
 def yuv_frame_shape(layout, h, w):
     """The words of one h x w frame: (3h/2, w) for 4:2:0, (h, 2w) for packed 4:2:2, (3h, w) for planar 4:4:4,
     (2h, w) for P210 / I422_10 and (h, v210_stride(w)) bytes for v210."""
-    if layout == 'v210':
-        return (h, v210_stride(w))
-    if layout in ('p210', 'i422_10'):
-        return (2 * h, w)
-    if layout in YUV422_LAYOUTS:
-        return (h, 2 * w)
-    return (3 * h, w) if layout in YUV444_LAYOUTS else (3 * h // 2, w)
+    return YUV_LAYOUT_TABLE[layout].shape(h, w)
 
 
 def yuv_size_error(layout, h, w):
     """None if an h x w frame fits the layout's chroma subsampling, else why not: 4:2:0 needs an even height and
     width, 4:2:2 an even width, 4:4:4 any size."""
-    if layout in YUV422_LAYOUTS + YUV422_10_LAYOUTS:
-        return None if w % 2 == 0 else f'YUV 4:2:2 needs an even width, got {w}'
-    if layout in YUV444_LAYOUTS:
-        return None
-    return None if h % 2 == 0 and w % 2 == 0 else f'YUV 4:2:0 needs an even height and width, got {h}x{w}'
+    sy, sx = YUV_LAYOUT_TABLE[layout].size_grid
+    if sy == 2:
+        return None if h % 2 == 0 and w % 2 == 0 else f'YUV 4:2:0 needs an even height and width, got {h}x{w}'
+    return None if w % sx == 0 else f'YUV 4:2:2 needs an even width, got {w}'
 
 
 def yuv_format(layout, color, name='yuv_format'):
@@ -610,17 +623,13 @@ def yuv_frame_size(layout, shape, w=None):
     row's bytes do not give its width (rows are padded to 128 bytes): w must be given; for the other layouts a w
     that is given must be the shape's."""
     a, b = shape
-    if layout == 'v210':
+    lay = YUV_LAYOUT_TABLE[layout]
+    if lay.needs_width:
         if w is None:
-            raise L.TecoganB200Error('v210 frames do not give their width (rows are padded to 128 bytes): pass it '
+            raise L.TecoganB200Error(f'{layout} frames do not give their width (rows are padded to 128 bytes): pass it '
                                      '(frame_w)')
         return a, int(w)
-    if layout in ('p210', 'i422_10'):
-        hw = (a // 2, b)
-    elif layout in YUV422_LAYOUTS:
-        hw = (a, b // 2)
-    else:
-        hw = (a // 3, b) if layout in YUV444_LAYOUTS else (2 * a // 3, b)
+    hw = lay.size(a, b)
     if w is not None and int(w) != hw[1]:
         raise L.TecoganB200Error(f'{layout} frames of shape {tuple(shape)} are {hw[1]} wide, not {w}')
     return hw
@@ -717,6 +726,15 @@ def fill_black_v210(out, color, frame_w):
     return _fill_black(out, 'v210', color, frame_w)
 
 
+def _yuv_stack(name, t, arg, layout, frame_w):
+    """(fh, fw) of the frames of t, a stack [n,*yuv_frame_shape(layout, fh, fw)] of a YUV layout's frames."""
+    _req(t, yuv_word_dtype(layout), arg, 3)
+    fh, fw = yuv_frame_size(layout, t.shape[1:], frame_w)
+    if tuple(t.shape[1:]) != yuv_frame_shape(layout, fh, fw):
+        raise L.TecoganB200Error(f'{name}: {tuple(t.shape)} is not a stack of {layout} frames')
+    return fh, fw
+
+
 def _fill_black(out, layout, color, frame_w):
     fmt = None
     if layout is None:
@@ -724,10 +742,7 @@ def _fill_black(out, layout, color, frame_w):
         n, fh, fw, c = out.shape
     else:
         fmt = yuv_format(layout, color, 'fill_black')
-        _req(out, yuv_word_dtype(layout), 'out', 3)
-        (fh, fw), n, c = yuv_frame_size(layout, out.shape[1:], frame_w), out.shape[0], 3
-        if tuple(out.shape[1:]) != yuv_frame_shape(layout, fh, fw):
-            raise L.TecoganB200Error(f'fill_black: {tuple(out.shape)} is not a stack of {layout} frames')
+        (fh, fw), n, c = _yuv_stack('fill_black', out, 'out', layout, frame_w), out.shape[0], 3
     L.check(L.load().tg_fill_black(_ptr(out), ctypes.byref(fmt) if fmt is not None else None, n, c, fh, fw,
                                    _stream()), 'tg_fill_black')
     return out
@@ -743,10 +758,7 @@ def luma_line_sums(frames, layout=None, bgr=False, frame_w=None):
         n, h, w, c = frames.shape
     else:
         fmt = yuv_format(layout, 'bt601', 'luma_line_sums')
-        _req(frames, yuv_word_dtype(layout), 'frames', 3)
-        (h, w), n, c = yuv_frame_size(layout, frames.shape[1:], frame_w), frames.shape[0], 3
-        if tuple(frames.shape[1:]) != yuv_frame_shape(layout, h, w):
-            raise L.TecoganB200Error(f'luma_line_sums: {tuple(frames.shape)} is not a stack of {layout} frames')
+        (h, w), n, c = _yuv_stack('luma_line_sums', frames, 'frames', layout, frame_w), frames.shape[0], 3
     rows = torch.empty((n, h), dtype=torch.int64, device=frames.device)
     cols = torch.empty((n, w), dtype=torch.int64, device=frames.device)
     L.check(L.load().tg_luma_line_sums(_ptr(frames), ctypes.byref(fmt) if fmt is not None else None, int(bool(bgr)),
