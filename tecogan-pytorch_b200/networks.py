@@ -268,6 +268,14 @@ class FRNet(BaseSequenceGenerator):
 
     def __init__(self, in_nc, out_nc, nf, nb, degradation, scale):
         super().__init__()
+        # SRNet adds upsample_func(lr_curr) (in_nc channels) to its out_nc-channel output, and its input -- lr_curr
+        # and the space_to_depth of the warped out_nc-channel HR frame -- is one NHWC map of at most 64 channels
+        if in_nc != out_nc:
+            raise L.TecoganB200Error(f'FRNet: in_nc={in_nc} != out_nc={out_nc}: the residual and the recurrent HR '
+                                     'frame need as many output channels as input channels')
+        if (scale ** 2 + 1) * in_nc > 64:
+            raise L.TecoganB200Error(f'FRNet: (scale^2 + 1) * in_nc = {(scale ** 2 + 1) * in_nc} SRNet input '
+                                     f'channels at scale {scale}, in_nc {in_nc}: at most 64')
         self.scale = scale
         self.degradation = degradation
         self.upsample_func = get_upsampling_func(self.scale, degradation)

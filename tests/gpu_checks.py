@@ -62,51 +62,90 @@ def from_nhwc(y, c):
 
 
 # =============================================================================== elementwise
-def check_warp_hrflow(scale=4, h=11, w=37, n=2):
-    hr_prev = rand(1, n, 3, scale * h, scale * w)
-    flow = rand(2, n, 2, scale * h, scale * w, lo=-6, hi=6)
+def _contract(names, run):
+    """run() with the ops `names` replayed against their float64 CPU contracts (tests/kernel_contracts.py): every
+    output element of every call within its bound, poisoned outputs (NaN) written, pad channels exactly 0.
+    -> {op: worst |err| / bound}"""
+    import pytest
+    import kernel_contracts as KC
+    with pytest.MonkeyPatch.context() as mp:
+        rec = KC.Recorder(ops, mp, names)
+        run()
+        torch.cuda.synchronize()
+    assert not rec.failures, '\n'.join(rec.failures[:5])
+    assert set(names) <= rec.seen, sorted(set(names) - rec.seen)
+    return {k: round(v, 4) for k, v in rec.worst.items()}
+
+
+def _nan_out(n, h, w, cpad=64):
+    return torch.full((n, h, w, cpad), float('nan'), dtype=torch.float16, device=DEV)
+
+
+def _border_flow(n, H, W):
+    """integer HR flows that land every sample exactly on the image border: column X goes to 0 (X even) or W-1
+    (X odd), row Y to 0 or H-1 -- the corner pair x1 = min(x0+1, W-1) at the far border, weight 0 at the near one"""
+    X, Y = torch.arange(W, dtype=torch.float32), torch.arange(H, dtype=torch.float32)
+    u = torch.where(X % 2 == 0, -X, W - 1 - X).view(1, W).expand(H, W)
+    v = torch.where(Y % 2 == 0, -Y, H - 1 - Y).view(H, 1).expand(H, W)
+    return torch.stack([u, v]).unsqueeze(0).expand(n, 2, H, W).contiguous()
+
+
+def check_warp_hrflow(scale=4, h=11, w=37, n=2, c=3, amp=6.0):
+    """warp + space_to_depth + concat on a given HR flow: c = 3 runs the warp-autonomous kernel (tg_warp_w.cu),
+    every other c the CTA-lock-step one.  Output poisoned with NaN first: all 64 channels must come back written."""
+    hr_prev = rand(1, n, c, scale * h, scale * w)
+    flow = rand(2, n, 2, scale * h, scale * w, lo=-amp, hi=amp)
     flow[0, :, 0, 0] = torch.tensor([-100.0, 100.0])
     flow[0, :, -1, -1] = torch.tensor([100.0, -100.0])
-    lr = rand(3, n, 3, h, w)
-    got = ops.warp_s2d_concat_hrflow(hr_prev.to(DEV), flow.to(DEV), lr.to(DEV), scale)
+    lr = rand(3, n, c, h, w)
+    got = ops.warp_s2d_concat_hrflow(hr_prev.to(DEV), flow.to(DEV), lr.to(DEV), scale, out=_nan_out(n, h, w))
     torch.cuda.synchronize()
     ref = K.warp_s2d_concat(hr_prev.numpy(), flow.numpy(), lr.numpy(), scale)
-    c_used = (scale * scale + 1) * 3
+    c_used = (scale * scale + 1) * c
     got_f = from_nhwc(got, c_used).numpy()
     # index math: every output element must be the fp16 rounding of the oracle value up to the
     # closed-form grid (x+u vs the reference's normalised round trip: <= ~1e-4 px)
     err = np.abs(got_f - ref).max()
     assert err <= 2e-3, f'warp_hrflow max abs err {err}'
-    assert np.array_equal(got_f[:, :3], f16(lr).numpy()), 'lr_curr channels must be exact fp16 copies'
+    assert np.array_equal(got_f[:, :c], f16(lr).numpy()), 'lr_curr channels must be exact fp16 copies'
     assert float(got[..., c_used:].abs().max()) == 0.0, 'pad channels must be zero'
-    # space_to_depth placement exactness: integer flow -> warp is an exact gather
+    # space_to_depth placement exactness: integer flow -> warp is an exact gather (image 1: onto the borders)
     flow_i = torch.round(flow)
-    got_i = ops.warp_s2d_concat_hrflow(hr_prev.to(DEV), flow_i.to(DEV), lr.to(DEV), scale)
+    if n > 1:
+        flow_i[1] = _border_flow(1, scale * h, scale * w)[0]
+    got_i = ops.warp_s2d_concat_hrflow(hr_prev.to(DEV), flow_i.to(DEV), lr.to(DEV), scale, out=_nan_out(n, h, w))
     ref_i = K.warp_s2d_concat(hr_prev.numpy(), flow_i.numpy(), lr.numpy(), scale, exact_reference_grid=False)
     assert np.array_equal(from_nhwc(got_i, c_used).numpy(), f16(torch.from_numpy(ref_i)).numpy()), \
         'integer-flow warp + space_to_depth must be bit exact'
-    return {'max_abs': float(err)}
+    assert float(got_i[..., c_used:].abs().max()) == 0.0, 'pad channels must be zero'
+    worst = _contract(('warp_s2d_concat_hrflow',), lambda: ops.warp_s2d_concat_hrflow(
+        hr_prev.to(DEV), flow.to(DEV), lr.to(DEV), scale, out=_nan_out(n, h, w)))
+    return {'max_abs': float(err), 'contract': worst}
 
 
-def check_warp_lrflow(scale=4, mode='BD', h=18, w=28, n=2):
+def check_warp_lrflow(scale=4, mode='BD', h=18, w=28, n=2, c=3, amp=3.0):
     h8, w8 = h // 8 * 8, w // 8 * 8
-    hr_prev = rand(4, n, 3, scale * h, scale * w)
-    lr_flow = rand(5, n, 2, h8, w8, lo=-3, hi=3)
-    lr = rand(6, n, 3, h, w)
+    hr_prev = rand(4, n, c, scale * h, scale * w)
+    lr_flow = rand(5, n, 2, h8, w8, lo=-amp, hi=amp)
+    lr = rand(6, n, c, h, w)
     up_mode = L.UP_BICUBIC if mode == 'BD' else L.UP_BILINEAR
-    got = ops.warp_s2d_concat_lrflow(hr_prev.to(DEV), lr_flow.to(DEV), lr.to(DEV), scale, up_mode)
+    got = ops.warp_s2d_concat_lrflow(hr_prev.to(DEV), lr_flow.to(DEV), lr.to(DEV), scale, up_mode,
+                                     out=_nan_out(n, h, w))
     pad = K.reflect_pad_flow(lr_flow.numpy(), h - h8, w - w8)
     up = K.bicubic_upsample(pad, scale) if mode == 'BD' else K.bilinear_upsample(pad, scale)
     hr_flow = np.float32(scale) * up
     ref = K.warp_s2d_concat(hr_prev.numpy(), hr_flow, lr.numpy(), scale)
-    c_used = (scale * scale + 1) * 3
+    c_used = (scale * scale + 1) * c
     err = np.abs(from_nhwc(got, c_used).numpy() - ref).max()
     assert err <= 2e-3, f'warp_lrflow({mode},{scale}) max abs err {err}'
-    # the standalone flow upsampler must agree with the oracle to fp32 rounding
+    assert float(got[..., c_used:].abs().max()) == 0.0, 'pad channels must be zero'
+    # the standalone flow upsampler must agree with the oracle to fp32 rounding (a few ulps of the largest HR flow)
     hf = ops.upsample(lr_flow.to(DEV), scale, up_mode, out_hw=(h, w), mul=float(scale)).cpu().numpy()
     e2 = np.abs(hf - hr_flow).max()
-    assert e2 <= 2e-5, f'flow upsample err {e2}'
-    return {'max_abs': float(err), 'flow_up_abs': float(e2)}
+    assert e2 <= max(2e-5, 8 * float(np.spacing(np.abs(hr_flow).max()))), f'flow upsample err {e2}'
+    worst = _contract(('warp_s2d_concat_lrflow',), lambda: ops.warp_s2d_concat_lrflow(
+        hr_prev.to(DEV), lr_flow.to(DEV), lr.to(DEV), scale, up_mode, out=_nan_out(n, h, w)))
+    return {'max_abs': float(err), 'flow_up_abs': float(e2), 'contract': worst}
 
 
 def check_pool_upsample():
@@ -1094,39 +1133,59 @@ def check_conv_pool_epilogue(cin=64, cout=64, h=37, w=45, n=2, a_mode=None, seed
     return {'bit_exact': True, 'shape': list(got.shape)}
 
 
-def check_fused_tail(scale=4, n=2, h=20, w=26, with_lr=True, seed=400, accumulate=False):
+def check_fused_tail(scale=4, n=2, h=20, w=26, with_lr=True, seed=400, accumulate=False, out_nc=3):
     """tg_convT_convout_tcgen05 (last transposed conv + ReLU + conv_out + upsample_func(lr) + uint8 in one
-    launch) against the same four stages run as separate kernels, and against torch CPU fp32."""
+    launch, conv_out to out_nc = 1..3 channels) against the same four stages run as separate kernels, against torch
+    CPU fp32 and, for frames up to 4096 input pixels, against the float64 contract of every kernel call
+    (tests/kernel_contracts.py)."""
     mid_h, mid_w = h, w                               # input of the last transposed conv
     lr_scale = scale
     x = rand(seed, n, 64, mid_h, mid_w, lo=-1, hi=1)
     wt = rand(seed + 1, 64, 64, 3, 3, lo=-0.08, hi=0.08)
     bu = rand(seed + 2, 64, lo=-0.2, hi=0.2)
-    wo = rand(seed + 3, 3, 64, 3, 3, lo=-0.08, hi=0.08)
-    bo = rand(seed + 4, 3, lo=-0.2, hi=0.2)
+    wo = rand(seed + 3, out_nc, 64, 3, 3, lo=-0.08, hi=0.08)
+    bo = rand(seed + 4, out_nc, lo=-0.2, hi=0.2)
     assert (2 * mid_h) % lr_scale == 0 and (2 * mid_w) % lr_scale == 0
-    lr = rand(seed + 5, n, 3, 2 * mid_h // lr_scale, 2 * mid_w // lr_scale)
-    up = ops.PackedConv(wt.to(DEV), bu.to(DEV), L.CONVT_3X3_S2, L.ACT_RELU)
-    oc = ops.PackedConv(wo.to(DEV), bo.to(DEV), L.CONV_3X3, L.ACT_NONE, L.EPI_OUT_NCHW_F32)
+    lr = rand(seed + 5, n, out_nc, 2 * mid_h // lr_scale, 2 * mid_w // lr_scale)
     mode = L.UP_BICUBIC if scale == 4 else L.UP_BILINEAR
     xg = nhwc(x)
-    # separate kernels
-    ref = oc(up(xg))
-    if with_lr:
-        ops.upsample(lr.to(DEV), lr_scale, mode, y=ref, accumulate=True)
-    ref_u8 = ops.float_to_uint8_nhwc(ref)
-    # fused (output buffers poisoned first: every pixel must be written exactly once)
-    got = torch.full((n, 3, 2 * mid_h, 2 * mid_w), float('nan'), device=DEV)
-    got_u8 = torch.full((n, 2 * mid_h, 2 * mid_w, 3), 77, dtype=torch.uint8, device=DEV)
-    if accumulate:       # y pre-filled with the residual, the kernel adds conv + bias onto it (no uint8 inside)
-        ops.upsample(lr.to(DEV), lr_scale, mode, y=got)
-        ops.fused_tail(up, oc, xg, None, lr_scale, mode, y=got, accumulate=True)
-        ops.float_to_uint8_nhwc(got, got_u8)
+    res = {}
+
+    def run():
+        up = ops.PackedConv(wt.to(DEV), bu.to(DEV), L.CONVT_3X3_S2, L.ACT_RELU)
+        oc = ops.PackedConv(wo.to(DEV), bo.to(DEV), L.CONV_3X3, L.ACT_NONE, L.EPI_OUT_NCHW_F32)
+        # separate kernels
+        ref = oc(up(xg))
+        if with_lr:
+            ops.upsample(lr.to(DEV), lr_scale, mode, y=ref, accumulate=True)
+        res['ref'], res['ref_u8'] = ref, ops.float_to_uint8_nhwc(ref)
+        # fused (output buffers poisoned first: every pixel must be written exactly once); the uint8 frame sits in a
+        # band of 0xAB bytes on either side that must come back untouched
+        got = torch.full((n, out_nc, 2 * mid_h, 2 * mid_w), float('nan'), device=DEV)
+        size, band = n * 2 * mid_h * 2 * mid_w * out_nc, 4096
+        buf = torch.full((band + size + band,), 0xAB, dtype=torch.uint8, device=DEV)
+        got_u8 = buf[band:band + size].view(n, 2 * mid_h, 2 * mid_w, out_nc).fill_(77)
+        if accumulate:       # y pre-filled with the residual, the kernel adds conv + bias onto it (no uint8 inside)
+            ops.upsample(lr.to(DEV), lr_scale, mode, y=got)
+            ops.fused_tail(up, oc, xg, None, lr_scale, mode, y=got, accumulate=True)
+            ops.float_to_uint8_nhwc(got, got_u8)
+        else:
+            ops.fused_tail(up, oc, xg, lr.to(DEV) if with_lr else None, lr_scale, mode, y=got, y_u8=got_u8)
+        torch.cuda.synchronize()
+        assert bool((buf[:band] == 0xAB).all()) and bool((buf[band + size:] == 0xAB).all()), \
+            'uint8 frame written outside its bounds'
+        res['got'], res['got_u8'] = got, got_u8
+
+    out = {}
+    if n * mid_h * mid_w <= 4096:
+        names = ('PackedConv', 'fused_tail', 'float_to_uint8_nhwc') + (('upsample',) if with_lr else ())
+        out['contract'] = _contract(names, run)
     else:
-        ops.fused_tail(up, oc, xg, lr.to(DEV) if with_lr else None, lr_scale, mode, y=got, y_u8=got_u8)
-    torch.cuda.synchronize()
+        run()
+    got, got_u8, ref, ref_u8 = res['got'], res['got_u8'], res['ref'], res['ref_u8']
     assert not torch.isnan(got).any(), 'fused tail left output pixels unwritten'
-    out = {'vs_separate_max_abs': float((got - ref).abs().max()), 'vs_separate_rel_l2': rell2(got.cpu().numpy(), ref.cpu().numpy())}
+    out.update({'vs_separate_max_abs': float((got - ref).abs().max()),
+                'vs_separate_rel_l2': rell2(got.cpu().numpy(), ref.cpu().numpy())})
     du8 = (got_u8.int() - ref_u8.int()).abs()
     out['u8_max_lsb'] = int(du8.max())
     out['u8_frac_diff'] = float((du8 != 0).float().mean())
@@ -1146,6 +1205,18 @@ CHECKS = {
     'warp_hrflow_s2': lambda: check_warp_hrflow(2, h=9, w=70),
     'warp_lrflow_bd4': lambda: check_warp_lrflow(4, 'BD'),
     'warp_lrflow_bi2': lambda: check_warp_lrflow(2, 'BI', h=20, w=24),
+    # the CTA-lock-step kernel (c != 3): widths that leave a partial last CTA of 128 / S LR pixels, odd heights (the
+    # last CTA of RY = 2 rows has one), flows of +-30 px; c = 12 at s = 2 is the widest that fits 64 channels
+    'warp_hrflow_s4_c1': lambda: check_warp_hrflow(4, h=11, w=37, c=1, amp=30.0),
+    'warp_hrflow_s4_c2': lambda: check_warp_hrflow(4, h=9, w=45, c=2, amp=30.0),
+    'warp_hrflow_s2_c1': lambda: check_warp_hrflow(2, h=9, w=70, c=1, amp=30.0),
+    'warp_hrflow_s2_c4': lambda: check_warp_hrflow(2, h=13, w=75, c=4, amp=30.0),
+    'warp_hrflow_s2_c12': lambda: check_warp_hrflow(2, h=7, w=67, c=12, amp=30.0),
+    'warp_lrflow_bd4_c1': lambda: check_warp_lrflow(4, 'BD', h=19, w=37, c=1, amp=30.0),
+    'warp_lrflow_bd4_c2': lambda: check_warp_lrflow(4, 'BD', h=13, w=22, c=2, amp=30.0),
+    'warp_lrflow_bi2_c1': lambda: check_warp_lrflow(2, 'BI', h=11, w=70, c=1, amp=30.0),
+    'warp_lrflow_bi2_c4': lambda: check_warp_lrflow(2, 'BI', h=11, w=19, c=4, amp=30.0),
+    'warp_lrflow_bi2_c12': lambda: check_warp_lrflow(2, 'BI', h=9, w=67, c=12, amp=30.0),
     'pool_upsample': check_pool_upsample,
     'module_ops': check_module_ops,
     'downsample_bd': check_downsample_bd,
@@ -1202,6 +1273,18 @@ CHECKS = {
     'fused_tail_accumulate_bd4': lambda: check_fused_tail(4, n=2, h=34, w=22, seed=450, accumulate=True),
     'fused_tail_accumulate_bi2': lambda: check_fused_tail(2, n=1, h=17, w=31, seed=460, accumulate=True),
     'fused_tail_no_residual': lambda: check_fused_tail(4, with_lr=False, h=18, w=8, seed=440),
+    # conv_out to 1 and 2 channels: the co < cout_real guards, conv_out's packing past cout, the uint8 stride and
+    # the residual planes of a 1- / 2-channel frame
+    'fused_tail_bd4_out1': lambda: check_fused_tail(4, n=2, h=20, w=26, seed=470, out_nc=1),
+    'fused_tail_bd4_out2': lambda: check_fused_tail(4, n=1, h=30, w=14, seed=471, out_nc=2),
+    'fused_tail_bi2_out1': lambda: check_fused_tail(2, n=3, h=21, w=33, seed=472, out_nc=1),
+    'fused_tail_bi2_out2': lambda: check_fused_tail(2, n=2, h=17, w=31, seed=473, out_nc=2),
+    'fused_tail_accumulate_bd4_out1': lambda: check_fused_tail(4, n=2, h=34, w=22, seed=474, accumulate=True, out_nc=1),
+    'fused_tail_accumulate_bd4_out2': lambda: check_fused_tail(4, n=1, h=18, w=26, seed=475, accumulate=True, out_nc=2),
+    'fused_tail_accumulate_bi2_out1': lambda: check_fused_tail(2, n=1, h=17, w=31, seed=476, accumulate=True, out_nc=1),
+    'fused_tail_accumulate_bi2_out2': lambda: check_fused_tail(2, n=2, h=42, w=26, seed=477, accumulate=True, out_nc=2),
+    'fused_tail_no_residual_out1': lambda: check_fused_tail(4, with_lr=False, h=18, w=8, seed=478, out_nc=1),
+    'fused_tail_no_residual_out2': lambda: check_fused_tail(4, with_lr=False, h=18, w=8, seed=479, out_nc=2),
     'autograd_guards': check_autograd_guards,
     'dgrad_simt_conv': lambda: check_conv_dgrad('simt'),
     'dgrad_simt_convT': lambda: check_conv_dgrad('simt', kind=L.CONVT_3X3_S2, h=10, w=12),

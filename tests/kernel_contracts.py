@@ -473,13 +473,15 @@ def _rand(seed, *shape, lo=0.0, hi=1.0, dev='cpu'):
     return torch.from_numpy(np.random.default_rng(seed).uniform(lo, hi, size=shape).astype(np.float32)).to(dev)
 
 
-def run_sequence(T, dev, seed, nb, n, t, h, w, degradation='BD', scale=4, flow_losses=True, loss_mul=1.0):
-    """one training step of FRNet.forward_sequence: loss on hr_data (and hr_flow / lr_flow), backward"""
+def run_sequence(T, dev, seed, nb, n, t, h, w, degradation='BD', scale=4, flow_losses=True, loss_mul=1.0, nc=3):
+    """one training step of FRNet.forward_sequence of an nc-channel net: loss on hr_data (and hr_flow / lr_flow),
+    backward"""
     from oracle import frnet_oracle as O
-    net = T.FRNet(3, 3, 64, nb, degradation, scale)
-    net.load_state_dict(O.make_frnet_params(seed, nb=nb, scale=scale, degradation=degradation, gain=1.5), strict=True)
+    net = T.FRNet(nc, nc, 64, nb, degradation, scale)
+    net.load_state_dict(O.make_frnet_params(seed, in_nc=nc, out_nc=nc, nb=nb, scale=scale, degradation=degradation,
+                                            gain=1.5), strict=True)
     net = net.to(dev).train()
-    d = net(_rand(seed + 1, n, t, 3, h, w, dev=dev))
+    d = net(_rand(seed + 1, n, t, nc, h, w, dev=dev))
     keys = ('hr_data', 'hr_flow', 'lr_flow') if flow_losses else ('hr_data',)
     loss = sum((d[k] * _rand(seed + 2 + i, *d[k].shape, lo=-1, hi=1, dev=dev)).sum() for i, k in enumerate(keys))
     (loss * loss_mul).backward()
@@ -536,7 +538,7 @@ def inference_ops(tail, pool):
 
 
 def run_frames(T, net, clips, dev):
-    """the recurrent eval step over clips [n,t,c,h,w] from zero state -- ClipEngine.run_frame without a CUDA graph on
+    """the recurrent eval step over clips [n,t,c,h,w] (c = the net's in_nc) from zero state -- ClipEngine.run_frame without a CUDA graph on
     a GPU (the step bench.py times), FRNet.step_into with a uint8 output on the CPU.  Returns the last (hr, u8)."""
     n, t, c, h, w = clips.shape
     s = net.scale
@@ -557,18 +559,18 @@ def run_frames(T, net, clips, dev):
     return hr, u8
 
 
-def run_inference(T, ops, dev, seed, nb, n, t, h, w, degradation='BD', scale=4, params=None, clips=None):
-    """t recurrent eval steps of n lock-stepped clips of h x w (O.make_clip, or `clips` [n,t,3,h,w]) through a net
-    with O.make_frnet_params(gain=1.5) (or `params`).  The net is built here, after the Recorder is installed:
-    layer objects made earlier would bypass its wrapped classes."""
+def run_inference(T, ops, dev, seed, nb, n, t, h, w, degradation='BD', scale=4, params=None, clips=None, nc=3):
+    """t recurrent eval steps of n lock-stepped clips of nc x h x w (O.make_clip, or `clips` [n,t,nc,h,w]) through an
+    nc-channel net with O.make_frnet_params(gain=1.5) (or `params`).  The net is built here, after the Recorder is
+    installed: layer objects made earlier would bypass its wrapped classes."""
     from oracle import frnet_oracle as O
-    net = T.FRNet(3, 3, 64, nb, degradation, scale)
+    net = T.FRNet(nc, nc, 64, nb, degradation, scale)
     if params is None:
-        params = O.make_frnet_params(seed, nb=nb, scale=scale, degradation=degradation, gain=1.5)
+        params = O.make_frnet_params(seed, in_nc=nc, out_nc=nc, nb=nb, scale=scale, degradation=degradation, gain=1.5)
     net.load_state_dict(params, strict=True)
     net = net.to(dev).eval()
     if clips is None:
-        clips = torch.stack([O.make_clip(seed + 1 + k, t, 3, h, w) for k in range(n)])
+        clips = torch.stack([O.make_clip(seed + 1 + k, t, nc, h, w) for k in range(n)])
     return run_frames(T, net, clips, dev)
 
 

@@ -100,6 +100,23 @@ def test_state_dict_is_reference_compatible(scale, deg):
         assert np.array_equal(T.BicubicUpsampler(scale).kernels.numpy(), bicubic_kernels(scale))
 
 
+@pytest.mark.parametrize('nc,scale', [(1, 4), (2, 4), (3, 4), (4, 2), (12, 2)])
+def test_frnet_accepts_channel_counts_its_kernels_run(nc, scale):
+    """(scale^2 + 1) * nc SRNet input channels fit the 64-channel map: 17 / 34 / 51 at 4x, 20 / 60 at 2x"""
+    net = T.FRNet(nc, nc, 64, 1, 'BD', scale)
+    assert net.fnet.in_nc == nc and net.srnet.conv_in[0].in_channels == (scale ** 2 + 1) * nc
+    assert net.srnet.conv_out.out_channels == nc
+    net.load_state_dict(O.make_frnet_params(1, in_nc=nc, out_nc=nc, nb=1, scale=scale), strict=True)
+
+
+@pytest.mark.parametrize('in_nc,out_nc,scale,match', [
+    (3, 1, 4, r'in_nc=3 != out_nc=1'), (1, 3, 2, r'in_nc=1 != out_nc=3'),
+    (4, 4, 4, r'= 68 SRNet input channels .* at most 64'), (13, 13, 2, r'= 65 SRNet input channels .* at most 64')])
+def test_frnet_refuses_channel_counts_no_kernel_runs(in_nc, out_nc, scale, match):
+    with pytest.raises(T.TecoganB200Error, match=match):
+        T.FRNet(in_nc, out_nc, 64, 1, 'BD', scale)
+
+
 def test_profile_matches_reference_counter():
     net = T.FRNet(3, 3, 64, 10, 'BD', 4)
     g, p = net.profile((3, 134, 320))

@@ -45,19 +45,22 @@ def _dispatch(monkeypatch, ops, tail, pool):
 # ----------------------------------------------------------------------------------- the stand-ins are the reference
 @pytest.mark.parametrize('pool', [True, False], ids=['pool_fused', 'pool_separate'])
 @pytest.mark.parametrize('tail', ['acc', 'fused', None], ids=['tail_acc', 'tail_fused', 'tail_separate'])
-@pytest.mark.parametrize('degradation,scale,h,w', [('BD', 4, 17, 23), ('BI', 2, 20, 24)], ids=['bd4_17x23', 'bi2_20x24'])
-def test_stand_ins_match_the_reference_step(monkeypatch, degradation, scale, h, w, tail, pool):
+@pytest.mark.parametrize('degradation,scale,h,w,nc', [('BD', 4, 17, 23, 3), ('BI', 2, 20, 24, 3), ('BD', 4, 17, 23, 1),
+                                                       ('BI', 2, 20, 24, 1), ('BD', 4, 17, 23, 2), ('BI', 2, 20, 24, 2)],
+                         ids=['bd4_17x23', 'bi2_20x24', 'bd4_17x23_nc1', 'bi2_20x24_nc1', 'bd4_17x23_nc2',
+                              'bi2_20x24_nc2'])
+def test_stand_ins_match_the_reference_step(monkeypatch, degradation, scale, h, w, nc, tail, pool):
     ops = _install(monkeypatch, torch.float32)
     _dispatch(monkeypatch, ops, tail, pool)
-    p = O.make_frnet_params(41, nb=2, scale=scale, degradation=degradation, gain=1.5)
-    net = T.FRNet(3, 3, 64, 2, degradation, scale)
+    p = O.make_frnet_params(41, in_nc=nc, out_nc=nc, nb=2, scale=scale, degradation=degradation, gain=1.5)
+    net = T.FRNet(nc, nc, 64, 2, degradation, scale)
     net.load_state_dict(p, strict=True)
     net.eval()
     n = 2
-    lr_curr, lr_prev = KC._rand(42, n, 3, h, w), KC._rand(43, n, 3, h, w)
-    hr_prev = KC._rand(44, n, 3, scale * h, scale * w)
-    hr = torch.empty(n, 3, scale * h, scale * w)
-    u8 = torch.empty(n, scale * h, scale * w, 3, dtype=torch.uint8)
+    lr_curr, lr_prev = KC._rand(42, n, nc, h, w), KC._rand(43, n, nc, h, w)
+    hr_prev = KC._rand(44, n, nc, scale * h, scale * w)
+    hr = torch.empty(n, nc, scale * h, scale * w)
+    u8 = torch.empty(n, scale * h, scale * w, nc, dtype=torch.uint8)
     net.step_into(lr_curr, lr_prev, hr_prev, hr, out_u8=u8)
     with torch.no_grad():
         ref = R.step(p, lr_curr, lr_prev, hr_prev, scale, degradation, nb=2)
@@ -74,7 +77,7 @@ SCENARIOS = [('acc', True, 2, 17, 23, 'BD', 4), ('fused', False, 1, 17, 23, 'BD'
              ('fused', True, 1, 20, 24, 'BI', 2)]
 
 
-def _replay(monkeypatch, perturb=None):
+def _replay(monkeypatch, perturb=None, nc=3):
     ops = _install(monkeypatch, torch.float16)
     for name, fn in (perturb or {}).items():
         monkeypatch.setattr(ops, name, fn)
@@ -82,7 +85,7 @@ def _replay(monkeypatch, perturb=None):
     reached = set()
     for i, (tail, pool, n, h, w, degradation, scale) in enumerate(SCENARIOS):
         _dispatch(monkeypatch, ops, tail, pool)
-        KC.run_inference(T, ops, 'cpu', 50 + i, 2, n, 2, h, w, degradation, scale)
+        KC.run_inference(T, ops, 'cpu', 50 + i, 2, n, 2, h, w, degradation, scale, nc=nc)
         reached |= KC.inference_ops(tail, pool)
     KC.run_inference_module_ops(T, ops, 'cpu', 60)
     return rec, reached
@@ -127,6 +130,16 @@ def _tail_drops_a_seam_tap(up, outc, x, lr_curr, lr_scale, up_mode, y=None, y_u8
     return y
 
 
+def _tail_copies_channel_0(up, outc, x, lr_curr, lr_scale, up_mode, y=None, y_u8=None, max_ctas=0,
+                           accumulate=False):
+    """output channel 0 written into every output channel (a tail that ignores co past the first)"""
+    y = FK.fused_tail(up, outc, x, lr_curr, lr_scale, up_mode, y, None, max_ctas, accumulate)
+    y[:, 1:] = y[:, :1]
+    if y_u8 is not None:
+        FK.float_to_uint8_nhwc(y, y_u8)
+    return y
+
+
 def _tail_overwrites(up, outc, x, lr_curr, lr_scale, up_mode, y=None, y_u8=None, max_ctas=0, accumulate=False):
     return FK.fused_tail(up, outc, x, lr_curr, lr_scale, up_mode, y, y_u8, max_ctas, False)
 
@@ -142,16 +155,19 @@ def _uint8_truncates(x, y=None):
     return FK._out(v.contiguous(), y)
 
 
-@pytest.mark.parametrize('name,fn', [
-    ('PackedConv', _PoolDropsLastWindowElement),
-    ('fused_tail', _tail_drops_a_seam_tap),
-    ('fused_tail', _tail_overwrites),
-    ('warp_s2d_concat_lrflow', _lrflow_replicate_pad),
-    ('float_to_uint8_nhwc', _uint8_truncates),
+@pytest.mark.parametrize('name,fn,nc', [
+    ('PackedConv', _PoolDropsLastWindowElement, 3),
+    ('fused_tail', _tail_drops_a_seam_tap, 3),
+    ('fused_tail', _tail_overwrites, 3),
+    ('warp_s2d_concat_lrflow', _lrflow_replicate_pad, 3),
+    ('float_to_uint8_nhwc', _uint8_truncates, 3),
+    ('fused_tail', _tail_copies_channel_0, 2),
+    ('warp_s2d_concat_lrflow', _lrflow_replicate_pad, 1),
 ], ids=['pool_drops_last_window_element', 'tail_drops_a_seam_tap', 'tail_accumulate_overwrites',
-        'lrflow_replicate_pads_the_flow', 'uint8_truncates'])
-def test_replay_flags_a_wrong_inference_stand_in(monkeypatch, name, fn):
-    rec, _ = _replay(monkeypatch, {name: fn})
+        'lrflow_replicate_pads_the_flow', 'uint8_truncates', 'tail_copies_channel_0_nc2',
+        'lrflow_replicate_pads_the_flow_nc1'])
+def test_replay_flags_a_wrong_inference_stand_in(monkeypatch, name, fn, nc):
+    rec, _ = _replay(monkeypatch, {name: fn}, nc)
     flagged = [f for f in rec.failures if f.startswith(name + ' ')]
     print(KC.report(rec), rec.failures[:3])
     assert flagged, f'the replay did not flag the perturbed {name}'

@@ -2,7 +2,7 @@
 its CPU contract (tests/kernel_contracts.py), each judged per element on its own inputs against a float64 reference:
 the benchmark's workload itself, the other tail mode at full size, small ragged shapes under every dispatch (tail
 fused / accumulating / separate launches, max-pool in the conv epilogue or separate), SRNet's convs forced to
-either A-operand path, the 2x BI tail, and warp_s2d_concat_lrflow at its edges.  Each scenario prints its wall
+either A-operand path, the 2x BI tail, 1-, 2- and 4-channel nets, and warp_s2d_concat_lrflow at its edges.  Each scenario prints its wall
 time and the per-op (checked calls, worst |err| / bound)."""
 import os
 import sys
@@ -52,6 +52,7 @@ def _replay(monkeypatch, tag, run, tail='acc', pool=True, a_mode=None, expect=No
     assert expect <= rec.seen, f'ops never exercised: {sorted(expect - rec.seen)}'
     assert not rec.unfaked, f'kernels launched without a CPU contract: {sorted(set(rec.unfaked))}'
     assert not rec.failures, '\n'.join(rec.failures[:20])
+    return rec
 
 
 def test_bench_workload_kernel_calls_honour_their_contracts(monkeypatch):
@@ -98,6 +99,34 @@ def test_bi2_tail(monkeypatch, n, h, w):
     import kernel_contracts as KC
     _replay(monkeypatch, f'2xBI {n}x{h}x{w}',
             lambda T, ops: KC.run_inference(T, ops, DEV, 100, 10 if h > 100 else 2, n, 2, h, w, 'BI', 2))
+
+
+@pytest.mark.parametrize('pool', [True, False], ids=['pool_fused', 'pool_separate'])
+@pytest.mark.parametrize('tail', ['acc', 'fused', None], ids=['tail_acc', 'tail_fused', 'tail_separate'])
+def test_one_and_two_channel_nets(monkeypatch, tail, pool):
+    """FRNet(1, 1) and FRNet(2, 2) at 4x BD 13x22 and 2x BI 11x19: the CTA-lock-step warp (C != 3) on its LR flow,
+    conv_in at 17 / 34 / 5 / 10 real channels, the fused tail and conv_out at 1 / 2 output channels"""
+    import kernel_contracts as KC
+    runs = [(nc, deg, s, h, w) for nc in (1, 2) for deg, s, h, w in (('BD', 4, 13, 22), ('BI', 2, 11, 19))]
+
+    def run(T, ops):
+        for i, (nc, deg, s, h, w) in enumerate(runs):
+            KC.run_inference(T, ops, DEV, 120 + i, 2, 2, 2, h, w, deg, s, nc=nc)
+    rec = _replay(monkeypatch, f'nc=1,2 tail={tail} pool={pool}', run, tail=tail, pool=pool)
+    # one warp per frame: every run of two frames reached the lrflow warp
+    assert rec.calls['warp_s2d_concat_lrflow'] == 2 * len(runs), rec.calls
+
+
+@pytest.mark.parametrize('tail', ['acc', 'fused'], ids=['tail_acc', 'tail_fused'])
+def test_four_channel_net_runs_the_separate_tail(monkeypatch, tail):
+    """FRNet(4, 4) at 2x BI: 5 * 4 = 20 SRNet input channels, 4 output channels -- more than the fused tail
+    writes, so the tail runs as separate launches whatever the tail mode"""
+    import kernel_contracts as KC
+    rec = _replay(monkeypatch, f'nc=4 2xBI tail={tail}',
+                  lambda T, ops: KC.run_inference(T, ops, DEV, 130, 2, 2, 2, 11, 19, 'BI', 2, nc=4),
+                  tail=tail, expect=KC.inference_ops(None, True))
+    assert 'fused_tail' not in rec.seen
+    assert rec.calls['warp_s2d_concat_lrflow'] == 2, rec.calls
 
 
 def test_inference_module_ops(monkeypatch):

@@ -28,10 +28,11 @@ BD4 = dict(scale=4, degradation='BD', c=3, h=134, w=320)      # bench.py's bd4 f
 BI2 = dict(scale=2, degradation='BI', c=3, h=36, w=52)
 
 
-def _net(scale, degradation):
-    """bench.make_params() weights (seed 0, gain 1) for the given workload."""
-    net = T.FRNet(3, 3, 64, 10, degradation, scale)
-    net.load_state_dict(synthetic.make_frnet_params(0, scale=scale, degradation=degradation, gain=1.0), strict=True)
+def _net(scale, degradation, nc=3):
+    """bench.make_params() weights (seed 0, gain 1) for the given workload (of an nc-channel net)."""
+    net = T.FRNet(nc, nc, 64, 10, degradation, scale)
+    net.load_state_dict(synthetic.make_frnet_params(0, in_nc=nc, out_nc=nc, scale=scale, degradation=degradation,
+                                                    gain=1.0), strict=True)
     return net.to(DEV).eval()
 
 
@@ -66,12 +67,18 @@ def _frame_in(u8, reset, lr_curr, lr_prev, hr_prev, scale, bgr):
     torch.cuda.synchronize()
 
 
+def _with_c(cases, ids):
+    """the cases at c = 3 (RGB) under their own ids, then at c = 1, 2 and 4 (the frames of 1-, 2- and 4-channel nets)"""
+    return [pytest.param(*case, c, id=i if c == 3 else f'{i}-c{c}') for c in (3, 1, 2, 4) for case, i in zip(cases, ids)]
+
+
 @pytest.mark.parametrize('bgr', [False, True], ids=['rgb', 'bgr'])
-@pytest.mark.parametrize('n,h,w,offset', [(1, 16, 16, 0), (3, 37, 53, 0), (3, 37, 53, 5), (2, 7, 5, 13)])
-def test_frame_in_decodes_bit_exactly(n, h, w, offset, bgr):
-    """Every uint8 value (the 16x16 frame holds 0..255 three times) and random frames whose rows are not a multiple
-    of 16 bytes, read from a source `offset` bytes past a 16-byte boundary."""
-    c, s = 3, 4
+@pytest.mark.parametrize('n,h,w,offset,c', _with_c([(1, 16, 16, 0), (3, 37, 53, 0), (3, 37, 53, 5), (2, 7, 5, 13)],
+                                                   ['1-16-16-0', '3-37-53-0', '3-37-53-5', '2-7-5-13']))
+def test_frame_in_decodes_bit_exactly(n, h, w, offset, c, bgr):
+    """Every uint8 value (the 16x16 frame holds 0..255 c times) and random frames whose rows are not a multiple
+    of 16 bytes, read from a source `offset` bytes past a 16-byte boundary; bgr reverses the c channels."""
+    s = 4
     rng = np.random.default_rng(100 + n + h + offset)
     if h == 16:
         img = np.arange(n * h * w * c, dtype=np.int64).reshape(n, h, w, c) % 256
@@ -92,9 +99,9 @@ def test_frame_in_decodes_bit_exactly(n, h, w, offset, bgr):
     assert bool((prev == 3.0).all()) and bool((hr == 5.0).all())          # no reset mask: state untouched
 
 
-@pytest.mark.parametrize('with_frames', [True, False], ids=['decode_and_reset', 'reset_only'])
-def test_frame_in_reset_zeroes_flagged_slots_only(with_frames):
-    n, c, h, w, s = 3, 3, 37, 53, 4         # a slot of lr_prev is 5883 floats: its start is not 16-byte aligned
+@pytest.mark.parametrize('with_frames,c', _with_c([(True,), (False,)], ['decode_and_reset', 'reset_only']))
+def test_frame_in_reset_zeroes_flagged_slots_only(with_frames, c):
+    n, h, w, s = 3, 37, 53, 4               # a slot of lr_prev is c * 1961 floats: its start is not 16-byte aligned
     g = torch.Generator(device=DEV).manual_seed(7)
     lr = torch.full((n, c, h, w), float('nan'), device=DEV)
     prev = torch.rand((n, c, h, w), generator=g, device=DEV) + 1.0
@@ -118,12 +125,13 @@ def test_frame_in_reset_zeroes_flagged_slots_only(with_frames):
 
 
 # ------------------------------------------------------------------------------------------------ streams
-@pytest.mark.parametrize('geom', [BD4, BI2], ids=['bd4', 'bi2'])
+@pytest.mark.parametrize('geom', [BD4, BI2, dict(BD4, c=1), dict(BI2, c=2)], ids=['bd4', 'bi2', 'bd4_nc1', 'bi2_nc2'])
 def test_chunked_push_matches_infer_sequence(geom, bd4_net):
     """n=2 clips of 10 frames pushed as chunks [1,4,2,3]: uint8 input, fp32 input and BGR uint8 input all give the
-    bytes of one infer_sequence call on the reference loader's fp32 frames."""
-    net = bd4_net if geom is BD4 else _net(geom['scale'], geom['degradation'])
+    bytes of one infer_sequence call on the reference loader's fp32 frames -- for RGB nets and for nets of c = 1 and
+    2 channels (frames [n,k,h,w,c], the lock-step warp, the tail at 1 / 2 output channels)."""
     c, h, w = geom['c'], geom['h'], geom['w']
+    net = bd4_net if geom is BD4 else _net(geom['scale'], geom['degradation'], c)
     u8 = _clips_u8(11, 2, 10, c, h, w)
     f32 = _to_f32(u8)
     ref = net.infer_sequence(f32.pin_memory(), DEV)                        # [n,t,H,W,c]
@@ -133,7 +141,7 @@ def test_chunked_push_matches_infer_sequence(geom, bd4_net):
     assert np.array_equal(got, ref), int((got != ref).sum())
     got = _push_chunks(net.stream(2, h, w, device=DEV, input='float32'), f32, chunks)
     assert np.array_equal(got, ref), int((got != ref).sum())
-    bgr = np.ascontiguousarray(u8[..., ::-1])
+    bgr = u8[..., ::-1].copy()            # (ascontiguousarray keeps the negative stride of a 1-channel axis)
     got = _push_chunks(net.stream(2, h, w, device=DEV, channel_order='bgr'), bgr, chunks)   # NumPy input
     assert np.array_equal(got, ref), int((got != ref).sum())
 

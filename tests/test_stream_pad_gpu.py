@@ -285,3 +285,25 @@ def test_pad_front_0_is_the_plain_stream(nets):
     assert b.flush().shape == (3, 0, 4 * g['h'], 4 * g['w'], 3)
     a.close()
     b.close()
+
+
+def test_single_channel_stream_with_scene_cut_and_padding():
+    """FRNet(1, 1) at 2x BI, n = 3 slots of single-channel frames (channel 0 of the RGB clips: cuts at 9, 3 and 5),
+    scene_cut=10, reflect p = 3, pushes of 4: frames [n,k,h,w,1] in, the bytes of infer_sequence over each padded shot
+    out, and the cuts the oracle finds"""
+    g, p, mode, n = BI2, 3, 'reflect', 3
+    net = T.FRNet(1, 1, 64, 10, 'BI', 2)
+    net.load_state_dict(synthetic.make_frnet_params(0, in_nc=1, out_nc=1, scale=2, degradation='BI', gain=1.0),
+                        strict=True)
+    net = net.to(DEV).eval()
+    gray = np.ascontiguousarray(_clips(g['h'], g['w'])[..., :1])
+    t = gray.shape[1]
+    dec = _f32(gray)
+    o_cuts = np.stack([S.stream(dec[k].transpose(0, 3, 1, 2), set(), THR)[1] for k in range(n)])
+    assert o_cuts[0, 9] and o_cuts[2, 3] and o_cuts[2, 5], np.nonzero(o_cuts)
+    want = _expected(net, dec, [set(np.flatnonzero(o_cuts[k])) for k in range(n)], p, mode)
+    s = net.stream(n, g['h'], g['w'], device=DEV, scene_cut=THR, pad_front=p, padding_mode=mode)
+    got, cuts, _, _ = _drive(s, gray, [4] * (t // 4) + [t % 4], {})
+    s.close()
+    assert got.shape == (n, t, 2 * g['h'], 2 * g['w'], 1) and np.array_equal(got, want), int((got != want).sum())
+    assert np.array_equal(cuts, o_cuts)
